@@ -3,6 +3,7 @@
 
     python bench.py --gpus N --steps K --warmup W            # our arm (1 process per GPU under torchrun)
     python bench.py --impl reference --steps K --warmup W    # the reference's CPU path (oracle port)
+    python bench.py --steps K --dump-outputs DIR             # + what the last timed step computed, as DIR/*.npy
 
 A *step* is one pass of the hot path over one batch of 50 (user,item) pairs per GPU of the synthetic
 ml_1m-shaped matrix (max-nodes-per-hop 100): H2D(indices) -> extract -> adjacency -> fused RGCN
@@ -45,7 +46,7 @@ def peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3), not measured"
 
 
 class ClockSampler(object):
@@ -105,7 +106,7 @@ def _pool_init(adj_blob, cv, mnph, use_ref):
     _G["cv"], _G["mnph"], _G["ref"] = cv, mnph, None
     if use_ref:
         from oracle import ref_shim
-        m = ref_shim.load()                      # the reference's own util_functions.py (oracle/_ref or /root/reference)
+        m = ref_shim.load()                      # the reference's own util_functions.py (oracle/_ref)
         _G["ref"] = m
         _G["idx"] = (m.SparseRowIndexer(A), m.SparseColIndexer(A.tocsc()))
     else:
@@ -259,7 +260,7 @@ def run_reference(args, ds, B, rank):
 
 def cpu_baseline_dict(r):
     # kind: the model half is a restatement (PyG 1.4.2 is not installable here), so the arm as a whole is a port;
-    # the extraction half runs the reference's own code whenever oracle/_ref (or /root/reference) is present
+    # the extraction half runs the reference's own code whenever oracle/_ref is present
     return {"value": r["value"], "unit": "subgraphs/s", "cores": r["cores"], "kind": "port",
             "extraction_kind": r["extraction_kind"], "model_kind": "port (PyG 1.4.2 RGCNConv restated)",
             "sample": r["sample"], "extraction_subgraphs_per_s": r["extraction_subgraphs_per_s"],
@@ -277,7 +278,7 @@ def make_config(desc, G, world, no_graph=False):
 
 
 def gpu_baseline(ds, train, steps_idx, B, model_kind="igmc", steps=12):
-    """BASELINE config 2 / SURVEY 8(d): "vs PyG on the same B200".  PyG is not installable, so this is the restated
+    """BASELINE config 2 / SURVEY 8(d): "vs PyG on the same GPU".  PyG is not installable, so this is the restated
     PyG-1.4.2 formulation (index_select of per-edge weights + bmm + scatter-mean, autograd, torch.optim.Adam) run with
     torch CUDA ops on the same batches - what the reference does when a GPU is present (train_eval.py:20,159-177).
     The batches come from OUR extractor (collated on the device), so only the model half is the baseline's."""
@@ -317,7 +318,7 @@ def gpu_baseline(ds, train, steps_idx, B, model_kind="igmc", steps=12):
     torch.cuda.empty_cache()
     return {"value": B / (ms / 1000.0), "unit": "subgraphs/s", "ms_per_step": ms, "steps": steps,
             "kind": "port (PyG-1.4.2 formulation: index_select + bmm + scatter-mean, autograd, torch.optim.Adam; "
-                    "torch CUDA ops on the same B200, model half only - batches pre-extracted on the device)",
+                    "torch CUDA ops on the same GPU, model half only - batches pre-extracted on the device)",
             "peak_mem_gib": round(peak, 2)}
 
 
@@ -352,6 +353,37 @@ def batch_stats(ds, engine, idx_list):
         for k in range(len(idx)):
             tot["Du"] += int(rowdeg[nu[k, :cu[k]]].sum())
     return tot
+
+
+DUMP_ARRAY_BYTES = 6 << 20   # per array (at most 9: 54 MiB in all); larger arrays are written as a fixed, seeded sample of their elements
+
+
+def snapshot_outputs(eng, model, opt):
+    """what the last timed step computed, copied before later steps reuse the buffers: its loss and predictions, the
+    parameters and Adam moments after its update, and the batch it extracted for the next step"""
+    b = eng.batches[eng.slot]      # step_pipe flipped the slot: this is the batch the last step extracted
+    out = dict(loss=eng.last_loss, params=model.flat_params, adam_exp_avg=opt.exp_avg, adam_exp_avg_sq=opt.exp_avg_sq,
+               next_x=b.x, next_edge_index=b.edge_index, next_edge_type=b.edge_type, next_y=b.y)
+    ws = getattr(eng, "_last_ws", None)   # workspace of the one-launch train kernel (IGMC readout)
+    if ws is not None:
+        out["pred"] = ws["pred"]
+    return {k: v.detach().clone() for k, v in out.items()}
+
+
+def write_outputs(dirpath, arrays):
+    """DIR/<name>.npy in float32 (float arrays) or float64 (integer arrays: exact); returns {name: [shape, sampled]}"""
+    os.makedirs(dirpath, exist_ok=True)
+    info = {}
+    for name, t in sorted(arrays.items()):
+        a = t.cpu().numpy()
+        a = a.astype(np.float32 if a.dtype.kind == "f" else np.float64)
+        shape, sampled = list(a.shape), a.nbytes > DUMP_ARRAY_BYTES
+        if sampled:
+            n = DUMP_ARRAY_BYTES // a.itemsize
+            a = a.reshape(-1)[np.sort(np.random.default_rng(0).choice(a.size, n, replace=False))]
+        np.save(os.path.join(dirpath, name + ".npy"), a)
+        info[name] = [shape, sampled]
+    return info
 
 
 def run_ours(args):
@@ -417,7 +449,7 @@ def run_ours(args):
     for s in range(W + 4):
         eng.step_pipe(next_idx(), epoch=1, next_G=G)
     eng.check()
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")   # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")   # > 50 MB L2 of an H100
 
     # ---- (1) value: inputs resident in HBM, per-step CUDA events, L2 flushed between steps ----
     staged = torch.zeros(K, B + 4, dtype=torch.int64)
@@ -472,6 +504,7 @@ def run_ours(args):
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     dev_ms = float(t.item())
     value = G * K / (dev_ms / 1000.0)
+    dumped = snapshot_outputs(eng, model, opt) if args.dump_outputs else None
 
     # ---- (1b) informative: back-to-back steps, warm L2 (what a real epoch looks like) ----
     barrier()
@@ -509,9 +542,8 @@ def run_ours(args):
         if world > 1:
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
         e2e_runs.append(float(t.item()))
-        if zc:
-            assert K <= eng.LOSS_RING
-            for k in range(K):
+        if zc:   # the ring keeps the last LOSS_RING losses
+            for k in range(max(0, K - eng.LOSS_RING), K):
                 loss_host[k] = eng.loss_of_update(u0 + k)
     e2e_s = min(e2e_runs)
     eng.check()
@@ -568,11 +600,6 @@ def run_ours(args):
         # branch of the step graph and get their own line (`roofline.extract`)
         dom = "forward_backward" if one_launch else max(("forward", "backward"), key=lambda n: kern_ms[n])
         peak, peak_src = peaks()
-        traffic = None     # DRAM bytes per launch from an `ncu --set full` capture OF THIS workload + model, else null
-        tp = os.path.join(ROOT, "profiles", "traffic.json")
-        if os.path.exists(tp):
-            with open(tp) as f:
-                traffic = json.load(f).get("%s/%s" % (args.workload, args.model), {}).get(dom)
         per_launch_bytes = ab[dom] / nb_batches
         achieved = per_launch_bytes / (kern_ms[dom] * 1e-3) / 1e9
         step_bytes = ab["step"] / nb_batches
@@ -602,7 +629,7 @@ def run_ours(args):
             "warm_l2": {"value": G * K / (warm_ms / 1000.0), "ms_per_step": warm_ms / K,
                         "note": "same steps back to back without the L2 flush (informative)"},
             "roofline": {"bound": "hbm", "kernel": dom, "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src,
+                         "frac": achieved / peak, "traffic": None, "peak_source": peak_src,
                          "algorithmic_bytes_per_launch": per_launch_bytes,
                          "kernel_ms": kern_ms, "step_algorithmic_bytes": step_bytes,
                          "extract": {"achieved": ab["extract"] / nb_batches / (kern_ms["extract"] * 1e-3) / 1e9,
@@ -615,6 +642,8 @@ def run_ours(args):
             "batch_stats": {k: v / stats["B"] for k, v in stats.items() if k != "B"},
             "wall_s_timed_region": wall,
         }
+        if dumped is not None:
+            out["dumped_outputs"] = write_outputs(args.dump_outputs, dumped)
     if world > 1:
         # NCCL communicators that were captured into CUDA graphs do not tear down reliably
         # (destroy_process_group was observed to hang): drop the graphs, align the ranks, and let main() leave
@@ -636,6 +665,8 @@ def main():
     ap.add_argument("--no-graph", action="store_true")
     ap.add_argument("--skip-cpu-baseline", action="store_true")
     ap.add_argument("--cpu-steps", type=int, default=12)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed as DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     # stdout carries exactly ONE line (the JSON): anything a library prints to fd 1 during the run (NCCL's version

@@ -162,8 +162,8 @@ def load():
         fn = getattr(lib, name)  # AttributeError if the symbol is not exported
         fn.argtypes = argtypes
         fn.restype = C.c_int
-    if lib.igmc_build_info() != 100:
-        raise RuntimeError("igmc_b200: library was not built for sm_100a")
+    if lib.igmc_build_info() != 90:
+        raise RuntimeError("igmc_b200: library was not built for sm_90a")
     _lib = lib
     return lib
 

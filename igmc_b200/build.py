@@ -1,4 +1,4 @@
-"""Build libigmc_b200.so (sm_100a) in-tree with nvcc.  No torch headers: the library is a plain C-ABI."""
+"""Build libigmc_b200.so (sm_90a, H100) in-tree with nvcc.  No torch headers: the library is a plain C-ABI."""
 import os
 import subprocess
 import sys
@@ -8,8 +8,8 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libigmc_b200.so")
 SOURCES = ["extract.cu", "batch.cu", "rgcn.cu", "rgcn_rs.cu", "optim.cu", "sortpool.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
-         "-Xcompiler", "-fPIC", "-shared", "-DIGMC_SM_ARCH=100"]
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
+         "-Xcompiler", "-fPIC", "-shared", "-DIGMC_SM_ARCH=90"]
 
 
 def needs_build():

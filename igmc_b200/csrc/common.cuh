@@ -1,4 +1,4 @@
-// Shared device helpers for the IGMC hot-path kernels (sm_100a).
+// Shared device helpers for the IGMC hot-path kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1004,8 +1004,8 @@ extern "C" int igmc_extract_batch(const igmc_csr_t* G, const igmc_pairs_t* P, in
       return 0;
     }
   }
-  // generic two-kernel path (any hop count / capacity): 1024-thread CTAs.  Measured on the headline workload
-  // (profiles/README.md): 131 us per batch-50 at 1024 threads, 170 us at 512, 240 us at 256 - latency-bound.
+  // generic two-kernel path (any hop count / capacity): 1024-thread CTAs - the kernels are latency-bound, and more
+  // threads per subgraph keep more independent loads in flight.
   static int ex_threads = 0;
   if (!ex_threads) {
     const char* e = getenv("IGMC_EX_THREADS");

@@ -444,8 +444,9 @@ __device__ __forceinline__ float ld_relaxed_sys(const float* p) {
 //            applies the torch-Adam update
 // Two parities are enough: a rank overwrites parity p in step t + 2 only after it has seen every peer's flag t + 1,
 // which a peer raises after its step-t kernel (and thus its reads of parity p) has finished.
-// The grid (<= 300 blocks of 256 threads) is always co-resident, so spinning inside the grid is safe.
-__global__ void __launch_bounds__(256, 2)   // <= 128 registers: two blocks per SM keep the <= 296-block grid co-resident
+// Spinning inside the grid is safe only while every block is resident at once: igmc_reduce_update refuses a grid larger
+// than the device holds (two blocks per SM: 264 on an H100; the 4-layer IGMC needs 230).
+__global__ void __launch_bounds__(256, 2)   // <= 128 registers: two blocks per SM
 k_reduce_allreduce_adam(igmc_model_t M, float* __restrict__ params, int B, int rows, int NA,
                         const float* __restrict__ gpart, const float* __restrict__ dhid, const float* __restrict__ feat,
                         const float* __restrict__ hid, const float* __restrict__ dpred, const float* __restrict__ sqerr,
@@ -684,6 +685,16 @@ extern "C" int igmc_reduce_update(const igmc_model_t* M, float* params, int B, i
   if (M->readout != 0) return -16;   // external readouts write their own gradient slice: use the separate kernels
   const int NA = M->in_dim0 + (M->num_layers - 1) * HID;
   const int PBr = (M->param_count - M->conv_param_count + 255) / 256;
+  static int resident = 0;   // blocks of k_reduce_allreduce_adam the device runs at once
+  if (!resident) {
+    int dev = 0, sms = 0, per_sm = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_reduce_allreduce_adam, 256, 0);
+    if (e != cudaSuccess) return (int)e + 1000;
+    resident = sms * per_sm;
+  }
+  if (NA + PBr > resident) return -21;   // the grid barrier would wait for blocks that cannot be scheduled
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(NA + PBr);
   cfg.blockDim = dim3(256);

@@ -262,7 +262,7 @@ __device__ __forceinline__ Lists stage_lists(const uint32_t* adj, const int32_t*
 // Segments are handed out through a shared-memory ticket (`ticket`, zero on entry, reset by the caller after the
 // barrier that follows) in order of decreasing length (Ls.seg_ord): the four groups of a warp run in lockstep, so
 // segments of similar length taken at the same time keep their lanes busy (a warp-instruction of the edge loop had
-// 14 of 32 lanes active with the node-order assignment, profiles/README.md).  Which group computes a segment does
+// less than half of its lanes active with the node-order assignment).  Which group computes a segment does
 // not change its result (own staging row, fixed summation order): the output stays bitwise deterministic.
 // GL = lanes per segment (one float4 each): 8 for the 32-wide layers; 1 for a 4-wide input layer (one-hot labels) -
 // there seven of the eight lanes of a group had nothing to do, now a warp works on 32 segments at a time.
@@ -362,8 +362,8 @@ __device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], 
 }
 // x = hi + lo:  hi = x with the 13 low mantissa bits cleared (exactly a tf32 value), lo = x - hi (exact in fp32;
 // the tensor core reads its top 10 mantissa bits).  a*b ~= lo_a*hi_b + hi_a*lo_b + hi_a*hi_b  (small terms first);
-// the dropped lo*lo term and the truncation of lo are O(2^-21) relative.  cvt.rna.tf32 is NOT used: on sm_100a it
-// expands to ~16 SASS instructions per value, which made the split dominate the tile loop (profiles/).
+// the dropped lo*lo term and the truncation of lo are O(2^-21) relative.  The split is a mask and a subtraction
+// (cvt.rna.tf32 would round instead of truncate and costs more instructions per value).
 __device__ __forceinline__ void mma_3xtf32(float (&d)[4], float (&dsm)[4], const float (&af)[4], const float (&bf)[2]) {
   uint32_t ah[4], al[4], bh[2], bl[2];
 #pragma unroll
@@ -1420,11 +1420,8 @@ int rs_plan(const igmc_model_t* M, int n_cap, int cluster, int backward, int* th
       const char* e = getenv("IGMC_RS_THREADS");
       nt_env = e ? atoi(e) : 0;
     }
-    // default: 512 threads when the weight-gradient tiles fit 4 per warp with 16 warps (R <= 7); measured 4 % faster
-    // per step than 1024 threads at R = 5 (profiles/README.md)
     // 512 threads x 128 registers for every R <= 12: beyond 4 weight-gradient column tiles per warp (R > 7) the tiles
-    // run in a second pass over the nodes.  Measured on flixster (R = 10, profiles/README.md): 280 k subgraphs/s at
-    // 512 threads, 255 k at 1024 (64 registers: spills, address rematerialisation); R = 5: +5 % (round 1).
+    // run in a second pass over the nodes.  1024 threads leave 64 registers per thread, and the kernels spill there.
     int nt = 512;
     if (nt_env == 512 || nt_env == 1024) nt = nt_env;
     (void)tiles;
@@ -1440,8 +1437,8 @@ static int pdl_enabled() {
   static int v = -1;
   if (v < 0) {
     const char* e = getenv("IGMC_PDL");
-    v = e ? atoi(e) : 0;   // off by default: see profiles/README.md (a pre-launched grid that cannot be placed yet blocks the
-                            // dispatch of the extraction kernel of the other stream: 258 k subgraphs/s with, 270 k without)
+    v = e ? atoi(e) : 0;   // off by default: a pre-launched grid that cannot be placed yet blocks the dispatch of the
+                            // extraction kernel of the other stream
   }
   return v;
 }

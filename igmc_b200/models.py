@@ -1,4 +1,4 @@
-"""Drop-in for the reference's ``models.IGMC`` (models.py:170-217) on the fused sm_100a kernels.
+"""Drop-in for the reference's ``models.IGMC`` (models.py:170-217) on the fused sm_90a (H100) kernels.
 
 ``IGMC(dataset, gconv, latent_dim, num_relations, num_bases, regression, adj_dropout, ...)`` keeps the
 reference constructor, ``forward(data) -> Tensor[B]``, ``reset_parameters()``, the attribute surface
@@ -212,7 +212,6 @@ class IGMC(nn.Module):
     # ---- kernel launches ---------------------------------------------------------------------------------
     kernel_plan = "auto"   # "auto" | 0 (generic kernels) | 1 | 2 | 3 | 4 (relation-space kernels, CTAs per subgraph)
     hidden_dropout_p = 0.5   # F.dropout(x, p=0.5) before lin2 (models.py:212)
-    NUM_SMS = 148
 
     def _plan(self, batch):
         """cluster size for this batch: use the relation-space kernels when the relation count allows and
@@ -238,11 +237,11 @@ class IGMC(nn.Module):
         elif n_cap > 256 and self.num_relations <= 12:
             # large subgraphs (ml_100k*: up to 402 nodes): four CTAs per subgraph even when that is more than one wave
             # of the SMs - node features of the whole subgraph take 100 KB of every CTA's shared memory, and only with
-            # a quarter of the nodes per CTA do the edge lists still fit next to them.  Measured at batch 50
-            # (profiles/README.md): 143 k subgraphs/s with 4 CTAs, 136 k with 3, 67 k with 2.
+            # a quarter of the nodes per CTA do the edge lists still fit next to them.
             cands = [4, 3, 2, 1, 0]
         else:
-            cands = [cl for cl in (4, 2, 1) if B * cl <= self.NUM_SMS or cl == 1] + [0]
+            sms = torch.cuda.get_device_properties(self.flat_params.device).multi_processor_count
+            cands = [cl for cl in (4, 2, 1) if B * cl <= sms or cl == 1] + [0]
         for cl in cands:
             if self.__dict__.get("_max_edges") and int(cl) > 0:
                 self._cmodel.list_hint = int(1.25 * self._max_edges / int(cl)) + 256

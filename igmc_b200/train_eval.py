@@ -112,7 +112,7 @@ class TrainEngine(object):
         self.steps = 0
         # zero-copy step I/O (pipelined engine): the kernels of a step read its inputs straight out of one of two
         # pinned host buffers and the update kernel stores the step's loss into a pinned host ring - no copy-engine
-        # operation between two graph replays (the two per-step memcpys cost ~45 us of serialisation per 180 us step)
+        # operation between two graph replays (the two per-step memcpys serialise with the step's kernels)
         self.zero_copy = self.dev.type == "cuda" and os.environ.get("IGMC_ZERO_COPY", "1") != "0"
         if self.zero_copy:
             from .util_functions import mapped_view
@@ -259,10 +259,9 @@ class TrainEngine(object):
             with torch.cuda.stream(self.side):
                 if nb > 0:
                     # hold the extraction back until every cluster of this step's forward is resident: the forward
-                    # needs 100 SMs to itself (one CTA per SM); extraction CTAs that start first spread one per SM over
-                    # 50 SMs, leave room for 49 of the 50 clusters and cost the forward a second wave (measured: 235
-                    # us per step instead of 180, profiles/README.md).  Started behind it they pack two per SM on the
-                    # 48 SMs that are left.
+                    # needs one SM per CTA (100 SMs at batch 50 with 2-CTA clusters); extraction CTAs that start first
+                    # spread one per SM and can push the last clusters into a second wave.  Started behind the forward
+                    # they pack two per SM on the SMs that are left.
                     self.model.gate_wait(self.batches[slot])
                 self.batches[slot ^ 1] = self.dataset.extractor.extract(idx=buf[:nb_next], seed_dev=buf[B:B + 1],
                                                                         reuse=True, slot=slot ^ 1)

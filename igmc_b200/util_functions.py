@@ -21,7 +21,7 @@ __all__ = ["RatingGraph", "Data", "Batch", "SubgraphExtractor", "MyDynamicDatase
 
 def _require_cuda(device=None):
     if not torch.cuda.is_available():
-        raise RuntimeError("igmc_b200 needs a CUDA device (B200); there is no CPU path")
+        raise RuntimeError("igmc_b200 needs a CUDA device (H100); there is no CPU path")
     return torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
 
 

@@ -1,4 +1,4 @@
-/* igmc_b200 — C-ABI of the B200-native IGMC hot path (libigmc_b200.so).
+/* igmc_b200 — C-ABI of the H100-native IGMC hot path (libigmc_b200.so).
  *
  * The reference (muhanzhang/IGMC) has no FFI: its boundary is the Python API that Main.py
  * star-imports (Main.py:11-15).  The host side in igmc_b200/{util_functions,models,train_eval}.py
@@ -333,7 +333,8 @@ int igmc_comm_free(void* dev_ptr);
  * every step's loss (`loss.item()`, train_eval.py:176) without a copy launch or a sync.  `wprep` (optional): after
  * the update (second grid barrier) the kernel also rebuilds the prepared weights of igmc_prep_weights from the NEW
  * parameters, so that the next step's forward needs no separate preparation launch.
- * IGMC readout only (readout = 0), cluster plans only. */
+ * IGMC readout only (readout = 0), cluster plans only.  Returns -21 when the grid (one block per layer input row plus
+ * the readout parameters) is larger than the device runs at once: its grid barriers need every block resident. */
 int igmc_reduce_update(const igmc_model_t* M, float* params, int B, int gpart_rows, const float* gpart,
                        const float* dhid, const float* feat, const float* hid, const float* dpred,
                        const float* sqerr, float loss_scale, float arr, const igmc_comm_t* comm,
@@ -390,7 +391,7 @@ int igmc_sortpool_backward(const igmc_sortpool_t* P, const float* params, const 
                            const float* dpred, float* dstate, float grad_scale, float* grad, int* err,
                            void* stream);
 
-/* Version / build info: returns the compiled SM arch (100) so the host can refuse stale builds. */
+/* Version / build info: returns the compiled SM arch (90) so the host can refuse stale builds. */
 int igmc_build_info(void);
 
 #ifdef __cplusplus

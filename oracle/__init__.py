@@ -7,8 +7,8 @@ Nothing in the shipped package ``igmc_b200`` may import this package.  Only
 Contents
 --------
 ref_shim        imports the *unmodified* reference ``util_functions.py`` from
-                /root/reference (this container only; it does not travel) to
-                pin ``extract_np`` and to generate ``tests/golden``.
+                oracle/_ref/ (built by ``make_ref.py``) to pin ``extract_np``
+                and to generate ``tests/golden``.
 extract_np      numpy restatement of ``subgraph_extraction_labeling`` +
                 ``construct_pyg_graph`` + PyG collate, in canonical form.
 pyg_restated    pure-torch restatement of PyG 1.4.2 ``RGCNConv`` / ``dropout_adj``

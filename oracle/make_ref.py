@@ -1,15 +1,15 @@
 """Recipe for oracle/_ref/: the reference's OWN Python files, byte for byte, as a build product.
 
 The reference is pure Python (SURVEY.md §0: no native code, nothing to compile), so "building the reference" means
-placing the unmodified files where the checker can import them on a box that has no /root/reference:
+placing the unmodified files of a reference checkout (IGMC_REFERENCE_DIR) where the tree can import them:
 
-    python oracle/make_ref.py            # /root/reference -> oracle/_ref/{util_functions.py, Main.py}
+    python oracle/make_ref.py            # $IGMC_REFERENCE_DIR -> oracle/_ref/{util_functions.py, Main.py}
 
-oracle/_ref/ is git-ignored (no reference source enters the history) but not gpurun-ignored, so it travels with the
-repository snapshot.  Users: oracle/ref_shim.py (falls back to it), bench.py's CPU arm (extraction = the reference's
-own subgraph_extraction_labeling + construct_pyg_graph, `cpu_baseline.extraction_kind = "reference"`), and
-tests/test_gpu_main_script.py (runs the unmodified Main.py on the drop-in modules).  __graft_entry__.build() calls
-this whenever /root/reference exists.
+oracle/_ref/ is git-ignored: no reference source enters the history.  Users: oracle/ref_shim.py, bench.py's CPU arm
+(extraction = the reference's own subgraph_extraction_labeling + construct_pyg_graph,
+`cpu_baseline.extraction_kind = "reference"`), tests/golden/make_golden.py, and tests/test_gpu_main_script.py (runs
+the unmodified Main.py on the drop-in modules).  __graft_entry__.build() calls this; without a readable reference
+checkout it does nothing.
 """
 import hashlib
 import os

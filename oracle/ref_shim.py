@@ -1,14 +1,13 @@
-"""Import the UNMODIFIED reference extraction code (container only).
+"""Import the UNMODIFIED reference extraction code from oracle/_ref/ (placed there by oracle/make_ref.py).
 
-/root/reference/util_functions.py needs ``torch_geometric.data`` (line 13) for
+The reference's util_functions.py needs ``torch_geometric.data`` (line 13) for
 three class names only; we register a stub module before importing it.  On
 Python >= 3.11 ``random.sample`` refuses sets (reference line 223-229 passes
 sets), so calls are wrapped to pass ``tuple(population)`` which is what
 CPython <= 3.10 did internally.  Nothing else is changed.
 
-This module is used by ``tests/golden/make_golden.py`` and by the optional
-``test_oracle_vs_reference`` tests (skipped when /root/reference is absent, as
-on the GPU box).
+This module is used by ``tests/golden/make_golden.py`` and by bench.py's CPU
+arm (the numpy port stands in when oracle/_ref/ was not built).
 """
 import importlib.util
 import os
@@ -16,13 +15,8 @@ import random
 import sys
 import types
 
-# the reference checkout (this container), else the vendored copy oracle/make_ref.py placed under oracle/_ref/
-# (git-ignored build product that travels to the GPU box with the snapshot)
-_VENDORED = os.path.join(os.path.dirname(os.path.abspath(__file__)), "_ref")
-REF_DIR = os.environ.get("IGMC_REFERENCE_DIR", "/root/reference")
-if not os.path.isfile(os.path.join(REF_DIR, "util_functions.py")) and \
-        os.path.isfile(os.path.join(_VENDORED, "util_functions.py")):
-    REF_DIR = _VENDORED
+# the vendored copy oracle/make_ref.py places under oracle/_ref/ (a git-ignored build product)
+REF_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "_ref")
 
 
 def available():
@@ -67,7 +61,7 @@ def load():
     if _ref is not None:
         return _ref
     if not available():
-        raise RuntimeError("reference checkout not present at %s" % REF_DIR)
+        raise RuntimeError("reference code not present at %s (python oracle/make_ref.py)" % REF_DIR)
     _install_pyg_stub()
     spec = importlib.util.spec_from_file_location(
         "_igmc_reference_util_functions", os.path.join(REF_DIR, "util_functions.py"))

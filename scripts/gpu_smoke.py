@@ -1,4 +1,4 @@
-"""Small end-to-end exercise of every kernel (used under compute-sanitizer and by smoke())."""
+"""Small end-to-end exercise of every kernel (smoke())."""
 import os
 import sys
 

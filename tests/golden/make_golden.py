@@ -1,6 +1,6 @@
 """Generate tests/golden/*.npz from the UNMODIFIED reference extraction code.
 
-Run in the build container only (needs /root/reference):
+Needs the reference's own code under oracle/_ref/ (``python oracle/make_ref.py``):
 
     python tests/golden/make_golden.py
 
@@ -116,7 +116,34 @@ def main():
         rnd[tag + "__cv"] = cvv
     rnd["tags"] = np.array([s[0] for s in specs])
     np.savez_compressed(os.path.join(HERE, "random_cases.npz"), **rnd)
+    live_cases()
     print("wrote", os.listdir(HERE))
+
+
+LIVE_SPECS = ((1, None), (1, 6), (2, None), (2, 3))   # (h, max_nodes_per_hop) of tests/test_oracle_extract.py
+
+
+def live_cases():
+    """3. the first 40 training pairs of a 50 x 45 matrix per (h, mnph), reference RNG seeded with 5: canonical
+    arrays (with the reference's own draw) and the shapes of the PyG Data it built."""
+    out = {}
+    cv = np.array([1, 2, 3, 4, 5.0])
+    for h, mnph in LIVE_SPECS:
+        tag = "h%d_m%d" % (h, -1 if mnph is None else mnph)
+        u, v, lab = synth_ratings(50, 45, 420, 5, seed=99 + h)
+        A = build_adj(u, v, lab, 50, 45)
+        idx = ref_shim.make_indexers(A)
+        random.seed(5)
+        cases, shapes = [], []
+        for c in range(40):
+            canon, raw = ref_shim.extract_ref_canonical(A, int(u[c]), int(v[c]), int(lab[c]), cv, h, 1.0, mnph, idx)
+            data = raw[-1]
+            cases.append(canon)
+            shapes.append(tuple(data.x.shape) + (data.edge_index.shape[1],))
+        for k, val in pack(cases).items():
+            out["%s__%s" % (tag, k)] = val
+        out[tag + "__shapes"] = np.array(shapes, np.int64)   # [x rows, x cols, edges]
+    np.savez_compressed(os.path.join(HERE, "live_reference_cases.npz"), **out)
 
 
 if __name__ == "__main__":

@@ -27,7 +27,7 @@ def test_header_symbols_are_exported_and_bound():
 
 def test_build_info_and_plans():
     lib = _lib.load()
-    assert lib.igmc_build_info() == 100
+    assert lib.igmc_build_info() == 90
     from igmc_b200.models import IGMC
     m = IGMC(4, latent_dim=[32] * 4, num_relations=5, num_bases=4, regression=True)
     c = ctypes.byref(m._cmodel)
