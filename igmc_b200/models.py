@@ -40,7 +40,8 @@ def edge_keep_reference(seed, num_edges, p):
     """Host twin of ``edge_keep`` in csrc/common.cuh: bool keep mask for directed edges 0..E-1."""
     import numpy as np
     thresh = min(int(float(np.float32(p)) * 4294967296.0), 0xFFFFFFFF)   # the kernel sees p as fp32
-    return torch.tensor([(splitmix64((seed + e) & ((1 << 64) - 1)) >> 32) >= thresh for e in range(num_edges)])
+    return torch.tensor([(splitmix64((seed + e) & ((1 << 64) - 1)) >> 32) >= thresh for e in range(num_edges)],
+                        dtype=torch.bool)   # (a batch without edges still gets a bool mask)
 
 
 class RGCNConv(nn.Module):

@@ -1,4 +1,4 @@
-"""Shared loaders for tests/golden."""
+"""Shared loaders for tests/golden, the train-step parity check and the kernel-regime shapes of the test suite."""
 import os
 
 import numpy as np
@@ -83,6 +83,100 @@ def batch_equal(b, ob):
     out["y"] = np.array_equal(b.y.cpu().numpy(), ob["y"].astype(np.float32))
     out["node_label"] = np.array_equal(b.node_label.cpu().numpy().astype(np.int64), ob["node_labels"])
     return out
+
+
+# ---- staging regimes of the relation-space kernels (csrc/rgcn_rs.cu) and the shapes that pin them -------------------
+# Constants restated from csrc/rgcn_rs.cu: edges per segment, extra staging rows per chunk, chunks that may use extra
+# rows, destination nodes per warp group (the granularity of a CTA's node range), list-image header ints.
+SEG, XR, XCH, GN, IMG_HDR = 32, 16, 8, 4, 4
+
+# name -> shape of one regime test in tests/test_gpu_regimes.py.  ``own``: the own-node count of the CTA that enters
+# the regime in that test's batch (its subgraphs are built so that some CTA reaches it; the GPU test asserts that).
+REGIMES = {
+    # backward chunks with index >= XCH get no extra segment rows (stage_lists: allowed = ci < XCH ? ... : 0)
+    "bwd_chunks_past_xch": dict(R=12, in0=4, n_cap=202, plan=1, own=200),
+    # layer-0 weight gradient in several tile passes (backward_body, layer-0 branch: t0 > 0)
+    "layer0_tile_passes_in4": dict(R=12, in0=4, n_cap=202, plan=1, own=200),
+    "layer0_tile_passes_in8": dict(R=12, in0=8, n_cap=202, plan=1, own=180),
+    # backward lists read from global memory (Ls.lst == nullptr) while the forward's lists are staged: in-entries of
+    # the two CTAs of a 101 x 101 fully rated block (every CTA between ``entries`` bounds after 20 % edge dropout)
+    "fwd_staged_bwd_global": dict(R=5, in0=4, n_cap=202, plan=2, entries=(7400, 10600)),
+    # CTAs of a cluster that own no node (forward / backward n_own == 0 branches): a 2-node subgraph at plan 4
+    "ctas_without_nodes": dict(R=5, in0=4, n_cap=202, plan=4, n=2),
+}
+
+
+def a4(x):
+    return (x + 3) & ~3
+
+
+def a8(x):
+    return (x + 7) & ~7
+
+
+def own_cap_of(n_cap, cluster):
+    """most nodes one CTA of a ``cluster``-CTA plan owns (own_cap_of in csrc/rgcn_rs.cu)"""
+    per = (n_cap + cluster - 1) // cluster
+    return (per + GN - 1) // GN * GN
+
+
+def own_counts(n, cluster):
+    """own-node count of every CTA of a cluster for an ``n``-node subgraph (own_range in csrc/rgcn_rs.cu)"""
+    per = own_cap_of(n, cluster)
+    return [min(n, (r + 1) * per) - min(n, r * per) for r in range(cluster)]
+
+
+def layer0_tile_rows(R, in0, bwd_chunk):
+    """node rows of one layer-0 weight-gradient tile pass (``trows`` in backward_body): the pass reuses the staging
+    rows (chunk + XR rows of R*32+4 floats) as a tile of KRp + 8 floats per node."""
+    inp = a4(in0)
+    KRp = a8(R * inp) + a8(inp)
+    return ((bwd_chunk + XR) * (R * 32 + 4) // (KRp + 8)) & ~7
+
+
+def image_tables(tab_row, n_cap, cluster):
+    """(list lengths, extra-segment counts) of the own nodes of one list image row (``tab[blk]`` after
+    ``IGMC.stage_batch``): the header is followed by lptr[own_cap+4], segbase[own_cap+4], ex[own_cap+4]."""
+    import numpy as np
+    t = np.asarray(tab_row)
+    n_own, oc = int(t[3]), own_cap_of(n_cap, cluster)
+    lptr = t[IMG_HDR:IMG_HDR + n_own + 1]
+    ex = t[IMG_HDR + 2 * (oc + 4):IMG_HDR + 2 * (oc + 4) + n_own]
+    return np.diff(lptr), ex >> 16
+
+
+def check_step(m, ref, b, ob, ARR, adj_dropout, hk, step=30, edge_keep=None):
+    """One ``fused_step`` of ``m`` on batch ``b`` against fp64 autograd of the restated oracle ``ref`` on the collated
+    oracle batch ``ob``: predictions within 1e-4 RMSE, the loss within 1e-4 relative and every parameter gradient within
+    2e-4 of the largest entry of that tensor's reference gradient.  The edge dropout is the kernels' own hash draw of
+    step ``step + 1`` unless ``edge_keep`` injects one.  Returns (prediction RMSE, worst relative gradient error)."""
+    import torch
+    from oracle import pyg_restated
+    from igmc_b200.models import edge_keep_reference, splitmix64
+    E, B = ob["edge_index"].shape[1], ob["num_graphs"]
+    m._step = step
+    ek = edge_keep
+    if ek is None and adj_dropout > 0:
+        ek = edge_keep_reference(splitmix64(m.drop_seed + step + 1), E, adj_dropout)
+    tb = pyg_restated.to_torch_batch(ob, torch.float64)
+    loss_ref, out_ref = pyg_restated.train_loss(ref, tb, ARR, ek, hk)
+    loss_ref.backward()
+    loss = m.fused_step(b, ARR=ARR, hidden_keep=hk, edge_keep=edge_keep)
+    b.check()
+    ws = next(iter(v for k, v in m._ws.items() if k[2] and k[1] == B))
+    rmse = float(torch.sqrt(torch.mean((ws["pred"].double().cpu() - out_ref.detach()) ** 2)))
+    assert rmse <= 1e-4, rmse
+    assert abs(float(loss) - float(loss_ref)) <= 1e-4 * max(1.0, abs(float(loss_ref)))
+    names = {id(p): n for n, p in m.named_parameters()}
+    sd_ref = dict(ref.named_parameters())
+    worst = 0.0
+    for (o, n, s), (_, _, p) in zip(m._layout, m._named_order()):
+        gref = sd_ref[names[id(p)]].grad.reshape(-1)
+        err = float((m.flat_grad[o:o + n].double().cpu() - gref).abs().max()) / (float(gref.abs().max()) + 1e-12)
+        assert err <= 2e-4, (names[id(p)], err)
+        worst = max(worst, err)
+    print("check_step: prediction RMSE %.2e, worst relative gradient error %.2e" % (rmse, worst))
+    return rmse, worst
 
 
 def load_flixster_cases():

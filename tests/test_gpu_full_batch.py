@@ -9,31 +9,9 @@ import pytest
 import torch
 
 from oracle import extract_np, pyg_restated
+from tests.helpers import check_step
 
 pytestmark = pytest.mark.gpu
-
-
-def _check_step(m, ref, b, ob, ARR, adj_dropout, hk, step=30):
-    from igmc_b200.models import edge_keep_reference, splitmix64
-    E, B = ob["edge_index"].shape[1], ob["num_graphs"]
-    m._step = step
-    ek = edge_keep_reference(splitmix64(m.drop_seed + step + 1), E, adj_dropout) if adj_dropout > 0 else None
-    tb = pyg_restated.to_torch_batch(ob, torch.float64)
-    loss_ref, out_ref = pyg_restated.train_loss(ref, tb, ARR, ek, hk)
-    loss_ref.backward()
-    loss = m.fused_step(b, ARR=ARR, hidden_keep=hk)
-    b.check()
-    ws = next(iter(v for k, v in m._ws.items() if k[2] and k[1] == B))
-    rmse = float(torch.sqrt(torch.mean((ws["pred"].double().cpu() - out_ref.detach()) ** 2)))
-    assert rmse <= 1e-4, rmse
-    assert abs(float(loss) - float(loss_ref)) <= 1e-4 * max(1.0, abs(float(loss_ref)))
-    names = {id(p): n for n, p in m.named_parameters()}
-    sd_ref = dict(ref.named_parameters())
-    for (o, n, s), (_, _, p) in zip(m._layout, m._named_order()):
-        gref = sd_ref[names[id(p)]].grad.reshape(-1)
-        err = float((m.flat_grad[o:o + n].double().cpu() - gref).abs().max()) / (float(gref.abs().max()) + 1e-12)
-        assert err <= 2e-4, (names[id(p)], err)
-    return rmse
 
 
 @pytest.mark.parametrize("name,mnph,B,plan", [("ml_100k", 200, 50, "auto"), ("ml_1m", 100, 50, "auto"),
@@ -61,7 +39,7 @@ def test_full_batch_train_step_parity_dynamic(name, mnph, B, plan):
     m.load_state_dict({k: v.float() for k, v in ref.state_dict().items()})
     m.kernel_plan = plan
     hk = torch.rand(B, 128, generator=torch.Generator().manual_seed(2)) > 0.5
-    _check_step(m, ref, b, ob, 0.001, ds["adj_dropout"], hk)
+    check_step(m, ref, b, ob, 0.001, ds["adj_dropout"], hk)
     if plan == "auto":
         # batch 50: two CTAs per subgraph; four for the 402-node subgraphs of ml_100k* (edge lists must fit in shared
         # memory next to the node features)
@@ -99,7 +77,7 @@ def test_full_batch_train_step_parity_flixster_static():
     m = IGMC(d, latent_dim=[32] * 4, num_relations=R, num_bases=4, regression=True, adj_dropout=0.2).cuda().train()
     m.load_state_dict({k: v.float() for k, v in ref.state_dict().items()})
     hk = torch.rand(50, 128, generator=torch.Generator().manual_seed(3)) > 0.5
-    _check_step(m, ref, b, ob, 0.001, 0.2, hk)
+    check_step(m, ref, b, ob, 0.001, 0.2, hk)
     assert m._plan(b) > 0
 
 
