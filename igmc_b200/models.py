@@ -44,6 +44,18 @@ def edge_keep_reference(seed, num_edges, p):
                         dtype=torch.bool)   # (a batch without edges still gets a bool mask)
 
 
+def hidden_keep_reference(seed, num_graphs, p):
+    """Host twin of the hidden dropout before ``lin2`` (the kernels' own draw when no ``hidden_keep`` is injected):
+    bool keep mask [num_graphs, 128]; unit ``o`` of graph ``g`` is an ``edge_keep`` draw of index ``g*128 + o`` on the
+    seed ``seed ^ 0x5bd1e995a5a5a5a5``.  Kept units are scaled by 1 / (1 - p)."""
+    import numpy as np
+    M = (1 << 64) - 1
+    thresh = min(int(float(np.float32(p)) * 4294967296.0), 0xFFFFFFFF)
+    s = (seed ^ 0x5bd1e995a5a5a5a5) & M
+    keep = [(splitmix64((s + i) & M) >> 32) >= thresh for i in range(num_graphs * 128)]
+    return torch.tensor(keep, dtype=torch.bool).view(num_graphs, 128)
+
+
 class RGCNConv(nn.Module):
     """Parameter holder with PyG 1.4.2 ``RGCNConv`` names/shapes/init (SURVEY.md A.1).  The arithmetic
     lives in the fused kernels of the owning ``IGMC``."""

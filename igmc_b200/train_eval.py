@@ -96,6 +96,7 @@ class TrainEngine(object):
         self.use_graph = bool(use_graph) and hasattr(dataset, "extractor") and not hasattr(dataset, "slices")
         self.sample_seed = int(sample_seed)
         self.graphs = {}
+        self.graph_loss = {}      # loss tensor each captured step writes (a replay runs no Python: last_loss is set here)
         self.eager_done = set()
         # [idx(B) | sample_seed | drop_seed | global batch size | drop_seed of the NEXT step]  per step, pinned ring +
         # one device copy (the next step's seed is what the list images of the batch being extracted are built with)
@@ -213,11 +214,12 @@ class TrainEngine(object):
         key = (nb, G)
         if self.use_graph and key in self.graphs:
             self.graphs[key].replay()
+            self.last_loss = self.graph_loss[key]
         elif self.use_graph and key in self.eager_done and nb > 0:
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
                 self._launch(nb, G)
-            self.graphs[key] = g
+            self.graphs[key], self.graph_loss[key] = g, self.last_loss
             g.replay()
         else:
             self._launch(nb, G)
@@ -316,11 +318,12 @@ class TrainEngine(object):
         key = (nb, G, self.slot, nb_next, zc)
         if self.use_graph and key in self.graphs:
             self.graphs[key].replay()
+            self.last_loss = self.graph_loss[key]
         elif self.use_graph and key in self.eager_done:
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
                 self._launch_pipe(nb, G, self.slot, nb_next, buf)
-            self.graphs[key] = g
+            self.graphs[key], self.graph_loss[key] = g, self.last_loss
             g.replay()
         else:
             self._launch_pipe(nb, G, self.slot, nb_next, buf)
@@ -337,6 +340,7 @@ class TrainEngine(object):
         every rank calls it, nobody may still be reading a buffer that is being freed)"""
         torch.cuda.synchronize()
         self.graphs.clear()
+        self.graph_loss.clear()
         if self.exchange is not None:
             self.exchange.close()
             self.exchange = None

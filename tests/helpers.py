@@ -101,6 +101,12 @@ REGIMES = {
     # backward lists read from global memory (Ls.lst == nullptr) while the forward's lists are staged: in-entries of
     # the two CTAs of a 101 x 101 fully rated block (every CTA between ``entries`` bounds after 20 % edge dropout)
     "fwd_staged_bwd_global": dict(R=5, in0=4, n_cap=202, plan=2, entries=(7400, 10600)),
+    # eval-mode forward lists read from global memory: without dropout every in-entry of a pair inside that block counts
+    # (101 x 101 - 1 ratings, both directions), all on the one CTA of plan 1 - beyond the forward's list capacity
+    "fwd_global_eval": dict(R=5, in0=4, n_cap=202, plan=1, entries=20400),
+    # the same at mnph 200 after a sparse first batch set list_hint: a pair inside a fully rated 201 x 201 block has
+    # 90-104 own nodes with ~201 in-entries each on every CTA of plan 4, above the largest list capacity any hint buys
+    "fwd_global_eval_hinted": dict(R=5, in0=4, n_cap=402, plan=4, entries=18000),
     # CTAs of a cluster that own no node (forward / backward n_own == 0 branches): a 2-node subgraph at plan 4
     "ctas_without_nodes": dict(R=5, in0=4, n_cap=202, plan=4, n=2),
 }
@@ -145,38 +151,79 @@ def image_tables(tab_row, n_cap, cluster):
     return np.diff(lptr), ex >> 16
 
 
-def check_step(m, ref, b, ob, ARR, adj_dropout, hk, step=30, edge_keep=None):
-    """One ``fused_step`` of ``m`` on batch ``b`` against fp64 autograd of the restated oracle ``ref`` on the collated
-    oracle batch ``ob``: predictions within 1e-4 RMSE, the loss within 1e-4 relative and every parameter gradient within
-    2e-4 of the largest entry of that tensor's reference gradient.  The edge dropout is the kernels' own hash draw of
-    step ``step + 1`` unless ``edge_keep`` injects one.  Returns (prediction RMSE, worst relative gradient error)."""
+def oracle_train_step(ref, ob, ARR, edge_keep, hidden_keep):
+    """fp64 autograd of one train step of the restated oracle ``ref`` (IGMCRef or DGCNN_RSRef, train mode) on the
+    collated oracle batch ``ob``: fills the parameters' ``.grad`` and returns (loss, predictions)."""
     import torch
     from oracle import pyg_restated
-    from igmc_b200.models import edge_keep_reference, splitmix64
-    E, B = ob["edge_index"].shape[1], ob["num_graphs"]
-    m._step = step
-    ek = edge_keep
-    if ek is None and adj_dropout > 0:
-        ek = edge_keep_reference(splitmix64(m.drop_seed + step + 1), E, adj_dropout)
     tb = pyg_restated.to_torch_batch(ob, torch.float64)
-    loss_ref, out_ref = pyg_restated.train_loss(ref, tb, ARR, ek, hk)
-    loss_ref.backward()
-    loss = m.fused_step(b, ARR=ARR, hidden_keep=hk, edge_keep=edge_keep)
-    b.check()
-    ws = next(iter(v for k, v in m._ws.items() if k[2] and k[1] == B))
-    rmse = float(torch.sqrt(torch.mean((ws["pred"].double().cpu() - out_ref.detach()) ** 2)))
-    assert rmse <= 1e-4, rmse
-    assert abs(float(loss) - float(loss_ref)) <= 1e-4 * max(1.0, abs(float(loss_ref)))
+    ref.zero_grad()
+    if isinstance(ref, pyg_restated.DGCNN_RSRef):
+        out = ref(tb["x"], tb["edge_index"], tb["edge_type"], tb["batch"], edge_keep, hidden_keep, tb["num_graphs"])
+        loss = torch.nn.functional.mse_loss(out, tb["y"].view(-1))
+        if ARR != 0:
+            loss = loss + ARR * pyg_restated.arr_regulariser(ref)
+    else:
+        loss, out = pyg_restated.train_loss(ref, tb, ARR, edge_keep, hidden_keep)
+    loss.backward()
+    return loss.detach(), out.detach()
+
+
+def assert_step_matches(m, ref, pred, loss, grad, loss_ref, out_ref, tag="step"):
+    """a train step of ``m`` (device predictions ``pred``, loss ``loss``, flat gradient ``grad`` in ``m``'s layout)
+    against the oracle's (``loss_ref``, ``out_ref`` and ``ref``'s parameter ``.grad``): predictions within 1e-4 RMSE, the
+    loss within 1e-4 relative and every parameter gradient within 2e-4 of the largest entry of that tensor's reference
+    gradient (DGCNN_RS: 3e-4 of it + 2e-6 of the largest entry of any tensor, the bar of tests/test_gpu_full_batch.py:
+    its first-layer att gradients cancel to ~1e-3 of the largest).  Returns (prediction RMSE, worst gradient error in
+    units of the relative bar's scale)."""
+    import torch
+    from oracle import pyg_restated
+    rmse = float(torch.sqrt(torch.mean((pred.double().cpu() - out_ref.detach()) ** 2)))
+    assert rmse <= 1e-4, (tag, rmse)
+    assert abs(float(loss) - float(loss_ref)) <= 1e-4 * max(1.0, abs(float(loss_ref))), (tag, float(loss),
+                                                                                         float(loss_ref))
     names = {id(p): n for n, p in m.named_parameters()}
     sd_ref = dict(ref.named_parameters())
+    table = []
+    for e, (_, _, p) in zip(m._layout, m._named_order()):
+        gref = sd_ref[names[id(p)]].grad
+        table.append((names[id(p)], float((m._pview(grad, e).double().cpu() - gref).abs().max()),
+                      float(gref.abs().max())))
     worst = 0.0
-    for (o, n, s), (_, _, p) in zip(m._layout, m._named_order()):
-        gref = sd_ref[names[id(p)]].grad.reshape(-1)
-        err = float((m.flat_grad[o:o + n].double().cpu() - gref).abs().max()) / (float(gref.abs().max()) + 1e-12)
-        assert err <= 2e-4, (names[id(p)], err)
-        worst = max(worst, err)
-    print("check_step: prediction RMSE %.2e, worst relative gradient error %.2e" % (rmse, worst))
+    if isinstance(ref, pyg_restated.DGCNN_RSRef):
+        gmax = max(t[2] for t in table)
+        for name, err, scale in table:
+            assert err <= 3e-4 * scale + 2e-6 * gmax, (tag, name, err, scale, gmax)
+            worst = max(worst, err / (scale + gmax / 150.0))
+    else:
+        for name, err, scale in table:
+            rel = err / (scale + 1e-12)
+            assert rel <= 2e-4, (tag, name, rel)
+            worst = max(worst, rel)
+    print("%s: prediction RMSE %.2e, worst relative gradient error %.2e" % (tag, rmse, worst))
     return rmse, worst
+
+
+def check_step(m, ref, b, ob, ARR, adj_dropout, hk, step=30, edge_keep=None):
+    """One ``fused_step`` of ``m`` on batch ``b`` against fp64 autograd of the restated oracle ``ref`` on the collated
+    oracle batch ``ob`` (bars: ``assert_step_matches``).  The edge dropout is the kernels' own hash draw of step
+    ``step + 1`` unless ``edge_keep`` injects one; so is the hidden dropout when ``hk`` is None (the oracle then gets
+    the host twin's mask).  Returns (prediction RMSE, worst relative gradient error)."""
+    from igmc_b200.models import edge_keep_reference, hidden_keep_reference, splitmix64
+    E, B = ob["edge_index"].shape[1], ob["num_graphs"]
+    m._step = step
+    seed = splitmix64(m.drop_seed + step + 1)          # fused_step draws after its _step += 1
+    ek = edge_keep
+    if ek is None and adj_dropout > 0:
+        ek = edge_keep_reference(seed, E, adj_dropout)
+    hk_ref = hk if hk is not None else hidden_keep_reference(seed, B, m.hidden_dropout_p)
+    loss_ref, out_ref = oracle_train_step(ref, ob, ARR, ek, hk_ref)
+    loss = m.fused_step(b, ARR=ARR, hidden_keep=hk, edge_keep=edge_keep)
+    b.check()
+    assert m._step == step + 1
+    ws = next(iter(v for k, v in m._ws.items() if k[2] and k[1] == B))
+    pred = ws["sp"]["pred"] if "sp" in ws else ws["pred"]
+    return assert_step_matches(m, ref, pred, loss, m.flat_grad, loss_ref, out_ref, "check_step")
 
 
 def load_flixster_cases():

@@ -7,7 +7,7 @@ import pytest
 import torch
 
 from oracle import pyg_restated
-from igmc_b200.models import IGMC, FusedAdam, edge_keep_reference, splitmix64
+from igmc_b200.models import IGMC, FusedAdam, edge_keep_reference, hidden_keep_reference, splitmix64
 from igmc_b200.train_eval import shard_batches
 
 
@@ -79,6 +79,15 @@ def test_shard_batches_partition():
 def test_edge_keep_reference_rate():
     k = edge_keep_reference(splitmix64(7), 4000, 0.2)
     assert 0.76 < float(k.float().mean()) < 0.84
+
+
+def test_hidden_keep_reference_rate():
+    k = hidden_keep_reference(splitmix64(7), 50, 0.5)
+    assert k.dtype == torch.bool and k.shape == (50, 128)
+    assert 0.45 < float(k.float().mean()) < 0.55
+    # its own stream: not the edge draw of the same seed
+    assert not torch.equal(k.view(-1), edge_keep_reference(splitmix64(7), 50 * 128, 0.5))
+    assert bool(hidden_keep_reference(3, 2, 0.0).all()) and not bool(hidden_keep_reference(3, 2, 1.0).any())
 
 
 def _dp_worker(rank, world, port, out):

@@ -53,6 +53,20 @@ def test_fwd_staged_bwd_global():
     assert bwd.lcap < lo and fwd.lcap >= hi, ("fwd_staged_bwd_global", fwd.lcap, bwd.lcap)
 
 
+def test_fwd_global_eval():
+    r = REGIMES["fwd_global_eval"]
+    fwd = _stage(_model(r["R"], r["in0"]), r["n_cap"], r["plan"], 0)
+    assert fwd.lcap < r["entries"], ("fwd_global_eval", fwd.lcap)
+
+
+def test_fwd_global_eval_hinted():
+    r = REGIMES["fwd_global_eval_hinted"]
+    m = _model(r["R"], r["in0"])
+    m._cmodel.list_hint = 1 << 20            # any hint: the capacity it buys is capped
+    fwd = _stage(m, r["n_cap"], r["plan"], 0)
+    assert fwd.lcap < r["entries"], ("fwd_global_eval_hinted", fwd.lcap)
+
+
 def test_ctas_without_nodes():
     r = REGIMES["ctas_without_nodes"]
     assert 0 in own_counts(r["n"], r["plan"])
