@@ -23,7 +23,32 @@ ERR_NAMES = {
     3: "batch node capacity exceeded",
     4: "subgraph larger than the shared-memory plan of the model kernels (n_cap)",
     5: "malformed batch (edges not grouped by graph / node outside its graph / no target node)",
+    6: "subgraph of more than 65535 nodes (beyond the 16-bit neighbour field of the edge lists)",
 }
+
+# Kernel plan values (igmc_model_plan): 0 generic kernels, 1..4 relation-space cluster kernels (CTAs per subgraph),
+# PLAN_L2_BASE + c (c = 1, 2, 4, 8) the L2 plan with c CTAs per subgraph (IGMC_PLAN_L2 in include/igmc_b200.h).
+PLAN_L2_BASE = 16
+L2_MAX_NODES = 65535
+
+
+def plan_l2(c):
+    return PLAN_L2_BASE + int(c)
+
+
+def l2_csize(plan):
+    """CTAs per subgraph of an L2 plan value, 0 for every other plan"""
+    c = int(plan) - PLAN_L2_BASE
+    return c if c in (1, 2, 4, 8) else 0
+
+
+def is_rs(plan):
+    """a relation-space cluster plan (raw gradient rows, prepared weights, list images)"""
+    return 0 < int(plan) <= 4
+
+
+def ctas_per_graph(plan):
+    return l2_csize(plan) or max(int(plan), 1)
 
 p_i32 = C.c_void_p  # all device pointers travel as raw addresses
 vp = C.c_void_p
@@ -78,7 +103,7 @@ class Dropout(C.Structure):
 class Saved(C.Structure):
     _fields_ = [("states", vp), ("zsave", vp), ("inv_deg", vp), ("feat", vp), ("hid", vp),
                 ("hid_gscale", vp), ("pred", vp), ("target", vp), ("node_cap", C.c_int32), ("dstate", vp), ("wprep", vp), ("prof", vp),
-                ("gate", vp)]
+                ("gate", vp), ("l2_scratch", vp)]
 
 
 class Stage(C.Structure):

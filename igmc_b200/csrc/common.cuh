@@ -14,6 +14,7 @@ enum {
   IGMC_ERR_NODE_TOTAL = 3,  // batch node capacity exceeded
   IGMC_ERR_SMEM_NODES = 4,  // subgraph larger than the model kernel's shared-memory plan
   IGMC_ERR_BAD_BATCH = 5,   // edges not grouped by graph / node ids outside their graph
+  IGMC_ERR_NODE_ID16 = 6,   // subgraph of more than 65 535 nodes: beyond the 16-bit neighbour field of the lists
 };
 
 __device__ __forceinline__ void igmc_set_err(int* err, int code) {

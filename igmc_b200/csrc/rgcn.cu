@@ -11,8 +11,7 @@
 // deg(v) = number of kept incoming edges of ANY type (aggr='mean').  Backward is the same pair of
 // passes on the transposed lists with [basis ; root]^T, plus K=n weight-gradient GEMM tiles.
 // All reductions have a fixed order: results are run-to-run deterministic.
-#include "common.cuh"
-#include "../../include/igmc_b200.h"
+#include "lists.cuh"
 
 namespace {
 
@@ -22,62 +21,11 @@ constexpr int TM = 64;   // node tile of the dense phases
 constexpr int WS = 36;   // row stride of transposed weights in backward
 constexpr int HID = IGMC_HIDDEN;
 constexpr int L1O = IGMC_LIN1_OUT;
-constexpr uint32_t DROPPED = 0xFFFFFFFFu;
 
 // Activation tiles [n][32] live in shared memory with an XOR swizzle of the column by the row:
 // a row stays one contiguous 128 B line (lane = channel: conflict-free, float4 groups intact) and
 // a fixed channel over 8 consecutive rows hits 8 different banks (column reads of the dense phases).
 __device__ __forceinline__ int hix(int v, int c) { return (v << 5) + (c ^ ((v & 7) << 2)); }
-
-struct EdgeKeep {
-  bool active;
-  const uint8_t* mask;
-  uint64_t seed;
-  uint32_t thresh;
-  __device__ __forceinline__ bool keep(int e) const {
-    return mask ? (mask[e] != 0) : edge_keep(seed, (uint32_t)e, thresh);
-  }
-};
-
-__device__ __forceinline__ EdgeKeep make_keep(const igmc_dropout_t& D, int training) {
-  EdgeKeep K;
-  K.mask = D.edge_keep;
-  K.seed = D.seed_dev ? *D.seed_dev : D.seed;
-  K.active = training && (D.adj_dropout > 0.0f || D.edge_keep != nullptr);
-  double t = (double)D.adj_dropout * 4294967296.0;
-  K.thresh = t >= 4294967295.0 ? 0xFFFFFFFFu : (uint32_t)t;
-  return K;
-}
-
-// Walks list [p0,p1) of one node with the whole warp; body(nbr, type) is called warp-uniformly for
-// every kept entry, in list order.  `mirror`: the entry describes edge nbr->x but the caller wants
-// the reverse edge x->nbr of a symmetric batch, whose id is the mirror image inside the graph.
-template <class Body>
-__device__ __forceinline__ int list_foreach(const uint32_t* __restrict__ adj, const int32_t* __restrict__ eid,
-                                            int p0, int p1, const EdgeKeep& K, bool mirror, int eb, int m_half,
-                                            int lane, Body&& body) {
-  int kept = 0;
-  for (int c = p0; c < p1; c += 32) {
-    const int p = c + lane;
-    uint32_t ent = DROPPED;
-    if (p < p1) {
-      ent = adj[p];
-      if (K.active) {
-        int e = eid[p];
-        if (mirror) { const int el = e - eb; e = eb + (el < m_half ? el + m_half : el - m_half); }
-        if (!K.keep(e)) ent = DROPPED;
-      }
-    }
-    const int cnt = min(32, p1 - c);
-    for (int q = 0; q < cnt; ++q) {
-      const uint32_t en = __shfl_sync(IGMC_FULL, ent, q);
-      if (en == DROPPED) continue;
-      ++kept;
-      body((int)(en & 0xffffu), (int)((en >> 16) & 0xffu));
-    }
-  }
-  return kept;
-}
 
 // Type-run segment reduce: acc[b] = sum over kept entries of att[type][b] * feat[nbr][lane] * scale[nbr]
 template <int NB, bool SCALE>
@@ -609,6 +557,23 @@ int rs_train(const igmc_model_t* M, const float* params, const uint8_t* node_lab
              cudaStream_t st);
 int rs_gate_wait(int* gate, int target, int timeout_us, cudaStream_t st);
 
+// L2 plan (csrc/rgcn_l2.cu)
+size_t l2_smem_bytes(const igmc_model_t* M, int backward);
+int l2_forward(const igmc_model_t* M, const float* params, const uint8_t* node_label, const int32_t* node_ptr,
+               const int32_t* edge_ptr, const igmc_adj_t* A, int B, int csize, const igmc_dropout_t* D, int training,
+               const igmc_saved_t* S, const float* y, float loss_scale, float* dpred, float* sqerr, int* err,
+               cudaStream_t st);
+int l2_backward(const igmc_model_t* M, const float* params, const uint8_t* node_label, const int32_t* node_ptr,
+                const int32_t* edge_ptr, const igmc_adj_t* A, int B, int csize, const igmc_dropout_t* D,
+                const igmc_saved_t* S, const float* dpred, float* gpart, float* dhid, float* dbuf, int* err,
+                cudaStream_t st);
+
+// CTAs per subgraph of an IGMC_PLAN_L2(c) value, 0 for every other plan value
+static int l2_csize(int cluster) {
+  const int c = cluster - IGMC_PLAN_L2_BASE;
+  return (c == 1 || c == 2 || c == 4 || c == 8) ? c : 0;
+}
+
 extern "C" int igmc_gate_wait(int32_t* gate, int target, int timeout_us, void* stream) {
   if (!gate || target < 0 || timeout_us < 0) return -21;
   return rs_gate_wait(gate, target, timeout_us, (cudaStream_t)stream);
@@ -624,6 +589,11 @@ extern "C" int igmc_prep_weights(const igmc_model_t* M, const float* params, flo
 extern "C" int igmc_model_plan(const igmc_model_t* M, int n_cap, int cluster, int backward) {
   int rc = check_model(M);
   if (rc) return rc;
+  if (l2_csize(cluster)) {
+    if (n_cap > IGMC_L2_MAX_NODES) return -3;
+    const size_t b = l2_smem_bytes(M, backward);
+    return b > 227 * 1024 ? -3 : (int)b;
+  }
   if (cluster == 0) {
     const size_t b = backward ? bwd_smem_bytes(n_cap, M->num_relations, M->num_bases, M->num_layers)
                               : fwd_smem_bytes(n_cap, M->num_relations, M->num_bases, M->num_layers);
@@ -671,6 +641,11 @@ extern "C" int igmc_forward(const igmc_model_t* M, const float* params, const ui
   int rc = check_model(M);
   if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
+  if (const int c = l2_csize(cluster)) {   // (before the relation-space branch: every cluster > 0 goes there)
+    if (n_cap > IGMC_L2_MAX_NODES) return -3;
+    return l2_forward(M, params, node_label, node_ptr, edge_ptr, A, B, c, D, training, S, y, loss_scale, dpred, sqerr,
+                      err, st);
+  }
   if (cluster > 0) {
     if (!rs_supported(M)) return -16;
     if (!S->wprep) return -17;
@@ -701,7 +676,8 @@ extern "C" int igmc_forward_backward(const igmc_model_t* M, const float* params,
   if (B <= 0) return 0;
   int rc = check_model(M);
   if (rc) return rc;
-  if (cluster <= 0 || M->readout != 0 || !rs_supported(M)) return -16;   // cluster plans, IGMC readout
+  if (cluster <= 0 || l2_csize(cluster) || M->readout != 0 || !rs_supported(M)) return -16;   // relation-space plans,
+                                                                                                // IGMC readout
   if (!S->wprep || !S->zsave || !y || !dpred) return -17;
   return rs_train(M, params, node_label, node_ptr, edge_ptr, A, B, n_cap, D, S, y, loss_scale, dpred, sqerr, gpart, dhid,
                   cluster, stage_fwd, stage_bwd, err, (cudaStream_t)stream);
@@ -717,6 +693,12 @@ extern "C" int igmc_backward(const igmc_model_t* M, const float* params, const u
   if (!S->zsave) return -14;
   if (M->readout != 0 && !S->dstate) return -17;
   cudaStream_t st = (cudaStream_t)stream;
+  if (const int c = l2_csize(cluster)) {
+    if (n_cap > IGMC_L2_MAX_NODES) return -3;
+    if (!S->l2_scratch) return -17;
+    return l2_backward(M, params, node_label, node_ptr, edge_ptr, A, B, c, D, S, dpred, gpart, dhid, S->l2_scratch,
+                       err, st);
+  }
   if (cluster > 0) {
     if (!rs_supported(M)) return -16;
     if (!S->wprep) return -17;

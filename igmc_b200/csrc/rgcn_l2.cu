@@ -1,0 +1,559 @@
+// L2 plan: the generic (basis-space) message passing of csrc/rgcn.cu for enclosing subgraphs of any size up to
+// 65 535 nodes.  The other plans keep a whole subgraph's node features in shared memory, which caps the subgraph size;
+// here they live in global memory (L2-resident at these sizes) and shared memory holds only a node tile, the layer's
+// weights, att and the readout, so its size does not depend on n.
+//
+// One thread-block cluster of c CTAs (c = 1, 2, 4, 8) per subgraph; CTA `rank` owns the contiguous destination range
+// own_range(n, c, rank).  Forward: layer l is written straight into S.states[:, 32l:32l+32] and gathered from there
+// by layer l+1 (layer 0 gathers the one-hot of node_label).  Backward: two [node_cap][32] global buffers hold d pre_l
+// and d h_{l-1} and swap roles every layer.  Rows written by another CTA of the cluster during the same launch are read
+// with ld.global.cg (__ldcg) after a barrier.cluster arrive.release / wait.acquire, never through the non-coherent
+// path.  Gradients: every CTA writes one partial row in parameter layout (gpart[B*c][conv_param_count], as plan 0)
+// that igmc_grad_reduce sums in a fixed order.  No float atomics: results are run-to-run deterministic.
+#include "lists.cuh"
+
+namespace {
+
+constexpr int THREADS = 256;
+constexpr int WARPS = THREADS / 32;
+constexpr int TM = 64;              // destination-node tile of the dense phases
+constexpr int WS = 36;              // row stride of the transposed weights in backward
+constexpr int HID = IGMC_HIDDEN;
+constexpr int L1O = IGMC_LIN1_OUT;
+constexpr int MAX_NODES = 65535;    // the neighbour field of an adjacency entry is 16 bits
+
+__device__ __forceinline__ void cluster_sync_rel_acq() {
+  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
+  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+
+__device__ __forceinline__ void own_range(int n, int csize, int rank, int& v0, int& v1) {
+  const int per = (n + csize - 1) / csize;
+  v0 = min(n, rank * per);
+  v1 = min(n, v0 + per);
+}
+
+__device__ __forceinline__ size_t align4(size_t x) { return (x + 3) & ~(size_t)3; }
+
+// Type-run segment reduce over kept list entries: acc[b] = sum_runs att[type][b] * sum_run feat(nbr)
+template <int NB, class Feat>
+__device__ __forceinline__ int gather_runs(const uint32_t* __restrict__ adj, const int32_t* __restrict__ eid, int p0,
+                                           int p1, const EdgeKeep& K, bool mirror, int eb, int m_half, int lane,
+                                           Feat&& feat, const float* __restrict__ att_s, float (&acc)[NB]) {
+  float run = 0.f;
+  int cur = -1;
+#pragma unroll
+  for (int b = 0; b < NB; ++b) acc[b] = 0.f;
+  const int kept = list_foreach(adj, eid, p0, p1, K, mirror, eb, m_half, lane, [&](int nbr, int ty) {
+    if (ty != cur) {
+      if (cur >= 0) {
+#pragma unroll
+        for (int b = 0; b < NB; ++b) acc[b] = fmaf(att_s[cur * NB + b], run, acc[b]);
+      }
+      run = 0.f;
+      cur = ty;
+    }
+    run += feat(nbr);
+  });
+  if (cur >= 0) {
+#pragma unroll
+    for (int b = 0; b < NB; ++b) acc[b] = fmaf(att_s[cur * NB + b], run, acc[b]);
+  }
+  return kept;
+}
+
+// h_{l-1}[v][c]: one-hot of the node label for l = 0, else layer l-1 of concat_states (possibly another CTA's row)
+struct PrevLayer {
+  const uint8_t* label;
+  const float* states;
+  int l, in0, CW;
+  __device__ __forceinline__ float operator()(int v, int c) const {
+    if (l == 0) return (c == (int)label[v] && c < in0) ? 1.f : 0.f;
+    return __ldcg(states + (size_t)v * CW + (l - 1) * HID + c);
+  }
+};
+
+// ------------------------------------------------------------------------------------------------
+// forward
+// ------------------------------------------------------------------------------------------------
+template <int NB>
+__global__ void __launch_bounds__(THREADS)
+k_l2_forward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __restrict__ node_label,
+             const int32_t* __restrict__ node_ptr, const int32_t* __restrict__ edge_ptr, igmc_adj_t A, int csize,
+             igmc_dropout_t D, int training, igmc_saved_t S, const float* __restrict__ y, float loss_scale,
+             float* __restrict__ dpred, float* __restrict__ sqerr, int* err) {
+  extern __shared__ __align__(16) float smem[];
+  constexpr int ZS = (NB + 1) * HID + 4;   // tile row: [Z (NB*in) | h_{l-1} (in)]
+  const int L = M.num_layers, R = M.num_relations, CW = HID * L, F = 2 * CW;
+  float* Zs = smem;
+  float* Wc = Zs + TM * ZS;                // [basis ; root] rows
+  float* att_s = Wc + (NB + 1) * HID * HID;
+  float* bias_s = att_s + align4((size_t)R * NB);
+  float* feat_s = bias_s + HID;
+  float* hid_s = feat_s + align4(F);
+  __shared__ int s_t[2];
+
+  const int g = blockIdx.x / csize, rank = blockIdx.x % csize;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int nb = node_ptr[g], n = node_ptr[g + 1] - nb;
+  const int eb = edge_ptr[g], m_half = (edge_ptr[g + 1] - eb) >> 1;
+  if (n > MAX_NODES) {   // (the whole cluster returns: no CTA waits at a barrier)
+    if (tid == 0) igmc_set_err(err, IGMC_ERR_NODE_ID16);
+    return;
+  }
+  const EdgeKeep K = make_keep(D, training);
+  const int in0 = M.in_dim0;
+  int v0, v1;
+  own_range(n, csize, rank, v0, v1);
+
+  // target rows (models.py:205-206): every CTA of the cluster scans the labels, so all of them agree
+  if (tid == 0) { s_t[0] = 0x7fffffff; s_t[1] = 0x7fffffff; }
+  __syncthreads();
+  for (int v = tid; v < n; v += THREADS) {
+    const int lab = node_label[nb + v];
+    if (lab == 0) atomicMin(&s_t[0], v);
+    if (lab == 1) atomicMin(&s_t[1], v);
+  }
+  __syncthreads();
+  const int tu = s_t[0], ti = s_t[1];
+  if (M.readout == 0 && (tu >= n || ti >= n)) {
+    if (tid == 0) igmc_set_err(err, IGMC_ERR_BAD_BATCH);
+    return;
+  }
+
+  for (int l = 0; l < L; ++l) {
+    const int in = l == 0 ? in0 : HID;
+    const int K1 = NB * in;
+    const PrevLayer hp{node_label + nb, S.states + (size_t)nb * CW, l, in0, CW};
+    {
+      const float* bs = params + M.off_basis[l];
+      const float* rt = params + M.off_root[l];
+      for (int idx = tid; idx < K1 * HID; idx += THREADS) Wc[idx] = bs[idx];
+      for (int idx = tid; idx < in * HID; idx += THREADS) Wc[K1 * HID + idx] = rt[idx];
+      for (int idx = tid; idx < R * NB; idx += THREADS) att_s[idx] = params[M.off_att[l] + idx];
+      if (tid < HID) bias_s[tid] = params[M.off_bias[l] + tid];
+    }
+    __syncthreads();
+    for (int t0 = v0; t0 < v1; t0 += TM) {
+      const int tend = min(t0 + TM, v1);
+      // ---- phase G: basis-space aggregate of the tile's nodes (warp per destination node) + their own rows ----
+      for (int v = t0 + warp; v < tend; v += WARPS) {
+        float z[NB];
+        const int kept = gather_runs<NB>(A.in_adj, A.in_eid, A.in_ptr[nb + v], A.in_ptr[nb + v + 1], K, false, eb,
+                                         m_half, lane, [&](int u) { return hp(u, lane); }, att_s, z);
+        const float id = 1.f / (float)max(kept, 1);   // kept in-degree: the same for every layer
+        if (l == 0 && lane == 0) S.inv_deg[nb + v] = id;
+        float* zr = Zs + (v - t0) * ZS;
+#pragma unroll
+        for (int b = 0; b < NB; ++b) {
+          z[b] *= id;
+          if (lane < in) zr[b * in + lane] = z[b];
+          if (S.zsave) S.zsave[((size_t)l * S.node_cap + nb + v) * (NB * HID) + b * HID + lane] = z[b];
+        }
+        if (lane < in) zr[K1 + lane] = hp(v, lane);
+      }
+      __syncthreads();
+      // ---- phase T: [Z | h] . [basis ; root] + bias, tanh (thread = 2 nodes x 4 channels) ----
+      {
+        const int r0 = (tid >> 3) * 2, c0 = (tid & 7) * 4;
+        float a0[4], a1[4];
+#pragma unroll
+        for (int c = 0; c < 4; ++c) { a0[c] = bias_s[c0 + c]; a1[c] = a0[c]; }
+        const float* z0 = Zs + r0 * ZS;
+        const float* z1 = z0 + ZS;
+        for (int kk = 0; kk < K1 + in; ++kk) {
+          const float x0 = z0[kk], x1 = z1[kk];
+          const float4 w = *reinterpret_cast<const float4*>(Wc + kk * HID + c0);
+          a0[0] = fmaf(x0, w.x, a0[0]); a0[1] = fmaf(x0, w.y, a0[1]); a0[2] = fmaf(x0, w.z, a0[2]); a0[3] = fmaf(x0, w.w, a0[3]);
+          a1[0] = fmaf(x1, w.x, a1[0]); a1[1] = fmaf(x1, w.y, a1[1]); a1[2] = fmaf(x1, w.z, a1[2]); a1[3] = fmaf(x1, w.w, a1[3]);
+        }
+        const int va = t0 + r0, vb = va + 1;
+        if (va < tend)
+          *reinterpret_cast<float4*>(S.states + (size_t)(nb + va) * CW + l * HID + c0) =
+              make_float4(tanhf(a0[0]), tanhf(a0[1]), tanhf(a0[2]), tanhf(a0[3]));
+        if (vb < tend)
+          *reinterpret_cast<float4*>(S.states + (size_t)(nb + vb) * CW + l * HID + c0) =
+              make_float4(tanhf(a1[0]), tanhf(a1[1]), tanhf(a1[2]), tanhf(a1[3]));
+      }
+      __syncthreads();
+    }
+    cluster_sync_rel_acq();   // layer l of every CTA's nodes is in L2 before any CTA gathers it
+  }
+
+  if (M.readout != 0 || rank != 0) return;   // concat_states only (csrc/sortpool.cu takes over) / readout on rank 0
+  // ---- readout: concat rows of the target user and item (models.py:205-207) ----
+  for (int c = tid; c < F; c += THREADS) {
+    const int node = c < CW ? tu : ti;
+    const float v = __ldcg(S.states + (size_t)(nb + node) * CW + (c < CW ? c : c - CW));
+    feat_s[c] = v;
+    S.feat[(size_t)g * F + c] = v;
+  }
+  if (tid == 0) { S.target[2 * g] = nb + tu; S.target[2 * g + 1] = nb + ti; }
+  __syncthreads();
+  const float* W1 = params + M.off_lin1_w;
+  for (int o = warp; o < L1O; o += WARPS) {
+    float s = 0.f;
+    for (int i = lane; i < F; i += 32) s = fmaf(W1[(size_t)o * F + i], feat_s[i], s);
+    s = warp_sum_f(s);
+    if (lane == 0) {
+      float h = fmaxf(s + params[M.off_lin1_b + o], 0.f);                 // relu(lin1) models.py:211
+      float scale = 1.f;
+      if (training && (D.hidden_dropout > 0.f || D.hidden_keep)) {        // F.dropout models.py:212
+        bool keep;
+        if (D.hidden_keep) keep = D.hidden_keep[(size_t)g * L1O + o] != 0;
+        else {
+          double t = (double)D.hidden_dropout * 4294967296.0;
+          keep = edge_keep(K.seed ^ 0x5bd1e995a5a5a5a5ull, (uint32_t)(g * L1O + o),
+                           t >= 4294967295.0 ? 0xFFFFFFFFu : (uint32_t)t);
+        }
+        const float p = D.hidden_keep ? 0.5f : D.hidden_dropout;
+        scale = keep ? 1.f / (1.f - p) : 0.f;
+      }
+      hid_s[o] = h * scale;
+      S.hid[(size_t)g * L1O + o] = h * scale;
+      S.hid_gscale[(size_t)g * L1O + o] = h > 0.f ? scale : 0.f;
+    }
+  }
+  __syncthreads();
+  if (warp == 0) {
+    float s = 0.f;
+    for (int o = lane; o < L1O; o += 32) s = fmaf(params[M.off_lin2_w + o], hid_s[o], s);
+    s = warp_sum_f(s);
+    if (lane == 0) {
+      const float out = (s + params[M.off_lin2_b]) * M.multiply_by;       // models.py:213-215
+      S.pred[g] = out;
+      if (y) {
+        const float diff = out - y[g];
+        if (sqerr) sqerr[g] = diff * diff;
+        if (dpred) dpred[g] = 2.f * diff * loss_scale * M.multiply_by;   // d mse / d lin2-output
+      }
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// backward
+// ------------------------------------------------------------------------------------------------
+template <int NB>
+__global__ void __launch_bounds__(THREADS)
+k_l2_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __restrict__ node_label,
+              const int32_t* __restrict__ node_ptr, const int32_t* __restrict__ edge_ptr, igmc_adj_t A, int csize,
+              igmc_dropout_t D, igmc_saved_t S, const float* __restrict__ dpred, float* __restrict__ gpart,
+              float* __restrict__ dhid_out, float* __restrict__ dbuf, int* err) {
+  extern __shared__ __align__(16) float smem[];
+  constexpr int ZB = (NB + 2) * HID + 4;   // tile row: [Z or G or dZ' (NB*32) | d pre (32) | h_{l-1} (32)]
+  constexpr int ZS2 = NB * HID + 4;        // row stride of basis^T in the d att pass
+  constexpr int WT = (NB + 1) * HID * WS > HID * ZS2 ? (NB + 1) * HID * WS : HID * ZS2;
+  const int L = M.num_layers, R = M.num_relations, CW = HID * L, F = 2 * CW;
+  float* Zs = smem;
+  float* Wt = Zs + TM * ZB;                // transposed [basis ; root] | basis as W2[j][b*32+k]
+  float* att_s = Wt + WT;
+  float* dfeat = att_s + align4((size_t)R * NB);
+  float* dhid_s = dfeat + align4(F);
+  double* datt_w = reinterpret_cast<double*>(dhid_s + L1O);   // [WARPS][R*NB], fp64: the sums over a large
+                                                                 // subgraph cancel to a small fraction of their terms
+
+  const int g = blockIdx.x / csize, rank = blockIdx.x % csize;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int nb = node_ptr[g], n = node_ptr[g + 1] - nb;
+  const int eb = edge_ptr[g], m_half = (edge_ptr[g + 1] - eb) >> 1;
+  if (n > MAX_NODES) {
+    if (tid == 0) igmc_set_err(err, IGMC_ERR_NODE_ID16);
+    return;
+  }
+  const EdgeKeep K = make_keep(D, 1);
+  const bool sym = A.symmetric != 0;
+  const int32_t* optr = sym ? A.in_ptr : A.out_ptr;
+  const uint32_t* oadj = sym ? A.in_adj : A.out_adj;
+  const int32_t* oeid = sym ? A.in_eid : A.out_eid;
+  const int in0 = M.in_dim0;
+  const bool ext = M.readout != 0;   // d concat_states comes from an external readout (S.dstate)
+  const int tu = ext ? -1 : S.target[2 * g] - nb, ti = ext ? -1 : S.target[2 * g + 1] - nb;
+  float* gp = gpart + (size_t)blockIdx.x * M.conv_param_count;
+  const float* invdeg = S.inv_deg + nb;
+  const float* states = S.states + (size_t)nb * CW;
+  int v0, v1;
+  own_range(n, csize, rank, v0, v1);
+
+  // ---- readout backward: d hid, d feat (models.py:211-213) ----
+  if (!ext) {
+    const float dp = dpred[g];
+    for (int o = tid; o < L1O; o += THREADS) {
+      const float d = dp * params[M.off_lin2_w + o] * S.hid_gscale[(size_t)g * L1O + o];
+      dhid_s[o] = d;
+      if (rank == 0) dhid_out[(size_t)g * L1O + o] = d;
+    }
+    __syncthreads();
+    const float* W1 = params + M.off_lin1_w;
+    for (int i = tid; i < F; i += THREADS) {
+      float s = 0.f;
+      for (int o = 0; o < L1O; ++o) s = fmaf(W1[(size_t)o * F + i], dhid_s[o], s);
+      dfeat[i] = s;
+    }
+  }
+  __syncthreads();
+  // d loss / d h_l[v][c] from the readout: S.dstate (external readout) and the two target rows
+  auto seed = [&](int l, int v, int c) {
+    float gval = 0.f;
+    if (ext) gval = S.dstate[(size_t)(nb + v) * CW + l * HID + c];
+    if (v == tu) gval += dfeat[l * HID + c];
+    if (v == ti) gval += dfeat[CW + l * HID + c];
+    return gval;
+  };
+
+  for (int l = L - 1; l >= 0; --l) {
+    const int in = l == 0 ? in0 : HID;
+    float* X = dbuf + (size_t)((L - 1 - l) & 1) * S.node_cap * HID + (size_t)nb * HID;   // d h_l -> d pre_l
+    float* Y = dbuf + (size_t)((L - l) & 1) * S.node_cap * HID + (size_t)nb * HID;       // d h_{l-1}
+    const PrevLayer hp{node_label + nb, states, l, in0, CW};
+    // (0) d pre = d h * (1 - h^2) of the own nodes, in place
+    for (int idx = tid; idx < (v1 - v0) * HID; idx += THREADS) {
+      const int v = v0 + (idx >> 5), c = idx & 31;
+      const float dh = l == L - 1 ? seed(l, v, c) : __ldcg(X + (size_t)v * HID + c);
+      const float h = __ldcg(states + (size_t)v * CW + l * HID + c);
+      X[(size_t)v * HID + c] = dh * (1.f - h * h);
+    }
+    for (int idx = tid; idx < R * NB; idx += THREADS) att_s[idx] = params[M.off_att[l] + idx];
+    for (int idx = tid; idx < WARPS * R * NB; idx += THREADS) datt_w[idx] = 0.f;
+    // d pre_l of every node of the subgraph is in L2 from here on.  (Y, written below, was last read by the previous
+    // layer's pass (1) of the other CTAs, which they finished before arriving here.)
+    cluster_sync_rel_acq();
+
+    // (1) data gradient: d h_{l-1} = readout rows + [G | dpre] . [basis ; root]^T, G = out-list aggregate of dpre/deg
+    if (l > 0) {
+      const float* bs = params + M.off_basis[l];
+      const float* rt = params + M.off_root[l];
+      for (int idx = tid; idx < NB * HID * HID; idx += THREADS) {   // basis[b][k][j] -> Wt[(b*32+j)][k]
+        const int j = idx & 31, k = (idx >> 5) & 31, b = idx >> 10;
+        Wt[(b * HID + j) * WS + k] = bs[idx];
+      }
+      for (int idx = tid; idx < HID * HID; idx += THREADS) {        // root[k][j] -> Wt[(NB*32+j)][k]
+        const int j = idx & 31, k = idx >> 5;
+        Wt[(NB * HID + j) * WS + k] = rt[idx];
+      }
+      __syncthreads();
+      for (int t0 = v0; t0 < v1; t0 += TM) {
+        const int tend = min(t0 + TM, v1);
+        for (int u = t0 + warp; u < tend; u += WARPS) {
+          float gz[NB];
+          gather_runs<NB>(oadj, oeid, optr[nb + u], optr[nb + u + 1], K, sym, eb, m_half, lane,
+                          [&](int w) { return __ldcg(X + (size_t)w * HID + lane) * __ldcg(invdeg + w); }, att_s, gz);
+          float* zr = Zs + (u - t0) * ZB;
+#pragma unroll
+          for (int b = 0; b < NB; ++b) zr[b * HID + lane] = gz[b];
+          zr[NB * HID + lane] = __ldcg(X + (size_t)u * HID + lane);
+        }
+        __syncthreads();
+        {
+          const int r0 = (tid >> 3) * 2, c0 = (tid & 7) * 4;
+          float a0[4] = {0.f, 0.f, 0.f, 0.f}, a1[4] = {0.f, 0.f, 0.f, 0.f};
+          const float* z0 = Zs + r0 * ZB;
+          const float* z1 = z0 + ZB;
+          for (int kk = 0; kk < (NB + 1) * HID; ++kk) {
+            const float x0 = z0[kk], x1 = z1[kk];
+            const float4 w = *reinterpret_cast<const float4*>(Wt + kk * WS + c0);
+            a0[0] = fmaf(x0, w.x, a0[0]); a0[1] = fmaf(x0, w.y, a0[1]); a0[2] = fmaf(x0, w.z, a0[2]); a0[3] = fmaf(x0, w.w, a0[3]);
+            a1[0] = fmaf(x1, w.x, a1[0]); a1[1] = fmaf(x1, w.y, a1[1]); a1[2] = fmaf(x1, w.z, a1[2]); a1[3] = fmaf(x1, w.w, a1[3]);
+          }
+          const int va = t0 + r0, vb = va + 1;
+          if (va < tend) {
+            float4 t;
+            t.x = seed(l - 1, va, c0) + a0[0]; t.y = seed(l - 1, va, c0 + 1) + a0[1];
+            t.z = seed(l - 1, va, c0 + 2) + a0[2]; t.w = seed(l - 1, va, c0 + 3) + a0[3];
+            *reinterpret_cast<float4*>(Y + (size_t)va * HID + c0) = t;
+          }
+          if (vb < tend) {
+            float4 t;
+            t.x = seed(l - 1, vb, c0) + a1[0]; t.y = seed(l - 1, vb, c0 + 1) + a1[1];
+            t.z = seed(l - 1, vb, c0 + 2) + a1[2]; t.w = seed(l - 1, vb, c0 + 3) + a1[3];
+            *reinterpret_cast<float4*>(Y + (size_t)vb * HID + c0) = t;
+          }
+        }
+        __syncthreads();
+      }
+    }
+
+    // (2) weight gradients d[basis ; root] = [Z | h_{l-1}]^T . dpre (K = own nodes), d bias = sum_v dpre, and
+    // (3) d att[r,b] = sum_v sum_{in-runs of type r} < sum_run h_{l-1}[src,:] , dZ'[v,b,:] >,
+    //     dZ'[v,b,k] = 1/deg(v) * sum_j dpre[v,j] basis[b][k][j]  - one pass over the own-node tiles
+    {
+      const float* bs = params + M.off_basis[l];
+      for (int idx = tid; idx < NB * in * HID; idx += THREADS) {   // basis[b][k][j] -> W2[j][b*32+k]
+        const int j = idx & 31, k = (idx >> 5) % in, b = (idx >> 5) / in;
+        Wt[j * ZS2 + b * HID + k] = bs[idx];
+      }
+      const int kg = tid >> 3, c0 = (tid & 7) * 4;   // thread: row kg, channels c0..c0+3
+      float acc[NB + 1][4];
+      float accb[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+      for (int i = 0; i <= NB; ++i)
+#pragma unroll
+        for (int c = 0; c < 4; ++c) acc[i][c] = 0.f;
+      double* dw = datt_w + warp * (R * NB);
+      for (int t0 = v0; t0 < v1; t0 += TM) {
+        const int tend = min(t0 + TM, v1), rows = tend - t0;
+        for (int idx = tid; idx < rows * (NB * HID); idx += THREADS) {
+          const int r = idx / (NB * HID), c = idx - r * (NB * HID);
+          Zs[r * ZB + c] = S.zsave[((size_t)l * S.node_cap + nb + t0 + r) * (NB * HID) + c];
+        }
+        for (int idx = tid; idx < rows * HID; idx += THREADS) {
+          const int r = idx >> 5, c = idx & 31;
+          Zs[r * ZB + NB * HID + c] = __ldcg(X + (size_t)(t0 + r) * HID + c);
+          Zs[r * ZB + (NB + 1) * HID + c] = hp(t0 + r, c);
+        }
+        __syncthreads();
+        if (kg < in) {
+          for (int r = 0; r < rows; ++r) {
+            const float* zr = Zs + r * ZB;
+            const float4 d = *reinterpret_cast<const float4*>(zr + NB * HID + c0);
+#pragma unroll
+            for (int i = 0; i < NB; ++i) {
+              const float zv = zr[i * HID + kg];
+              acc[i][0] = fmaf(zv, d.x, acc[i][0]); acc[i][1] = fmaf(zv, d.y, acc[i][1]);
+              acc[i][2] = fmaf(zv, d.z, acc[i][2]); acc[i][3] = fmaf(zv, d.w, acc[i][3]);
+            }
+            const float hv = zr[(NB + 1) * HID + kg];
+            acc[NB][0] = fmaf(hv, d.x, acc[NB][0]); acc[NB][1] = fmaf(hv, d.y, acc[NB][1]);
+            acc[NB][2] = fmaf(hv, d.z, acc[NB][2]); acc[NB][3] = fmaf(hv, d.w, acc[NB][3]);
+            if (kg == 0) { accb[0] += d.x; accb[1] += d.y; accb[2] += d.z; accb[3] += d.w; }
+          }
+        }
+        __syncthreads();
+        {
+          // dZ' of the tile's nodes over the Z columns (thread: node r = tid/4, columns [cg*8NB, (cg+1)*8NB))
+          const int r = tid >> 2, cg = tid & 3;
+          constexpr int CPT = 8 * NB;
+          float a[CPT];
+#pragma unroll
+          for (int c = 0; c < CPT; ++c) a[c] = 0.f;
+          if (r < rows) {
+            const float* dr = Zs + r * ZB + NB * HID;
+            for (int j = 0; j < HID; ++j) {
+              const float x = dr[j];
+              const float* w = Wt + j * ZS2 + cg * CPT;
+#pragma unroll
+              for (int c = 0; c < CPT; c += 4) {
+                const float4 w4 = *reinterpret_cast<const float4*>(w + c);
+                a[c] = fmaf(x, w4.x, a[c]); a[c + 1] = fmaf(x, w4.y, a[c + 1]);
+                a[c + 2] = fmaf(x, w4.z, a[c + 2]); a[c + 3] = fmaf(x, w4.w, a[c + 3]);
+              }
+            }
+          }
+          __syncthreads();   // every thread of the row has read d pre before the row's Z columns are overwritten
+          if (r < rows) {
+            const float id = __ldcg(invdeg + t0 + r);
+#pragma unroll
+            for (int c = 0; c < CPT; ++c) Zs[r * ZB + cg * CPT + c] = a[c] * id;
+          }
+        }
+        __syncthreads();
+        for (int v = t0 + warp; v < tend; v += WARPS) {
+          float dz[NB];
+#pragma unroll
+          for (int b = 0; b < NB; ++b) dz[b] = (lane < in) ? Zs[(v - t0) * ZB + b * HID + lane] : 0.f;
+          float run = 0.f;
+          int cur = -1;
+          auto flush = [&]() {
+#pragma unroll
+            for (int b = 0; b < NB; ++b) {
+              const float p = warp_sum_f(run * dz[b]);
+              if (lane == 0) dw[cur * NB + b] += (double)p;
+            }
+          };
+          list_foreach(A.in_adj, A.in_eid, A.in_ptr[nb + v], A.in_ptr[nb + v + 1], K, false, eb, m_half, lane,
+                       [&](int nbr, int ty) {
+                         if (ty != cur) {
+                           if (cur >= 0) flush();
+                           run = 0.f;
+                           cur = ty;
+                         }
+                         run += hp(nbr, lane);
+                       });
+          if (cur >= 0) flush();
+        }
+        __syncthreads();
+      }
+      if (kg < in) {
+#pragma unroll
+        for (int i = 0; i < NB; ++i)
+          *reinterpret_cast<float4*>(gp + M.off_basis[l] + (i * in + kg) * HID + c0) =
+              make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
+        *reinterpret_cast<float4*>(gp + M.off_root[l] + kg * HID + c0) =
+            make_float4(acc[NB][0], acc[NB][1], acc[NB][2], acc[NB][3]);
+        if (kg == 0)
+          *reinterpret_cast<float4*>(gp + M.off_bias[l] + c0) = make_float4(accb[0], accb[1], accb[2], accb[3]);
+      }
+      __syncthreads();
+      for (int idx = tid; idx < R * NB; idx += THREADS) {
+        double s = 0.0;
+        for (int w = 0; w < WARPS; ++w) s += datt_w[w * (R * NB) + idx];
+        gp[M.off_att[l] + idx] = (float)s;
+      }
+      __syncthreads();
+    }
+  }
+}
+
+size_t fwd_smem(int R, int NB, int L) {
+  const size_t ZS = (NB + 1) * HID + 4, F = 2 * HID * L;
+  const size_t fl = TM * ZS + (size_t)(NB + 1) * HID * HID + ((R * NB + 3) & ~3) + HID + ((F + 3) & ~3) + L1O;
+  return fl * sizeof(float);
+}
+size_t bwd_smem(int R, int NB, int L) {
+  const size_t ZB = (NB + 2) * HID + 4, ZS2 = NB * HID + 4, F = 2 * HID * L;
+  size_t wt = (size_t)(NB + 1) * HID * WS;
+  if (HID * ZS2 > wt) wt = HID * ZS2;
+  const size_t fl = TM * ZB + wt + ((R * NB + 3) & ~3) + ((F + 3) & ~3) + L1O + 2 * (size_t)WARPS * R * NB;
+  return fl * sizeof(float);
+}
+
+template <class Kern, class... Args>
+int launch(Kern kern, int B, int csize, size_t smem, cudaStream_t st, Args... args) {
+  cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(B * csize);
+  cfg.blockDim = dim3(THREADS);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeClusterDimension;
+  at[0].val.clusterDim.x = csize;
+  at[0].val.clusterDim.y = 1;
+  at[0].val.clusterDim.z = 1;
+  cfg.attrs = at;
+  cfg.numAttrs = 1;
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, args...);
+  return e != cudaSuccess ? (int)e + 1000 : 0;
+}
+
+}  // namespace
+
+// bytes of dynamic shared memory of the L2 plan's forward / backward kernel (independent of the subgraph size)
+size_t l2_smem_bytes(const igmc_model_t* M, int backward) {
+  return backward ? bwd_smem(M->num_relations, M->num_bases, M->num_layers)
+                  : fwd_smem(M->num_relations, M->num_bases, M->num_layers);
+}
+
+int l2_forward(const igmc_model_t* M, const float* params, const uint8_t* node_label, const int32_t* node_ptr,
+               const int32_t* edge_ptr, const igmc_adj_t* A, int B, int csize, const igmc_dropout_t* D, int training,
+               const igmc_saved_t* S, const float* y, float loss_scale, float* dpred, float* sqerr, int* err,
+               cudaStream_t st) {
+  const size_t smem = l2_smem_bytes(M, 0);
+  if (M->num_bases == 4)
+    return launch(k_l2_forward<4>, B, csize, smem, st, *M, params, node_label, node_ptr, edge_ptr, *A, csize, *D,
+                  training, *S, y, loss_scale, dpred, sqerr, err);
+  return launch(k_l2_forward<2>, B, csize, smem, st, *M, params, node_label, node_ptr, edge_ptr, *A, csize, *D,
+                training, *S, y, loss_scale, dpred, sqerr, err);
+}
+
+int l2_backward(const igmc_model_t* M, const float* params, const uint8_t* node_label, const int32_t* node_ptr,
+                const int32_t* edge_ptr, const igmc_adj_t* A, int B, int csize, const igmc_dropout_t* D,
+                const igmc_saved_t* S, const float* dpred, float* gpart, float* dhid, float* dbuf, int* err,
+                cudaStream_t st) {
+  const size_t smem = l2_smem_bytes(M, 1);
+  if (M->num_bases == 4)
+    return launch(k_l2_backward<4>, B, csize, smem, st, *M, params, node_label, node_ptr, edge_ptr, *A, csize, *D, *S,
+                  dpred, gpart, dhid, dbuf, err);
+  return launch(k_l2_backward<2>, B, csize, smem, st, *M, params, node_label, node_ptr, edge_ptr, *A, csize, *D, *S,
+                dpred, gpart, dhid, dbuf, err);
+}

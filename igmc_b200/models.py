@@ -56,6 +56,52 @@ def hidden_keep_reference(seed, num_graphs, p):
     return torch.tensor(keep, dtype=torch.bool).view(num_graphs, 128)
 
 
+def l2_cluster(n_cap, B, sms):
+    """CTAs per subgraph of the L2 plan (csrc/rgcn_l2.cu).  A CTA owns a contiguous range of destination nodes and
+    works through it in 64-node tiles; the cluster shares one subgraph's layers through L2 with one cluster barrier
+    per layer.  Rule: the most CTAs (8, 4, 2, 1) that keep the grid within four CTAs per SM and still give every CTA
+    at least one tile of the largest subgraph.  Measured at batch 50 only, on an H100 80GB HBM3 (700 W), train step
+    subgraphs/s with 1 / 2 / 4 / 8 CTAs (scripts/large_subgraph_rate.py): ml_100k* h = 1 without a node cap (n_cap
+    1236) 3.3 k / 5.6 k / 8.3 k / 13.1 k; h = 2 at mnph 200 (n_cap 802) 3.2 k / 5.9 k / 8.1 k / 10.2 k; R = 71 at n_cap
+    564: 5.3 k / 9.9 k / 17.6 k / 17.5 k.  More CTAs per subgraph never lost, even past one wave (400 CTAs on 132
+    SMs).  The four-per-SM bound (other batch sizes) and the one-tile bound (smaller n_cap) are unmeasured choices."""
+    for c in (8, 4, 2):
+        if B * c <= 4 * sms and n_cap >= 64 * c:
+            return c
+    return 1
+
+
+def select_plan(cmodel, n_cap, B, sms, want="auto", max_edges=None):
+    """kernel plan of ``cmodel`` for batches of ``B`` subgraphs of up to ``n_cap`` nodes on a device with ``sms`` SMs
+    (host only: plan queries through igmc_model_plan).  ``want`` forces one plan value; ``max_edges`` (longest
+    per-subgraph directed edge list seen) sizes the list buffers of the relation-space plans through
+    ``cmodel.list_hint``.  Raises RuntimeError when no plan accepts the shape."""
+    lib = _lib.load()
+    R = cmodel.num_relations
+    if want != "auto":
+        cands = [int(want)]
+    elif n_cap > 256 and R <= 12:
+        # large subgraphs (ml_100k*: up to 402 nodes): four CTAs per subgraph even when that is more than one wave
+        # of the SMs - node features of the whole subgraph take 100 KB of every CTA's shared memory, and only with
+        # a quarter of the nodes per CTA do the edge lists still fit next to them.
+        cands = [4, 3, 2, 1, 0]
+    else:
+        cands = [cl for cl in (4, 2, 1) if B * cl <= sms or cl == 1] + [0]
+    if want == "auto":
+        # node features in L2 instead of shared memory: subgraphs too large for every plan above
+        cands.append(_lib.plan_l2(l2_cluster(n_cap, B, sms)))
+    for cl in cands:
+        if max_edges and _lib.is_rs(cl):
+            cmodel.list_hint = int(1.25 * max_edges / int(cl)) + 256
+        f = lib.igmc_model_plan(C.byref(cmodel), n_cap, int(cl), 0)
+        b = lib.igmc_model_plan(C.byref(cmodel), n_cap, int(cl), 1)
+        if f > 0 and b > 0:
+            return int(cl)
+    raise RuntimeError("igmc_b200: no kernel plan fits subgraphs of up to %d nodes with %d relations (the L2 plan "
+                       "takes up to %d nodes per subgraph); lower --max-nodes-per-hop"
+                       % (n_cap, R, _lib.L2_MAX_NODES))
+
+
 class RGCNConv(nn.Module):
     """Parameter holder with PyG 1.4.2 ``RGCNConv`` names/shapes/init (SURVEY.md A.1).  The arithmetic
     lives in the fused kernels of the owning ``IGMC``."""
@@ -224,17 +270,18 @@ class IGMC(nn.Module):
 
     # ---- kernel launches ---------------------------------------------------------------------------------
     kernel_plan = "auto"   # "auto" | 0 (generic kernels) | 1 | 2 | 3 | 4 (relation-space kernels, CTAs per subgraph)
+    #                        | 17 | 18 | 20 | 24 (L2 plan with 1 / 2 / 4 / 8 CTAs per subgraph, _lib.plan_l2)
     hidden_dropout_p = 0.5   # F.dropout(x, p=0.5) before lin2 (models.py:212)
 
     def _plan(self, batch):
-        """cluster size for this batch: use the relation-space kernels when the relation count allows and
-        spread each subgraph over as many CTAs (1/2/4) as keeps the grid within one wave of the SMs."""
+        """kernel plan for this batch (``select_plan``): the relation-space kernels when the relation count allows,
+        each subgraph spread over as many CTAs (1/2/4) as keeps the grid within one wave of the SMs; the generic
+        kernels otherwise; the L2 plan when no shared-memory plan fits the subgraphs."""
         p = batch._priv
         key = (p["n_cap"], batch.num_graphs)
         c = self._plans.get(key)
         if c is not None:
             return c
-        lib = _lib.load()
         n_cap, B = p["n_cap"], batch.num_graphs
         want = self.kernel_plan
         env = os.environ.get("IGMC_PLAN")
@@ -245,26 +292,10 @@ class IGMC(nn.Module):
             # this first batch, one host sync per model; the lists of one CTA hold its share of the directed edges)
             ep = p["edge_ptr"][:B + 1].cpu()
             self._max_edges = int((ep[1:] - ep[:-1]).max())
-        if want != "auto":
-            cands = [want]
-        elif n_cap > 256 and self.num_relations <= 12:
-            # large subgraphs (ml_100k*: up to 402 nodes): four CTAs per subgraph even when that is more than one wave
-            # of the SMs - node features of the whole subgraph take 100 KB of every CTA's shared memory, and only with
-            # a quarter of the nodes per CTA do the edge lists still fit next to them.
-            cands = [4, 3, 2, 1, 0]
-        else:
-            sms = torch.cuda.get_device_properties(self.flat_params.device).multi_processor_count
-            cands = [cl for cl in (4, 2, 1) if B * cl <= sms or cl == 1] + [0]
-        for cl in cands:
-            if self.__dict__.get("_max_edges") and int(cl) > 0:
-                self._cmodel.list_hint = int(1.25 * self._max_edges / int(cl)) + 256
-            f = lib.igmc_model_plan(C.byref(self._cmodel), n_cap, int(cl), 0)
-            b = lib.igmc_model_plan(C.byref(self._cmodel), n_cap, int(cl), 1)
-            if f > 0 and b > 0:
-                self._plans[key] = int(cl)
-                return int(cl)
-        raise RuntimeError("igmc_b200: no kernel plan fits subgraphs of up to %d nodes with %d relations in %d B of "
-                           "shared memory per CTA; lower --max-nodes-per-hop" % (n_cap, self.num_relations, SMEM_LIMIT))
+        sms = torch.cuda.get_device_properties(self.flat_params.device).multi_processor_count
+        cl = select_plan(self._cmodel, n_cap, B, sms, want, self.__dict__.get("_max_edges"))
+        self._plans[key] = cl
+        return cl
 
     def _workspace(self, batch, train):
         p = batch._priv
@@ -282,15 +313,17 @@ class IGMC(nn.Module):
                       dpred=torch.zeros(B, **f32), sqerr=torch.zeros(B, **f32), loss=torch.zeros(1, **f32),
                       reg_ws=torch.zeros(_lib.REDUCE_WS_FLOATS, **f32), cluster=cl)
             if train:
-                if cl > 0:   # cluster plans: layer-0 aggregate only; raw partial rows (chain rule in igmc_grad_reduce)
+                if _lib.is_rs(cl):   # cluster plans: layer-0 aggregate only; raw partial rows (chain rule in igmc_grad_reduce)
                     zs = torch.empty(ncap, self.num_relations * _align4(self.num_features), **f32)
                     width = _lib.load().igmc_raw_grad_count(C.byref(self._cmodel))
                 else:
                     zs = torch.empty(L, ncap, NB * HID, **f32)
                     width = self._cmodel.conv_param_count
                 ws.update(zsave=zs, dstate=torch.empty(L, ncap, HID, **f32),
-                          gpart=torch.zeros(B * max(cl, 1), width, **f32),
+                          gpart=torch.zeros(B * _lib.ctas_per_graph(cl), width, **f32),
                           dhid=torch.empty(B, 128, **f32))
+                if _lib.l2_csize(cl):   # d pre / d h of the backward (node features are not in shared memory)
+                    ws["l2_scratch"] = torch.empty(2, ncap, HID, **f32)
             # never evicted: captured CUDA graphs hold raw pointers into these buffers (a handful of
             # (capacity, batch size, mode) keys per run; a few MB each)
             self._ws[key] = ws
@@ -300,9 +333,9 @@ class IGMC(nn.Module):
     def stage_batch(self, batch, training=True, drop=None, slot=0):
         """Build the list images of ``batch`` for the forward (and, when training, backward) kernel of its plan and
         attach them to the batch.  ``drop`` must be the dropout descriptor the step will use (same seed source).
-        No-op for the generic plan."""
+        No-op for the generic and L2 plans."""
         cl = self._plan(batch)
-        if cl <= 0:
+        if not _lib.is_rs(cl):
             batch._stage = None
             return None
         lib = _lib.load()
@@ -347,13 +380,14 @@ class IGMC(nn.Module):
         return C.byref(st[name][0])
 
     def _saved_struct(self, ws, ncap):
+        rs = _lib.is_rs(ws["cluster"])
         return _lib.Saved(ws["states"].data_ptr(), _lib.ptr(ws.get("zsave")), ws["inv_deg"].data_ptr(),
                           ws["feat"].data_ptr(), ws["hid"].data_ptr(), ws["hid_gscale"].data_ptr(),
                           ws["pred"].data_ptr(), ws["target"].data_ptr(), ncap, _lib.ptr(ws.get("dstate")),
-                          _lib.ptr(self._wprep_buf()) if ws["cluster"] > 0 else None,
+                          _lib.ptr(self._wprep_buf()) if rs else None,
                           _lib.ptr(getattr(self, "_prof_buf", None)),
-                          _lib.ptr(self._gate) if (ws["cluster"] > 0 and self.__dict__.pop("_gate_armed", False))
-                          else None)
+                          _lib.ptr(self._gate) if (rs and self.__dict__.pop("_gate_armed", False)) else None,
+                          _lib.ptr(ws.get("l2_scratch")))
 
     def prep_weights(self, mark=False):
         """launch igmc_prep_weights on the current stream; ``mark`` lets the next forward skip its own launch (the
@@ -368,7 +402,7 @@ class IGMC(nn.Module):
         forward of ``batch``'s shape is resident: work queued behind it runs BESIDE that forward instead of in front
         of it (igmc_gate_wait).  The forward must be launched after this call (the gate pointer is armed here)."""
         cl = self._plan(batch)
-        if cl <= 0:
+        if not _lib.is_rs(cl):
             return
         if self.__dict__.get("_gate") is None:
             self._gate = torch.zeros(2, dtype=torch.int32, device=self.flat_params.device)
@@ -411,7 +445,7 @@ class IGMC(nn.Module):
         ws = self._workspace(batch, training)
         S = self._saved_struct(ws, p["node_cap"])
         d, keep = drop
-        if ws["cluster"] > 0 and not self.__dict__.pop("_prepped", False):
+        if _lib.is_rs(ws["cluster"]) and not self.__dict__.pop("_prepped", False):
             # W_r / W_r^T of the current parameters (one tiny launch per step, unless prep_weights() just ran)
             self.prep_weights()
         _lib.check(lib.igmc_forward(C.byref(self._cmodel), self.flat_params.data_ptr(), p["node_label"].data_ptr(),
@@ -441,8 +475,8 @@ class IGMC(nn.Module):
         lib = _lib.load()
         ws = saved["ws"]
         _lib.check(lib.igmc_grad_reduce(C.byref(self._cmodel), self.flat_params.data_ptr(), batch.num_graphs,
-                                        batch.num_graphs * max(ws["cluster"], 1),
-                                        ws["gpart"].data_ptr(), 1 if ws["cluster"] > 0 else 0,
+                                        batch.num_graphs * _lib.ctas_per_graph(ws["cluster"]),
+                                        ws["gpart"].data_ptr(), 1 if _lib.is_rs(ws["cluster"]) else 0,
                                         ws["dhid"].data_ptr(), ws["feat"].data_ptr(),
                                         ws["hid"].data_ptr(), saved["dpred_used"].data_ptr(),
                                         ws["sqerr"].data_ptr() if with_loss else None, float(loss_scale),
@@ -476,7 +510,7 @@ class IGMC(nn.Module):
         self._step += 1
         drop = self.make_dropout(True, edge_keep, hidden_keep, seed_dev=seed_dev)
         G = batch.num_graphs if global_num_graphs is None else int(global_num_graphs)
-        if self._cmodel.readout == 0 and self._plan(batch) > 0 and os.environ.get("IGMC_FUSED_FB", "1") != "0":
+        if self._cmodel.readout == 0 and _lib.is_rs(self._plan(batch)) and os.environ.get("IGMC_FUSED_FB", "1") != "0":
             return self._launch_train(batch, drop, batch.y, 1.0 / G)
         out, saved = self._launch_forward(batch, True, drop, y=batch.y, loss_scale=1.0 / G)
         self._launch_backward(batch, drop, saved, saved["ws"]["dpred"])
@@ -505,7 +539,7 @@ class IGMC(nn.Module):
     def fused_update_ok(self, batch):
         """the one-kernel reduce -> all-reduce -> Adam path needs raw partial rows (cluster plans) and the IGMC
         readout (an external readout writes its own gradient slice)."""
-        return self._cmodel.readout == 0 and self._plan(batch) > 0
+        return self._cmodel.readout == 0 and _lib.is_rs(self._plan(batch))
 
     def fused_step(self, batch, ARR=0.0, global_num_graphs=None, edge_keep=None, hidden_keep=None,
                    seed_dev=None):

@@ -199,6 +199,7 @@ typedef struct {
   const float* wprep; /* [L * 2 * 32*((R+1)*32+4)] per-step prepared weights (igmc_prep_weights), cluster plans only */
   long long* prof;    /* optional debug: [grid][64] clock64() stamps of the kernel phases (cluster plans), or NULL */
   int32_t* gate;      /* optional: every CTA of igmc_forward (cluster plans) adds 1 when it starts, see igmc_gate_wait */
+  float* l2_scratch;  /* [2 * node_cap * 32] backward scratch of the L2 plan (d pre / d h of two layers), else unused */
 } igmc_saved_t;
 
 /* Launch-order gate for work that should run BESIDE the forward kernel without taking SMs from it (the extraction of
@@ -241,9 +242,15 @@ int igmc_prep_weights(const igmc_model_t* M, const float* params, float* wprep, 
 
 /* Kernel plan.  `cluster` = 0 selects the generic kernels (csrc/rgcn.cu: one 256-thread CTA per
  * subgraph, any num_relations <= 256); 1/2/4 select the relation-space kernels (csrc/rgcn_rs.cu,
- * num_relations <= 12) with that many CTAs (a thread-block cluster) per subgraph.  Returns the dynamic
- * shared memory in bytes the chosen kernel needs for subgraphs of up to n_cap nodes, or a negative value
- * if the plan is not available (too many relations / does not fit in 227 KB). */
+ * num_relations <= 12) with that many CTAs (a thread-block cluster) per subgraph; IGMC_PLAN_L2(c), c = 1/2/4/8,
+ * selects the L2 plan (csrc/rgcn_l2.cu): the generic plan's arithmetic on a cluster of c CTAs per subgraph with the
+ * node features in global memory (L2) instead of shared memory, for subgraphs of up to 65 535 nodes and any
+ * num_relations <= 256.  Returns the dynamic shared memory in bytes the chosen kernel needs for subgraphs of up to
+ * n_cap nodes (for the L2 plan the same for every n_cap <= 65 535), or a negative value if the plan is not available
+ * (too many relations / does not fit in 227 KB / n_cap > 65 535). */
+#define IGMC_PLAN_L2_BASE 16
+#define IGMC_PLAN_L2(c) (IGMC_PLAN_L2_BASE + (c))
+#define IGMC_L2_MAX_NODES 65535
 int igmc_model_plan(const igmc_model_t* M, int n_cap, int cluster, int backward);
 
 /* IGMC.forward for a prepared batch (models.py:190-217): 4x (RGCNConv + tanh), concat, target-row
@@ -258,7 +265,8 @@ int igmc_forward(const igmc_model_t* M, const float* params, const uint8_t* node
 
 /* Backward of igmc_forward given dpred [B] (gradient wrt the lin2 output).  Writes partial gradients of
  * the conv parameters, one row per CTA, and the readout factors dhid [B*128]; igmc_grad_reduce turns them into the
- * flat gradient.  Row layout: cluster 0 -> gpart[B][conv_param_count] in parameter layout; cluster > 0 ->
+ * flat gradient.  Row layout: cluster 0 -> gpart[B][conv_param_count] in parameter layout; IGMC_PLAN_L2(c) ->
+ * gpart[B*c][conv_param_count] in parameter layout (S.l2_scratch required); cluster 1..4 ->
  * gpart[B*cluster][igmc_raw_grad_count()] "raw" rows (per layer dW_r [R][in0p|32][32] | d root | d bias): the
  * (att, basis) chain rule is linear and is applied once to the sum by igmc_grad_reduce.  Must use the same `cluster`
  * as the forward that produced S.  `stage` (optional) = the backward image of igmc_stage_lists.
@@ -270,7 +278,7 @@ int igmc_backward(const igmc_model_t* M, const float* params, const uint8_t* nod
 
 /* igmc_forward (training, with the loss) immediately followed by igmc_backward for the same batch, as ONE launch: a
  * cluster goes from its subgraph's readout straight into its backward (d loss / d pred of a subgraph depends on that
- * subgraph's forward only).  Same arguments, same results bit for bit as the two calls; cluster plans with the IGMC
+ * subgraph's forward only).  Same arguments, same results bit for bit as the two calls; relation-space plans (1..4) with the IGMC
  * readout only.  What `loss = mse_loss(model(data), y); loss.backward()` spans in train_eval.py:160-175. */
 int igmc_forward_backward(const igmc_model_t* M, const float* params, const uint8_t* node_label,
                           const int32_t* node_ptr, const int32_t* edge_ptr, const igmc_adj_t* A, int B, int n_cap,
