@@ -103,7 +103,7 @@ class Dropout(C.Structure):
 class Saved(C.Structure):
     _fields_ = [("states", vp), ("zsave", vp), ("inv_deg", vp), ("feat", vp), ("hid", vp),
                 ("hid_gscale", vp), ("pred", vp), ("target", vp), ("node_cap", C.c_int32), ("dstate", vp), ("wprep", vp), ("prof", vp),
-                ("gate", vp), ("l2_scratch", vp)]
+                ("gate", vp), ("l2_scratch", vp), ("rel_inv_deg", vp)]
 
 
 class Stage(C.Structure):

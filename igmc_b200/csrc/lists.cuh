@@ -58,4 +58,24 @@ __device__ __forceinline__ int list_foreach(const uint32_t* __restrict__ adj, co
   return kept;
 }
 
+// Per-relation mean (igmc_saved_t.rel_inv_deg): out[r] = 1/max(kept entries of type r, 1) for r < R, for one node's
+// list.  Lists are sorted by type, so every type is one run.  Warp-wide; returns the kept count.
+__device__ __forceinline__ int rel_inv_deg_row(const uint32_t* __restrict__ adj, const int32_t* __restrict__ eid,
+                                               int p0, int p1, const EdgeKeep& K, int eb, int m_half, int lane, int R,
+                                               float* __restrict__ out) {
+  for (int r = lane; r < R; r += 32) out[r] = 1.f;
+  __syncwarp();
+  int cur = -1, cnt = 0;
+  const int kept = list_foreach(adj, eid, p0, p1, K, false, eb, m_half, lane, [&](int, int ty) {
+    if (ty != cur) {
+      if (cur >= 0 && lane == 0) out[cur] = 1.f / (float)cnt;
+      cur = ty;
+      cnt = 0;
+    }
+    ++cnt;
+  });
+  if (cur >= 0 && lane == 0) out[cur] = 1.f / (float)cnt;
+  return kept;
+}
+
 }  // namespace

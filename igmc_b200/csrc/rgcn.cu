@@ -8,7 +8,9 @@
 // Formulation (never materialises the per-edge weight):  with W_r = sum_b att[r,b] basis[b],
 //   Z[v,b,:]  = 1/deg(v) * sum_{(u->v, type r) kept} att[r,b] * h[u,:]          (segment reduce, run per type)
 //   pre[v,:]  = [Z[v] | h[v]] . [basis ; root] + bias ,   h'[v] = tanh(pre[v])     (dense K=(NB+1)*in GEMM tile)
-// deg(v) = number of kept incoming edges of ANY type (aggr='mean').  Backward is the same pair of
+// deg(v) = number of kept incoming edges of ANY type (aggr='mean').  PR = true (PyG >= 1.6 RGCNConv, selected by
+// igmc_saved_t.rel_inv_deg) moves the mean inside the relation sum: each type run is divided by its own length, and
+// the backward weighs an out-list entry u->d of type r by 1/|N_r(d)| instead of 1/deg(d).  Backward is the same pair of
 // passes on the transposed lists with [basis ; root]^T, plus K=n weight-gradient GEMM tiles.
 // All reductions have a fixed order: results are run-to-run deterministic.
 #include "lists.cuh"
@@ -57,12 +59,45 @@ __device__ __forceinline__ int gather_runs(const uint32_t* __restrict__ adj, con
   return kept;
 }
 
+// The same for the mean per relation (igmc_saved_t.rel_inv_deg): with SCALE an entry is weighed by
+// rinv[nbr*R + type] (1/|N_r| of the destination nbr, backward), without SCALE every run is divided by its length
+// (forward).  Kept apart from gather_runs so that the default kernels compile exactly as before.
+template <int NB, bool SCALE>
+__device__ __forceinline__ int gather_runs_rel(const uint32_t* __restrict__ adj, const int32_t* __restrict__ eid,
+                                               int p0, int p1, const EdgeKeep& K, bool mirror, int eb, int m_half,
+                                               int lane, const float* __restrict__ feat, const float* __restrict__ rinv,
+                                               int R, const float* __restrict__ att_s, float (&acc)[NB]) {
+  float run = 0.f;
+  int cur = -1, cnt = 0;
+#pragma unroll
+  for (int b = 0; b < NB; ++b) acc[b] = 0.f;
+  auto flush = [&]() {
+    const float rv = SCALE ? run : run * (1.f / (float)cnt);
+#pragma unroll
+    for (int b = 0; b < NB; ++b) acc[b] = fmaf(att_s[cur * NB + b], rv, acc[b]);
+  };
+  const int kept = list_foreach(adj, eid, p0, p1, K, mirror, eb, m_half, lane, [&](int nbr, int ty) {
+    if (ty != cur) {
+      if (cur >= 0) flush();
+      run = 0.f;
+      cur = ty;
+      cnt = 0;
+    }
+    float v = feat[hix(nbr, lane)];
+    if (SCALE) v *= __ldg(rinv + nbr * R + ty);
+    run += v;
+    ++cnt;
+  });
+  if (cur >= 0) flush();
+  return kept;
+}
+
 __device__ __forceinline__ size_t align4(size_t x) { return (x + 3) & ~(size_t)3; }
 
 // ------------------------------------------------------------------------------------------------
 // forward
 // ------------------------------------------------------------------------------------------------
-template <int NB>
+template <int NB, bool PR>
 __global__ void __launch_bounds__(MP_THREADS)
 k_forward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __restrict__ node_label,
           const int32_t* __restrict__ node_ptr, const int32_t* __restrict__ edge_ptr, igmc_adj_t A, int n_cap,
@@ -102,11 +137,14 @@ k_forward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __res
     if (c == 0 && lab == 0) atomicMin(&s_t[0], v);   // users = x[:,0]==1 (models.py:205)
     if (c == 0 && lab == 1) atomicMin(&s_t[1], v);   // items = x[:,1]==1 (models.py:206)
   }
-  // kept in-degree (same for every layer: dropout_adj is applied once, models.py:193)
+  // kept in-degree (same for every layer: dropout_adj is applied once, models.py:193); per relation too in PR mode
   for (int v = warp; v < n; v += MP_WARPS) {
     const int p0 = A.in_ptr[nb + v], p1 = A.in_ptr[nb + v + 1];
     int kept = p1 - p0;
-    if (K.active) kept = list_foreach(A.in_adj, A.in_eid, p0, p1, K, false, eb, m_half, lane, [](int, int) {});
+    if (PR)
+      kept = rel_inv_deg_row(A.in_adj, A.in_eid, p0, p1, K, eb, m_half, lane, R, S.rel_inv_deg + (size_t)(nb + v) * R);
+    else if (K.active)
+      kept = list_foreach(A.in_adj, A.in_eid, p0, p1, K, false, eb, m_half, lane, [](int, int) {});
     if (lane == 0) {
       const float id = 1.f / (float)max(kept, 1);
       invdeg[v] = id;
@@ -138,12 +176,16 @@ k_forward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __res
       // ---- phase G: basis-space aggregate of the tile's nodes (warp per destination node) ----
       for (int v = t0 + warp; v < tend; v += MP_WARPS) {
         float z[NB];
-        gather_runs<NB, false>(A.in_adj, A.in_eid, A.in_ptr[nb + v], A.in_ptr[nb + v + 1], K, false, eb, m_half,
-                               lane, HA, nullptr, att_s, z);
+        if (PR)
+          gather_runs_rel<NB, false>(A.in_adj, A.in_eid, A.in_ptr[nb + v], A.in_ptr[nb + v + 1], K, false, eb, m_half,
+                                     lane, HA, nullptr, R, att_s, z);
+        else
+          gather_runs<NB, false>(A.in_adj, A.in_eid, A.in_ptr[nb + v], A.in_ptr[nb + v + 1], K, false, eb, m_half,
+                                 lane, HA, nullptr, att_s, z);
         const float id = invdeg[v];
 #pragma unroll
         for (int b = 0; b < NB; ++b) {
-          z[b] *= id;
+          if (!PR) z[b] *= id;   // (PR: every relation's run is already a mean)
           if (lane < in) Zs[(v - t0) * ZS + b * in + lane] = z[b];
           if (S.zsave)
             S.zsave[((size_t)l * S.node_cap + nb + v) * (NB * HID) + b * HID + lane] = z[b];
@@ -242,7 +284,7 @@ k_forward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __res
 // ------------------------------------------------------------------------------------------------
 // backward
 // ------------------------------------------------------------------------------------------------
-template <int NB>
+template <int NB, bool PR>
 __global__ void __launch_bounds__(MP_THREADS)
 k_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __restrict__ node_label,
            const int32_t* __restrict__ node_ptr, const int32_t* __restrict__ edge_ptr, igmc_adj_t A, int n_cap,
@@ -350,8 +392,12 @@ k_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __re
         const int tend = min(t0 + TM, n);
         for (int u = t0 + warp; u < tend; u += MP_WARPS) {
           float gz[NB];
-          gather_runs<NB, true>(oadj, oeid, optr[nb + u], optr[nb + u + 1], K, sym, eb, m_half, lane, GA, invdeg,
-                                att_s, gz);
+          if (PR)
+            gather_runs_rel<NB, true>(oadj, oeid, optr[nb + u], optr[nb + u + 1], K, sym, eb, m_half, lane, GA,
+                                      S.rel_inv_deg + (size_t)nb * R, R, att_s, gz);
+          else
+            gather_runs<NB, true>(oadj, oeid, optr[nb + u], optr[nb + u + 1], K, sym, eb, m_half, lane, GA, invdeg,
+                                  att_s, gz);
 #pragma unroll
           for (int b = 0; b < NB; ++b) Zs[(u - t0) * ZS + b * HID + lane] = gz[b];
         }
@@ -463,7 +509,7 @@ k_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __re
                 a[c + 2] = fmaf(x, w4.z, a[c + 2]); a[c + 3] = fmaf(x, w4.w, a[c + 3]);
               }
             }
-            const float id = invdeg[v];
+            const float id = PR ? 1.f : invdeg[v];   // (PR: the 1/|N_r(v)| factor is applied per run below)
 #pragma unroll
             for (int c = 0; c < CPT; ++c) Zs[r * ZS + cg * CPT + c] = a[c] * id;
           }
@@ -474,12 +520,13 @@ k_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __re
 #pragma unroll
           for (int b = 0; b < NB; ++b) dz[b] = (lane < in) ? Zs[(v - t0) * ZS + b * HID + lane] : 0.f;
           float run = 0.f;
-          int cur = -1;
+          int cur = -1, cnt = 0;
           float* dw = datt_w + warp * (R * NB);
           auto flush = [&]() {
+            const float rv = PR ? run * (1.f / (float)cnt) : run;
 #pragma unroll
             for (int b = 0; b < NB; ++b) {
-              const float p = warp_sum_f(run * dz[b]);
+              const float p = warp_sum_f(rv * dz[b]);
               if (lane == 0) dw[cur * NB + b] += p;
             }
           };
@@ -489,8 +536,10 @@ k_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __re
                            if (cur >= 0) flush();
                            run = 0.f;
                            cur = ty;
+                           cnt = 0;
                          }
                          run += HP[hix(nbr, lane)];
+                         ++cnt;
                        });
           if (cur >= 0) flush();
         }
@@ -654,15 +703,11 @@ extern "C" int igmc_forward(const igmc_model_t* M, const float* params, const ui
   }
   const size_t smem = fwd_smem_bytes(n_cap, M->num_relations, M->num_bases, M->num_layers);
   if (smem > 227 * 1024) return -3;
-  if (M->num_bases == 4) {
-    cudaFuncSetAttribute(k_forward<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    k_forward<4><<<B, MP_THREADS, smem, st>>>(*M, params, node_label, node_ptr, edge_ptr, *A, n_cap, *D, training, *S,
-                                              y, loss_scale, dpred, sqerr, err);
-  } else {
-    cudaFuncSetAttribute(k_forward<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    k_forward<2><<<B, MP_THREADS, smem, st>>>(*M, params, node_label, node_ptr, edge_ptr, *A, n_cap, *D, training, *S,
-                                              y, loss_scale, dpred, sqerr, err);
-  }
+  auto kern = M->num_bases == 4 ? (S->rel_inv_deg ? k_forward<4, true> : k_forward<4, false>)
+                                : (S->rel_inv_deg ? k_forward<2, true> : k_forward<2, false>);
+  cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  kern<<<B, MP_THREADS, smem, st>>>(*M, params, node_label, node_ptr, edge_ptr, *A, n_cap, *D, training, *S, y,
+                                    loss_scale, dpred, sqerr, err);
   IGMC_CUDA_CHECK_LAUNCH();
   return 0;
 }
@@ -707,15 +752,11 @@ extern "C" int igmc_backward(const igmc_model_t* M, const float* params, const u
   }
   const size_t smem = bwd_smem_bytes(n_cap, M->num_relations, M->num_bases, M->num_layers);
   if (smem > 227 * 1024) return -3;
-  if (M->num_bases == 4) {
-    cudaFuncSetAttribute(k_backward<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    k_backward<4><<<B, MP_THREADS, smem, st>>>(*M, params, node_label, node_ptr, edge_ptr, *A, n_cap, *D, *S, dpred,
-                                               gpart, dhid, err);
-  } else {
-    cudaFuncSetAttribute(k_backward<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    k_backward<2><<<B, MP_THREADS, smem, st>>>(*M, params, node_label, node_ptr, edge_ptr, *A, n_cap, *D, *S, dpred,
-                                               gpart, dhid, err);
-  }
+  auto kern = M->num_bases == 4 ? (S->rel_inv_deg ? k_backward<4, true> : k_backward<4, false>)
+                                : (S->rel_inv_deg ? k_backward<2, true> : k_backward<2, false>);
+  cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  kern<<<B, MP_THREADS, smem, st>>>(*M, params, node_label, node_ptr, edge_ptr, *A, n_cap, *D, *S, dpred, gpart, dhid,
+                                    err);
   IGMC_CUDA_CHECK_LAUNCH();
   return 0;
 }

@@ -35,30 +35,33 @@ __device__ __forceinline__ void own_range(int n, int csize, int rank, int& v0, i
 
 __device__ __forceinline__ size_t align4(size_t x) { return (x + 3) & ~(size_t)3; }
 
-// Type-run segment reduce over kept list entries: acc[b] = sum_runs att[type][b] * sum_run feat(nbr)
-template <int NB, class Feat>
+// Type-run segment reduce over kept list entries: acc[b] = sum_runs att[type][b] * sum_run feat(nbr, type);
+// MEAN: every run divided by its length (the forward's mean per relation, igmc_saved_t.rel_inv_deg)
+template <int NB, bool MEAN = false, class Feat>
 __device__ __forceinline__ int gather_runs(const uint32_t* __restrict__ adj, const int32_t* __restrict__ eid, int p0,
                                            int p1, const EdgeKeep& K, bool mirror, int eb, int m_half, int lane,
                                            Feat&& feat, const float* __restrict__ att_s, float (&acc)[NB]) {
   float run = 0.f;
-  int cur = -1;
+  int cur = -1, cnt = 0;
 #pragma unroll
   for (int b = 0; b < NB; ++b) acc[b] = 0.f;
+  auto flush = [&]() {
+    float rv = run;
+    if (MEAN) rv *= 1.f / (float)cnt;
+#pragma unroll
+    for (int b = 0; b < NB; ++b) acc[b] = fmaf(att_s[cur * NB + b], rv, acc[b]);
+  };
   const int kept = list_foreach(adj, eid, p0, p1, K, mirror, eb, m_half, lane, [&](int nbr, int ty) {
     if (ty != cur) {
-      if (cur >= 0) {
-#pragma unroll
-        for (int b = 0; b < NB; ++b) acc[b] = fmaf(att_s[cur * NB + b], run, acc[b]);
-      }
+      if (cur >= 0) flush();
       run = 0.f;
       cur = ty;
+      cnt = 0;
     }
-    run += feat(nbr);
+    run += feat(nbr, ty);
+    ++cnt;
   });
-  if (cur >= 0) {
-#pragma unroll
-    for (int b = 0; b < NB; ++b) acc[b] = fmaf(att_s[cur * NB + b], run, acc[b]);
-  }
+  if (cur >= 0) flush();
   return kept;
 }
 
@@ -76,7 +79,7 @@ struct PrevLayer {
 // ------------------------------------------------------------------------------------------------
 // forward
 // ------------------------------------------------------------------------------------------------
-template <int NB>
+template <int NB, bool PR>
 __global__ void __launch_bounds__(THREADS)
 k_l2_forward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __restrict__ node_label,
              const int32_t* __restrict__ node_ptr, const int32_t* __restrict__ edge_ptr, igmc_adj_t A, int csize,
@@ -139,14 +142,17 @@ k_l2_forward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __
       // ---- phase G: basis-space aggregate of the tile's nodes (warp per destination node) + their own rows ----
       for (int v = t0 + warp; v < tend; v += WARPS) {
         float z[NB];
-        const int kept = gather_runs<NB>(A.in_adj, A.in_eid, A.in_ptr[nb + v], A.in_ptr[nb + v + 1], K, false, eb,
-                                         m_half, lane, [&](int u) { return hp(u, lane); }, att_s, z);
+        const int kept = gather_runs<NB, PR>(A.in_adj, A.in_eid, A.in_ptr[nb + v], A.in_ptr[nb + v + 1], K, false, eb,
+                                             m_half, lane, [&](int u, int) { return hp(u, lane); }, att_s, z);
         const float id = 1.f / (float)max(kept, 1);   // kept in-degree: the same for every layer
         if (l == 0 && lane == 0) S.inv_deg[nb + v] = id;
+        if (PR && l == 0)   // per-relation table for the backward (the runs above are means already)
+          rel_inv_deg_row(A.in_adj, A.in_eid, A.in_ptr[nb + v], A.in_ptr[nb + v + 1], K, eb, m_half, lane, R,
+                          S.rel_inv_deg + (size_t)(nb + v) * R);
         float* zr = Zs + (v - t0) * ZS;
 #pragma unroll
         for (int b = 0; b < NB; ++b) {
-          z[b] *= id;
+          if (!PR) z[b] *= id;
           if (lane < in) zr[b * in + lane] = z[b];
           if (S.zsave) S.zsave[((size_t)l * S.node_cap + nb + v) * (NB * HID) + b * HID + lane] = z[b];
         }
@@ -234,7 +240,7 @@ k_l2_forward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __
 // ------------------------------------------------------------------------------------------------
 // backward
 // ------------------------------------------------------------------------------------------------
-template <int NB>
+template <int NB, bool PR>
 __global__ void __launch_bounds__(THREADS)
 k_l2_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __restrict__ node_label,
               const int32_t* __restrict__ node_ptr, const int32_t* __restrict__ edge_ptr, igmc_adj_t A, int csize,
@@ -271,6 +277,7 @@ k_l2_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* _
   const int tu = ext ? -1 : S.target[2 * g] - nb, ti = ext ? -1 : S.target[2 * g + 1] - nb;
   float* gp = gpart + (size_t)blockIdx.x * M.conv_param_count;
   const float* invdeg = S.inv_deg + nb;
+  const float* rinv = PR ? S.rel_inv_deg + (size_t)nb * R : nullptr;   // [n][R] 1/|N_r(v)| (PR mode)
   const float* states = S.states + (size_t)nb * CW;
   int v0, v1;
   own_range(n, csize, rank, v0, v1);
@@ -337,7 +344,10 @@ k_l2_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* _
         for (int u = t0 + warp; u < tend; u += WARPS) {
           float gz[NB];
           gather_runs<NB>(oadj, oeid, optr[nb + u], optr[nb + u + 1], K, sym, eb, m_half, lane,
-                          [&](int w) { return __ldcg(X + (size_t)w * HID + lane) * __ldcg(invdeg + w); }, att_s, gz);
+                          [&](int w, int ty) {
+                            return __ldcg(X + (size_t)w * HID + lane) *
+                                   (PR ? __ldcg(rinv + (size_t)w * R + ty) : __ldcg(invdeg + w));
+                          }, att_s, gz);
           float* zr = Zs + (u - t0) * ZB;
 #pragma unroll
           for (int b = 0; b < NB; ++b) zr[b * HID + lane] = gz[b];
@@ -441,7 +451,7 @@ k_l2_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* _
           }
           __syncthreads();   // every thread of the row has read d pre before the row's Z columns are overwritten
           if (r < rows) {
-            const float id = __ldcg(invdeg + t0 + r);
+            const float id = PR ? 1.f : __ldcg(invdeg + t0 + r);   // (PR: 1/|N_r(v)| is applied per run below)
 #pragma unroll
             for (int c = 0; c < CPT; ++c) Zs[r * ZB + cg * CPT + c] = a[c] * id;
           }
@@ -452,11 +462,12 @@ k_l2_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* _
 #pragma unroll
           for (int b = 0; b < NB; ++b) dz[b] = (lane < in) ? Zs[(v - t0) * ZB + b * HID + lane] : 0.f;
           float run = 0.f;
-          int cur = -1;
+          int cur = -1, cnt = 0;
           auto flush = [&]() {
+            const float rv = PR ? run * (1.f / (float)cnt) : run;
 #pragma unroll
             for (int b = 0; b < NB; ++b) {
-              const float p = warp_sum_f(run * dz[b]);
+              const float p = warp_sum_f(rv * dz[b]);
               if (lane == 0) dw[cur * NB + b] += (double)p;
             }
           };
@@ -466,8 +477,10 @@ k_l2_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* _
                            if (cur >= 0) flush();
                            run = 0.f;
                            cur = ty;
+                           cnt = 0;
                          }
                          run += hp(nbr, lane);
+                         ++cnt;
                        });
           if (cur >= 0) flush();
         }
@@ -539,11 +552,10 @@ int l2_forward(const igmc_model_t* M, const float* params, const uint8_t* node_l
                const igmc_saved_t* S, const float* y, float loss_scale, float* dpred, float* sqerr, int* err,
                cudaStream_t st) {
   const size_t smem = l2_smem_bytes(M, 0);
-  if (M->num_bases == 4)
-    return launch(k_l2_forward<4>, B, csize, smem, st, *M, params, node_label, node_ptr, edge_ptr, *A, csize, *D,
-                  training, *S, y, loss_scale, dpred, sqerr, err);
-  return launch(k_l2_forward<2>, B, csize, smem, st, *M, params, node_label, node_ptr, edge_ptr, *A, csize, *D,
-                training, *S, y, loss_scale, dpred, sqerr, err);
+  auto kern = M->num_bases == 4 ? (S->rel_inv_deg ? k_l2_forward<4, true> : k_l2_forward<4, false>)
+                                : (S->rel_inv_deg ? k_l2_forward<2, true> : k_l2_forward<2, false>);
+  return launch(kern, B, csize, smem, st, *M, params, node_label, node_ptr, edge_ptr, *A, csize, *D, training, *S, y,
+                loss_scale, dpred, sqerr, err);
 }
 
 int l2_backward(const igmc_model_t* M, const float* params, const uint8_t* node_label, const int32_t* node_ptr,
@@ -551,9 +563,8 @@ int l2_backward(const igmc_model_t* M, const float* params, const uint8_t* node_
                 const igmc_saved_t* S, const float* dpred, float* gpart, float* dhid, float* dbuf, int* err,
                 cudaStream_t st) {
   const size_t smem = l2_smem_bytes(M, 1);
-  if (M->num_bases == 4)
-    return launch(k_l2_backward<4>, B, csize, smem, st, *M, params, node_label, node_ptr, edge_ptr, *A, csize, *D, *S,
-                  dpred, gpart, dhid, dbuf, err);
-  return launch(k_l2_backward<2>, B, csize, smem, st, *M, params, node_label, node_ptr, edge_ptr, *A, csize, *D, *S,
-                dpred, gpart, dhid, dbuf, err);
+  auto kern = M->num_bases == 4 ? (S->rel_inv_deg ? k_l2_backward<4, true> : k_l2_backward<4, false>)
+                                : (S->rel_inv_deg ? k_l2_backward<2, true> : k_l2_backward<2, false>);
+  return launch(kern, B, csize, smem, st, *M, params, node_label, node_ptr, edge_ptr, *A, csize, *D, *S, dpred, gpart,
+                dhid, dbuf, err);
 }

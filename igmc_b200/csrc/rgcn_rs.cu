@@ -7,6 +7,7 @@
 //   AGG[v,r,:] = sum_{(u->v) of type r, kept} h[u,:]      warp owns 4 destination nodes; 8-lane groups x float4,
 //                                                          edge lists staged in shared memory, software-pipelined
 //   h'[v]      = tanh( 1/deg(v) * sum_r AGG[v,r,:] W_r + h[v] root + bias )    lane = (node, 4 output channels)
+// PR = true (PyG >= 1.6 RGCNConv, igmc_saved_t.rel_inv_deg): 1/|N_r(v)| per relation block in place of 1/deg(v).
 // Node features of the WHOLE subgraph stay in shared memory; CTAs of a cluster exchange their rows through
 // L2 (ld/st.cg) + barrier.cluster once per layer.  Backward = same two passes on the out-lists with W_r^T,
 // a K=n weight-gradient tile GEMM, and the (att,basis) chain rule applied to the per-CTA dW_r.
@@ -256,6 +257,37 @@ __device__ __forceinline__ Lists stage_lists(const uint32_t* adj, const int32_t*
   return Ls;
 }
 
+__device__ __forceinline__ float4 scale_row(float4 a, float s) { return make_float4(a.x * s, a.y * s, a.z * s, a.w * s); }
+
+// Mean per relation (igmc_saved_t.rel_inv_deg): out[v*R + r] = 1/max(kept in-edges of type r at v, 1) for the own
+// nodes v = lo + i, counted from the staged (compacted) in-lists, or from the global lists when they are not staged.
+// Warp per node, lane r counts type r (R <= RS_MAX_R < 32).  Block-wide; the caller's next barrier publishes it.
+__device__ __forceinline__ void rel_inv_deg_own(const Lists& Ls, const Keep& K, const int32_t* __restrict__ in_ptr,
+                                                int nb, int lo, int n_own, int R, float* __restrict__ out) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+  for (int i = warp; i < n_own; i += nwarps) {
+    const int p0 = Ls.lst ? Ls.lptr[i] : in_ptr[nb + lo + i], p1 = Ls.lst ? Ls.lptr[i + 1] : in_ptr[nb + lo + i + 1];
+    int cnt = 0;
+    for (int c = p0; c < p1; c += 32) {
+      const int p = c + lane;
+      int ty = -1;
+      if (p < p1) {
+        if (Ls.lst) {
+          ty = (int)(Ls.lst[p] >> 24);
+        } else {
+          const uint32_t e = load_entry(Ls.adj, Ls.eid, p, K, false, Ls.eb, Ls.m_half);
+          if (e != DROPPED) ty = (int)((e >> 16) & 0xffu);
+        }
+      }
+      for (int r = 0; r < R; ++r) {
+        const int c_r = __popc(__ballot_sync(IGMC_FULL, ty == r));
+        if (lane == r) cnt += c_r;
+      }
+    }
+    if (lane < R) out[(size_t)(lo + i) * R + lane] = 1.f / (float)max(cnt, 1);
+  }
+}
+
 // Relation-space aggregate of the segments [sg0, sg1) of one chunk into their staging rows
 // stage[row][r*inp + k] (row stride SS): one 8-lane group per segment, float4 per lane.
 // `K` is only consulted for unstaged lists (dropout draws evaluated per edge).
@@ -266,10 +298,12 @@ __device__ __forceinline__ Lists stage_lists(const uint32_t* adj, const int32_t*
 // not change its result (own staging row, fixed summation order): the output stays bitwise deterministic.
 // GL = lanes per segment (one float4 each): 8 for the 32-wide layers; 1 for a 4-wide input layer (one-hot labels) -
 // there seven of the eight lanes of a group had nothing to do, now a warp works on 32 segments at a time.
-template <int GL>
+// PR (backward of the mean per relation): every entry (nbr, type r) is weighed by rinv[nbr*R + r] = 1/|N_r(nbr)|,
+// read through L2 (the table is written by the forward, possibly by a peer CTA of the same launch).
+template <int GL, bool PR = false>
 __device__ __forceinline__ void gather_segments(const Lists& Ls, const Keep& K, int sg0, int sg1, int lane,
                                                 const float* __restrict__ feat, float* __restrict__ stage, int SS,
-                                                int inp, int* ticket) {
+                                                int inp, int* ticket, const float* rinv = nullptr, int R = 0) {
   const int q = lane & (GL - 1);
   const int fo = 4 * q;
   const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -295,7 +329,9 @@ __device__ __forceinline__ void gather_segments(const Lists& Ls, const Keep& K, 
       const uint32_t* lst = Ls.lst;
       float4 acc = z4;
       int cur = -1;
-#define IGMC_HROW(e_) (*reinterpret_cast<const float4*>(feat + (((e_) & 0xffffffu) ^ (uint32_t)fo)))
+#define IGMC_HROW(e_) (PR ? scale_row(*reinterpret_cast<const float4*>(feat + (((e_) & 0xffffffu) ^ (uint32_t)fo)), \
+                                      __ldcg(rinv + (int)(((e_) & 0xffffffu) >> 5) * R + (int)((e_) >> 24)))       \
+                         : *reinterpret_cast<const float4*>(feat + (((e_) & 0xffffffu) ^ (uint32_t)fo)))
 #define IGMC_STEP(e_, a_)                                                            \
       do {                                                                           \
         const int ty_ = (int)((e_) >> 24);                                           \
@@ -336,7 +372,8 @@ __device__ __forceinline__ void gather_segments(const Lists& Ls, const Keep& K, 
         const uint32_t ent = load_entry(Ls.adj, Ls.eid, p, K, Ls.mirror, Ls.eb, Ls.m_half);
         if (ent == DROPPED) continue;
         const int src = (int)(ent & 0xffffu);
-        const float4 a = *reinterpret_cast<const float4*>(feat + (src << 5) + (fo ^ ((src & 7) << 2)));
+        float4 a = *reinterpret_cast<const float4*>(feat + (src << 5) + (fo ^ ((src & 7) << 2)));
+        if (PR) a = scale_row(a, __ldcg(rinv + src * R + (int)((ent >> 16) & 0xffu)));
         float4* d = reinterpret_cast<float4*>(row + (int)((ent >> 16) & 0xffu) * inp);
         float4 t = *d;
         t.x += a.x; t.y += a.y; t.z += a.z; t.w += a.w;
@@ -534,7 +571,7 @@ __device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.w
 // ------------------------------------------------------------------------------------------------
 // The forward of one subgraph as a device function (returns false when it bailed out on a data error, uniformly over
 // the cluster): body of k_forward_rs, and first half of the fused train kernel k_train_rs.
-template <int NTMAX>
+template <int NTMAX, bool PR>
 __device__ __forceinline__ bool forward_body(const igmc_model_t& M, const float* __restrict__ params,
                                              const uint8_t* __restrict__ node_label,
                                              const int32_t* __restrict__ node_ptr,
@@ -633,6 +670,8 @@ __device__ __forceinline__ bool forward_body(const igmc_model_t& M, const float*
     Ls = stage_lists(A.in_adj, A.in_eid, A.in_ptr, nb, own.lo, own.hi, K, false, eb, m_half, lbuf, lcap, ibuf, own_cap,
                      chunk, ws, invdeg, S.inv_deg);
   }
+  float* rinv = PR ? S.rel_inv_deg + (size_t)nb * R : nullptr;   // [n][R] 1/|N_r(v)| (own rows written here)
+  if (PR) rel_inv_deg_own(Ls, K, A.in_ptr, nb, own.lo, n_own, R, rinv);
   if (tid == 0) ws[33] = 0;   // segment ticket of gather_segments (made visible by the barrier at the top of the layer loop)
   const bool ext = M.readout != 0;   // concat_states only: an external readout (csrc/sortpool.cu) takes over
   const int tu = s_t[0], ti = s_t[1];
@@ -669,7 +708,8 @@ __device__ __forceinline__ bool forward_body(const igmc_model_t& M, const float*
       if (l == 0) IGMC_STAMP(33);
       if (tid == 0) ws[33] = 0;   // re-arm the segment ticket (the next gather is several barriers away)
       IGMC_STAMP_T(0, 41); IGMC_STAMP_T(992, 44);
-      // ---- fold the extra segments of long lists into their node row, scale by 1/deg, keep a copy for backward ----
+      // ---- fold the extra segments of long lists into their node row, scale by 1/deg (PR: the relation block by
+      //      1/|N_r(v)|), keep a copy for backward ----
       {
         const int kq = K1 >> 2, SS4 = SS >> 2;
         float4* st4 = reinterpret_cast<float4*>(stage);
@@ -679,7 +719,7 @@ __device__ __forceinline__ bool forward_body(const igmc_model_t& M, const float*
         for (int idx = tid; idx < crow * kq; idx += NT, r += dr, k4 += dk) {
           if (k4 >= kq) { k4 -= kq; ++r; }
           const int v = own.lo + c0 + r;
-          const float id2 = invdeg[v];
+          const float id2 = PR ? __ldcg(rinv + (size_t)v * R + k4 / (inp >> 2)) : invdeg[v];
           const int e = Ls.ex[c0 + r], x0 = e & 0xffff, nex = e >> 16;
           float4 t = st4[(size_t)r * SS4 + k4];
           for (int j = 0; j < nex; ++j) {
@@ -839,14 +879,14 @@ __device__ __forceinline__ bool forward_body(const igmc_model_t& M, const float*
   return true;
 }
 
-template <int NTMAX>
+template <int NTMAX, bool PR>
 __global__ void __launch_bounds__(NTMAX, 1)
 k_forward_rs(igmc_model_t M, const float* __restrict__ params, const uint8_t* __restrict__ node_label,
              const int32_t* __restrict__ node_ptr, const int32_t* __restrict__ edge_ptr, igmc_adj_t A, int n_cap,
              int lcap, int chunk, igmc_dropout_t D, int training, igmc_saved_t S, const float* __restrict__ y,
              float loss_scale, float* __restrict__ dpred, float* __restrict__ sqerr, igmc_stage_t IMG, int* err) {
   extern __shared__ __align__(16) float smem[];
-  forward_body<NTMAX>(M, params, node_label, node_ptr, edge_ptr, A, n_cap, lcap, chunk, D, training, S, y, loss_scale,
+  forward_body<NTMAX, PR>(M, params, node_label, node_ptr, edge_ptr, A, n_cap, lcap, chunk, D, training, S, y, loss_scale,
                       dpred, sqerr, IMG, err, smem);
 }
 
@@ -876,14 +916,15 @@ __device__ __forceinline__ void wgrad_pass(const float* __restrict__ ha, const f
 }
 
 // Per layer l (top down), for the own nodes u of this CTA:
-//   (0) dpre = d h_l (1 - h_l^2); gather source DPS = dpre / deg of ALL nodes, DP = dpre of the own rows
+//   (0) dpre = d h_l (1 - h_l^2); gather source DPS = dpre / deg of ALL nodes (PR: dpre, the gather weighs every
+//       entry (d, r) by 1/|N_r(d)| instead), DP = dpre of the own rows
 //   (1) Q[u,r,:] = sum_{(u->d) of type r, kept} DPS[d,:]                  (gather over the out-lists, as forward)
 //       d h_{l-1}[u] = [Q[u] | dpre[u]] . [W_r^T ; root^T]                (tensor cores) -> pushed to every CTA
 //   (2) dW_r = sum_u h_{l-1}[u]^T Q[u,r,:],  d root = sum_u h_{l-1}[u]^T dpre[u],  d bias = sum_u dpre[u]
 //       (tensor cores, K = own nodes; A = the h_{l-1} rows fetched by TMA under the gather)  -> raw partial row
 //   Layer 0 has no data gradient; its dW_r come from the saved aggregate of the one-hot input (S.zsave).
 // The (att, basis) chain rule is NOT applied here: it is linear and runs once on the sum (igmc_grad_reduce).
-template <int NTMAX>
+template <int NTMAX, bool PR>
 __device__ __forceinline__ void backward_body(const igmc_model_t& M, const float* __restrict__ params,
                                               const uint8_t* __restrict__ node_label,
                                               const int32_t* __restrict__ node_ptr,
@@ -985,7 +1026,10 @@ __device__ __forceinline__ void backward_body(const igmc_model_t& M, const float
       if (rank == 0) dhid_out[(size_t)g * L1O + o] = d;
     }
   }
-  for (int v = tid; v < n; v += NT) invdeg[v] = __ldcg(S.inv_deg + nb + v);   // (peer rows: L2, see k_train_rs)
+  if (!PR)
+    for (int v = tid; v < n; v += NT) invdeg[v] = __ldcg(S.inv_deg + nb + v);   // (peer rows: L2, see k_train_rs)
+  // PR: 1/|N_r(d)| of every node d, read through L2 by the gather (peer rows, as inv_deg above)
+  const float* rinv = PR ? S.rel_inv_deg + (size_t)nb * R : nullptr;
   __syncthreads();
   if (!ext) {
     // d feat[i] = sum_o W1[o][i] d hid[o]: thread slice p of NT/F takes every (NT/F)-th o, partials in `stage`
@@ -1044,7 +1088,7 @@ __device__ __forceinline__ void backward_body(const igmc_model_t& M, const float
       const float4 h = __ldcg(reinterpret_cast<const float4*>(S.states + (size_t)(nb + v) * CW + l * HID + c4));
       const float4 dpre = make_float4(dh.x * (1.f - h.x * h.x), dh.y * (1.f - h.y * h.y), dh.z * (1.f - h.z * h.z),
                                       dh.w * (1.f - h.w * h.w));
-      const float id = invdeg[v];
+      const float id = PR ? 1.f : invdeg[v];   // (PR: the factor depends on the relation - applied per entry in (1))
       *reinterpret_cast<float4*>(DPS + hix(v, c4)) = make_float4(dpre.x * id, dpre.y * id, dpre.z * id, dpre.w * id);
       if (v >= own.lo && v < own.hi) *reinterpret_cast<float4*>(DP + (size_t)(v - own.lo) * DPS_ + c4) = dpre;
     }
@@ -1078,7 +1122,8 @@ __device__ __forceinline__ void backward_body(const igmc_model_t& M, const float
         }
         // (1) data gradient of the own nodes:  d h_{l-1}[u] = [Q[u] | dpre[u]] . [W_r^T ; root^T],
         //     Q[u,r,:] = sum_{(u->d) of type r, kept} dpre[d,:]/deg(d)         -> pushed to every CTA's DH
-        gather_segments<8>(Ls, K, Ls.segbase[c0], Ls.segbase[c0 + crow], lane, DPS, stage, SS, HID, &ws[33]);
+        gather_segments<8, PR>(Ls, K, Ls.segbase[c0], Ls.segbase[c0 + crow], lane, DPS, stage, SS, HID, &ws[33], rinv,
+                               R);
         __syncthreads();
         if (tid == 0) ws[33] = 0;
         {   // fold the extra segments of long lists into their node row
@@ -1293,14 +1338,14 @@ __device__ __forceinline__ void backward_body(const igmc_model_t& M, const float
   IGMC_WALL(54);
 }
 
-template <int NTMAX>
+template <int NTMAX, bool PR>
 __global__ void __launch_bounds__(NTMAX, 1)
 k_backward_rs(igmc_model_t M, const float* __restrict__ params, const uint8_t* __restrict__ node_label,
               const int32_t* __restrict__ node_ptr, const int32_t* __restrict__ edge_ptr, igmc_adj_t A, int n_cap,
               int lcap, int chunk, igmc_dropout_t D, igmc_saved_t S, const float* __restrict__ dpred,
               float* __restrict__ gpart, float* __restrict__ dhid_out, igmc_stage_t IMG, int* err) {
   extern __shared__ __align__(16) float smem[];
-  backward_body<NTMAX>(M, params, node_label, node_ptr, edge_ptr, A, n_cap, lcap, chunk, D, S, dpred, gpart, dhid_out,
+  backward_body<NTMAX, PR>(M, params, node_label, node_ptr, edge_ptr, A, n_cap, lcap, chunk, D, S, dpred, gpart, dhid_out,
                        IMG, err, smem);
 }
 
@@ -1309,8 +1354,9 @@ k_backward_rs(igmc_model_t M, const float* __restrict__ params, const uint8_t* _
 // second launch, and the spread of the forward times over the clusters is not paid twice (every cluster used to wait
 // for the slowest forward before any backward could start).  The shared memory is re-carved for the backward; what the
 // backward reads of the forward travels through global memory exactly as between the two separate kernels, ordered
-// by a device fence + cluster barrier (the peer CTA wrote half of the states / inv_deg rows, rank 0 the readout).
-template <int NTMAX>
+// by a device fence + cluster barrier (the peer CTA wrote half of the states / inv_deg / rel_inv_deg rows, rank 0 the
+// readout).
+template <int NTMAX, bool PR>
 __global__ void __launch_bounds__(NTMAX, 1)
 k_train_rs(igmc_model_t M, const float* __restrict__ params, const uint8_t* __restrict__ node_label,
            const int32_t* __restrict__ node_ptr, const int32_t* __restrict__ edge_ptr, igmc_adj_t A, int n_cap,
@@ -1318,13 +1364,13 @@ k_train_rs(igmc_model_t M, const float* __restrict__ params, const uint8_t* __re
            const float* __restrict__ y, float loss_scale, float* __restrict__ dpred, float* __restrict__ sqerr,
            float* __restrict__ gpart, float* __restrict__ dhid_out, igmc_stage_t IMGF, igmc_stage_t IMGB, int* err) {
   extern __shared__ __align__(16) float smem[];
-  const bool ok = forward_body<NTMAX>(M, params, node_label, node_ptr, edge_ptr, A, n_cap, lcap_f, chunk_f, D, 1, S, y,
+  const bool ok = forward_body<NTMAX, PR>(M, params, node_label, node_ptr, edge_ptr, A, n_cap, lcap_f, chunk_f, D, 1, S, y,
                                       loss_scale, dpred, sqerr, IMGF, err, smem);
   if (!ok) return;   // uniform over the cluster
   __threadfence();
   asm volatile("fence.proxy.async;" ::: "memory");   // the backward's bulk copies read state rows written above
   cg::this_cluster().sync();   // (a cluster of one CTA: a block barrier)
-  backward_body<NTMAX>(M, params, node_label, node_ptr, edge_ptr, A, n_cap, lcap_b, chunk_b, D, S, dpred, gpart,
+  backward_body<NTMAX, PR>(M, params, node_label, node_ptr, edge_ptr, A, n_cap, lcap_b, chunk_b, D, S, dpred, gpart,
                        dhid_out, IMGB, err, smem);
 }
 
@@ -1534,12 +1580,11 @@ int rs_forward(const igmc_model_t* M, const float* params, const uint8_t* node_l
   rc = check_image(stage, n_cap, cluster, lcap, chunk, &img);
   if (rc) return rc;
   if (img.tab && !img.inv_deg) return -19;
-  if (threads == 512)
-    return launch_cluster(rs::k_forward_rs<512>, B * cluster, threads, smem, cluster, false, st, *M, params, node_label,
-                          node_ptr, edge_ptr, *A, n_cap, lcap, chunk, *D, training, *S, y, loss_scale, dpred, sqerr, img,
-                          err);
-  return launch_cluster(rs::k_forward_rs<1024>, B * cluster, threads, smem, cluster, false, st, *M, params, node_label, node_ptr,
-                        edge_ptr, *A, n_cap, lcap, chunk, *D, training, *S, y, loss_scale, dpred, sqerr, img, err);
+  const bool pr = S->rel_inv_deg != nullptr;
+  auto kern = threads == 512 ? (pr ? rs::k_forward_rs<512, true> : rs::k_forward_rs<512, false>)
+                             : (pr ? rs::k_forward_rs<1024, true> : rs::k_forward_rs<1024, false>);
+  return launch_cluster(kern, B * cluster, threads, smem, cluster, false, st, *M, params, node_label, node_ptr, edge_ptr,
+                        *A, n_cap, lcap, chunk, *D, training, *S, y, loss_scale, dpred, sqerr, img, err);
 }
 
 int rs_backward(const igmc_model_t* M, const float* params, const uint8_t* node_label, const int32_t* node_ptr,
@@ -1553,11 +1598,11 @@ int rs_backward(const igmc_model_t* M, const float* params, const uint8_t* node_
   igmc_stage_t img;
   rc = check_image(stage, n_cap, cluster, lcap, chunk, &img);
   if (rc) return rc;
-  if (threads == 512)
-    return launch_cluster(rs::k_backward_rs<512>, B * cluster, threads, smem, cluster, true, st, *M, params, node_label,
-                          node_ptr, edge_ptr, *A, n_cap, lcap, chunk, *D, *S, dpred, gpart, dhid, img, err);
-  return launch_cluster(rs::k_backward_rs<1024>, B * cluster, threads, smem, cluster, true, st, *M, params, node_label, node_ptr,
-                        edge_ptr, *A, n_cap, lcap, chunk, *D, *S, dpred, gpart, dhid, img, err);
+  const bool pr = S->rel_inv_deg != nullptr;
+  auto kern = threads == 512 ? (pr ? rs::k_backward_rs<512, true> : rs::k_backward_rs<512, false>)
+                             : (pr ? rs::k_backward_rs<1024, true> : rs::k_backward_rs<1024, false>);
+  return launch_cluster(kern, B * cluster, threads, smem, cluster, true, st, *M, params, node_label, node_ptr, edge_ptr,
+                        *A, n_cap, lcap, chunk, *D, *S, dpred, gpart, dhid, img, err);
 }
 
 namespace rs {
@@ -1600,13 +1645,11 @@ int rs_train(const igmc_model_t* M, const float* params, const uint8_t* node_lab
   rc = check_image(stage_b, n_cap, cluster, lcb, chb, &imb);
   if (rc) return rc;
   const size_t smem = smf > smb ? smf : smb;
-  if (tf == 512)
-    return launch_cluster(rs::k_train_rs<512>, B * cluster, tf, smem, cluster, false, st, *M, params, node_label, node_ptr,
-                          edge_ptr, *A, n_cap, lcf, chf, lcb, chb, *D, *S, y, loss_scale, dpred, sqerr, gpart, dhid, imf,
-                          imb, err);
-  return launch_cluster(rs::k_train_rs<1024>, B * cluster, tf, smem, cluster, false, st, *M, params, node_label, node_ptr,
-                        edge_ptr, *A, n_cap, lcf, chf, lcb, chb, *D, *S, y, loss_scale, dpred, sqerr, gpart, dhid, imf, imb,
-                        err);
+  const bool pr = S->rel_inv_deg != nullptr;
+  auto kern = tf == 512 ? (pr ? rs::k_train_rs<512, true> : rs::k_train_rs<512, false>)
+                        : (pr ? rs::k_train_rs<1024, true> : rs::k_train_rs<1024, false>);
+  return launch_cluster(kern, B * cluster, tf, smem, cluster, false, st, *M, params, node_label, node_ptr, edge_ptr, *A,
+                        n_cap, lcf, chf, lcb, chb, *D, *S, y, loss_scale, dpred, sqerr, gpart, dhid, imf, imb, err);
 }
 
 int rs_prep_weights(const igmc_model_t* M, const float* params, float* wprep, cudaStream_t st) {

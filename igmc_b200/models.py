@@ -3,7 +3,8 @@
 ``IGMC(dataset, gconv, latent_dim, num_relations, num_bases, regression, adj_dropout, ...)`` keeps the
 reference constructor, ``forward(data) -> Tensor[B]``, ``reset_parameters()``, the attribute surface
 ``convs[l].{att, basis, root, bias, num_bases, num_relations, in_channels, out_channels}``, ``lin1``,
-``lin2`` and therefore the reference's ``state_dict`` keys, so its checkpoints load.
+``lin2`` and therefore the reference's ``state_dict`` keys, so its checkpoints load.  ``rgcn="pyg-2"`` swaps in the
+RGCNConv of PyG >= 1.6 (``convs[l].{comp, weight, root, bias}``, one mean per relation) on the same kernels.
 
 All parameters are views into ONE flat fp32 buffer (``flat_params``), gradients into ``flat_grad``:
 that buffer is what the kernels read, what the single NCCL all-reduce per step moves and what the fused
@@ -122,9 +123,54 @@ class RGCNConv(nn.Module):
             for p in (self.basis, self.att, self.root, self.bias):
                 p.uniform_(-bound, bound)
 
+    def att_basis(self):
+        """(coefficients [R,NB], bases [NB,in,out]) of W_r = sum_b att[r,b] basis[b]"""
+        return self.att, self.basis
+
     def __repr__(self):
         return "RGCNConv(%d, %d, num_relations=%d, num_bases=%d)" % (
             self.in_channels, self.out_channels, self.num_relations, self.num_bases)
+
+
+class RGCNConv2(nn.Module):
+    """Parameter holder with the names/shapes/init of PyG >= 1.6 ``RGCNConv(in, out, num_relations, num_bases)``:
+    ``weight [NB,in,out]``, ``comp [R,NB]``, ``root [in,out]``, ``bias [out]``; glorot(weight, comp, root), zeros(bias)
+    (PyG 2.x ``reset_parameters``).  W_r = sum_b comp[r,b] weight[b] - the 1.4.2 layer's ``att @ basis`` - but the
+    aggregation is a mean PER RELATION (``IGMC(..., rgcn="pyg-2")``; DESIGN.md §2)."""
+
+    def __init__(self, in_channels, out_channels, num_relations, num_bases):
+        super().__init__()
+        self.in_channels, self.out_channels = in_channels, out_channels
+        self.num_relations, self.num_bases = num_relations, num_bases
+        self.weight = nn.Parameter(torch.empty(num_bases, in_channels, out_channels))
+        self.comp = nn.Parameter(torch.empty(num_relations, num_bases))
+        self.root = nn.Parameter(torch.empty(in_channels, out_channels))
+        self.bias = nn.Parameter(torch.empty(out_channels))
+        self.reset_parameters()
+
+    def reset_parameters(self):
+        with torch.no_grad():
+            for p in (self.weight, self.comp, self.root):   # PyG inits.glorot: U(+-sqrt(6 / (size(-2) + size(-1))))
+                bound = math.sqrt(6.0 / (p.size(-2) + p.size(-1)))
+                p.uniform_(-bound, bound)
+            self.bias.zero_()
+
+    def att_basis(self):
+        return self.comp, self.weight
+
+    def __repr__(self):
+        return "RGCNConv(%d, %d, num_relations=%d, num_bases=%d)" % (
+            self.in_channels, self.out_channels, self.num_relations, self.num_bases)
+
+
+# rgcn= keyword of IGMC / DGCNN_RS: which RGCNConv the model is (names, init and aggregation go together)
+RGCN_LAYERS = {"pyg-1.4": RGCNConv, "pyg-2": RGCNConv2}
+
+
+def _rgcn_layer(rgcn):
+    if not isinstance(rgcn, str) or rgcn not in RGCN_LAYERS:
+        raise ValueError("rgcn must be one of %s, not %r" % (sorted(RGCN_LAYERS), rgcn))
+    return RGCN_LAYERS[rgcn]
 
 
 class _IGMCFunction(torch.autograd.Function):
@@ -152,8 +198,10 @@ class _IGMCFunction(torch.autograd.Function):
 class IGMC(nn.Module):
     def __init__(self, dataset, gconv=RGCNConv, latent_dim=[32, 32, 32, 32], num_relations=5, num_bases=2,
                  regression=False, adj_dropout=0.2, force_undirected=False, side_features=False,
-                 n_side_features=0, multiply_by=1):
+                 n_side_features=0, multiply_by=1, rgcn="pyg-1.4"):
         super().__init__()
+        conv_cls = _rgcn_layer(rgcn)
+        self.rgcn = rgcn
         if not regression:
             raise NotImplementedError("igmc_b200.IGMC implements the regression head Main.py uses (Main.py:396)")
         if force_undirected:
@@ -172,7 +220,7 @@ class IGMC(nn.Module):
             raise NotImplementedError("node feature width > 32")
         self.num_relations, self.num_bases = int(num_relations), int(num_bases)
         dims = [self.num_features] + [int(d) for d in latent_dim]
-        self.convs = nn.ModuleList([RGCNConv(dims[l], dims[l + 1], num_relations, num_bases)
+        self.convs = nn.ModuleList([conv_cls(dims[l], dims[l + 1], num_relations, num_bases)
                                     for l in range(len(latent_dim))])
         self.lin1 = nn.Linear(2 * sum(latent_dim), 128)
         self.lin2 = nn.Linear(128, 1)
@@ -184,8 +232,9 @@ class IGMC(nn.Module):
     # ---- flat parameter bucket ---------------------------------------------------------------------
     def _named_order(self):
         for l, c in enumerate(self.convs):
-            yield ("att", l, c.att)
-            yield ("basis", l, c.basis)
+            att, basis = c.att_basis()    # (comp, weight) of a PyG >= 1.6 layer: the same slots of the bucket
+            yield ("att", l, att)
+            yield ("basis", l, basis)
             yield ("root", l, c.root)
             yield ("bias", l, c.bias)
         yield ("lin1_w", 0, self.lin1.weight)
@@ -258,9 +307,17 @@ class IGMC(nn.Module):
         self._flatten()
         return out
 
-    def load_state_dict(self, *a, **kw):
+    def load_state_dict(self, state_dict, *a, **kw):
+        # the two RGCNConv layers compute different functions of equally shaped parameters: refuse the other layer's
+        # checkpoint by its key names even when strict=False would load the rest of it
+        own, other = (("att", "basis"), ("comp", "weight")) if self.rgcn == "pyg-1.4" else \
+            (("comp", "weight"), ("att", "basis"))
+        foreign = [k for k in state_dict if k.startswith("convs.") and k.rsplit(".", 1)[-1] in other]
+        if foreign:
+            raise RuntimeError("igmc_b200: %s belongs to the other RGCNConv layer (this model has rgcn=%r: convs.*.%s / "
+                               "convs.*.%s); build the model with the matching rgcn= keyword" % ((foreign[0], self.rgcn) + own))
         self._prepped = False         # prepared weights (igmc_prep_weights) belong to the old parameters
-        return super().load_state_dict(*a, **kw)
+        return super().load_state_dict(state_dict, *a, **kw)
 
     def reset_parameters(self):
         for c in self.convs:
@@ -312,6 +369,8 @@ class IGMC(nn.Module):
                       target=torch.empty(B, 2, dtype=torch.int32, device=dev),
                       dpred=torch.zeros(B, **f32), sqerr=torch.zeros(B, **f32), loss=torch.zeros(1, **f32),
                       reg_ws=torch.zeros(_lib.REDUCE_WS_FLOATS, **f32), cluster=cl)
+            if self.rgcn == "pyg-2":   # mean per relation: 1/|N_r(v)| table, filled by the forward
+                ws["rel_inv_deg"] = torch.empty(ncap, self.num_relations, **f32)
             if train:
                 if _lib.is_rs(cl):   # cluster plans: layer-0 aggregate only; raw partial rows (chain rule in igmc_grad_reduce)
                     zs = torch.empty(ncap, self.num_relations * _align4(self.num_features), **f32)
@@ -387,7 +446,7 @@ class IGMC(nn.Module):
                           _lib.ptr(self._wprep_buf()) if rs else None,
                           _lib.ptr(getattr(self, "_prof_buf", None)),
                           _lib.ptr(self._gate) if (rs and self.__dict__.pop("_gate_armed", False)) else None,
-                          _lib.ptr(ws.get("l2_scratch")))
+                          _lib.ptr(ws.get("l2_scratch")), _lib.ptr(ws.get("rel_inv_deg")))
 
     def prep_weights(self, mark=False):
         """launch igmc_prep_weights on the current stream; ``mark`` lets the next forward skip its own launch (the
@@ -579,8 +638,10 @@ class DGCNN_RS(IGMC):
     C1, C2, KW2 = 16, 32, 5   # conv1d_channels and the second kernel width (models.py:75-79)
 
     def __init__(self, dataset, gconv=RGCNConv, latent_dim=[32, 32, 32, 1], k=30, num_relations=5, num_bases=2,
-                 regression=False, adj_dropout=0.2, force_undirected=False):
+                 regression=False, adj_dropout=0.2, force_undirected=False, rgcn="pyg-1.4"):
         nn.Module.__init__(self)
+        conv_cls = _rgcn_layer(rgcn)
+        self.rgcn = rgcn
         if not regression:
             raise NotImplementedError("igmc_b200.DGCNN_RS implements the regression head (x[:, 0], models.py:165)")
         if force_undirected:
@@ -610,7 +671,7 @@ class DGCNN_RS(IGMC):
         self.num_relations, self.num_bases = int(num_relations), int(num_bases)
         self.latent_dim = latent_dim
         dims = [self.num_features] + latent_dim
-        self.convs = nn.ModuleList([RGCNConv(dims[l], dims[l + 1], num_relations, num_bases)
+        self.convs = nn.ModuleList([conv_cls(dims[l], dims[l + 1], num_relations, num_bases)
                                     for l in range(len(latent_dim))])
         self.total_latent_dim = sum(latent_dim)
         self.conv1d_params1 = nn.Conv1d(1, self.C1, self.total_latent_dim, self.total_latent_dim)
@@ -629,8 +690,9 @@ class DGCNN_RS(IGMC):
 
     def _named_order(self):
         for l, c in enumerate(self.convs):
-            yield ("att", l, c.att)
-            yield ("basis", l, c.basis)
+            att, basis = c.att_basis()
+            yield ("att", l, att)
+            yield ("basis", l, basis)
             yield ("root", l, c.root)
             yield ("bias", l, c.bias)
         yield ("conv1_w", 0, self.conv1d_params1.weight)

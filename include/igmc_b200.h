@@ -200,6 +200,12 @@ typedef struct {
   long long* prof;    /* optional debug: [grid][64] clock64() stamps of the kernel phases (cluster plans), or NULL */
   int32_t* gate;      /* optional: every CTA of igmc_forward (cluster plans) adds 1 when it starts, see igmc_gate_wait */
   float* l2_scratch;  /* [2 * node_cap * 32] backward scratch of the L2 plan (d pre / d h of two layers), else unused */
+  float* rel_inv_deg; /* NULL: PyG 1.4.2 RGCNConv, one mean over all kept in-edges of a node (1/deg(v), inv_deg).
+                       * Non-NULL, [node_cap * R]: PyG >= 1.6 RGCNConv(aggr='mean'), one mean per relation -
+                       * x'_v = x_v root + bias + sum_r 1/|N_r(v)| sum_{u in N_r(v)} x_u W_r.  igmc_forward fills
+                       * rel_inv_deg[v*R + r] = 1/max(kept in-edges of type r at v, 1) and normalises with it;
+                       * igmc_backward / igmc_forward_backward read it.  The forward and backward of one step must agree
+                       * on the mode.  Every plan supports both; plans, shared memory and list images are the same. */
 } igmc_saved_t;
 
 /* Launch-order gate for work that should run BESIDE the forward kernel without taking SMs from it (the extraction of
