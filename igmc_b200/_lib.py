@@ -24,7 +24,10 @@ ERR_NAMES = {
     4: "subgraph larger than the shared-memory plan of the model kernels (n_cap)",
     5: "malformed batch (edges not grouped by graph / node outside its graph / no target node)",
     6: "subgraph of more than 65535 nodes (beyond the 16-bit neighbour field of the edge lists)",
+    7: "inference candidates: a user / item id outside the rating matrix or an inconsistent candidate plan",
 }
+
+TOPK_MAX = 256       # IGMC_TOPK_MAX
 
 # Kernel plan values (igmc_model_plan): 0 generic kernels, 1..4 relation-space cluster kernels (CTAs per subgraph),
 # PLAN_L2_BASE + c (c = 1, 2, 4, 8) the L2 plan with c CTAs per subgraph (IGMC_PLAN_L2 in include/igmc_b200.h).
@@ -111,6 +114,12 @@ class Stage(C.Structure):
                 ("chunk", C.c_int32), ("cluster", C.c_int32)]
 
 
+class Candidates(C.Structure):
+    _fields_ = [("users", vp), ("cand", vp), ("pair_u", vp), ("pair_v", vp), ("user_off", vp), ("rated_off", vp),
+                ("rated_pos", vp), ("num_pairs", C.c_int64), ("num_query", C.c_int32), ("num_cand", C.c_int32),
+                ("exclude_rated", C.c_int32), ("pad_", C.c_int32)]
+
+
 MAX_RANKS = 8
 
 
@@ -160,6 +169,10 @@ _SIGS = {
     "igmc_comm_free": [vp],
     "igmc_prep_weights": [C.POINTER(Model), vp, vp, vp],
     "igmc_gate_wait": [vp, C.c_int, C.c_int, vp],
+    "igmc_candidate_plan": [C.POINTER(CSR), C.POINTER(Candidates), vp, vp],
+    "igmc_candidate_pairs": [C.POINTER(CSR), C.POINTER(Candidates), vp, C.c_int, vp, vp, vp, vp, vp, vp],
+    "igmc_topk_merge": [vp, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp, vp],
+    "igmc_score_scatter": [vp, C.c_int, C.c_int, vp, vp, vp],
     "igmc_build_info": [],
     "igmc_model_plan": [C.POINTER(Model), C.c_int, C.c_int, C.c_int],
     "igmc_sortpool_plan": [C.POINTER(SortPool), C.c_int, C.c_int],

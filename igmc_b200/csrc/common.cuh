@@ -15,6 +15,7 @@ enum {
   IGMC_ERR_SMEM_NODES = 4,  // subgraph larger than the model kernel's shared-memory plan
   IGMC_ERR_BAD_BATCH = 5,   // edges not grouped by graph / node ids outside their graph
   IGMC_ERR_NODE_ID16 = 6,   // subgraph of more than 65 535 nodes: beyond the 16-bit neighbour field of the lists
+  IGMC_ERR_CANDIDATES = 7,  // inference candidates: a user / item id outside the rating matrix or an inconsistent plan
 };
 
 __device__ __forceinline__ void igmc_set_err(int* err, int code) {

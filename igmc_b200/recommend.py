@@ -1,0 +1,425 @@
+"""Score unrated (user, item) pairs and recommend the top-k items per user on the fused kernels.
+
+IGMC is inductive: it scores any (user, item) pair from the pair's enclosing subgraph.  The reference only reduces
+predictions to an RMSE over a labelled dataset (train_eval.py:182-245); ranking the items a user has not rated means
+building a dataset of every candidate pair and looping over it in Python.  Here:
+
+* ``predict_pairs(model, graph, users, items)`` -> fp32 scores of the explicit pairs ``(users[i], items[i])``;
+* ``recommend(model, graph, users, k)`` -> per query user the ``k`` best candidate items and their scores (candidates:
+  ``items`` or every item, without the user's rated items when ``exclude_rated``), ranked by score descending, then
+  item ascending; a NaN score ranks last; missing slots hold item -1 and score -inf;
+* ``InferenceEngine``: the pipelined, graph-replayed loop behind both.  Per step the side stream produces the next
+  batch's candidate pairs (``igmc_candidate_pairs``, from a device cursor) and extracts it while the main stream runs
+  the eval forward of the current batch (once per checkpoint) and merges its scores into the running per-user top-k
+  lists (``igmc_topk_merge``) or scatters them to their pair index (``igmc_score_scatter``).  The step is one CUDA graph
+  per batch slot, captured after an eager warm-up; between steps there is no host copy and no host synchronisation.
+
+Every pair samples its subgraph with ``pair_id = u * num_items + v``: its subgraph, and so its score, does not depend on
+the API that scored it, the batch it fell into or the candidate list.  The host twins below restate the kernels'
+integer arithmetic for the CPU tests (tests/test_recommend_host.py).
+"""
+import contextlib
+import ctypes as C
+
+import numpy as np
+import torch
+
+from . import _lib
+from .util_functions import RatingGraph, SubgraphExtractor, _stream_ptr
+
+__all__ = ["predict_pairs", "recommend", "InferenceEngine"]
+
+
+# ---- input validation (host) ----------------------------------------------------------------------------------------
+def _host_ids(a, name, hi):
+    """ids as a host int64 vector (device tensors: one copy to the host), each in [0, hi) or IndexError"""
+    if torch.is_tensor(a):
+        a = a.detach().cpu().numpy()
+    a = np.asarray(a).reshape(-1)
+    if a.size == 0:
+        return np.zeros(0, np.int64)
+    if not np.issubdtype(a.dtype, np.integer):
+        raise TypeError("%s must be integer ids, not %s" % (name, a.dtype))
+    a = a.astype(np.int64)
+    lo, top = int(a.min()), int(a.max())
+    if lo < 0 or top >= hi:
+        raise IndexError("%s: id %d out of range [0, %d)" % (name, lo if lo < 0 else top, hi))
+    return a
+
+
+def _check_k(k):
+    k = int(k)
+    if k < 1:
+        raise ValueError("k must be >= 1, not %d" % k)
+    if k > _lib.TOPK_MAX:
+        raise NotImplementedError("the top-k merge kernel keeps at most k = %d items per user" % _lib.TOPK_MAX)
+    return k
+
+
+# ---- host twins of the candidate and merge kernels (csrc/recommend.cu) ----------------------------------------------
+def candidate_plan_host(row_ptr, col_idx, num_items, users, cand=None, exclude_rated=True):
+    """twin of igmc_candidate_plan: (user_off [U+1], rated_off [U+1] or None, rated_pos or None)"""
+    users = np.asarray(users, np.int64)
+    U = len(users)
+    deg = np.asarray(row_ptr[users + 1] - row_ptr[users], np.int64) if U else np.zeros(0, np.int64)
+    lists = cand is not None and exclude_rated
+    rated_pos = []
+    if cand is None:
+        cnt = num_items - deg if exclude_rated else np.full(U, num_items, np.int64)
+    elif not exclude_rated:
+        cnt = np.full(U, len(cand), np.int64)
+    else:
+        cand = np.asarray(cand, np.int64)
+        hits = np.zeros(U, np.int64)
+        for j, u in enumerate(users):
+            row = np.asarray(col_idx[row_ptr[u]:row_ptr[u + 1]], np.int64)
+            p = np.searchsorted(cand, row)
+            found = (p < len(cand)) & (cand[np.minimum(p, max(len(cand) - 1, 0))] == row) if len(cand) else \
+                np.zeros(len(row), bool)
+            rated_pos.append(p[found])
+            hits[j] = int(found.sum())
+        cnt = len(cand) - hits
+    user_off = np.concatenate([[0], np.cumsum(cnt)]).astype(np.int64)
+    if not lists:
+        return user_off, None, None
+    rated_off = np.concatenate([[0], np.cumsum([len(r) for r in rated_pos])]).astype(np.int64)
+    return user_off, rated_off, (np.concatenate(rated_pos) if rated_pos else np.zeros(0, np.int64)).astype(np.int64)
+
+
+def candidate_pairs_host(row_ptr, col_idx, num_items, users, cand, exclude_rated, plan, pos, B):
+    """twin of igmc_candidate_pairs for global positions [pos, pos + B): (links_u, links_v, pair_id, tag)"""
+    user_off, rated_off, rated_pos = plan
+    P = int(user_off[-1])
+    out = np.zeros((4, B), np.int64)
+    for i in range(B):
+        g = pos + i
+        real = g < P
+        if not real:
+            g = P - 1
+        j = int(np.searchsorted(user_off, g, side="right")) - 1      # the last j with user_off[j] <= g
+        j = min(j, len(users) - 1)
+        c = g - int(user_off[j])
+        u = int(users[j])
+        p = c
+        if exclude_rated:
+            r = rated_pos[rated_off[j]:rated_off[j + 1]] if cand is not None else col_idx[row_ptr[u]:row_ptr[u + 1]]
+            r = np.asarray(r, np.int64)
+            p = c + int(np.count_nonzero(r - np.arange(len(r)) <= c))
+        v = int(cand[p]) if cand is not None else p
+        out[:, i] = (u, v, u * num_items + v, j if real else -1)
+    return out
+
+
+def _before(a_s, a_i, b_s, b_i):
+    """the ranking order of igmc_topk_merge: score descending, item ascending, NaN last, empty slots (item < 0) after
+    everything"""
+    if a_i < 0:
+        return False
+    if b_i < 0:
+        return True
+    an, bn = np.isnan(a_s), np.isnan(b_s)
+    if an or bn:
+        return a_i < b_i if (an and bn) else bool(bn)
+    return a_s > b_s or (a_s == b_s and a_i < b_i)
+
+
+def topk_merge_host(top_s, top_i, seg_s, seg_i):
+    """twin of one CTA of igmc_topk_merge: the running list (k, ranked) merged with one segment of new candidates by
+    rank counting; returns the new (scores, items)"""
+    k = len(top_s)
+    S = list(np.asarray(top_s, np.float32)) + list(np.asarray(seg_s, np.float32))
+    It = list(np.asarray(top_i, np.int64)) + list(np.asarray(seg_i, np.int64))
+    out_s, out_i = np.array(top_s, np.float32), np.array(top_i, np.int64)
+    for e in range(len(S)):
+        if e < k:
+            r = e
+        else:
+            r = sum(1 for o in range(k) if _before(S[o], It[o], S[e], It[e]))
+        r += sum(1 for x in range(k, len(S)) if x != e and _before(S[x], It[x], S[e], It[e]))
+        if r < k:
+            out_s[r], out_i[r] = S[e], It[e]
+    return out_s, out_i
+
+
+def rank_host(scores, items, k):
+    """brute-force ranking: the first ``k`` of ``items`` by (score descending, item ascending, NaN last), padded
+    with (-1, -inf)"""
+    scores, items = np.asarray(scores, np.float32), np.asarray(items, np.int64)
+    o = np.argsort(items, kind="stable")
+    o = o[np.argsort(-scores[o], kind="stable")]          # numpy sorts NaN last
+    top_i = np.full(k, -1, np.int64)
+    top_s = np.full(k, -np.inf, np.float32)
+    n = min(k, len(o))
+    top_i[:n], top_s[:n] = items[o[:n]], scores[o[:n]]
+    return top_s, top_i
+
+
+# ---- the engine -----------------------------------------------------------------------------------------------------
+class InferenceEngine(object):
+    """Pipelined, graph-replayed scoring of candidate pairs (module docstring).  ``checkpoints``: state_dict files of
+    ``model``'s class, each scored and averaged (fp32 sum in checkpoint order / K); None scores ``model``'s own
+    parameters as they are when a run starts.
+
+        eng = InferenceEngine(model, graph, batch_size=256)
+        eng.start_recommend(users, k)          # or eng.start_pairs(users, items)
+        while eng.step():
+            pass
+        top_items, top_scores = eng.finish()   # (predict: scores)
+    """
+
+    def __init__(self, model, graph, h=1, sample_ratio=1.0, max_nodes_per_hop=None, batch_size=256,
+                 checkpoints=None, sample_seed=0, use_graph=True):
+        dev = model.flat_params.device
+        if dev.type != "cuda":
+            raise RuntimeError("igmc_b200 inference needs the model on a CUDA device (there is no CPU path)")
+        if model.num_features != 2 * int(h) + 2:
+            raise ValueError("the model takes %d node features, hop %d extraction gives %d"
+                             % (model.num_features, int(h), 2 * int(h) + 2))
+        self.B = int(batch_size)
+        if self.B < 1:
+            raise ValueError("batch_size must be >= 1")
+        self.lib = _lib.load()
+        self.model, self.dev, self.use_graph = model, dev, bool(use_graph)
+        self.graph = graph if isinstance(graph, RatingGraph) else RatingGraph(graph, dev)
+        if self.graph.device is None or self.graph.device != dev:
+            self.graph.to(dev)
+        R = model.num_relations
+        self.extractor = SubgraphExtractor(self.graph, [0], [0], [0], np.arange(1, R + 1, dtype=np.float32), h,
+                                           sample_ratio, max_nodes_per_hop, max_batch=self.B, seed=sample_seed)
+        self.drop = model.make_dropout(False)        # eval: no edge dropout, no hidden dropout
+        if checkpoints:
+            own = model.flat_params.clone()
+            self.params = []
+            for path in checkpoints:
+                model.load_state_dict(torch.load(path, map_location=dev))
+                self.params.append(model.flat_params.clone())
+            with torch.no_grad():
+                model.flat_params.copy_(own)
+            model._prepped = False
+        else:
+            self.params = [model.flat_params]
+        self.K = len(self.params)
+        self.wprep = [torch.zeros_like(model._wprep_buf()) for _ in range(self.K)]
+        i32, i64 = dict(dtype=torch.int32, device=dev), dict(dtype=torch.int64, device=dev)
+        self.cursor = torch.zeros(1, **i64)
+        # per batch slot: the candidate pairs igmc_extract_batch reads (idx = NULL) and their query slot / pair index
+        self.slots = [dict(u=torch.zeros(self.B, **i32), v=torch.zeros(self.B, **i32), pid=torch.zeros(self.B, **i64),
+                           tag=torch.zeros(self.B, **i64)) for _ in range(2)]
+        self.preds = torch.zeros(self.K, self.B, dtype=torch.float32, device=dev)
+        self.side = torch.cuda.Stream(dev)
+        self.run = None
+
+    # ---- one run: plan, prime, steps, finish --------------------------------------------------------------------
+    def start_recommend(self, users, k, items=None, exclude_rated=True):
+        """plan a ranking run (one host sync: the candidate total).  Returns the number of candidate pairs."""
+        k = _check_k(k)
+        g = self.graph
+        users = _host_ids(users, "users", g.num_users)
+        cand = None if items is None else np.unique(_host_ids(items, "items", g.num_items))
+        U, dev = len(users), self.dev
+        run = dict(kind="recommend", U=U, k=k,
+                   top_s=torch.full((U, k), -float("inf"), dtype=torch.float32, device=dev),
+                   top_i=torch.full((U, k), -1, dtype=torch.int64, device=dev))
+        self.run = run
+        if U == 0 or (cand is not None and len(cand) == 0):
+            run["P"] = 0
+            return 0
+        i64 = dict(dtype=torch.int64, device=dev)
+        run["users"] = torch.from_numpy(users.astype(np.int32)).to(dev)
+        run["cand"] = None if cand is None else torch.from_numpy(cand.astype(np.int32)).to(dev)
+        run["user_off"] = torch.zeros(U + 1, **i64)
+        lists = cand is not None and bool(exclude_rated)
+        if lists:
+            rp = g.host["row_ptr"]
+            run["rated_off"] = torch.zeros(U + 1, **i64)
+            run["rated_pos"] = torch.zeros(max(int((rp[users + 1] - rp[users]).sum()), 1), dtype=torch.int32,
+                                           device=dev)
+        Cd = _lib.Candidates()
+        Cd.users, Cd.cand = run["users"].data_ptr(), _lib.ptr(run["cand"])
+        Cd.user_off = run["user_off"].data_ptr()
+        Cd.rated_off, Cd.rated_pos = _lib.ptr(run.get("rated_off")), _lib.ptr(run.get("rated_pos"))
+        Cd.num_query, Cd.num_cand = U, 0 if cand is None else len(cand)
+        Cd.exclude_rated = int(bool(exclude_rated))
+        _lib.check(self.lib.igmc_candidate_plan(C.byref(g._c), C.byref(Cd), self.extractor.err.data_ptr(),
+                                                _stream_ptr()), "igmc_candidate_plan")
+        Cd.num_pairs = run["P"] = int(run["user_off"][U].item())
+        run["Cd"] = Cd
+        if run["P"] > 0:
+            self._prime()
+        return run["P"]
+
+    def start_pairs(self, users, items):
+        """plan a run over the explicit pairs (users[i], items[i]).  Returns their number."""
+        g = self.graph
+        users = _host_ids(users, "users", g.num_users)
+        items = _host_ids(items, "items", g.num_items)
+        if len(users) != len(items):
+            raise ValueError("users and items must have the same length (%d vs %d)" % (len(users), len(items)))
+        P = len(users)
+        run = dict(kind="pairs", P=P, scores=torch.empty(P, dtype=torch.float32, device=self.dev))
+        self.run = run
+        if P == 0:
+            return 0
+        run["pu"] = torch.from_numpy(users.astype(np.int32)).to(self.dev)
+        run["pv"] = torch.from_numpy(items.astype(np.int32)).to(self.dev)
+        Cd = _lib.Candidates()
+        Cd.pair_u, Cd.pair_v, Cd.num_pairs = run["pu"].data_ptr(), run["pv"].data_ptr(), P
+        run["Cd"] = Cd
+        self._prime()
+        return P
+
+    def _prime(self):
+        """candidate pairs + extraction of the first batch, the model's plan for it (its one host sync, if any) and
+        the prepared weights of every parameter set; captured graphs of an earlier run are dropped (they hold its
+        buffers and candidate total)"""
+        run = self.run
+        run["steps"] = (run["P"] + self.B - 1) // self.B
+        run["done"] = 0
+        self.graphs, self.eager_done = {}, set()
+        self.cursor.zero_()
+        self.batches = [None, None]
+        self._next(0)
+        if _lib.is_rs(self.model._plan(self.batches[0])):
+            for j in range(self.K):
+                with self._params(j):
+                    self.model.prep_weights()
+
+    def _next(self, slot):
+        """candidate pairs of the next B positions (device cursor) + their extraction into batch slot ``slot``"""
+        s, run = self.slots[slot], self.run
+        _lib.check(self.lib.igmc_candidate_pairs(C.byref(self.graph._c), C.byref(run["Cd"]), self.cursor.data_ptr(),
+                                                 self.B, s["u"].data_ptr(), s["v"].data_ptr(), s["pid"].data_ptr(),
+                                                 s["tag"].data_ptr(), self.extractor.err.data_ptr(), _stream_ptr()),
+                   "igmc_candidate_pairs")
+        self.batches[slot] = self.extractor.extract(pairs=(s["u"], s["v"], None), pair_ids=s["pid"], reuse=True,
+                                                    slot=slot)
+
+    @contextlib.contextmanager
+    def _params(self, j):
+        """the model's kernels read parameter set ``j`` and its prepared weights inside the block (the launch code of
+        the model is used as it is; only the buffers it reads are exchanged)"""
+        m = self.model
+        own = (m.flat_params, m._wprep, m.__dict__.get("_prepped", False))
+        m.flat_params, m._wprep, m._prepped = self.params[j], self.wprep[j], True
+        try:
+            yield
+        finally:
+            m.flat_params, m._wprep, m._prepped = own
+
+    def _score(self, slot):
+        """eval forward of batch ``slot`` with every parameter set, then the merge / scatter of the mean"""
+        m, b, s, run = self.model, self.batches[slot], self.slots[slot], self.run
+        preds = None
+        for j in range(self.K):
+            with self._params(j):
+                pred, _ = m._launch_forward(b, False, self.drop)
+            if self.K == 1:
+                preds = pred
+            else:
+                self.preds[j].copy_(pred)
+                preds = self.preds
+        if run["kind"] == "recommend":
+            _lib.check(self.lib.igmc_topk_merge(preds.data_ptr(), self.K, self.B, s["tag"].data_ptr(),
+                                                s["v"].data_ptr(), run["k"], run["top_s"].data_ptr(),
+                                                run["top_i"].data_ptr(), _stream_ptr()), "igmc_topk_merge")
+        else:
+            _lib.check(self.lib.igmc_score_scatter(preds.data_ptr(), self.K, self.B, s["tag"].data_ptr(),
+                                                   run["scores"].data_ptr(), _stream_ptr()), "igmc_score_scatter")
+
+    def _launch(self, slot):
+        main = torch.cuda.current_stream()
+        self.side.wait_stream(main)
+        with torch.cuda.stream(self.side):
+            # the next batch is produced and extracted beside this batch's forward (gate: only once the forward's
+            # clusters are resident, see TrainEngine._launch_pipe); after the last batch it is all padding
+            self.model.gate_wait(self.batches[slot])
+            self._next(slot ^ 1)
+        self._score(slot)
+        main.wait_stream(self.side)
+
+    def step(self):
+        """score the current batch while the next one is extracted.  Returns False once every batch is scored."""
+        run = self.run
+        if run is None or run["P"] == 0 or run["done"] >= run["steps"]:
+            return False
+        slot = run["done"] & 1
+        if self.use_graph and slot in self.graphs:
+            self.graphs[slot].replay()
+        elif self.use_graph and slot in self.eager_done:
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                self._launch(slot)
+            self.graphs[slot] = g
+            g.replay()
+        else:
+            self._launch(slot)
+            self.eager_done.add(slot)
+        run["done"] += 1
+        return run["done"] < run["steps"]
+
+    def finish(self):
+        """wait for the run, check the error word (one host sync) and return (top_items [U, k] int64, top_scores
+        [U, k] fp32) or the scores [P] fp32, on the device"""
+        run = self.run
+        while self.step():
+            pass
+        code = int(self.extractor.err.item())
+        if code:
+            self.extractor.err.zero_()
+            raise RuntimeError("igmc_b200 kernel error %d: %s" % (code, _lib.ERR_NAMES.get(code, "?")))
+        self.run = None
+        if run["kind"] == "recommend":
+            return run["top_i"], run["top_s"]
+        return run["scores"]
+
+    def recommend(self, users, k, items=None, exclude_rated=True):
+        self.start_recommend(users, k, items, exclude_rated)
+        return self.finish()
+
+    def predict_pairs(self, users, items):
+        self.start_pairs(users, items)
+        return self.finish()
+
+    def close(self):
+        torch.cuda.synchronize()
+        self.graphs = {}
+
+
+# ---- public API -----------------------------------------------------------------------------------------------------
+def predict_pairs(model, graph, users, items, *, h=1, sample_ratio=1.0, max_nodes_per_hop=None, batch_size=256,
+                  checkpoints=None, sample_seed=0):
+    """eval-mode scores [P] (fp32, on the model's device) of the pairs (users[i], items[i]); a pair rated in ``graph``
+    is scored on its subgraph without the target edge, as in training.  ``checkpoints``: average of the checkpoints'
+    scores (fp32 sum in checkpoint order / K)."""
+    nu, ni = graph.shape
+    users, items = _host_ids(users, "users", nu), _host_ids(items, "items", ni)
+    if len(users) != len(items):
+        raise ValueError("users and items must have the same length (%d vs %d)" % (len(users), len(items)))
+    if len(users) == 0:
+        return torch.zeros(0, dtype=torch.float32, device=model.flat_params.device)
+    eng = InferenceEngine(model, graph, h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
+    try:
+        return eng.predict_pairs(users, items)
+    finally:
+        eng.close()
+
+
+def recommend(model, graph, users, k, *, items=None, exclude_rated=True, h=1, sample_ratio=1.0,
+              max_nodes_per_hop=None, batch_size=256, checkpoints=None, sample_seed=0):
+    """for every query user the ``k`` best candidate items: (top_items [U, k] int64, top_scores [U, k] fp32), on the
+    model's device.  Candidates: ``items`` (sorted, deduplicated) or every item, minus the user's rated items when
+    ``exclude_rated``.  Order: score descending, then item ascending; a NaN score ranks last; a user with fewer than
+    ``k`` candidates gets item -1 / score -inf in the empty slots."""
+    k = _check_k(k)
+    nu, ni = graph.shape
+    users = _host_ids(users, "users", nu)
+    if items is not None:
+        items = _host_ids(items, "items", ni)
+    if len(users) == 0:
+        dev = model.flat_params.device
+        return (torch.zeros(0, k, dtype=torch.int64, device=dev), torch.zeros(0, k, dtype=torch.float32, device=dev))
+    eng = InferenceEngine(model, graph, h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
+    try:
+        return eng.recommend(users, k, items, exclude_rated)
+    finally:
+        eng.close()

@@ -29,6 +29,14 @@ def _stream_ptr():
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
+def _on_device(a, dtype, dev):
+    """``a`` (host array or tensor) as a contiguous ``dtype`` tensor on ``dev``; a tensor that already is one is
+    returned as is (no copy)."""
+    if not torch.is_tensor(a):
+        a = torch.as_tensor(np.asarray(a), dtype=dtype)
+    return a.to(device=dev, dtype=dtype).contiguous()
+
+
 class DevView(object):
     """Device-visible window of a PINNED host tensor: ``data_ptr()`` is the address the kernels use (under unified
     addressing a cudaHostAlloc'd buffer has the same address on the host and on the device), so they read / write the
@@ -373,14 +381,16 @@ class SubgraphExtractor(object):
         dev = self.device
         keep = []
         if pairs is not None:
-            pu = torch.as_tensor(np.asarray(pairs[0]), dtype=torch.int32).to(dev)
-            pv = torch.as_tensor(np.asarray(pairs[1]), dtype=torch.int32).to(dev)
-            pl = torch.as_tensor(np.asarray(pairs[2]), dtype=torch.int32).to(dev)
+            # (device tensors of the right type are used in place: the inference engine's candidate buffers, read by
+            # a captured CUDA graph; a label array of None extracts with label 0)
+            pu = _on_device(pairs[0], torch.int32, dev)
+            pv = _on_device(pairs[1], torch.int32, dev)
+            pl = None if pairs[2] is None else _on_device(pairs[2], torch.int32, dev)
             B = int(pu.numel())
             pid = None
             if pair_ids is not None:
-                pid = torch.as_tensor(np.asarray(pair_ids), dtype=torch.int64).to(dev)
-            P = _lib.Pairs(None, pu.data_ptr(), pv.data_ptr(), pl.data_ptr(), _lib.ptr(pid))
+                pid = _on_device(pair_ids, torch.int64, dev)
+            P = _lib.Pairs(None, pu.data_ptr(), pv.data_ptr(), _lib.ptr(pl), _lib.ptr(pid))
             keep += [pu, pv, pl, pid]
         else:
             if not isinstance(idx, DevView):     # (a DevView is int64 indices in mapped host memory: used as is)

@@ -405,6 +405,52 @@ int igmc_sortpool_backward(const igmc_sortpool_t* P, const float* params, const 
                            const float* dpred, float* dstate, float grad_scale, float* grad, int* err,
                            void* stream);
 
+/* ---- inference: candidate pairs + streaming per-user top-k (csrc/recommend.cu) ----
+ * Scores pairs that have no rating and ranks them per user - what a trained model is for.  The reference has no such
+ * path (its train_eval.py:182-245 only reduces labelled predictions to an RMSE); a user of it would build a dataset of
+ * every candidate pair and loop over it in Python.  Here the candidates of a batch are produced on the device and
+ * handed to igmc_extract_batch as an igmc_pairs_t with idx = NULL, the eval forward scores them (K checkpoints: K
+ * forwards on the same batch), and the scores are merged into the running per-user top-k lists or scattered to
+ * their pair index.  Sampling stream of every pair: pair_id = u * num_items + v, whatever batch it falls into. */
+#define IGMC_TOPK_MAX 256
+typedef struct {
+  const int32_t* users;     /* recommend: [num_query] query users; NULL selects explicit pairs (pair_u, pair_v) */
+  const int32_t* cand;      /* recommend: [num_cand] ascending, unique candidate items; NULL = every item of G */
+  const int32_t* pair_u;    /* explicit pairs: [num_pairs] user / item of pair i */
+  const int32_t* pair_v;
+  int64_t* user_off;        /* recommend: [num_query+1] exclusive prefix of the per-user candidate counts (the plan) */
+  int64_t* rated_off;       /* recommend with cand and exclude_rated: [num_query+1] offsets into rated_pos (the plan) */
+  int32_t* rated_pos;       /* recommend with cand and exclude_rated: [sum of the query users' degrees] ascending
+                             * positions in cand of each user's rated items (|row(u) & cand| entries per user) */
+  int64_t num_pairs;        /* candidate pairs in all (recommend: user_off[num_query], known once the plan ran) */
+  int32_t num_query, num_cand, exclude_rated, pad_;
+} igmc_candidates_t;
+
+/* Per query user the number of candidate items (cand or every item, minus the user's rated items when exclude_rated:
+ * num_items - deg(u) without a list) and their exclusive prefix user_off; with a list and exclude_rated also rated_off /
+ * rated_pos.  ONE single-CTA launch.  User ids outside G set IGMC_ERR_CANDIDATES (and count 0). */
+int igmc_candidate_plan(const igmc_csr_t* G, const igmc_candidates_t* Cd, int* err, void* stream);
+
+/* The pairs of global candidate positions [*cursor, *cursor + B) (positions ordered by query slot, then item), then
+ * *cursor += B: `cursor` is a device word, so a captured graph replays with no host input.  Writes links_u / links_v /
+ * pair_id [B] for igmc_extract_batch (idx = NULL) and tag [B] = the query slot (recommend) or the pair index
+ * (explicit pairs).  Positions past num_pairs (the tail batch) repeat the last pair with tag -1, so every batch has the
+ * same size and kernel plan.  Candidate rank c of a user maps to list position c + t, t = the number of the user's
+ * rated positions r_q with r_q - q <= c (binary search; without a list the rated positions are the row's col_idx). */
+int igmc_candidate_pairs(const igmc_csr_t* G, const igmc_candidates_t* Cd, int64_t* cursor, int B,
+                         int32_t* links_u, int32_t* links_v, int64_t* pair_id, int64_t* tag, int* err, void* stream);
+
+/* Streaming top-k: s = (preds[0][i] + ... + preds[K-1][i]) / K in fp32, summed in checkpoint order (preds row stride B),
+ * then every contiguous run of equal tag (one query user's candidates in this batch; tag -1 = padding) is merged into
+ * that user's running list top_score / top_item [*, k] (ranked: score descending, then item ascending; NaN after every
+ * number; empty slots = item -1, initialised by the caller, last).  One CTA per run, no float atomics: the result does
+ * not depend on where batch boundaries fall.  1 <= k <= IGMC_TOPK_MAX. */
+int igmc_topk_merge(const float* preds, int K, int B, const int64_t* tag, const int32_t* items, int k,
+                    float* top_score, int64_t* top_item, void* stream);
+
+/* Explicit pairs: scores[tag[i]] = the same fp32 checkpoint mean for every i with tag[i] >= 0. */
+int igmc_score_scatter(const float* preds, int K, int B, const int64_t* tag, float* scores, void* stream);
+
 /* Version / build info: returns the compiled SM arch (90) so the host can refuse stale builds. */
 int igmc_build_info(void);
 
