@@ -170,3 +170,32 @@ __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.lau
     cudaError_t e__ = cudaGetLastError();             \
     if (e__ != cudaSuccess) return (int)e__ + 1000;   \
   } while (0)
+
+// Launches `kern` on `grid` CTAs of `threads` threads in thread-block clusters of `cluster` CTAs along x, with `smem`
+// bytes of dynamic shared memory.  `pdl`: programmatic stream serialization, so the kernel may start under the tail of
+// the previous kernel of the stream (it must pdl_wait() before reading that kernel's results).  Returns 0 or the CUDA
+// error + 1000.
+template <class Kern, class... Args>
+int launch_cluster(Kern kern, int grid, int threads, size_t smem, int cluster, bool pdl, cudaStream_t st,
+                   Args... args) {
+  cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(grid);
+  cfg.blockDim = dim3(threads);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cudaLaunchAttribute at[2];
+  at[0].id = cudaLaunchAttributeClusterDimension;
+  at[0].val.clusterDim.x = cluster;
+  at[0].val.clusterDim.y = 1;
+  at[0].val.clusterDim.z = 1;
+  cfg.attrs = at;
+  cfg.numAttrs = 1;
+  if (pdl) {
+    at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[1].val.programmaticStreamSerializationAllowed = 1;
+    cfg.numAttrs = 2;
+  }
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, kern, args...);
+  return e != cudaSuccess ? (int)e + 1000 : 0;
+}

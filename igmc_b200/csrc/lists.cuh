@@ -1,12 +1,30 @@
-// Edge-list walking shared by the basis-space kernels (csrc/rgcn.cu, csrc/rgcn_l2.cu): the step's edge-dropout
-// draws and a warp-wide walk over one node's (type, neighbour)-sorted list.
+// Device pieces shared by the model kernels: csrc/rgcn.cu (plan 0), csrc/rgcn_l2.cu (L2 plan), csrc/rgcn_rs.cu
+// (relation-space / cluster plans) and csrc/sortpool.cu (DGCNN_RS readout).
+//   - the step's dropout draws: edge dropout (EdgeKeep) and the hidden dropout before lin2 (hidden_scale)
+//   - a warp-wide walk over one node's (type, neighbour)-sorted list and the type-run segment reduce on it
+//   - the readout head: lin1 / ReLU / dropout / save, lin2 / loss, and their backward (d hid, d feat)
+//   - the basis-space weight staging and weight-gradient row store of plan 0 and the L2 plan
+// Each is one computation in one place: a kernel that calls it computes bit-for-bit what the others do.
 #pragma once
 #include "common.cuh"
 #include "../../include/igmc_b200.h"
 
 namespace {
 
+// Activation tiles [n][32] live in shared memory with an XOR swizzle of the column by the row in 4-float groups:
+// a row stays one contiguous 128 B line (lane = channel: conflict-free, float4 groups intact) and a fixed channel
+// over 8 consecutive rows hits 8 different banks (column reads of the dense phases).
+__device__ __forceinline__ int hix(int v, int c) { return (v << 5) + (c ^ ((v & 7) << 2)); }
+__host__ __device__ __forceinline__ int a4(int x) { return (x + 3) & ~3; }
+
+// ---- dropout draws of the step ---------------------------------------------------------------------------------
 constexpr uint32_t DROPPED = 0xFFFFFFFFu;
+
+// keep threshold p * 2^32 of a hash draw (p >= 1 drops everything).  Twin: igmc_b200/models.py::_keep_threshold.
+__device__ __forceinline__ uint32_t keep_thresh(float p) {
+  const double t = (double)p * 4294967296.0;
+  return t >= 4294967295.0 ? 0xFFFFFFFFu : (uint32_t)t;
+}
 
 struct EdgeKeep {
   bool active;
@@ -23,11 +41,26 @@ __device__ __forceinline__ EdgeKeep make_keep(const igmc_dropout_t& D, int train
   K.mask = D.edge_keep;
   K.seed = D.seed_dev ? *D.seed_dev : D.seed;
   K.active = training && (D.adj_dropout > 0.0f || D.edge_keep != nullptr);
-  double t = (double)D.adj_dropout * 4294967296.0;
-  K.thresh = t >= 4294967295.0 ? 0xFFFFFFFFu : (uint32_t)t;
+  K.thresh = keep_thresh(D.adj_dropout);
   return K;
 }
 
+// F.dropout before lin2 (models.py:212): factor of unit o of graph g, 0 or 1/(1-p) in training, else 1.  The draw is
+// an edge_keep draw of index g*128 + o on the step seed ^ 0x5bd1e995a5a5a5a5 (twin: models.py::hidden_keep_reference);
+// an injected D.hidden_keep mask stands for p = 0.5.
+__device__ __forceinline__ float hidden_scale(const igmc_dropout_t& D, uint64_t seed, int training, int g, int o) {
+  float scale = 1.f;
+  if (training && (D.hidden_dropout > 0.f || D.hidden_keep)) {
+    bool keep;
+    if (D.hidden_keep) keep = D.hidden_keep[(size_t)g * IGMC_LIN1_OUT + o] != 0;
+    else keep = edge_keep(seed ^ 0x5bd1e995a5a5a5a5ull, (uint32_t)(g * IGMC_LIN1_OUT + o), keep_thresh(D.hidden_dropout));
+    const float p = D.hidden_keep ? 0.5f : D.hidden_dropout;
+    scale = keep ? 1.f / (1.f - p) : 0.f;
+  }
+  return scale;
+}
+
+// ---- list walking ------------------------------------------------------------------------------------------------
 // Walks list [p0,p1) of one node with the whole warp; body(nbr, type) is called warp-uniformly for
 // every kept entry, in list order.  `mirror`: the entry describes edge nbr->x but the caller wants
 // the reverse edge x->nbr of a symmetric batch, whose id is the mirror image inside the graph.
@@ -76,6 +109,191 @@ __device__ __forceinline__ int rel_inv_deg_row(const uint32_t* __restrict__ adj,
   });
   if (cur >= 0 && lane == 0) out[cur] = 1.f / (float)cnt;
   return kept;
+}
+
+// Type-run segment reduce over kept list entries: acc[b] = sum_runs att[type][b] * sum_run feat(nbr, type);
+// MEAN: every run divided by its length (the forward's mean per relation, igmc_saved_t.rel_inv_deg)
+template <int NB, bool MEAN = false, class Feat>
+__device__ __forceinline__ int gather_runs(const uint32_t* __restrict__ adj, const int32_t* __restrict__ eid, int p0,
+                                           int p1, const EdgeKeep& K, bool mirror, int eb, int m_half, int lane,
+                                           Feat&& feat, const float* __restrict__ att_s, float (&acc)[NB]) {
+  float run = 0.f;
+  int cur = -1, cnt = 0;
+#pragma unroll
+  for (int b = 0; b < NB; ++b) acc[b] = 0.f;
+  auto flush = [&]() {
+    float rv = run;
+    if (MEAN) rv *= 1.f / (float)cnt;
+#pragma unroll
+    for (int b = 0; b < NB; ++b) acc[b] = fmaf(att_s[cur * NB + b], rv, acc[b]);
+  };
+  const int kept = list_foreach(adj, eid, p0, p1, K, mirror, eb, m_half, lane, [&](int nbr, int ty) {
+    if (ty != cur) {
+      if (cur >= 0) flush();
+      run = 0.f;
+      cur = ty;
+      cnt = 0;
+    }
+    run += feat(nbr, ty);
+    ++cnt;
+  });
+  if (cur >= 0) flush();
+  return kept;
+}
+
+// ---- readout head (models.py:205-215 IGMC, 160-165 DGCNN_RS) ---------------------------------------------------
+// `M` is the model or readout descriptor (igmc_model_t / igmc_sortpool_t: the lin1 / lin2 offsets into params), `S`
+// the saved tensors of the step (igmc_saved_t / igmc_sortpool_saved_t: hid, hid_gscale).
+// relu(lin1 pre-activation) of unit o of graph g, hidden dropout, and what the backward needs: hid = h * scale (to
+// shared hid_s and S.hid), S.hid_gscale = d hid / d pre-activation
+template <class Saved>
+__device__ __forceinline__ void readout_hidden(float pre, int g, int o, const igmc_dropout_t& D, uint64_t seed,
+                                               int training, float* hid_s, const Saved& S) {
+  const float h = fmaxf(pre, 0.f);
+  const float scale = hidden_scale(D, seed, training, g, o);
+  hid_s[o] = h * scale;
+  S.hid[(size_t)g * IGMC_LIN1_OUT + o] = h * scale;
+  S.hid_gscale[(size_t)g * IGMC_LIN1_OUT + o] = h > 0.f ? scale : 0.f;
+}
+
+// lin1 of the readout row feat_s[F] (shared memory) of graph g, then readout_hidden.  Eight outputs per warp and pass
+// (16 warps x 8 = all 128 in one pass of L2 latency); each output is one per-lane fmaf chain over i = lane, lane + 32,
+// .. and one warp_sum_f.
+template <class Model, class Saved>
+__device__ __forceinline__ void readout_lin1(const Model& M, const float* params, const float* feat_s, int F, int g,
+                                             const igmc_dropout_t& D, uint64_t seed, int training, float* hid_s,
+                                             const Saved& S, int warp, int nwarps, int lane) {
+  constexpr int OW = 8;
+  const float* W1 = params + M.off_lin1_w;
+  for (int ob = warp * OW; ob < IGMC_LIN1_OUT; ob += nwarps * OW) {
+    float s4[OW];
+#pragma unroll
+    for (int u = 0; u < OW; ++u) s4[u] = 0.f;
+    const float bias_o = lane < OW ? __ldg(params + M.off_lin1_b + ob + lane) : 0.f;   // independent of the dot products
+#pragma unroll 4   // 32 independent L2 loads in flight per lane (the loop is latency bound)
+    for (int i = lane; i < F; i += 32) {
+      const float f = feat_s[i];
+#pragma unroll
+      for (int u = 0; u < OW; ++u) s4[u] = fmaf(__ldg(W1 + (size_t)(ob + u) * F + i), f, s4[u]);
+    }
+#pragma unroll
+    for (int u = 0; u < OW; ++u) s4[u] = warp_sum_f(s4[u]);
+#pragma unroll
+    for (int u = 0; u < OW; ++u)
+      if (lane == u) readout_hidden(s4[u] + bias_o, g, ob + u, D, seed, training, hid_s, S);
+  }
+}
+
+// lin2 and the loss of graph g on one warp: pred = (lin2 . hid + b) * multiply_by; with targets y also the squared
+// error and dpred = d (loss_scale * mse) / d lin2 output
+template <class Model>
+__device__ __forceinline__ void readout_lin2(const Model& M, const float* params, const float* hid_s,
+                                             float multiply_by, int g, const float* y, float loss_scale, float* pred,
+                                             float* sqerr, float* dpred, int lane) {
+  float s = 0.f;
+  const float b2 = __ldg(params + M.off_lin2_b), yg = y ? __ldg(y + g) : 0.f;   // issued with the weight loads
+  for (int o = lane; o < IGMC_LIN1_OUT; o += 32) s = fmaf(params[M.off_lin2_w + o], hid_s[o], s);
+  s = warp_sum_f(s);
+  if (lane == 0) {
+    const float out = (s + b2) * multiply_by;
+    pred[g] = out;
+    if (y) {
+      const float diff = out - yg;
+      if (sqerr) sqerr[g] = diff * diff;
+      if (dpred) dpred[g] = 2.f * diff * loss_scale * multiply_by;
+    }
+  }
+}
+
+// d hid = dpred[g] * lin2.weight * S.hid_gscale[g] (lin2, dropout and ReLU backward) -> dhid_s [128] and, if
+// `store`, row g of dhid_out
+template <class Model, class Saved>
+__device__ __forceinline__ void readout_dhid(const Model& M, const float* params, const Saved& S, const float* dpred,
+                                             int g, float* dhid_s, float* dhid_out, bool store, int tid, int NT) {
+  const float dp = dpred[g];
+  for (int o = tid; o < IGMC_LIN1_OUT; o += NT) {
+    const float d = dp * params[M.off_lin2_w + o] * S.hid_gscale[(size_t)g * IGMC_LIN1_OUT + o];
+    dhid_s[o] = d;
+    if (store) dhid_out[(size_t)g * IGMC_LIN1_OUT + o] = d;
+  }
+}
+
+// One partial of d feat[i] = sum_o lin1.weight[o][i] d hid[o]: slot t = part * F + i (nothing for t >= parts * F)
+// sums every parts-th o from `part` on, in order, into out[t].  With parts = 1 and out = d feat this is the whole
+// sum of column i; with more slices the caller adds the parts of a column in slice order after a barrier.
+template <class Model>
+__device__ __forceinline__ void readout_dfeat_part(const Model& M, const float* params, const float* dhid_s, int F,
+                                                   int parts, int t, float* out) {
+  const float* W1 = params + M.off_lin1_w;
+  const int i = t % F, part = t / F;
+  if (part < parts) {
+    float s = 0.f;
+#pragma unroll 32   // independent L2 loads in flight (latency bound)
+    for (int o = part; o < IGMC_LIN1_OUT; o += parts) s = fmaf(__ldg(W1 + (size_t)o * F + i), dhid_s[o], s);
+    out[part * F + i] = s;
+  }
+}
+
+// ---- basis-space weights of plan 0 and the L2 plan --------------------------------------------------------------
+// layer l's [basis ; root] rows -> Wc [(NB+1)*in][32] (rows NB*in.. are root), att -> att_s, bias -> bias_s
+template <int NB, int NT>
+__device__ __forceinline__ void stage_layer(const igmc_model_t& M, const float* __restrict__ params, int l, int in,
+                                            float* Wc, float* att_s, float* bias_s, int tid) {
+  constexpr int HID = IGMC_HIDDEN;
+  const float* bs = params + M.off_basis[l];
+  const float* rt = params + M.off_root[l];
+  const int K1 = NB * in;
+  for (int idx = tid; idx < K1 * HID; idx += NT) Wc[idx] = bs[idx];
+  for (int idx = tid; idx < in * HID; idx += NT) Wc[K1 * HID + idx] = rt[idx];
+  for (int idx = tid; idx < M.num_relations * NB; idx += NT) att_s[idx] = params[M.off_att[l] + idx];
+  if (tid < HID) bias_s[tid] = params[M.off_bias[l] + tid];
+}
+
+// the transposed [basis ; root] of a 32-wide layer l for the data gradient: basis[b][k][j] -> Wt[b*32+j][k],
+// root[k][j] -> Wt[NB*32+j][k], row stride WS
+template <int NB, int NT, int WS>
+__device__ __forceinline__ void stage_layer_t(const igmc_model_t& M, const float* __restrict__ params, int l,
+                                              float* Wt, int tid) {
+  constexpr int HID = IGMC_HIDDEN;
+  const float* bs = params + M.off_basis[l];
+  const float* rt = params + M.off_root[l];
+  for (int idx = tid; idx < NB * HID * HID; idx += NT) {
+    const int j = idx & 31, k = (idx >> 5) & 31, b = idx >> 10;
+    Wt[(b * HID + j) * WS + k] = bs[idx];
+  }
+  for (int idx = tid; idx < HID * HID; idx += NT) {
+    const int j = idx & 31, k = idx >> 5;
+    Wt[(NB * HID + j) * WS + k] = rt[idx];
+  }
+}
+
+// basis of layer l (input width in) for the d att pass: basis[b][k][j] -> W2[j][b*32+k], row stride NB*32+4
+template <int NB, int NT>
+__device__ __forceinline__ void stage_basis_w2(const igmc_model_t& M, const float* __restrict__ params, int l, int in,
+                                               float* W2, int tid) {
+  constexpr int HID = IGMC_HIDDEN, ZS = NB * HID + 4;
+  const float* bs = params + M.off_basis[l];
+  for (int idx = tid; idx < NB * in * HID; idx += NT) {
+    const int j = idx & 31, k = (idx >> 5) % in, b = (idx >> 5) / in;
+    W2[j * ZS + b * HID + k] = bs[idx];
+  }
+}
+
+// weight-gradient rows of layer l in parameter layout: thread (kg, c0) holds d basis[i][kg][c0..c0+3] (acc[i], i < NB),
+// d root[kg][c0..] (acc[NB]) and, for kg = 0, d bias[c0..] (accb)
+template <int NB>
+__device__ __forceinline__ void store_wgrad_rows(const igmc_model_t& M, int l, int in, int kg, int c0,
+                                                 const float (&acc)[NB + 1][4], const float (&accb)[4],
+                                                 float* __restrict__ gp) {
+  constexpr int HID = IGMC_HIDDEN;
+  if (kg >= in) return;
+#pragma unroll
+  for (int i = 0; i < NB; ++i)
+    *reinterpret_cast<float4*>(gp + M.off_basis[l] + (i * in + kg) * HID + c0) =
+        make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
+  *reinterpret_cast<float4*>(gp + M.off_root[l] + kg * HID + c0) =
+      make_float4(acc[NB][0], acc[NB][1], acc[NB][2], acc[NB][3]);
+  if (kg == 0) *reinterpret_cast<float4*>(gp + M.off_bias[l] + c0) = make_float4(accb[0], accb[1], accb[2], accb[3]);
 }
 
 }  // namespace

@@ -24,76 +24,6 @@ constexpr int WS = 36;   // row stride of transposed weights in backward
 constexpr int HID = IGMC_HIDDEN;
 constexpr int L1O = IGMC_LIN1_OUT;
 
-// Activation tiles [n][32] live in shared memory with an XOR swizzle of the column by the row:
-// a row stays one contiguous 128 B line (lane = channel: conflict-free, float4 groups intact) and
-// a fixed channel over 8 consecutive rows hits 8 different banks (column reads of the dense phases).
-__device__ __forceinline__ int hix(int v, int c) { return (v << 5) + (c ^ ((v & 7) << 2)); }
-
-// Type-run segment reduce: acc[b] = sum over kept entries of att[type][b] * feat[nbr][lane] * scale[nbr]
-template <int NB, bool SCALE>
-__device__ __forceinline__ int gather_runs(const uint32_t* __restrict__ adj, const int32_t* __restrict__ eid,
-                                           int p0, int p1, const EdgeKeep& K, bool mirror, int eb, int m_half,
-                                           int lane, const float* __restrict__ feat, const float* __restrict__ scale,
-                                           const float* __restrict__ att_s, float (&acc)[NB]) {
-  float run = 0.f;
-  int cur = -1;
-#pragma unroll
-  for (int b = 0; b < NB; ++b) acc[b] = 0.f;
-  const int kept = list_foreach(adj, eid, p0, p1, K, mirror, eb, m_half, lane, [&](int nbr, int ty) {
-    if (ty != cur) {
-      if (cur >= 0) {
-#pragma unroll
-        for (int b = 0; b < NB; ++b) acc[b] = fmaf(att_s[cur * NB + b], run, acc[b]);
-      }
-      run = 0.f;
-      cur = ty;
-    }
-    float v = feat[hix(nbr, lane)];
-    if (SCALE) v *= scale[nbr];
-    run += v;
-  });
-  if (cur >= 0) {
-#pragma unroll
-    for (int b = 0; b < NB; ++b) acc[b] = fmaf(att_s[cur * NB + b], run, acc[b]);
-  }
-  return kept;
-}
-
-// The same for the mean per relation (igmc_saved_t.rel_inv_deg): with SCALE an entry is weighed by
-// rinv[nbr*R + type] (1/|N_r| of the destination nbr, backward), without SCALE every run is divided by its length
-// (forward).  Kept apart from gather_runs so that the default kernels compile exactly as before.
-template <int NB, bool SCALE>
-__device__ __forceinline__ int gather_runs_rel(const uint32_t* __restrict__ adj, const int32_t* __restrict__ eid,
-                                               int p0, int p1, const EdgeKeep& K, bool mirror, int eb, int m_half,
-                                               int lane, const float* __restrict__ feat, const float* __restrict__ rinv,
-                                               int R, const float* __restrict__ att_s, float (&acc)[NB]) {
-  float run = 0.f;
-  int cur = -1, cnt = 0;
-#pragma unroll
-  for (int b = 0; b < NB; ++b) acc[b] = 0.f;
-  auto flush = [&]() {
-    const float rv = SCALE ? run : run * (1.f / (float)cnt);
-#pragma unroll
-    for (int b = 0; b < NB; ++b) acc[b] = fmaf(att_s[cur * NB + b], rv, acc[b]);
-  };
-  const int kept = list_foreach(adj, eid, p0, p1, K, mirror, eb, m_half, lane, [&](int nbr, int ty) {
-    if (ty != cur) {
-      if (cur >= 0) flush();
-      run = 0.f;
-      cur = ty;
-      cnt = 0;
-    }
-    float v = feat[hix(nbr, lane)];
-    if (SCALE) v *= __ldg(rinv + nbr * R + ty);
-    run += v;
-    ++cnt;
-  });
-  if (cur >= 0) flush();
-  return kept;
-}
-
-__device__ __forceinline__ size_t align4(size_t x) { return (x + 3) & ~(size_t)3; }
-
 // ------------------------------------------------------------------------------------------------
 // forward
 // ------------------------------------------------------------------------------------------------
@@ -111,10 +41,10 @@ k_forward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __res
   float* Zs = HB + (size_t)n_cap * HID;
   float* Wc = Zs + TM * ZS;
   float* att_s = Wc + (NB + 1) * HID * HID;
-  float* bias_s = att_s + align4((size_t)R * NB);
+  float* bias_s = att_s + a4(R * NB);
   float* invdeg = bias_s + HID;
-  float* feat_s = invdeg + align4(n_cap);
-  float* hid_s = feat_s + align4(F);
+  float* feat_s = invdeg + a4(n_cap);
+  float* hid_s = feat_s + a4(F);
   __shared__ int s_t[2];
 
   const int g = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -161,27 +91,15 @@ k_forward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __res
   for (int l = 0; l < L; ++l) {
     const int in = l == 0 ? in0 : HID;
     const int K1 = NB * in;
-    // [basis ; root] rows, att, bias -> shared
-    {
-      const float* bs = params + M.off_basis[l];
-      const float* rt = params + M.off_root[l];
-      for (int idx = tid; idx < K1 * HID; idx += MP_THREADS) Wc[idx] = bs[idx];
-      for (int idx = tid; idx < in * HID; idx += MP_THREADS) Wc[K1 * HID + idx] = rt[idx];
-      for (int idx = tid; idx < R * NB; idx += MP_THREADS) att_s[idx] = params[M.off_att[l] + idx];
-      if (tid < HID) bias_s[tid] = params[M.off_bias[l] + tid];
-    }
+    stage_layer<NB, MP_THREADS>(M, params, l, in, Wc, att_s, bias_s, tid);   // [basis ; root] rows, att, bias
     __syncthreads();
     for (int t0 = 0; t0 < n; t0 += TM) {
       const int tend = min(t0 + TM, n);
       // ---- phase G: basis-space aggregate of the tile's nodes (warp per destination node) ----
       for (int v = t0 + warp; v < tend; v += MP_WARPS) {
         float z[NB];
-        if (PR)
-          gather_runs_rel<NB, false>(A.in_adj, A.in_eid, A.in_ptr[nb + v], A.in_ptr[nb + v + 1], K, false, eb, m_half,
-                                     lane, HA, nullptr, R, att_s, z);
-        else
-          gather_runs<NB, false>(A.in_adj, A.in_eid, A.in_ptr[nb + v], A.in_ptr[nb + v + 1], K, false, eb, m_half,
-                                 lane, HA, nullptr, att_s, z);
+        gather_runs<NB, PR>(A.in_adj, A.in_eid, A.in_ptr[nb + v], A.in_ptr[nb + v + 1], K, false, eb, m_half, lane,
+                            [&](int u, int) { return HA[hix(u, lane)]; }, att_s, z);
         const float id = invdeg[v];
 #pragma unroll
         for (int b = 0; b < NB; ++b) {
@@ -240,45 +158,11 @@ k_forward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __res
   }
   if (tid == 0) { S.target[2 * g] = nb + tu; S.target[2 * g + 1] = nb + ti; }
   __syncthreads();
-  const float* W1 = params + M.off_lin1_w;
-  for (int o = warp; o < L1O; o += MP_WARPS) {
-    float s = 0.f;
-    for (int i = lane; i < F; i += 32) s = fmaf(W1[(size_t)o * F + i], feat_s[i], s);
-    s = warp_sum_f(s);
-    if (lane == 0) {
-      float h = fmaxf(s + params[M.off_lin1_b + o], 0.f);                 // relu(lin1) models.py:211
-      float scale = 1.f;
-      if (training && (D.hidden_dropout > 0.f || D.hidden_keep)) {        // F.dropout models.py:212
-        bool keep;
-        if (D.hidden_keep) keep = D.hidden_keep[(size_t)g * L1O + o] != 0;
-        else {
-          double t = (double)D.hidden_dropout * 4294967296.0;
-          keep = edge_keep(K.seed ^ 0x5bd1e995a5a5a5a5ull, (uint32_t)(g * L1O + o),
-                           t >= 4294967295.0 ? 0xFFFFFFFFu : (uint32_t)t);
-        }
-        const float p = D.hidden_keep ? 0.5f : D.hidden_dropout;
-        scale = keep ? 1.f / (1.f - p) : 0.f;
-      }
-      hid_s[o] = h * scale;
-      S.hid[(size_t)g * L1O + o] = h * scale;
-      S.hid_gscale[(size_t)g * L1O + o] = h > 0.f ? scale : 0.f;
-    }
-  }
+  readout_lin1(M, params, feat_s, F, g, D, K.seed, training, hid_s, S, warp, MP_WARPS, lane);
   __syncthreads();
-  if (warp == 0) {
-    float s = 0.f;
-    for (int o = lane; o < L1O; o += 32) s = fmaf(params[M.off_lin2_w + o], hid_s[o], s);
-    s = warp_sum_f(s);
-    if (lane == 0) {
-      const float out = (s + params[M.off_lin2_b]) * M.multiply_by;       // models.py:213-215
-      S.pred[g] = out;
-      if (y) {
-        const float diff = out - y[g];
-        if (sqerr) sqerr[g] = diff * diff;
-        if (dpred) dpred[g] = 2.f * diff * loss_scale * M.multiply_by;   // d mse / d lin2-output
-      }
-    }
-  }
+  if (warp == 0)
+    readout_lin2(M, params, hid_s, M.multiply_by, g, y, loss_scale, S.pred, sqerr,
+                 dpred, lane);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -299,9 +183,9 @@ k_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __re
   float* Zs = HP + (size_t)n_cap * HID;           // tile scratch [TM][ZS]
   float* Wt = Zs + TM * ZS;                       // transposed weights, (NB+1)*32 rows x WS  |  W2 [32][ZS]
   float* att_s = Wt + (NB + 1) * HID * WS;
-  float* invdeg = att_s + align4((size_t)R * NB);
-  float* dfeat = invdeg + align4(n_cap);
-  float* dhid_s = dfeat + align4(F);
+  float* invdeg = att_s + a4(R * NB);
+  float* dfeat = invdeg + a4(n_cap);
+  float* dhid_s = dfeat + a4(F);
   float* datt_w = dhid_s + L1O;                   // [MP_WARPS][R*NB]
 
   const int g = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -322,24 +206,12 @@ k_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __re
   float* gp = gpart + (size_t)g * M.conv_param_count;
 
   // ---- readout backward: d hid, d feat (models.py:211-213) ----
-  if (!ext) {
-    const float dp = dpred[g];
-    for (int o = tid; o < L1O; o += MP_THREADS) {
-      const float d = dp * params[M.off_lin2_w + o] * S.hid_gscale[(size_t)g * L1O + o];
-      dhid_s[o] = d;
-      dhid_out[(size_t)g * L1O + o] = d;
-    }
-  }
+  if (!ext)
+    readout_dhid(M, params, S, dpred, g, dhid_s, dhid_out, true, tid, MP_THREADS);
   for (int v = tid; v < n; v += MP_THREADS) invdeg[v] = S.inv_deg[nb + v];
   __syncthreads();
-  if (!ext) {
-    const float* W1 = params + M.off_lin1_w;
-    for (int i = tid; i < F; i += MP_THREADS) {
-      float s = 0.f;
-      for (int o = 0; o < L1O; ++o) s = fmaf(W1[(size_t)o * F + i], dhid_s[o], s);
-      dfeat[i] = s;
-    }
-  }
+  if (!ext)
+    for (int i = tid; i < F; i += MP_THREADS) readout_dfeat_part(M, params, dhid_s, F, 1, i, dfeat);
   __syncthreads();
   // d h_L : only the two target rows receive gradient from the IGMC readout
   for (int idx = tid; idx < n * HID; idx += MP_THREADS) {
@@ -377,27 +249,17 @@ k_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __re
 
     // (1) data gradient: d h_{l-1} += [G | dpre] . [basis ; root]^T , G = out-list aggregate of dpre/deg
     if (l > 0) {
-      const float* bs = params + M.off_basis[l];
-      const float* rt = params + M.off_root[l];
-      for (int idx = tid; idx < NB * HID * HID; idx += MP_THREADS) {   // basis[b][k][j] -> Wt[(b*32+j)][k]
-        const int j = idx & 31, k = (idx >> 5) & 31, b = idx >> 10;
-        Wt[(b * HID + j) * WS + k] = bs[idx];
-      }
-      for (int idx = tid; idx < HID * HID; idx += MP_THREADS) {        // root[k][j] -> Wt[(NB*32+j)][k]
-        const int j = idx & 31, k = idx >> 5;
-        Wt[(NB * HID + j) * WS + k] = rt[idx];
-      }
+      stage_layer_t<NB, MP_THREADS, WS>(M, params, l, Wt, tid);
       __syncthreads();
+      const float* rinv = PR ? S.rel_inv_deg + (size_t)nb * R : nullptr;   // 1/|N_r(d)| of the destination d
       for (int t0 = 0; t0 < n; t0 += TM) {
         const int tend = min(t0 + TM, n);
         for (int u = t0 + warp; u < tend; u += MP_WARPS) {
           float gz[NB];
-          if (PR)
-            gather_runs_rel<NB, true>(oadj, oeid, optr[nb + u], optr[nb + u + 1], K, sym, eb, m_half, lane, GA,
-                                      S.rel_inv_deg + (size_t)nb * R, R, att_s, gz);
-          else
-            gather_runs<NB, true>(oadj, oeid, optr[nb + u], optr[nb + u + 1], K, sym, eb, m_half, lane, GA, invdeg,
-                                  att_s, gz);
+          gather_runs<NB>(oadj, oeid, optr[nb + u], optr[nb + u + 1], K, sym, eb, m_half, lane,
+                          [&](int d, int ty) {
+                            return GA[hix(d, lane)] * (PR ? __ldg(rinv + d * R + ty) : invdeg[d]);
+                          }, att_s, gz);
 #pragma unroll
           for (int b = 0; b < NB; ++b) Zs[(u - t0) * ZS + b * HID + lane] = gz[b];
         }
@@ -467,26 +329,13 @@ k_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __re
         }
         __syncthreads();
       }
-      if (kg < in) {
-#pragma unroll
-        for (int i = 0; i < NB; ++i)
-          *reinterpret_cast<float4*>(gp + M.off_basis[l] + (i * in + kg) * HID + c0) =
-              make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
-        *reinterpret_cast<float4*>(gp + M.off_root[l] + kg * HID + c0) =
-            make_float4(acc[NB][0], acc[NB][1], acc[NB][2], acc[NB][3]);
-        if (kg == 0)
-          *reinterpret_cast<float4*>(gp + M.off_bias[l] + c0) = make_float4(accb[0], accb[1], accb[2], accb[3]);
-      }
+      store_wgrad_rows<NB>(M, l, in, kg, c0, acc, accb, gp);
     }
 
     // (3) d att[r,b] = sum_v sum_{in-runs of type r} < sum_run h_{l-1}[src,:] , dZ'[v,b,:] >,
     //     dZ'[v,b,k] = 1/deg(v) * sum_j dpre[v,j] basis[b][k][j]
     {
-      const float* bs = params + M.off_basis[l];
-      for (int idx = tid; idx < NB * in * HID; idx += MP_THREADS) {   // basis[b][k][j] -> W2[j][b*32+k]
-        const int j = idx & 31, k = (idx >> 5) % in, b = (idx >> 5) / in;
-        Wt[j * ZS + b * HID + k] = bs[idx];
-      }
+      stage_basis_w2<NB, MP_THREADS>(M, params, l, in, Wt, tid);
       __syncthreads();
       for (int t0 = 0; t0 < n; t0 += TM) {
         const int tend = min(t0 + TM, n);

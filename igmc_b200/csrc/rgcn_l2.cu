@@ -33,38 +33,6 @@ __device__ __forceinline__ void own_range(int n, int csize, int rank, int& v0, i
   v1 = min(n, v0 + per);
 }
 
-__device__ __forceinline__ size_t align4(size_t x) { return (x + 3) & ~(size_t)3; }
-
-// Type-run segment reduce over kept list entries: acc[b] = sum_runs att[type][b] * sum_run feat(nbr, type);
-// MEAN: every run divided by its length (the forward's mean per relation, igmc_saved_t.rel_inv_deg)
-template <int NB, bool MEAN = false, class Feat>
-__device__ __forceinline__ int gather_runs(const uint32_t* __restrict__ adj, const int32_t* __restrict__ eid, int p0,
-                                           int p1, const EdgeKeep& K, bool mirror, int eb, int m_half, int lane,
-                                           Feat&& feat, const float* __restrict__ att_s, float (&acc)[NB]) {
-  float run = 0.f;
-  int cur = -1, cnt = 0;
-#pragma unroll
-  for (int b = 0; b < NB; ++b) acc[b] = 0.f;
-  auto flush = [&]() {
-    float rv = run;
-    if (MEAN) rv *= 1.f / (float)cnt;
-#pragma unroll
-    for (int b = 0; b < NB; ++b) acc[b] = fmaf(att_s[cur * NB + b], rv, acc[b]);
-  };
-  const int kept = list_foreach(adj, eid, p0, p1, K, mirror, eb, m_half, lane, [&](int nbr, int ty) {
-    if (ty != cur) {
-      if (cur >= 0) flush();
-      run = 0.f;
-      cur = ty;
-      cnt = 0;
-    }
-    run += feat(nbr, ty);
-    ++cnt;
-  });
-  if (cur >= 0) flush();
-  return kept;
-}
-
 // h_{l-1}[v][c]: one-hot of the node label for l = 0, else layer l-1 of concat_states (possibly another CTA's row)
 struct PrevLayer {
   const uint8_t* label;
@@ -91,9 +59,9 @@ k_l2_forward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __
   float* Zs = smem;
   float* Wc = Zs + TM * ZS;                // [basis ; root] rows
   float* att_s = Wc + (NB + 1) * HID * HID;
-  float* bias_s = att_s + align4((size_t)R * NB);
+  float* bias_s = att_s + a4(R * NB);
   float* feat_s = bias_s + HID;
-  float* hid_s = feat_s + align4(F);
+  float* hid_s = feat_s + a4(F);
   __shared__ int s_t[2];
 
   const int g = blockIdx.x / csize, rank = blockIdx.x % csize;
@@ -128,14 +96,7 @@ k_l2_forward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __
     const int in = l == 0 ? in0 : HID;
     const int K1 = NB * in;
     const PrevLayer hp{node_label + nb, S.states + (size_t)nb * CW, l, in0, CW};
-    {
-      const float* bs = params + M.off_basis[l];
-      const float* rt = params + M.off_root[l];
-      for (int idx = tid; idx < K1 * HID; idx += THREADS) Wc[idx] = bs[idx];
-      for (int idx = tid; idx < in * HID; idx += THREADS) Wc[K1 * HID + idx] = rt[idx];
-      for (int idx = tid; idx < R * NB; idx += THREADS) att_s[idx] = params[M.off_att[l] + idx];
-      if (tid < HID) bias_s[tid] = params[M.off_bias[l] + tid];
-    }
+    stage_layer<NB, THREADS>(M, params, l, in, Wc, att_s, bias_s, tid);
     __syncthreads();
     for (int t0 = v0; t0 < v1; t0 += TM) {
       const int tend = min(t0 + TM, v1);
@@ -196,45 +157,11 @@ k_l2_forward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __
   }
   if (tid == 0) { S.target[2 * g] = nb + tu; S.target[2 * g + 1] = nb + ti; }
   __syncthreads();
-  const float* W1 = params + M.off_lin1_w;
-  for (int o = warp; o < L1O; o += WARPS) {
-    float s = 0.f;
-    for (int i = lane; i < F; i += 32) s = fmaf(W1[(size_t)o * F + i], feat_s[i], s);
-    s = warp_sum_f(s);
-    if (lane == 0) {
-      float h = fmaxf(s + params[M.off_lin1_b + o], 0.f);                 // relu(lin1) models.py:211
-      float scale = 1.f;
-      if (training && (D.hidden_dropout > 0.f || D.hidden_keep)) {        // F.dropout models.py:212
-        bool keep;
-        if (D.hidden_keep) keep = D.hidden_keep[(size_t)g * L1O + o] != 0;
-        else {
-          double t = (double)D.hidden_dropout * 4294967296.0;
-          keep = edge_keep(K.seed ^ 0x5bd1e995a5a5a5a5ull, (uint32_t)(g * L1O + o),
-                           t >= 4294967295.0 ? 0xFFFFFFFFu : (uint32_t)t);
-        }
-        const float p = D.hidden_keep ? 0.5f : D.hidden_dropout;
-        scale = keep ? 1.f / (1.f - p) : 0.f;
-      }
-      hid_s[o] = h * scale;
-      S.hid[(size_t)g * L1O + o] = h * scale;
-      S.hid_gscale[(size_t)g * L1O + o] = h > 0.f ? scale : 0.f;
-    }
-  }
+  readout_lin1(M, params, feat_s, F, g, D, K.seed, training, hid_s, S, warp, WARPS, lane);
   __syncthreads();
-  if (warp == 0) {
-    float s = 0.f;
-    for (int o = lane; o < L1O; o += 32) s = fmaf(params[M.off_lin2_w + o], hid_s[o], s);
-    s = warp_sum_f(s);
-    if (lane == 0) {
-      const float out = (s + params[M.off_lin2_b]) * M.multiply_by;       // models.py:213-215
-      S.pred[g] = out;
-      if (y) {
-        const float diff = out - y[g];
-        if (sqerr) sqerr[g] = diff * diff;
-        if (dpred) dpred[g] = 2.f * diff * loss_scale * M.multiply_by;   // d mse / d lin2-output
-      }
-    }
-  }
+  if (warp == 0)
+    readout_lin2(M, params, hid_s, M.multiply_by, g, y, loss_scale, S.pred, sqerr,
+                 dpred, lane);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -254,8 +181,8 @@ k_l2_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* _
   float* Zs = smem;
   float* Wt = Zs + TM * ZB;                // transposed [basis ; root] | basis as W2[j][b*32+k]
   float* att_s = Wt + WT;
-  float* dfeat = att_s + align4((size_t)R * NB);
-  float* dhid_s = dfeat + align4(F);
+  float* dfeat = att_s + a4(R * NB);
+  float* dhid_s = dfeat + a4(F);
   double* datt_w = reinterpret_cast<double*>(dhid_s + L1O);   // [WARPS][R*NB], fp64: the sums over a large
                                                                  // subgraph cancel to a small fraction of their terms
 
@@ -284,19 +211,9 @@ k_l2_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* _
 
   // ---- readout backward: d hid, d feat (models.py:211-213) ----
   if (!ext) {
-    const float dp = dpred[g];
-    for (int o = tid; o < L1O; o += THREADS) {
-      const float d = dp * params[M.off_lin2_w + o] * S.hid_gscale[(size_t)g * L1O + o];
-      dhid_s[o] = d;
-      if (rank == 0) dhid_out[(size_t)g * L1O + o] = d;
-    }
+    readout_dhid(M, params, S, dpred, g, dhid_s, dhid_out, rank == 0, tid, THREADS);
     __syncthreads();
-    const float* W1 = params + M.off_lin1_w;
-    for (int i = tid; i < F; i += THREADS) {
-      float s = 0.f;
-      for (int o = 0; o < L1O; ++o) s = fmaf(W1[(size_t)o * F + i], dhid_s[o], s);
-      dfeat[i] = s;
-    }
+    for (int i = tid; i < F; i += THREADS) readout_dfeat_part(M, params, dhid_s, F, 1, i, dfeat);
   }
   __syncthreads();
   // d loss / d h_l[v][c] from the readout: S.dstate (external readout) and the two target rows
@@ -328,16 +245,7 @@ k_l2_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* _
 
     // (1) data gradient: d h_{l-1} = readout rows + [G | dpre] . [basis ; root]^T, G = out-list aggregate of dpre/deg
     if (l > 0) {
-      const float* bs = params + M.off_basis[l];
-      const float* rt = params + M.off_root[l];
-      for (int idx = tid; idx < NB * HID * HID; idx += THREADS) {   // basis[b][k][j] -> Wt[(b*32+j)][k]
-        const int j = idx & 31, k = (idx >> 5) & 31, b = idx >> 10;
-        Wt[(b * HID + j) * WS + k] = bs[idx];
-      }
-      for (int idx = tid; idx < HID * HID; idx += THREADS) {        // root[k][j] -> Wt[(NB*32+j)][k]
-        const int j = idx & 31, k = idx >> 5;
-        Wt[(NB * HID + j) * WS + k] = rt[idx];
-      }
+      stage_layer_t<NB, THREADS, WS>(M, params, l, Wt, tid);
       __syncthreads();
       for (int t0 = v0; t0 < v1; t0 += TM) {
         const int tend = min(t0 + TM, v1);
@@ -387,11 +295,7 @@ k_l2_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* _
     // (3) d att[r,b] = sum_v sum_{in-runs of type r} < sum_run h_{l-1}[src,:] , dZ'[v,b,:] >,
     //     dZ'[v,b,k] = 1/deg(v) * sum_j dpre[v,j] basis[b][k][j]  - one pass over the own-node tiles
     {
-      const float* bs = params + M.off_basis[l];
-      for (int idx = tid; idx < NB * in * HID; idx += THREADS) {   // basis[b][k][j] -> W2[j][b*32+k]
-        const int j = idx & 31, k = (idx >> 5) % in, b = (idx >> 5) / in;
-        Wt[j * ZS2 + b * HID + k] = bs[idx];
-      }
+      stage_basis_w2<NB, THREADS>(M, params, l, in, Wt, tid);
       const int kg = tid >> 3, c0 = (tid & 7) * 4;   // thread: row kg, channels c0..c0+3
       float acc[NB + 1][4];
       float accb[4] = {0.f, 0.f, 0.f, 0.f};
@@ -486,16 +390,7 @@ k_l2_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* _
         }
         __syncthreads();
       }
-      if (kg < in) {
-#pragma unroll
-        for (int i = 0; i < NB; ++i)
-          *reinterpret_cast<float4*>(gp + M.off_basis[l] + (i * in + kg) * HID + c0) =
-              make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
-        *reinterpret_cast<float4*>(gp + M.off_root[l] + kg * HID + c0) =
-            make_float4(acc[NB][0], acc[NB][1], acc[NB][2], acc[NB][3]);
-        if (kg == 0)
-          *reinterpret_cast<float4*>(gp + M.off_bias[l] + c0) = make_float4(accb[0], accb[1], accb[2], accb[3]);
-      }
+      store_wgrad_rows<NB>(M, l, in, kg, c0, acc, accb, gp);
       __syncthreads();
       for (int idx = tid; idx < R * NB; idx += THREADS) {
         double s = 0.0;
@@ -520,25 +415,6 @@ size_t bwd_smem(int R, int NB, int L) {
   return fl * sizeof(float);
 }
 
-template <class Kern, class... Args>
-int launch(Kern kern, int B, int csize, size_t smem, cudaStream_t st, Args... args) {
-  cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(B * csize);
-  cfg.blockDim = dim3(THREADS);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = csize;
-  at[0].val.clusterDim.y = 1;
-  at[0].val.clusterDim.z = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = 1;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, args...);
-  return e != cudaSuccess ? (int)e + 1000 : 0;
-}
-
 }  // namespace
 
 // bytes of dynamic shared memory of the L2 plan's forward / backward kernel (independent of the subgraph size)
@@ -554,8 +430,8 @@ int l2_forward(const igmc_model_t* M, const float* params, const uint8_t* node_l
   const size_t smem = l2_smem_bytes(M, 0);
   auto kern = M->num_bases == 4 ? (S->rel_inv_deg ? k_l2_forward<4, true> : k_l2_forward<4, false>)
                                 : (S->rel_inv_deg ? k_l2_forward<2, true> : k_l2_forward<2, false>);
-  return launch(kern, B, csize, smem, st, *M, params, node_label, node_ptr, edge_ptr, *A, csize, *D, training, *S, y,
-                loss_scale, dpred, sqerr, err);
+  return launch_cluster(kern, B * csize, THREADS, smem, csize, false, st, *M, params, node_label, node_ptr, edge_ptr, *A,
+                        csize, *D, training, *S, y, loss_scale, dpred, sqerr, err);
 }
 
 int l2_backward(const igmc_model_t* M, const float* params, const uint8_t* node_label, const int32_t* node_ptr,
@@ -565,6 +441,6 @@ int l2_backward(const igmc_model_t* M, const float* params, const uint8_t* node_
   const size_t smem = l2_smem_bytes(M, 1);
   auto kern = M->num_bases == 4 ? (S->rel_inv_deg ? k_l2_backward<4, true> : k_l2_backward<4, false>)
                                 : (S->rel_inv_deg ? k_l2_backward<2, true> : k_l2_backward<2, false>);
-  return launch(kern, B, csize, smem, st, *M, params, node_label, node_ptr, edge_ptr, *A, csize, *D, *S, dpred, gpart,
-                dhid, dbuf, err);
+  return launch_cluster(kern, B * csize, THREADS, smem, csize, false, st, *M, params, node_label, node_ptr, edge_ptr, *A,
+                        csize, *D, *S, dpred, gpart, dhid, dbuf, err);
 }

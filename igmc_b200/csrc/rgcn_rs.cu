@@ -15,8 +15,7 @@
 #include <cooperative_groups.h>
 #include <cstdlib>
 
-#include "common.cuh"
-#include "../../include/igmc_b200.h"
+#include "lists.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -28,35 +27,10 @@ constexpr int RS_MAX_R = 12;
 constexpr int GN = 4;          // destination nodes per warp group (one 8-lane group each)
 constexpr int TW = 32;         // node tile of the weight-gradient GEMM
 constexpr int WP = 33;         // padded row stride of the transposition scratch
-constexpr uint32_t DROPPED = 0xFFFFFFFFu;
-
-// activation tiles [n][32]: column XOR-swizzled by the row in 4-float groups (a row stays one 128 B line,
-// a fixed column group over 8 consecutive rows hits 8 different bank groups)
-__device__ __forceinline__ int hix(int v, int c) { return (v << 5) + (c ^ ((v & 7) << 2)); }
-__host__ __device__ __forceinline__ int a4(int x) { return (x + 3) & ~3; }
-
-struct Keep {
-  bool active;
-  const uint8_t* mask;
-  uint64_t seed;
-  uint32_t thresh;
-  __device__ __forceinline__ bool keep(int e) const {
-    return mask ? (mask[e] != 0) : edge_keep(seed, (uint32_t)e, thresh);
-  }
-};
-__device__ __forceinline__ Keep make_keep(const igmc_dropout_t& D, int training) {
-  Keep K;
-  K.mask = D.edge_keep;
-  K.seed = D.seed_dev ? *D.seed_dev : D.seed;
-  K.active = training && (D.adj_dropout > 0.0f || D.edge_keep != nullptr);
-  double t = (double)D.adj_dropout * 4294967296.0;
-  K.thresh = t >= 4294967295.0 ? 0xFFFFFFFFu : (uint32_t)t;
-  return K;
-}
 
 // entry of list position p, DROPPED if the (possibly mirrored) edge is dropped this step
 __device__ __forceinline__ uint32_t load_entry(const uint32_t* __restrict__ adj, const int32_t* __restrict__ eid,
-                                               int p, const Keep& K, bool mirror, int eb, int m_half) {
+                                               int p, const EdgeKeep& K, bool mirror, int eb, int m_half) {
   uint32_t ent = __ldg(adj + p);
   if (K.active) {
     int e = __ldg(eid + p);
@@ -123,7 +97,7 @@ __device__ __forceinline__ Lists lists_view(int* ibuf, int own_cap, const uint32
 // Block-wide; ends with a barrier.  `ibuf` has list_ints(own_cap) ints and is preceded by the IMG_HDR header ints
 // (written here too).  invdeg_out/invdeg_glob (each optional) get 1/max(kept degree,1) of the own nodes.
 __device__ __forceinline__ Lists stage_lists(const uint32_t* adj, const int32_t* eid, const int32_t* ptr, int nb, int lo,
-                                             int hi, const Keep& K, bool mirror, int eb, int m_half, uint32_t* lbuf,
+                                             int hi, const EdgeKeep& K, bool mirror, int eb, int m_half, uint32_t* lbuf,
                                              int lcap, int* ibuf, int own_cap, int chunk, int* ws, float* invdeg_out,
                                              float* invdeg_glob) {
   const int tid = threadIdx.x, NT = blockDim.x, lane = tid & 31, warp = tid >> 5, nwarps = NT >> 5;
@@ -262,7 +236,7 @@ __device__ __forceinline__ float4 scale_row(float4 a, float s) { return make_flo
 // Mean per relation (igmc_saved_t.rel_inv_deg): out[v*R + r] = 1/max(kept in-edges of type r at v, 1) for the own
 // nodes v = lo + i, counted from the staged (compacted) in-lists, or from the global lists when they are not staged.
 // Warp per node, lane r counts type r (R <= RS_MAX_R < 32).  Block-wide; the caller's next barrier publishes it.
-__device__ __forceinline__ void rel_inv_deg_own(const Lists& Ls, const Keep& K, const int32_t* __restrict__ in_ptr,
+__device__ __forceinline__ void rel_inv_deg_own(const Lists& Ls, const EdgeKeep& K, const int32_t* __restrict__ in_ptr,
                                                 int nb, int lo, int n_own, int R, float* __restrict__ out) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
   for (int i = warp; i < n_own; i += nwarps) {
@@ -301,7 +275,7 @@ __device__ __forceinline__ void rel_inv_deg_own(const Lists& Ls, const Keep& K, 
 // PR (backward of the mean per relation): every entry (nbr, type r) is weighed by rinv[nbr*R + r] = 1/|N_r(nbr)|,
 // read through L2 (the table is written by the forward, possibly by a peer CTA of the same launch).
 template <int GL, bool PR = false>
-__device__ __forceinline__ void gather_segments(const Lists& Ls, const Keep& K, int sg0, int sg1, int lane,
+__device__ __forceinline__ void gather_segments(const Lists& Ls, const EdgeKeep& K, int sg0, int sg1, int lane,
                                                 const float* __restrict__ feat, float* __restrict__ stage, int SS,
                                                 int inp, int* ticket, const float* rinv = nullptr, int R = 0) {
   const int q = lane & (GL - 1);
@@ -608,7 +582,7 @@ __device__ __forceinline__ bool forward_body(const igmc_model_t& M, const float*
     if (tid == 0) igmc_set_err(err, IGMC_ERR_SMEM_NODES);
     return false;
   }
-  const Keep K = make_keep(D, training);
+  const EdgeKeep K = make_keep(D, training);
   const Split own = own_range(n, rank, CL);
   const int n_own = own.hi - own.lo;
   IGMC_STAMP(0);
@@ -819,61 +793,13 @@ __device__ __forceinline__ bool forward_body(const igmc_model_t& M, const float*
   IGMC_STAMP(27);
   for (int c = tid; c < F; c += NT) S.feat[(size_t)g * F + c] = feat_s[c];
   if (tid == 0) { S.target[2 * g] = nb + tu; S.target[2 * g + 1] = nb + ti; }
-  const float* W1 = params + M.off_lin1_w;
-  constexpr int OW = 8;   // outputs per warp and pass: 16 warps x 8 = all 128 in one pass of L2 latency
-  for (int ob = warp * OW; ob < L1O; ob += nwarps * OW) {
-    float s4[OW];
-#pragma unroll
-    for (int u = 0; u < OW; ++u) s4[u] = 0.f;
-    const float bias_o = lane < OW ? __ldg(params + M.off_lin1_b + ob + lane) : 0.f;   // independent of the dot products
-#pragma unroll 4   // 32 independent L2 loads in flight per lane (the loop is latency bound)
-    for (int i = lane; i < F; i += 32) {
-      const float f = feat_s[i];
-#pragma unroll
-      for (int u = 0; u < OW; ++u) s4[u] = fmaf(__ldg(W1 + (size_t)(ob + u) * F + i), f, s4[u]);
-    }
-#pragma unroll
-    for (int u = 0; u < OW; ++u) s4[u] = warp_sum_f(s4[u]);
-#pragma unroll
-    for (int u = 0; u < OW; ++u) if (lane == u) {
-      const int o = ob + u;
-      const float s = s4[u];
-      float h = fmaxf(s + bias_o, 0.f);
-      float scale = 1.f;
-      if (training && (D.hidden_dropout > 0.f || D.hidden_keep)) {
-        bool keep;
-        if (D.hidden_keep) keep = D.hidden_keep[(size_t)g * L1O + o] != 0;
-        else {
-          double t = (double)D.hidden_dropout * 4294967296.0;
-          keep = edge_keep(K.seed ^ 0x5bd1e995a5a5a5a5ull, (uint32_t)(g * L1O + o),
-                           t >= 4294967295.0 ? 0xFFFFFFFFu : (uint32_t)t);
-        }
-        const float p = D.hidden_keep ? 0.5f : D.hidden_dropout;
-        scale = keep ? 1.f / (1.f - p) : 0.f;
-      }
-      hid_s[o] = h * scale;
-      S.hid[(size_t)g * L1O + o] = h * scale;
-      S.hid_gscale[(size_t)g * L1O + o] = h > 0.f ? scale : 0.f;
-    }
-  }
+  readout_lin1(M, params, feat_s, F, g, D, K.seed, training, hid_s, S, warp, nwarps, lane);
   IGMC_STAMP(28);
   __syncthreads();
   IGMC_STAMP(29);
-  if (warp == 0) {
-    float s = 0.f;
-    const float b2 = __ldg(params + M.off_lin2_b), yg = y ? __ldg(y + g) : 0.f;   // issued with the weight loads
-    for (int o = lane; o < L1O; o += 32) s = fmaf(params[M.off_lin2_w + o], hid_s[o], s);
-    s = warp_sum_f(s);
-    if (lane == 0) {
-      const float out = (s + b2) * M.multiply_by;
-      S.pred[g] = out;
-      if (y) {
-        const float diff = out - yg;
-        if (sqerr) sqerr[g] = diff * diff;
-        if (dpred) dpred[g] = 2.f * diff * loss_scale * M.multiply_by;
-      }
-    }
-  }
+  if (warp == 0)
+    readout_lin2(M, params, hid_s, M.multiply_by, g, y, loss_scale, S.pred, sqerr,
+                 dpred, lane);
   IGMC_STAMP(2 + 6 * L);
   IGMC_WALL(51);
   return true;
@@ -963,7 +889,7 @@ __device__ __forceinline__ void backward_body(const igmc_model_t& M, const float
     if (tid == 0) igmc_set_err(err, IGMC_ERR_SMEM_NODES);
     return;
   }
-  const Keep K = make_keep(D, 1);
+  const EdgeKeep K = make_keep(D, 1);
   const bool sym = A.symmetric != 0;
   const Split own = own_range(n, rank, CL);
   const int n_own = own.hi - own.lo;
@@ -1018,30 +944,16 @@ __device__ __forceinline__ void backward_body(const igmc_model_t& M, const float
   const int tu = ext ? -1 : S.target[2 * g] - nb, ti = ext ? -1 : S.target[2 * g + 1] - nb;
 
   // ---- readout backward (every CTA needs d feat to seed its target rows) ----
-  if (!ext) {
-    const float dp = dpred[g];
-    for (int o = tid; o < L1O; o += NT) {
-      const float d = dp * params[M.off_lin2_w + o] * S.hid_gscale[(size_t)g * L1O + o];
-      dhid_s[o] = d;
-      if (rank == 0) dhid_out[(size_t)g * L1O + o] = d;
-    }
-  }
+  if (!ext) readout_dhid(M, params, S, dpred, g, dhid_s, dhid_out, rank == 0, tid, NT);
   if (!PR)
     for (int v = tid; v < n; v += NT) invdeg[v] = __ldcg(S.inv_deg + nb + v);   // (peer rows: L2, see k_train_rs)
   // PR: 1/|N_r(d)| of every node d, read through L2 by the gather (peer rows, as inv_deg above)
   const float* rinv = PR ? S.rel_inv_deg + (size_t)nb * R : nullptr;
   __syncthreads();
   if (!ext) {
-    // d feat[i] = sum_o W1[o][i] d hid[o]: thread slice p of NT/F takes every (NT/F)-th o, partials in `stage`
-    const float* W1 = params + M.off_lin1_w;
+    // d feat: thread slice p of NT/F takes every (NT/F)-th o, partials in `stage`, summed in slice order
     const int parts = max(1, NT / F);
-    const int i = tid % F, part = tid / F;
-    if (part < parts) {
-      float s = 0.f;
-#pragma unroll 32   // independent L2 loads in flight (latency bound)
-      for (int o = part; o < L1O; o += parts) s = fmaf(__ldg(W1 + (size_t)o * F + i), dhid_s[o], s);
-      stage[part * F + i] = s;
-    }
+    readout_dfeat_part(M, params, dhid_s, F, parts, tid, stage);
     __syncthreads();
     for (int j = tid; j < F; j += NT) {
       float s = 0.f;
@@ -1397,7 +1309,7 @@ k_stage_lists(const int32_t* __restrict__ node_ptr, const int32_t* __restrict__ 
     if (tid < IMG_HDR) gt[tid] = 0;
     return;
   }
-  const Keep K = make_keep(D, training);
+  const EdgeKeep K = make_keep(D, training);
   const bool sym = A.symmetric != 0;
   const Split own = own_range(n, rank, CL);
   if (dir == 0)
@@ -1489,32 +1401,6 @@ static int pdl_enabled() {
   return v;
 }
 
-template <class Kern, class... Args>
-static int launch_cluster(Kern kern, int grid, int threads, size_t smem, int cluster, bool pdl, cudaStream_t st,
-                          Args... args) {
-  cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(threads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute at[2];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = cluster;
-  at[0].val.clusterDim.y = 1;
-  at[0].val.clusterDim.z = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = 1;
-  if (pdl && (pdl_enabled() & 1)) {   // IGMC_PDL bit 0: backward behind the forward; bit 1: update kernel (csrc/optim.cu)   // may start under the tail of the previous kernel of the stream (pdl_wait inside)
-    at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.numAttrs = 2;
-  }
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, args...);
-  if (e != cudaSuccess) return (int)e + 1000;
-  return 0;
-}
-
 // the image a kernel is handed must have been built for exactly its plan
 static int check_image(const igmc_stage_t* I, int n_cap, int cluster, int lcap, int chunk, igmc_stage_t* out) {
   igmc_stage_t none = {};
@@ -1601,7 +1487,9 @@ int rs_backward(const igmc_model_t* M, const float* params, const uint8_t* node_
   const bool pr = S->rel_inv_deg != nullptr;
   auto kern = threads == 512 ? (pr ? rs::k_backward_rs<512, true> : rs::k_backward_rs<512, false>)
                              : (pr ? rs::k_backward_rs<1024, true> : rs::k_backward_rs<1024, false>);
-  return launch_cluster(kern, B * cluster, threads, smem, cluster, true, st, *M, params, node_label, node_ptr, edge_ptr,
+  // IGMC_PDL bit 0: the backward may start under the tail of the forward (bit 1: the update kernel, csrc/optim.cu)
+  const bool pdl = pdl_enabled() & 1;
+  return launch_cluster(kern, B * cluster, threads, smem, cluster, pdl, st, *M, params, node_label, node_ptr, edge_ptr,
                         *A, n_cap, lcap, chunk, *D, *S, dpred, gpart, dhid, img, err);
 }
 

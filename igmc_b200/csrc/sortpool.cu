@@ -6,8 +6,7 @@
 // last channel descending, ties by node index (torch's sort leaves ties unspecified).  All reductions have a fixed
 // order: results are bitwise run-to-run deterministic.  HBM traffic per graph: the k pooled rows of concat_states,
 // the saved activations (c1*k + c1*t1 + dense_dim floats) and, through L2, lin1.weight.
-#include "common.cuh"
-#include "../../include/igmc_b200.h"
+#include "lists.cuh"
 
 namespace {
 
@@ -163,40 +162,12 @@ k_sortpool_forward(igmc_sortpool_t P, const float* __restrict__ params, const fl
     }
     for (; i < P.dense_dim; i += 32) s0 = fmaf(__ldg(wr + i), flat[i], s0);
     const float s = warp_sum_f((s0 + s1) + (s2 + s3));
-    if (lane == 0) {
-      const float h = fmaxf(s + params[P.off_lin1_b + o], 0.f);
-      float scale = 1.f;
-      if (training && (D.hidden_dropout > 0.f || D.hidden_keep)) {        // F.dropout models.py:163
-        bool keep;
-        if (D.hidden_keep) keep = D.hidden_keep[(size_t)g * L1O + o] != 0;
-        else {
-          const double t = (double)D.hidden_dropout * 4294967296.0;
-          keep = edge_keep(seed ^ 0x5bd1e995a5a5a5a5ull, (uint32_t)(g * L1O + o),
-                           t >= 4294967295.0 ? 0xFFFFFFFFu : (uint32_t)t);
-        }
-        const float p = D.hidden_keep ? 0.5f : D.hidden_dropout;
-        scale = keep ? 1.f / (1.f - p) : 0.f;
-      }
-      hid_s[o] = h * scale;
-      S.hid[(size_t)g * L1O + o] = h * scale;
-      S.hid_gscale[(size_t)g * L1O + o] = h > 0.f ? scale : 0.f;
-    }
+    if (lane == 0)   // dropout models.py:163
+      readout_hidden(s + params[P.off_lin1_b + o], g, o, D, seed, training, hid_s, S);
   }
   __syncthreads();
-  if (warp == 0) {
-    float s = 0.f;
-    for (int o = lane; o < L1O; o += 32) s = fmaf(params[P.off_lin2_w + o], hid_s[o], s);
-    s = warp_sum_f(s);
-    if (lane == 0) {
-      const float out = s + params[P.off_lin2_b];                          // x[:, 0]  models.py:165
-      S.pred[g] = out;
-      if (y) {
-        const float diff = out - y[g];
-        if (sqerr) sqerr[g] = diff * diff;
-        if (dpred) dpred[g] = 2.f * diff * loss_scale;
-      }
-    }
-  }
+  if (warp == 0)   // x[:, 0]  models.py:165 (no multiply_by: the factor 1 is exact)
+    readout_lin2(P, params, hid_s, 1.f, g, y, loss_scale, S.pred, sqerr, dpred, lane);
 }
 
 __global__ void __launch_bounds__(SP_THREADS)
@@ -226,12 +197,7 @@ k_sortpool_backward(igmc_sortpool_t P, const float* __restrict__ params, const f
   float* gp_w1 = gp, *gp_b1 = gp + c1 * W, *gp_w2 = gp_b1 + c1, *gp_b2 = gp_w2 + c2 * c1 * kw2;
 
   // d hid (lin2, dropout, relu) ; operands of the later phases -> shared
-  const float dpg = dpred[g];
-  for (int o = tid; o < L1O; o += SP_THREADS) {
-    const float d = dpg * params[P.off_lin2_w + o] * S.hid_gscale[(size_t)g * L1O + o];
-    dhid_s[o] = d;
-    S.dhid[(size_t)g * L1O + o] = d;
-  }
+  readout_dhid(P, params, S, dpred, g, dhid_s, S.dhid, true, tid, SP_THREADS);
   for (int i = tid; i < c1 * W; i += SP_THREADS) w1[i] = params[P.off_conv1_w + i];
   for (int i = tid; i < c2 * c1 * kw2; i += SP_THREADS) w2[i] = params[P.off_conv2_w + i];
   for (int i = tid; i < c1 * k; i += SP_THREADS) act1[i] = S.act1[(size_t)g * c1 * k + i];

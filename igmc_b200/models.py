@@ -37,10 +37,15 @@ def splitmix64(x):
     return x ^ (x >> 31)
 
 
+def _keep_threshold(p):
+    """Host twin of ``keep_thresh`` in csrc/lists.cuh: a draw keeps its unit iff hash >= p * 2^32 (clamped)."""
+    import numpy as np
+    return min(int(float(np.float32(p)) * 4294967296.0), 0xFFFFFFFF)   # the kernel sees p as fp32
+
+
 def edge_keep_reference(seed, num_edges, p):
     """Host twin of ``edge_keep`` in csrc/common.cuh: bool keep mask for directed edges 0..E-1."""
-    import numpy as np
-    thresh = min(int(float(np.float32(p)) * 4294967296.0), 0xFFFFFFFF)   # the kernel sees p as fp32
+    thresh = _keep_threshold(p)
     return torch.tensor([(splitmix64((seed + e) & ((1 << 64) - 1)) >> 32) >= thresh for e in range(num_edges)],
                         dtype=torch.bool)   # (a batch without edges still gets a bool mask)
 
@@ -49,9 +54,8 @@ def hidden_keep_reference(seed, num_graphs, p):
     """Host twin of the hidden dropout before ``lin2`` (the kernels' own draw when no ``hidden_keep`` is injected):
     bool keep mask [num_graphs, 128]; unit ``o`` of graph ``g`` is an ``edge_keep`` draw of index ``g*128 + o`` on the
     seed ``seed ^ 0x5bd1e995a5a5a5a5``.  Kept units are scaled by 1 / (1 - p)."""
-    import numpy as np
     M = (1 << 64) - 1
-    thresh = min(int(float(np.float32(p)) * 4294967296.0), 0xFFFFFFFF)
+    thresh = _keep_threshold(p)
     s = (seed ^ 0x5bd1e995a5a5a5a5) & M
     keep = [(splitmix64((s + i) & M) >> 32) >= thresh for i in range(num_graphs * 128)]
     return torch.tensor(keep, dtype=torch.bool).view(num_graphs, 128)
