@@ -25,6 +25,7 @@ ERR_NAMES = {
     5: "malformed batch (edges not grouped by graph / node outside its graph / no target node)",
     6: "subgraph of more than 65535 nodes (beyond the 16-bit neighbour field of the edge lists)",
     7: "inference candidates: a user / item id outside the rating matrix or an inconsistent candidate plan",
+    8: "graph update: a user / item id outside the graph's capacity or a value outside 0..256",
 }
 
 TOPK_MAX = 256       # IGMC_TOPK_MAX
@@ -120,6 +121,11 @@ class Candidates(C.Structure):
                 ("exclude_rated", C.c_int32), ("pad_", C.c_int32)]
 
 
+GRAPH_UPDATE_HEADER = ("nnz", "num_users", "num_items", "max_row_deg", "max_col_deg", "inserted", "changed",
+                       "removed")   # igmc_graph_update_header_t: these int64 fields, then int32 status, int32 err
+GRAPH_UPDATE_OVER_CAPACITY, GRAPH_UPDATE_OVER_INT32 = 1, 2
+
+
 MAX_RANKS = 8
 
 
@@ -173,6 +179,11 @@ _SIGS = {
     "igmc_candidate_pairs": [C.POINTER(CSR), C.POINTER(Candidates), vp, C.c_int, vp, vp, vp, vp, vp, vp],
     "igmc_topk_merge": [vp, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp, vp],
     "igmc_score_scatter": [vp, C.c_int, C.c_int, vp, vp, vp],
+    "igmc_graph_update_ws_bytes": [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int64)],
+    "igmc_graph_update_plan": [C.POINTER(CSR), C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, C.c_int, C.c_int,
+                               C.c_int, vp, C.c_int64, vp, vp, vp],
+    "igmc_graph_update_apply": [C.POINTER(CSR), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, C.c_int64, C.c_int,
+                                C.c_int, C.c_int, vp],
     "igmc_build_info": [],
     "igmc_model_plan": [C.POINTER(Model), C.c_int, C.c_int, C.c_int],
     "igmc_sortpool_plan": [C.POINTER(SortPool), C.c_int, C.c_int],

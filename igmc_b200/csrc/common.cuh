@@ -16,6 +16,7 @@ enum {
   IGMC_ERR_BAD_BATCH = 5,   // edges not grouped by graph / node ids outside their graph
   IGMC_ERR_NODE_ID16 = 6,   // subgraph of more than 65 535 nodes: beyond the 16-bit neighbour field of the lists
   IGMC_ERR_CANDIDATES = 7,  // inference candidates: a user / item id outside the rating matrix or an inconsistent plan
+  IGMC_ERR_GRAPH_UPDATE = 8,  // graph update: an id outside the capacity or a value outside 0..256
 };
 
 __device__ __forceinline__ void igmc_set_err(int* err, int code) {

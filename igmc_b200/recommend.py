@@ -165,6 +165,9 @@ class InferenceEngine(object):
         while eng.step():
             pass
         top_items, top_scores = eng.finish()   # (predict: scores)
+
+    An engine serves across updates of its ``RatingGraph`` (``graph.update``) between runs; an update during a run
+    makes its next ``step`` raise RuntimeError.
     """
 
     def __init__(self, model, graph, h=1, sample_ratio=1.0, max_nodes_per_hop=None, batch_size=256,
@@ -217,7 +220,7 @@ class InferenceEngine(object):
         users = _host_ids(users, "users", g.num_users)
         cand = None if items is None else np.unique(_host_ids(items, "items", g.num_items))
         U, dev = len(users), self.dev
-        run = dict(kind="recommend", U=U, k=k,
+        run = dict(kind="recommend", U=U, k=k, version=g.version,
                    top_s=torch.full((U, k), -float("inf"), dtype=torch.float32, device=dev),
                    top_i=torch.full((U, k), -1, dtype=torch.int64, device=dev))
         self.run = run
@@ -256,7 +259,8 @@ class InferenceEngine(object):
         if len(users) != len(items):
             raise ValueError("users and items must have the same length (%d vs %d)" % (len(users), len(items)))
         P = len(users)
-        run = dict(kind="pairs", P=P, scores=torch.empty(P, dtype=torch.float32, device=self.dev))
+        run = dict(kind="pairs", P=P, version=g.version,
+                   scores=torch.empty(P, dtype=torch.float32, device=self.dev))
         self.run = run
         if P == 0:
             return 0
@@ -271,7 +275,7 @@ class InferenceEngine(object):
     def _prime(self):
         """candidate pairs + extraction of the first batch, the model's plan for it (its one host sync, if any) and
         the prepared weights of every parameter set; captured graphs of an earlier run are dropped (they hold its
-        buffers and candidate total)"""
+        buffers, its candidate total and the graph's shape as it was; the extractor follows an updated graph)"""
         run = self.run
         run["steps"] = (run["P"] + self.B - 1) // self.B
         run["done"] = 0
@@ -342,6 +346,9 @@ class InferenceEngine(object):
         run = self.run
         if run is None or run["P"] == 0 or run["done"] >= run["steps"]:
             return False
+        if self.graph.version != run["version"]:
+            raise RuntimeError("the rating graph was updated during this run: its candidates and captured steps belong "
+                               "to the old graph; start the run again")
         slot = run["done"] & 1
         if self.use_graph and slot in self.graphs:
             self.graphs[slot].replay()

@@ -111,6 +111,7 @@ class TrainEngine(object):
         self.loss_acc = torch.zeros(1, dtype=torch.float32, device=self.dev)   # sum_steps loss*G (this rank)
         self.last_loss = torch.zeros(1, dtype=torch.float32, device=self.dev)
         self.steps = 0
+        self._graph_version = None    # version of the dataset's rating graph at the first step
         # zero-copy step I/O (pipelined engine): the kernels of a step read its inputs straight out of one of two
         # pinned host buffers and the update kernel stores the step's loss into a pinned host ring - no copy-engine
         # operation between two graph replays (the two per-step memcpys serialise with the step's kernels)
@@ -204,8 +205,21 @@ class TrainEngine(object):
         self.ring_used[slot] = True
         return nb
 
+    def _check_graph(self):
+        """the captured steps hold launch arguments derived from the rating graph (its shape, max_row_deg, the
+        extractor's capacities): training on a graph updated after the first step is refused"""
+        g = getattr(self.dataset, "graph", None)
+        if g is None or not self.pipelined():
+            return
+        if self._graph_version is None:
+            self._graph_version = g.version
+        elif g.version != self._graph_version:
+            raise RuntimeError("the rating graph was updated after this TrainEngine's first step; training on a "
+                               "changing graph is not supported (build a new engine)")
+
     def step(self, idx, epoch=0, G=None, staged=False):
         """One optimisation step on this rank's ``idx`` (host int array).  H2D copy + graph replay."""
+        self._check_graph()
         G = len(idx) * self.world if G is None else int(G)
         self.steps += 1
         if not hasattr(self.dataset, "extractor") or hasattr(self.dataset, "slices"):
@@ -276,6 +290,7 @@ class TrainEngine(object):
 
     def prime(self, idx, epoch=0, G=None):
         """extract the first batch of a pipelined sequence (no model work)."""
+        self._check_graph()
         if not hasattr(self, "side"):
             self.side = torch.cuda.Stream()
             self.batches = [None, None]
@@ -294,6 +309,7 @@ class TrainEngine(object):
     def step_pipe(self, next_idx=None, epoch=0, next_G=None, staged=False):
         """train on the batch extracted by the previous call (or prime) while extracting ``next_idx``.
         One H2D copy of the next indices + one graph replay."""
+        self._check_graph()
         nb, G = self.cur
         self.steps += 1
         if self._adam_base is None:

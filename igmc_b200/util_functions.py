@@ -8,6 +8,7 @@ model and train loop touch (``x, edge_index, edge_type, y, batch, num_graphs, to
 
 No CPU fallback: constructing a dataset or extracting without a CUDA device raises.
 """
+import collections
 import ctypes as C
 import os
 
@@ -16,7 +17,7 @@ import torch
 
 from . import _lib
 
-__all__ = ["RatingGraph", "Data", "Batch", "SubgraphExtractor", "MyDynamicDataset", "MyDataset"]
+__all__ = ["RatingGraph", "GraphCapacity", "graph_update_host", "Data", "Batch", "SubgraphExtractor", "MyDynamicDataset", "MyDataset"]
 
 
 def _require_cuda(device=None):
@@ -68,12 +69,24 @@ def mapped_view(pinned):
     return DevView(pinned)
 
 
+GraphCapacity = collections.namedtuple("GraphCapacity", "users items nnz")
+
+_GRAPH_ARRAYS = (("row_ptr", np.int32), ("col_idx", np.int32), ("rating", np.uint8), ("col_ptr", np.int32),
+                 ("row_idx", np.int32))
+
+
 class RatingGraph(object):
     """Flat device CSR + CSC of ``adj_train`` (scipy CSR, stored value = rating label + 1,
-    preprocessing.py:190-197).  Replaces SparseRowIndexer/SparseColIndexer (util_functions.py:20-66)."""
+    preprocessing.py:190-197).  Replaces SparseRowIndexer/SparseColIndexer (util_functions.py:20-66).
 
-    def __init__(self, A, device=None):
+    The device arrays are allocated at capacity (``reserve_*`` beyond the matrix) so that ``update`` can insert ratings
+    and add users / items in place; the five device pointers never change.  ``version`` counts the updates that
+    changed the graph; ``host`` is a mirror refreshed on its first access after one."""
+
+    def __init__(self, A, device=None, *, reserve_nnz=0, reserve_users=0, reserve_items=0):
         import scipy.sparse as ssp
+        if min(int(reserve_nnz), int(reserve_users), int(reserve_items)) < 0:
+            raise ValueError("reserve_nnz / reserve_users / reserve_items must be >= 0")
         A = ssp.csr_matrix(A)
         A.sum_duplicates()
         A.sort_indices()
@@ -87,25 +100,57 @@ class RatingGraph(object):
         Cc.sort_indices()
         self.max_row_deg = int(np.diff(A.indptr).max()) if self.nnz else 0
         self.max_col_deg = int(np.diff(Cc.indptr).max()) if self.nnz else 0
-        self.host = dict(row_ptr=A.indptr.astype(np.int32), col_idx=A.indices.astype(np.int32),
-                         rating=lab.astype(np.uint8), col_ptr=Cc.indptr.astype(np.int32),
-                         row_idx=Cc.indices.astype(np.int32))
+        self._host = dict(row_ptr=A.indptr.astype(np.int32), col_idx=A.indices.astype(np.int32),
+                          rating=lab.astype(np.uint8), col_ptr=Cc.indptr.astype(np.int32),
+                          row_idx=Cc.indices.astype(np.int32))
+        self._cap = GraphCapacity(self.num_users + int(reserve_users), self.num_items + int(reserve_items),
+                                  self.nnz + int(reserve_nnz))
+        self.version = 0
+        self._host_version = 0
+        self._upd = None           # update workspace, header and error word (allocated on the first update)
         self.device = None
         self.dev = {}
         if device is not None or torch.cuda.is_available():
             self.to(_require_cuda(device))
 
+    @property
+    def capacity(self):
+        """(users, items, nnz) the device arrays hold: ids up to users - 1 / items - 1 and nnz ratings"""
+        return self._cap
+
+    @property
+    def host(self):
+        """host copies of the five arrays, cut to the current shape and nnz (one device-to-host copy per array on the
+        first access after an update)"""
+        if self._host_version != self.version:
+            d, n = self.dev, self.nnz
+            self._host = dict(row_ptr=d["row_ptr"][:self.num_users + 1].cpu().numpy(),
+                              col_idx=d["col_idx"][:n].cpu().numpy(), rating=d["rating"][:n].cpu().numpy(),
+                              col_ptr=d["col_ptr"][:self.num_items + 1].cpu().numpy(),
+                              row_idx=d["row_idx"][:n].cpu().numpy())
+            self._host_version = self.version
+        return self._host
+
     def to(self, device):
+        h = self.host
         self.device = torch.device(device)
-        self.dev = {k: torch.from_numpy(v).to(self.device) for k, v in self.host.items()}
-        # a zero-length index array still needs a valid pointer
-        for k, v in self.dev.items():
-            if v.numel() == 0:
-                self.dev[k] = torch.zeros(1, dtype=v.dtype, device=self.device)
+        cu, ci, cn = self._cap
+        size = dict(row_ptr=cu + 1, col_idx=cn, rating=cn, col_ptr=ci + 1, row_idx=cn)
+        self.dev = {}
+        for k, dt in _GRAPH_ARRAYS:
+            # a zero-length index array still needs a valid pointer
+            t = torch.zeros(max(size[k], 1), dtype=_TORCH_OF[dt], device=self.device)
+            if len(h[k]):
+                t[:len(h[k])] = torch.from_numpy(h[k]).to(self.device)
+            self.dev[k] = t
+        self._upd = None
+        self._make_c()
+        return self
+
+    def _make_c(self):
         self._c = _lib.CSR(self.dev["row_ptr"].data_ptr(), self.dev["col_idx"].data_ptr(),
                            self.dev["rating"].data_ptr(), self.dev["col_ptr"].data_ptr(),
                            self.dev["row_idx"].data_ptr(), self.num_users, self.num_items)
-        return self
 
     def node_cap(self, max_nodes_per_hop, h=1):
         """capacity of one side's node list: target + per hop min(mnph, largest possible fringe) (hop 1: a row or
@@ -116,6 +161,206 @@ class RatingGraph(object):
             d = min(d, int(max_nodes_per_hop))
             side = min(side, int(max_nodes_per_hop))
         return min(1 + d + (int(h) - 1) * side, 1 + max(self.num_users, self.num_items))
+
+    # ---- in-place update (igmc_graph_update_plan / _apply, csrc/graph_update.cu) ------------------------------------
+    def update(self, users, items, values, shape=None):
+        """Apply ratings in place: ``values[i]`` = rating label + 1 (1..256) inserts or overwrites the rating of
+        (users[i], items[i]), 0 deletes it (an absent rating: nothing); the last occurrence of a pair wins.  Ids below
+        ``capacity`` grow ``shape`` to cover them, ``shape=`` grows it further (users / items without ratings); the
+        shape never shrinks.  Host arrays are validated here; int32 device tensors are used in place and validated by
+        the kernel (RuntimeError with IGMC_ERR_GRAPH_UPDATE, nothing changed).  ValueError, with nothing changed, if
+        the result would exceed the nnz capacity.  One host synchronisation.  Returns dict(inserted=, changed=,
+        removed=): the ratings added, relabelled and deleted."""
+        cu, ci, cn = self._cap
+        u, v, x, D = _update_inputs(users, items, values, cu, ci)
+        req = _update_shape(shape, self.shape, self._cap)
+        counts = dict(inserted=0, changed=0, removed=0)
+        if D == 0 and req == self.shape:
+            return counts
+        if self.device is None:
+            raise RuntimeError("igmc_b200 graph updates run on a CUDA device (there is no CPU path)")
+        if D == 0:      # shape only: the new rows / columns are empty
+            self.dev["row_ptr"][self.num_users + 1:req[0] + 1] = self.nnz
+            self.dev["col_ptr"][self.num_items + 1:req[1] + 1] = self.nnz
+            self._commit(self.nnz, req[0], req[1], self.max_row_deg, self.max_col_deg)
+            return counts
+        lib, dev = _lib.load(), self.device
+        u, v, x = (_on_device_i32(a, dev) for a in (u, v, x))
+        nbytes = C.c_int64(0)
+        _lib.check(lib.igmc_graph_update_ws_bytes(D, cu, ci, cn, C.byref(nbytes)), "igmc_graph_update_ws_bytes")
+        if self._upd is None:
+            self._upd = dict(ws=torch.empty(0, dtype=torch.uint8, device=dev),
+                             header=torch.zeros(len(_lib.GRAPH_UPDATE_HEADER) + 1, dtype=torch.int64, device=dev),
+                             err=torch.zeros(1, dtype=torch.int32, device=dev))
+        w = self._upd
+        if w["ws"].numel() < nbytes.value:
+            w["ws"] = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+        args = (C.byref(self._c), self.nnz, cu, ci, cn)
+        _lib.check(lib.igmc_graph_update_plan(*args, u.data_ptr(), v.data_ptr(), x.data_ptr(), D, req[0], req[1],
+                                              w["ws"].data_ptr(), w["ws"].numel(), w["header"].data_ptr(),
+                                              w["err"].data_ptr(), _stream_ptr()), "igmc_graph_update_plan")
+        hdr = w["header"].cpu().numpy()             # the update's one host synchronisation
+        h = dict(zip(_lib.GRAPH_UPDATE_HEADER, (int(a) for a in hdr)))
+        status, err = (int(a) for a in hdr[-1:].view(np.int32))
+        if err:
+            w["err"].zero_()
+            raise RuntimeError("igmc_b200 kernel error %d: %s" % (err, _lib.ERR_NAMES.get(err, "?")))
+        if status:
+            raise ValueError("the update would leave %d ratings, beyond the graph's capacity of %d%s (reserve_nnz "
+                             "makes room)" % (h["nnz"], cn, " and int32" if status == _lib.GRAPH_UPDATE_OVER_INT32
+                                              else ""))
+        counts = dict(inserted=h["inserted"], changed=h["changed"], removed=h["removed"])
+        if any(counts.values()) or (h["num_users"], h["num_items"]) != self.shape:
+            _lib.check(lib.igmc_graph_update_apply(*args, D, w["ws"].data_ptr(), w["ws"].numel(), h["nnz"],
+                                                   h["num_users"], h["num_items"], _stream_ptr()),
+                       "igmc_graph_update_apply")
+            self._commit(h["nnz"], h["num_users"], h["num_items"], h["max_row_deg"], h["max_col_deg"])
+        return counts
+
+    def _commit(self, nnz, nu, ni, max_row_deg, max_col_deg):
+        self.nnz, self.max_row_deg, self.max_col_deg = int(nnz), int(max_row_deg), int(max_col_deg)
+        if (nu, ni) != self.shape:
+            self.num_users, self.num_items = int(nu), int(ni)
+            self.shape = (self.num_users, self.num_items)
+            self._make_c()
+        self.version += 1
+
+
+_TORCH_OF = {np.int32: torch.int32, np.uint8: torch.uint8}
+
+
+def _update_inputs(users, items, values, cap_users, cap_items):
+    """(users, items, values, D) of an update: host arrays validated here (IndexError for an id outside the capacity,
+    ValueError for a value outside 0..256 or unequal lengths); device tensors are passed on unchecked (the kernel
+    checks them)"""
+    arrs = []
+    for name, a in (("users", users), ("items", items), ("values", values)):
+        if torch.is_tensor(a) and a.device.type == "cuda":
+            if a.is_floating_point() or a.is_complex() or a.dtype == torch.bool:
+                raise TypeError("%s must be integers, not %s" % (name, a.dtype))
+            arrs.append(a.reshape(-1))
+            continue
+        a = np.asarray(a.cpu().numpy() if torch.is_tensor(a) else a).reshape(-1)
+        if a.size and not np.issubdtype(a.dtype, np.integer):
+            raise TypeError("%s must be integers, not %s" % (name, a.dtype))
+        arrs.append(a.astype(np.int64))
+    n = [int(a.numel()) if torch.is_tensor(a) else len(a) for a in arrs]
+    if len(set(n)) != 1:
+        raise ValueError("users, items and values must have the same length (%d, %d, %d)" % tuple(n))
+    for a, name, hi in ((arrs[0], "users", cap_users), (arrs[1], "items", cap_items)):
+        if not torch.is_tensor(a) and a.size and (a.min() < 0 or a.max() >= hi):
+            bad = int(a.min()) if a.min() < 0 else int(a.max())
+            raise IndexError("%s: id %d outside the graph's capacity [0, %d)" % (name, bad, hi))
+    x = arrs[2]
+    if not torch.is_tensor(x) and x.size and (x.min() < 0 or x.max() > 256):
+        raise ValueError("values must be rating label + 1 (1..256) or 0 (delete), got %d"
+                         % (int(x.min()) if x.min() < 0 else int(x.max())))
+    return arrs[0], arrs[1], arrs[2], n[0]
+
+
+def _update_shape(shape, cur, cap):
+    if shape is None:
+        return tuple(cur)
+    shape = tuple(int(a) for a in shape)
+    if len(shape) != 2:
+        raise ValueError("shape must be (num_users, num_items)")
+    if shape[0] < cur[0] or shape[1] < cur[1]:
+        raise ValueError("shape %s would shrink the graph's %s: the id space never shrinks" % (shape, tuple(cur)))
+    if shape[0] > cap.users or shape[1] > cap.items:
+        raise ValueError("shape %s beyond the graph's capacity (%d, %d)" % (shape, cap.users, cap.items))
+    return shape
+
+
+def _on_device_i32(a, dev):
+    """int32 device tensor (an int32 device tensor is used in place; wider ones are clamped first, so that an id
+    beyond int32 stays invalid)"""
+    if torch.is_tensor(a) and a.device.type == "cuda":
+        if a.dtype != torch.int32:
+            a = a.clamp(-1, 2 ** 31 - 1).to(torch.int32)
+        return a.contiguous()
+    return torch.from_numpy(np.clip(a, -1, 2 ** 31 - 1).astype(np.int32)).to(dev)
+
+
+def graph_update_host(host, shape, users, items, values, shape_req=None):
+    """numpy twin of igmc_graph_update_plan + _apply on the host arrays of a graph of ``shape``: (new host arrays,
+    header dict).  Restates the kernels' steps: stable (u, v) order, last entry of a pair kept, classification by
+    binary search in the row, new lengths and pointers from the net counts, merge positions
+    n0 + (j - o0) + (inserted - deleted with a smaller id) for old entries and n0 + q + the same for inserted ones."""
+    users, items, values = (np.asarray(a, np.int64).reshape(-1) for a in (users, items, values))
+    nu, ni = shape
+    rp, ci, rt = (np.asarray(host[k], np.int64) for k in ("row_ptr", "col_idx", "rating"))
+    cp, ri = (np.asarray(host[k], np.int64) for k in ("col_ptr", "row_idx"))
+    D = len(users)
+    req = (0, 0) if shape_req is None else shape_req
+    if D == 0:
+        raise ValueError("the twin models a non-empty delta")
+    o = np.lexsort((items, users))                             # stable
+    su, sv, sx = users[o], items[o], values[o]
+    keep = np.r_[(su[1:] != su[:-1]) | (sv[1:] != sv[:-1]), True]
+    cls = np.zeros(D, np.int64)                                # 0 no-op, 1 insert, 2 change, 3 delete
+    lab = np.zeros(D, np.int64)
+    for i in np.flatnonzero(keep):
+        a, b, x = su[i], sv[i], sx[i]
+        p = -1
+        if a < nu and b < ni:
+            q = rp[a] + np.searchsorted(ci[rp[a]:rp[a + 1]], b)
+            if q < rp[a + 1] and ci[q] == b:
+                p = q
+        if x > 0:
+            lab[i] = x - 1
+            cls[i] = 1 if p < 0 else (2 if rt[p] != x - 1 else 0)
+        elif p >= 0:
+            cls[i] = 3
+    nu2 = max(nu, req[0], int(su.max()) + 1)
+    ni2 = max(ni, req[1], int(sv.max()) + 1)
+    # the column side: the same entries stably ordered by (v, u)
+    oc = np.lexsort((su, sv))
+    new_rp, new_ci, new_rt = _merge_side_host(rp, ci, rt, nu, nu2, su, sv, cls, lab)
+    new_cp, new_ri, _ = _merge_side_host(cp, ri, None, ni, ni2, sv[oc], su[oc], cls[oc], None)
+    nnz = int(new_rp[-1])
+    hdr = dict(nnz=nnz, num_users=nu2, num_items=ni2, max_row_deg=int(np.diff(new_rp).max(initial=0)),
+               max_col_deg=int(np.diff(new_cp).max(initial=0)), inserted=int((cls == 1).sum()),
+               changed=int((cls == 2).sum()), removed=int((cls == 3).sum()))
+    out = dict(row_ptr=new_rp.astype(np.int32), col_idx=new_ci.astype(np.int32), rating=new_rt.astype(np.uint8),
+               col_ptr=new_cp.astype(np.int32), row_idx=new_ri.astype(np.int32))
+    return out, hdr
+
+
+def _merge_side_host(ptr, idx, rating, n_old, n_new, a, b, cls, lab):
+    """one side of the twin: rows r < n_new from the old rows (ptr, idx[, rating]) and the delta entries (a = row,
+    b = other id, ascending (a, b)) classified ``cls``"""
+    pk = np.where(cls == 1, 1, np.where(cls == 3, -1, 0))
+    scan = np.concatenate([[0], np.cumsum(pk)])                 # exclusive net counts, scan[D] = total
+    ds = np.searchsorted(a, np.arange(n_new), "left")
+    de = np.searchsorted(a, np.arange(n_new), "right")
+    old_len = np.zeros(n_new, np.int64)
+    old_len[:n_old] = np.diff(ptr)
+    new_ptr = np.concatenate([[0], np.cumsum(old_len + scan[de] - scan[ds])])
+    optr = np.concatenate([ptr, np.full(n_new - n_old, ptr[-1], np.int64)])    # rows past the old shape: empty
+    M = int(max(idx.max(initial=0), b.max(initial=0))) + 1
+    rows = np.repeat(np.arange(n_old), np.diff(ptr))
+    key_old, key_d = rows * M + idx, a * M + b
+    out_idx = np.full(int(new_ptr[-1]), -1, np.int64)
+    out_rt = np.zeros(int(new_ptr[-1]), np.int64) if rating is not None else None
+    # old entry j: dropped when deleted, else n0 + (j - o0) + net count of the run's entries with a smaller id
+    lo, hi = np.searchsorted(key_d, key_old, "left"), np.searchsorted(key_d, key_old, "right")
+    k = np.where(hi > lo, cls[np.maximum(hi - 1, 0)], 0)
+    j = np.arange(len(idx))
+    dst = new_ptr[rows] + (j - ptr[rows]) + scan[lo] - scan[ds[rows]]
+    live = k != 3
+    out_idx[dst[live]] = idx[live]
+    if rating is not None:
+        out_rt[dst[live]] = np.where(k == 2, lab[np.maximum(hi - 1, 0)], rating)[live]
+    # inserted entry p: n0 + (old entries of the row with a smaller id) + the same count
+    p = np.flatnonzero(cls == 1)
+    r = a[p]
+    q = np.searchsorted(key_old, key_d[p]) - optr[r]
+    dst = new_ptr[r] + q + scan[p] - scan[ds[r]]
+    out_idx[dst] = b[p]
+    if rating is not None:
+        out_rt[dst] = lab[p]
+    assert (out_idx >= 0).all()
+    return new_ptr, out_idx, out_rt
 
 
 class Data(object):
@@ -304,6 +549,7 @@ class SubgraphExtractor(object):
         self.h = int(h)
         self.sample_ratio = float(sample_ratio)
         self.mnph = -1 if max_nodes_per_hop is None else int(max_nodes_per_hop)
+        self._mnph_arg = max_nodes_per_hop
         self.seed = int(seed)
         self.num_links = len(links_u)
         self.links_u = torch.as_tensor(np.asarray(links_u), dtype=torch.int32).to(dev)
@@ -311,6 +557,7 @@ class SubgraphExtractor(object):
         self.links_label = torch.as_tensor(np.asarray(labels), dtype=torch.int32).to(dev)
         self.class_values = torch.as_tensor(np.asarray(class_values, dtype=np.float32)).to(dev)
         self.cap = graph.node_cap(max_nodes_per_hop, self.h)
+        self._graph_version = graph.version
         self.feat_dim = 2 * self.h + 2
         self.emit_x = emit_x
         self.err = torch.zeros(1, dtype=torch.int32, device=dev)   # shared device error word
@@ -318,17 +565,34 @@ class SubgraphExtractor(object):
         self.max_batch = 0
         self._reserve(max_batch)
 
-    def _reserve(self, B):
-        if B <= self.max_batch:
+    def _edges_per_graph(self):
+        g = self.graph
+        return 2 * min(self.cap * min(self.cap, max(g.max_row_deg, 1)), max(g.nnz, 1))
+
+    def _sync_graph(self):
+        """after an update of the graph: re-derive ``cap`` and the edge capacity, and re-reserve the workspace if they
+        grew beyond what it holds (a smaller cap uses the larger buffers as they are)"""
+        g = self.graph
+        if g.version == self._graph_version:
             return
-        dev, cap, g = self.device, self.cap, self.graph
+        self._graph_version = g.version
+        self.cap = g.node_cap(self._mnph_arg, self.h)
+        if self.cap > self._ws_cap or self._edges_per_graph() > self._ws_edges:
+            self._reserve(self.max_batch, regrow=True)
+
+    def _reserve(self, B, regrow=False):
+        if B <= self.max_batch and not regrow:
+            return
+        B = max(B, self.max_batch)
+        dev, cap = self.device, self.cap
         if self.max_batch:
             # captured CUDA graphs hold raw pointers into the workspace of the batch sizes seen so far: keep the old
             # buffers alive instead of handing them back to the allocator
             self.__dict__.setdefault("_retired_ws", []).append((self.ws, self._out_cache))
             self._out_cache = {}
         self.max_batch = B
-        per_graph_edges = 2 * min(cap * min(cap, max(g.max_row_deg, 1)), max(g.nnz, 1))
+        per_graph_edges = self._edges_per_graph()
+        self._ws_cap, self._ws_edges = cap, per_graph_edges
         self.node_cap = B * 2 * cap
         self.edge_cap = max(B * per_graph_edges, 2)
         i32 = dict(dtype=torch.int32, device=dev)
@@ -379,6 +643,7 @@ class SubgraphExtractor(object):
         the previous batch of that size is overwritten).  ``seed_dev``: device uint64 overriding the seed.
         Returns a ``Batch`` whose public tensors are materialised lazily."""
         dev = self.device
+        self._sync_graph()
         keep = []
         if pairs is not None:
             # (device tensors of the right type are used in place: the inference engine's candidate buffers, read by
@@ -499,9 +764,10 @@ class MyDynamicDataset(object):
     def pair_cost(self):
         """a-priori size estimate of every pair's subgraph from the matrix degrees alone (hop 1: raters of the item
         + items of the user, each capped by max_nodes_per_hop): what the data-parallel sharding balances the ranks'
-        batches by (train_eval.deal_balanced).  Host arrays, computed once."""
+        batches by (train_eval.deal_balanced).  Host arrays, computed once per version of the graph."""
         c = getattr(self, "_pair_cost", None)
-        if c is None:
+        if c is None or self._pair_cost_version != self.graph.version:
+            self._pair_cost_version = self.graph.version
             h = self.graph.host
             du, dv = np.diff(h["row_ptr"]), np.diff(h["col_ptr"])
             cap = self.max_nodes_per_hop if self.max_nodes_per_hop is not None else (1 << 30)

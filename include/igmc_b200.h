@@ -451,6 +451,43 @@ int igmc_topk_merge(const float* preds, int K, int B, const int64_t* tag, const 
 /* Explicit pairs: scores[tag[i]] = the same fp32 checkpoint mean for every i with tag[i] >= 0. */
 int igmc_score_scatter(const float* preds, int K, int B, const int64_t* tag, float* scores, void* stream);
 
+/* ---- in-place update of the rating graph (csrc/graph_update.cu) ----
+ * The reference can only change its rating matrix by rebuilding everything from a new scipy matrix.  Here a delta of D
+ * entries (users[i], items[i], values[i]) is applied to the graph's own device arrays; value = rating label + 1 (1..256)
+ * inserts the rating or overwrites it, 0 deletes it (absent: nothing happens); within one call the last occurrence of a
+ * pair wins.  The graph's arrays are allocated at capacity (cap_users + 1 / cap_items + 1 pointers, cap_nnz entries);
+ * G describes the current shape and `nnz` its current entry count.  Afterwards the arrays are byte-identical, up to the
+ * new nnz and shape, to a graph built from the updated matrix (CSR columns and CSC rows ascending), and the five
+ * pointers are unchanged.  Ids below the capacity grow the shape to cover every id of the call; the shape never
+ * shrinks.  The update is two calls with one host synchronisation between them (reading the header). */
+typedef struct {
+  int64_t nnz;                     /* entries after the update */
+  int64_t num_users, num_items;    /* shape after the update */
+  int64_t max_row_deg, max_col_deg;
+  int64_t inserted, changed, removed;   /* kept entries that insert / change a label / delete; the rest change nothing */
+  int32_t status;                  /* 0, or IGMC_GRAPH_UPDATE_OVER_CAPACITY / _OVER_INT32: apply must not run */
+  int32_t err;                     /* the error word as the plan left it (IGMC_ERR_GRAPH_UPDATE: invalid delta) */
+} igmc_graph_update_header_t;
+#define IGMC_GRAPH_UPDATE_OVER_CAPACITY 1   /* new nnz > cap_nnz */
+#define IGMC_GRAPH_UPDATE_OVER_INT32 2      /* new nnz beyond int32 */
+
+/* Bytes of the workspace plan and apply share for a delta of D entries at these capacities. */
+int igmc_graph_update_ws_bytes(int D, int cap_users, int cap_items, int cap_nnz, int64_t* bytes);
+
+/* Validate (ids in [0, cap), values 0..256, else IGMC_ERR_GRAPH_UPDATE in `err`), order and classify the delta and
+ * compute the new row_ptr / col_ptr into the workspace and the header (device).  `shape_users` / `shape_items`: the
+ * least shape the call asks for (0 = none).  Changes nothing in G. */
+int igmc_graph_update_plan(const igmc_csr_t* G, int nnz, int cap_users, int cap_items, int cap_nnz,
+                           const int32_t* users, const int32_t* items, const int32_t* values, int D,
+                           int shape_users, int shape_items, void* ws, int64_t ws_bytes,
+                           igmc_graph_update_header_t* header, int* err, void* stream);
+
+/* Merge the planned delta into G's arrays, written THROUGH G's pointers (they must be the graph's writable buffers).
+ * Same G, nnz, capacities, D and workspace as the plan; new_nnz / new_users / new_items from its header, which must
+ * report status 0 and err 0. */
+int igmc_graph_update_apply(const igmc_csr_t* G, int nnz, int cap_users, int cap_items, int cap_nnz, int D,
+                            void* ws, int64_t ws_bytes, int new_nnz, int new_users, int new_items, void* stream);
+
 /* Version / build info: returns the compiled SM arch (90) so the host can refuse stale builds. */
 int igmc_build_info(void);
 
