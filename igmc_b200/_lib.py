@@ -222,6 +222,12 @@ def check(rc, what):
         raise RuntimeError("igmc_b200: %s failed with code %d" % (what, rc))
 
 
+def check_kernel_error(code):
+    """raise for a nonzero code read from a kernel error word (the caller reads, and if it wants clears, the word)"""
+    if code:
+        raise RuntimeError("igmc_b200 kernel error %d: %s" % (code, ERR_NAMES.get(code, "?")))
+
+
 def ptr(t):
     """device address of a torch tensor (or None -> NULL)."""
     return None if t is None else t.data_ptr()

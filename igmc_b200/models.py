@@ -107,19 +107,36 @@ def select_plan(cmodel, n_cap, B, sms, want="auto", max_edges=None):
                        % (n_cap, R, _lib.L2_MAX_NODES))
 
 
-class RGCNConv(nn.Module):
-    """Parameter holder with PyG 1.4.2 ``RGCNConv`` names/shapes/init (SURVEY.md A.1).  The arithmetic
-    lives in the fused kernels of the owning ``IGMC``."""
+class _RGCNParams(nn.Module):
+    """Sizes, parameters and ``repr`` of an RGCNConv parameter holder.  The arithmetic lives in the fused kernels of
+    the owning ``IGMC``.  ``NAMES``: the subclass's names of its [NB,in,out], [R,NB], [in,out] and [out] parameters, in
+    the order they are registered (the order of ``parameters()``, which optimizer state_dicts are indexed by)."""
+
+    NAMES = ()
 
     def __init__(self, in_channels, out_channels, num_relations, num_bases):
         super().__init__()
         self.in_channels, self.out_channels = in_channels, out_channels
         self.num_relations, self.num_bases = num_relations, num_bases
-        self.basis = nn.Parameter(torch.empty(num_bases, in_channels, out_channels))
-        self.att = nn.Parameter(torch.empty(num_relations, num_bases))
-        self.root = nn.Parameter(torch.empty(in_channels, out_channels))
-        self.bias = nn.Parameter(torch.empty(out_channels))
+        shapes = ((num_bases, in_channels, out_channels), (num_relations, num_bases), (in_channels, out_channels),
+                  (out_channels,))
+        for name, shape in zip(self.NAMES, shapes):
+            setattr(self, name, nn.Parameter(torch.empty(*shape)))
         self.reset_parameters()
+
+    def att_basis(self):
+        """(coefficients [R,NB], bases [NB,in,out]) of W_r = sum_b att[r,b] basis[b]"""
+        return getattr(self, self.NAMES[1]), getattr(self, self.NAMES[0])
+
+    def __repr__(self):
+        return "RGCNConv(%d, %d, num_relations=%d, num_bases=%d)" % (
+            self.in_channels, self.out_channels, self.num_relations, self.num_bases)
+
+
+class RGCNConv(_RGCNParams):
+    """Parameter holder with PyG 1.4.2 ``RGCNConv`` names/shapes/init (SURVEY.md A.1)."""
+
+    NAMES = ("basis", "att", "root", "bias")
 
     def reset_parameters(self):
         bound = 1.0 / math.sqrt(self.num_bases * self.in_channels)   # PyG inits.uniform(size, tensor)
@@ -127,30 +144,14 @@ class RGCNConv(nn.Module):
             for p in (self.basis, self.att, self.root, self.bias):
                 p.uniform_(-bound, bound)
 
-    def att_basis(self):
-        """(coefficients [R,NB], bases [NB,in,out]) of W_r = sum_b att[r,b] basis[b]"""
-        return self.att, self.basis
 
-    def __repr__(self):
-        return "RGCNConv(%d, %d, num_relations=%d, num_bases=%d)" % (
-            self.in_channels, self.out_channels, self.num_relations, self.num_bases)
-
-
-class RGCNConv2(nn.Module):
+class RGCNConv2(_RGCNParams):
     """Parameter holder with the names/shapes/init of PyG >= 1.6 ``RGCNConv(in, out, num_relations, num_bases)``:
     ``weight [NB,in,out]``, ``comp [R,NB]``, ``root [in,out]``, ``bias [out]``; glorot(weight, comp, root), zeros(bias)
     (PyG 2.x ``reset_parameters``).  W_r = sum_b comp[r,b] weight[b] - the 1.4.2 layer's ``att @ basis`` - but the
     aggregation is a mean PER RELATION (``IGMC(..., rgcn="pyg-2")``; DESIGN.md §2)."""
 
-    def __init__(self, in_channels, out_channels, num_relations, num_bases):
-        super().__init__()
-        self.in_channels, self.out_channels = in_channels, out_channels
-        self.num_relations, self.num_bases = num_relations, num_bases
-        self.weight = nn.Parameter(torch.empty(num_bases, in_channels, out_channels))
-        self.comp = nn.Parameter(torch.empty(num_relations, num_bases))
-        self.root = nn.Parameter(torch.empty(in_channels, out_channels))
-        self.bias = nn.Parameter(torch.empty(out_channels))
-        self.reset_parameters()
+    NAMES = ("weight", "comp", "root", "bias")
 
     def reset_parameters(self):
         with torch.no_grad():
@@ -158,13 +159,6 @@ class RGCNConv2(nn.Module):
                 bound = math.sqrt(6.0 / (p.size(-2) + p.size(-1)))
                 p.uniform_(-bound, bound)
             self.bias.zero_()
-
-    def att_basis(self):
-        return self.comp, self.weight
-
-    def __repr__(self):
-        return "RGCNConv(%d, %d, num_relations=%d, num_bases=%d)" % (
-            self.in_channels, self.out_channels, self.num_relations, self.num_bases)
 
 
 # rgcn= keyword of IGMC / DGCNN_RS: which RGCNConv the model is (names, init and aggregation go together)
@@ -200,20 +194,35 @@ class _IGMCFunction(torch.autograd.Function):
 
 
 class IGMC(nn.Module):
+    REGRESSION_ONLY = "igmc_b200.IGMC implements the regression head Main.py uses (Main.py:396)"
+
     def __init__(self, dataset, gconv=RGCNConv, latent_dim=[32, 32, 32, 32], num_relations=5, num_bases=2,
                  regression=False, adj_dropout=0.2, force_undirected=False, side_features=False,
                  n_side_features=0, multiply_by=1, rgcn="pyg-1.4"):
         super().__init__()
+        self._init_convs(dataset, latent_dim, num_relations, num_bases, regression, adj_dropout, force_undirected,
+                         side_features, multiply_by, rgcn)
+        self.lin1 = nn.Linear(2 * sum(latent_dim), 128)
+        self.lin2 = nn.Linear(128, 1)
+        self._init_bucket()
+
+    @staticmethod
+    def _check_latent_dim(latent_dim):
+        if any(int(d) != HID for d in latent_dim) or not (1 <= len(latent_dim) <= _lib.MAX_LAYERS):
+            raise NotImplementedError("latent_dim entries must be 32 (Main.py:391 hard-codes [32,32,32,32])")
+
+    def _init_convs(self, dataset, latent_dim, num_relations, num_bases, regression, adj_dropout, force_undirected,
+                    side_features, multiply_by, rgcn):
+        """the constructor part IGMC and DGCNN_RS share: argument checks, node feature width and the conv stack"""
         conv_cls = _rgcn_layer(rgcn)
         self.rgcn = rgcn
         if not regression:
-            raise NotImplementedError("igmc_b200.IGMC implements the regression head Main.py uses (Main.py:396)")
+            raise NotImplementedError(self.REGRESSION_ONLY)
         if force_undirected:
             raise NotImplementedError("force_undirected edge dropout is not on the hot path")
         if side_features:
             raise NotImplementedError("side features are outside the hot path (SURVEY.md §2)")
-        if any(int(d) != HID for d in latent_dim) or not (1 <= len(latent_dim) <= _lib.MAX_LAYERS):
-            raise NotImplementedError("latent_dim entries must be 32 (Main.py:391 hard-codes [32,32,32,32])")
+        self._check_latent_dim(latent_dim)
         if num_bases not in (2, 4):
             raise NotImplementedError("num_bases must be 2 or 4")
         self.regression, self.adj_dropout, self.force_undirected = regression, adj_dropout, force_undirected
@@ -226,12 +235,15 @@ class IGMC(nn.Module):
         dims = [self.num_features] + [int(d) for d in latent_dim]
         self.convs = nn.ModuleList([conv_cls(dims[l], dims[l + 1], num_relations, num_bases)
                                     for l in range(len(latent_dim))])
-        self.lin1 = nn.Linear(2 * sum(latent_dim), 128)
-        self.lin2 = nn.Linear(128, 1)
+
+    def _init_bucket(self):
         self.drop_seed = 0x1234ABCD
         self._step = 0
-        self._ws = {}
         self._flatten()
+
+    def _readout(self):
+        """(bucket name prefix, module) of the layers after the convs, in bucket order"""
+        return (("lin1", self.lin1), ("lin2", self.lin2))
 
     # ---- flat parameter bucket ---------------------------------------------------------------------
     def _named_order(self):
@@ -241,10 +253,9 @@ class IGMC(nn.Module):
             yield ("basis", l, basis)
             yield ("root", l, c.root)
             yield ("bias", l, c.bias)
-        yield ("lin1_w", 0, self.lin1.weight)
-        yield ("lin1_b", 0, self.lin1.bias)
-        yield ("lin2_w", 0, self.lin2.weight)
-        yield ("lin2_b", 0, self.lin2.bias)
+        for name, mod in self._readout():
+            yield (name + "_w", 0, mod.weight)
+            yield (name + "_b", 0, mod.bias)
 
     def _slot(self, kind, l, p):
         """(floats reserved in the bucket, padded shape or None) of one parameter."""
@@ -326,8 +337,8 @@ class IGMC(nn.Module):
     def reset_parameters(self):
         for c in self.convs:
             c.reset_parameters()
-        self.lin1.reset_parameters()
-        self.lin2.reset_parameters()
+        for _, mod in self._readout():
+            mod.reset_parameters()
 
     # ---- kernel launches ---------------------------------------------------------------------------------
     kernel_plan = "auto"   # "auto" | 0 (generic kernels) | 1 | 2 | 3 | 4 (relation-space kernels, CTAs per subgraph)
@@ -452,6 +463,12 @@ class IGMC(nn.Module):
                           _lib.ptr(self._gate) if (rs and self.__dict__.pop("_gate_armed", False)) else None,
                           _lib.ptr(ws.get("l2_scratch")), _lib.ptr(ws.get("rel_inv_deg")))
 
+    def _prep_weights_unless_prepped(self):
+        """W_r / W_r^T of the current parameters (one tiny launch per step), unless ``prep_weights(mark=True)`` or the
+        update kernel has just written them"""
+        if not self.__dict__.pop("_prepped", False):
+            self.prep_weights()
+
     def prep_weights(self, mark=False):
         """launch igmc_prep_weights on the current stream; ``mark`` lets the next forward skip its own launch (the
         train engine issues it early so that the extraction branch of the step can be ordered after it)."""
@@ -508,9 +525,8 @@ class IGMC(nn.Module):
         ws = self._workspace(batch, training)
         S = self._saved_struct(ws, p["node_cap"])
         d, keep = drop
-        if _lib.is_rs(ws["cluster"]) and not self.__dict__.pop("_prepped", False):
-            # W_r / W_r^T of the current parameters (one tiny launch per step, unless prep_weights() just ran)
-            self.prep_weights()
+        if _lib.is_rs(ws["cluster"]):
+            self._prep_weights_unless_prepped()
         _lib.check(lib.igmc_forward(C.byref(self._cmodel), self.flat_params.data_ptr(), p["node_label"].data_ptr(),
                                     p["node_ptr"].data_ptr(), p["edge_ptr"].data_ptr(), C.byref(adj_c),
                                     batch.num_graphs, p["n_cap"], C.byref(d), int(training), C.byref(S),
@@ -587,8 +603,7 @@ class IGMC(nn.Module):
         ws = self._workspace(batch, True)
         S = self._saved_struct(ws, p["node_cap"])
         d, keep = drop
-        if not self.__dict__.pop("_prepped", False):
-            self.prep_weights()
+        self._prep_weights_unless_prepped()
         _lib.check(lib.igmc_forward_backward(C.byref(self._cmodel), self.flat_params.data_ptr(),
                                              p["node_label"].data_ptr(), p["node_ptr"].data_ptr(),
                                              p["edge_ptr"].data_ptr(), C.byref(adj_c), batch.num_graphs, p["n_cap"],
@@ -640,28 +655,14 @@ class DGCNN_RS(IGMC):
     """
 
     C1, C2, KW2 = 16, 32, 5   # conv1d_channels and the second kernel width (models.py:75-79)
+    REGRESSION_ONLY = "igmc_b200.DGCNN_RS implements the regression head (x[:, 0], models.py:165)"
 
     def __init__(self, dataset, gconv=RGCNConv, latent_dim=[32, 32, 32, 1], k=30, num_relations=5, num_bases=2,
                  regression=False, adj_dropout=0.2, force_undirected=False, rgcn="pyg-1.4"):
         nn.Module.__init__(self)
-        conv_cls = _rgcn_layer(rgcn)
-        self.rgcn = rgcn
-        if not regression:
-            raise NotImplementedError("igmc_b200.DGCNN_RS implements the regression head (x[:, 0], models.py:165)")
-        if force_undirected:
-            raise NotImplementedError("force_undirected edge dropout is not on the hot path")
         latent_dim = [int(d) for d in latent_dim]
-        if not (1 <= len(latent_dim) <= _lib.MAX_LAYERS) or any(d != HID for d in latent_dim[:-1]) \
-                or not (1 <= latent_dim[-1] <= HID):
-            raise NotImplementedError("latent_dim must be [32, ..., 32, d] with 1 <= d <= 32")
-        if num_bases not in (2, 4):
-            raise NotImplementedError("num_bases must be 2 or 4")
-        self.regression, self.adj_dropout, self.force_undirected = regression, adj_dropout, force_undirected
-        self.side_features, self.multiply_by = False, 1
-        num_features = dataset if isinstance(dataset, int) else dataset.num_features
-        self.num_features = int(num_features)
-        if self.num_features > HID:
-            raise NotImplementedError("node feature width > 32")
+        self._init_convs(dataset, latent_dim, num_relations, num_bases, regression, adj_dropout, force_undirected,
+                         False, 1, rgcn)
         if k < 1:   # transform percentile to number (models.py:69-73)
             if isinstance(dataset, int):
                 raise ValueError("a percentile k needs the dataset")
@@ -672,11 +673,7 @@ class DGCNN_RS(IGMC):
             k = node_nums[int(math.ceil(k * len(node_nums))) - 1]
             k = max(10, k)
         self.k = int(k)
-        self.num_relations, self.num_bases = int(num_relations), int(num_bases)
         self.latent_dim = latent_dim
-        dims = [self.num_features] + latent_dim
-        self.convs = nn.ModuleList([conv_cls(dims[l], dims[l + 1], num_relations, num_bases)
-                                    for l in range(len(latent_dim))])
         self.total_latent_dim = sum(latent_dim)
         self.conv1d_params1 = nn.Conv1d(1, self.C1, self.total_latent_dim, self.total_latent_dim)
         self.maxpool1d = nn.MaxPool1d(2, 2)
@@ -687,26 +684,17 @@ class DGCNN_RS(IGMC):
             raise ValueError("k = %d is too small for the 1-D convolutions" % self.k)
         self.lin1 = nn.Linear(self.dense_dim, 128)
         self.lin2 = nn.Linear(128, 1)
-        self.drop_seed = 0x1234ABCD
-        self._step = 0
-        self._ws = {}
-        self._flatten()
+        self._init_bucket()
 
-    def _named_order(self):
-        for l, c in enumerate(self.convs):
-            att, basis = c.att_basis()
-            yield ("att", l, att)
-            yield ("basis", l, basis)
-            yield ("root", l, c.root)
-            yield ("bias", l, c.bias)
-        yield ("conv1_w", 0, self.conv1d_params1.weight)
-        yield ("conv1_b", 0, self.conv1d_params1.bias)
-        yield ("conv2_w", 0, self.conv1d_params2.weight)
-        yield ("conv2_b", 0, self.conv1d_params2.bias)
-        yield ("lin1_w", 0, self.lin1.weight)
-        yield ("lin1_b", 0, self.lin1.bias)
-        yield ("lin2_w", 0, self.lin2.weight)
-        yield ("lin2_b", 0, self.lin2.bias)
+    @staticmethod
+    def _check_latent_dim(latent_dim):
+        if not (1 <= len(latent_dim) <= _lib.MAX_LAYERS) or any(d != HID for d in latent_dim[:-1]) \
+                or not (1 <= latent_dim[-1] <= HID):
+            raise NotImplementedError("latent_dim must be [32, ..., 32, d] with 1 <= d <= 32")
+
+    def _readout(self):
+        return (("conv1", self.conv1d_params1), ("conv2", self.conv1d_params2), ("lin1", self.lin1),
+                ("lin2", self.lin2))
 
     def _slot(self, kind, l, p):
         if kind in ("basis", "root", "bias") and p.shape[-1] != HID:
@@ -729,14 +717,6 @@ class DGCNN_RS(IGMC):
         sp.off_lin1_w, sp.off_lin1_b, sp.off_lin2_w, sp.off_lin2_b = o["lin1_w"], o["lin1_b"], o["lin2_w"], o["lin2_b"]
         sp.param_begin, sp.param_end = self._cmodel.conv_param_count, self._cmodel.param_count
         self._csort = sp
-
-    def reset_parameters(self):
-        for c in self.convs:
-            c.reset_parameters()
-        self.conv1d_params1.reset_parameters()
-        self.conv1d_params2.reset_parameters()
-        self.lin1.reset_parameters()
-        self.lin2.reset_parameters()
 
     def _workspace(self, batch, train):
         ws = super()._workspace(batch, train)

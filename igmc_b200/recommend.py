@@ -25,6 +25,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .train_eval import replay_step
 from .util_functions import RatingGraph, SubgraphExtractor, _stream_ptr
 
 __all__ = ["predict_pairs", "recommend", "InferenceEngine"]
@@ -350,17 +351,7 @@ class InferenceEngine(object):
             raise RuntimeError("the rating graph was updated during this run: its candidates and captured steps belong "
                                "to the old graph; start the run again")
         slot = run["done"] & 1
-        if self.use_graph and slot in self.graphs:
-            self.graphs[slot].replay()
-        elif self.use_graph and slot in self.eager_done:
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self._launch(slot)
-            self.graphs[slot] = g
-            g.replay()
-        else:
-            self._launch(slot)
-            self.eager_done.add(slot)
+        replay_step(self.graphs, self.eager_done, slot, lambda: self._launch(slot), self.use_graph)
         run["done"] += 1
         return run["done"] < run["steps"]
 
@@ -373,7 +364,7 @@ class InferenceEngine(object):
         code = int(self.extractor.err.item())
         if code:
             self.extractor.err.zero_()
-            raise RuntimeError("igmc_b200 kernel error %d: %s" % (code, _lib.ERR_NAMES.get(code, "?")))
+        _lib.check_kernel_error(code)
         self.run = None
         if run["kind"] == "recommend":
             return run["top_i"], run["top_s"]

@@ -20,8 +20,9 @@ import time
 import numpy as np
 import torch
 
+from . import _lib
 from .models import FusedAdam, splitmix64
-from .util_functions import MyDynamicDataset  # noqa: F401  (re-export, Main.py star-imports)
+from .util_functions import DevView, MyDynamicDataset  # noqa: F401  (re-export, Main.py star-imports)
 
 try:
     import torch.distributed as dist
@@ -77,6 +78,26 @@ def shard_batches(perm, batch_size, rank, world, cost=None):
     return out
 
 
+def replay_step(graphs, warm, key, launch, use_graph=True, capture=True):
+    """Run one step, ``launch()``, whose launches depend only on ``key``: eagerly the first time ``key`` is seen (plans,
+    workspaces and their host syncs happen outside a capture), captured into a CUDA graph and replayed the second
+    time, replayed from then on.  ``graphs``: key -> captured graph; ``warm``: keys that ran eagerly; ``capture=False``
+    runs the step eagerly again.  Returns True when this call captured the graph."""
+    if use_graph and key in graphs:
+        graphs[key].replay()
+        return False
+    if use_graph and capture and key in warm:
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            launch()
+        graphs[key] = g
+        g.replay()
+        return True
+    launch()
+    warm.add(key)
+    return False
+
+
 def _u64_as_i64(x):
     x &= (1 << 64) - 1
     return x - (1 << 64) if x >= (1 << 63) else x
@@ -93,7 +114,10 @@ class TrainEngine(object):
         self.B, self.ARR = int(batch_size), float(ARR)
         self.rank, self.world = _dist_info()
         self.dev = model.flat_params.device
-        self.use_graph = bool(use_graph) and hasattr(dataset, "extractor") and not hasattr(dataset, "slices")
+        # a dataset with an extractor trains through the pipelined, graph-replayed step; one that carries PyG's
+        # ``slices`` through an eager step per batch
+        self._pipelined = hasattr(dataset, "extractor") and not hasattr(dataset, "slices")
+        self.use_graph = bool(use_graph) and self._pipelined
         self.sample_seed = int(sample_seed)
         self.graphs = {}
         self.graph_loss = {}      # loss tensor each captured step writes (a replay runs no Python: last_loss is set here)
@@ -117,14 +141,13 @@ class TrainEngine(object):
         # operation between two graph replays (the two per-step memcpys serialise with the step's kernels)
         self.zero_copy = self.dev.type == "cuda" and os.environ.get("IGMC_ZERO_COPY", "1") != "0"
         if self.zero_copy:
-            from .util_functions import mapped_view
             self.hostbuf = [torch.zeros(self.B + 4, dtype=torch.int64).pin_memory() for _ in range(2)]
             self.hostbuf_np = [t.numpy() for t in self.hostbuf]
-            self.hostview = [mapped_view(t) for t in self.hostbuf]
+            self.hostview = [DevView(t) for t in self.hostbuf]
             self.slot_ev = [torch.cuda.Event() for _ in range(2)]
             self.slot_used = [False, False]
             self.loss_ring = torch.zeros(self.LOSS_RING, dtype=torch.float32).pin_memory()
-            self.loss_ring_view = mapped_view(self.loss_ring)
+            self.loss_ring_view = DevView(self.loss_ring)
         self._adam_base = None    # Adam step number before this engine's first update (index base of the loss ring)
         self._updates = 0
         self.exchange = None      # peer-mapped gradient buffers of the fused update kernel (created on first use)
@@ -217,32 +240,28 @@ class TrainEngine(object):
             raise RuntimeError("the rating graph was updated after this TrainEngine's first step; training on a "
                                "changing graph is not supported (build a new engine)")
 
+    def _replay(self, key, launch, capture=True):
+        """one step through ``replay_step``; a replay runs no Python, so last_loss is set to the loss tensor the
+        captured launches write"""
+        if replay_step(self.graphs, self.eager_done, key, launch, self.use_graph, capture):
+            self.graph_loss[key] = self.last_loss
+        elif key in self.graphs:
+            self.last_loss = self.graph_loss[key]
+
     def step(self, idx, epoch=0, G=None, staged=False):
         """One optimisation step on this rank's ``idx`` (host int array).  H2D copy + graph replay."""
         self._check_graph()
         G = len(idx) * self.world if G is None else int(G)
         self.steps += 1
-        if not hasattr(self.dataset, "extractor") or hasattr(self.dataset, "slices"):
+        if not self._pipelined:
             return self._launch_static(np.asarray(idx), G)
         nb = len(idx) if staged else self.stage(idx, epoch, G)
-        key = (nb, G)
-        if self.use_graph and key in self.graphs:
-            self.graphs[key].replay()
-            self.last_loss = self.graph_loss[key]
-        elif self.use_graph and key in self.eager_done and nb > 0:
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self._launch(nb, G)
-            self.graphs[key], self.graph_loss[key] = g, self.last_loss
-            g.replay()
-        else:
-            self._launch(nb, G)
-            self.eager_done.add(key)
+        self._replay((nb, G), lambda: self._launch(nb, G), capture=nb > 0)
 
     # ---- software pipeline: extract batch k+1 on a side stream while the model trains on batch k ------------
     # (what the reference's DataLoader workers do, train_eval.py:40-45, as two branches of one CUDA graph)
     def pipelined(self):
-        return hasattr(self.dataset, "extractor") and not hasattr(self.dataset, "slices")
+        return self._pipelined
 
     def loss_of_update(self, k):
         """loss of this engine's k-th update (0-based) read from the pinned ring; valid after the step has finished
@@ -266,8 +285,15 @@ class TrainEngine(object):
         h[B + 3] = nxt
         return nb
 
-    def _launch_pipe(self, nb, G, slot, nb_next, buf=None):
+    def _extract(self, slot, nb, buf):
+        """extract the ``nb`` indices of step inputs ``buf`` into batch slot ``slot`` and stage its edge lists with the
+        dropout draws of the step that trains on it (seed at buf[B + 3])"""
         B = self.B
+        self.batches[slot] = self.dataset.extractor.extract(idx=buf[:nb], seed_dev=buf[B:B + 1], reuse=True, slot=slot)
+        self.model.stage_batch(self.batches[slot], True, self.model.make_dropout(True, seed_dev=buf[B + 3:B + 4]),
+                               slot=slot)
+
+    def _launch_pipe(self, nb, G, slot, nb_next, buf=None):
         buf = self.stepbuf_dev if buf is None else buf
         main = torch.cuda.current_stream()
         if nb_next > 0:
@@ -279,12 +305,8 @@ class TrainEngine(object):
                     # spread one per SM and can push the last clusters into a second wave.  Started behind the forward
                     # they pack two per SM on the SMs that are left.
                     self.model.gate_wait(self.batches[slot])
-                self.batches[slot ^ 1] = self.dataset.extractor.extract(idx=buf[:nb_next], seed_dev=buf[B:B + 1],
-                                                                        reuse=True, slot=slot ^ 1)
-                # the next step's edge lists (after its dropout draws), staged for the model kernels' bulk loads
-                self.model.stage_batch(self.batches[slot ^ 1], True,
-                                       self.model.make_dropout(True, seed_dev=buf[B + 3:B + 4]), slot=slot ^ 1)
-        self._model_step(self.batches[slot] if nb > 0 else None, nb, G, buf[B + 1:B + 2])
+                self._extract(slot ^ 1, nb_next, buf)
+        self._model_step(self.batches[slot] if nb > 0 else None, nb, G, buf[self.B + 1:self.B + 2])
         if nb_next > 0:
             main.wait_stream(self.side)
 
@@ -298,12 +320,7 @@ class TrainEngine(object):
         nb = self.stage(idx, epoch, G)
         self.slot = 0
         if nb > 0:
-            self.batches[0] = self.dataset.extractor.extract(idx=self.stepbuf_dev[:nb],
-                                                             seed_dev=self.stepbuf_dev[self.B:self.B + 1], reuse=True,
-                                                             slot=0)
-            self.model.stage_batch(self.batches[0], True,
-                                   self.model.make_dropout(True, seed_dev=self.stepbuf_dev[self.B + 3:self.B + 4]),
-                                   slot=0)
+            self._extract(0, nb, self.stepbuf_dev)
         self.cur = (nb, G)
 
     def step_pipe(self, next_idx=None, epoch=0, next_G=None, staged=False):
@@ -331,19 +348,8 @@ class TrainEngine(object):
             nb_next = self.stage(next_idx, epoch, next_G)
         else:
             self.stage(np.zeros(0, np.int64), epoch, 0)    # still refresh the dropout seed of this step
-        key = (nb, G, self.slot, nb_next, zc)
-        if self.use_graph and key in self.graphs:
-            self.graphs[key].replay()
-            self.last_loss = self.graph_loss[key]
-        elif self.use_graph and key in self.eager_done:
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self._launch_pipe(nb, G, self.slot, nb_next, buf)
-            self.graphs[key], self.graph_loss[key] = g, self.last_loss
-            g.replay()
-        else:
-            self._launch_pipe(nb, G, self.slot, nb_next, buf)
-            self.eager_done.add(key)
+        slot = self.slot
+        self._replay((nb, G, slot, nb_next, zc), lambda: self._launch_pipe(nb, G, slot, nb_next, buf))
         if zc:
             self.slot_ev[self.slot].record()
             self.slot_used[self.slot] = True
@@ -362,10 +368,7 @@ class TrainEngine(object):
             self.exchange = None
 
     def check(self):
-        code = int(self.dataset.extractor.err.item()) if hasattr(self.dataset, "extractor") else 0
-        if code:
-            from . import _lib
-            raise RuntimeError("igmc_b200 kernel error %d: %s" % (code, _lib.ERR_NAMES.get(code, "?")))
+        _check_dataset(self.dataset)
 
 
 def train_multiple_epochs(train_dataset, test_dataset, model, epochs, batch_size, lr, lr_decay_factor,
@@ -471,13 +474,10 @@ def _eval_sqerr_sum(model, dataset, batch_size):
 
 
 def _check_dataset(dataset):
-    ex = getattr(dataset, "extractor", None)
-    err = getattr(ex, "err", None)
+    """raise if a kernel flagged an error in the error word of the dataset's extractor (host sync)"""
+    err = getattr(getattr(dataset, "extractor", None), "err", None)
     if err is not None:
-        code = int(err.item())
-        if code:
-            from . import _lib
-            raise RuntimeError("igmc_b200 kernel error %d: %s" % (code, _lib.ERR_NAMES.get(code, "?")))
+        _lib.check_kernel_error(int(err.item()))
 
 
 def eval_loss(model, loader, device, regression=False, show_progress=False, batch_size=50):

@@ -65,8 +65,13 @@ class DevView(object):
         return DevView(self.pinned, self.off + lo, max(0, hi - lo))
 
 
-def mapped_view(pinned):
-    return DevView(pinned)
+def _device_index(idx, dev):
+    """dataset indices as an int64 device tensor; a ``DevView`` (int64 indices in mapped host memory) is used as is"""
+    if isinstance(idx, DevView):
+        return idx
+    if not torch.is_tensor(idx):
+        idx = torch.as_tensor(np.asarray(idx), dtype=torch.int64)
+    return idx.to(device=dev, dtype=torch.int64)
 
 
 GraphCapacity = collections.namedtuple("GraphCapacity", "users items nnz")
@@ -204,7 +209,7 @@ class RatingGraph(object):
         status, err = (int(a) for a in hdr[-1:].view(np.int32))
         if err:
             w["err"].zero_()
-            raise RuntimeError("igmc_b200 kernel error %d: %s" % (err, _lib.ERR_NAMES.get(err, "?")))
+        _lib.check_kernel_error(err)
         if status:
             raise ValueError("the update would leave %d ratings, beyond the graph's capacity of %d%s (reserve_nnz "
                              "makes room)" % (h["nnz"], cn, " and int32" if status == _lib.GRAPH_UPDATE_OVER_INT32
@@ -432,9 +437,7 @@ class Batch(Data):
     def check(self):
         """raise if a kernel flagged a data-dependent error (host sync)."""
         if self._err is not None:
-            code = int(self._err.item())
-            if code != 0:
-                raise RuntimeError("igmc_b200 kernel error %d: %s" % (code, _lib.ERR_NAMES.get(code, "?")))
+            _lib.check_kernel_error(int(self._err.item()))
 
     def to(self, device):
         device = torch.device(device)
@@ -528,7 +531,65 @@ class Batch(Data):
         return self._adj
 
 
-class SubgraphExtractor(object):
+class _BatchWriter(object):
+    """Output side of ``SubgraphExtractor`` and ``StaticStore``, so that the train engine treats both alike: the
+    capacity-sized buffers a batch kernel writes (one cached set per (batch size, slot) with ``reuse``), the
+    ``BatchOut`` struct that points at them and the ``Batch`` that wraps them.  A subclass sets ``device``,
+    ``feat_dim``, ``emit_x``, ``cap``, ``err`` and ``_out_cache`` and defines ``_out_caps(B)``."""
+
+    def _out_caps(self, B):
+        """(node capacity, edge capacity, length of adj_tmp) of a batch of ``B`` subgraphs"""
+        raise NotImplementedError
+
+    def _alloc_out(self, B, reuse=False, slot=0):
+        if reuse and (B, slot) in self._out_cache:
+            return self._out_cache[(B, slot)]
+        dev = self.device
+        ncap, ecap, tmp = self._out_caps(B)
+        o = dict(x=torch.empty(ncap, self.feat_dim, dtype=torch.float32, device=dev) if self.emit_x else None,
+                 node_label=torch.empty(ncap, dtype=torch.uint8, device=dev),
+                 batch=torch.empty(ncap, dtype=torch.int64, device=dev),
+                 node_gid=torch.empty(ncap, dtype=torch.int32, device=dev),
+                 edge_index=torch.empty(2, ecap, dtype=torch.int64, device=dev),
+                 edge_type=torch.empty(ecap, dtype=torch.int64, device=dev),
+                 y=torch.empty(B, dtype=torch.float32, device=dev),
+                 node_ptr=torch.zeros(B + 1, dtype=torch.int32, device=dev),
+                 edge_ptr=torch.zeros(B + 1, dtype=torch.int32, device=dev),
+                 graph_nu=torch.zeros(B, dtype=torch.int32, device=dev),
+                 counts=torch.zeros(2, dtype=torch.int32, device=dev),
+                 adj_in_ptr=torch.zeros(ncap + 1, dtype=torch.int32, device=dev),
+                 adj_in=torch.empty(ecap, dtype=torch.int32, device=dev),
+                 adj_eid=torch.empty(ecap, dtype=torch.int32, device=dev),
+                 adj_tmp=torch.empty(tmp, dtype=torch.int64, device=dev),
+                 err=self.err)
+        o["_caps"] = (ncap, ecap)
+        o["_c"] = _lib.BatchOut(ncap, ecap, self.feat_dim, _lib.ptr(o["x"]), o["node_label"].data_ptr(),
+                                o["batch"].data_ptr(), o["node_gid"].data_ptr(), o["edge_index"].data_ptr(),
+                                o["edge_type"].data_ptr(), o["y"].data_ptr(), o["node_ptr"].data_ptr(),
+                                o["edge_ptr"].data_ptr(), o["graph_nu"].data_ptr(), o["counts"].data_ptr(),
+                                o["adj_in_ptr"].data_ptr(), o["adj_in"].data_ptr(), o["adj_eid"].data_ptr(),
+                                o["adj_tmp"].data_ptr())
+        if reuse:
+            self._out_cache[(B, slot)] = o
+        return o
+
+    def _batch(self, B, o, keep):
+        """the ``Batch`` of ``B`` subgraphs written into ``o``; ``keep``: inputs the launch reads, kept alive with it"""
+        ncap, ecap = o["_caps"]
+        b = Batch(B, self.device, y=o["y"])
+        b._lazy = o
+        b._err = o["err"]
+        b._keep = keep
+        b._priv = dict(node_label=o["node_label"], node_ptr=o["node_ptr"], edge_ptr=o["edge_ptr"],
+                       node_cap=ncap, edge_cap=ecap, n_cap=2 * self.cap, symmetric=1, edge_row_stride=ecap,
+                       graph_nu=o["graph_nu"], counts=o["counts"])
+        # the batch kernel already built the (symmetric) message-passing adjacency in the same pass
+        b._adj = (_lib.Adj(o["adj_in_ptr"].data_ptr(), o["adj_in"].data_ptr(), o["adj_eid"].data_ptr(), None, None,
+                           None, o["adj_tmp"].data_ptr(), 1), o)
+        return b
+
+
+class SubgraphExtractor(_BatchWriter):
     """Owns the workspace for batches of up to ``max_batch`` pairs and runs igmc_extract_batch.
 
     One instance per dataset; ``extract(idx)`` is what the reference's DataLoader workers do with
@@ -608,31 +669,9 @@ class SubgraphExtractor(object):
             ptrs[-1] = None      # no flags -> the generic two-launch path
         self._ws_c = _lib.ExtractWS(*ptrs)
 
-    def _alloc_out(self, B, reuse=False, slot=0):
-        if reuse and (B, slot) in self._out_cache:
-            return self._out_cache[(B, slot)]
-        dev = self.device
-        ncap, ecap = B * 2 * self.cap, max(B * (self.edge_cap // self.max_batch), 2)
-        o = dict(x=torch.empty(ncap, self.feat_dim, dtype=torch.float32, device=dev) if self.emit_x else None,
-                 node_label=torch.empty(ncap, dtype=torch.uint8, device=dev),
-                 batch=torch.empty(ncap, dtype=torch.int64, device=dev),
-                 node_gid=torch.empty(ncap, dtype=torch.int32, device=dev),
-                 edge_index=torch.empty(2, ecap, dtype=torch.int64, device=dev),
-                 edge_type=torch.empty(ecap, dtype=torch.int64, device=dev),
-                 y=torch.empty(B, dtype=torch.float32, device=dev),
-                 node_ptr=torch.zeros(B + 1, dtype=torch.int32, device=dev),
-                 edge_ptr=torch.zeros(B + 1, dtype=torch.int32, device=dev),
-                 graph_nu=torch.zeros(B, dtype=torch.int32, device=dev),
-                 counts=torch.zeros(2, dtype=torch.int32, device=dev),
-                 adj_in_ptr=torch.zeros(ncap + 1, dtype=torch.int32, device=dev),
-                 adj_in=torch.empty(ecap, dtype=torch.int32, device=dev),
-                 adj_eid=torch.empty(ecap, dtype=torch.int32, device=dev),
-                 adj_tmp=torch.empty(ecap, dtype=torch.int64, device=dev),
-                 err=self.err)
-        o["_caps"] = (ncap, ecap)
-        if reuse:
-            self._out_cache[(B, slot)] = o
-        return o
+    def _out_caps(self, B):
+        ecap = max(B * (self.edge_cap // self.max_batch), 2)
+        return B * 2 * self.cap, ecap, ecap
 
     def extract(self, idx=None, pairs=None, pair_ids=None, out=None, inject=None, seed=None, seed_dev=None,
                 reuse=False, slot=0):
@@ -658,23 +697,13 @@ class SubgraphExtractor(object):
             P = _lib.Pairs(None, pu.data_ptr(), pv.data_ptr(), _lib.ptr(pl), _lib.ptr(pid))
             keep += [pu, pv, pl, pid]
         else:
-            if not isinstance(idx, DevView):     # (a DevView is int64 indices in mapped host memory: used as is)
-                if not torch.is_tensor(idx):
-                    idx = torch.as_tensor(np.asarray(idx), dtype=torch.int64)
-                idx = idx.to(device=dev, dtype=torch.int64)
+            idx = _device_index(idx, dev)
             B = int(idx.numel())
             P = _lib.Pairs(idx.data_ptr(), self.links_u.data_ptr(), self.links_v.data_ptr(),
                            self.links_label.data_ptr(), None)
             keep += [idx]
         self._reserve(B)
         o = out if out is not None else self._alloc_out(B, reuse, slot)
-        ncap, ecap = o["_caps"]
-        O = _lib.BatchOut(ncap, ecap, self.feat_dim, _lib.ptr(o["x"]), o["node_label"].data_ptr(),
-                          o["batch"].data_ptr(), o["node_gid"].data_ptr(), o["edge_index"].data_ptr(),
-                          o["edge_type"].data_ptr(), o["y"].data_ptr(), o["node_ptr"].data_ptr(),
-                          o["edge_ptr"].data_ptr(), o["graph_nu"].data_ptr(), o["counts"].data_ptr(),
-                          o["adj_in_ptr"].data_ptr(), o["adj_in"].data_ptr(), o["adj_eid"].data_ptr(),
-                          o["adj_tmp"].data_ptr())
         inj = [None] * 4
         if inject is not None:
             inj_t = [torch.as_tensor(np.asarray(a), dtype=torch.int32).to(dev).contiguous() for a in inject]
@@ -686,19 +715,9 @@ class SubgraphExtractor(object):
                                                _lib.ptr(seed_dev), self.cap, inj[0], inj[1], inj[2], inj[3],
                                                C.byref(self._ws_c),
                                                self.class_values.data_ptr(), int(self.class_values.numel()),
-                                               int(self.graph.max_row_deg), C.byref(O), o["err"].data_ptr(),
+                                               int(self.graph.max_row_deg), C.byref(o["_c"]), o["err"].data_ptr(),
                                                _stream_ptr()), "igmc_extract_batch")
-        b = Batch(B, dev, y=o["y"])
-        b._lazy = o
-        b._err = o["err"]
-        b._keep = keep
-        b._priv = dict(node_label=o["node_label"], node_ptr=o["node_ptr"], edge_ptr=o["edge_ptr"],
-                       node_cap=ncap, edge_cap=ecap, n_cap=2 * self.cap, symmetric=1, edge_row_stride=ecap,
-                       graph_nu=o["graph_nu"], counts=o["counts"])
-        # the extractor already built the (symmetric) message-passing adjacency in the same pass
-        b._adj = (_lib.Adj(o["adj_in_ptr"].data_ptr(), o["adj_in"].data_ptr(), o["adj_eid"].data_ptr(), None, None,
-                           None, o["adj_tmp"].data_ptr(), 1), o)
-        return b
+        return self._batch(B, o, keep)
 
     def node_lists(self, B):
         """(nodes_u [B,cap], nodes_v [B,cap], n_u [B], n_v [B]) of the last extract (host copies)."""
@@ -787,7 +806,7 @@ class MyDynamicDataset(object):
         return np.concatenate(out) if out else np.zeros(0, np.int64)
 
 
-class StaticStore(object):
+class StaticStore(_BatchWriter):
     """Device-resident store of pre-extracted subgraphs + batch assembly (igmc_assemble_batch).  Has the
     ``extract`` / ``err`` / ``cap`` surface of ``SubgraphExtractor`` so that the train engine treats both alike."""
 
@@ -911,59 +930,16 @@ class StaticStore(object):
                                                               "adj_eid")])
         self._out_cache = {}
 
-    def _alloc_out(self, B, reuse=False, slot=0):
-        if reuse and (B, slot) in self._out_cache:
-            return self._out_cache[(B, slot)]
-        dev = self.device
-        ncap, ecap = max(B * self.max_n, 2), max(B * self.max_e, 2)
-        o = dict(x=torch.empty(ncap, self.feat_dim, dtype=torch.float32, device=dev) if self.emit_x else None,
-                 node_label=torch.empty(ncap, dtype=torch.uint8, device=dev),
-                 batch=torch.empty(ncap, dtype=torch.int64, device=dev),
-                 node_gid=torch.empty(ncap, dtype=torch.int32, device=dev),
-                 edge_index=torch.empty(2, ecap, dtype=torch.int64, device=dev),
-                 edge_type=torch.empty(ecap, dtype=torch.int64, device=dev),
-                 y=torch.empty(B, dtype=torch.float32, device=dev),
-                 node_ptr=torch.zeros(B + 1, dtype=torch.int32, device=dev),
-                 edge_ptr=torch.zeros(B + 1, dtype=torch.int32, device=dev),
-                 graph_nu=torch.zeros(B, dtype=torch.int32, device=dev),
-                 counts=torch.zeros(2, dtype=torch.int32, device=dev),
-                 adj_in_ptr=torch.zeros(ncap + 1, dtype=torch.int32, device=dev),
-                 adj_in=torch.empty(ecap, dtype=torch.int32, device=dev),
-                 adj_eid=torch.empty(ecap, dtype=torch.int32, device=dev),
-                 adj_tmp=torch.empty(1, dtype=torch.int64, device=dev),
-                 err=self.err)
-        o["_caps"] = (ncap, ecap)
-        if reuse:
-            self._out_cache[(B, slot)] = o
-        return o
+    def _out_caps(self, B):
+        return max(B * self.max_n, 2), max(B * self.max_e, 2), 1
 
     def extract(self, idx=None, seed_dev=None, reuse=False, slot=0, **unused):
-        dev = self.device
-        if not isinstance(idx, DevView):
-            if not torch.is_tensor(idx):
-                idx = torch.as_tensor(np.asarray(idx), dtype=torch.int64)
-            idx = idx.to(device=dev, dtype=torch.int64)
+        idx = _device_index(idx, self.device)
         B = int(idx.numel())
         o = self._alloc_out(B, reuse, slot)
-        ncap, ecap = o["_caps"]
-        O = _lib.BatchOut(ncap, ecap, self.feat_dim, _lib.ptr(o["x"]), o["node_label"].data_ptr(),
-                          o["batch"].data_ptr(), o["node_gid"].data_ptr(), o["edge_index"].data_ptr(),
-                          o["edge_type"].data_ptr(), o["y"].data_ptr(), o["node_ptr"].data_ptr(),
-                          o["edge_ptr"].data_ptr(), o["graph_nu"].data_ptr(), o["counts"].data_ptr(),
-                          o["adj_in_ptr"].data_ptr(), o["adj_in"].data_ptr(), o["adj_eid"].data_ptr(),
-                          o["adj_tmp"].data_ptr())
-        _lib.check(self.lib.igmc_assemble_batch(C.byref(self._c), idx.data_ptr(), B, C.byref(O), self.err.data_ptr(),
-                                                _stream_ptr()), "igmc_assemble_batch")
-        b = Batch(B, dev, y=o["y"])
-        b._lazy = o
-        b._err = self.err
-        b._keep = [idx]
-        b._priv = dict(node_label=o["node_label"], node_ptr=o["node_ptr"], edge_ptr=o["edge_ptr"], node_cap=ncap,
-                       edge_cap=ecap, n_cap=2 * self.cap, symmetric=1, edge_row_stride=ecap, graph_nu=o["graph_nu"],
-                       counts=o["counts"])
-        b._adj = (_lib.Adj(o["adj_in_ptr"].data_ptr(), o["adj_in"].data_ptr(), o["adj_eid"].data_ptr(), None, None,
-                           None, o["adj_tmp"].data_ptr(), 1), o)
-        return b
+        _lib.check(self.lib.igmc_assemble_batch(C.byref(self._c), idx.data_ptr(), B, C.byref(o["_c"]),
+                                                self.err.data_ptr(), _stream_ptr()), "igmc_assemble_batch")
+        return self._batch(B, o, [idx])
 
 
 class MyDataset(MyDynamicDataset):
