@@ -1,0 +1,298 @@
+"""Per-element fp32 error bounds of the model kernels, one layer at a time.
+
+Every quantity a kernel writes (a layer's states, the predictions, ``d hid`` and the assembled parameter gradient) is
+recomputed in fp64 from the kernel's OWN inputs to that step: layer l from the kernel's saved ``h_{l-1}``, the readout
+from the kernel's concatenated states, the backward from the kernel's ``dpred`` with ``tanh' = 1 - h^2`` of the
+kernel's ``h``.  Every branch (ReLU masks, hidden dropout scales, MaxPool argmax, the SortPooling order) is taken from
+what the kernel saved, so a value within rounding of a kink cannot put the two sides on different branches;
+``branch_mismatches`` checks separately that every branch away from its kink is the one the fp64 value takes.  The
+per-layer arithmetic is the restated conv (oracle/pyg_restated.py ``RGCNConvRef``; tests/pyg2_oracle.py for the mean
+per relation of ``rgcn="pyg-2"``) in its memory-light "transform" formulation.
+
+The magnitude pass runs the same code on ``|x|``, ``|h|``, ``|att|``, ``|basis|`` (not ``|W_r|``: the kernels round W_r
+themselves), ``|root|``, ``|bias|``, the absolute readout weights and ``|dpred|``, with the same masks and the positive
+mean weights.  Its output ``M`` is, per element, the sum of the absolute values of the terms behind that element, so a
+kernel that sums those terms in fp32 in any order is off by at most a small multiple of ``u * M`` (``u = 2^-24``):
+
+    |got - ref| <= KAPPA[quantity] * u * M,     and got == 0 exactly where M == 0 (padding columns, empty rows).
+
+A state ``h = tanh(pre)`` is bounded by ``(1 - h^2) M_pre + |h|``: the pre-activation's bound through tanh' plus the
+rounding of tanhf itself."""
+import torch
+import torch.nn.functional as F
+
+U = 2.0 ** -24
+
+# The smallest power of two at least 4x the largest err / (u M) measured over every case of
+# tests/test_gpu_error_bounds.py on an H100 80GB HBM3 (700 W): states 10.3 (plan 0 and the L2 plan, fp32 sums in
+# sequence), predictions 0.097, d hid 0.99 (two roundings of one product), gradients 5.0 (ml_1m* batch 50).  A lost
+# 3xTF32 cross term or an operand truncated to TF32 is off by ~2^-11 of its products: hundreds to thousands of u M.
+# The prediction bound is below one rounding of u M.  It holds because a prediction is a heavily cancelling sum over
+# 128 hidden units and the lin1 sums behind them, so |pred| is far below M.  A prediction whose |pred| came close to
+# M could exceed 0.5 u M with correct fp32 arithmetic; a reordering of those sums that trips it is not by itself a
+# kernel bug.
+KAPPA = dict(states=64, pred=0.5, dhid=4, grad=32)
+
+
+class Graph:
+    """one collated batch (an oracle ``extract_batch`` dict) in fp64, edge dropout applied by ``edge_keep``"""
+
+    def __init__(self, ob, edge_keep=None):
+        self.x = torch.as_tensor(ob["x"]).double()
+        ei = torch.as_tensor(ob["edge_index"]).long()
+        et = torch.as_tensor(ob["edge_type"]).long()
+        if edge_keep is not None:
+            keep = torch.as_tensor(edge_keep).bool()
+            ei, et = ei[:, keep], et[keep]
+        self.edge_index, self.edge_type = ei, et
+        self.users, self.items = self.x[:, 0] == 1, self.x[:, 1] == 1
+        self.num_graphs = int(ob["num_graphs"])
+        counts = torch.bincount(torch.as_tensor(ob["batch"]).long(), minlength=self.num_graphs)
+        self.node_ptr = torch.cat([torch.zeros(1, dtype=torch.long), torch.cumsum(counts, 0)])
+
+
+def conv_names(params):
+    """state_dict suffixes of the [R,NB], [NB,in,out], [in,out], [out] parameters of a conv layer"""
+    return ("att", "basis", "root", "bias") if any(k.endswith(".att") for k in params) else \
+        ("comp", "weight", "root", "bias")
+
+
+def _conv(att, basis, root, bias, aggr):
+    """the restated conv with the given tensors in place of its parameters (autograd flows into them)"""
+    from tests import pyg2_oracle
+    NB, fin, fout = basis.shape
+    with torch.random.fork_rng(devices=[]):      # construction draws an init; keep the caller's RNG stream
+        c = pyg2_oracle.RGCNConvRelMeanRef(fin, fout, att.shape[0], NB, aggr)
+    for name, t in (("att", att), ("basis", basis), ("root", root), ("bias", bias)):
+        delattr(c, name)
+        setattr(c, name, t)
+    c.formulation = "transform"
+    return c
+
+
+def layer_pre(h, p4, g, aggr):
+    """pre-activation of one conv layer: mean aggregate of h W_r + h root + bias"""
+    return _conv(*p4, aggr)(h, g.edge_index, g.edge_type)
+
+
+def head(cs, P, g, saved, dgcnn, parts=None):
+    """readout of the concatenated states ``cs`` up to the lin2 output (before ``multiply_by``), on the kernel's
+    branches: IGMC target rows -> lin1 -> ReLU / dropout (``gscale``) -> lin2; DGCNN_RS SortPooling in the kernel's
+    order (``perm``) -> conv1 -> ReLU (``act1 > 0``) -> MaxPool (argmax of ``act1``) -> conv2 -> ReLU (``flat > 0``) ->
+    lin1 -> ReLU / dropout -> lin2.  ``parts`` (a dict) receives the arguments of those branches: the pre-activations
+    "conv1", "conv2" and "lin1" """
+    parts = {} if parts is None else parts
+    if not dgcnn:
+        z = torch.cat([cs[g.users], cs[g.items]], 1)
+    else:
+        perm, act1, flat = saved["perm"], saved["act1"], saved["flat"]
+        B, k = perm.shape
+        W = cs.shape[1]
+        rows = cs[perm.clamp(min=0)] * (perm >= 0).unsqueeze(-1).to(cs.dtype)      # padding rows are zero
+        a1 = F.conv1d(rows.reshape(B, 1, k * W), P["conv1d_params1.weight"], P["conv1d_params1.bias"], stride=W)
+        parts["conv1"] = a1
+        a1 = a1 * (act1 > 0).to(cs.dtype)
+        t1 = k // 2
+        arg = (act1[..., 1:2 * t1:2] > act1[..., 0:2 * t1:2]).long()           # first maximum wins
+        pool = a1.gather(2, 2 * torch.arange(t1).view(1, 1, t1) + arg)
+        a2 = F.conv1d(pool, P["conv1d_params2.weight"], P["conv1d_params2.bias"])
+        parts["conv2"] = a2
+        z = (a2 * (flat.view(a2.shape) > 0).to(cs.dtype)).reshape(B, -1)
+    parts["lin1"] = z @ P["lin1.weight"].t() + P["lin1.bias"]
+    hid = parts["lin1"] * saved["gscale"]
+    return hid @ P["lin2.weight"][0] + P["lin2.bias"][0]
+
+
+def _readout_keys(params):
+    return [k for k in params if not k.startswith("convs.")]
+
+
+def _prep(params, saved, mag):
+    A = torch.abs if mag else (lambda t: t)
+    P = {k: A(v) for k, v in params.items()}
+    states = [A(h) for h in saved["states"]]
+    return A, P, states
+
+
+def forward(params, g, saved, aggr, dgcnn, mag=False):
+    """(per-layer pre-activations from the kernel's own inputs, readout output before multiply_by)"""
+    A, P, states = _prep(params, saved, mag)
+    names = conv_names(params)
+    with torch.no_grad():
+        pres = [layer_pre(g.x if l == 0 else states[l - 1], [P["convs.%d.%s" % (l, n)] for n in names], g, aggr)
+                for l in range(len(states))]
+        out = head(torch.cat(states, 1), P, g, saved, dgcnn)
+    return pres, out
+
+
+def _arr_dW(W, arr, mag):
+    """d (arr * sum_r ||W_{r+1} - W_r||^2) / d W; the magnitude pass adds where the value subtracts"""
+    s = 1.0 if mag else -1.0
+    D = torch.zeros_like(W)
+    D[1:] += W[1:] + s * W[:-1]
+    D[:-1] += W[:-1] + s * W[1:]
+    return 2.0 * arr * D
+
+
+def backward(params, g, saved, aggr, dgcnn, arr, mag=False):
+    """(d hid [B,128], parameter gradients by state_dict name) of the loss whose lin2-output gradient is the kernel's
+    ``dpred``, plus the ARR term: per-layer vector-Jacobian products from the readout down to layer 0"""
+    A, P0, states = _prep(params, saved, mag)
+    P = {k: v.detach().clone().requires_grad_(True) for k, v in P0.items()}
+    dpred = A(saved["dpred"])
+    names = conv_names(params)
+    L = len(states)
+    cs = torch.cat(states, 1).requires_grad_(True)
+    rk = _readout_keys(params)
+    gr = torch.autograd.grad(head(cs, P, g, saved, dgcnn), [cs] + [P[k] for k in rk], dpred)
+    grads = dict(zip(rk, gr[1:]))
+    dh = list(torch.split(gr[0], [h.shape[1] for h in states], 1))
+    for l in reversed(range(L)):
+        h = saved["states"][l]
+        dpre = dh[l] * (1.0 - h * h)
+        keys = ["convs.%d.%s" % (l, n) for n in names]
+        hin = g.x if l == 0 else states[l - 1].clone().requires_grad_(True)
+        pre = layer_pre(hin, [P[k] for k in keys], g, aggr)
+        gr = torch.autograd.grad(pre, [P[k] for k in keys] + ([hin] if l else []), dpre)
+        grads.update(zip(keys, gr[:4]))
+        if l:
+            dh[l - 1] = dh[l - 1] + gr[4]
+        if arr:
+            att, basis = P[keys[0]], P[keys[1]]
+            W = torch.einsum("rb,bio->rio", att, basis)
+            ga, gb = torch.autograd.grad(W, [att, basis], _arr_dW(W.detach(), arr, mag))
+            grads[keys[0]] = grads[keys[0]] + ga
+            grads[keys[1]] = grads[keys[1]] + gb
+    dhid = dpred.unsqueeze(1) * A(params["lin2.weight"])[0] * saved["gscale"]
+    return dhid, grads
+
+
+def branch_mismatches(params, g, saved, dgcnn, hidden_keep=None):
+    """the number of branches the kernel took against the fp64 value of their argument, counted only where that value
+    is farther than KAPPA["states"] u M from the kink (closer than that, either side is correct): the lin1 ReLU
+    (``gscale > 0`` iff pre-activation > 0 and the unit is kept by ``hidden_keep``), and for DGCNN_RS the conv1 ReLU
+    (``act1``), the MaxPool side, the conv2 ReLU (``flat``) and the SortPooling order, which must be exactly the stable
+    descending order of the kernel's own last-channel keys"""
+    _, P, states = _prep(params, saved, False)
+    _, MP, mstates = _prep(params, saved, True)
+    parts, mparts = {}, {}
+    with torch.no_grad():
+        head(torch.cat(states, 1), P, g, saved, dgcnn, parts)
+        head(torch.cat(mstates, 1), MP, g, saved, dgcnn, mparts)
+
+    def wrong(kernel_side, ref, M, forced=None):
+        """kernel_side: the branch taken (bool); forced: elements whose side is known without ref (dropped units)"""
+        sure = ref.abs() > KAPPA["states"] * U * M
+        want = ref > 0
+        if forced is not None:
+            sure, want = sure | forced, want & ~forced
+        return int((kernel_side != want)[sure].sum())
+
+    pre1 = parts["lin1"]
+    dropped = torch.zeros_like(pre1, dtype=torch.bool) if hidden_keep is None else ~torch.as_tensor(hidden_keep).bool()
+    bad = wrong(saved["gscale"] > 0, pre1, mparts["lin1"], dropped)
+    if dgcnn:
+        act1, a1, ma1 = saved["act1"], parts["conv1"], mparts["conv1"]
+        bad += wrong(act1 > 0, a1, ma1)
+        t1 = act1.shape[-1] // 2
+        z = a1.clamp(min=0)
+        odd, even = slice(1, 2 * t1, 2), slice(0, 2 * t1, 2)
+        bad += wrong(act1[..., odd] > act1[..., even], z[..., odd] - z[..., even], ma1[..., odd] + ma1[..., even])
+        bad += wrong(saved["flat"].view(parts["conv2"].shape) > 0, parts["conv2"], mparts["conv2"])
+        key = torch.cat(saved["states"], 1)[:, -1]
+        perm = saved["perm"]
+        for gi, (lo, hi) in enumerate(zip(g.node_ptr[:-1].tolist(), g.node_ptr[1:].tolist())):
+            order = lo + torch.sort(-key[lo:hi], stable=True).indices[:perm.shape[1]]
+            want = torch.full_like(perm[gi], -1)
+            want[:len(order)] = order
+            bad += int((perm[gi] != want).sum())
+    return bad
+
+
+# ---- device side ----------------------------------------------------------------------------------------------------
+def device_saved(m, ws, num_nodes, train):
+    """the kernel's saved tensors of the last forward (and backward) of ``m`` on workspace ``ws``, on the host in fp64:
+    per-layer states at their true widths, hidden dropout scales, dpred, and DGCNN_RS's SortPooling order and ReLU
+    outputs"""
+    st = ws["states"][:num_nodes].double().cpu()
+    widths = [c.out_channels for c in m.convs]
+    src = ws["sp"] if "sp" in ws else ws
+    saved = dict(states=[st[:, 32 * l:32 * l + w] for l, w in enumerate(widths)], states_full=st,
+                 gscale=src["hid_gscale"].double().cpu(), pred=src["pred"].double().cpu())
+    if "sp" in ws:
+        sp = ws["sp"]
+        saved.update(perm=sp["perm"].long().cpu(), act1=sp["act1"].double().cpu(), flat=sp["flat"].double().cpu())
+    if train:
+        saved.update(dpred=ws["dpred"].double().cpu(), dhid=src["dhid"].double().cpu())
+    return saved
+
+
+def ratio(got, ref, M):
+    """largest |got - ref| / (u M) over the elements with M > 0, and the number of elements with M == 0 where got is
+    not exactly zero; also the flat index of the worst element.  A NaN or infinity anywhere (in got, or in ref or M
+    from non-finite kernel inputs) gives an infinite ratio: it can never pass, and it hides no other element"""
+    got, ref, M = got.reshape(-1).double(), ref.reshape(-1).double(), M.reshape(-1).double()
+    zero = M == 0
+    nonzero_pad = int((got[zero] != 0).sum())
+    r = (got - ref).abs() / (U * M.clamp(min=1e-300))
+    r[zero] = 0.0
+    r[~(torch.isfinite(r) & torch.isfinite(got))] = float("inf")
+    worst = int(r.argmax()) if r.numel() else -1
+    return (float(r.max()) if r.numel() else 0.0), nonzero_pad, worst
+
+
+def _pad32(t, w):
+    return F.pad(t, (0, w - t.shape[1]))
+
+
+def check_device(m, ob, ws, train, edge_keep=None, arr=0.0, hidden_keep=None):
+    """every quantity of the last forward (eval) or train step of ``m`` on the oracle batch ``ob`` against its fp64
+    recomputation; returns {quantity: (largest err / (u M), elements that must be zero but are not, worst index)} and
+    under "branches" the count of ``branch_mismatches`` (``edge_keep`` / ``hidden_keep``: the step's dropout draws)"""
+    params = {k: v.detach().double().cpu().contiguous() for k, v in m.state_dict().items()}
+    dgcnn = "sp" in ws
+    aggr = "mean_per_relation" if m.rgcn == "pyg-2" else "mean_all"
+    N = ob["x"].shape[0]
+    g = Graph(ob, edge_keep if train else None)
+    saved = device_saved(m, ws, N, train)
+    pres, out = forward(params, g, saved, aggr, dgcnn)
+    mpres, mout = forward(params, g, saved, aggr, dgcnn, mag=True)
+    res = dict(branches=branch_mismatches(params, g, saved, dgcnn, hidden_keep if train else None))
+    for l, (pre, mpre) in enumerate(zip(pres, mpres)):
+        got = saved["states_full"][:, 32 * l:32 * l + 32]
+        h = saved["states"][l]
+        res["states%d" % l] = ratio(got, _pad32(torch.tanh(pre), 32), _pad32((1 - h * h) * mpre + h.abs(), 32))
+    mult = float(m.multiply_by)
+    res["pred"] = ratio(saved["pred"], out * mult, mout * abs(mult))
+    if train:
+        dhid, grads = backward(params, g, saved, aggr, dgcnn, arr)
+        mdhid, mgrads = backward(params, g, saved, aggr, dgcnn, arr, mag=True)
+        res["dhid"] = ratio(saved["dhid"], dhid, mdhid)
+        names = {id(p): n for n, p in m.named_parameters()}
+        fg = m.flat_grad.double().cpu()
+        got, ref, M = [], [], []
+        for e, (_, _, p) in zip(m._layout, m._named_order()):
+            o, n, s = e[:3]
+            full = e[3] if len(e) == 4 else s
+            name = names[id(p)]
+            r, mm = torch.zeros(full, dtype=torch.float64), torch.zeros(full, dtype=torch.float64)
+            r[..., :s[-1]] = grads[name].reshape(s)
+            mm[..., :s[-1]] = mgrads[name].reshape(s)
+            got.append(fg[o:o + n])
+            ref.append(r.reshape(-1))
+            M.append(mm.reshape(-1))
+        res["grad"] = ratio(torch.cat(got), torch.cat(ref), torch.cat(M))
+    return res
+
+
+def violations(res):
+    """the entries of a ``check_device`` result that fail: a ratio not within its KAPPA (NaN included), an element that
+    must be zero and is not, or a branch mismatch"""
+    bad = [("branches", res["branches"])] if res["branches"] else []
+    for key, val in res.items():
+        if key == "branches":
+            continue
+        r, pad, worst = val
+        if not r <= KAPPA["states" if key.startswith("states") else key] or pad:
+            bad.append((key, r, pad, worst))
+    return bad

@@ -1,0 +1,251 @@
+"""CPU checks of the layer-by-layer fp64 oracle and its magnitude pass (tests/error_bounds.py), and a numpy emulation of
+the relation-space kernels' 3xTF32 tensor-core products that ties the committed error constants to the arithmetic."""
+import numpy as np
+import pytest
+import torch
+import torch.nn.functional as F
+
+from oracle import pyg_restated
+from tests import error_bounds as eb
+from tests import pyg2_oracle
+from tests.test_gpu_model import _oracle_batch
+
+
+def _ref(rgcn, in0, L, R=5, NB=4, dgcnn_last=None, k=30):
+    torch.manual_seed(0)
+    if dgcnn_last is None:
+        ref = pyg2_oracle.igmc_ref(rgcn, in0, (32,) * L, R, NB, 0.2, 2)     # multiply_by 2: scales dpred too
+    else:
+        ref = pyg2_oracle.dgcnn_rs_ref(rgcn, in0, (32, 32, 32, dgcnn_last), k, R, NB, 0.2)
+    with torch.no_grad():
+        for c in ref.convs:
+            c.bias.uniform_(-0.3, 0.3)     # PyG 2 zero-inits the bias
+    return pyg_restated.set_formulation(ref.double().train(), "transform")
+
+
+def _oracle_saved(ref, ob, ek, hk):
+    """what the kernels would save, computed by the whole restated model: states, hidden scales, SortPooling order and
+    ReLU outputs, and dpred of the MSE + ARR loss; with the model's own fp64 loss gradients in ``.grad``"""
+    tb = pyg_restated.to_torch_batch(ob, torch.float64)
+    ref.zero_grad()
+    dg = isinstance(ref, pyg_restated.DGCNN_RSRef)
+    B = ob["num_graphs"]
+    if dg:
+        out, cs = ref(tb["x"], tb["edge_index"], tb["edge_type"], tb["batch"], ek, hk, B, return_states=True)
+    else:
+        out, cs = ref(tb["x"], tb["edge_index"], tb["edge_type"], ek, hk, return_states=True)
+    loss = F.mse_loss(out, tb["y"].view(-1)) + 0.001 * pyg_restated.arr_regulariser(ref)
+    loss.backward()
+    cs = cs.detach()
+    widths = [c.out_channels for c in ref.convs]
+    saved = dict(states=list(torch.split(cs, widths, 1)), out=out.detach(), hidden_keep=hk)
+    mult = 1.0 if dg else float(ref.multiply_by)
+    saved["dpred"] = 2.0 * (out.detach() - tb["y"].view(-1)) / B * mult
+    with torch.no_grad():
+        if dg:
+            z = pyg_restated.global_sort_pool(cs, tb["batch"], ref.k, B).unsqueeze(1)
+            act1 = F.relu(ref.conv1d_params1(z))
+            flat = F.relu(ref.conv1d_params2(ref.maxpool1d(act1))).reshape(B, -1)
+            feat = flat
+            nptr = np.concatenate([[0], np.cumsum(np.bincount(ob["batch"], minlength=B))])
+            perm = torch.full((B, ref.k), -1, dtype=torch.long)
+            for gi in range(B):
+                order = nptr[gi] + np.argsort(-cs[nptr[gi]:nptr[gi + 1], -1].numpy(), kind="stable")[:ref.k]
+                perm[gi, :len(order)] = torch.from_numpy(order)
+            saved.update(perm=perm, act1=act1, flat=flat)
+        else:
+            x = tb["x"]
+            feat = torch.cat([cs[x[:, 0] == 1], cs[x[:, 1] == 1]], 1)
+        pre1 = ref.lin1(feat)
+        saved["gscale"] = (pre1 > 0).double() * hk.double() * 2.0
+    return saved
+
+
+def _case(rgcn, in0, L, dgcnn_last=None, R=5):
+    ob = _oracle_batch(R=R, h=(in0 - 2) // 2)[3]
+    assert ob["x"].shape[1] == in0
+    ref = _ref(rgcn, in0, L, R=R, dgcnn_last=dgcnn_last)
+    gen = torch.Generator().manual_seed(11)
+    ek = torch.rand(ob["edge_index"].shape[1], generator=gen) > 0.2
+    hk = torch.rand(ob["num_graphs"], 128, generator=gen) > 0.5
+    saved = _oracle_saved(ref, ob, ek, hk)
+    params = {k: v.detach().clone() for k, v in ref.state_dict().items()}
+    aggr = ref.convs[0].aggr
+    return ref, ob, eb.Graph(ob, ek), saved, params, aggr, dgcnn_last is not None
+
+
+def _close(a, b, rel=1e-12):
+    assert float((a - b).abs().max()) <= rel * (float(b.abs().max()) + 1e-300), (float((a - b).abs().max()),
+                                                                               float(b.abs().max()))
+
+
+CASES = [("pyg-1.4", 4, 4, None), ("pyg-1.4", 4, 1, None), ("pyg-1.4", 4, 8, None), ("pyg-1.4", 6, 4, None),
+         ("pyg-1.4", 8, 4, None), ("pyg-2", 4, 4, None), ("pyg-2", 6, 1, None), ("pyg-2", 8, 8, None),
+         ("pyg-1.4", 4, 4, 1), ("pyg-1.4", 4, 4, 8), ("pyg-2", 4, 4, 1), ("pyg-2", 6, 4, 8)]
+
+
+@pytest.mark.parametrize("rgcn,in0,L,last", CASES)
+def test_chained_layers_equal_whole_model_autograd(rgcn, in0, L, last):
+    """per-layer forward from the saved states and the chained per-layer VJPs from dpred equal the whole restated model
+    and its fp64 autograd (train mode, injected edge and hidden masks, ARR term): 1e-12 relative"""
+    ref, ob, g, saved, params, aggr, dg = _case(rgcn, in0, L, last)
+    pres, out = eb.forward(params, g, saved, aggr, dg)
+    for pre, h in zip(pres, saved["states"]):
+        _close(torch.tanh(pre), h)
+    mult = 1.0 if dg else float(ref.multiply_by)
+    _close(out * mult, saved["out"])
+    dhid, grads = eb.backward(params, g, saved, aggr, dg, 0.001)
+    assert set(grads) == set(params)
+    for name, p in ref.named_parameters():
+        _close(grads[name], p.grad)
+    # d hid is d loss / d (lin1 output after ReLU and dropout): its sum over graphs is lin1.bias's gradient
+    _close((dhid).sum(0), ref.lin1.bias.grad)
+
+
+@pytest.mark.parametrize("rgcn,in0,L,last", [CASES[0], CASES[5], CASES[9], CASES[11]])
+def test_magnitude_bounds_every_element(rgcn, in0, L, last):
+    """M >= |ref| element by element (pre-activations, readout output, d hid, every gradient, ARR included)"""
+    ref, ob, g, saved, params, aggr, dg = _case(rgcn, in0, L, last)
+    pres, out = eb.forward(params, g, saved, aggr, dg)
+    mpres, mout = eb.forward(params, g, saved, aggr, dg, mag=True)
+    for a, m in list(zip(pres, mpres)) + [(out, mout)]:
+        assert bool((m >= a.abs()).all())
+    dhid, grads = eb.backward(params, g, saved, aggr, dg, 0.001)
+    mdhid, mgrads = eb.backward(params, g, saved, aggr, dg, 0.001, mag=True)
+    assert bool((mdhid >= dhid.abs()).all())
+    for k in grads:
+        assert bool((mgrads[k] >= grads[k].abs() * (1 - 1e-12)).all()), k
+        assert float(mgrads[k].abs().max()) > 0, k
+
+
+@pytest.mark.parametrize("rgcn,in0,L,last", [CASES[0], CASES[6], CASES[10]])
+def test_magnitude_equals_value_on_nonnegative_inputs(rgcn, in0, L, last):
+    """with every operand non-negative (and no ARR: its differences turn into sums) M is the value itself"""
+    ref, ob, g, saved, params, aggr, dg = _case(rgcn, in0, L, last)
+    params = {k: v.abs() for k, v in params.items()}
+    saved = dict(saved, states=[h.abs() for h in saved["states"]], dpred=saved["dpred"].abs())
+    for a, m in zip(eb.forward(params, g, saved, aggr, dg)[0], eb.forward(params, g, saved, aggr, dg, mag=True)[0]):
+        assert torch.equal(a, m)
+    dhid, grads = eb.backward(params, g, saved, aggr, dg, 0.0)
+    mdhid, mgrads = eb.backward(params, g, saved, aggr, dg, 0.0, mag=True)
+    assert torch.equal(dhid, mdhid)
+    for k in grads:
+        assert torch.equal(grads[k], mgrads[k]), k
+
+
+def test_ratio_fails_on_nan_and_nonzero_padding():
+    """a NaN or infinity in got makes the ratio infinite wherever it sits, so it cannot hide the other elements; a
+    nonzero value where M == 0 is counted"""
+    ref = torch.tensor([1.0, 2.0, 3.0, 0.0], dtype=torch.float64)
+    M = ref.clone()
+    assert eb.ratio(ref + eb.U * M, ref, M)[:2] == (1.0, 0)
+    for bad in (float("nan"), float("inf")):
+        got = ref.clone()
+        got[1] = bad
+        r, pad, worst = eb.ratio(got, ref, M)
+        assert r == float("inf") and pad == 0 and worst == 1
+        res = dict(branches=0, pred=(r, pad, worst))
+        assert eb.violations(res) == [("pred", r, pad, worst)]
+    got = ref.clone()
+    got[3] = float("nan")
+    assert eb.ratio(got, ref, M)[1] == 1
+    assert eb.violations(dict(branches=2, states0=(0.0, 0, 0))) == [("branches", 2)]
+
+
+@pytest.mark.parametrize("rgcn,in0,L,last", [CASES[0], CASES[9], CASES[11]])
+def test_branches_agree_and_flipped_branches_are_found(rgcn, in0, L, last):
+    """on the whole model's own branches nothing mismatches; a hidden unit zeroed although its pre-activation is
+    clearly positive, a conv1 ReLU flipped and two swapped sort-pool positions are each found"""
+    ref, ob, g, saved, params, aggr, dg = _case(rgcn, in0, L, last)
+    hk = saved["hidden_keep"]
+    assert eb.branch_mismatches(params, g, saved, dg, hk) == 0
+    parts = {}
+    with torch.no_grad():
+        eb.head(torch.cat(saved["states"], 1), params, g, saved, dg, parts)
+    pos = torch.nonzero((parts["lin1"] > 1e-3) & hk)[0]
+    gscale = saved["gscale"].clone()
+    gscale[pos[0], pos[1]] = 0.0
+    assert eb.branch_mismatches(params, g, dict(saved, gscale=gscale), dg, hk) == 1
+    gscale = saved["gscale"].clone()
+    gscale[pos[0], pos[1]] = 2.0
+    gscale[~hk] = 2.0                                   # a dropped unit kept
+    assert eb.branch_mismatches(params, g, dict(saved, gscale=gscale), dg, hk) >= 1
+    if dg:
+        act1 = saved["act1"].clone()
+        c = torch.nonzero(parts["conv1"] > 1e-3)[0]
+        act1[c[0], c[1], c[2]] = 0.0
+        assert eb.branch_mismatches(params, g, dict(saved, act1=act1), dg, hk) >= 1
+        perm = saved["perm"].clone()
+        perm[0, [0, 1]] = perm[0, [1, 0]]
+        assert eb.branch_mismatches(params, g, dict(saved, perm=perm), dg, hk) >= 2
+
+
+# ---- 3xTF32 separation ----------------------------------------------------------------------------------------------
+def _tf32(a):
+    """the top 10 mantissa bits: a mask of the 13 low ones (what the kernels' split and the tensor core's read keep)"""
+    return (np.asarray(a, np.float32).view(np.uint32) & np.uint32(0xFFFFE000)).view(np.float32)
+
+
+def emulate_3xtf32(A, B, K1, drop=None):
+    """[A1 | A2] . B of csrc/rgcn_rs.cu ``tiles_span`` / ``tiles_span2`` in fp32: k-steps of 8, even steps of the
+    first span (K1 columns) into (d, e), odd steps and the second span into (d2, e2), e / e2 taking the cross terms
+    lo_a hi_b then hi_a lo_b, result (d + d2) + (e + e2).  One k-step's 8 products (exact tf32 x tf32) are summed
+    exactly and added to the fp32 accumulator with one rounding.  ``drop``: "al_bh" or "ah_bl" leaves that term out."""
+    A, B = np.asarray(A, np.float32), np.asarray(B, np.float32)
+    ah, bh = _tf32(A), _tf32(B)
+    al, bl = _tf32(A - ah), _tf32(B - bh)          # lo = x - hi is exact in fp32; the tensor core reads 10 bits of it
+    acc = {n: np.zeros((A.shape[0], B.shape[1]), np.float32) for n in ("d", "e", "d2", "e2")}
+
+    def add(name, a, b, k0):
+        s = slice(k0, k0 + 8)
+        acc[name] = (acc[name].astype(np.float64) + a[:, s].astype(np.float64) @ b[s].astype(np.float64)) \
+            .astype(np.float32)
+
+    for k0 in range(0, A.shape[1], 8):
+        second = k0 >= K1 or (k0 // 8) % 2 == 1 and (k0 // 16 + 1) * 16 <= K1
+        d, e = ("d2", "e2") if second else ("d", "e")
+        if drop != "al_bh":
+            add(e, al, bh, k0)
+        if drop != "ah_bl":
+            add(e, ah, bl, k0)
+        add(d, ah, bh, k0)
+    return (acc["d"] + acc["d2"]) + (acc["e"] + acc["e2"])
+
+
+def _layer1_operands():
+    """one real layer-1 transform of the relation-space kernels on the R = 5 oracle batch: A = [AGG' | h] (the
+    1/deg-scaled per-relation sums of the layer-0 states, fp32) and B = [W_1 .. W_R ; root] (fp32)"""
+    R = 5
+    ob = _oracle_batch(R=R)[3]
+    ref = _ref("pyg-1.4", 4, 4, R=R)
+    tb = pyg_restated.to_torch_batch(ob, torch.float64)
+    with torch.no_grad():
+        h = torch.tanh(ref.convs[0](tb["x"], tb["edge_index"], tb["edge_type"])).float().double()
+        src, dst = tb["edge_index"]
+        N = h.shape[0]
+        agg = torch.zeros(N * R, 32, dtype=torch.float64).index_add_(0, dst * R + tb["edge_type"], h[src])
+        deg = torch.bincount(dst, minlength=N).clamp(min=1).double()
+        agg = (agg.view(N, R, 32).float() * (1.0 / deg.float()).view(N, 1, 1)).reshape(N, R * 32)
+        c = ref.convs[1]
+        W = torch.einsum("rb,bio->rio", c.att, c.basis).float().reshape(R * 32, 32)
+        B = torch.cat([W, c.root.float()], 0)
+    return torch.cat([agg, h.float()], 1).numpy(), B.numpy(), R * 32
+
+
+def _worst(C, A, B):
+    A64, B64 = A.astype(np.float64), B.astype(np.float64)
+    return float((np.abs(C.astype(np.float64) - A64 @ B64) / (eb.U * (np.abs(A64) @ np.abs(B64)))).max())
+
+
+def test_3xtf32_emulation_within_kappa_and_lost_cross_term_beyond():
+    """the kernels' 3xTF32 product on real operands stays within KAPPA["states"] u M; the same product without either
+    cross term exceeds it (so the committed constant separates fp32-level accuracy from a TF32 slip)"""
+    A, B, K1 = _layer1_operands()
+    assert A.shape[1] == K1 + 32 and np.count_nonzero(A[:, :K1]) > 0
+    ok = _worst(emulate_3xtf32(A, B, K1), A, B)
+    print("3xTF32 emulation: largest err / (u M) = %.2f (KAPPA states %g)" % (ok, eb.KAPPA["states"]))
+    assert ok <= eb.KAPPA["states"]
+    for drop in ("ah_bl", "al_bh"):
+        bad = _worst(emulate_3xtf32(A, B, K1, drop), A, B)
+        print("  without %s: %.0f" % (drop, bad))
+        assert bad > eb.KAPPA["states"], drop

@@ -79,9 +79,8 @@ def test_multi_hop_large(h, mnph):
     assert _is_l2(m, b)
 
 
-@pytest.mark.parametrize("NB", [2, 4])
-def test_many_relations(NB):
-    """R = 71 (YahooMusic's rating levels) at n_cap 564: beyond the generic plan's 422 nodes"""
+def _many_relations_batch():
+    """(R, batch, oracle batch): four pairs of a 600 x 600 matrix with R = 71 rating levels, n_cap 564"""
     R, nu, nv = 71, 600, 600
     rng = np.random.default_rng(4)
     u, v = np.nonzero(rng.random((nu, nv)) < 0.3)
@@ -95,6 +94,13 @@ def test_many_relations(NB):
     pairs = (A.nonzero()[0][:4], A.nonzero()[1][:4], np.asarray(A[A.nonzero()[0][:4], A.nonzero()[1][:4]]).ravel() - 1)
     b, ob = _extracted(A, pairs, R, 1, None)
     assert b._priv["n_cap"] == 564
+    return R, b, ob
+
+
+@pytest.mark.parametrize("NB", [2, 4])
+def test_many_relations(NB):
+    """R = 71 (YahooMusic's rating levels) at n_cap 564: beyond the generic plan's 422 nodes"""
+    R, b, ob = _many_relations_batch()
     ref, m = _models(4, R, NB=NB)
     check_step(m, ref, b, ob, 0.001, 0.2, _hk(4))
     assert _is_l2(m, b)

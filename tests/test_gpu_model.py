@@ -12,12 +12,12 @@ from igmc_b200.data import synth_ratings, build_adj
 pytestmark = pytest.mark.gpu
 
 
-def _oracle_batch(nu=120, nv=90, nnz=2500, R=5, B=16, mnph=30, seed=3):
+def _oracle_batch(nu=120, nv=90, nnz=2500, R=5, B=16, mnph=30, seed=3, h=1):
     u, v, lab = synth_ratings(nu, nv, nnz, R, seed)
     A = build_adj(u, v, lab, nu, nv)
     g = extract_np.RatingCSR(A)
     cv = np.arange(1, R + 1, dtype=np.float32)
-    ob = extract_np.extract_batch(g, u[:B], v[:B], lab[:B], cv, 1, 1.0, mnph, seed=5)
+    ob = extract_np.extract_batch(g, u[:B], v[:B], lab[:B], cv, h, 1.0, mnph, seed=5)
     return A, (u, v, lab), cv, ob
 
 
