@@ -118,7 +118,7 @@ class Stage(C.Structure):
 class Candidates(C.Structure):
     _fields_ = [("users", vp), ("cand", vp), ("pair_u", vp), ("pair_v", vp), ("user_off", vp), ("rated_off", vp),
                 ("rated_pos", vp), ("num_pairs", C.c_int64), ("num_query", C.c_int32), ("num_cand", C.c_int32),
-                ("exclude_rated", C.c_int32), ("pad_", C.c_int32)]
+                ("exclude_rated", C.c_int32), ("per_user", C.c_int32)]
 
 
 GRAPH_UPDATE_HEADER = ("nnz", "num_users", "num_items", "max_row_deg", "max_col_deg", "inserted", "changed",
@@ -179,6 +179,10 @@ _SIGS = {
     "igmc_candidate_pairs": [C.POINTER(CSR), C.POINTER(Candidates), vp, C.c_int, vp, vp, vp, vp, vp, vp],
     "igmc_topk_merge": [vp, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp, vp],
     "igmc_score_scatter": [vp, C.c_int, C.c_int, vp, vp, vp],
+    "igmc_candidate_lists_ws_bytes": [C.c_int, C.c_int, C.POINTER(C.c_int64)],
+    "igmc_candidate_lists": [C.POINTER(CSR), C.POINTER(Candidates), vp, C.c_int, vp, vp, C.c_int64, vp, vp],
+    "igmc_corated_ws_bytes": [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int64)],
+    "igmc_corated_items": [C.POINTER(CSR), vp, C.c_int, C.c_int, C.c_int, vp, C.c_int64, vp, vp, vp, vp],
     "igmc_graph_update_ws_bytes": [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int64)],
     "igmc_graph_update_plan": [C.POINTER(CSR), C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, C.c_int, C.c_int,
                                C.c_int, vp, C.c_int64, vp, vp, vp],

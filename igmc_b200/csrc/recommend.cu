@@ -4,6 +4,8 @@
 // (optionally) a candidate item list once; from then on every batch is produced, scored and merged on the device:
 //   k_candidate_plan   one CTA: per query user the candidate count and its exclusive prefix user_off[U+1]; with a
 //                      candidate list and exclude_rated, also the positions in the list of the user's rated items
+//   k_lists_rows       per-user candidate rows (after a segmented sort): one CTA per row counts, then writes, the valid,
+//                      distinct, (with exclude_rated) unrated items; k_lists_scan turns the counts into user_off
 //   k_candidate_pairs  one CTA: the pairs of global candidate positions [cursor, cursor + B) for igmc_extract_batch
 //                      (idx = NULL), then cursor += B - a captured graph replays with no host input
 //   k_topk_merge       one CTA per per-user segment of the batch: fp32 checkpoint mean + merge into the running
@@ -11,11 +13,14 @@
 //   k_score_scatter    explicit pairs: the fp32 checkpoint mean stored at the pair's index
 // No float atomics: the ranking order (score descending, item ascending, NaN last, empty slots after everything) is a
 // strict total order on distinct items, so the top-k of a user does not depend on where batch boundaries fall.
+#include <cub/device/device_segmented_radix_sort.cuh>
+
 #include "common.cuh"
 #include "../../include/igmc_b200.h"
 
 namespace {
 
+constexpr int LIST_THREADS = 256;
 constexpr int PLAN_THREADS = 1024;
 constexpr int PAIR_THREADS = 512;
 constexpr int MERGE_THREADS = 256;
@@ -111,6 +116,67 @@ __global__ void __launch_bounds__(PLAN_THREADS) k_candidate_plan(igmc_csr_t G, i
   }
 }
 
+__global__ void k_segment_offsets(int32_t* __restrict__ off, int U, int width) {
+  for (int j = blockIdx.x * blockDim.x + threadIdx.x; j <= U; j += gridDim.x * blockDim.x) off[j] = j * width;
+}
+
+// one CTA per query slot j over its sorted row srt[j*width, (j+1)*width): the items kept are in [0, num_items), not
+// equal to their predecessor and (exclude_rated) not rated by the user.  Counting pass (WRITE = false): the count goes
+// to user_off[j] and ids outside [-1, num_items) set the error; writing pass: the kept items, ascending, from lists[
+// user_off[j]] on.
+template <bool WRITE>
+__global__ void __launch_bounds__(LIST_THREADS)
+k_lists_rows(igmc_csr_t G, igmc_candidates_t Cd, const int32_t* __restrict__ srt, int width, int32_t* __restrict__ lists,
+             int* err) {
+  __shared__ long long ws[33];
+  const int j = blockIdx.x;
+  const int u = Cd.users[j];
+  const bool user_ok = u >= 0 && u < G.num_users;
+  if (!user_ok) {
+    if (!WRITE && threadIdx.x == 0) {
+      igmc_set_err(err, IGMC_ERR_CANDIDATES);
+      Cd.user_off[j] = 0;
+    }
+    return;
+  }
+  const int32_t* row = srt + (size_t)j * width;
+  const int32_t* rated = G.col_idx + G.row_ptr[u];
+  const int nr = G.row_ptr[u + 1] - G.row_ptr[u];
+  const long long out0 = WRITE ? Cd.user_off[j] : 0;
+  long long carry = 0;
+  for (int c0 = 0; c0 < width; c0 += blockDim.x) {
+    const int t = c0 + threadIdx.x;
+    bool keep = false;
+    if (t < width) {
+      const int x = row[t];
+      if (!WRITE && (x < -1 || x >= G.num_items)) igmc_set_err(err, IGMC_ERR_CANDIDATES);
+      keep = x >= 0 && x < G.num_items && (t == 0 || row[t - 1] != x) &&
+             !(Cd.exclude_rated && find_sorted(rated, nr, x) >= 0);
+    }
+    long long tot;
+    const long long off = block_excl_scan_ll(keep ? 1 : 0, ws, &tot);
+    if (WRITE && keep) lists[out0 + carry + off] = row[t];
+    carry += tot;
+  }
+  if (!WRITE && threadIdx.x == 0) Cd.user_off[j] = carry;
+}
+
+// user_off[0..U) holds the per-user counts: turn it into their exclusive prefix, user_off[U] = the total
+__global__ void __launch_bounds__(PLAN_THREADS) k_lists_scan(igmc_candidates_t Cd) {
+  __shared__ long long ws[33];
+  const int U = Cd.num_query;
+  long long carry = 0;
+  for (int base = 0; base < U; base += blockDim.x) {
+    const int j = base + threadIdx.x;
+    const long long cnt = j < U ? Cd.user_off[j] : 0;
+    long long tot;
+    const long long off = block_excl_scan_ll(cnt, ws, &tot);
+    if (j < U) Cd.user_off[j] = carry + off;
+    carry += tot;
+  }
+  if (threadIdx.x == 0) Cd.user_off[U] = carry;
+}
+
 __global__ void __launch_bounds__(PAIR_THREADS)
 k_candidate_pairs(igmc_csr_t G, igmc_candidates_t Cd, int64_t* __restrict__ cursor, int B,
                   int32_t* __restrict__ links_u, int32_t* __restrict__ links_v, int64_t* __restrict__ pair_id,
@@ -139,7 +205,9 @@ k_candidate_pairs(igmc_csr_t G, igmc_candidates_t Cd, int64_t* __restrict__ curs
       const long long c = g - Cd.user_off[lo];
       u = Cd.users[lo];
       long long p = c;
-      if (Cd.exclude_rated) {
+      if (Cd.per_user) {
+        p = Cd.user_off[lo] + c;    // the user's own list in cand; its rated items are already gone
+      } else if (Cd.exclude_rated) {
         // candidate rank c -> list position c + t, t = number of rated positions r_q with r_q - q <= c (r_q - q counts
         // the unrated positions below r_q, non-decreasing in q)
         const int32_t* r;
@@ -158,7 +226,7 @@ k_candidate_pairs(igmc_csr_t G, igmc_candidates_t Cd, int64_t* __restrict__ curs
         }
         p = c + a;
       }
-      const long long lim = Cd.cand ? Cd.num_cand : G.num_items;
+      const long long lim = Cd.per_user ? P : Cd.cand ? Cd.num_cand : G.num_items;
       if (p < 0 || p >= lim) {
         igmc_set_err(err, IGMC_ERR_CANDIDATES);
         p = 0;
@@ -268,11 +336,74 @@ extern "C" int igmc_candidate_plan(const igmc_csr_t* G, const igmc_candidates_t*
   return 0;
 }
 
+namespace {
+
+size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
+
+// the carve-up of igmc_candidate_lists' workspace: sorted rows [U * width], segment offsets [U + 1], CUB scratch
+struct ListsLayout {
+  int32_t *srt, *seg;
+  void* temp;
+  size_t temp_bytes, total;
+};
+
+ListsLayout lists_layout(void* base, int U, int width, cudaStream_t st) {
+  ListsLayout L = {};
+  unsigned char* b = static_cast<unsigned char*>(base);
+  const size_t a = align256((size_t)U * width * 4), s = align256(((size_t)U + 1) * 4);
+  L.srt = b ? reinterpret_cast<int32_t*>(b) : nullptr;
+  L.seg = b ? reinterpret_cast<int32_t*>(b + a) : nullptr;
+  cub::DeviceSegmentedRadixSort::SortKeys(nullptr, L.temp_bytes, (const int32_t*)nullptr, (int32_t*)nullptr,
+                                          U * width, U, (const int32_t*)nullptr, (const int32_t*)nullptr, 0, 32, st);
+  L.temp = b ? b + a + s : nullptr;
+  L.total = a + s + align256(L.temp_bytes);
+  return L;
+}
+
+bool lists_shape_ok(int U, int width) { return U >= 0 && width >= 0 && (long long)U * width < (1ll << 31) - 1; }
+
+}  // namespace
+
+extern "C" int igmc_candidate_lists_ws_bytes(int num_query, int width, int64_t* bytes) {
+  if (!bytes || !lists_shape_ok(num_query, width)) return -1;
+  *bytes = (int64_t)lists_layout(nullptr, num_query, width, 0).total;
+  return 0;
+}
+
+extern "C" int igmc_candidate_lists(const igmc_csr_t* G, const igmc_candidates_t* Cd, const int32_t* rows, int width,
+                                    int32_t* lists, void* ws, int64_t ws_bytes, int* err, void* stream) {
+  if (!G || !Cd || !Cd->users || !Cd->user_off || !lists_shape_ok(Cd->num_query, width)) return -1;
+  const int U = Cd->num_query;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (U == 0 || width == 0) {
+    cudaMemsetAsync(Cd->user_off, 0, ((size_t)U + 1) * sizeof(int64_t), st);
+    IGMC_CUDA_CHECK_LAUNCH();
+    return 0;
+  }
+  if (!rows || !lists || !ws) return -1;
+  const ListsLayout L = lists_layout(ws, U, width, st);
+  if ((int64_t)L.total > ws_bytes) return -2;
+  k_segment_offsets<<<(U + 1 + 255) / 256, 256, 0, st>>>(L.seg, U, width);
+  IGMC_CUDA_CHECK_LAUNCH();
+  size_t tb = L.temp_bytes;
+  if (cub::DeviceSegmentedRadixSort::SortKeys(L.temp, tb, rows, L.srt, U * width, U, L.seg, L.seg + 1, 0, 32, st) !=
+      cudaSuccess)
+    return -3;
+  k_lists_rows<false><<<U, LIST_THREADS, 0, st>>>(*G, *Cd, L.srt, width, lists, err);
+  IGMC_CUDA_CHECK_LAUNCH();
+  k_lists_scan<<<1, PLAN_THREADS, 0, st>>>(*Cd);
+  IGMC_CUDA_CHECK_LAUNCH();
+  k_lists_rows<true><<<U, LIST_THREADS, 0, st>>>(*G, *Cd, L.srt, width, lists, err);
+  IGMC_CUDA_CHECK_LAUNCH();
+  return 0;
+}
+
 extern "C" int igmc_candidate_pairs(const igmc_csr_t* G, const igmc_candidates_t* Cd, int64_t* cursor, int B,
                                     int32_t* links_u, int32_t* links_v, int64_t* pair_id, int64_t* tag, int* err,
                                     void* stream) {
   if (!G || !Cd || !cursor || B <= 0 || Cd->num_pairs <= 0) return -1;
   if (Cd->users ? !Cd->user_off : (!Cd->pair_u || !Cd->pair_v)) return -1;
+  if (Cd->per_user && (!Cd->users || !Cd->cand)) return -1;
   k_candidate_pairs<<<1, PAIR_THREADS, 0, (cudaStream_t)stream>>>(*G, *Cd, cursor, B, links_u, links_v, pair_id, tag,
                                                                    err);
   IGMC_CUDA_CHECK_LAUNCH();

@@ -6,8 +6,11 @@ building a dataset of every candidate pair and looping over it in Python.  Here:
 
 * ``predict_pairs(model, graph, users, items)`` -> fp32 scores of the explicit pairs ``(users[i], items[i])``;
 * ``recommend(model, graph, users, k)`` -> per query user the ``k`` best candidate items and their scores (candidates:
-  ``items`` or every item, without the user's rated items when ``exclude_rated``), ranked by score descending, then
-  item ascending; a NaN score ranks last; missing slots hold item -1 and score -inf;
+  ``items``, per-user lists ``items[U, width]``, the retriever's ``retrieve=M`` items or every item, without the
+  user's rated items when ``exclude_rated``), ranked by score descending, then item ascending; a NaN score ranks
+  last; missing slots hold item -1 and score -inf;
+* ``corated_items(graph, users, m)`` -> per query user the ``m`` items with the most bridges (3-paths u - i - u' - v,
+  ``igmc_corated_items``): the cheap first stage that proposes each user's candidates for the model to rank;
 * ``InferenceEngine``: the pipelined, graph-replayed loop behind both.  Per step the side stream produces the next
   batch's candidate pairs (``igmc_candidate_pairs``, from a device cursor) and extracts it while the main stream runs
   the eval forward of the current batch (once per checkpoint) and merges its scores into the running per-user top-k
@@ -28,7 +31,7 @@ from . import _lib
 from .train_eval import replay_step
 from .util_functions import RatingGraph, SubgraphExtractor, _stream_ptr
 
-__all__ = ["predict_pairs", "recommend", "InferenceEngine"]
+__all__ = ["predict_pairs", "recommend", "corated_items", "InferenceEngine"]
 
 
 # ---- input validation (host) ----------------------------------------------------------------------------------------
@@ -46,6 +49,56 @@ def _host_ids(a, name, hi):
     if lo < 0 or top >= hi:
         raise IndexError("%s: id %d out of range [0, %d)" % (name, lo if lo < 0 else top, hi))
     return a
+
+
+def _is_rows(items):
+    """a 2-D ``items`` names per-user candidate lists"""
+    return items is not None and (items.dim() == 2 if torch.is_tensor(items) else np.ndim(items) == 2)
+
+
+def _user_rows(items, U, num_items, dev):
+    """per-user candidate rows [U, width] as an int32 device tensor.  Host arrays are checked here (IndexError for an
+    id outside [-1, num_items)); integer device tensors are used as they are and checked by the kernel.  ValueError
+    when the row count is not U."""
+    if not torch.is_tensor(items):
+        items = np.asarray(items)
+    if items.shape[0] != U:
+        raise ValueError("items has %d rows, one per query user is %d" % (items.shape[0], U))
+    if torch.is_tensor(items) and items.device.type == "cuda":
+        if items.is_floating_point() or items.is_complex() or items.dtype == torch.bool:
+            raise TypeError("items must be integer ids, not %s" % items.dtype)
+        return items.to(device=dev, dtype=torch.int32).contiguous()
+    a = np.asarray(items.cpu().numpy() if torch.is_tensor(items) else items)
+    if a.size and not np.issubdtype(a.dtype, np.integer):
+        raise TypeError("items must be integer ids, not %s" % a.dtype)
+    a = a.astype(np.int64)
+    if a.size and (a.min() < -1 or a.max() >= num_items):
+        bad = int(a.min()) if a.min() < -1 else int(a.max())
+        raise IndexError("items: id %d out of range [-1, %d)" % (bad, num_items))
+    return torch.from_numpy(a.astype(np.int32)).to(dev)
+
+
+def _check_m(m, num_items):
+    m = int(m)
+    if m < 1 or m > num_items:
+        raise ValueError("the number of retrieved items must lie in [1, %d], not %d" % (num_items, m))
+    return m
+
+
+def _corated(lib, g, users, m, exclude_rated, err, ws):
+    """igmc_corated_items for the int32 device tensor ``users`` on graph ``g``: (items, paths) [U, m] int32.  ``ws``: a
+    dict whose "ws" tensor is grown to the workspace the shape needs"""
+    U, dev = int(users.numel()), g.device
+    nbytes = C.c_int64(0)
+    _lib.check(lib.igmc_corated_ws_bytes(g.num_users, g.num_items, U, m, C.byref(nbytes)), "igmc_corated_ws_bytes")
+    if ws.get("ws") is None or ws["ws"].numel() < nbytes.value:
+        ws["ws"] = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=dev)
+    items = torch.empty(U, m, dtype=torch.int32, device=dev)
+    paths = torch.empty(U, m, dtype=torch.int32, device=dev)
+    _lib.check(lib.igmc_corated_items(C.byref(g._c), users.data_ptr(), U, m, int(bool(exclude_rated)),
+                                      ws["ws"].data_ptr(), ws["ws"].numel(), items.data_ptr(), paths.data_ptr(),
+                                      err.data_ptr(), _stream_ptr()), "igmc_corated_items")
+    return items, paths
 
 
 def _check_k(k):
@@ -142,6 +195,48 @@ def topk_merge_host(top_s, top_i, seg_s, seg_i):
     return out_s, out_i
 
 
+def corated_host(row_ptr, col_idx, num_users, num_items, users, m, exclude_rated=True):
+    """twin of igmc_corated_items: per query user the ``m`` items with the most bridges, paths[v] = sum over u' != u
+    of |N(u) & N(u')| * [u' rated v] (B B^T B without the u' = u term), ordered by paths descending then item
+    ascending, items without a bridge dropped; (items [U, m], paths [U, m]) int32 padded with -1 / 0"""
+    import scipy.sparse as ssp
+    users = np.asarray(users, np.int64).reshape(-1)
+    rp = np.asarray(row_ptr, np.int64)
+    nnz = int(rp[num_users])
+    Bm = ssp.csr_matrix((np.ones(nnz, np.int64), np.asarray(col_idx[:nnz], np.int64), rp[:num_users + 1]),
+                        shape=(num_users, num_items))
+    Bu = Bm[users]                                           # [U, ni]
+    W = (Bu @ Bm.T).toarray()                                # |N(u) & N(u')|
+    W[np.arange(len(users)), users] = 0                      # u' != u
+    P = W @ Bm                                               # [U, ni] (dense @ sparse: dense)
+    P = np.asarray(P, np.int64)
+    if exclude_rated:
+        P[Bu.toarray() > 0] = 0
+    items = np.full((len(users), m), -1, np.int32)
+    paths = np.zeros((len(users), m), np.int32)
+    for j in range(len(users)):
+        o = np.argsort(-P[j], kind="stable")[:m]            # paths descending, then item ascending
+        o = o[P[j][o] > 0]
+        items[j, :len(o)], paths[j, :len(o)] = o, P[j][o]
+    return items, paths
+
+
+def candidate_lists_host(row_ptr, col_idx, num_items, users, rows, exclude_rated=True):
+    """twin of igmc_candidate_lists: (user_off [U+1] int64, lists) - per query slot its row sorted, deduplicated, -1
+    slots dropped and (exclude_rated) the user's rated items removed"""
+    users = np.asarray(users, np.int64).reshape(-1)
+    rows = np.asarray(rows, np.int64).reshape(len(users), -1)
+    out = []
+    for j, u in enumerate(users):
+        r = np.unique(rows[j])
+        r = r[(r >= 0) & (r < num_items)]
+        if exclude_rated:
+            r = r[~np.isin(r, np.asarray(col_idx[row_ptr[u]:row_ptr[u + 1]], np.int64))]
+        out.append(r)
+    user_off = np.concatenate([[0], np.cumsum([len(r) for r in out])]).astype(np.int64)
+    return user_off, (np.concatenate(out) if out else np.zeros(0, np.int64)).astype(np.int32)
+
+
 def rank_host(scores, items, k):
     """brute-force ranking: the first ``k`` of ``items`` by (score descending, item ascending, NaN last), padded
     with (-1, -inf)"""
@@ -212,24 +307,34 @@ class InferenceEngine(object):
         self.preds = torch.zeros(self.K, self.B, dtype=torch.float32, device=dev)
         self.side = torch.cuda.Stream(dev)
         self.run = None
+        self._retrieve_ws = {}       # the retriever's workspace when its histograms do not fit in shared memory
 
     # ---- one run: plan, prime, steps, finish --------------------------------------------------------------------
-    def start_recommend(self, users, k, items=None, exclude_rated=True):
-        """plan a ranking run (one host sync: the candidate total).  Returns the number of candidate pairs."""
+    def start_recommend(self, users, k, items=None, exclude_rated=True, retrieve=None):
+        """plan a ranking run (one host sync: the candidate total).  ``items``: one candidate list for every user, or
+        a 2-D [U, width] array of per-user lists (-1 = empty slot); ``retrieve=M``: each user's M items with the most
+        bridges (``corated_items``) are its candidates.  Returns the number of candidate pairs."""
         k = _check_k(k)
         g = self.graph
+        if retrieve is not None and items is not None:
+            raise ValueError("retrieve= chooses the candidates itself: pass it without items=")
+        per_user = retrieve is not None or _is_rows(items)
+        m = None if retrieve is None else _check_m(retrieve, g.num_items)
         users = _host_ids(users, "users", g.num_users)
-        cand = None if items is None else np.unique(_host_ids(items, "items", g.num_items))
+        cand = None if items is None or per_user else np.unique(_host_ids(items, "items", g.num_items))
         U, dev = len(users), self.dev
+        rows = _user_rows(items, U, g.num_items, dev) if per_user and m is None else None
         run = dict(kind="recommend", U=U, k=k, version=g.version,
                    top_s=torch.full((U, k), -float("inf"), dtype=torch.float32, device=dev),
                    top_i=torch.full((U, k), -1, dtype=torch.int64, device=dev))
         self.run = run
-        if U == 0 or (cand is not None and len(cand) == 0):
+        if U == 0 or (cand is not None and len(cand) == 0) or (rows is not None and rows.shape[1] == 0):
             run["P"] = 0
             return 0
         i64 = dict(dtype=torch.int64, device=dev)
         run["users"] = torch.from_numpy(users.astype(np.int32)).to(dev)
+        if per_user:
+            return self._plan_lists(run, rows, m, exclude_rated)
         run["cand"] = None if cand is None else torch.from_numpy(cand.astype(np.int32)).to(dev)
         run["user_off"] = torch.zeros(U + 1, **i64)
         lists = cand is not None and bool(exclude_rated)
@@ -246,6 +351,34 @@ class InferenceEngine(object):
         Cd.exclude_rated = int(bool(exclude_rated))
         _lib.check(self.lib.igmc_candidate_plan(C.byref(g._c), C.byref(Cd), self.extractor.err.data_ptr(),
                                                 _stream_ptr()), "igmc_candidate_plan")
+        Cd.num_pairs = run["P"] = int(run["user_off"][U].item())
+        run["Cd"] = Cd
+        if run["P"] > 0:
+            self._prime()
+        return run["P"]
+
+    def _plan_lists(self, run, rows, m, exclude_rated):
+        """the plan of a run over per-user candidate rows (``rows``, or the retriever's top ``m`` per user):
+        igmc_candidate_lists compacts them into run["lists"] and user_off"""
+        g, U, dev = self.graph, run["U"], self.dev
+        err = self.extractor.err
+        if rows is None:
+            rows, _ =_corated(self.lib, g, run["users"], m, exclude_rated, err, self._retrieve_ws)
+        width = int(rows.shape[1])
+        run["rows"] = rows
+        run["lists"] = torch.empty(max(U * width, 1), dtype=torch.int32, device=dev)
+        run["user_off"] = torch.zeros(U + 1, dtype=torch.int64, device=dev)
+        nbytes = C.c_int64(0)
+        _lib.check(self.lib.igmc_candidate_lists_ws_bytes(U, width, C.byref(nbytes)), "igmc_candidate_lists_ws_bytes")
+        run["lists_ws"] = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=dev)
+        Cd = _lib.Candidates()
+        Cd.users, Cd.user_off = run["users"].data_ptr(), run["user_off"].data_ptr()
+        Cd.num_query, Cd.exclude_rated = U, int(bool(exclude_rated))
+        _lib.check(self.lib.igmc_candidate_lists(C.byref(g._c), C.byref(Cd), rows.data_ptr(), width,
+                                                 run["lists"].data_ptr(), run["lists_ws"].data_ptr(),
+                                                 run["lists_ws"].numel(), err.data_ptr(), _stream_ptr()),
+                   "igmc_candidate_lists")
+        Cd.cand, Cd.per_user = run["lists"].data_ptr(), 1
         Cd.num_pairs = run["P"] = int(run["user_off"][U].item())
         run["Cd"] = Cd
         if run["P"] > 0:
@@ -370,8 +503,8 @@ class InferenceEngine(object):
             return run["top_i"], run["top_s"]
         return run["scores"]
 
-    def recommend(self, users, k, items=None, exclude_rated=True):
-        self.start_recommend(users, k, items, exclude_rated)
+    def recommend(self, users, k, items=None, exclude_rated=True, retrieve=None):
+        self.start_recommend(users, k, items, exclude_rated, retrieve)
         return self.finish()
 
     def predict_pairs(self, users, items):
@@ -402,22 +535,54 @@ def predict_pairs(model, graph, users, items, *, h=1, sample_ratio=1.0, max_node
         eng.close()
 
 
-def recommend(model, graph, users, k, *, items=None, exclude_rated=True, h=1, sample_ratio=1.0,
+def recommend(model, graph, users, k, *, items=None, exclude_rated=True, retrieve=None, h=1, sample_ratio=1.0,
               max_nodes_per_hop=None, batch_size=256, checkpoints=None, sample_seed=0):
     """for every query user the ``k`` best candidate items: (top_items [U, k] int64, top_scores [U, k] fp32), on the
-    model's device.  Candidates: ``items`` (sorted, deduplicated) or every item, minus the user's rated items when
-    ``exclude_rated``.  Order: score descending, then item ascending; a NaN score ranks last; a user with fewer than
-    ``k`` candidates gets item -1 / score -inf in the empty slots."""
+    model's device.  Candidates: ``items`` (sorted, deduplicated), a 2-D ``items`` [U, width] of per-user lists (-1 =
+    empty slot; each row sorted and deduplicated), the user's ``retrieve`` items with the most bridges
+    (``corated_items``), or every item; minus the user's rated items when ``exclude_rated``.  Order: score
+    descending, then item ascending; a NaN score ranks last; a user with fewer than ``k`` candidates gets item -1 /
+    score -inf in the empty slots.  A pair's score does not depend on the candidates it was ranked among."""
     k = _check_k(k)
     nu, ni = graph.shape
+    if retrieve is not None and items is not None:
+        raise ValueError("retrieve= chooses the candidates itself: pass it without items=")
+    if retrieve is not None:
+        _check_m(retrieve, ni)
     users = _host_ids(users, "users", nu)
-    if items is not None:
+    if _is_rows(items):
+        if torch.is_tensor(items) and items.device.type == "cuda":
+            if items.shape[0] != len(users):
+                raise ValueError("items has %d rows, one per query user is %d" % (items.shape[0], len(users)))
+        else:
+            items = _user_rows(items, len(users), ni, torch.device("cpu")).numpy()
+    elif items is not None:
         items = _host_ids(items, "items", ni)
     if len(users) == 0:
         dev = model.flat_params.device
         return (torch.zeros(0, k, dtype=torch.int64, device=dev), torch.zeros(0, k, dtype=torch.float32, device=dev))
     eng = InferenceEngine(model, graph, h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
     try:
-        return eng.recommend(users, k, items, exclude_rated)
+        return eng.recommend(users, k, items, exclude_rated, retrieve)
     finally:
         eng.close()
+
+
+def corated_items(graph, users, m, exclude_rated=True):
+    """per query user the ``m`` items with the most bridges to it: (items [U, m], paths [U, m]) int32 on the graph's
+    device.  paths[v] counts the 3-paths u - i - u' - v (u' != u): the edges that join u's and v's stars in their
+    h = 1 enclosing subgraph, without which the model has no collaborative signal for the pair.  Ordered by paths
+    descending, then item ascending; items without a bridge are never returned, the rest of a row is item -1 /
+    paths 0; ``exclude_rated`` drops the user's rated items.  Exact integer counts: runs are bit-identical.
+    ``graph``: a RatingGraph or a rating matrix (copied to the current CUDA device).  One host synchronisation (the
+    error word)."""
+    g = graph if isinstance(graph, RatingGraph) else RatingGraph(graph)
+    if g.device is None:
+        raise RuntimeError("igmc_b200 retrieval runs on a CUDA device (there is no CPU path)")
+    m = _check_m(m, g.num_items)
+    users = _host_ids(users, "users", g.num_users)
+    lib = _lib.load()
+    err = torch.zeros(1, dtype=torch.int32, device=g.device)
+    items, paths = _corated(lib, g, torch.from_numpy(users.astype(np.int32)).to(g.device), m, exclude_rated, err, {})
+    _lib.check_kernel_error(int(err.item()))
+    return items, paths

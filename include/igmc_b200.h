@@ -415,7 +415,9 @@ int igmc_sortpool_backward(const igmc_sortpool_t* P, const float* params, const 
 #define IGMC_TOPK_MAX 256
 typedef struct {
   const int32_t* users;     /* recommend: [num_query] query users; NULL selects explicit pairs (pair_u, pair_v) */
-  const int32_t* cand;      /* recommend: [num_cand] ascending, unique candidate items; NULL = every item of G */
+  const int32_t* cand;      /* recommend: [num_cand] ascending, unique candidate items; NULL = every item of G.  With
+                             * per_user: every query user's own list (igmc_candidate_lists), j's at [user_off[j],
+                             * user_off[j+1]) */
   const int32_t* pair_u;    /* explicit pairs: [num_pairs] user / item of pair i */
   const int32_t* pair_v;
   int64_t* user_off;        /* recommend: [num_query+1] exclusive prefix of the per-user candidate counts (the plan) */
@@ -423,13 +425,26 @@ typedef struct {
   int32_t* rated_pos;       /* recommend with cand and exclude_rated: [sum of the query users' degrees] ascending
                              * positions in cand of each user's rated items (|row(u) & cand| entries per user) */
   int64_t num_pairs;        /* candidate pairs in all (recommend: user_off[num_query], known once the plan ran) */
-  int32_t num_query, num_cand, exclude_rated, pad_;
+  int32_t num_query, num_cand, exclude_rated;
+  int32_t per_user;         /* 0: cand is one list shared by every query user (or NULL); 1: cand holds per-user lists
+                             * and user_off from igmc_candidate_lists (which replaces igmc_candidate_plan) */
 } igmc_candidates_t;
 
 /* Per query user the number of candidate items (cand or every item, minus the user's rated items when exclude_rated:
  * num_items - deg(u) without a list) and their exclusive prefix user_off; with a list and exclude_rated also rated_off /
  * rated_pos.  ONE single-CTA launch.  User ids outside G set IGMC_ERR_CANDIDATES (and count 0). */
 int igmc_candidate_plan(const igmc_csr_t* G, const igmc_candidates_t* Cd, int* err, void* stream);
+
+/* Per-user candidate lists: `rows` [num_query, width] int32 names query slot j's candidate items, -1 = an empty slot.
+ * The plan of a per_user run: every row sorted ascending (segmented radix sort into the workspace), deduplicated,
+ * without the user's rated items when exclude_rated, written compactly to `lists` ([num_query * width] capacity)
+ * at [user_off[j], user_off[j+1]), and the exclusive prefix user_off [num_query+1] of the counts.  Ids outside
+ * [-1, num_items) and user ids outside G set IGMC_ERR_CANDIDATES (the slot / the user counts nothing).  Afterwards
+ * set Cd->cand = lists, Cd->per_user = 1 and Cd->num_pairs = user_off[num_query] for igmc_candidate_pairs.
+ * num_query * width < 2^31 - 1. */
+int igmc_candidate_lists_ws_bytes(int num_query, int width, int64_t* bytes);
+int igmc_candidate_lists(const igmc_csr_t* G, const igmc_candidates_t* Cd, const int32_t* rows, int width,
+                         int32_t* lists, void* ws, int64_t ws_bytes, int* err, void* stream);
 
 /* The pairs of global candidate positions [*cursor, *cursor + B) (positions ordered by query slot, then item), then
  * *cursor += B: `cursor` is a device word, so a captured graph replays with no host input.  Writes links_u / links_v /
@@ -450,6 +465,22 @@ int igmc_topk_merge(const float* preds, int K, int B, const int64_t* tag, const 
 
 /* Explicit pairs: scores[tag[i]] = the same fp32 checkpoint mean for every i with tag[i] >= 0. */
 int igmc_score_scatter(const float* preds, int K, int B, const int64_t* tag, float* scores, void* stream);
+
+/* ---- candidate retrieval by bridge count (csrc/retrieve.cu) ----
+ * For h = 1 the enclosing subgraph of an unrated pair (u, v) joins u's star and v's star only through the bridge edges
+ * (u', i): u' != u rated v and i, u rated i.  Their number is
+ *   paths[v] = sum over u' != u of |N(u) & N(u')| * [u' rated v]
+ * (the 3-paths u - i - u' - v).  Per query user the m items with the most bridges: items [num_query, m] and paths
+ * [num_query, m] int32, ordered by paths descending, then item ascending; items with no bridge are never returned and
+ * the rest of a row is item -1 / paths 0.  exclude_rated drops the user's rated items.  One CTA per user: pass 1 pushes
+ * w[u'] (integer atomics, sum over i in N(u) of deg(i)), pass 2 pulls paths[v] = sum over col(v) of w (nnz reads), a
+ * radix select of the m-th count (ties at it in ascending item order) and a bitonic sort of the chosen keys.  The
+ * histograms w [num_users] and paths [num_items] live in shared memory when they fit, else in a workspace row per CTA
+ * of a fixed grid (igmc_corated_ws_bytes: 0 in the shared-memory regime).  Integer arithmetic only: bit-identical
+ * across runs.  User ids outside G set IGMC_ERR_CANDIDATES (their row is padding).  1 <= m <= num_items. */
+int igmc_corated_ws_bytes(int num_users, int num_items, int num_query, int m, int64_t* bytes);
+int igmc_corated_items(const igmc_csr_t* G, const int32_t* users, int num_query, int m, int exclude_rated, void* ws,
+                       int64_t ws_bytes, int32_t* items, int32_t* paths, int* err, void* stream);
 
 /* ---- in-place update of the rating graph (csrc/graph_update.cu) ----
  * The reference can only change its rating matrix by rebuilding everything from a new scipy matrix.  Here a delta of D
