@@ -49,8 +49,14 @@ constexpr int SEG = 32;        // edges per segment
 constexpr int XR = 16;         // extra staging rows per chunk
 constexpr int XCH = 8;         // chunks that may use extra rows
 
-// staged list entry: type << 24 | swizzled float offset of the neighbour's feature row ((nbr << 5) | ((nbr & 7) << 2)),
-// so that the edge loop gets a lane's address with one LOP3 (offset ^ column) instead of re-deriving the swizzle
+// staged list entry: type << 24 | RUN_END | swizzled float offset of the neighbour's feature row
+// ((nbr << 5) | ((nbr & 7) << 2), below 2^21), so that the edge loop gets a lane's address with one LOP3
+// ((entry & ENT_OFF) ^ column) instead of re-deriving the swizzle.  RUN_END marks the last entry of a type run within
+// its segment (set by stage_lists once the segments are known).
+constexpr uint32_t ENT_OFF = 0x1fffffu;
+constexpr uint32_t RUN_END = 1u << 21;
+// seg_row of a staged segment: staging row | types present in the segment << 16 (rows are below 2^16, R <= 12)
+constexpr int SEG_ROW = 0xffff;
 __device__ __forceinline__ uint32_t enc_entry(uint32_t ent) {
   const uint32_t nbr = ent & 0xffffu;
   return ((ent >> 16) << 24) | (nbr << 5) | ((nbr & 7u) << 2);
@@ -211,6 +217,26 @@ __device__ __forceinline__ Lists stage_lists(const uint32_t* adj, const int32_t*
     }
   }
   __syncthreads();
+  // run structure of the staged segments (warp per segment): lists are sorted by (type, neighbour), so every type
+  // is at most one run of a segment; its last entry gets RUN_END and the segment's row its type mask
+  if (staged) {
+    const int nseg = segbase[n_own];
+    for (int sg = warp; sg < nseg; sg += nwarps) {
+      const int p0 = seg_p0[sg], p1 = seg_p1[sg];
+      uint32_t types = 0;
+      for (int c = p0; c < p1; c += 32) {
+        const int p = c + lane;
+        const uint32_t e = p < p1 ? lbuf[p] : 0u, en = p + 1 < p1 ? lbuf[p + 1] : 0u;
+        __syncwarp();   // every lane has read its successor before any flag is written
+        if (p < p1) {
+          types |= 1u << (e >> 24);
+          if (p + 1 == p1 || (en >> 24) != (e >> 24)) lbuf[p] = e | RUN_END;
+        }
+      }
+      types = __reduce_or_sync(IGMC_FULL, types);
+      if (lane == 0) seg_row[sg] |= (int)(types << 16);
+    }
+  }
   // hand-out order: within every chunk, segments by decreasing length (rank sort, ties by index)
   {
     const int nseg = segbase[n_own];
@@ -277,7 +303,7 @@ __device__ __forceinline__ void rel_inv_deg_own(const Lists& Ls, const EdgeKeep&
 template <int GL, bool PR = false>
 __device__ __forceinline__ void gather_segments(const Lists& Ls, const EdgeKeep& K, int sg0, int sg1, int lane,
                                                 const float* __restrict__ feat, float* __restrict__ stage, int SS,
-                                                int inp, int* ticket, const float* rinv = nullptr, int R = 0) {
+                                                int inp, int R, int* ticket, const float* rinv = nullptr) {
   const int q = lane & (GL - 1);
   const int fo = 4 * q;
   const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -291,36 +317,38 @@ __device__ __forceinline__ void gather_segments(const Lists& Ls, const EdgeKeep&
     float* rowb = stage;
     int p = 0, p1 = 0;
     if (valid) {
-      rowb = stage + (size_t)Ls.seg_row[sg] * SS;
-      for (int i = q * 4; i < SS; i += 4 * GL) *reinterpret_cast<float4*>(rowb + i) = z4;
+      const int sr = Ls.seg_row[sg];
+      rowb = stage + (size_t)(sr & SEG_ROW) * SS;
+      if (Ls.lst) {
+        // every type present gets one plain store of its run below: zero only the blocks of the other types (a
+        // lane owns column fo of every block) and the padding behind the last block
+        if (fo < inp)
+          for (uint32_t m = ~((uint32_t)sr >> 16) & ((1u << R) - 1u); m; m &= m - 1u)
+            *reinterpret_cast<float4*>(rowb + (__ffs(m) - 1) * inp + fo) = z4;
+        for (int i = R * inp + fo; i < SS; i += 4 * GL) *reinterpret_cast<float4*>(rowb + i) = z4;
+      } else {
+        for (int i = fo; i < SS; i += 4 * GL) *reinterpret_cast<float4*>(rowb + i) = z4;
+      }
       if (fo < inp) { p = Ls.seg_p0[sg]; p1 = Ls.seg_p1[sg]; }
     }
     __syncwarp();
     float* row = rowb + fo;
     if (Ls.lst) {
-      // lists arrive sorted by (type, neighbour): sum each type run in registers, touch the staging row once
-      // per run (still a read-modify-write, so any order stays correct - unsorted lists just flush more often)
+      // each type run is summed in registers from zero, in list order, and written with one plain store at its
+      // RUN_END entry (the last entry of a segment always carries it): the row equals the zeroed row plus the run
       const uint32_t* lst = Ls.lst;
       float4 acc = z4;
-      int cur = -1;
-#define IGMC_HROW(e_) (PR ? scale_row(*reinterpret_cast<const float4*>(feat + (((e_) & 0xffffffu) ^ (uint32_t)fo)), \
-                                      __ldcg(rinv + (int)(((e_) & 0xffffffu) >> 5) * R + (int)((e_) >> 24)))       \
-                         : *reinterpret_cast<const float4*>(feat + (((e_) & 0xffffffu) ^ (uint32_t)fo)))
-#define IGMC_STEP(e_, a_)                                                            \
-      do {                                                                           \
-        const int ty_ = (int)((e_) >> 24);                                           \
-        if (ty_ != cur) {                                                            \
-          if (cur >= 0) {                                                            \
-            float4* d_ = reinterpret_cast<float4*>(row + cur * inp);                 \
-            float4 t_ = *d_;                                                         \
-            t_.x += acc.x; t_.y += acc.y; t_.z += acc.z; t_.w += acc.w;              \
-            *d_ = t_;                                                                \
-          }                                                                          \
-          acc = (a_);                                                                \
-          cur = ty_;                                                                 \
-        } else {                                                                     \
-          acc.x += (a_).x; acc.y += (a_).y; acc.z += (a_).z; acc.w += (a_).w;        \
-        }                                                                            \
+#define IGMC_HROW(e_) (PR ? scale_row(*reinterpret_cast<const float4*>(feat + (((e_) & ENT_OFF) ^ (uint32_t)fo)), \
+                                      __ldcg(rinv + (int)(((e_) & ENT_OFF) >> 5) * R + (int)((e_) >> 24)))       \
+                         : *reinterpret_cast<const float4*>(feat + (((e_) & ENT_OFF) ^ (uint32_t)fo)))
+#define IGMC_STEP(e_, a_)                                                                             \
+      do {                                                                                            \
+        acc.x = __fadd_rn(acc.x, (a_).x); acc.y = __fadd_rn(acc.y, (a_).y);                           \
+        acc.z = __fadd_rn(acc.z, (a_).z); acc.w = __fadd_rn(acc.w, (a_).w);                           \
+        if ((e_) & RUN_END) {                                                                         \
+          *reinterpret_cast<float4*>(row + (int)((e_) >> 24) * inp) = acc;                            \
+          acc = z4;                                                                                   \
+        }                                                                                             \
       } while (0)
       // four edges in flight: the entry and source-row loads of a batch are independent
       for (; p + 4 <= p1; p += 4) {
@@ -332,12 +360,6 @@ __device__ __forceinline__ void gather_segments(const Lists& Ls, const EdgeKeep&
         const uint32_t e0 = lst[p];
         const float4 a0 = IGMC_HROW(e0);
         IGMC_STEP(e0, a0);
-      }
-      if (cur >= 0) {
-        float4* d = reinterpret_cast<float4*>(row + cur * inp);
-        float4 t = *d;
-        t.x += acc.x; t.y += acc.y; t.z += acc.z; t.w += acc.w;
-        *d = t;
       }
 #undef IGMC_STEP
 #undef IGMC_HROW
@@ -674,8 +696,8 @@ __device__ __forceinline__ bool forward_body(const igmc_model_t& M, const float*
       // ---- aggregate: one 8-lane group per list segment ----
 #define IGMC_STAMP_T(t_, i_) do { if (S.prof && l == 1 && threadIdx.x == (t_)) S.prof[(size_t)blockIdx.x * 64 + (i_)] = clock64(); } while (0)
       IGMC_STAMP_T(0, 39); IGMC_STAMP_T(992, 49);
-      if (inp == 4) gather_segments<1>(Ls, K, Ls.segbase[c0], Ls.segbase[c0 + crow], lane, H, stage, SS, inp, &ws[33]);
-      else gather_segments<8>(Ls, K, Ls.segbase[c0], Ls.segbase[c0 + crow], lane, H, stage, SS, inp, &ws[33]);
+      if (inp == 4) gather_segments<1>(Ls, K, Ls.segbase[c0], Ls.segbase[c0 + crow], lane, H, stage, SS, inp, R, &ws[33]);
+      else gather_segments<8>(Ls, K, Ls.segbase[c0], Ls.segbase[c0 + crow], lane, H, stage, SS, inp, R, &ws[33]);
       IGMC_STAMP_T(0, 40); IGMC_STAMP_T(992, 43); IGMC_STAMP_T(480, 46);
       if (l == 0) IGMC_STAMP(32);
       __syncthreads();
@@ -1034,8 +1056,7 @@ __device__ __forceinline__ void backward_body(const igmc_model_t& M, const float
         }
         // (1) data gradient of the own nodes:  d h_{l-1}[u] = [Q[u] | dpre[u]] . [W_r^T ; root^T],
         //     Q[u,r,:] = sum_{(u->d) of type r, kept} dpre[d,:]/deg(d)         -> pushed to every CTA's DH
-        gather_segments<8, PR>(Ls, K, Ls.segbase[c0], Ls.segbase[c0 + crow], lane, DPS, stage, SS, HID, &ws[33], rinv,
-                               R);
+        gather_segments<8, PR>(Ls, K, Ls.segbase[c0], Ls.segbase[c0 + crow], lane, DPS, stage, SS, HID, R, &ws[33], rinv);
         __syncthreads();
         if (tid == 0) ws[33] = 0;
         {   // fold the extra segments of long lists into their node row
