@@ -181,7 +181,13 @@ _SIGS = {
     "igmc_score_scatter": [vp, C.c_int, C.c_int, vp, vp, vp],
     "igmc_candidate_lists_ws_bytes": [C.c_int, C.c_int, C.POINTER(C.c_int64)],
     "igmc_candidate_lists": [C.POINTER(CSR), C.POINTER(Candidates), vp, C.c_int, vp, vp, C.c_int64, vp, vp],
-    "igmc_corated_ws_bytes": [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int64)],
+    "igmc_explain_count": [vp, vp, C.c_int, vp, vp],
+    "igmc_explain_offsets": [vp, C.c_int, vp, vp],
+    "igmc_occlusion_pairs": [C.POINTER(CSR), vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp],
+    "igmc_occlusion_mask": [C.POINTER(BatchOut), C.c_int, vp, vp, vp, vp, vp, vp, vp, vp],
+    "igmc_occlusion_order_ws_bytes": [C.c_int, C.c_int64, C.POINTER(C.c_int64)],
+    "igmc_occlusion_order": [vp, vp, vp, C.c_int, C.c_int64, vp, vp, vp, C.c_int, vp, C.c_int64, vp, vp, vp, vp, vp],
+    "igmc_corated_ws_bytes":[C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int64)],
     "igmc_corated_items": [C.POINTER(CSR), vp, C.c_int, C.c_int, C.c_int, vp, C.c_int64, vp, vp, vp, vp],
     "igmc_graph_update_ws_bytes": [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int64)],
     "igmc_graph_update_plan": [C.POINTER(CSR), C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, C.c_int, C.c_int,

@@ -11,7 +11,10 @@ building a dataset of every candidate pair and looping over it in Python.  Here:
   last; missing slots hold item -1 and score -inf;
 * ``corated_items(graph, users, m)`` -> per query user the ``m`` items with the most bridges (3-paths u - i - u' - v,
   ``igmc_corated_items``): the cheap first stage that proposes each user's candidates for the model to rank;
-* ``InferenceEngine``: the pipelined, graph-replayed loop behind both.  Per step the side stream produces the next
+* ``explain_pairs(model, graph, users, items, m)`` -> per pair its score and, for every rating in its enclosing
+  subgraph, the score change from removing that rating (csrc/explain.cu): a base pass of the pairs, then an occlusion
+  pass over (pair, rating) positions whose batches carry an edge mask into a training-mode forward without dropout;
+* ``InferenceEngine``: the pipelined, graph-replayed loop behind all of them.  Per step the side stream produces the next
   batch's candidate pairs (``igmc_candidate_pairs``, from a device cursor) and extracts it while the main stream runs
   the eval forward of the current batch (once per checkpoint) and merges its scores into the running per-user top-k
   lists (``igmc_topk_merge``) or scatters them to their pair index (``igmc_score_scatter``).  The step is one CUDA graph
@@ -21,6 +24,7 @@ Every pair samples its subgraph with ``pair_id = u * num_items + v``: its subgra
 the API that scored it, the batch it fell into or the candidate list.  The host twins below restate the kernels'
 integer arithmetic for the CPU tests (tests/test_recommend_host.py).
 """
+import collections
 import contextlib
 import ctypes as C
 
@@ -31,7 +35,7 @@ from . import _lib
 from .train_eval import replay_step
 from .util_functions import RatingGraph, SubgraphExtractor, _stream_ptr
 
-__all__ = ["predict_pairs", "recommend", "corated_items", "InferenceEngine"]
+__all__ = ["predict_pairs", "recommend", "corated_items", "explain_pairs", "Explanation", "InferenceEngine"]
 
 
 # ---- input validation (host) ----------------------------------------------------------------------------------------
@@ -108,6 +112,25 @@ def _check_k(k):
     if k > _lib.TOPK_MAX:
         raise NotImplementedError("the top-k merge kernel keeps at most k = %d items per user" % _lib.TOPK_MAX)
     return k
+
+
+def _check_top(m, name):
+    """None, or a count in [1, IGMC_TOPK_MAX] of entries to keep per pair"""
+    if m is None:
+        return None
+    m = int(m)
+    if m < 1:
+        raise ValueError("%s must be >= 1, not %d" % (name, m))
+    if m > _lib.TOPK_MAX:
+        raise NotImplementedError("an explanation keeps at most %s = %d ratings per pair" % (name, _lib.TOPK_MAX))
+    return m
+
+
+# The result of explain_pairs, device tensors: score [P] fp32 (= predict_pairs), num_edges [P] int32 (the ratings of
+# each pair's subgraph), offsets [P+1] int64 (their exclusive prefix) and, per rating, user / item / rating int32 and
+# delta fp32 (score without the rating - score): flat [offsets[P]] with pair p at [offsets[p], offsets[p+1]), or
+# [P, m] padded with -1 / -1 / -1 / 0.
+Explanation = collections.namedtuple("Explanation", "score num_edges offsets user item rating delta")
 
 
 # ---- host twins of the candidate and merge kernels (csrc/recommend.cu) ----------------------------------------------
@@ -250,6 +273,62 @@ def rank_host(scores, items, k):
     return top_s, top_i
 
 
+# ---- host twins of the explanation kernels (csrc/explain.cu) --------------------------------------------------------
+def explain_offsets_host(num_edges):
+    """twin of igmc_explain_offsets: the exclusive int64 prefix [P+1] of the per-pair rating counts"""
+    return np.concatenate([[0], np.cumsum(np.asarray(num_edges, np.int64))]).astype(np.int64)
+
+
+def occlusion_pairs_host(offsets, pair_u, pair_v, num_items, pos, B):
+    """twin of igmc_occlusion_pairs for positions [pos, pos + B): (links_u, links_v, pair_id, tag, edge_j)"""
+    offsets = np.asarray(offsets, np.int64)
+    P, T = len(offsets) - 1, int(offsets[-1])
+    out = np.zeros((5, B), np.int64)
+    for i in range(B):
+        c = pos + i
+        real = c < T
+        if not real:
+            c = T - 1
+        q = min(int(np.searchsorted(offsets, c, side="right")) - 1, P - 1)     # the last q with offsets[q] <= c
+        u, v = int(pair_u[q]), int(pair_v[q])
+        out[:, i] = (u, v, u * num_items + v, c if real else -1, c - offsets[q])
+    return out
+
+
+def occlusion_mask_host(edge_ptr, tag, edge_j):
+    """twin of igmc_occlusion_mask's edge_keep [edge_ptr[B]]: graph g with tag >= 0 drops its directed edges
+    edge_ptr[g] + j and edge_ptr[g] + E_g/2 + j"""
+    edge_ptr = np.asarray(edge_ptr, np.int64)
+    keep = np.ones(int(edge_ptr[-1]), np.uint8)
+    for g in range(len(edge_ptr) - 1):
+        m = int(edge_ptr[g + 1] - edge_ptr[g]) // 2
+        if tag[g] >= 0 and 0 <= edge_j[g] < m:
+            keep[edge_ptr[g] + edge_j[g]] = keep[edge_ptr[g] + m + edge_j[g]] = 0
+    return keep
+
+
+def explain_order_host(score, occluded, offsets, m=None):
+    """twin of igmc_occlusion_order's permutation: (delta [T] fp32, order) where order is, per pair q, the positions of
+    its segment by |delta| descending, NaN after every number, ties by j - flat [T] (m None) or [P, m] padded with -1"""
+    score, occluded = np.asarray(score, np.float32), np.asarray(occluded, np.float32)
+    offsets = np.asarray(offsets, np.int64)
+    P = len(offsets) - 1
+    q = np.repeat(np.arange(P), np.diff(offsets))
+    delta = (occluded - score[q]).astype(np.float32)
+    order = []
+    for p in range(P):
+        seg = np.arange(offsets[p], offsets[p + 1])
+        a = np.abs(delta[seg])
+        o = np.lexsort((seg, np.where(np.isnan(a), np.inf, -a), np.isnan(a)))    # NaN last, |delta| desc, then j
+        order.append(seg[o])
+    if m is None:
+        return delta, (np.concatenate(order) if order else np.zeros(0, np.int64)).astype(np.int64)
+    top = np.full((P, m), -1, np.int64)
+    for p, o in enumerate(order):
+        top[p, :min(m, len(o))] = o[:m]
+    return delta, top
+
+
 # ---- the engine -----------------------------------------------------------------------------------------------------
 class InferenceEngine(object):
     """Pipelined, graph-replayed scoring of candidate pairs (module docstring).  ``checkpoints``: state_dict files of
@@ -257,10 +336,10 @@ class InferenceEngine(object):
     parameters as they are when a run starts.
 
         eng = InferenceEngine(model, graph, batch_size=256)
-        eng.start_recommend(users, k)          # or eng.start_pairs(users, items)
+        eng.start_recommend(users, k)          # or eng.start_pairs(users, items) / eng.start_explain(users, items, m)
         while eng.step():
             pass
-        top_items, top_scores = eng.finish()   # (predict: scores)
+        top_items, top_scores = eng.finish()   # (predict: scores; explain: an Explanation)
 
     An engine serves across updates of its ``RatingGraph`` (``graph.update``) between runs; an update during a run
     makes its next ``step`` raise RuntimeError.
@@ -387,31 +466,75 @@ class InferenceEngine(object):
 
     def start_pairs(self, users, items):
         """plan a run over the explicit pairs (users[i], items[i]).  Returns their number."""
+        return self._start_explicit("pairs", users, items)
+
+    def start_explain(self, users, items, m=None):
+        """plan an explanation run over the explicit pairs (users[i], items[i]) (``explain_pairs``): the base pass
+        scores them and counts their subgraphs' ratings; once it is done, ``step`` reads the total (the run's one host
+        sync) and goes on with the occlusion pass.  ``m``: keep each pair's first m ratings.  Returns the number of
+        pairs."""
+        m = _check_top(m, "m")
+        return self._start_explicit("explain", users, items, m=m, phase="base")
+
+    def _start_explicit(self, kind, users, items, **extra):
         g = self.graph
         users = _host_ids(users, "users", g.num_users)
         items = _host_ids(items, "items", g.num_items)
         if len(users) != len(items):
             raise ValueError("users and items must have the same length (%d vs %d)" % (len(users), len(items)))
-        P = len(users)
-        run = dict(kind="pairs", P=P, version=g.version,
-                   scores=torch.empty(P, dtype=torch.float32, device=self.dev))
+        P, dev = len(users), self.dev
+        run = dict(kind=kind, P=P, version=g.version, scores=torch.empty(P, dtype=torch.float32, device=dev), **extra)
         self.run = run
+        if kind == "explain":
+            run["num_edges"] = torch.zeros(P, dtype=torch.int32, device=dev)
+            run["offsets"] = torch.zeros(P + 1, dtype=torch.int64, device=dev)
+            for s in self.slots:
+                if "j" not in s:
+                    s["j"] = torch.zeros(self.B, dtype=torch.int32, device=dev)
         if P == 0:
             return 0
-        run["pu"] = torch.from_numpy(users.astype(np.int32)).to(self.dev)
-        run["pv"] = torch.from_numpy(items.astype(np.int32)).to(self.dev)
+        run["pu"] = torch.from_numpy(users.astype(np.int32)).to(dev)
+        run["pv"] = torch.from_numpy(items.astype(np.int32)).to(dev)
         Cd = _lib.Candidates()
         Cd.pair_u, Cd.pair_v, Cd.num_pairs = run["pu"].data_ptr(), run["pv"].data_ptr(), P
         run["Cd"] = Cd
         self._prime()
         return P
 
-    def _prime(self):
+    def _start_occlusion(self):
+        """after the base pass of an explanation run: the offsets of the pairs' ratings, their total T (the run's one
+        host sync), the output buffers [T] and the occlusion pass primed.  Returns True when it has positions."""
+        run, dev = self.run, self.dev
+        _lib.check(self.lib.igmc_explain_offsets(run["num_edges"].data_ptr(), run["P"], run["offsets"].data_ptr(),
+                                                 _stream_ptr()), "igmc_explain_offsets")
+        T = run["T"] = int(run["offsets"][run["P"]].item())
+        run["phase"] = "occlude"
+        run["occ"] = torch.empty(T, dtype=torch.float32, device=dev)
+        for k in ("user", "item", "rating"):
+            run[k] = torch.empty(T, dtype=torch.int32, device=dev)
+        if T == 0:
+            run["steps"] = run["done"] = 0
+            return False
+        if T >= (1 << 31) - 1:
+            raise NotImplementedError("an explanation run covers fewer than 2^31 - 1 ratings, not %d" % T)
+        ecap = self.extractor._out_caps(self.B)[1]
+        for s in self.slots:
+            if s.get("keep") is None or s["keep"].numel() < ecap:
+                s["keep"] = torch.ones(ecap, dtype=torch.uint8, device=dev)
+            # a training-mode forward with both dropout rates 0: the eval forward of the kept edges
+            d = self.model.make_dropout(False)[0]
+            d.edge_keep = s["keep"].data_ptr()
+            s["drop"] = (d, [s["keep"]])
+        self._prime(T)
+        return True
+
+    def _prime(self, total=None):
         """candidate pairs + extraction of the first batch, the model's plan for it (its one host sync, if any) and
-        the prepared weights of every parameter set; captured graphs of an earlier run are dropped (they hold its
-        buffers, its candidate total and the graph's shape as it was; the extractor follows an updated graph)"""
+        the prepared weights of every parameter set; captured graphs of an earlier run or pass are dropped (they hold
+        its buffers, its candidate total and the graph's shape as it was; the extractor follows an updated graph).
+        ``total``: the positions of the pass (default: the run's pairs)."""
         run = self.run
-        run["steps"] = (run["P"] + self.B - 1) // self.B
+        run["steps"] = ((run["P"] if total is None else total) + self.B - 1) // self.B
         run["done"] = 0
         self.graphs, self.eager_done = {}, set()
         self.cursor.zero_()
@@ -424,13 +547,29 @@ class InferenceEngine(object):
 
     def _next(self, slot):
         """candidate pairs of the next B positions (device cursor) + their extraction into batch slot ``slot``"""
-        s, run = self.slots[slot], self.run
-        _lib.check(self.lib.igmc_candidate_pairs(C.byref(self.graph._c), C.byref(run["Cd"]), self.cursor.data_ptr(),
-                                                 self.B, s["u"].data_ptr(), s["v"].data_ptr(), s["pid"].data_ptr(),
-                                                 s["tag"].data_ptr(), self.extractor.err.data_ptr(), _stream_ptr()),
-                   "igmc_candidate_pairs")
-        self.batches[slot] = self.extractor.extract(pairs=(s["u"], s["v"], None), pair_ids=s["pid"], reuse=True,
-                                                    slot=slot)
+        s, run, err = self.slots[slot], self.run, self.extractor.err.data_ptr()
+        occlude = run.get("phase") == "occlude"
+        if occlude:
+            _lib.check(self.lib.igmc_occlusion_pairs(C.byref(self.graph._c), run["pu"].data_ptr(),
+                                                     run["pv"].data_ptr(), run["offsets"].data_ptr(), run["P"],
+                                                     self.cursor.data_ptr(), self.B, s["u"].data_ptr(),
+                                                     s["v"].data_ptr(), s["pid"].data_ptr(), s["tag"].data_ptr(),
+                                                     s["j"].data_ptr(), err, _stream_ptr()), "igmc_occlusion_pairs")
+        else:
+            _lib.check(self.lib.igmc_candidate_pairs(C.byref(self.graph._c), C.byref(run["Cd"]),
+                                                     self.cursor.data_ptr(), self.B, s["u"].data_ptr(),
+                                                     s["v"].data_ptr(), s["pid"].data_ptr(), s["tag"].data_ptr(), err,
+                                                     _stream_ptr()), "igmc_candidate_pairs")
+        b = self.batches[slot] = self.extractor.extract(pairs=(s["u"], s["v"], None), pair_ids=s["pid"], reuse=True,
+                                                        slot=slot)
+        if occlude:
+            _lib.check(self.lib.igmc_occlusion_mask(C.byref(b._lazy["_c"]), self.B, s["tag"].data_ptr(),
+                                                    s["j"].data_ptr(), s["keep"].data_ptr(), run["user"].data_ptr(),
+                                                    run["item"].data_ptr(), run["rating"].data_ptr(), err,
+                                                    _stream_ptr()), "igmc_occlusion_mask")
+        elif run["kind"] == "explain":
+            _lib.check(self.lib.igmc_explain_count(b._priv["edge_ptr"].data_ptr(), s["tag"].data_ptr(), self.B,
+                                                   run["num_edges"].data_ptr(), _stream_ptr()), "igmc_explain_count")
 
     @contextlib.contextmanager
     def _params(self, j):
@@ -445,12 +584,16 @@ class InferenceEngine(object):
             m.flat_params, m._wprep, m._prepped = own
 
     def _score(self, slot):
-        """eval forward of batch ``slot`` with every parameter set, then the merge / scatter of the mean"""
+        """eval forward of batch ``slot`` with every parameter set, then the merge / scatter of the mean.  An occlusion
+        batch runs the training-mode forward with its slot's edge mask and no dropout: the eval forward of each
+        subgraph without its masked rating."""
         m, b, s, run = self.model, self.batches[slot], self.slots[slot], self.run
+        occlude = run.get("phase") == "occlude"
+        training, drop = (True, s["drop"]) if occlude else (False, self.drop)
         preds = None
         for j in range(self.K):
             with self._params(j):
-                pred, _ = m._launch_forward(b, False, self.drop)
+                pred, _ = m._launch_forward(b, training, drop)
             if self.K == 1:
                 preds = pred
             else:
@@ -461,8 +604,9 @@ class InferenceEngine(object):
                                                 s["v"].data_ptr(), run["k"], run["top_s"].data_ptr(),
                                                 run["top_i"].data_ptr(), _stream_ptr()), "igmc_topk_merge")
         else:
+            out = run["occ"] if occlude else run["scores"]
             _lib.check(self.lib.igmc_score_scatter(preds.data_ptr(), self.K, self.B, s["tag"].data_ptr(),
-                                                   run["scores"].data_ptr(), _stream_ptr()), "igmc_score_scatter")
+                                                   out.data_ptr(), _stream_ptr()), "igmc_score_scatter")
 
     def _launch(self, slot):
         main = torch.cuda.current_stream()
@@ -486,14 +630,18 @@ class InferenceEngine(object):
         slot = run["done"] & 1
         replay_step(self.graphs, self.eager_done, slot, lambda: self._launch(slot), self.use_graph)
         run["done"] += 1
-        return run["done"] < run["steps"]
+        if run["done"] < run["steps"]:
+            return True
+        return run["kind"] == "explain" and run["phase"] == "base" and self._start_occlusion()
 
     def finish(self):
         """wait for the run, check the error word (one host sync) and return (top_items [U, k] int64, top_scores
-        [U, k] fp32) or the scores [P] fp32, on the device"""
+        [U, k] fp32), the scores [P] fp32 or the ``Explanation``, on the device"""
         run = self.run
         while self.step():
             pass
+        if run["kind"] == "explain" and run["phase"] == "base":    # no pairs: the run has no occlusion pass
+            self._start_occlusion()
         code = int(self.extractor.err.item())
         if code:
             self.extractor.err.zero_()
@@ -501,7 +649,30 @@ class InferenceEngine(object):
         self.run = None
         if run["kind"] == "recommend":
             return run["top_i"], run["top_s"]
+        if run["kind"] == "explain":
+            return self._order(run)
         return run["scores"]
+
+    def _order(self, run):
+        """igmc_occlusion_order: every pair's ratings by |delta| descending (NaN last, ties by position), all of them
+        or the first m"""
+        P, T, m, dev = run["P"], run["T"], run["m"], self.dev
+        shape = (P, m) if m else (T,)
+        out = dict(user=torch.empty(shape, dtype=torch.int32, device=dev),
+                   item=torch.empty(shape, dtype=torch.int32, device=dev),
+                   rating=torch.empty(shape, dtype=torch.int32, device=dev),
+                   delta=torch.empty(shape, dtype=torch.float32, device=dev))
+        nbytes = C.c_int64(0)
+        _lib.check(self.lib.igmc_occlusion_order_ws_bytes(P, T, C.byref(nbytes)), "igmc_occlusion_order_ws_bytes")
+        ws = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=dev)
+        _lib.check(self.lib.igmc_occlusion_order(run["scores"].data_ptr(), run["occ"].data_ptr(),
+                                                 run["offsets"].data_ptr(), P, T, run["user"].data_ptr(),
+                                                 run["item"].data_ptr(), run["rating"].data_ptr(), m or 0,
+                                                 ws.data_ptr(), ws.numel(), out["user"].data_ptr(),
+                                                 out["item"].data_ptr(), out["rating"].data_ptr(),
+                                                 out["delta"].data_ptr(), _stream_ptr()), "igmc_occlusion_order")
+        return Explanation(run["scores"], run["num_edges"], run["offsets"], out["user"], out["item"], out["rating"],
+                           out["delta"])
 
     def recommend(self, users, k, items=None, exclude_rated=True, retrieve=None):
         self.start_recommend(users, k, items, exclude_rated, retrieve)
@@ -509,6 +680,10 @@ class InferenceEngine(object):
 
     def predict_pairs(self, users, items):
         self.start_pairs(users, items)
+        return self.finish()
+
+    def explain_pairs(self, users, items, m=None):
+        self.start_explain(users, items, m)
         return self.finish()
 
     def close(self):
@@ -531,6 +706,36 @@ def predict_pairs(model, graph, users, items, *, h=1, sample_ratio=1.0, max_node
     eng = InferenceEngine(model, graph, h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
     try:
         return eng.predict_pairs(users, items)
+    finally:
+        eng.close()
+
+
+def explain_pairs(model, graph, users, items, m=None, *, h=1, sample_ratio=1.0, max_nodes_per_hop=None, batch_size=256,
+                  checkpoints=None, sample_seed=0):
+    """why each pair (users[i], items[i]) got its score: for every rating in the pair's enclosing subgraph (a rated
+    pair's own rating excluded, as in ``predict_pairs``), delta = the score of that subgraph without the rating (both
+    directed edges removed; same nodes, no re-sampling) - the pair's score.  Returns an ``Explanation`` of device
+    tensors: score [P] (bit for bit ``predict_pairs``), num_edges [P], offsets [P+1] and per rating user / item /
+    rating (its label) / delta, ordered within a pair by |delta| descending, NaN after every number, ties by the
+    rating's position in the subgraph's edge_index; flat with pair p at [offsets[p], offsets[p+1]) when ``m`` is None,
+    else the first ``m`` per pair [P, m], padded with user / item / rating -1 and delta 0.  ``checkpoints``: every score
+    is the fp32 checkpoint mean, as in ``predict_pairs``."""
+    nu, ni = graph.shape
+    m = _check_top(m, "m")
+    users, items = _host_ids(users, "users", nu), _host_ids(items, "items", ni)
+    if len(users) != len(items):
+        raise ValueError("users and items must have the same length (%d vs %d)" % (len(users), len(items)))
+    if len(users) == 0:
+        dev = model.flat_params.device
+        shape = (0, m) if m else (0,)
+        i32 = dict(dtype=torch.int32, device=dev)
+        return Explanation(torch.zeros(0, dtype=torch.float32, device=dev), torch.zeros(0, **i32),
+                           torch.zeros(1, dtype=torch.int64, device=dev), torch.zeros(shape, **i32),
+                           torch.zeros(shape, **i32), torch.zeros(shape, **i32),
+                           torch.zeros(shape, dtype=torch.float32, device=dev))
+    eng = InferenceEngine(model, graph, h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
+    try:
+        return eng.explain_pairs(users, items, m)
     finally:
         eng.close()
 

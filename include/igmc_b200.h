@@ -466,6 +466,50 @@ int igmc_topk_merge(const float* preds, int K, int B, const int64_t* tag, const 
 /* Explicit pairs: scores[tag[i]] = the same fp32 checkpoint mean for every i with tag[i] >= 0. */
 int igmc_score_scatter(const float* preds, int K, int B, const int64_t* tag, float* scores, void* stream);
 
+/* ---- explanation by occlusion (csrc/explain.cu) ----
+ * Why a pair got its score: for every rating of the pair's enclosing subgraph, the score of that subgraph without the
+ * rating (both directed edges dropped, nodes unchanged, no re-sampling).  The reference only draws subgraphs for a look
+ * (visualize, train_eval.py:248-322); a user of it would rebuild the subgraph per rating and call the model in a Python
+ * loop.  Here a base pass of explicit pairs (igmc_candidate_pairs, igmc_score_scatter) counts each subgraph's ratings,
+ * and an occlusion pass scores position c = (pair q, rating j) for every c < T = offsets[P]: igmc_extract_batch
+ * extracts pair q again (same pair id: the same subgraph), igmc_occlusion_mask drops rating j through the model
+ * kernels' edge_keep (training-mode forward, adj_dropout = hidden_dropout = 0: dropout_adj with that draw,
+ * train_eval.py:160 / models.py:193-198) and igmc_score_scatter stores the score at c. */
+
+/* After the extraction of a base batch: num_edges[tag[i]] = (edge_ptr[i+1] - edge_ptr[i]) / 2, the undirected edges of
+ * graph i, for every i with tag[i] >= 0. */
+int igmc_explain_count(const int32_t* edge_ptr, const int64_t* tag, int B, int32_t* num_edges, void* stream);
+
+/* offsets [num_pairs+1]: the exclusive int64 prefix of num_edges; offsets[num_pairs] = T.  One CTA. */
+int igmc_explain_offsets(const int32_t* num_edges, int num_pairs, int64_t* offsets, void* stream);
+
+/* The pairs of occlusion positions [*cursor, *cursor + B), then *cursor += B (the igmc_candidate_pairs of an occlusion
+ * pass): position c belongs to pair q, the last q with offsets[q] <= c, and names its rating j = c - offsets[q].
+ * Writes links_u / links_v / pair_id = u * num_items + v (as predict_pairs samples the pair) / tag = c / edge_j = j.
+ * Positions past T repeat the last position with tag -1.  Pair ids outside G set IGMC_ERR_CANDIDATES. */
+int igmc_occlusion_pairs(const igmc_csr_t* G, const int32_t* pair_u, const int32_t* pair_v, const int64_t* offsets,
+                         int num_pairs, int64_t* cursor, int B, int32_t* links_u, int32_t* links_v, int64_t* pair_id,
+                         int64_t* tag, int32_t* edge_j, int* err, void* stream);
+
+/* For the batch O of B graphs extracted from igmc_occlusion_pairs' output: edge_keep [O->edge_ptr[B]] is 1 except, in
+ * every graph with tag >= 0, the two directed copies of its rating j (edge_ptr[g] + j and edge_ptr[g] + E_g/2 + j in
+ * the [u|v ; v|u] edge_index); and user / item / rating [T] at position tag = the rating's global user, global item
+ * and label.  One CTA per graph.  j outside the graph's ratings (a subgraph unlike the base pass's) sets
+ * IGMC_ERR_CANDIDATES and drops nothing. */
+int igmc_occlusion_mask(const igmc_batch_out_t* O, int B, const int64_t* tag, const int32_t* edge_j,
+                        uint8_t* edge_keep, int32_t* user, int32_t* item, int32_t* rating, int* err, void* stream);
+
+/* delta[c] = occluded[c] - score[q] (fp32) for every position, then each pair's segment [offsets[q], offsets[q+1])
+ * ordered by |delta| descending, NaN after every number, ties by j (a segmented radix sort on the 64-bit key
+ * (~orderable(|delta|) << 32) | j).  m = 0: out_* [T] in that order; 1 <= m <= IGMC_TOPK_MAX: out_* [num_pairs, m],
+ * the first m entries of each segment, padded with user / item / rating -1 and delta 0.  `ws`: at least
+ * igmc_occlusion_order_ws_bytes bytes.  num_pairs, num_positions < 2^31 - 1. */
+int igmc_occlusion_order_ws_bytes(int num_pairs, int64_t num_positions, int64_t* bytes);
+int igmc_occlusion_order(const float* score, const float* occluded, const int64_t* offsets, int num_pairs,
+                         int64_t num_positions, const int32_t* user, const int32_t* item, const int32_t* rating,
+                         int m, void* ws, int64_t ws_bytes, int32_t* out_user, int32_t* out_item, int32_t* out_rating,
+                         float* out_delta, void* stream);
+
 /* ---- candidate retrieval by bridge count (csrc/retrieve.cu) ----
  * For h = 1 the enclosing subgraph of an unrated pair (u, v) joins u's star and v's star only through the bridge edges
  * (u', i): u' != u rated v and i, u rated i.  Their number is

@@ -1,0 +1,405 @@
+"""Explaining predicted ratings on the GPU (igmc_b200/recommend.py explain_pairs, csrc/explain.cu).
+
+* the base score is predict_pairs bit for bit; the ratings listed per pair are the undirected edges of the pair's
+  extracted subgraph (a rated pair's own rating excluded);
+* every occluded score equals the eval forward of a foreign batch built from the subgraph with that rating filtered out
+  of edge_index / edge_type, bit for bit, on plans 2, 1, 4, 0 and L2, h = 2, rgcn="pyg-2" and DGCNN_RS, with a rated
+  and a cold-start (no ratings) pair; and the fp64 restated forward within 1e-4 RMSE;
+* a masked forward that drops nothing is the eval forward bit for bit;
+* the order is the documented one, top-m is a prefix of it, and results do not depend on B or graph replay;
+* checkpoints, graph updates, and steady-state steps without a host synchronisation."""
+import functools
+import os
+import tempfile
+
+import numpy as np
+import pytest
+import scipy.sparse as ssp
+import torch
+
+from igmc_b200 import _lib
+from igmc_b200 import recommend as rc
+from igmc_b200.data import build_adj, make_synthetic_dataset, synth_ratings
+from igmc_b200.util_functions import Batch, RatingGraph, SubgraphExtractor
+from oracle import extract_np, pyg_restated
+from tests import pyg2_oracle
+from tests.test_gpu_graph_update import _apply_scipy
+
+pytestmark = pytest.mark.gpu
+
+
+@functools.lru_cache(maxsize=None)
+def _ds(name):
+    return make_synthetic_dataset(name, seed=0)
+
+
+@functools.lru_cache(maxsize=None)
+def _r13():
+    nu, ni = 400, 300
+    u, v, lab = synth_ratings(nu, ni, 9000, 13, seed=4)
+    return build_adj(u, v, lab, nu, ni)
+
+
+def _with_cold_start(A):
+    """A with one more user and one more item, neither rated: the pair (new user, new item) has no ratings at all"""
+    return ssp.csr_matrix(ssp.bmat([[A, None], [None, ssp.csr_matrix((1, 1), dtype=A.dtype)]]), dtype=A.dtype)
+
+
+def _model(R, h=1, rgcn="pyg-1.4", dgcnn=False, seed=0):
+    from igmc_b200.models import DGCNN_RS, IGMC
+    torch.manual_seed(seed)
+    if dgcnn:
+        m = DGCNN_RS(2 * h + 2, latent_dim=[32, 32, 32, 1], k=30, num_relations=R, num_bases=4, regression=True,
+                     rgcn=rgcn)
+    else:
+        m = IGMC(2 * h + 2, latent_dim=[32] * 4, num_relations=R, num_bases=4, regression=True, rgcn=rgcn)
+    if rgcn == "pyg-2":
+        with torch.no_grad():
+            for c in m.convs:
+                c.bias.uniform_(-0.3, 0.3)
+    return m.cuda()
+
+
+def _pairs(A, small=False):
+    """a rated pair, an unrated pair and the cold-start pair of _with_cold_start(A) (its last user and item); with
+    ``small`` the rated and unrated pairs are taken among low-degree users and items"""
+    nu, ni = A.shape[0] - 1, A.shape[1] - 1
+    du, di = np.diff(A.indptr)[:nu], np.diff(A.tocsc().indptr)[:ni]
+    coo = A.tocoo()
+    score = du[coo.row] + di[coo.col] if small else -(du[coo.row] + di[coo.col])
+    k = int(np.argsort(score, kind="stable")[len(score) // 3 if not small else 0])
+    ru, rv = int(coo.row[k]), int(coo.col[k])
+    users = np.argsort(np.where(du > 0, du, du.max() + 1), kind="stable")      # users with ratings, fewest first
+    uu = int(users[1 if small else nu // 2])
+    rated = set(A.indices[A.indptr[uu]:A.indptr[uu + 1]].tolist())
+    order = np.argsort(np.where(di > 0, di, di.max() + 1), kind="stable")
+    uv = int(next(x for x in (order if small else order[::-1][ni - int((di > 0).sum()):]) if int(x) not in rated))
+    return np.array([ru, uu, nu]), np.array([rv, uv, ni])
+
+
+def _run(eng, u, v, m=None):
+    """(Explanation, occluded scores [T] in position order) of one engine run"""
+    eng.start_explain(u, v, m)
+    while eng.step():
+        pass
+    occ = eng.run["occ"]
+    return eng.finish(), occ
+
+
+def _subgraph(A, R, u, v, h, mnph, seed):
+    """the pair's extracted subgraph (one graph): x, edge_index [2, E], edge_type [E], node_gid, on the device, and
+    the extractor's per-subgraph node capacity n_cap"""
+    ni = A.shape[1]
+    ex = SubgraphExtractor(RatingGraph(A), [0], [0], [0], np.arange(1, R + 1, dtype=np.float32), h, 1.0, mnph,
+                           max_batch=1, seed=seed)
+    b = ex.extract(pairs=(np.array([u]), np.array([v]), np.zeros(1, np.int64)), pair_ids=np.array([u * ni + v]))
+    return (b.x.clone(), b.edge_index.clone(), b.edge_type.clone(), b.node_gid.clone()), b._priv["n_cap"]
+
+
+def _masked_forward(model, sub, plan, n_cap, B=256):
+    """eval scores [m] of the subgraph without rating j for every j: foreign batches of copies with the two directed
+    edges of rating j filtered out of edge_index / edge_type, on the engine's kernel plan and with the extractor's node
+    capacity (the shared-memory layout, and with it whether a plan stages its lists, follows n_cap)"""
+    x, ei, et, _ = sub
+    n, E = x.shape[0], ei.shape[1]
+    mm = E // 2
+    out = []
+    own = model.kernel_plan
+    model.kernel_plan = plan
+    model.eval()
+    try:
+        with torch.no_grad():
+            for j0 in range(0, mm, B):
+                js = torch.arange(j0, min(j0 + B, mm), device="cuda")
+                G = len(js)
+                e = torch.arange(E, device="cuda")
+                keep = (e[None, :] != js[:, None]) & (e[None, :] != js[:, None] + mm)          # [G, E]
+                g_of, e_of = keep.nonzero(as_tuple=True)
+                b = Batch.from_arrays(x.repeat(G, 1), ei[:, e_of] + g_of * n, et[e_of],
+                                      torch.arange(G, device="cuda").repeat_interleave(n), torch.zeros(G),
+                                      num_graphs=G)
+                b._priv["n_cap"] = n_cap
+                out.append(model(b).clone())
+    finally:
+        model.kernel_plan = own
+    return torch.cat(out) if out else torch.zeros(0, device="cuda")
+
+
+def _expected_order(q0, q1, delta_of_pos):
+    """the positions of one pair's ratings by |delta| descending, NaN last, ties by position"""
+    seg = np.arange(q0, q1)
+    a = np.abs(delta_of_pos[seg])
+    return seg[np.lexsort((seg, np.where(np.isnan(a), np.inf, -a), np.isnan(a)))]
+
+
+# ---- 1. base score, edge set, occluded scores == masked foreign forward -------------------------------------------------
+CASES = {
+    # name: (dataset, h, mnph, model kwargs, forced kernel plan, expected plan, small pairs)
+    "plan 2 ml_1m": ("ml_1m", 1, 100, {}, "auto", 2, False),
+    "plan 1 ml_1m": ("ml_1m", 1, 100, {}, 1, 1, False),
+    "plan 4 ml_100k": ("ml_100k", 1, 200, {}, "auto", 4, False),
+    "plan 0 R=13": ("r13", 1, 50, {}, "auto", 0, False),
+    "L2 plan ml_100k uncapped": ("ml_100k", 1, None, {}, "auto", "l2", True),
+    "h=2": ("ml_1m", 2, 20, {}, "auto", None, False),
+    "pyg-2": ("ml_1m", 1, 100, dict(rgcn="pyg-2"), "auto", 2, False),
+    "DGCNN_RS": ("ml_1m", 1, 100, dict(dgcnn=True), "auto", None, False),
+}
+
+INEXACT = {"plan 1 ml_1m"}      # the cases held to a bound instead of bit equality (see below)
+
+
+@pytest.mark.parametrize("name", list(CASES))
+def test_occluded_scores_equal_the_masked_forward(name):
+    dsn, h, mnph, kw, force, plan, small = CASES[name]
+    A0 = _r13() if dsn == "r13" else _ds(dsn)["adj_train"]
+    R = 13 if dsn == "r13" else 5
+    A = _with_cold_start(A0)
+    m = _model(R, h, **kw)
+    m.kernel_plan = force
+    u, v = _pairs(A, small)
+    B, seed = 64, 7
+    eng = rc.InferenceEngine(m, A, h=h, max_nodes_per_hop=mnph, batch_size=B, sample_seed=seed)
+    ex, occ = _run(eng, u, v)
+    eng.close()
+    cl = next(iter(m._plans.values()))
+    if plan == "l2":
+        assert _lib.l2_csize(cl) > 0
+    elif plan is not None:
+        assert cl == plan, (name, cl)
+    base = rc.predict_pairs(m, A, u, v, h=h, max_nodes_per_hop=mnph, batch_size=B, sample_seed=seed)
+    assert torch.equal(ex.score, base), name
+    off = ex.offsets.cpu().numpy()
+    ne = ex.num_edges.cpu().numpy()
+    assert np.array_equal(np.diff(off), ne) and ne[2] == 0 and ne[0] > 0 and ne[1] > 0
+    score, occ = ex.score.cpu().numpy(), occ.cpu().numpy()
+    delta_of_pos = np.concatenate([occ[off[q]:off[q + 1]] - score[q] for q in range(3)]).astype(np.float32)
+    users, items, ratings, deltas = (t.cpu().numpy() for t in (ex.user, ex.item, ex.rating, ex.delta))
+    for q in range(3):
+        sub, n_cap = _subgraph(A, R, int(u[q]), int(v[q]), h, mnph, seed)
+        x, ei, et, gid = sub
+        mm = ei.shape[1] // 2
+        assert mm == ne[q]
+        ei_h, gid_h = ei.cpu().numpy(), gid.cpu().numpy()
+        su, sv, sr = gid_h[ei_h[0, :mm]], gid_h[ei_h[1, :mm]], et[:mm].cpu().numpy()
+        assert not ((su == u[q]) & (sv == v[q])).any()                 # a rated pair's own rating is not listed
+        seg = slice(off[q], off[q + 1])
+        o = _expected_order(off[q], off[q + 1], delta_of_pos) - off[q]       # j of every listed entry
+        assert np.array_equal(users[seg], su[o]) and np.array_equal(items[seg], sv[o]), (name, q)
+        assert np.array_equal(ratings[seg], sr[o]), (name, q)
+        assert np.array_equal(deltas[seg], delta_of_pos[off[q]:off[q + 1]][o], equal_nan=True), (name, q)
+        if mm == 0:
+            continue
+        want = _masked_forward(m, sub, cl, n_cap).cpu().numpy()
+        got = occ[off[q]:off[q + 1]]
+        if name in INEXACT:
+            # plan 1 on these subgraphs: a few occluded scores differ from the filtered batch's in their last bits
+            # (at most 2^-27 measured on an H100); the masked and the filtered lists do not group their sums alike
+            # there.  Bound: 8 ulps of the pair's largest occluded score.
+            bound = 8 * float(np.spacing(np.abs(want).max().astype(np.float32)))
+            assert float(np.abs(got - want).max()) <= bound, (name, q, float(np.abs(got - want).max()), bound)
+        else:
+            bad = int((got != want).sum())
+            assert bad == 0, (name, q, bad, float(np.abs(got - want).max()))
+
+
+def test_all_ones_mask_is_the_eval_forward():
+    for dsn, kw, force in (("ml_1m", {}, "auto"), ("ml_1m", dict(dgcnn=True), "auto"), ("ml_1m", {}, 0),
+                           ("ml_1m", dict(rgcn="pyg-2"), 4)):
+        A = _ds(dsn)["adj_train"]
+        m = _model(5, **kw)
+        m.kernel_plan = force
+        ex = SubgraphExtractor(RatingGraph(A), [0], [0], [0], np.arange(1, 6, dtype=np.float32), 1, 1.0, 100,
+                               max_batch=50, seed=3)
+        u, v = np.arange(50) * 7, np.arange(50) * 11
+        b = ex.extract(pairs=(u, v, np.zeros(50, np.int64)), pair_ids=u * A.shape[1] + v)
+        m.eval()
+        with torch.no_grad():
+            want = m._launch_forward(b, False, m.make_dropout(False))[0].clone()
+            d = m.make_dropout(False, edge_keep=torch.ones(b._priv["edge_cap"], dtype=torch.uint8))
+            got = m._launch_forward(b, True, d)[0].clone()
+        b.check()
+        assert torch.equal(got, want), (kw, force)
+
+
+# ---- 2. against the fp64 restated forward --------------------------------------------------------------------------------
+@pytest.mark.parametrize("rgcn", ["pyg-1.4", "pyg-2"])
+def test_occluded_scores_against_oracle(rgcn):
+    A0 = _ds("ml_1m")["adj_train"]
+    A = _with_cold_start(A0)
+    R, mnph, seed = 5, 100, 7
+    m = _model(R, rgcn=rgcn)
+    ref = pyg2_oracle.igmc_ref(rgcn, 4, (32,) * 4, R, 4, 0.0)
+    ref.load_state_dict({k: v.double().cpu() for k, v in m.state_dict().items()})
+    ref = pyg_restated.set_formulation(ref.double(), "transform").cuda().eval()
+    u, v = _pairs(A)
+    ex = rc.explain_pairs(m, A, u[:2], v[:2], max_nodes_per_hop=mnph, batch_size=128, sample_seed=seed)
+    ni = A.shape[1]
+    errs = []
+    for q in range(2):
+        ob = extract_np.extract_batch(extract_np.RatingCSR(A), u[q:q + 1], v[q:q + 1], np.zeros(1, np.int64),
+                                      np.arange(1, R + 1, dtype=np.float32), 1, 1.0, mnph, seed=seed,
+                                      pair_ids=u[q:q + 1] * ni + v[q:q + 1])
+        sub = ob["subs"][0]
+        tb = pyg_restated.to_torch_batch(ob, torch.float64, device="cuda")
+        ei, et = tb["edge_index"], tb["edge_type"]
+        E = ei.shape[1]
+        mm = E // 2
+        src, dst = ei[0, :mm].cpu().numpy(), ei[1, :mm].cpu().numpy()
+        nu_ = len(sub["u_nodes"])
+        key = {(int(sub["u_nodes"][a]), int(sub["v_nodes"][b - nu_])): j for j, (a, b) in enumerate(zip(src, dst))}
+        o0, o1 = int(ex.offsets[q]), int(ex.offsets[q + 1])
+        assert o1 - o0 == mm
+        js = np.array([key[(int(a), int(b))] for a, b in zip(ex.user[o0:o1].tolist(), ex.item[o0:o1].tolist())])
+        got = (ex.score[q] + ex.delta[o0:o1]).double().cpu().numpy()
+        want = np.zeros(mm)
+        n = tb["x"].shape[0]
+        with torch.no_grad():
+            for j0 in range(0, mm, 128):
+                jj = torch.as_tensor(js[j0:j0 + 128], device="cuda")
+                G = len(jj)
+                e = torch.arange(E, device="cuda")
+                keep = (e[None, :] != jj[:, None]) & (e[None, :] != jj[:, None] + mm)
+                eig, etg = pyg_restated.dropout_adj(ei.repeat(1, G), et.repeat(G), 1.0, True, keep.reshape(-1))
+                eig = eig + torch.repeat_interleave(torch.arange(G, device="cuda") * n, keep.sum(1))[None, :]
+                xg = tb["x"].repeat(G, 1)
+                want[j0:j0 + G] = ref(xg, eig, etg).cpu().numpy()
+        errs.append(got - want)
+    rmse = float(np.sqrt(np.mean(np.concatenate(errs) ** 2)))
+    print("%s: occluded scores vs fp64 oracle RMSE %.2e" % (rgcn, rmse))
+    assert rmse <= 1e-4, rmse
+
+
+# ---- 3. order, top-m, determinism ----------------------------------------------------------------------------------------
+def test_order_topm_and_determinism():
+    A = _with_cold_start(_ds("ml_1m")["adj_train"])
+    m = _model(5)
+    m.kernel_plan = 2                  # the same plan at both batch sizes
+    u, v = _pairs(A)
+    results = {}
+    for B in (50, 512):
+        for use_graph in (True, False):
+            eng = rc.InferenceEngine(m, A, max_nodes_per_hop=100, batch_size=B, sample_seed=2, use_graph=use_graph)
+            results[(B, use_graph)] = _run(eng, u, v)[0]
+            tops = {k: eng.explain_pairs(u, v, k) for k in (1, 10, 256)} if (B, use_graph) == (50, True) else None
+            eng.close()
+            if tops:
+                ex = results[(B, use_graph)]
+                off = ex.offsets.cpu().numpy()
+                for k, t in tops.items():
+                    assert t.user.shape == (3, k) and t.offsets is not None
+                    assert torch.equal(t.score, ex.score)
+                    for q in range(3):
+                        n = min(k, off[q + 1] - off[q])
+                        for f in ("user", "item", "rating", "delta"):
+                            a, b = getattr(t, f)[q], getattr(ex, f)[off[q]:off[q] + n]
+                            assert torch.equal(a[:n], b), (k, q, f)
+                            assert (a[n:] == (0 if f == "delta" else -1)).all(), (k, q, f)
+    first = results[(50, True)]
+    d = first.delta.cpu().numpy()
+    off = first.offsets.cpu().numpy()
+    for q in range(3):
+        a = np.abs(d[off[q]:off[q + 1]])
+        assert (np.diff(a[~np.isnan(a)]) <= 0).all() and not np.isnan(a[:int((~np.isnan(a)).sum())]).any()
+    for key, r in results.items():
+        for f in r._fields:
+            assert torch.equal(getattr(r, f), getattr(first, f)), (key, f)
+
+
+def test_validation_and_empty_input():
+    A = _ds("ml_100k")["adj_train"]
+    m = _model(5)
+    with pytest.raises(IndexError):
+        rc.explain_pairs(m, A, [A.shape[0]], [0])
+    with pytest.raises(ValueError):
+        rc.explain_pairs(m, A, [0, 1], [0])
+    with pytest.raises(ValueError):
+        rc.explain_pairs(m, A, [0], [0], 0)
+    with pytest.raises(NotImplementedError):
+        rc.explain_pairs(m, A, [0], [0], _lib.TOPK_MAX + 1)
+    ex = rc.explain_pairs(m, A, [], [])
+    assert ex.score.shape == (0,) and ex.offsets.tolist() == [0] and ex.delta.shape == (0,)
+    ex = rc.explain_pairs(m, A, [], [], 5)
+    assert ex.user.shape == (0, 5)
+    eng = rc.InferenceEngine(m, A, max_nodes_per_hop=200, batch_size=50)
+    ex = eng.explain_pairs([], [], 3)
+    assert ex.user.shape == (0, 3) and ex.offsets.tolist() == [0]
+    eng.close()
+
+
+# ---- 4. checkpoints --------------------------------------------------------------------------------------------------------
+def test_two_checkpoints_are_the_fp32_mean():
+    A = _with_cold_start(_ds("ml_100k")["adj_train"])
+    m = _model(5)
+    u, v = _pairs(A, small=True)
+    with tempfile.TemporaryDirectory() as tmp:
+        paths = []
+        for c in range(2):
+            paths.append(os.path.join(tmp, "model_checkpoint%d.pth" % c))
+            torch.save(_model(5, seed=c + 1).state_dict(), paths[-1])
+        runs = []
+        for ck in (paths, paths[:1], paths[1:]):
+            eng = rc.InferenceEngine(m, A, max_nodes_per_hop=200, batch_size=50, checkpoints=ck)
+            runs.append(_run(eng, u, v))
+            eng.close()
+    (ens, occ), (e0, o0), (e1, o1) = runs
+    assert torch.equal(ens.score, (e0.score + e1.score) / 2)
+    assert torch.equal(occ, (o0 + o1) / 2)
+    assert torch.equal(ens.num_edges, e0.num_edges)
+    assert ens.delta.numel() > 0 and not torch.equal(ens.delta, e0.delta)
+
+
+# ---- 5. graph updates --------------------------------------------------------------------------------------------------------
+def test_engine_explains_across_updates():
+    A = _ds("ml_1m")["adj_train"]
+    m = _model(5)
+    g = RatingGraph(A, reserve_nnz=2000)
+    eng = rc.InferenceEngine(m, g, max_nodes_per_hop=100, batch_size=64, sample_seed=4)
+    rng = np.random.default_rng(5)
+    u, v = _pairs(_with_cold_start(A))
+    u, v = u[:2], v[:2]
+    try:
+        eng.explain_pairs(u, v, 10)
+        coo = A.tocoo()
+        k = rng.choice(A.nnz, 300, replace=False)
+        du = np.concatenate([coo.row[k[:150]], rng.integers(0, A.shape[0], 150)])
+        dv = np.concatenate([coo.col[k[:150]], rng.integers(0, A.shape[1], 150)])
+        dx = np.concatenate([np.zeros(75, np.int64), rng.integers(1, 6, 225)])
+        g.update(du, dv, dx)
+        A2 = _apply_scipy(A, du, dv, dx, g.shape)
+        got = eng.explain_pairs(u, v)
+        fresh = rc.InferenceEngine(m, RatingGraph(A2), max_nodes_per_hop=100, batch_size=64, sample_seed=4)
+        want = fresh.explain_pairs(u, v)
+        fresh.close()
+    finally:
+        eng.close()
+    for f in got._fields:
+        assert torch.equal(getattr(got, f), getattr(want, f)), f
+
+
+# ---- 6. steady state ----------------------------------------------------------------------------------------------------------
+def test_steady_state_steps_do_not_sync():
+    A = _ds("ml_1m")["adj_train"]
+    m = _model(5)
+    eng = rc.InferenceEngine(m, A, max_nodes_per_hop=100, batch_size=50, sample_seed=1)
+    u, v = np.array([11, 12]), np.array([40, 41])
+    outs = []
+    try:
+        for rep in range(2):
+            eng.start_explain(u, v)
+            while eng.run["phase"] == "base":
+                assert eng.step()
+            for _ in range(4):              # eager warm-up and capture of both slots of the occlusion pass
+                assert eng.step()
+            assert len(eng.graphs) == 2
+            torch.cuda.set_sync_debug_mode("error")
+            try:
+                while eng.step():
+                    pass
+            finally:
+                torch.cuda.set_sync_debug_mode("default")
+            outs.append(eng.finish())
+            assert int(eng.extractor.err.item()) == 0
+    finally:
+        eng.close()
+    for f in outs[0]._fields:
+        assert torch.equal(getattr(outs[0], f), getattr(outs[1], f)), f
