@@ -187,6 +187,9 @@ _SIGS = {
     "igmc_occlusion_mask": [C.POINTER(BatchOut), C.c_int, vp, vp, vp, vp, vp, vp, vp, vp],
     "igmc_occlusion_order_ws_bytes": [C.c_int, C.c_int64, C.POINTER(C.c_int64)],
     "igmc_occlusion_order": [vp, vp, vp, C.c_int, C.c_int64, vp, vp, vp, C.c_int, vp, C.c_int64, vp, vp, vp, vp, vp],
+    "igmc_edge_grad": [C.POINTER(Model), vp, vp, vp, vp, C.POINTER(Adj), C.c_int, C.c_int, C.POINTER(Dropout),
+                       C.POINTER(Saved), vp, vp, C.c_int, vp, vp],
+    "igmc_edge_grad_scatter": [C.POINTER(BatchOut), C.c_int, vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp],
     "igmc_corated_ws_bytes":[C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int64)],
     "igmc_corated_items": [C.POINTER(CSR), vp, C.c_int, C.c_int, C.c_int, vp, C.c_int64, vp, vp, vp, vp],
     "igmc_graph_update_ws_bytes": [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int64)],

@@ -14,6 +14,9 @@
 //                       (~orderable(|delta|) << 32) | j, then all of each segment or its first m entries
 // Every copy of pair q samples its subgraph with the same pair id, so it is the same subgraph and edge j is the same
 // rating in every copy.  The sort key is a strict total order, so nothing depends on batch boundaries.
+// Attribution (attribute_pairs) reuses the count, offsets and order: its gradient pass extracts the P pairs again and
+// k_edge_grad_scatter sums each rating's two directed-edge gradients of igmc_edge_grad (csrc/rgcn_l2.cu) into its
+// position; igmc_occlusion_order then orders those values as they are (score = NULL).
 #include <algorithm>
 
 #include <cub/block/block_scan.cuh>
@@ -95,6 +98,17 @@ k_occlusion_pairs(igmc_csr_t G, const int32_t* __restrict__ pair_u, const int32_
   if (threadIdx.x == 0) *cursor = pos + B;
 }
 
+// global user, item and label of the rating whose user -> item edge is a (an extracted batch's edge_index, row stride
+// row_stride) at position c
+__device__ __forceinline__ void record_rating(const int64_t* __restrict__ edge_index, long long row_stride,
+                                              const int64_t* __restrict__ edge_type, const int32_t* __restrict__ node_gid,
+                                              int a, long long c, int32_t* __restrict__ out_user,
+                                              int32_t* __restrict__ out_item, int32_t* __restrict__ out_rating) {
+  out_user[c] = node_gid[edge_index[a]];
+  out_item[c] = node_gid[edge_index[row_stride + a]];
+  out_rating[c] = (int32_t)edge_type[a];
+}
+
 // graph i of an extracted occlusion batch; its edge_index is [u|v ; v|u], so undirected edge j is the directed pair
 // edge_ptr[i] + j (user -> item) and edge_ptr[i] + m + j (item -> user), m = the graph's undirected edge count
 __global__ void __launch_bounds__(MASK_THREADS)
@@ -114,10 +128,34 @@ k_occlusion_mask(const int32_t* __restrict__ edge_ptr, const int64_t* __restrict
   }
   const int a = e0 + j, b = a + m;
   for (int e = e0 + threadIdx.x; e < e1; e += blockDim.x) edge_keep[e] = (drop && (e == a || e == b)) ? 0 : 1;
-  if (drop && threadIdx.x == 0) {
-    out_user[c] = node_gid[edge_index[a]];
-    out_item[c] = node_gid[edge_index[row_stride + a]];
-    out_rating[c] = (int32_t)edge_type[a];
+  if (drop && threadIdx.x == 0)
+    record_rating(edge_index, row_stride, edge_type, node_gid, a, c, out_user, out_item, out_rating);
+}
+
+// graph i of an attribution batch with tag q >= 0: rating j's value is the sum of its two directed edges' gradients,
+// out[offsets[q] + j] = (checkpoint k = 0 ? 0 : out) + that sum, divided by K after the last checkpoint k = K - 1
+__global__ void __launch_bounds__(MASK_THREADS)
+k_edge_grad_scatter(const int32_t* __restrict__ edge_ptr, const int64_t* __restrict__ edge_index, long long row_stride,
+                    const int64_t* __restrict__ edge_type, const int32_t* __restrict__ node_gid,
+                    const int64_t* __restrict__ tag, const float* __restrict__ edge_grad,
+                    const int64_t* __restrict__ offsets, int k, int K, float* __restrict__ out,
+                    int32_t* __restrict__ out_user, int32_t* __restrict__ out_item, int32_t* __restrict__ out_rating,
+                    int* err) {
+  const int i = blockIdx.x;
+  const long long q = tag[i];
+  if (q < 0) return;
+  const int e0 = edge_ptr[i], m = (edge_ptr[i + 1] - e0) >> 1;
+  const long long o = offsets[q];
+  if (offsets[q + 1] - o != m) {   // the subgraph is not the one the base pass counted
+    if (threadIdx.x == 0) igmc_set_err(err, IGMC_ERR_CANDIDATES);
+    return;
+  }
+  for (int j = threadIdx.x; j < m; j += blockDim.x) {
+    float v = edge_grad[e0 + j] + edge_grad[e0 + m + j];
+    if (k > 0) v = out[o + j] + v;
+    if (k == K - 1) v = v / (float)K;
+    out[o + j] = v;
+    if (k == 0) record_rating(edge_index, row_stride, edge_type, node_gid, e0 + j, o + j, out_user, out_item, out_rating);
   }
 }
 
@@ -132,7 +170,7 @@ __global__ void k_order_keys(const float* __restrict__ score, const float* __res
                              int32_t* __restrict__ pos, float* __restrict__ delta) {
   for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < T; c += gridDim.x * blockDim.x) {
     const int q = owner(offsets, P, c);
-    const float d = __fsub_rn(occluded[c], score[q]);
+    const float d = score ? __fsub_rn(occluded[c], score[q]) : occluded[c];
     const uint32_t j = (uint32_t)(c - offsets[q]);
     keys[c] = ((uint64_t)~orderable_abs(d) << 32) | j;
     pos[c] = c;
@@ -245,6 +283,18 @@ extern "C" int igmc_occlusion_mask(const igmc_batch_out_t* O, int B, const int64
   return 0;
 }
 
+extern "C" int igmc_edge_grad_scatter(const igmc_batch_out_t* O, int B, const int64_t* tag, const float* edge_grad,
+                                      const int64_t* offsets, int k, int K, float* out, int32_t* user, int32_t* item,
+                                      int32_t* rating, int* err, void* stream) {
+  if (!O || !O->edge_ptr || !O->edge_index || !O->edge_type || !O->node_gid || B <= 0) return -1;
+  if (!tag || !edge_grad || !offsets || !out || !user || !item || !rating || K < 1 || k < 0 || k >= K) return -1;
+  k_edge_grad_scatter<<<B, MASK_THREADS, 0, (cudaStream_t)stream>>>(O->edge_ptr, O->edge_index, O->edge_cap,
+                                                                     O->edge_type, O->node_gid, tag, edge_grad, offsets,
+                                                                     k, K, out, user, item, rating, err);
+  IGMC_CUDA_CHECK_LAUNCH();
+  return 0;
+}
+
 extern "C" int igmc_occlusion_order_ws_bytes(int num_pairs, int64_t num_positions, int64_t* bytes) {
   if (!bytes || !order_shape_ok(num_pairs, num_positions)) return -1;
   *bytes = (int64_t)order_layout(nullptr, num_pairs, (int)num_positions, 0).total;
@@ -259,7 +309,7 @@ extern "C" int igmc_occlusion_order(const float* score, const float* occluded, c
   const int P = num_pairs, T = (int)num_positions;
   if (P == 0 || (T == 0 && m == 0)) return 0;
   if (!offsets || !out_user || !out_item || !out_rating || !out_delta || !ws) return -1;
-  if (T > 0 && (!score || !occluded || !user || !item || !rating)) return -1;
+  if (T > 0 && (!occluded || !user || !item || !rating)) return -1;
   cudaStream_t st = (cudaStream_t)stream;
   const OrderLayout L = order_layout(ws, P, T, st);
   if ((int64_t)L.total > ws_bytes) return -2;

@@ -64,7 +64,8 @@ __device__ __forceinline__ float hidden_scale(const igmc_dropout_t& D, uint64_t 
 // Walks list [p0,p1) of one node with the whole warp; body(nbr, type) is called warp-uniformly for
 // every kept entry, in list order.  `mirror`: the entry describes edge nbr->x but the caller wants
 // the reverse edge x->nbr of a symmetric batch, whose id is the mirror image inside the graph.
-template <class Body>
+// WITH_ID: body(nbr, type, e) also gets that directed edge's id e (the id the keep draw reads).
+template <bool WITH_ID = false, class Body>
 __device__ __forceinline__ int list_foreach(const uint32_t* __restrict__ adj, const int32_t* __restrict__ eid,
                                             int p0, int p1, const EdgeKeep& K, bool mirror, int eb, int m_half,
                                             int lane, Body&& body) {
@@ -72,12 +73,13 @@ __device__ __forceinline__ int list_foreach(const uint32_t* __restrict__ adj, co
   for (int c = p0; c < p1; c += 32) {
     const int p = c + lane;
     uint32_t ent = DROPPED;
+    int e = -1;
     if (p < p1) {
       ent = adj[p];
-      if (K.active) {
-        int e = eid[p];
+      if (WITH_ID || K.active) {
+        e = eid[p];
         if (mirror) { const int el = e - eb; e = eb + (el < m_half ? el + m_half : el - m_half); }
-        if (!K.keep(e)) ent = DROPPED;
+        if (K.active && !K.keep(e)) ent = DROPPED;
       }
     }
     const int cnt = min(32, p1 - c);
@@ -85,7 +87,8 @@ __device__ __forceinline__ int list_foreach(const uint32_t* __restrict__ adj, co
       const uint32_t en = __shfl_sync(IGMC_FULL, ent, q);
       if (en == DROPPED) continue;
       ++kept;
-      body((int)(en & 0xffffu), (int)((en >> 16) & 0xffu));
+      if constexpr (WITH_ID) body((int)(en & 0xffffu), (int)((en >> 16) & 0xffu), __shfl_sync(IGMC_FULL, e, q));
+      else body((int)(en & 0xffffu), (int)((en >> 16) & 0xffu));
     }
   }
   return kept;

@@ -465,6 +465,9 @@ int l2_backward(const igmc_model_t* M, const float* params, const uint8_t* node_
                 const int32_t* edge_ptr, const igmc_adj_t* A, int B, int csize, const igmc_dropout_t* D,
                 const igmc_saved_t* S, const float* dpred, float* gpart, float* dhid, float* dbuf, int* err,
                 cudaStream_t st);
+int l2_edge_grad(const igmc_model_t* M, const float* params, const uint8_t* node_label, const int32_t* node_ptr,
+                 const int32_t* edge_ptr, const igmc_adj_t* A, int B, int csize, const igmc_dropout_t* D,
+                 const igmc_saved_t* S, const float* dpred, float* edge_grad, float* dbuf, int* err, cudaStream_t st);
 
 // CTAs per subgraph of an IGMC_PLAN_L2(c) value, 0 for every other plan value
 static int l2_csize(int cluster) {
@@ -608,4 +611,21 @@ extern "C" int igmc_backward(const igmc_model_t* M, const float* params, const u
                                     err);
   IGMC_CUDA_CHECK_LAUNCH();
   return 0;
+}
+
+extern "C" int igmc_edge_grad(const igmc_model_t* M, const float* params, const uint8_t* node_label,
+                              const int32_t* node_ptr, const int32_t* edge_ptr, const igmc_adj_t* A, int B, int n_cap,
+                              const igmc_dropout_t* D, const igmc_saved_t* S, const float* dpred, float* edge_grad,
+                              int cluster, int* err, void* stream) {
+  if (B <= 0) return 0;
+  int rc = check_model(M);
+  if (rc) return rc;
+  const int c = l2_csize(cluster);
+  if (!c) return -16;
+  if (D->adj_dropout > 0.f || D->edge_keep) return -18;   // every edge kept: each one gets its gradient
+  if (M->readout != 0 && !S->dstate) return -17;
+  if (!S->l2_scratch || !dpred || !edge_grad) return -17;
+  if (n_cap > IGMC_L2_MAX_NODES) return -3;
+  return l2_edge_grad(M, params, node_label, node_ptr, edge_ptr, A, B, c, D, S, dpred, edge_grad, S->l2_scratch, err,
+                      (cudaStream_t)stream);
 }

@@ -164,10 +164,61 @@ k_l2_forward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __
                  dpred, lane);
 }
 
+// Per-edge score gradient of layer l at own node v (warp-wide; the EG mode of k_l2_backward).  dz[b] = dZ'[v,b,lane]
+// (1/deg(v) applied; under PR not), so t = <h_{l-1}[j], sum_b att[r,b] dZ'[v,b]> is s/deg(v) (PR: s).  A first walk
+// sums t over the segment (one per-lane partial, a warp sum per segment; PR: per type run, its mean kept in mean_r[r]),
+// a second forms each entry's t again and writes t - mean (PR: (t - mean_r) / |N_r(v)|) into edge_grad[e]: stored
+// when `first` (the top layer), added otherwise.  A segment of one entry gives exactly 0: both walks round the same
+// products and sum them in the same order.
+template <int NB, bool PR, class H>
+__device__ __forceinline__ void edge_terms(const igmc_adj_t& A, const EdgeKeep& K, int nb, int v, int eb, int m_half,
+                                           int lane, int R, const H& hp, const float* __restrict__ att_s,
+                                           const float (&dz)[NB], const float* __restrict__ rinv, float* mean_r,
+                                           bool first, float* __restrict__ edge_grad) {
+  const int p0 = A.in_ptr[nb + v], p1 = A.in_ptr[nb + v + 1];
+  auto term = [&](int nbr, int ty) {
+    float p = 0.f;
+#pragma unroll
+    for (int b = 0; b < NB; ++b) p = fmaf(att_s[ty * NB + b], dz[b], p);
+    return hp(nbr, lane) * p;
+  };
+  float part = 0.f;
+  int cur = -1, cnt = 0;
+  auto flush = [&]() {
+    const float s = warp_sum_f(part);
+    if (lane == 0) mean_r[cur] = s / (float)cnt;
+  };
+  const int kept = list_foreach(A.in_adj, A.in_eid, p0, p1, K, false, eb, m_half, lane, [&](int nbr, int ty) {
+    if (PR && ty != cur) {
+      if (cur >= 0) flush();
+      part = 0.f;
+      cur = ty;
+      cnt = 0;
+    }
+    part += term(nbr, ty);
+    ++cnt;
+  });
+  if (kept == 0) return;
+  float mean = 0.f;
+  if (PR) flush();
+  else mean = warp_sum_f(part) / (float)kept;
+  __syncwarp();
+  list_foreach<true>(A.in_adj, A.in_eid, p0, p1, K, false, eb, m_half, lane, [&](int nbr, int ty, int e) {
+    const float t = warp_sum_f(term(nbr, ty));
+    const float d = PR ? (t - mean_r[ty]) * __ldcg(rinv + (size_t)v * R + ty) : t - mean;
+    if (lane == 0) edge_grad[e] = first ? d : edge_grad[e] + d;
+  });
+  __syncwarp();   // mean_r is read before the warp's next node overwrites it
+}
+
 // ------------------------------------------------------------------------------------------------
 // backward
 // ------------------------------------------------------------------------------------------------
-template <int NB, bool PR>
+// EG (igmc_edge_grad): no parameter gradients.  Passes (0) and (1) and the dZ' tile run as in training; pass (3)'s
+// in-list walk forms, per directed edge j->v of type r, s/|seg| - mean over the segment, s = <h_{l-1}[j] W_r, dpre[v]>
+// (segment: v's in-list, or its type run under PR), and adds it into gpart[edge id] (there: edge_grad[edge_ptr[B]])
+// layer by layer.  Every edge is an in-edge of one own node of one CTA: one writer per element, in a fixed order.
+template <int NB, bool PR, bool EG = false>
 __global__ void __launch_bounds__(THREADS)
 k_l2_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* __restrict__ node_label,
               const int32_t* __restrict__ node_ptr, const int32_t* __restrict__ edge_ptr, igmc_adj_t A, int csize,
@@ -211,7 +262,7 @@ k_l2_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* _
 
   // ---- readout backward: d hid, d feat (models.py:211-213) ----
   if (!ext) {
-    readout_dhid(M, params, S, dpred, g, dhid_s, dhid_out, rank == 0, tid, THREADS);
+    readout_dhid(M, params, S, dpred, g, dhid_s, dhid_out, !EG && rank == 0, tid, THREADS);
     __syncthreads();
     for (int i = tid; i < F; i += THREADS) readout_dfeat_part(M, params, dhid_s, F, 1, i, dfeat);
   }
@@ -238,7 +289,8 @@ k_l2_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* _
       X[(size_t)v * HID + c] = dh * (1.f - h * h);
     }
     for (int idx = tid; idx < R * NB; idx += THREADS) att_s[idx] = params[M.off_att[l] + idx];
-    for (int idx = tid; idx < WARPS * R * NB; idx += THREADS) datt_w[idx] = 0.f;
+    if (!EG)
+      for (int idx = tid; idx < WARPS * R * NB; idx += THREADS) datt_w[idx] = 0.f;
     // d pre_l of every node of the subgraph is in L2 from here on.  (Y, written below, was last read by the previous
     // layer's pass (1) of the other CTAs, which they finished before arriving here.)
     cluster_sync_rel_acq();
@@ -306,17 +358,18 @@ k_l2_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* _
       double* dw = datt_w + warp * (R * NB);
       for (int t0 = v0; t0 < v1; t0 += TM) {
         const int tend = min(t0 + TM, v1), rows = tend - t0;
-        for (int idx = tid; idx < rows * (NB * HID); idx += THREADS) {
-          const int r = idx / (NB * HID), c = idx - r * (NB * HID);
-          Zs[r * ZB + c] = S.zsave[((size_t)l * S.node_cap + nb + t0 + r) * (NB * HID) + c];
-        }
+        if (!EG)
+          for (int idx = tid; idx < rows * (NB * HID); idx += THREADS) {
+            const int r = idx / (NB * HID), c = idx - r * (NB * HID);
+            Zs[r * ZB + c] = S.zsave[((size_t)l * S.node_cap + nb + t0 + r) * (NB * HID) + c];
+          }
         for (int idx = tid; idx < rows * HID; idx += THREADS) {
           const int r = idx >> 5, c = idx & 31;
           Zs[r * ZB + NB * HID + c] = __ldcg(X + (size_t)(t0 + r) * HID + c);
-          Zs[r * ZB + (NB + 1) * HID + c] = hp(t0 + r, c);
+          if (!EG) Zs[r * ZB + (NB + 1) * HID + c] = hp(t0 + r, c);
         }
         __syncthreads();
-        if (kg < in) {
+        if (!EG && kg < in) {
           for (int r = 0; r < rows; ++r) {
             const float* zr = Zs + r * ZB;
             const float4 d = *reinterpret_cast<const float4*>(zr + NB * HID + c0);
@@ -365,6 +418,11 @@ k_l2_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* _
           float dz[NB];
 #pragma unroll
           for (int b = 0; b < NB; ++b) dz[b] = (lane < in) ? Zs[(v - t0) * ZB + b * HID + lane] : 0.f;
+          if constexpr (EG) {
+            edge_terms<NB, PR>(A, K, nb, v, eb, m_half, lane, R, hp, att_s, dz, rinv,
+                               reinterpret_cast<float*>(datt_w) + warp * R, l == L - 1, gpart);
+            continue;
+          }
           float run = 0.f;
           int cur = -1, cnt = 0;
           auto flush = [&]() {
@@ -390,12 +448,14 @@ k_l2_backward(igmc_model_t M, const float* __restrict__ params, const uint8_t* _
         }
         __syncthreads();
       }
-      store_wgrad_rows<NB>(M, l, in, kg, c0, acc, accb, gp);
-      __syncthreads();
-      for (int idx = tid; idx < R * NB; idx += THREADS) {
-        double s = 0.0;
-        for (int w = 0; w < WARPS; ++w) s += datt_w[w * (R * NB) + idx];
-        gp[M.off_att[l] + idx] = (float)s;
+      if (!EG) {
+        store_wgrad_rows<NB>(M, l, in, kg, c0, acc, accb, gp);
+        __syncthreads();
+        for (int idx = tid; idx < R * NB; idx += THREADS) {
+          double s = 0.0;
+          for (int w = 0; w < WARPS; ++w) s += datt_w[w * (R * NB) + idx];
+          gp[M.off_att[l] + idx] = (float)s;
+        }
       }
       __syncthreads();
     }
@@ -443,4 +503,15 @@ int l2_backward(const igmc_model_t* M, const float* params, const uint8_t* node_
                                 : (S->rel_inv_deg ? k_l2_backward<2, true> : k_l2_backward<2, false>);
   return launch_cluster(kern, B * csize, THREADS, smem, csize, false, st, *M, params, node_label, node_ptr, edge_ptr, *A,
                         csize, *D, *S, dpred, gpart, dhid, dbuf, err);
+}
+
+int l2_edge_grad(const igmc_model_t* M, const float* params, const uint8_t* node_label, const int32_t* node_ptr,
+                 const int32_t* edge_ptr, const igmc_adj_t* A, int B, int csize, const igmc_dropout_t* D,
+                 const igmc_saved_t* S, const float* dpred, float* edge_grad, float* dbuf, int* err, cudaStream_t st) {
+  const size_t smem = l2_smem_bytes(M, 1);
+  auto kern = M->num_bases == 4
+                  ? (S->rel_inv_deg ? k_l2_backward<4, true, true> : k_l2_backward<4, false, true>)
+                  : (S->rel_inv_deg ? k_l2_backward<2, true, true> : k_l2_backward<2, false, true>);
+  return launch_cluster(kern, B * csize, THREADS, smem, csize, false, st, *M, params, node_label, node_ptr, edge_ptr, *A,
+                        csize, *D, *S, dpred, edge_grad, (float*)nullptr, dbuf, err);
 }

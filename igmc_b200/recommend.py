@@ -14,6 +14,9 @@ building a dataset of every candidate pair and looping over it in Python.  Here:
 * ``explain_pairs(model, graph, users, items, m)`` -> per pair its score and, for every rating in its enclosing
   subgraph, the score change from removing that rating (csrc/explain.cu): a base pass of the pairs, then an occlusion
   pass over (pair, rating) positions whose batches carry an edge mask into a training-mode forward without dropout;
+* ``attribute_pairs(model, graph, users, items, m)`` -> the same layout with, per rating, the score's gradient with
+  respect to a weight on that rating (igmc_edge_grad): the same base pass, then one gradient pass over the P pairs, each
+  an L2-plan eval forward and one backward whose list walk writes every edge's term;
 * ``InferenceEngine``: the pipelined, graph-replayed loop behind all of them.  Per step the side stream produces the next
   batch's candidate pairs (``igmc_candidate_pairs``, from a device cursor) and extracts it while the main stream runs
   the eval forward of the current batch (once per checkpoint) and merges its scores into the running per-user top-k
@@ -35,7 +38,8 @@ from . import _lib
 from .train_eval import replay_step
 from .util_functions import RatingGraph, SubgraphExtractor, _stream_ptr
 
-__all__ = ["predict_pairs", "recommend", "corated_items", "explain_pairs", "Explanation", "InferenceEngine"]
+__all__ = ["predict_pairs", "recommend", "corated_items", "explain_pairs", "Explanation", "attribute_pairs",
+           "Attribution", "InferenceEngine"]
 
 
 # ---- input validation (host) ----------------------------------------------------------------------------------------
@@ -131,6 +135,10 @@ def _check_top(m, name):
 # delta fp32 (score without the rating - score): flat [offsets[P]] with pair p at [offsets[p], offsets[p+1]), or
 # [P, m] padded with -1 / -1 / -1 / 0.
 Explanation = collections.namedtuple("Explanation", "score num_edges offsets user item rating delta")
+
+# The result of attribute_pairs: Explanation's layout and order with grad (d score / d m_e, the rating's weight m_e at
+# m = 1) in place of delta.  -grad is the first-order estimate of explain_pairs' delta.
+Attribution = collections.namedtuple("Attribution", "score num_edges offsets user item rating grad")
 
 
 # ---- host twins of the candidate and merge kernels (csrc/recommend.cu) ----------------------------------------------
@@ -309,12 +317,13 @@ def occlusion_mask_host(edge_ptr, tag, edge_j):
 
 def explain_order_host(score, occluded, offsets, m=None):
     """twin of igmc_occlusion_order's permutation: (delta [T] fp32, order) where order is, per pair q, the positions of
-    its segment by |delta| descending, NaN after every number, ties by j - flat [T] (m None) or [P, m] padded with -1"""
-    score, occluded = np.asarray(score, np.float32), np.asarray(occluded, np.float32)
+    its segment by |delta| descending, NaN after every number, ties by j - flat [T] (m None) or [P, m] padded with -1.
+    ``score`` None: delta = occluded (attribution gradients)"""
+    occluded = np.asarray(occluded, np.float32)
     offsets = np.asarray(offsets, np.int64)
     P = len(offsets) - 1
     q = np.repeat(np.arange(P), np.diff(offsets))
-    delta = (occluded - score[q]).astype(np.float32)
+    delta = occluded.copy() if score is None else (occluded - np.asarray(score, np.float32)[q]).astype(np.float32)
     order = []
     for p in range(P):
         seg = np.arange(offsets[p], offsets[p + 1])
@@ -329,6 +338,27 @@ def explain_order_host(score, occluded, offsets, m=None):
     return delta, top
 
 
+def edge_grad_scatter_host(edge_ptr, tag, edge_grad, offsets, out, k=0, K=1):
+    """twin of igmc_edge_grad_scatter's values for checkpoint ``k`` of ``K``: graph g with tag q >= 0 writes rating j's
+    edge_grad[e0 + j] + edge_grad[e0 + E_g/2 + j] to out[offsets[q] + j] (k = 0), or adds it (k > 0), then divides by
+    K (k = K - 1); fp32 throughout.  ``out`` [T] is updated in place and returned"""
+    edge_ptr, offsets = np.asarray(edge_ptr, np.int64), np.asarray(offsets, np.int64)
+    edge_grad = np.asarray(edge_grad, np.float32)
+    for g in range(len(edge_ptr) - 1):
+        q = int(tag[g])
+        if q < 0:
+            continue
+        e0, m = int(edge_ptr[g]), int(edge_ptr[g + 1] - edge_ptr[g]) // 2
+        v = edge_grad[e0:e0 + m] + edge_grad[e0 + m:e0 + 2 * m]
+        o = int(offsets[q])
+        if k > 0:
+            v = out[o:o + m] + v
+        if k == K - 1:
+            v = v / np.float32(K)
+        out[o:o + m] = v
+    return out
+
+
 # ---- the engine -----------------------------------------------------------------------------------------------------
 class InferenceEngine(object):
     """Pipelined, graph-replayed scoring of candidate pairs (module docstring).  ``checkpoints``: state_dict files of
@@ -336,10 +366,10 @@ class InferenceEngine(object):
     parameters as they are when a run starts.
 
         eng = InferenceEngine(model, graph, batch_size=256)
-        eng.start_recommend(users, k)          # or eng.start_pairs(users, items) / eng.start_explain(users, items, m)
+        eng.start_recommend(users, k)          # or start_pairs(users, items) / start_explain / start_attribute(users, items, m)
         while eng.step():
             pass
-        top_items, top_scores = eng.finish()   # (predict: scores; explain: an Explanation)
+        top_items, top_scores = eng.finish()   # (predict: scores; explain: an Explanation; attribute: an Attribution)
 
     An engine serves across updates of its ``RatingGraph`` (``graph.update``) between runs; an update during a run
     makes its next ``step`` raise RuntimeError.
@@ -387,6 +417,7 @@ class InferenceEngine(object):
         self.side = torch.cuda.Stream(dev)
         self.run = None
         self._retrieve_ws = {}       # the retriever's workspace when its histograms do not fit in shared memory
+        self._grad_plans = {}        # the model's plan cache while a gradient pass forces the L2 plan
 
     # ---- one run: plan, prime, steps, finish --------------------------------------------------------------------
     def start_recommend(self, users, k, items=None, exclude_rated=True, retrieve=None):
@@ -476,6 +507,13 @@ class InferenceEngine(object):
         m = _check_top(m, "m")
         return self._start_explicit("explain", users, items, m=m, phase="base")
 
+    def start_attribute(self, users, items, m=None):
+        """plan an attribution run over the explicit pairs (users[i], items[i]) (``attribute_pairs``): the base pass of
+        ``start_explain``, then (after the run's one host sync, the rating total) a gradient pass over the same pairs.
+        ``m``: keep each pair's first m ratings.  Returns the number of pairs."""
+        m = _check_top(m, "m")
+        return self._start_explicit("attribute", users, items, m=m, phase="base")
+
     def _start_explicit(self, kind, users, items, **extra):
         g = self.graph
         users = _host_ids(users, "users", g.num_users)
@@ -485,11 +523,11 @@ class InferenceEngine(object):
         P, dev = len(users), self.dev
         run = dict(kind=kind, P=P, version=g.version, scores=torch.empty(P, dtype=torch.float32, device=dev), **extra)
         self.run = run
-        if kind == "explain":
+        if kind in ("explain", "attribute"):
             run["num_edges"] = torch.zeros(P, dtype=torch.int32, device=dev)
             run["offsets"] = torch.zeros(P + 1, dtype=torch.int64, device=dev)
             for s in self.slots:
-                if "j" not in s:
+                if kind == "explain" and "j" not in s:
                     s["j"] = torch.zeros(self.B, dtype=torch.int32, device=dev)
         if P == 0:
             return 0
@@ -501,22 +539,29 @@ class InferenceEngine(object):
         self._prime()
         return P
 
-    def _start_occlusion(self):
-        """after the base pass of an explanation run: the offsets of the pairs' ratings, their total T (the run's one
-        host sync), the output buffers [T] and the occlusion pass primed.  Returns True when it has positions."""
+    def _rating_total(self, phase):
+        """after the base pass of an explanation or attribution run: the offsets of the pairs' ratings, their total T
+        (the run's one host sync) and the output buffers [T] (run["occ"]: occluded scores or gradients).  Returns T."""
         run, dev = self.run, self.dev
         _lib.check(self.lib.igmc_explain_offsets(run["num_edges"].data_ptr(), run["P"], run["offsets"].data_ptr(),
                                                  _stream_ptr()), "igmc_explain_offsets")
         T = run["T"] = int(run["offsets"][run["P"]].item())
-        run["phase"] = "occlude"
+        run["phase"] = phase
         run["occ"] = torch.empty(T, dtype=torch.float32, device=dev)
         for k in ("user", "item", "rating"):
             run[k] = torch.empty(T, dtype=torch.int32, device=dev)
         if T == 0:
             run["steps"] = run["done"] = 0
-            return False
         if T >= (1 << 31) - 1:
             raise NotImplementedError("an explanation run covers fewer than 2^31 - 1 ratings, not %d" % T)
+        return T
+
+    def _start_occlusion(self):
+        """the occlusion pass of an explanation run primed.  Returns True when it has positions."""
+        T = self._rating_total("occlude")
+        if T == 0:
+            return False
+        run, dev = self.run, self.dev
         ecap = self.extractor._out_caps(self.B)[1]
         for s in self.slots:
             if s.get("keep") is None or s["keep"].numel() < ecap:
@@ -527,6 +572,44 @@ class InferenceEngine(object):
             s["drop"] = (d, [s["keep"]])
         self._prime(T)
         return True
+
+    def _start_gradient(self):
+        """the gradient pass of an attribution run primed: the P pairs again, on the L2 plan with as many CTAs per
+        subgraph as ``l2_cluster`` gives this batch shape, whatever plan the model chose for the base pass.  Returns
+        True when there are ratings."""
+        from .models import l2_cluster
+        n_cap = self.batches[0]._priv["n_cap"]
+        if self._rating_total("grad") == 0:
+            return False
+        run, m, dev = self.run, self.model, self.dev
+        sms = torch.cuda.get_device_properties(dev).multi_processor_count
+        run["plan"] = _lib.plan_l2(l2_cluster(n_cap, self.B, sms))
+        ncap, ecap = self.extractor._out_caps(self.B)[:2]
+        L, f32 = len(m.convs), dict(dtype=torch.float32, device=dev)
+        ext = m._cmodel.readout != 0
+        # d score / d lin2 output of every graph: multiply_by for IGMC, 1 for DGCNN_RS (its lin2 output is the score)
+        run["gws"] = dict(seed=torch.full((self.B,), 1.0 if ext else float(m._cmodel.multiply_by), **f32),
+                          scratch=torch.empty(2, ncap, _lib.HIDDEN, **f32), edge_grad=torch.empty(ecap, **f32),
+                          dstate=torch.empty(ncap, _lib.HIDDEN * L, **f32) if ext else None,
+                          pgrad=torch.zeros(m._cmodel.param_count, **f32) if ext else None)
+        with self._forced_plan():
+            self._prime()
+        return True
+
+    @contextlib.contextmanager
+    def _forced_plan(self):
+        """inside the block the model launches the gradient pass's plan (run["plan"], with its own plan cache); the
+        model's plan and cache are restored after it"""
+        run, m = self.run, self.model
+        if run is None or run.get("plan") is None:
+            yield
+            return
+        own = (m.kernel_plan, m._plans)
+        m.kernel_plan, m._plans = run["plan"], self._grad_plans
+        try:
+            yield
+        finally:
+            m.kernel_plan, m._plans = own
 
     def _prime(self, total=None):
         """candidate pairs + extraction of the first batch, the model's plan for it (its one host sync, if any) and
@@ -567,7 +650,7 @@ class InferenceEngine(object):
                                                     s["j"].data_ptr(), s["keep"].data_ptr(), run["user"].data_ptr(),
                                                     run["item"].data_ptr(), run["rating"].data_ptr(), err,
                                                     _stream_ptr()), "igmc_occlusion_mask")
-        elif run["kind"] == "explain":
+        elif run.get("phase") == "base":
             _lib.check(self.lib.igmc_explain_count(b._priv["edge_ptr"].data_ptr(), s["tag"].data_ptr(), self.B,
                                                    run["num_edges"].data_ptr(), _stream_ptr()), "igmc_explain_count")
 
@@ -588,6 +671,8 @@ class InferenceEngine(object):
         batch runs the training-mode forward with its slot's edge mask and no dropout: the eval forward of each
         subgraph without its masked rating."""
         m, b, s, run = self.model, self.batches[slot], self.slots[slot], self.run
+        if run.get("phase") == "grad":
+            return self._gradient(slot)
         occlude = run.get("phase") == "occlude"
         training, drop = (True, s["drop"]) if occlude else (False, self.drop)
         preds = None
@@ -608,15 +693,50 @@ class InferenceEngine(object):
             _lib.check(self.lib.igmc_score_scatter(preds.data_ptr(), self.K, self.B, s["tag"].data_ptr(),
                                                    out.data_ptr(), _stream_ptr()), "igmc_score_scatter")
 
+    def _gradient(self, slot):
+        """per parameter set: the eval forward of batch ``slot`` on the L2 plan, (DGCNN_RS) the SortPooling backward
+        seeded with d score / d lin2 output, igmc_edge_grad and the scatter of each rating's gradient to its position
+        (checkpoint k of K: stored, then added, then divided by K)"""
+        m, b, s, run = self.model, self.batches[slot], self.slots[slot], self.run
+        gw, p, st = run["gws"], b._priv, _stream_ptr()
+        adj_c, _ = b.adjacency()
+        d = self.drop[0]
+        for j in range(self.K):
+            with self._params(j):
+                _, saved = m._launch_forward(b, False, self.drop)
+                ws = saved["ws"]
+                S = _lib.Saved.from_buffer_copy(saved["S"])
+                S.l2_scratch = gw["scratch"].data_ptr()
+                if gw["dstate"] is not None:
+                    S.dstate = gw["dstate"].data_ptr()
+                    _lib.check(self.lib.igmc_sortpool_backward(C.byref(m._csort), m.flat_params.data_ptr(),
+                                                               ws["states"].data_ptr(), p["node_ptr"].data_ptr(),
+                                                               self.B, p["n_cap"], C.byref(ws["sp"]["S"]),
+                                                               gw["seed"].data_ptr(), gw["dstate"].data_ptr(), 1.0,
+                                                               gw["pgrad"].data_ptr(), b._err.data_ptr(), st),
+                               "igmc_sortpool_backward")
+                _lib.check(self.lib.igmc_edge_grad(C.byref(m._cmodel), m.flat_params.data_ptr(),
+                                                   p["node_label"].data_ptr(), p["node_ptr"].data_ptr(),
+                                                   p["edge_ptr"].data_ptr(), C.byref(adj_c), self.B, p["n_cap"],
+                                                   C.byref(d), C.byref(S), gw["seed"].data_ptr(),
+                                                   gw["edge_grad"].data_ptr(), ws["cluster"], b._err.data_ptr(), st),
+                           "igmc_edge_grad")
+            _lib.check(self.lib.igmc_edge_grad_scatter(C.byref(b._lazy["_c"]), self.B, s["tag"].data_ptr(),
+                                                       gw["edge_grad"].data_ptr(), run["offsets"].data_ptr(), j,
+                                                       self.K, run["occ"].data_ptr(), run["user"].data_ptr(),
+                                                       run["item"].data_ptr(), run["rating"].data_ptr(),
+                                                       self.extractor.err.data_ptr(), st), "igmc_edge_grad_scatter")
+
     def _launch(self, slot):
         main = torch.cuda.current_stream()
         self.side.wait_stream(main)
-        with torch.cuda.stream(self.side):
-            # the next batch is produced and extracted beside this batch's forward (gate: only once the forward's
-            # clusters are resident, see TrainEngine._launch_pipe); after the last batch it is all padding
-            self.model.gate_wait(self.batches[slot])
-            self._next(slot ^ 1)
-        self._score(slot)
+        with self._forced_plan():
+            with torch.cuda.stream(self.side):
+                # the next batch is produced and extracted beside this batch's forward (gate: only once the forward's
+                # clusters are resident, see TrainEngine._launch_pipe); after the last batch it is all padding
+                self.model.gate_wait(self.batches[slot])
+                self._next(slot ^ 1)
+            self._score(slot)
         main.wait_stream(self.side)
 
     def step(self):
@@ -632,7 +752,9 @@ class InferenceEngine(object):
         run["done"] += 1
         if run["done"] < run["steps"]:
             return True
-        return run["kind"] == "explain" and run["phase"] == "base" and self._start_occlusion()
+        if run.get("phase") != "base":
+            return False
+        return self._start_occlusion() if run["kind"] == "explain" else self._start_gradient()
 
     def finish(self):
         """wait for the run, check the error word (one host sync) and return (top_items [U, k] int64, top_scores
@@ -640,8 +762,8 @@ class InferenceEngine(object):
         run = self.run
         while self.step():
             pass
-        if run["kind"] == "explain" and run["phase"] == "base":    # no pairs: the run has no occlusion pass
-            self._start_occlusion()
+        if run.get("phase") == "base":    # no pairs: the run has no second pass
+            self._rating_total("none")
         code = int(self.extractor.err.item())
         if code:
             self.extractor.err.zero_()
@@ -649,13 +771,13 @@ class InferenceEngine(object):
         self.run = None
         if run["kind"] == "recommend":
             return run["top_i"], run["top_s"]
-        if run["kind"] == "explain":
+        if run["kind"] in ("explain", "attribute"):
             return self._order(run)
         return run["scores"]
 
     def _order(self, run):
-        """igmc_occlusion_order: every pair's ratings by |delta| descending (NaN last, ties by position), all of them
-        or the first m"""
+        """igmc_occlusion_order: every pair's ratings by |delta| (attribution: |grad|) descending (NaN last, ties by
+        position), all of them or the first m"""
         P, T, m, dev = run["P"], run["T"], run["m"], self.dev
         shape = (P, m) if m else (T,)
         out = dict(user=torch.empty(shape, dtype=torch.int32, device=dev),
@@ -665,14 +787,15 @@ class InferenceEngine(object):
         nbytes = C.c_int64(0)
         _lib.check(self.lib.igmc_occlusion_order_ws_bytes(P, T, C.byref(nbytes)), "igmc_occlusion_order_ws_bytes")
         ws = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=dev)
-        _lib.check(self.lib.igmc_occlusion_order(run["scores"].data_ptr(), run["occ"].data_ptr(),
+        explain = run["kind"] == "explain"
+        _lib.check(self.lib.igmc_occlusion_order(run["scores"].data_ptr() if explain else None, run["occ"].data_ptr(),
                                                  run["offsets"].data_ptr(), P, T, run["user"].data_ptr(),
                                                  run["item"].data_ptr(), run["rating"].data_ptr(), m or 0,
                                                  ws.data_ptr(), ws.numel(), out["user"].data_ptr(),
                                                  out["item"].data_ptr(), out["rating"].data_ptr(),
                                                  out["delta"].data_ptr(), _stream_ptr()), "igmc_occlusion_order")
-        return Explanation(run["scores"], run["num_edges"], run["offsets"], out["user"], out["item"], out["rating"],
-                           out["delta"])
+        return (Explanation if explain else Attribution)(run["scores"], run["num_edges"], run["offsets"], out["user"],
+                                                         out["item"], out["rating"], out["delta"])
 
     def recommend(self, users, k, items=None, exclude_rated=True, retrieve=None):
         self.start_recommend(users, k, items, exclude_rated, retrieve)
@@ -684,6 +807,10 @@ class InferenceEngine(object):
 
     def explain_pairs(self, users, items, m=None):
         self.start_explain(users, items, m)
+        return self.finish()
+
+    def attribute_pairs(self, users, items, m=None):
+        self.start_attribute(users, items, m)
         return self.finish()
 
     def close(self):
@@ -736,6 +863,40 @@ def explain_pairs(model, graph, users, items, m=None, *, h=1, sample_ratio=1.0, 
     eng = InferenceEngine(model, graph, h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
     try:
         return eng.explain_pairs(users, items, m)
+    finally:
+        eng.close()
+
+
+def attribute_pairs(model, graph, users, items, m=None, *, h=1, sample_ratio=1.0, max_nodes_per_hop=None,
+                    batch_size=256, checkpoints=None, sample_seed=0):
+    """why each pair (users[i], items[i]) got its score, to first order and in one backward pass per pair: every rating
+    e of the pair's enclosing subgraph (a rated pair's own rating excluded) gets a weight m_e on the messages of both
+    its directed edges in every layer, the mean normalisers counting the weights (deg(v) = sum of m over v's in-edges;
+    ``rgcn="pyg-2"``: |N_r(v)| per relation), so that a 0/1 weight is dropout_adj's mask and m = 1 the model.  grad =
+    d score / d m_e at m = 1; -grad estimates ``explain_pairs``' delta.  A node whose mean runs over one in-edge (its
+    only one; pyg-2: its only one of that relation) adds nothing at that layer: removing the edge jumps its aggregate
+    to 0, and the relaxation has no slope there.  DGCNN_RS: the gradient flows through the SortPooling order of the
+    forward.  Returns an ``Attribution`` in ``Explanation``'s layout: score [P] (bit for bit ``predict_pairs``),
+    num_edges [P], offsets [P+1], per rating user / item / rating / grad ordered by |grad| descending, NaN last, ties
+    by position; the first ``m`` per pair [P, m] padded with -1 / -1 / -1 / 0.  The gradient pass runs the L2 kernel
+    plan whatever plan the model uses.  ``checkpoints``: score and grad are fp32 checkpoint means (sum in checkpoint
+    order / K)."""
+    nu, ni = graph.shape
+    m = _check_top(m, "m")
+    users, items = _host_ids(users, "users", nu), _host_ids(items, "items", ni)
+    if len(users) != len(items):
+        raise ValueError("users and items must have the same length (%d vs %d)" % (len(users), len(items)))
+    if len(users) == 0:
+        dev = model.flat_params.device
+        shape = (0, m) if m else (0,)
+        i32 = dict(dtype=torch.int32, device=dev)
+        return Attribution(torch.zeros(0, dtype=torch.float32, device=dev), torch.zeros(0, **i32),
+                           torch.zeros(1, dtype=torch.int64, device=dev), torch.zeros(shape, **i32),
+                           torch.zeros(shape, **i32), torch.zeros(shape, **i32),
+                           torch.zeros(shape, dtype=torch.float32, device=dev))
+    eng = InferenceEngine(model, graph, h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
+    try:
+        return eng.attribute_pairs(users, items, m)
     finally:
         eng.close()
 

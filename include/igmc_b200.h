@@ -503,12 +503,39 @@ int igmc_occlusion_mask(const igmc_batch_out_t* O, int B, const int64_t* tag, co
  * ordered by |delta| descending, NaN after every number, ties by j (a segmented radix sort on the 64-bit key
  * (~orderable(|delta|) << 32) | j).  m = 0: out_* [T] in that order; 1 <= m <= IGMC_TOPK_MAX: out_* [num_pairs, m],
  * the first m entries of each segment, padded with user / item / rating -1 and delta 0.  `ws`: at least
- * igmc_occlusion_order_ws_bytes bytes.  num_pairs, num_positions < 2^31 - 1. */
+ * igmc_occlusion_order_ws_bytes bytes.  num_pairs, num_positions < 2^31 - 1.  score = NULL: delta[c] = occluded[c]
+ * (the values are ordered as they are; igmc_edge_grad_scatter's gradients). */
 int igmc_occlusion_order_ws_bytes(int num_pairs, int64_t num_positions, int64_t* bytes);
 int igmc_occlusion_order(const float* score, const float* occluded, const int64_t* offsets, int num_pairs,
                          int64_t num_positions, const int32_t* user, const int32_t* item, const int32_t* rating,
                          int m, void* ws, int64_t ws_bytes, int32_t* out_user, int32_t* out_item, int32_t* out_rating,
                          float* out_delta, void* stream);
+
+/* ---- attribution by the score's gradient per rating (csrc/rgcn_l2.cu, csrc/explain.cu) ----
+ * Each rating e of a subgraph gets a weight m_e that multiplies the messages of both its directed edges in every layer;
+ * the normalisers count the weights (deg(v) = sum of m over v's in-edges; PyG >= 1.6 layers: |N_r(v)| = sum over v's
+ * in-edges of type r), so that m in {0,1} is the edge_keep mask and m = 1 the model.  grad_e = d score / d m_e at m = 1.
+ * Per directed edge j -> v of type r at layer l the term is (s - mean of s over v's segment) / |segment|, s =
+ * <h_{l-1}[j] W_r, d pre_l[v]>; the segment is v's in-list (its in-edges of type r for PyG >= 1.6).  A single-edge
+ * segment contributes 0 at that layer. */
+
+/* Per directed edge, its terms summed over the layers: edge_grad [edge_ptr[B]], for a batch whose forward (evaluation:
+ * D without edge dropout or edge_keep, else -18) ran on the plan IGMC_PLAN_L2(c) = `cluster` (any other plan: -16).
+ * Operands as igmc_backward's, without gpart / dhid; dpred [B] = d score / d lin2 output (M->multiply_by for IGMC).
+ * With readout = 1, S.dstate is d score / d concat_states (igmc_sortpool_backward seeded with the same dpred).  S.zsave
+ * is not read.  Each element has one writer and a fixed layer order: bit-identical across runs. */
+int igmc_edge_grad(const igmc_model_t* M, const float* params, const uint8_t* node_label, const int32_t* node_ptr,
+                   const int32_t* edge_ptr, const igmc_adj_t* A, int B, int n_cap, const igmc_dropout_t* D,
+                   const igmc_saved_t* S, const float* dpred, float* edge_grad, int cluster, int* err, void* stream);
+
+/* One CTA per graph i of the batch O with tag[i] = q >= 0 (igmc_candidate_pairs over explicit pairs): for every rating
+ * j < E_i/2, out[offsets[q] + j] = edge_grad[e0 + j] + edge_grad[e0 + E_i/2 + j] (e0 = edge_ptr[i]), accumulated over
+ * checkpoints: checkpoint k = 0 stores, k > 0 adds in k order, k = K - 1 divides by K.  At k = 0 also user / item /
+ * rating [T] as igmc_occlusion_mask records them.  A graph whose rating count is not its base-pass count sets
+ * IGMC_ERR_CANDIDATES. */
+int igmc_edge_grad_scatter(const igmc_batch_out_t* O, int B, const int64_t* tag, const float* edge_grad,
+                           const int64_t* offsets, int k, int K, float* out, int32_t* user, int32_t* item,
+                           int32_t* rating, int* err, void* stream);
 
 /* ---- candidate retrieval by bridge count (csrc/retrieve.cu) ----
  * For h = 1 the enclosing subgraph of an unrated pair (u, v) joins u's star and v's star only through the bridge edges
