@@ -30,8 +30,16 @@ U = 2.0 ** -24
 # The prediction bound is below one rounding of u M.  It holds because a prediction is a heavily cancelling sum over
 # 128 hidden units and the lin1 sums behind them, so |pred| is far below M.  A prediction whose |pred| came close to
 # M could exceed 0.5 u M with correct fp32 arithmetic; a reordering of those sums that trips it is not by itself a
-# kernel bug.
-KAPPA = dict(states=64, pred=0.5, dhid=4, grad=32)
+# kernel bug.  The num_bases = 2 cases, on the same H100 and power limit, stay inside these constants: states 7.9 (R = 71
+# on the L2 plan), predictions 0.139 (ml_1m* batch 50, one-launch train kernel: 3.6x below 0.5, kept), d hid 0.98,
+# gradients 4.8.
+# edge (igmc_edge_grad per directed edge, tests/test_gpu_edge_grad_bounds.py): largest 0.24, DGCNN_RS NB 2 k 30 seeded
+# by the kernel's own dstate; IGMC cases 0.0001 to 0.15.  dstate (igmc_sortpool_backward seeded with 1): largest 0.51.
+# Both are far below one u M because M carries the magnitude pass's d pre, which bounds the kernel's own d pre error
+# and is far above |d pre|.  For the same reason a TF32-truncated h moves the edge ratio by only ~1 to 5 (numpy
+# emulation in tests/test_error_bounds_oracle.py): the edge bound catches a lost 1/|segment|, a wrong segment or a
+# missing layer by 500x and more, but not reliably a TF32 slip in h (the EG pass has no tensor-core path today).
+KAPPA = dict(states=64, pred=0.5, dhid=4, grad=32, edge=1, dstate=4)
 
 
 class Graph:
@@ -134,22 +142,43 @@ def _arr_dW(W, arr, mag):
     return 2.0 * arr * D
 
 
-def backward(params, g, saved, aggr, dgcnn, arr, mag=False):
+def _readout_vjp(P, states, g, saved, dgcnn, dpred, keys):
+    """(d concat_states, [d P[k] for k in keys]) of the readout output weighted by ``dpred``, on the kernel's branches"""
+    cs = torch.cat(states, 1).requires_grad_(True)
+    gr = torch.autograd.grad(head(cs, P, g, saved, dgcnn), [cs] + [P[k] for k in keys], dpred)
+    return gr[0], list(gr[1:])
+
+
+def readout_dstate(params, g, saved, dgcnn, mag=False):
+    """d (readout output . dpred) / d concat_states [N, total width]: what igmc_sortpool_backward writes to ``dstate``
+    (DGCNN_RS, seeded with ``dpred``)"""
+    A, P, states = _prep(params, saved, mag)
+    with torch.enable_grad():
+        return _readout_vjp(P, states, g, saved, dgcnn, A(saved["dpred"]), [])[0]
+
+
+def backward(params, g, saved, aggr, dgcnn, arr, mag=False, dpres=None, dstate=None):
     """(d hid [B,128], parameter gradients by state_dict name) of the loss whose lin2-output gradient is the kernel's
-    ``dpred``, plus the ARR term: per-layer vector-Jacobian products from the readout down to layer 0"""
+    ``dpred``, plus the ARR term: per-layer vector-Jacobian products from the readout down to layer 0.  ``dpres``: a
+    list that receives d pre_l of every layer, in layer order.  ``dstate``: d concat_states [N, total width] to start
+    from in place of the readout's VJP (the kernel's ``S.dstate`` of an external readout); the readout's gradients are
+    then left out and d hid is None"""
     A, P0, states = _prep(params, saved, mag)
     P = {k: v.detach().clone().requires_grad_(True) for k, v in P0.items()}
-    dpred = A(saved["dpred"])
     names = conv_names(params)
     L = len(states)
-    cs = torch.cat(states, 1).requires_grad_(True)
     rk = _readout_keys(params)
-    gr = torch.autograd.grad(head(cs, P, g, saved, dgcnn), [cs] + [P[k] for k in rk], dpred)
-    grads = dict(zip(rk, gr[1:]))
-    dh = list(torch.split(gr[0], [h.shape[1] for h in states], 1))
+    if dstate is None:
+        dcs, gr = _readout_vjp(P, states, g, saved, dgcnn, A(saved["dpred"]), rk)
+        grads = dict(zip(rk, gr))
+    else:
+        dcs, grads = A(dstate), {}
+    dh = list(torch.split(dcs, [h.shape[1] for h in states], 1))
     for l in reversed(range(L)):
         h = saved["states"][l]
         dpre = dh[l] * (1.0 - h * h)
+        if dpres is not None:
+            dpres.insert(0, dpre)
         keys = ["convs.%d.%s" % (l, n) for n in names]
         hin = g.x if l == 0 else states[l - 1].clone().requires_grad_(True)
         pre = layer_pre(hin, [P[k] for k in keys], g, aggr)
@@ -163,8 +192,44 @@ def backward(params, g, saved, aggr, dgcnn, arr, mag=False):
             ga, gb = torch.autograd.grad(W, [att, basis], _arr_dW(W.detach(), arr, mag))
             grads[keys[0]] = grads[keys[0]] + ga
             grads[keys[1]] = grads[keys[1]] + gb
-    dhid = dpred.unsqueeze(1) * A(params["lin2.weight"])[0] * saved["gscale"]
+    if dstate is not None:
+        return None, grads
+    dhid = A(saved["dpred"]).unsqueeze(1) * A(params["lin2.weight"])[0] * saved["gscale"]
     return dhid, grads
+
+
+def edge_terms(params, g, saved, aggr, dgcnn, mag=False):
+    """d (sum of the scores) / d w_e at w = 1 of every directed edge e = j -> v of type r [E] (the edge weights of
+    tests/edge_weight_oracle.py): the closed form of ``centred_edge_grad`` from the kernel's own inputs, summed over
+    the layers l of
+
+        (s_e - mean of s over e's segment) / |segment|,     s_e = <h_{l-1}[j] W_r, d pre_l[v]>,
+
+    the segment v's in-edges (mean_all) or v's in-edges of type r (mean_per_relation).  d pre_l comes from
+    ``backward`` seeded with the kernel's ``dpred`` (IGMC: d score / d lin2 output, ``multiply_by``) or, for DGCNN_RS,
+    with its ``dstate`` (``saved["dstate"]``, true widths) at the concat states.  The magnitude pass sums
+    (|s|_e + mean of |s| over the segment) / |segment|, |s| from |h|, |att|, |basis| and the magnitude pass's d pre:
+    an error the kernel carries in its own d pre is covered by M too"""
+    dpres = []
+    backward(params, g, saved, aggr, dgcnn, 0.0, mag, dpres, saved["dstate"] if dgcnn else None)
+    A, P, states = _prep(params, saved, mag)
+    att, basis = conv_names(params)[:2]
+    src, dst = g.edge_index
+    et = g.edge_type
+    R = P["convs.0." + att].shape[0]
+    per_rel = aggr == "mean_per_relation"
+    seg = dst * R + et if per_rel else dst
+    nseg = g.x.shape[0] * (R if per_rel else 1)
+    cnt = torch.zeros(nseg, dtype=torch.float64).index_add_(0, seg, torch.ones(len(seg), dtype=torch.float64))[seg]
+    out = torch.zeros(len(seg), dtype=torch.float64)
+    with torch.no_grad():
+        for l, dp in enumerate(dpres):
+            W = torch.einsum("rb,bio->rio", P["convs.%d.%s" % (l, att)], P["convs.%d.%s" % (l, basis)])
+            h = A(g.x) if l == 0 else states[l - 1]
+            s = (torch.einsum("ni,rio->nro", h, W)[src, et] * dp[dst]).sum(1)
+            mean = torch.zeros(nseg, dtype=torch.float64).index_add_(0, seg, s)[seg] / cnt
+            out += ((s + mean) if mag else (s - mean)) / cnt
+    return out
 
 
 def branch_mismatches(params, g, saved, dgcnn, hidden_keep=None):

@@ -6,6 +6,7 @@ import torch
 import torch.nn.functional as F
 
 from oracle import pyg_restated
+from tests import edge_weight_oracle as ewo
 from tests import error_bounds as eb
 from tests import pyg2_oracle
 from tests.test_gpu_model import _oracle_batch
@@ -41,8 +42,17 @@ def _oracle_saved(ref, ob, ek, hk):
     saved = dict(states=list(torch.split(cs, widths, 1)), out=out.detach(), hidden_keep=hk)
     mult = 1.0 if dg else float(ref.multiply_by)
     saved["dpred"] = 2.0 * (out.detach() - tb["y"].view(-1)) / B * mult
+    pre1 = _readout_branches(ref, ob, tb, cs, saved)
+    saved["gscale"] = (pre1 > 0).double() * hk.double() * 2.0
+    return saved
+
+
+def _readout_branches(ref, ob, tb, cs, saved):
+    """the readout branches the kernels save of the restated model's concat states ``cs`` into ``saved`` (DGCNN_RS:
+    SortPooling order, conv1 and conv2 ReLU outputs); returns the lin1 pre-activation"""
+    B = ob["num_graphs"]
     with torch.no_grad():
-        if dg:
+        if isinstance(ref, pyg_restated.DGCNN_RSRef):
             z = pyg_restated.global_sort_pool(cs, tb["batch"], ref.k, B).unsqueeze(1)
             act1 = F.relu(ref.conv1d_params1(z))
             flat = F.relu(ref.conv1d_params2(ref.maxpool1d(act1))).reshape(B, -1)
@@ -56,9 +66,7 @@ def _oracle_saved(ref, ob, ek, hk):
         else:
             x = tb["x"]
             feat = torch.cat([cs[x[:, 0] == 1], cs[x[:, 1] == 1]], 1)
-        pre1 = ref.lin1(feat)
-        saved["gscale"] = (pre1 > 0).double() * hk.double() * 2.0
-    return saved
+        return ref.lin1(feat)
 
 
 def _case(rgcn, in0, L, dgcnn_last=None, R=5):
@@ -249,3 +257,137 @@ def test_3xtf32_emulation_within_kappa_and_lost_cross_term_beyond():
         bad = _worst(emulate_3xtf32(A, B, K1, drop), A, B)
         print("  without %s: %.0f" % (drop, bad))
         assert bad > eb.KAPPA["states"], drop
+
+
+# ---- edge terms: the per-rating gradient of attribute_pairs (igmc_edge_grad) ---------------------------------------
+def _eval_case(rgcn, in0, L, NB, R, last):
+    """the restated model in eval mode on the oracle batch and what the kernels keep of its eval forward, seeded as
+    the gradient pass of attribute_pairs seeds them: dpred = d score / d lin2 output (multiply_by) for IGMC; for
+    DGCNN_RS dstate, the readout's VJP seeded with 1 at the concat states (true widths)"""
+    ob = _oracle_batch(R=R, h=(in0 - 2) // 2)[3]
+    assert ob["x"].shape[1] == in0
+    ref = _ref(rgcn, in0, L, R=R, NB=NB, dgcnn_last=last).eval()
+    tb = pyg_restated.to_torch_batch(ob, torch.float64)
+    B, dg = ob["num_graphs"], last is not None
+    with torch.no_grad():
+        if dg:
+            _, cs = ref(tb["x"], tb["edge_index"], tb["edge_type"], tb["batch"], num_graphs=B, return_states=True)
+        else:
+            _, cs = ref(tb["x"], tb["edge_index"], tb["edge_type"], return_states=True)
+    saved = dict(states=list(torch.split(cs, [c.out_channels for c in ref.convs], 1)))
+    saved["gscale"] = (_readout_branches(ref, ob, tb, cs, saved) > 0).double()
+    saved["dpred"] = torch.full((B,), 1.0 if dg else float(ref.multiply_by), dtype=torch.float64)
+    params = {k: v.detach().clone() for k, v in ref.state_dict().items()}
+    g = eb.Graph(ob)
+    if dg:
+        saved["dstate"] = eb.readout_dstate(params, g, saved, True)
+    return ref, ob, tb, g, saved, params, ref.convs[0].aggr, dg
+
+
+# (rgcn, in0, L, NB, R, DGCNN_RS last layer width or None)
+EDGE_CASES = [("pyg-1.4", 4, 4, 4, 5, None), ("pyg-1.4", 4, 1, 2, 5, None), ("pyg-1.4", 6, 8, 2, 1, None),
+              ("pyg-1.4", 8, 4, 4, 13, None), ("pyg-2", 4, 4, 2, 5, None), ("pyg-1.4", 6, 1, 4, 13, None),
+              ("pyg-2", 8, 8, 2, 1, None), ("pyg-1.4", 4, 4, 2, 5, 1), ("pyg-2", 4, 4, 4, 13, 1),
+              ("pyg-2", 6, 4, 2, 5, 8)]
+
+
+def _segments(g, aggr, R):
+    """segment id of every directed edge and the segment's size"""
+    dst, et = g.edge_index[1], g.edge_type
+    seg = dst * R + et if aggr == "mean_per_relation" else dst
+    return seg, torch.bincount(seg)[seg]
+
+
+@pytest.mark.parametrize("rgcn,in0,L,NB,R,last", EDGE_CASES)
+def test_edge_terms_equal_weighted_model_autograd(rgcn, in0, L, NB, R, last):
+    """edge_terms from the restated model's own fp64 states and seed equal d (sum of scores) / d w_e of the weighted
+    restatement by autograd (DGCNN_RS in the restatement's own pooling order): 1e-12 relative"""
+    ref, ob, tb, g, saved, params, aggr, dg = _eval_case(rgcn, in0, L, NB, R, last)
+    kw = dict(batch=tb["batch"], num_graphs=ob["num_graphs"], perm=saved["perm"]) if dg else {}
+    want = ewo.autograd_edge_grad(ref, tb["x"], tb["edge_index"], tb["edge_type"], **kw)
+    got = eb.edge_terms(params, g, saved, aggr, dg)
+    assert float(want.abs().max()) > 1e-6
+    _close(got, want)
+
+
+@pytest.mark.parametrize("rgcn,in0,L,NB,R,last", EDGE_CASES)
+def test_edge_magnitude_bounds_and_exact_zeros(rgcn, in0, L, NB, R, last):
+    """M >= |ref| per edge; an edge whose segment has one entry is exactly 0 in fp64 too; with L = 1 every edge into a
+    node other than the two targets has M == 0.  DGCNN_RS: the dstate magnitude bounds its value as well"""
+    _, _, _, g, saved, params, aggr, dg = _eval_case(rgcn, in0, L, NB, R, last)
+    ref, M = eb.edge_terms(params, g, saved, aggr, dg), eb.edge_terms(params, g, saved, aggr, dg, mag=True)
+    assert bool((M >= ref.abs() * (1 - 1e-12)).all()) and float(M.max()) > 0
+    _, size = _segments(g, aggr, R)
+    single = size == 1
+    print("edge terms %s: %d edges, %d in single-entry segments" % ((rgcn, in0, L, NB, R, last), len(M), int(single.sum())))
+    assert int(single.sum()) > 0 and bool((ref[single] == 0).all())
+    if L == 1:
+        target = (g.users | g.items)[g.edge_index[1]]
+        assert bool((M[~target] == 0).all()) and bool((M[target] > 0).any())
+    if dg:
+        ds, mds = eb.readout_dstate(params, g, saved, True), eb.readout_dstate(params, g, saved, True, mag=True)
+        assert bool((mds >= ds.abs()).all()) and float(mds.max()) > 0
+
+
+def emulate_edge_grad(params, g, saved, aggr, dpres, plant=None):
+    """igmc_edge_grad's arithmetic (csrc/rgcn_l2.cu ``edge_terms``) in numpy fp32 from fp32 operands (h, att, basis,
+    each layer's d pre): dZ' = d pre . basis^T rounded (1/deg(v) applied to it under mean_all), p = sum_b att dZ'
+    rounded, the products h * p rounded and summed to t, the segment's sum of t divided once by its size, t - mean
+    (mean_per_relation: times 1/|N_r(v)|), the layers added from the top one down.  ``plant`` is one slip: "inv_seg"
+    drops the 1/|segment|, "segment" takes v's whole in-list as the segment under mean_per_relation, "layer" leaves
+    layer 0's term out, "tf32_h" truncates h to TF32"""
+    f = np.float32
+    att_n, basis_n = eb.conv_names(params)[:2]
+    R = params["convs.0." + att_n].shape[0]
+    per_rel = aggr == "mean_per_relation" and plant != "segment"
+    seg, size = _segments(g, "mean_per_relation" if per_rel else "mean_all", R)
+    seg, size = seg.numpy(), size.numpy().astype(f)
+    src, dst, et = g.edge_index[0].numpy(), g.edge_index[1].numpy(), g.edge_type.numpy()
+    N = g.x.shape[0]
+    one = plant == "inv_seg"
+    invdeg = np.ones(N, f) if one else f(1) / np.maximum(np.bincount(dst, minlength=N), 1).astype(f)
+    inv = np.ones(len(seg), f) if one else f(1) / size
+    out = np.zeros(len(seg), f)
+    for l in reversed(range(len(dpres))):
+        if plant == "layer" and l == 0:
+            continue
+        h = (g.x if l == 0 else saved["states"][l - 1]).numpy().astype(f)
+        if plant == "tf32_h":
+            h = _tf32(h)
+        att = params["convs.%d.%s" % (l, att_n)].numpy().astype(f)
+        basis = params["convs.%d.%s" % (l, basis_n)].numpy().astype(f)[:, :h.shape[1]]
+        dz = np.einsum("vk,bik->vbi", dpres[l].numpy().astype(f).astype(np.float64), basis.astype(np.float64)).astype(f)
+        if not per_rel:
+            dz = dz * invdeg[:, None, None]
+        p = np.einsum("rb,vbi->vri", att.astype(np.float64), dz.astype(np.float64)).astype(f)
+        t = (h[src] * p[dst, et]).sum(1, dtype=f)
+        tot = np.zeros(seg.max() + 1 if len(seg) else 0, f)
+        np.add.at(tot, seg, t)
+        d = t - tot[seg] / size
+        out = out + (d * inv if per_rel else d)
+    return out
+
+
+@pytest.mark.parametrize("rgcn", ["pyg-1.4", "pyg-2"])
+def test_edge_emulation_within_kappa_and_planted_slips_beyond(rgcn):
+    """the fp32 emulation of igmc_edge_grad on fp32 operands stays within KAPPA["edge"] u M of edge_terms on the same
+    operands; a dropped 1/|segment|, the pyg-1.4 segment under pyg-2 and a layer's term left out each exceed it by far.
+    TF32-truncated h is 100s of times the emulation's own ratio but only a few KAPPA["edge"]: M carries the magnitude
+    pass's d pre (the bound on the kernel's own d pre error), far above |d pre|, so it cannot single out a 2^-11 error
+    in h"""
+    _, _, _, g, saved, params, aggr, _ = _eval_case(rgcn, 4, 4, 4, 5, None)
+    params = {k: v.float().double() for k, v in params.items()}
+    saved = dict(saved, states=[h.float().double() for h in saved["states"]])
+    dpres = []
+    eb.backward(params, g, saved, aggr, False, 0.0, dpres=dpres)
+    ref, M = eb.edge_terms(params, g, saved, aggr, False), eb.edge_terms(params, g, saved, aggr, False, mag=True)
+    ok, pad, _ = eb.ratio(torch.from_numpy(emulate_edge_grad(params, g, saved, aggr, dpres)), ref, M)
+    print("edge emulation %s: largest err / (u M) = %.3g (KAPPA edge %g)" % (rgcn, ok, eb.KAPPA["edge"]))
+    assert ok <= eb.KAPPA["edge"] and pad == 0
+    for plant in ("inv_seg", "layer", "tf32_h") + (("segment",) if rgcn == "pyg-2" else ()):
+        bad = eb.ratio(torch.from_numpy(emulate_edge_grad(params, g, saved, aggr, dpres, plant)), ref, M)[0]
+        print("  with %s: %.3g" % (plant, bad))
+        if plant == "tf32_h":
+            assert bad > 100 * ok, plant
+        else:
+            assert bad > 100 * eb.KAPPA["edge"], plant

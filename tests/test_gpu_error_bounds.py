@@ -30,9 +30,9 @@ def _igmc(in0, R, NB=4, plan="auto", adj_dropout=0.2, rgcn="pyg-1.4"):
     return _models(in0, R, NB=NB, adj_dropout=adj_dropout, plan=plan, rgcn=rgcn)[1]
 
 
-def _dgcnn(k, last, plan):
+def _dgcnn(k, last, plan, NB=4):
     from tests.test_gpu_dgcnn import _models
-    return _models(5, 4, k, adj_dropout=0.2, plan=plan, last=last)[1]
+    return _models(5, NB, k, adj_dropout=0.2, plan=plan, last=last)[1]
 
 
 def _small(R=5, h=1):
@@ -104,12 +104,20 @@ CASES = {
     **{"dgcnn_k%d_last%d" % (k, last): (lambda k=k, last=last: _dgcnn(k, last, 2), _small, 2)
        for k in (30, 80) for last in (1, 8)},
     **{"scaled4_plan%d" % p: (lambda p=p: _scaled(_igmc(4, 5, plan=p)), _small, p) for p in (2, 0)},
+    # num_bases = 2, the default of the reference's IGMC and DGCNN_RS: the NB = 2 instantiation of every model kernel
+    **{"nb2_oracle_batch_plan%d" % p: (lambda p=p: _igmc(4, 5, NB=2, plan=p), _small, p) for p in (0, 1, 2, 4)},
+    "nb2_ml_1m_full_plan2_one_launch": (lambda: _igmc(4, 5, NB=2, plan=2), _ml_1m_full, 2),
+    **{"nb2_R71_l2_c%d" % c: (lambda c=c: _igmc(4, 71, NB=2, plan=_lib.plan_l2(c)), _many_relations, _lib.plan_l2(c))
+       for c in (1, 8)},
+    **{"nb2_pyg2_plan%d" % p: (lambda p=p: _igmc(4, 5, NB=2, plan=p, rgcn="pyg-2"), _small, p)
+       for p in (0, 2, _lib.plan_l2(2))},
+    **{"nb2_dgcnn_k30_last1_plan%d" % p: (lambda p=p: _dgcnn(30, 1, p, NB=2), _small, p) for p in (2, _lib.plan_l2(2))},
 }
 # the regime a case is there for, asserted on its model and batch before the checks
 REGIME = {"ml_100k_mnph200_plan4": _chunked_staging}
 # cases whose train step runs the way the train engine runs it on cluster plans: forward, loss and backward in one
 # launch (igmc_forward_backward), then the gradient assembly (igmc_grad_reduce)
-ONE_LAUNCH = {"ml_1m_full_plan2_one_launch"}
+ONE_LAUNCH = {"ml_1m_full_plan2_one_launch", "nb2_ml_1m_full_plan2_one_launch"}
 
 
 def _ws(m, train):
