@@ -169,6 +169,7 @@ _SIGS = {
     "igmc_reduce_update": [C.POINTER(Model), vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, C.c_float, C.c_float,
                            C.POINTER(Comm), vp, vp, vp, C.c_float, vp, C.c_float, C.c_float, C.c_float, C.c_float,
                            C.c_float, vp, vp, C.c_float, vp, vp, vp, C.c_int, vp, vp],
+    "igmc_reduce_update_grid": [C.POINTER(Model), C.POINTER(C.c_int), C.POINTER(C.c_int)],
     "igmc_comm_alloc": [C.c_int64, C.POINTER(C.c_void_p), C.c_char_p],
     "igmc_comm_open": [C.c_char_p, C.POINTER(C.c_void_p)],
     "igmc_comm_close": [vp],

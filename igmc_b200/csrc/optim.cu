@@ -445,7 +445,8 @@ __device__ __forceinline__ float ld_relaxed_sys(const float* p) {
 // Two parities are enough: a rank overwrites parity p in step t + 2 only after it has seen every peer's flag t + 1,
 // which a peer raises after its step-t kernel (and thus its reads of parity p) has finished.
 // Spinning inside the grid is safe only while every block is resident at once: igmc_reduce_update refuses a grid larger
-// than the device holds (two blocks per SM: 264 on an H100; the 4-layer IGMC needs 230).
+// than the device holds (two blocks per SM: 264 on an H100; the 4-layer IGMC needs 230, 5 to 8 layers need 294 to 486
+// and train through the separate kernels instead: igmc_reduce_update_grid tells the caller beforehand).
 __global__ void __launch_bounds__(256, 2)   // <= 128 registers: two blocks per SM
 k_reduce_allreduce_adam(igmc_model_t M, float* __restrict__ params, int B, int rows, int NA,
                         const float* __restrict__ gpart, const float* __restrict__ dhid, const float* __restrict__ feat,
@@ -623,7 +624,35 @@ __global__ void k_adam(float* __restrict__ params, const float* __restrict__ gra
   }
 }
 
+// grid of k_reduce_allreduce_adam: one block per layer input row of the gradient assembly plus the blocks of the
+// readout parameters
+int reduce_update_rows(const igmc_model_t* M) { return M->in_dim0 + (M->num_layers - 1) * HID; }
+int reduce_update_blocks(const igmc_model_t* M) {
+  return reduce_update_rows(M) + (M->param_count - M->conv_param_count + 255) / 256;
+}
+
+// blocks of k_reduce_allreduce_adam the current device runs at once (queried once per process)
+int reduce_update_resident(int* resident) {
+  static int cached = 0;
+  if (!cached) {
+    int dev = 0, sms = 0, per_sm = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_reduce_allreduce_adam, 256, 0);
+    if (e != cudaSuccess) return (int)e + 1000;
+    cached = sms * per_sm;
+  }
+  *resident = cached;
+  return 0;
+}
+
 }  // namespace
+
+extern "C" int igmc_reduce_update_grid(const igmc_model_t* M, int* blocks, int* resident) {
+  if (!M || !blocks) return -20;
+  *blocks = reduce_update_blocks(M);
+  return resident ? reduce_update_resident(resident) : 0;
+}
 
 extern "C" int igmc_grad_reduce(const igmc_model_t* M, const float* params, int B, int gpart_rows, const float* gpart,
                                 int raw_rows, const float* dhid, const float* feat, const float* hid,
@@ -683,20 +712,13 @@ extern "C" int igmc_reduce_update(const igmc_model_t* M, float* params, int B, i
     if (!comm->grad[r] || !comm->flag[r]) return -20;
   if (M->num_relations > 12) return -16;
   if (M->readout != 0) return -16;   // external readouts write their own gradient slice: use the separate kernels
-  const int NA = M->in_dim0 + (M->num_layers - 1) * HID;
-  const int PBr = (M->param_count - M->conv_param_count + 255) / 256;
-  static int resident = 0;   // blocks of k_reduce_allreduce_adam the device runs at once
-  if (!resident) {
-    int dev = 0, sms = 0, per_sm = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_reduce_allreduce_adam, 256, 0);
-    if (e != cudaSuccess) return (int)e + 1000;
-    resident = sms * per_sm;
-  }
-  if (NA + PBr > resident) return -21;   // the grid barrier would wait for blocks that cannot be scheduled
+  const int NA = reduce_update_rows(M), blocks = reduce_update_blocks(M);
+  int resident = 0;
+  const int rc = reduce_update_resident(&resident);
+  if (rc) return rc;
+  if (blocks > resident) return -21;   // the grid barrier would wait for blocks that cannot be scheduled
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(NA + PBr);
+  cfg.gridDim = dim3(blocks);
   cfg.blockDim = dim3(256);
   cfg.stream = (cudaStream_t)stream;
   cudaLaunchAttribute at[1];

@@ -311,6 +311,7 @@ class IGMC(nn.Module):
         self._ws = {}
         self._plans = {}
         self._wprep = None
+        self._update_grid_fits = None
 
     def alias_grads(self):
         """point every ``p.grad`` at its slice of ``flat_grad`` (for stock torch optimizers)."""
@@ -616,8 +617,17 @@ class IGMC(nn.Module):
 
     def fused_update_ok(self, batch):
         """the one-kernel reduce -> all-reduce -> Adam path needs raw partial rows (cluster plans) and the IGMC
-        readout (an external readout writes its own gradient slice)."""
-        return self._cmodel.readout == 0 and _lib.is_rs(self._plan(batch))
+        readout (an external readout writes its own gradient slice), and a grid the device runs at once: the kernel's
+        grid barriers wait for every block (one per layer input row, so more than 4 layers do not fit on an H100)."""
+        if self._cmodel.readout != 0 or not _lib.is_rs(self._plan(batch)):
+            return False
+        fits = self.__dict__.get("_update_grid_fits")
+        if fits is None:
+            blocks, resident = C.c_int(), C.c_int()
+            _lib.check(_lib.load().igmc_reduce_update_grid(C.byref(self._cmodel), C.byref(blocks), C.byref(resident)),
+                       "igmc_reduce_update_grid")
+            fits = self._update_grid_fits = blocks.value <= resident.value
+        return fits
 
     def fused_step(self, batch, ARR=0.0, global_num_graphs=None, edge_keep=None, hidden_keep=None,
                    seed_dev=None):

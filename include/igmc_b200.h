@@ -357,6 +357,11 @@ int igmc_reduce_update(const igmc_model_t* M, float* params, int B, int gpart_ro
                        float* loss_out, float* loss_acc, float loss_weight, float* reg_ws, float* grad_copy,
                        float* loss_ring, int ring_size, float* wprep, void* stream);
 
+/* The grid igmc_reduce_update launches for model M: `blocks` (computed without a device) and, when `resident` is not
+ * NULL, the blocks of that kernel the current device runs at once.  igmc_reduce_update returns -21 when
+ * blocks > resident; callers then take igmc_grad_reduce -> all-reduce -> igmc_adam_step instead. */
+int igmc_reduce_update_grid(const igmc_model_t* M, int* blocks, int* resident);
+
 /* ---- SortPooling + 1-D convolution readout of DGCNN_RS (models.py:123-167 over DGCNN.__init__ models.py:65-85) ----
  * Consumes the concat_states a readout=1 igmc_forward produced.  latent_dim = [32,...,32,1] is run by the conv
  * kernels as 32-wide layers whose unused output columns have zero weights, so a states row has `state_stride` =

@@ -39,7 +39,16 @@ U = 2.0 ** -24
 # and is far above |d pre|.  For the same reason a TF32-truncated h moves the edge ratio by only ~1 to 5 (numpy
 # emulation in tests/test_error_bounds_oracle.py): the edge bound catches a lost 1/|segment|, a wrong segment or a
 # missing layer by 500x and more, but not reliably a TF32 slip in h (the EG pass has no tensor-core path today).
-KAPPA = dict(states=64, pred=0.5, dhid=4, grad=32, edge=1, dstate=4)
+# The regime cases (tests/test_gpu_regime_bounds.py: relation counts 1..11, 1 to 8 layers on every plan family,
+# degenerate batches, staging limits, readout variants) and the train engine's steps (tests/test_gpu_engine_bounds.py),
+# same H100 and power limit, stay inside these constants: states 9.1 (L 5, plan 0), predictions 0.41 (the engine's
+# third step after a resume at step 5000), d hid 0.99, gradients 11.0 (one 202-node pair on plan 4).
+# adam (k_adam and the fused update, per element of m, v and p; M in adam_terms): largest 3.3 (v, first step after
+# the resume), m 1.9, p 1.7; numpy fp32 emulation 1.9.  An off-by-one step in the bias corrections (steps 1 to 3), weight
+# decay left out or eps inside the square root is off by 2 000 to 16 000 000 u M.
+# wprep (prepared W_r / W_r^T slabs after a fused update; M = sum_b |att| |basis|): largest 2.8, emulation 1.9; a
+# TF32-rounded basis is off by ~10 000, a dropped basis by ~10^7.  Root columns are copies (exact) and padding is 0.
+KAPPA = dict(states=64, pred=0.5, dhid=4, grad=32, edge=1, dstate=4, adam=16, wprep=16)
 
 
 class Graph:
@@ -310,11 +319,15 @@ def _pad32(t, w):
     return F.pad(t, (0, w - t.shape[1]))
 
 
-def check_device(m, ob, ws, train, edge_keep=None, arr=0.0, hidden_keep=None):
+def check_device(m, ob, ws, train, edge_keep=None, arr=0.0, hidden_keep=None, params=None):
     """every quantity of the last forward (eval) or train step of ``m`` on the oracle batch ``ob`` against its fp64
     recomputation; returns {quantity: (largest err / (u M), elements that must be zero but are not, worst index)} and
-    under "branches" the count of ``branch_mismatches`` (``edge_keep`` / ``hidden_keep``: the step's dropout draws)"""
-    params = {k: v.detach().double().cpu().contiguous() for k, v in m.state_dict().items()}
+    under "branches" the count of ``branch_mismatches`` (``edge_keep`` / ``hidden_keep``: the step's dropout draws).
+    ``params``: the state_dict the step ran with (default ``m``'s current one; pass a snapshot when an optimizer
+    update has changed the parameters since)"""
+    if params is None:
+        params = m.state_dict()
+    params = {k: v.detach().double().cpu().contiguous() for k, v in params.items()}
     dgcnn = "sp" in ws
     aggr = "mean_per_relation" if m.rgcn == "pyg-2" else "mean_all"
     N = ob["x"].shape[0]
@@ -350,14 +363,109 @@ def check_device(m, ob, ws, train, edge_keep=None, arr=0.0, hidden_keep=None):
     return res
 
 
+def kappa_of(key):
+    """the KAPPA entry that bounds result ``key`` (states0..7 -> states, adam_m / adam_v / adam_p -> adam,
+    wprep_root -> wprep)"""
+    return KAPPA[next((k for k in ("states", "adam", "wprep") if key.startswith(k)), key)]
+
+
 def violations(res):
     """the entries of a ``check_device`` result that fail: a ratio not within its KAPPA (NaN included), an element that
     must be zero and is not, or a branch mismatch"""
-    bad = [("branches", res["branches"])] if res["branches"] else []
+    bad = [("branches", res.get("branches", 0))] if res.get("branches", 0) else []
     for key, val in res.items():
         if key == "branches":
             continue
         r, pad, worst = val
-        if not r <= KAPPA["states" if key.startswith("states") else key] or pad:
+        if not r <= kappa_of(key) or pad:
             bad.append((key, r, pad, worst))
     return bad
+
+
+# ---- optimizer and prepared weights ---------------------------------------------------------------------------------
+def f32(x):
+    """a hyperparameter as the kernels receive it (a float argument), in fp64"""
+    return float(torch.tensor(float(x), dtype=torch.float32))
+
+
+def adam_terms(p, m, v, g, step, lr, b1, b2, eps, wd, grad_mul=1.0):
+    """one torch-Adam update (k_adam and phase 3 of k_reduce_allreduce_adam: eps outside the square root, L2 weight
+    decay added to the gradient) in fp64 from the state before the step (``p``, ``m``, ``v``), the gradient it applied
+    (``g``, before ``grad_mul``) and the step number it ran as (``step``, counted from 1), with the bias corrections
+    1 - beta^step in fp64.  Hyperparameters are taken at fp32, as the kernel receives them.
+
+    Returns {"adam_m" | "adam_v" | "adam_p": (reference, M)}.  M sums the magnitudes of the terms: for the moments
+    b1 |m| + (1 - b1) |g'| and b2 v + (1 - b2) |g'|^2 with |g'| = |g grad_mul| + |wd p|; for the parameter |p| + |dp|
+    plus the first-order effect of the moments' own bounds on dp = lr/bc1 * m / (sqrt(v / bc2) + eps):
+    lr/bc1 * M_m / den + |dp| M_v / (2 v)."""
+    p, m, v, g = [t.double() for t in (p, m, v, g)]
+    lr, b1, b2, eps, wd, grad_mul = [f32(x) for x in (lr, b1, b2, eps, wd, grad_mul)]
+    gg = g * grad_mul + wd * p
+    Mg = (g * grad_mul).abs() + abs(wd) * p.abs()
+    m1 = b1 * m + (1 - b1) * gg
+    v1 = b2 * v + (1 - b2) * gg * gg
+    Mm = b1 * m.abs() + (1 - b1) * Mg
+    Mv = b2 * v.abs() + (1 - b2) * Mg * Mg
+    bc1, bc2 = 1.0 - b1 ** step, 1.0 - b2 ** step
+    den = torch.sqrt(v1) / bc2 ** 0.5 + eps
+    dp = (lr / bc1) * m1 / den
+    Mp = p.abs() + dp.abs() + (lr / bc1) * Mm / den + dp.abs() * torch.where(v1 > 0, Mv / (2 * v1.clamp(min=1e-300)),
+                                                                             torch.zeros_like(v1))
+    return {"adam_m": (m1, Mm), "adam_v": (v1, Mv), "adam_p": (p - dp, Mp)}
+
+
+def adam_check(got, terms):
+    """{key: ratio(...)} of the device's updated (exp_avg, exp_avg_sq, params) against ``adam_terms``"""
+    return {key: ratio(g, *terms[key]) for key, g in zip(("adam_m", "adam_v", "adam_p"), got)}
+
+
+def wprep_terms(params, L, R, in0):
+    """the prepared weight slabs (igmc_prep_weights, phase 4 of k_reduce_allreduce_adam) of ``params`` (a state_dict)
+    in fp64: slab (l, dir) holds 32 rows of KS = K1p + a8(inp) + 4 floats, inp = a4(in), K1 = R inp, K1p = a8(K1);
+    dir 0 row n: W_r[q][n] at r inp + q, root[q][n] at K1p + q; dir 1 (layers >= 1) row k: W_r[k][q] at r inp + q,
+    root[k][q] at K1p + q; every other float of a row is 0.  W_r = sum_b att[r,b] basis[b].
+
+    Returns (reference, M, copied, written) as flat tensors over the whole buffer: M = sum_b |att[r,b]| |basis[b]|,
+    ``copied`` marks the root entries (copied, so exact), ``written`` every float some row covers (slab (0, 1) and
+    the tail of the layer-0 slabs are not written)."""
+    a4 = lambda x: (x + 3) & ~3      # noqa: E731
+    a8 = lambda x: (x + 7) & ~7      # noqa: E731
+    att_n, basis_n = conv_names(params)[:2]
+    slab = 32 * ((R + 1) * 32 + 4)
+    ref = torch.zeros(L * 2 * slab, dtype=torch.float64)
+    M, copied, written = torch.zeros_like(ref), torch.zeros_like(ref, dtype=torch.bool), torch.zeros_like(ref, dtype=torch.bool)
+    for l in range(L):
+        at = params["convs.%d.%s" % (l, att_n)].double()
+        bs = params["convs.%d.%s" % (l, basis_n)].double()
+        rt = params["convs.%d.root" % l].double()
+        bs, rt = F.pad(bs, (0, 32 - bs.shape[2])), F.pad(rt, (0, 32 - rt.shape[1]))    # a narrow last layer
+        fin = bs.shape[1]
+        inp = a4(fin)
+        K1p = a8(R * inp)
+        KS = K1p + a8(inp) + 4
+        W = torch.einsum("rb,bio->rio", at, bs)                 # [R, in, 32]
+        MW = torch.einsum("rb,bio->rio", at.abs(), bs.abs())
+        for d in (0, 1) if l else (0,):
+            rows = torch.zeros(32, KS, dtype=torch.float64)
+            mrows, crows = torch.zeros_like(rows), torch.zeros_like(rows, dtype=torch.bool)
+            # [32 rows, R, in]: dir 0 row n, column (r, q) = W_r[q][n]; dir 1 row k, column (r, q) = W_r[k][q]
+            order = (2, 0, 1) if d == 0 else (1, 0, 2)
+            rows[:, :R * inp].view(32, R, inp)[:, :, :fin] = W.permute(*order)
+            mrows[:, :R * inp].view(32, R, inp)[:, :, :fin] = MW.permute(*order)
+            rows[:, K1p:K1p + fin] = rt.t() if d == 0 else rt
+            crows[:, K1p:K1p + fin] = True
+            o = (l * 2 + d) * slab
+            ref[o:o + 32 * KS] = rows.reshape(-1)
+            M[o:o + 32 * KS] = mrows.reshape(-1)
+            copied[o:o + 32 * KS] = crows.reshape(-1)
+            written[o:o + 32 * KS] = True
+    return ref, M, copied, written
+
+
+def wprep_check(got, terms):
+    """{"wprep": ratio of the W_r entries and padding, "wprep_root": (0, root entries not copied exactly, -1)}"""
+    ref, M, copied, written = terms
+    got = got.reshape(-1).double().cpu()
+    sel = written & ~copied
+    miss = int((got[copied] != ref[copied]).sum())
+    return {"wprep": ratio(got[sel], ref[sel], M[sel]), "wprep_root": (0.0, miss, -1)}

@@ -46,6 +46,21 @@ def test_build_info_and_plans():
     assert lib.igmc_model_plan(ctypes.byref(m30._cmodel), 100, 0, 0) > 0   # generic plan takes it
 
 
+def test_reduce_update_grid_blocks():
+    """the grid of the fused reduce -> all-reduce -> Adam kernel, one block per layer input row plus the readout
+    parameters, for in0 = 4 (R and NB do not enter), without a device.  Two blocks per SM hold 264 on a 132-SM H100:
+    from 5 layers on the engine takes the separate kernels"""
+    from igmc_b200.models import IGMC
+    want = {1: 38, 2: 102, 3: 166, 4: 230, 5: 294, 6: 358, 7: 422, 8: 486}
+    lib = _lib.load()
+    for L, blocks in want.items():
+        for R, NB in ((5, 4), (12, 2)):
+            m = IGMC(4, latent_dim=[32] * L, num_relations=R, num_bases=NB, regression=True)
+            got = ctypes.c_int(-1)
+            assert lib.igmc_reduce_update_grid(ctypes.byref(m._cmodel), ctypes.byref(got), None) == 0
+            assert got.value == blocks, (L, R, NB, got.value)
+
+
 def test_struct_sizes_match_header_layout():
     # pointer-sized fields and 4-byte ints exactly as declared (guards against a silent ABI drift)
     P = ctypes.sizeof(ctypes.c_void_p)

@@ -391,3 +391,124 @@ def test_edge_emulation_within_kappa_and_planted_slips_beyond(rgcn):
             assert bad > 100 * ok, plant
         else:
             assert bad > 100 * eb.KAPPA["edge"], plant
+
+
+# ---- optimizer and prepared weights ---------------------------------------------------------------------------------
+def emulate_adam(p, m, v, g, step, lr, b1, b2, eps, wd, plant=None):
+    """k_adam (csrc/optim.cu) in numpy fp32, one rounding per operation; bias corrections 1 - exp(step log beta) in
+    double, rounded to fp32.  ``plant``: "step" (bias corrections of the step after), "wd" (weight decay left out),
+    "eps_in_sqrt" (sqrt(v / bc2 + eps) in place of sqrt(v) / sqrt(bc2) + eps)"""
+    f = np.float32
+    p, m, v, g = [np.asarray(t, np.float32) for t in (p, m, v, g)]
+    s = step + (1 if plant == "step" else 0)
+    bc1 = f(1.0 - np.exp(s * np.log(np.float64(f(b1)))))
+    bc2 = f(1.0 - np.exp(s * np.log(np.float64(f(b2)))))
+    gg = g
+    if wd and plant != "wd":
+        gg = f(np.float64(f(wd)) * p + gg)        # fmaf: the fp32 product is exact in fp64
+    mi = f(b1) * m + (f(1) - f(b1)) * gg
+    vi = f(b2) * v + (f(1) - f(b2)) * gg * gg
+    den = np.sqrt(vi / bc2 + f(eps)) if plant == "eps_in_sqrt" else np.sqrt(vi) / np.sqrt(bc2) + f(eps)
+    return mi, vi, p - (f(lr) / bc1) * (mi / den)
+
+
+def _adam_state(fresh, n=4096, seed=3):
+    """parameters ~ 0.1, gradients ~ 1e-3 (a few exact zeros: padding slots), moments of a resumed run or zero"""
+    rng = np.random.default_rng(seed)
+    p = (rng.standard_normal(n) * 0.1).astype(np.float32)
+    g = (rng.standard_normal(n) * 1e-3).astype(np.float32)
+    p[:8], g[:8] = 0, 0
+    if fresh:
+        m = v = np.zeros(n, np.float32)
+    else:
+        m = (rng.standard_normal(n) * 1e-3).astype(np.float32)
+        v = ((1.5 * m) ** 2 + 1e-8).astype(np.float32)
+        m[:8], v[:8] = 0, 0
+    return p, m, v, g
+
+
+ADAM_CASES = {   # name -> (fresh state, step, weight decay, lr)
+    "step1": (True, 1, 0.0, 1e-3), "step2": (False, 2, 0.0, 1e-3), "step3_wd": (False, 3, 1e-2, 1e-3),
+    "step5000_wd": (False, 5000, 1e-2, 2e-4),
+}
+
+
+@pytest.mark.parametrize("case", sorted(ADAM_CASES))
+def test_adam_emulation_within_kappa(case):
+    fresh, step, wd, lr = ADAM_CASES[case]
+    p, m, v, g = _adam_state(fresh)
+    terms = eb.adam_terms(*[torch.from_numpy(t) for t in (p, m, v, g)], step, lr, 0.9, 0.999, 1e-8, wd)
+    res = eb.adam_check([torch.from_numpy(t) for t in emulate_adam(p, m, v, g, step, lr, 0.9, 0.999, 1e-8, wd)], terms)
+    print("adam emulation %s: %s" % (case, {k: round(r[0], 3) for k, r in res.items()}))
+    assert not eb.violations(res), res
+
+
+@pytest.mark.parametrize("plant,case", [("step", "step1"), ("step", "step2"), ("step", "step3_wd"),
+                                        ("wd", "step3_wd"), ("wd", "step5000_wd"),
+                                        ("eps_in_sqrt", "step2"), ("eps_in_sqrt", "step5000_wd")])
+def test_adam_planted_slips_beyond_kappa(plant, case):
+    """an off-by-one step in the bias corrections (steps 1 to 3: at step 5000 both are ~1 and the slip is below one
+    rounding of |p|), weight decay left out, eps inside the square root: each moves the parameter by far more than
+    KAPPA["adam"] u M.  The margins on these states are printed; the assertion asks for 100x"""
+    fresh, step, wd, lr = ADAM_CASES[case]
+    p, m, v, g = _adam_state(fresh)
+    terms = eb.adam_terms(*[torch.from_numpy(t) for t in (p, m, v, g)], step, lr, 0.9, 0.999, 1e-8, wd)
+    got = emulate_adam(p, m, v, g, step, lr, 0.9, 0.999, 1e-8, wd, plant)
+    res = eb.adam_check([torch.from_numpy(t) for t in got], terms)
+    worst = max(r[0] for r in res.values())
+    print("adam %s at %s: largest err / (u M) %.3g = %.0f x KAPPA" % (plant, case, worst, worst / eb.KAPPA["adam"]))
+    assert worst > 100 * eb.KAPPA["adam"]
+
+
+def emulate_wprep(params, L, R, in0, plant=None):
+    """igmc_prep_weights in fp32: W_r[k][j] = fma chain over the bases; ``plant`` "basis_tf32" rounds the basis
+    operand to TF32 (10 mantissa bits), "drop_basis" leaves the last basis out"""
+    ref, M, copied, written = eb.wprep_terms(params, L, R, in0)
+    out = torch.zeros_like(ref, dtype=torch.float32)
+    att_n, basis_n = eb.conv_names(params)[:2]
+    slab = 32 * ((R + 1) * 32 + 4)
+    for l in range(L):
+        at = params["convs.%d.%s" % (l, att_n)].float()
+        bs = params["convs.%d.%s" % (l, basis_n)].float()
+        if plant == "basis_tf32":
+            bs = (bs.view(torch.int32) & ~0x1FFF).view(torch.float32)
+        NB = at.shape[1] - (1 if plant == "drop_basis" else 0)
+        W = torch.zeros(R, bs.shape[1], 32, dtype=torch.float32)
+        for b in range(NB):       # w = fmaf(att, basis, w): product exact in fp64, one rounding per term
+            W = (at[:, b, None, None].double() * bs[b].double() + W.double()).float()
+        rt = params["convs.%d.root" % l].float()
+        fin = bs.shape[1]
+        inp = (fin + 3) & ~3
+        K1p = (R * inp + 7) & ~7
+        KS = K1p + ((inp + 7) & ~7) + 4
+        for d in (0, 1) if l else (0,):
+            rows = torch.zeros(32, KS)
+            rows[:, :R * inp].view(32, R, inp)[:, :, :fin] = W.permute(2, 0, 1) if d == 0 else W.permute(1, 0, 2)
+            rows[:, K1p:K1p + fin] = rt.t() if d == 0 else rt
+            o = (l * 2 + d) * slab
+            out[o:o + 32 * KS] = rows.reshape(-1)
+    return out, (ref, M, copied, written)
+
+
+@pytest.mark.parametrize("L,R,NB,rgcn", [(1, 5, 4, "pyg-1.4"), (4, 8, 2, "pyg-1.4"), (2, 5, 4, "pyg-2")])
+def test_wprep_emulation_within_kappa_and_planted_slips_beyond(L, R, NB, rgcn):
+    from igmc_b200.models import IGMC
+    torch.manual_seed(0)
+    m = IGMC(4, latent_dim=[32] * L, num_relations=R, num_bases=NB, regression=True, rgcn=rgcn)
+    params = {k: v.detach().clone() for k, v in m.state_dict().items()}
+    out, terms = emulate_wprep(params, L, R, 4)
+    res = eb.wprep_check(out, terms)
+    print("wprep emulation L%d R%d NB%d %s: %.3g" % (L, R, NB, rgcn, res["wprep"][0]))
+    assert not eb.violations(res), res
+    for plant in ("basis_tf32", "drop_basis"):
+        bad = eb.wprep_check(emulate_wprep(params, L, R, 4, plant)[0], terms)["wprep"][0]
+        print("  with %s: %.3g = %.0f x KAPPA" % (plant, bad, bad / eb.KAPPA["wprep"]))
+        assert bad > 100 * eb.KAPPA["wprep"], plant
+    # a root column off by one row, and a stray value in the padding, are each found exactly
+    _, M, copied, written = terms
+    for where in (copied, written & (M == 0) & ~copied):
+        o = out.clone()
+        i = int(torch.nonzero(where)[len(torch.nonzero(where)) // 2])
+        o[i] += 1e-3
+        r = eb.wprep_check(o, terms)
+        assert r["wprep_root"][1] + r["wprep"][1] == 1

@@ -125,12 +125,13 @@ def _ws(m, train):
 
 
 def _report(case, mode, res):
-    print("error bounds %-28s %-5s branches mismatched %d" % (case, mode, res["branches"]))
+    if "branches" in res:
+        print("error bounds %-28s %-5s branches mismatched %d" % (case, mode, res["branches"]))
     for key, val in res.items():
         if key != "branches":
             r, pad, worst = val
             print("error bounds %-28s %-5s %-8s err/(uM) %9.3f  kappa %4g  nonzero-at-M=0 %d  worst %d"
-                  % (case, mode, key, r, eb.KAPPA["states" if key.startswith("states") else key], pad, worst))
+                  % (case, mode, key, r, eb.kappa_of(key), pad, worst))
     return eb.violations(res)
 
 
