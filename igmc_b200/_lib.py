@@ -191,6 +191,15 @@ _SIGS = {
     "igmc_edge_grad": [C.POINTER(Model), vp, vp, vp, vp, C.POINTER(Adj), C.c_int, C.c_int, C.POINTER(Dropout),
                        C.POINTER(Saved), vp, vp, C.c_int, vp, vp],
     "igmc_edge_grad_scatter": [C.POINTER(BatchOut), C.c_int, vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp],
+    "igmc_pair_factor_count": [C.POINTER(Model)],
+    "igmc_pair_seed": [vp, vp, vp, C.c_int, C.c_float, vp, vp],
+    "igmc_pair_grad": [C.POINTER(Model), vp, C.c_int, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, C.c_int, vp, C.c_int,
+                       vp, vp],
+    "igmc_self_influence": [C.POINTER(Model), C.c_int, vp, vp, vp, C.c_float, vp, vp],
+    "igmc_influence_ws_bytes": [C.POINTER(Model), C.c_int, C.c_int, C.POINTER(C.c_int64)],
+    "igmc_influence_accum": [C.POINTER(Model), C.c_int, C.c_int, vp, vp, vp, vp, C.c_float, C.c_int, vp, C.c_int64,
+                             vp, vp],
+    "igmc_influence_topk": [vp, C.c_int, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp],
     "igmc_corated_ws_bytes":[C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int64)],
     "igmc_corated_items": [C.POINTER(CSR), vp, C.c_int, C.c_int, C.c_int, vp, C.c_int64, vp, vp, vp, vp],
     "igmc_graph_update_ws_bytes": [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int64)],

@@ -17,6 +17,11 @@ building a dataset of every candidate pair and looping over it in Python.  Here:
 * ``attribute_pairs(model, graph, users, items, m)`` -> the same layout with, per rating, the score's gradient with
   respect to a weight on that rating (igmc_edge_grad): the same base pass, then one gradient pass over the P pairs, each
   an L2-plan eval forward and one backward whose list walk writes every edge's term;
+* ``pair_gradients(model, graph, users, items, y)`` -> per-example gradients [K, P, param_count] of each pair's squared
+  error (or score), ``influence(model, graph, train, test, k)`` -> per test pair the k training pairs of largest and
+  smallest TracIn-CP influence, ``self_influence(model, graph, train)`` -> sum_k eta_k ||grad l_i||^2
+  (csrc/influence.cu): a per-graph gradient assembly after the training backward, a split-K GEMM of the conv blocks
+  plus the readout's rank-1 factors, and a streaming top-k merge;
 * ``InferenceEngine``: the pipelined, graph-replayed loop behind all of them.  Per step the side stream produces the next
   batch's candidate pairs (``igmc_candidate_pairs``, from a device cursor) and extracts it while the main stream runs
   the eval forward of the current batch (once per checkpoint) and merges its scores into the running per-user top-k
@@ -39,7 +44,7 @@ from .train_eval import replay_step
 from .util_functions import RatingGraph, SubgraphExtractor, _stream_ptr
 
 __all__ = ["predict_pairs", "recommend", "corated_items", "explain_pairs", "Explanation", "attribute_pairs",
-           "Attribution", "InferenceEngine"]
+           "Attribution", "pair_gradients", "influence", "self_influence", "Influence", "InferenceEngine"]
 
 
 # ---- input validation (host) ----------------------------------------------------------------------------------------
@@ -118,6 +123,71 @@ def _check_k(k):
     return k
 
 
+INFLUENCE_T_MAX = 1024   # test pairs of one influence run: the test-side store is K * T * (conv block + factors) floats
+
+
+def _host_y(y, name, n):
+    """targets as a host fp32 vector of length ``n``; ValueError when the length differs or a value is not finite"""
+    if torch.is_tensor(y):
+        y = y.detach().cpu().numpy()
+    y = np.asarray(y, dtype=np.float64).reshape(-1)
+    if len(y) != n:
+        raise ValueError("%s has %d values, one per pair is %d" % (name, len(y), n))
+    if not np.all(np.isfinite(y)):
+        raise ValueError("%s must be finite" % name)
+    return y.astype(np.float32)
+
+
+def _host_pairs(shape, users, items, y=None, name="pairs"):
+    """(users, items, y or None) checked on the host: ids in range, matching lengths, finite y"""
+    nu, ni = shape
+    users, items = _host_ids(users, name + " users", nu), _host_ids(items, name + " items", ni)
+    if len(users) != len(items):
+        raise ValueError("%s: users and items must have the same length (%d vs %d)" % (name, len(users), len(items)))
+    return users, items, (None if y is None else _host_y(y, name + " y", len(users)))
+
+
+def _split_pairs(pairs, name, need_y):
+    """(users, items) or (users, items, y) -> a 3-tuple; ValueError for another arity or a missing y"""
+    pairs = tuple(pairs)
+    if len(pairs) not in (2, 3) or (need_y and len(pairs) != 3):
+        raise ValueError("%s must be (users, items, y)%s" % (name, "" if need_y else " or (users, items)"))
+    return pairs if len(pairs) == 3 else pairs + (None,)
+
+
+def _check_lrs(lrs, K):
+    """eta_k per checkpoint as a list of K floats (None: all 1)"""
+    if lrs is None:
+        return [1.0] * K
+    lrs = [float(x) for x in np.asarray(lrs, dtype=np.float64).reshape(-1)]
+    if len(lrs) != K:
+        raise ValueError("lrs has %d values, one per checkpoint is %d" % (len(lrs), K))
+    if not all(np.isfinite(lrs)):
+        raise ValueError("lrs must be finite")
+    return lrs
+
+
+def _check_influence_k(k):
+    k = int(k)
+    if k < 1:
+        raise ValueError("k must be >= 1, not %d" % k)
+    if k > _lib.TOPK_MAX:
+        raise NotImplementedError("an influence run keeps at most k = %d training pairs per test pair" % _lib.TOPK_MAX)
+    return k
+
+
+def _check_test_count(T):
+    if T > INFLUENCE_T_MAX:
+        raise NotImplementedError("an influence run takes at most %d test pairs, not %d: split the test set"
+                                  % (INFLUENCE_T_MAX, T))
+
+
+def _check_per_pair_model(model):
+    if model._cmodel.readout != 0:
+        raise NotImplementedError("per-pair gradients need the IGMC readout: DGCNN_RS's SortPooling readout gradient "
+                                  "is summed over the batch")
+
+
 def _check_top(m, name):
     """None, or a count in [1, IGMC_TOPK_MAX] of entries to keep per pair"""
     if m is None:
@@ -139,6 +209,64 @@ Explanation = collections.namedtuple("Explanation", "score num_edges offsets use
 # The result of attribute_pairs: Explanation's layout and order with grad (d score / d m_e, the rating's weight m_e at
 # m = 1) in place of delta.  -grad is the first-order estimate of explain_pairs' delta.
 Attribution = collections.namedtuple("Attribution", "score num_edges offsets user item rating grad")
+
+# The result of influence: per test pair the k training pairs with the largest influence (pro_*, value descending) and
+# the k with the smallest (con_*, value ascending), [T, k] device tensors; index = position in the training list
+# (int64), value fp32; ties by index ascending, NaN after every number, empty slots index -1 and value -inf / +inf.
+Influence = collections.namedtuple("Influence", "pro_index pro_value con_index con_value")
+
+
+def influence_order_host(values, k):
+    """twin of igmc_influence_topk over a whole run: (pro_index, pro_value, con_index, con_value) for one test pair's
+    values [N] (index = position), padded with (-1, -inf) / (-1, +inf)"""
+    v = np.asarray(values, np.float32)
+    idx = np.arange(len(v))
+    out = []
+    for sign, pad in ((1.0, -np.inf), (-1.0, np.inf)):
+        key = np.where(np.isnan(v), np.inf, -sign * v.astype(np.float64))
+        o = np.lexsort((idx, key, np.isnan(v)))          # NaN last, key descending, then index
+        ti = np.full(k, -1, np.int64)
+        tv = np.full(k, pad, np.float32)
+        n = min(k, len(o))
+        ti[:n], tv[:n] = o[:n], v[o[:n]]
+        out += [ti, tv]
+    return tuple(out)
+
+
+def influence_merge_host(top_v, top_i, seg_v, seg_i, sign):
+    """twin of one side of one CTA of igmc_influence_topk: the running list (ranked under key sign * value) merged with
+    a batch's values (index < 0 skipped) by rank counting; returns the new (values, indices)"""
+    def before(av, ai, bv, bi):
+        if ai < 0:
+            return False
+        if bi < 0:
+            return True
+        ak, bk = np.float32(sign) * np.float32(av), np.float32(sign) * np.float32(bv)
+        an, bn = np.isnan(ak), np.isnan(bk)
+        if an or bn:
+            return ai < bi if (an and bn) else bool(bn)
+        return ak > bk or (ak == bk and ai < bi)
+    k = len(top_v)
+    V = list(np.asarray(top_v, np.float32)) + list(np.asarray(seg_v, np.float32))
+    I = list(np.asarray(top_i, np.int64)) + list(np.asarray(seg_i, np.int64))
+    out_v, out_i = np.array(top_v, np.float32), np.array(top_i, np.int64)
+    for e in range(len(V)):
+        if e >= k and I[e] < 0:
+            continue
+        r = e if e < k else sum(1 for o in range(k) if before(V[o], I[o], V[e], I[e]))
+        r += sum(1 for x in range(k, len(V)) if x != e and before(V[x], I[x], V[e], I[e]))
+        if r < k:
+            out_v[r], out_i[r] = V[e], I[e]
+    return out_v, out_i
+
+
+def readout_dot_host(fa, fb, F):
+    """the readout block's share of <G_a, G_b> from two factor rows dhid [128] | feat [F] | hid [128] | dpred"""
+    H = _lib.LIN1_OUT
+    dd = float(np.dot(fa[:H], fb[:H]))
+    ff = float(np.dot(fa[H:H + F], fb[H:H + F]))
+    hh = float(np.dot(fa[H + F:2 * H + F], fb[H + F:2 * H + F]))
+    return dd * (ff + 1.0) + float(fa[2 * H + F]) * float(fb[2 * H + F]) * (hh + 1.0)
 
 
 # ---- host twins of the candidate and merge kernels (csrc/recommend.cu) ----------------------------------------------
@@ -514,6 +642,132 @@ class InferenceEngine(object):
         m = _check_top(m, "m")
         return self._start_explicit("attribute", users, items, m=m, phase="base")
 
+    def start_pair_gradients(self, users, items, y=None):
+        """plan a per-pair gradient run (``pair_gradients``) over the explicit pairs: per checkpoint the gradient of
+        l_i = (f_i - y_i)^2 (``y`` given) or of the score f_i into run["out"] [K, P, param_count].  Returns P."""
+        _check_per_pair_model(self.model)
+        users, items, y = _host_pairs(self.graph.shape, users, items, y)
+        out = torch.zeros(self.K, len(users), self.model._cmodel.param_count, dtype=torch.float32, device=self.dev)
+        return self._start_explicit("pair_gradients", users, items, phase="pgrad", out=out, y=self._dev_y(y))
+
+    def start_influence(self, train, test, k, lrs=None):
+        """plan an influence run (``influence``): a test-gradient pass over ``test`` = (users, items[, y]) that stores
+        every checkpoint's test gradients, then a training pass over ``train`` = (users, items, y) that accumulates
+        S[b, t] = sum_k lrs[k] <G_b, G_t> per batch and merges it into each test pair's top-k lists.  Returns the
+        number of test pairs."""
+        k = _check_influence_k(k)
+        _check_per_pair_model(self.model)
+        tr = _host_pairs(self.graph.shape, *_split_pairs(train, "train", True), name="train")
+        te = _host_pairs(self.graph.shape, *_split_pairs(test, "test", False), name="test")
+        T = len(te[0])
+        _check_test_count(T)
+        lrs = _check_lrs(lrs, self.K)
+        m, dev = self.model._cmodel, self.dev
+        f32, i64 = dict(dtype=torch.float32, device=dev), dict(dtype=torch.int64, device=dev)
+        FW = self.lib.igmc_pair_factor_count(C.byref(m))
+        extra = dict(phase="test", train=tr, lrs=lrs, k=k, T=T, y=self._dev_y(te[2]),
+                     tconv=torch.zeros(self.K, T, m.conv_param_count, **f32), tfac=torch.zeros(self.K, T, FW, **f32),
+                     pro_i=torch.full((T, k), -1, **i64), pro_v=torch.full((T, k), -float("inf"), **f32),
+                     con_i=torch.full((T, k), -1, **i64), con_v=torch.full((T, k), float("inf"), **f32), self_out=None)
+        if T == 0:
+            self.run = dict(kind="influence", P=0, version=self.graph.version, **extra)
+            return 0
+        self._start_explicit("influence", te[0], te[1], **extra)
+        return T
+
+    def start_self_influence(self, train, lrs=None):
+        """plan a self-influence run (``self_influence``) over ``train`` = (users, items, y).  Returns its size."""
+        _check_per_pair_model(self.model)
+        tr = _host_pairs(self.graph.shape, *_split_pairs(train, "train", True), name="train")
+        lrs = _check_lrs(lrs, self.K)
+        N = len(tr[0])
+        self._start_explicit("self_influence", tr[0], tr[1], phase="train", lrs=lrs, T=0, y=self._dev_y(tr[2]),
+                             self_out=torch.zeros(N, dtype=torch.float32, device=self.dev))
+        if N:
+            self._train_buffers()
+        return N
+
+    def _dev_y(self, y):
+        return None if y is None else torch.from_numpy(y).to(self.dev)
+
+    def _train_buffers(self):
+        """the training pass's per-batch buffers: conv rows [B, PC], factor rows, S [B, T] and the GEMM workspace"""
+        run, m, dev = self.run, self.model._cmodel, self.dev
+        f32 = dict(dtype=torch.float32, device=dev)
+        FW = self.lib.igmc_pair_factor_count(C.byref(m))
+        nbytes = C.c_int64(0)
+        _lib.check(self.lib.igmc_influence_ws_bytes(C.byref(m), self.B, run["T"], C.byref(nbytes)),
+                   "igmc_influence_ws_bytes")
+        run["bufs"] = dict(conv=torch.zeros(self.B, m.conv_param_count, **f32), fac=torch.zeros(self.B, FW, **f32),
+                           S=torch.zeros(self.B, max(run["T"], 1), **f32),
+                           ws=torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=dev))
+
+    def _start_train_pass(self):
+        """after the test-gradient pass of an influence run: the training pairs primed.  Returns True when there are
+        any."""
+        run = self.run
+        users, items, y = run["train"]
+        run["phase"], run["P"], run["y"] = "train", len(users), self._dev_y(y)
+        if run["P"] == 0:
+            run["steps"] = run["done"] = 0
+            return False
+        run["pu"] = torch.from_numpy(users.astype(np.int32)).to(self.dev)
+        run["pv"] = torch.from_numpy(items.astype(np.int32)).to(self.dev)
+        Cd = _lib.Candidates()
+        Cd.pair_u, Cd.pair_v, Cd.num_pairs = run["pu"].data_ptr(), run["pv"].data_ptr(), run["P"]
+        run["Cd"] = Cd
+        self._train_buffers()
+        self._prime()
+        return True
+
+    def _pair_grad_step(self, slot):
+        """per parameter set: the training-mode forward of batch ``slot`` without dropout, the seed (loss or score),
+        the backward and the per-graph gradients - scattered to the pairs' rows (pair_gradients, the test-gradient
+        pass) or kept per batch and accumulated into the influence values and / or self-influence (training pass);
+        after the last checkpoint of a training batch the merge into the top-k lists"""
+        m, b, s, run, lib = self.model, self.batches[slot], self.slots[slot], self.run, self.lib
+        phase, tag, B = run["phase"], s["tag"].data_ptr(), self.B
+        st = _stream_ptr()
+        y = _lib.ptr(run["y"])
+        bufs = run.get("bufs")
+        dpred = self.preds[0]
+        for j in range(self.K):
+            with self._params(j):
+                pred, saved = m._launch_forward(b, True, self.drop)
+                ws = saved["ws"]
+                _lib.check(lib.igmc_pair_seed(pred.data_ptr(), y, tag, B, float(m._cmodel.multiply_by),
+                                              dpred.data_ptr(), st), "igmc_pair_seed")
+                m._launch_backward(b, self.drop, saved, dpred)
+                if phase == "pgrad":
+                    grad, fac, scatter, full = run["out"][j], None, 1, 1
+                elif phase == "test":
+                    grad, fac, scatter, full = run["tconv"][j], run["tfac"][j], 1, 0
+                else:
+                    grad, fac, scatter, full = bufs["conv"], bufs["fac"], 0, 0
+                cl = ws["cluster"]
+                _lib.check(lib.igmc_pair_grad(C.byref(m._cmodel), m.flat_params.data_ptr(), B, _lib.ctas_per_graph(cl),
+                                              ws["gpart"].data_ptr(), int(_lib.is_rs(cl)), ws["dhid"].data_ptr(),
+                                              ws["feat"].data_ptr(), ws["hid"].data_ptr(), dpred.data_ptr(), tag,
+                                              scatter, grad.data_ptr(), full, _lib.ptr(fac), st), "igmc_pair_grad")
+            if phase != "train":
+                continue
+            eta = run["lrs"][j]
+            if run["T"]:
+                _lib.check(lib.igmc_influence_accum(C.byref(m._cmodel), B, run["T"], bufs["conv"].data_ptr(),
+                                                    bufs["fac"].data_ptr(), run["tconv"][j].data_ptr(),
+                                                    run["tfac"][j].data_ptr(), eta, int(j == 0),
+                                                    bufs["ws"].data_ptr(), bufs["ws"].numel(), bufs["S"].data_ptr(),
+                                                    st), "igmc_influence_accum")
+            if run["self_out"] is not None:
+                _lib.check(lib.igmc_self_influence(C.byref(m._cmodel), B, bufs["conv"].data_ptr(),
+                                                   bufs["fac"].data_ptr(), tag, eta, run["self_out"].data_ptr(), st),
+                           "igmc_self_influence")
+        if phase == "train" and run["T"]:
+            _lib.check(lib.igmc_influence_topk(bufs["S"].data_ptr(), B, run["T"], tag, run["k"],
+                                               run["pro_v"].data_ptr(), run["pro_i"].data_ptr(),
+                                               run["con_v"].data_ptr(), run["con_i"].data_ptr(), st),
+                       "igmc_influence_topk")
+
     def _start_explicit(self, kind, users, items, **extra):
         g = self.graph
         users = _host_ids(users, "users", g.num_users)
@@ -673,6 +927,8 @@ class InferenceEngine(object):
         m, b, s, run = self.model, self.batches[slot], self.slots[slot], self.run
         if run.get("phase") == "grad":
             return self._gradient(slot)
+        if run.get("phase") in ("pgrad", "test", "train"):
+            return self._pair_grad_step(slot)
         occlude = run.get("phase") == "occlude"
         training, drop = (True, s["drop"]) if occlude else (False, self.drop)
         preds = None
@@ -752,6 +1008,8 @@ class InferenceEngine(object):
         run["done"] += 1
         if run["done"] < run["steps"]:
             return True
+        if run.get("phase") == "test":
+            return self._start_train_pass()
         if run.get("phase") != "base":
             return False
         return self._start_occlusion() if run["kind"] == "explain" else self._start_gradient()
@@ -773,6 +1031,12 @@ class InferenceEngine(object):
             return run["top_i"], run["top_s"]
         if run["kind"] in ("explain", "attribute"):
             return self._order(run)
+        if run["kind"] == "pair_gradients":
+            return run["out"]
+        if run["kind"] == "influence":
+            return Influence(run["pro_i"], run["pro_v"], run["con_i"], run["con_v"])
+        if run["kind"] == "self_influence":
+            return run["self_out"]
         return run["scores"]
 
     def _order(self, run):
@@ -811,6 +1075,18 @@ class InferenceEngine(object):
 
     def attribute_pairs(self, users, items, m=None):
         self.start_attribute(users, items, m)
+        return self.finish()
+
+    def pair_gradients(self, users, items, y=None):
+        self.start_pair_gradients(users, items, y)
+        return self.finish()
+
+    def influence(self, train, test, k, lrs=None):
+        self.start_influence(train, test, k, lrs)
+        return self.finish()
+
+    def self_influence(self, train, lrs=None):
+        self.start_self_influence(train, lrs)
         return self.finish()
 
     def close(self):
@@ -897,6 +1173,72 @@ def attribute_pairs(model, graph, users, items, m=None, *, h=1, sample_ratio=1.0
     eng = InferenceEngine(model, graph, h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
     try:
         return eng.attribute_pairs(users, items, m)
+    finally:
+        eng.close()
+
+
+def pair_gradients(model, graph, users, items, y=None, *, h=1, sample_ratio=1.0, max_nodes_per_hop=None,
+                   batch_size=256, checkpoints=None, sample_seed=0):
+    """per-example gradients [K, P, param_count] fp32 on the model's device, in the ``flat_params`` layout (conv
+    parameters, then lin1 and lin2), one row per pair and checkpoint (K = 1 without ``checkpoints``).  With ``y``: the
+    gradient of l_i = (f_i - y_i)^2, the squared error of ONE pair - the batch mean and the ARR regulariser are not
+    per-example terms and are left out; the backward's seed is 2 (f_i - y_i) * multiply_by.  Without ``y``: the gradient
+    of the score f_i (seed multiply_by).  Pair i's subgraph is the one ``predict_pairs`` scores (its own rating removed,
+    sampled by its pair id); the forward is the eval forward, run as a training-mode launch with both dropout rates 0,
+    on the model's own kernel plan.  Needs 4 * param_count bytes per pair and checkpoint (197 KB at R = 5): meant for
+    thousands of pairs; ``influence`` / ``self_influence`` never materialise them.  IGMC only (DGCNN_RS:
+    NotImplementedError)."""
+    _check_per_pair_model(model)
+    users, items, y = _host_pairs(graph.shape, users, items, y)
+    if len(users) == 0:
+        K = len(checkpoints) if checkpoints else 1
+        return torch.zeros(K, 0, model._cmodel.param_count, dtype=torch.float32, device=model.flat_params.device)
+    eng = InferenceEngine(model, graph, h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
+    try:
+        return eng.pair_gradients(users, items, y)
+    finally:
+        eng.close()
+
+
+def influence(model, graph, train, test, k, *, checkpoints=None, lrs=None, h=1, sample_ratio=1.0,
+              max_nodes_per_hop=None, batch_size=256, sample_seed=0):
+    """TracIn-CP influence of every training pair on every test pair:
+        influence(i, t) = sum over checkpoints k of lrs[k] * < grad l_i(theta_k), grad q_t(theta_k) >
+    with l_i = (f_i - y_i)^2 of one training pair (``pair_gradients``' definition: no batch mean, no ARR term) and q_t =
+    l_t for a labelled test pair, f_t (the score) otherwise.  ``train`` = (users, items, y) with y the value the model
+    was trained against; ``test`` = (users, items) or (users, items, y), at most INFLUENCE_T_MAX = 1024 pairs
+    (NotImplementedError above: split the test set).  ``lrs``: eta_k per checkpoint, default 1.  Sign: with test labels
+    a positive value marks a proponent - a gradient step on i lowers t's loss; without, a step theta <- theta - eta
+    grad l_i changes f_t by -eta * influence to first order.  Returns an ``Influence`` of [T, k] device tensors: the k
+    largest values (pro_*) and the k smallest (con_*) per test pair, index = position in ``train``; ties by index, NaN
+    after every number, empty slots -1 / -inf (pro) and -1 / +inf (con).  Conv block by a split-K FFMA GEMM, readout
+    block from its rank-1 factors; bit-identical across runs, batch sizes and graph replay.  IGMC only."""
+    k = _check_influence_k(k)
+    _check_per_pair_model(model)
+    users, items, y = _host_pairs(graph.shape, *_split_pairs(train, "train", True), name="train")
+    tu, ti, ty = _host_pairs(graph.shape, *_split_pairs(test, "test", False), name="test")
+    _check_test_count(len(tu))
+    _check_lrs(lrs, len(checkpoints) if checkpoints else 1)
+    eng = InferenceEngine(model, graph, h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
+    try:
+        return eng.influence((users, items, y), (tu, ti, ty), k, lrs)
+    finally:
+        eng.close()
+
+
+def self_influence(model, graph, train, *, checkpoints=None, lrs=None, h=1, sample_ratio=1.0, max_nodes_per_hop=None,
+                   batch_size=256, sample_seed=0):
+    """self_influence(i) = sum over checkpoints k of lrs[k] * ||grad l_i(theta_k)||^2 for every training pair of
+    ``train`` = (users, items, y), [N] fp32 on the model's device (``influence``'s definitions).  The usual detector
+    of mislabelled training examples: large values first.  IGMC only."""
+    _check_per_pair_model(model)
+    users, items, y = _host_pairs(graph.shape, *_split_pairs(train, "train", True), name="train")
+    _check_lrs(lrs, len(checkpoints) if checkpoints else 1)
+    if len(users) == 0:
+        return torch.zeros(0, dtype=torch.float32, device=model.flat_params.device)
+    eng = InferenceEngine(model, graph, h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
+    try:
+        return eng.self_influence((users, items, y), lrs)
     finally:
         eng.close()
 

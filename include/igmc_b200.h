@@ -542,6 +542,52 @@ int igmc_edge_grad_scatter(const igmc_batch_out_t* O, int B, const int64_t* tag,
                            const int64_t* offsets, int k, int K, float* out, int32_t* user, int32_t* item,
                            int32_t* rating, int* err, void* stream);
 
+/* ---- per-pair gradients and training-data influence (csrc/influence.cu) ----
+ * TracIn-CP (Pruthi et al., NeurIPS 2020): influence(i, t) = sum_k eta_k <grad l_i(theta_k), grad q_t(theta_k)> over
+ * checkpoints k, self_influence(i) = sum_k eta_k ||grad l_i(theta_k)||^2, with l_i = (f_i - y_i)^2 of ONE pair (no batch
+ * mean, no ARR term) and q_t = l_t (labelled test pair) or f_t (the score).  A gradient is the flat parameter vector in
+ * the model's layout.  The per-pair gradient of graph g comes from the same backward as a training step (dropout rates 0):
+ * its conv block is the sum of g's own partial rows, its readout block the rank-1 factors dhid (x) feat and dpred * hid. */
+
+/* floats of one pair's factor row: dhid [128] | feat [2*32*L] | hid [128] | dpred [1] */
+int igmc_pair_factor_count(const igmc_model_t* M);
+
+/* dpred[g] = d l / d lin2 output for the backward: 2 (pred[g] - y[tag[g]]) multiply_by with y (the loss seed, the
+ * forward's own dpred at loss_scale 1), multiply_by without (the score seed), 0 where tag[g] < 0 (padding). */
+int igmc_pair_seed(const float* pred, const float* y, const int64_t* tag, int B, float multiply_by, float* dpred,
+                   void* stream);
+
+/* Per-graph gradients of a batch whose backward left gpart (rows_per_graph rows per graph, graph-major; raw_rows != 0:
+ * the raw rows of the cluster plans, chain rule applied per graph) and the readout factors.  Row of graph g: g, or
+ * tag[g] when `scatter` (tag < 0: nothing written); padding graphs of an unscattered batch get zeros.  grad (optional):
+ * the conv block, row stride conv_param_count, or (full != 0) the whole gradient, row stride param_count, lin1 / lin2
+ * materialised from the factors.  fac (optional): the factor rows (igmc_pair_factor_count floats).  IGMC readout only
+ * (readout = 1: -16); raw rows need num_relations <= 12. */
+int igmc_pair_grad(const igmc_model_t* M, const float* params, int B, int rows_per_graph, const float* gpart,
+                   int raw_rows, const float* dhid, const float* feat, const float* hid, const float* dpred,
+                   const int64_t* tag, int scatter, float* grad, int full, float* fac, void* stream);
+
+/* self_out[tag[g]] += eta * ||G_g||^2 for every graph with tag >= 0, from its conv row (stride conv_param_count) and
+ * factor row; one CTA per graph, fixed order. */
+int igmc_self_influence(const igmc_model_t* M, int B, const float* conv, const float* fac, const int64_t* tag,
+                        float eta, float* self_out, void* stream);
+
+/* S[b][t] (= first ? 0 : S[b][t]) + eta * <G_b, G_t> for B training rows (conv_b [B][conv_param_count], fac_b) against T
+ * test rows (conv_t, fac_t).  Conv block: split-K FFMA over fixed chunks of 256 entries, the splits summed in a fixed
+ * order; readout block: (dhid_b . dhid_t)(feat_b . feat_t + 1) + dpred_b dpred_t (hid_b . hid_t + 1).  No float atomics:
+ * bit-identical across runs and batch sizes.  `ws`: igmc_influence_ws_bytes bytes. */
+int igmc_influence_ws_bytes(const igmc_model_t* M, int B, int T, int64_t* bytes);
+int igmc_influence_accum(const igmc_model_t* M, int B, int T, const float* conv_b, const float* fac_b,
+                         const float* conv_t, const float* fac_t, float eta, int first, void* ws, int64_t ws_bytes,
+                         float* S, void* stream);
+
+/* Per test pair t (one CTA each): the batch's values S[b][t] with index tag[b] (tag < 0 skipped) merged into the
+ * running proponents (value descending) and opponents (value ascending) [T][k]; ties by index ascending, NaN after
+ * every number, empty slots (index -1, value -inf / +inf, initialised by the caller) last.  A strict total order: the
+ * result does not depend on batch boundaries.  1 <= k <= IGMC_TOPK_MAX. */
+int igmc_influence_topk(const float* S, int B, int T, const int64_t* tag, int k, float* pro_value,
+                        int64_t* pro_index, float* con_value, int64_t* con_index, void* stream);
+
 /* ---- candidate retrieval by bridge count (csrc/retrieve.cu) ----
  * For h = 1 the enclosing subgraph of an unrated pair (u, v) joins u's star and v's star only through the bridge edges
  * (u', i): u' != u rated v and i, u rated i.  Their number is
