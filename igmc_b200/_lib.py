@@ -26,6 +26,7 @@ ERR_NAMES = {
     6: "subgraph of more than 65535 nodes (beyond the 16-bit neighbour field of the edge lists)",
     7: "inference candidates: a user / item id outside the rating matrix or an inconsistent candidate plan",
     8: "graph update: a user / item id outside the graph's capacity or a value outside 0..256",
+    9: "rating sessions: a session / item id out of range, a negative user id or a value outside 0..256",
 }
 
 TOPK_MAX = 256       # IGMC_TOPK_MAX
@@ -121,6 +122,11 @@ class Candidates(C.Structure):
                 ("exclude_rated", C.c_int32), ("per_user", C.c_int32)]
 
 
+class Sessions(C.Structure):
+    _fields_ = [("users", vp), ("row_ptr", vp), ("col_idx", vp), ("rating", vp), ("num_sessions", C.c_int32),
+                ("max_row_deg", C.c_int32)]
+
+
 GRAPH_UPDATE_HEADER = ("nnz", "num_users", "num_items", "max_row_deg", "max_col_deg", "inserted", "changed",
                        "removed")   # igmc_graph_update_header_t: these int64 fields, then int32 status, int32 err
 GRAPH_UPDATE_OVER_CAPACITY, GRAPH_UPDATE_OVER_INT32 = 1, 2
@@ -207,6 +213,14 @@ _SIGS = {
                                C.c_int, vp, C.c_int64, vp, vp, vp],
     "igmc_graph_update_apply": [C.POINTER(CSR), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, C.c_int64, C.c_int,
                                 C.c_int, C.c_int, vp],
+    "igmc_session_ws_bytes": [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int64)],
+    "igmc_session_plan": [C.POINTER(CSR), vp, C.c_int, vp, vp, vp, C.c_int, vp, C.c_int64, vp, vp, vp],
+    "igmc_session_apply": [C.POINTER(CSR), vp, C.c_int, C.c_int, vp, C.c_int64, vp, vp, vp, vp],
+    "igmc_session_pairs": [C.POINTER(Sessions), C.c_int, C.c_int, vp, vp, vp, vp, vp, vp],
+    "igmc_extract_sessions": [C.POINTER(CSR), C.POINTER(Sessions), vp, C.POINTER(Pairs), C.c_int, C.c_int, C.c_int,
+                              C.c_double, C.c_uint64, vp, C.c_int, C.POINTER(ExtractWS), vp, C.c_int, C.c_int,
+                              C.POINTER(BatchOut), vp, vp],
+    "igmc_corated_sessions": [C.POINTER(CSR), C.POINTER(Sessions), C.c_int, C.c_int, vp, C.c_int64, vp, vp, vp, vp],
     "igmc_build_info": [],
     "igmc_model_plan": [C.POINTER(Model), C.c_int, C.c_int, C.c_int],
     "igmc_sortpool_plan": [C.POINTER(SortPool), C.c_int, C.c_int],

@@ -17,6 +17,7 @@ enum {
   IGMC_ERR_NODE_ID16 = 6,   // subgraph of more than 65 535 nodes: beyond the 16-bit neighbour field of the lists
   IGMC_ERR_CANDIDATES = 7,  // inference candidates: a user / item id outside the rating matrix or an inconsistent plan
   IGMC_ERR_GRAPH_UPDATE = 8,  // graph update: an id outside the capacity or a value outside 0..256
+  IGMC_ERR_SESSIONS = 9,    // rating sessions: a session / item id out of range, a negative user or a value outside 0..256
 };
 
 __device__ __forceinline__ void igmc_set_err(int* err, int code) {

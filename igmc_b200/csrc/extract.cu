@@ -188,15 +188,36 @@ __device__ __forceinline__ void resolve_pair(const igmc_pairs_t& P, int g, int* 
   *pid = P.pair_id ? P.pair_id[g] : src;
 }
 
-__global__ void __launch_bounds__(EX_THREADS)
-k_extract_select_count(igmc_csr_t G, igmc_pairs_t P, int B, int mnph, double ratio, uint64_t seed_val,
-                       const uint64_t* __restrict__ seed_dev, int cap,
-                       const int32_t* __restrict__ inj_nodes_u, const int32_t* __restrict__ inj_nodes_v,
-                       const int32_t* __restrict__ inj_n_u, const int32_t* __restrict__ inj_n_v,
-                       int32_t* __restrict__ nodes_u, int32_t* __restrict__ nodes_v,
-                       int32_t* __restrict__ n_u, int32_t* __restrict__ n_v,
-                       int32_t* __restrict__ row_cnt, int32_t* __restrict__ m_cnt, int32_t* __restrict__ col_cnt,
-                       int h, int32_t* __restrict__ hop_off, int* err) {
+// Session mode (igmc_extract_sessions): graph g takes its target user's row from session row sess[g]; every other row
+// and column comes from G.  The extraction kernels are bodies templated on the mode; the plain kernels pass an empty
+// SessArg, which their code never reads.
+struct SessArg {
+  igmc_sessions_t S;
+  const int32_t* sess;   // [B] session of graph g
+};
+
+// the target row (ptr into its column ids, its ratings, its length) of graph g in session mode
+struct TargetRow {
+  const int32_t* col;
+  const uint8_t* rat;
+  int len;
+};
+__device__ __forceinline__ TargetRow session_row(const SessArg& A, int g) {
+  const int q = A.sess[g];
+  const int s = A.S.row_ptr[q];
+  return {A.S.col_idx + s, A.S.rating + s, A.S.row_ptr[q + 1] - s};
+}
+
+template <bool SESS>
+__device__ __forceinline__ void
+extract_select_count(const igmc_csr_t& G, const igmc_pairs_t& P, int B, int mnph, double ratio, uint64_t seed_val,
+                     const uint64_t* __restrict__ seed_dev, int cap,
+                     const int32_t* __restrict__ inj_nodes_u, const int32_t* __restrict__ inj_nodes_v,
+                     const int32_t* __restrict__ inj_n_u, const int32_t* __restrict__ inj_n_v,
+                     int32_t* __restrict__ nodes_u, int32_t* __restrict__ nodes_v,
+                     int32_t* __restrict__ n_u, int32_t* __restrict__ n_v,
+                     int32_t* __restrict__ row_cnt, int32_t* __restrict__ m_cnt, int32_t* __restrict__ col_cnt,
+                     int h, int32_t* __restrict__ hop_off, int* err, const SessArg& A) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   int* colcnt = reinterpret_cast<int*>(smem_raw);                 // [cap]
   uint16_t* tab = reinterpret_cast<uint16_t*>(colcnt + cap);      // [num_items]
@@ -216,6 +237,8 @@ k_extract_select_count(igmc_csr_t G, igmc_pairs_t P, int B, int mnph, double rat
   int i, j, lab;
   int64_t pid;
   resolve_pair(P, g, &i, &j, &lab, &pid);
+  TargetRow tr = {};
+  if (SESS) tr = session_row(A, g);
   int32_t* gu = nodes_u + (size_t)g * cap;
   int32_t* gv = nodes_v + (size_t)g * cap;
   if (tid == 0) s_m = 0;
@@ -233,8 +256,12 @@ k_extract_select_count(igmc_csr_t G, igmc_pairs_t P, int B, int mnph, double rat
     // user fringe = users who rated item j (CSC column j); item fringe = items rated by user i (CSR row i)
     select_side(G.row_idx + G.col_ptr[j], G.col_ptr[j + 1] - G.col_ptr[j], i, true, mnph, ratio,
                 sample_state(seed, pid, 0, 1), gu, cap, &s_nu, hist, ws, sh, err);
-    select_side(G.col_idx + G.row_ptr[i], G.row_ptr[i + 1] - G.row_ptr[i], j, true, mnph, ratio,
-                sample_state(seed, pid, 1, 1), gv, cap, &s_nv, hist, ws, sh, err);
+    if (SESS)
+      select_side(tr.col, tr.len, j, true, mnph, ratio, sample_state(seed, pid, 1, 1), gv, cap, &s_nv, hist, ws, sh,
+                  err);
+    else
+      select_side(G.col_idx + G.row_ptr[i], G.row_ptr[i + 1] - G.row_ptr[i], j, true, mnph, ratio,
+                  sample_state(seed, pid, 1, 1), gv, cap, &s_nv, hist, ws, sh, err);
   }
   __syncthreads();
   if (hop_off && tid == 0) {   // nodes within distance d per side: [users 0..3 | items 0..3]
@@ -247,9 +274,17 @@ k_extract_select_count(igmc_csr_t G, igmc_pairs_t P, int B, int mnph, double rat
     // util_functions.py:220-221)
     for (int w = tid; w < wu + wv; w += nt) vis_u[w] = 0;   // vis_u and vis_v are contiguous
     __syncthreads();
-    if (tid == 0) { atomicOr(&vis_u[i >> 5], 1u << (i & 31)); atomicOr(&vis_v[j >> 5], 1u << (j & 31)); }
+    // (a session's new user, i >= num_users, is in no column of G: it needs no visited bit and has none)
+    if (tid == 0) {
+      if (!SESS || i < G.num_users) atomicOr(&vis_u[i >> 5], 1u << (i & 31));
+      atomicOr(&vis_v[j >> 5], 1u << (j & 31));
+    }
     for (int p = G.col_ptr[j] + tid; p < G.col_ptr[j + 1]; p += nt) { const int t = G.row_idx[p]; atomicOr(&vis_u[t >> 5], 1u << (t & 31)); }
-    for (int p = G.row_ptr[i] + tid; p < G.row_ptr[i + 1]; p += nt) { const int t = G.col_idx[p]; atomicOr(&vis_v[t >> 5], 1u << (t & 31)); }
+    if (SESS) {
+      for (int p = tid; p < tr.len; p += nt) { const int t = tr.col[p]; atomicOr(&vis_v[t >> 5], 1u << (t & 31)); }
+    } else {
+      for (int p = G.row_ptr[i] + tid; p < G.row_ptr[i + 1]; p += nt) { const int t = G.col_idx[p]; atomicOr(&vis_v[t >> 5], 1u << (t & 31)); }
+    }
     __syncthreads();
     int lo_u = 1, hi_u = s_nu, lo_v = 1, hi_v = s_nv;
     for (int d = 2; d <= h; ++d) {
@@ -293,10 +328,13 @@ k_extract_select_count(igmc_csr_t G, igmc_pairs_t P, int B, int mnph, double rat
   // per-row match count (warp per user row); bit31 = row contains the target item j
   for (int a = warp; a < nu; a += nwarps) {
     const int u = gu[a];
-    const int s = G.row_ptr[u], e = G.row_ptr[u + 1];
+    const int32_t* ci = G.col_idx;
+    int s, e;
+    if (SESS && a == 0) { ci = tr.col; s = 0; e = tr.len; }
+    else { s = G.row_ptr[u]; e = G.row_ptr[u + 1]; }
     int cnt = 0, hasj = 0;
     for (int p = s + lane; p < e; p += 32) {
-      const uint16_t b = tab[G.col_idx[p]];
+      const uint16_t b = tab[ci[p]];
       if (b != NONE16) {
         if (b == 0) { hasj = 1; if (a != 0) { ++cnt; atomicAdd(&colcnt[0], 1); } }   // (0,0) = target edge: dropped (ref :238)
         else { ++cnt; atomicAdd(&colcnt[b], 1); }
@@ -314,13 +352,14 @@ k_extract_select_count(igmc_csr_t G, igmc_pairs_t P, int B, int mnph, double rat
   if (tid == 0) { n_u[g] = nu; n_v[g] = nv; m_cnt[g] = s_m; }
 }
 
-__global__ void __launch_bounds__(EX_THREADS)
-k_extract_fill(igmc_csr_t G, igmc_pairs_t P, int B, int cap,
-               const int32_t* __restrict__ nodes_u, const int32_t* __restrict__ nodes_v,
-               const int32_t* __restrict__ n_u, const int32_t* __restrict__ n_v,
-               const int32_t* __restrict__ row_cnt, const int32_t* __restrict__ m_cnt,
-               const int32_t* __restrict__ col_cnt, int h, const int32_t* __restrict__ hop_off,
-               const float* __restrict__ class_values, igmc_batch_out_t O, int* err) {
+template <bool SESS>
+__device__ __forceinline__ void
+extract_fill(const igmc_csr_t& G, const igmc_pairs_t& P, int B, int cap,
+             const int32_t* __restrict__ nodes_u, const int32_t* __restrict__ nodes_v,
+             const int32_t* __restrict__ n_u, const int32_t* __restrict__ n_v,
+             const int32_t* __restrict__ row_cnt, const int32_t* __restrict__ m_cnt,
+             const int32_t* __restrict__ col_cnt, int h, const int32_t* __restrict__ hop_off,
+             const float* __restrict__ class_values, const igmc_batch_out_t& O, int* err, const SessArg& A) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   int* rowoff = reinterpret_cast<int*>(smem_raw);                 // [cap]
   int* colfill = rowoff + cap;                                    // [cap] running fill pointer of the item lists
@@ -418,9 +457,15 @@ k_extract_fill(igmc_csr_t G, igmc_pairs_t P, int B, int cap,
   int64_t* ei0 = O.edge_index;
   int64_t* ei1 = O.edge_index + O.edge_cap;
   const unsigned lt_mask = (1u << lane) - 1u;
+  TargetRow tr = {};
+  if (SESS) tr = session_row(A, g);
   for (int a = warp; a < nu; a += nwarps) {
     const int u = gu[a];
-    const int s = G.row_ptr[u], e = G.row_ptr[u + 1];
+    const int32_t* ci = G.col_idx;
+    const uint8_t* rt = G.rating;
+    int s, e;
+    if (SESS && a == 0) { ci = tr.col; rt = tr.rat; s = 0; e = tr.len; }
+    else { s = G.row_ptr[u]; e = G.row_ptr[u + 1]; }
     const int jfirst = (a != 0 && (row_cnt[(size_t)g * cap + a] < 0)) ? 1 : 0;  // j sorts first (v_local 0)
     const int base = rowoff[a];
     int seen = 0;
@@ -432,7 +477,7 @@ k_extract_fill(igmc_csr_t G, igmc_pairs_t P, int B, int cap,
       for (int p0 = s; p0 < e; p0 += 32) {
         const int p = p0 + lane;
         uint16_t b = NONE16;
-        if (p < e) b = tab[G.col_idx[p]];
+        if (p < e) b = tab[ci[p]];
         const bool m_ = (b != NONE16) && b != 0;
 #pragma unroll
         for (int d = 1; d <= IGMC_MAX_HOP; ++d)
@@ -445,7 +490,7 @@ k_extract_fill(igmc_csr_t G, igmc_pairs_t P, int B, int cap,
     for (int p0 = s; p0 < e; p0 += 32) {
       const int p = p0 + lane;
       uint16_t b = NONE16;
-      if (p < e) b = tab[G.col_idx[p]];
+      if (p < e) b = tab[ci[p]];
       const bool match = (b != NONE16) && !(a == 0 && b == 0);
       const bool isj = match && b == 0;
       const unsigned bal = __ballot_sync(IGMC_FULL, match && !isj);
@@ -461,7 +506,7 @@ k_extract_fill(igmc_csr_t G, igmc_pairs_t P, int B, int cap,
       }
       if (match) {
         const int rank = isj ? 0 : (h > 1 ? jfirst + hrank : jfirst + seen + __popc(bal & lt_mask));
-        const int64_t r = G.rating[p];
+        const int64_t r = rt[p];
         const size_t e1 = (size_t)2 * Mbase + base + rank, e2 = e1 + m;
         const int64_t un = Nbase + a, vn = Nbase + nu + b;
         ei0[e1] = un; ei1[e1] = vn; O.edge_type[e1] = r;
@@ -547,12 +592,13 @@ __host__ __device__ __forceinline__ size_t fast_smem_ints(int cap, int R, int wo
          FX_CANO;
 }
 
-__global__ void __launch_bounds__(FX_THREADS, 2)
-k_extract_fast(igmc_csr_t G, igmc_pairs_t P, int B, int mnph, double ratio, uint64_t seed_val,
-               const uint64_t* __restrict__ seed_dev, int cap, const int32_t* __restrict__ inj_nodes_u,
-               const int32_t* __restrict__ inj_nodes_v, const int32_t* __restrict__ inj_n_u,
-               const int32_t* __restrict__ inj_n_v, igmc_extract_ws_t W, int R, int words, int slot_e,
-               const float* __restrict__ class_values, igmc_batch_out_t O, int* err) {
+template <bool SESS>
+__device__ __forceinline__ void
+extract_fast(const igmc_csr_t& G, const igmc_pairs_t& P, int B, int mnph, double ratio, uint64_t seed_val,
+             const uint64_t* __restrict__ seed_dev, int cap, const int32_t* __restrict__ inj_nodes_u,
+             const int32_t* __restrict__ inj_nodes_v, const int32_t* __restrict__ inj_n_u,
+             const int32_t* __restrict__ inj_n_v, const igmc_extract_ws_t& W, int R, int words, int slot_e,
+             const float* __restrict__ class_values, const igmc_batch_out_t& O, int* err, const SessArg& A) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   FastSmem S;
   {
@@ -589,6 +635,8 @@ k_extract_fast(igmc_csr_t G, igmc_pairs_t P, int B, int mnph, double ratio, uint
   int i, j, lab;
   int64_t pid;
   resolve_pair(P, g, &i, &j, &lab, &pid);
+  TargetRow tr = {};
+  if (SESS) tr = session_row(A, g);
   int32_t* gu = W.nodes_u + (size_t)g * cap;
   int32_t* gv = W.nodes_v + (size_t)g * cap;
 
@@ -606,8 +654,12 @@ k_extract_fast(igmc_csr_t G, igmc_pairs_t P, int B, int mnph, double ratio, uint
   } else {
     select_side(G.row_idx + G.col_ptr[j], G.col_ptr[j + 1] - G.col_ptr[j], i, true, mnph, ratio,
                 sample_state(seed, pid, 0, 1), gu, cap, &s_nu, hist, ws, sh, err);
-    select_side(G.col_idx + G.row_ptr[i], G.row_ptr[i + 1] - G.row_ptr[i], j, true, mnph, ratio,
-                sample_state(seed, pid, 1, 1), gv, cap, &s_nv, hist, ws, sh, err);
+    if (SESS)
+      select_side(tr.col, tr.len, j, true, mnph, ratio, sample_state(seed, pid, 1, 1), gv, cap, &s_nv, hist, ws, sh,
+                  err);
+    else
+      select_side(G.col_idx + G.row_ptr[i], G.row_ptr[i + 1] - G.row_ptr[i], j, true, mnph, ratio,
+                  sample_state(seed, pid, 1, 1), gv, cap, &s_nv, hist, ws, sh, err);
   }
   __syncthreads();
   const int nu = s_nu, nv = s_nv, n = nu + nv;
@@ -623,10 +675,15 @@ k_extract_fast(igmc_csr_t G, igmc_pairs_t P, int B, int mnph, double ratio, uint
       const int a = base + tid;
       int d = 0;
       if (a < nu) {
-        const int u = gu[a];
-        const int s0 = G.row_ptr[u];
-        S.rp[a] = s0;
-        d = G.row_ptr[u + 1] - s0;
+        if (SESS && a == 0) {   // the target row: offsets into the session's own arrays
+          S.rp[a] = 0;
+          d = tr.len;
+        } else {
+          const int u = gu[a];
+          const int s0 = G.row_ptr[u];
+          S.rp[a] = s0;
+          d = G.row_ptr[u + 1] - s0;
+        }
       }
       int tot;
       const int ex = block_excl_scan_i(d, ws, &tot);
@@ -662,8 +719,11 @@ k_extract_fast(igmc_csr_t G, igmc_pairs_t P, int B, int mnph, double ratio, uint
         if (q < D) {
           while (q >= S.rowstart[a + 1]) ++a;
           const int p = S.rp[a] + (q - S.rowstart[a]);
-          col[u] = __ldg(G.col_idx + p);
-          rat[u] = __ldg(G.rating + p);     // fetched with the index (1 B per entry): no second dependent L2 latency
+          const int32_t* cb = G.col_idx;
+          const uint8_t* rb = G.rating;
+          if (SESS && a == 0) { cb = tr.col; rb = tr.rat; }
+          col[u] = __ldg(cb + p);
+          rat[u] = __ldg(rb + p);     // fetched with the index (1 B per entry): no second dependent L2 latency
         }
         ar[u] = a;
       }
@@ -914,6 +974,66 @@ k_extract_fast(igmc_csr_t G, igmc_pairs_t P, int B, int mnph, double ratio, uint
   }
 }
 
+// The kernels: plain (the graph's rows only) and session mode.
+__global__ void __launch_bounds__(EX_THREADS)
+k_extract_select_count(igmc_csr_t G, igmc_pairs_t P, int B, int mnph, double ratio, uint64_t seed_val,
+                       const uint64_t* __restrict__ seed_dev, int cap,
+                       const int32_t* __restrict__ inj_nodes_u, const int32_t* __restrict__ inj_nodes_v,
+                       const int32_t* __restrict__ inj_n_u, const int32_t* __restrict__ inj_n_v,
+                       int32_t* __restrict__ nodes_u, int32_t* __restrict__ nodes_v,
+                       int32_t* __restrict__ n_u, int32_t* __restrict__ n_v,
+                       int32_t* __restrict__ row_cnt, int32_t* __restrict__ m_cnt, int32_t* __restrict__ col_cnt,
+                       int h, int32_t* __restrict__ hop_off, int* err) {
+  extract_select_count<false>(G, P, B, mnph, ratio, seed_val, seed_dev, cap, inj_nodes_u, inj_nodes_v, inj_n_u,
+                              inj_n_v, nodes_u, nodes_v, n_u, n_v, row_cnt, m_cnt, col_cnt, h, hop_off, err, SessArg{});
+}
+__global__ void __launch_bounds__(EX_THREADS)
+k_extract_select_count_sess(igmc_csr_t G, igmc_pairs_t P, int B, int mnph, double ratio, uint64_t seed_val,
+                            const uint64_t* __restrict__ seed_dev, int cap, int32_t* __restrict__ nodes_u,
+                            int32_t* __restrict__ nodes_v, int32_t* __restrict__ n_u, int32_t* __restrict__ n_v,
+                            int32_t* __restrict__ row_cnt, int32_t* __restrict__ m_cnt,
+                            int32_t* __restrict__ col_cnt, int h, int32_t* __restrict__ hop_off, int* err,
+                            SessArg A) {
+  extract_select_count<true>(G, P, B, mnph, ratio, seed_val, seed_dev, cap, nullptr, nullptr, nullptr, nullptr,
+                             nodes_u, nodes_v, n_u, n_v, row_cnt, m_cnt, col_cnt, h, hop_off, err, A);
+}
+__global__ void __launch_bounds__(EX_THREADS)
+k_extract_fill(igmc_csr_t G, igmc_pairs_t P, int B, int cap,
+               const int32_t* __restrict__ nodes_u, const int32_t* __restrict__ nodes_v,
+               const int32_t* __restrict__ n_u, const int32_t* __restrict__ n_v,
+               const int32_t* __restrict__ row_cnt, const int32_t* __restrict__ m_cnt,
+               const int32_t* __restrict__ col_cnt, int h, const int32_t* __restrict__ hop_off,
+               const float* __restrict__ class_values, igmc_batch_out_t O, int* err) {
+  extract_fill<false>(G, P, B, cap, nodes_u, nodes_v, n_u, n_v, row_cnt, m_cnt, col_cnt, h, hop_off, class_values, O,
+                      err, SessArg{});
+}
+__global__ void __launch_bounds__(EX_THREADS)
+k_extract_fill_sess(igmc_csr_t G, igmc_pairs_t P, int B, int cap,
+                    const int32_t* __restrict__ nodes_u, const int32_t* __restrict__ nodes_v,
+                    const int32_t* __restrict__ n_u, const int32_t* __restrict__ n_v,
+                    const int32_t* __restrict__ row_cnt, const int32_t* __restrict__ m_cnt,
+                    const int32_t* __restrict__ col_cnt, int h, const int32_t* __restrict__ hop_off,
+                    const float* __restrict__ class_values, igmc_batch_out_t O, int* err, SessArg A) {
+  extract_fill<true>(G, P, B, cap, nodes_u, nodes_v, n_u, n_v, row_cnt, m_cnt, col_cnt, h, hop_off, class_values, O,
+                     err, A);
+}
+__global__ void __launch_bounds__(FX_THREADS, 2)
+k_extract_fast(igmc_csr_t G, igmc_pairs_t P, int B, int mnph, double ratio, uint64_t seed_val,
+               const uint64_t* __restrict__ seed_dev, int cap, const int32_t* __restrict__ inj_nodes_u,
+               const int32_t* __restrict__ inj_nodes_v, const int32_t* __restrict__ inj_n_u,
+               const int32_t* __restrict__ inj_n_v, igmc_extract_ws_t W, int R, int words, int slot_e,
+               const float* __restrict__ class_values, igmc_batch_out_t O, int* err) {
+  extract_fast<false>(G, P, B, mnph, ratio, seed_val, seed_dev, cap, inj_nodes_u, inj_nodes_v, inj_n_u, inj_n_v, W, R,
+                      words, slot_e, class_values, O, err, SessArg{});
+}
+__global__ void __launch_bounds__(FX_THREADS, 2)
+k_extract_fast_sess(igmc_csr_t G, igmc_pairs_t P, int B, int mnph, double ratio, uint64_t seed_val,
+                    const uint64_t* __restrict__ seed_dev, int cap, igmc_extract_ws_t W, int R, int words,
+                    int slot_e, const float* __restrict__ class_values, igmc_batch_out_t O, int* err, SessArg A) {
+  extract_fast<true>(G, P, B, mnph, ratio, seed_val, seed_dev, cap, nullptr, nullptr, nullptr, nullptr, W, R, words,
+                     slot_e, class_values, O, err, A);
+}
+
 // Batch assembly from the static store (one CTA per output graph).
 __global__ void __launch_bounds__(256)
 k_assemble(igmc_store_t S, const int64_t* __restrict__ idx, int B, igmc_batch_out_t O, int* err) {
@@ -970,6 +1090,57 @@ k_assemble(igmc_store_t S, const int64_t* __restrict__ idx, int B, igmc_batch_ou
 
 }  // namespace
 
+namespace {
+
+// h = 1 fast path (one launch) whenever its tables fit: ids in 12 bits, <= 32 rating classes, the user rows of one
+// subgraph within the tile table, two CTAs per SM worth of shared memory, scratch slot >= the edge bound.  Returns
+// the dynamic shared memory of k_extract_fast, 0 when the batch takes the generic path.
+size_t fast_smem(const igmc_csr_t* G, int B, int h, int cap, const igmc_extract_ws_t* W, int num_classes,
+                 int max_row_deg, const igmc_batch_out_t* O) {
+  static int fast_env = -1;
+  if (fast_env < 0) {
+    const char* e = getenv("IGMC_EXTRACT_FAST");
+    fast_env = e ? atoi(e) : 1;
+  }
+  const int R = num_classes;
+  const int words = (cap + 31) / 32;
+  const int slot_e = O->edge_cap / B;
+  const size_t smemF = fast_smem_ints(cap, R > 0 ? R : 1, words) * 4 + (((size_t)G->num_items * 2 + 15) & ~(size_t)15);
+  const long long rows_max = (long long)cap * (long long)(max_row_deg > 0 ? max_row_deg : G->num_items);
+  if (fast_env && h == 1 && W->sync && O->adj_in_ptr && R >= 1 && R <= FX_MAXR && cap <= FX_MAXCAP &&
+      rows_max <= (long long)FX_TILE * FX_TCAP && smemF <= 110 * 1024 && slot_e >= 2)
+    return smemF;
+  return 0;
+}
+
+// generic two-kernel path (any hop count / capacity): 1024-thread CTAs - the kernels are latency-bound, and more
+// threads per subgraph keep more independent loads in flight.
+int generic_threads() {
+  static int ex_threads = 0;
+  if (!ex_threads) {
+    const char* e = getenv("IGMC_EX_THREADS");
+    ex_threads = e ? atoi(e) : 1024;
+    if (ex_threads != 256 && ex_threads != 512 && ex_threads != 1024) ex_threads = 1024;
+  }
+  return ex_threads;
+}
+
+// the dynamic shared memory of the two generic kernels; false when the item table or the bitmaps do not fit
+bool generic_smem(const igmc_csr_t* G, int h, int cap, size_t* smemA, size_t* smemB) {
+  size_t a = (size_t)cap * sizeof(int) + (size_t)G->num_items * sizeof(uint16_t);
+  if (h > 1) {   // visited / candidate bitmaps + the fringe list of the larger side
+    const size_t wu = (G->num_users + 31) / 32, wv = (G->num_items + 31) / 32;
+    a = ((a + 15) & ~(size_t)15) + (wu + wv + (wu > wv ? wu : wv)) * 4 +
+        (size_t)(G->num_users > G->num_items ? G->num_users : G->num_items) * 4;
+    if (a > 220 * 1024) return false;
+  }
+  *smemA = a;
+  *smemB = 2 * (size_t)cap * sizeof(int) + (size_t)G->num_items * sizeof(uint16_t);
+  return *smemB <= 220 * 1024;   // else the item table does not fit in shared memory
+}
+
+}  // namespace
+
 extern "C" int igmc_extract_batch(const igmc_csr_t* G, const igmc_pairs_t* P, int B, int h, int max_nodes_per_hop,
                                   double sample_ratio, uint64_t seed, const uint64_t* seed_dev, int cap,
                                   const int32_t* inj_nodes_u, const int32_t* inj_nodes_v,
@@ -981,46 +1152,18 @@ extern "C" int igmc_extract_batch(const igmc_csr_t* G, const igmc_pairs_t* P, in
   if (h < 1 || h > IGMC_MAX_HOP) return -4;
   if (h > 1 && (inj_nodes_u || !W->hop_off)) return -4;   // injected node lists carry no hop boundaries
   cudaStream_t st = (cudaStream_t)stream;
-  {
-    // h = 1 fast path (one launch) whenever its tables fit: ids in 12 bits, <= 32 rating classes, the user rows of
-    // one subgraph within the tile table, two CTAs per SM worth of shared memory, scratch slot >= the edge bound
-    static int fast_env = -1;
-    if (fast_env < 0) {
-      const char* e = getenv("IGMC_EXTRACT_FAST");
-      fast_env = e ? atoi(e) : 1;
-    }
-    const int R = num_classes;
-    const int words = (cap + 31) / 32;
-    const int slot_e = O->edge_cap / B;
-    const size_t smemF = fast_smem_ints(cap, R > 0 ? R : 1, words) * 4 + (((size_t)G->num_items * 2 + 15) & ~(size_t)15);
-    const long long rows_max = (long long)cap * (long long)(max_row_deg > 0 ? max_row_deg : G->num_items);
-    if (fast_env && h == 1 && W->sync && O->adj_in_ptr && R >= 1 && R <= FX_MAXR && cap <= FX_MAXCAP &&
-        rows_max <= (long long)FX_TILE * FX_TCAP && smemF <= 110 * 1024 && slot_e >= 2) {
-      cudaFuncSetAttribute(k_extract_fast, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemF);
-      k_extract_fast<<<B, FX_THREADS, smemF, st>>>(*G, *P, B, max_nodes_per_hop, sample_ratio, seed, seed_dev, cap,
-                                                   inj_nodes_u, inj_nodes_v, inj_n_u, inj_n_v, *W, R, words, slot_e,
-                                                   class_values, *O, err);
-      IGMC_CUDA_CHECK_LAUNCH();
-      return 0;
-    }
+  const size_t smemF = fast_smem(G, B, h, cap, W, num_classes, max_row_deg, O);
+  if (smemF) {
+    cudaFuncSetAttribute(k_extract_fast, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemF);
+    k_extract_fast<<<B, FX_THREADS, smemF, st>>>(*G, *P, B, max_nodes_per_hop, sample_ratio, seed, seed_dev, cap,
+                                                 inj_nodes_u, inj_nodes_v, inj_n_u, inj_n_v, *W, num_classes,
+                                                 (cap + 31) / 32, O->edge_cap / B, class_values, *O, err);
+    IGMC_CUDA_CHECK_LAUNCH();
+    return 0;
   }
-  // generic two-kernel path (any hop count / capacity): 1024-thread CTAs - the kernels are latency-bound, and more
-  // threads per subgraph keep more independent loads in flight.
-  static int ex_threads = 0;
-  if (!ex_threads) {
-    const char* e = getenv("IGMC_EX_THREADS");
-    ex_threads = e ? atoi(e) : 1024;
-    if (ex_threads != 256 && ex_threads != 512 && ex_threads != 1024) ex_threads = 1024;
-  }
-  size_t smemA = (size_t)cap * sizeof(int) + (size_t)G->num_items * sizeof(uint16_t);
-  if (h > 1) {   // visited / candidate bitmaps + the fringe list of the larger side
-    const size_t wu = (G->num_users + 31) / 32, wv = (G->num_items + 31) / 32;
-    smemA = ((smemA + 15) & ~(size_t)15) + (wu + wv + (wu > wv ? wu : wv)) * 4 +
-            (size_t)(G->num_users > G->num_items ? G->num_users : G->num_items) * 4;
-    if (smemA > 220 * 1024) return -3;
-  }
-  const size_t smemB = 2 * (size_t)cap * sizeof(int) + (size_t)G->num_items * sizeof(uint16_t);
-  if (smemB > 220 * 1024) return -3;  // item table does not fit in shared memory
+  const int ex_threads = generic_threads();
+  size_t smemA, smemB;
+  if (!generic_smem(G, h, cap, &smemA, &smemB)) return -3;
   cudaFuncSetAttribute(k_extract_select_count, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemA);
   cudaFuncSetAttribute(k_extract_fill, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemB);
   k_extract_select_count<<<B, ex_threads, smemA, st>>>(*G, *P, B, max_nodes_per_hop, sample_ratio, seed, seed_dev, cap,
@@ -1030,6 +1173,43 @@ extern "C" int igmc_extract_batch(const igmc_csr_t* G, const igmc_pairs_t* P, in
   IGMC_CUDA_CHECK_LAUNCH();
   k_extract_fill<<<B, ex_threads, smemB, st>>>(*G, *P, B, cap, W->nodes_u, W->nodes_v, W->n_u, W->n_v,
                                                W->row_cnt, W->m_cnt, W->col_cnt, h, W->hop_off, class_values, *O, err);
+  IGMC_CUDA_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" int igmc_extract_sessions(const igmc_csr_t* G, const igmc_sessions_t* S, const int32_t* sess,
+                                     const igmc_pairs_t* P, int B, int h, int max_nodes_per_hop, double sample_ratio,
+                                     uint64_t seed, const uint64_t* seed_dev, int cap, const igmc_extract_ws_t* W,
+                                     const float* class_values, int num_classes, int max_row_deg,
+                                     const igmc_batch_out_t* O, int* err, void* stream) {
+  if (B <= 0) return 0;
+  if (!S || !S->users || !S->row_ptr || !sess) return -1;
+  if (cap < 1 || cap > 65534) return -2;
+  if (h < 1 || h > IGMC_MAX_HOP) return -4;
+  if (h > 1 && !W->hop_off) return -4;
+  cudaStream_t st = (cudaStream_t)stream;
+  const SessArg A = {*S, sess};
+  const size_t smemF = fast_smem(G, B, h, cap, W, num_classes, max_row_deg, O);
+  if (smemF) {
+    cudaFuncSetAttribute(k_extract_fast_sess, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemF);
+    k_extract_fast_sess<<<B, FX_THREADS, smemF, st>>>(*G, *P, B, max_nodes_per_hop, sample_ratio, seed, seed_dev, cap,
+                                                      *W, num_classes, (cap + 31) / 32, O->edge_cap / B, class_values,
+                                                      *O, err, A);
+    IGMC_CUDA_CHECK_LAUNCH();
+    return 0;
+  }
+  const int ex_threads = generic_threads();
+  size_t smemA, smemB;
+  if (!generic_smem(G, h, cap, &smemA, &smemB)) return -3;
+  cudaFuncSetAttribute(k_extract_select_count_sess, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemA);
+  cudaFuncSetAttribute(k_extract_fill_sess, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemB);
+  k_extract_select_count_sess<<<B, ex_threads, smemA, st>>>(*G, *P, B, max_nodes_per_hop, sample_ratio, seed,
+                                                            seed_dev, cap, W->nodes_u, W->nodes_v, W->n_u, W->n_v,
+                                                            W->row_cnt, W->m_cnt, W->col_cnt, h, W->hop_off, err, A);
+  IGMC_CUDA_CHECK_LAUNCH();
+  k_extract_fill_sess<<<B, ex_threads, smemB, st>>>(*G, *P, B, cap, W->nodes_u, W->nodes_v, W->n_u, W->n_v,
+                                                    W->row_cnt, W->m_cnt, W->col_cnt, h, W->hop_off, class_values,
+                                                    *O, err, A);
   IGMC_CUDA_CHECK_LAUNCH();
   return 0;
 }

@@ -16,25 +16,12 @@
 #include <cub/device/device_scan.cuh>
 
 #include "common.cuh"
+#include "row_merge.cuh"
 #include "../../include/igmc_b200.h"
 
 namespace {
 
 constexpr int THREADS = 256;
-
-enum : uint8_t { C_NOOP = 0, C_INSERT = 1, C_CHANGE = 2, C_DELETE = 3 };
-
-// packed (inserted, deleted) count: inserted in the high 32 bits, deleted in the low 32 (D < 2^31: a scan never carries)
-__device__ __forceinline__ long long pack_count(uint8_t c) {
-  return c == C_INSERT ? (1ll << 32) : c == C_DELETE ? 1ll : 0ll;
-}
-__device__ __forceinline__ long long net(long long p) { return (p >> 32) - (p & 0xffffffffll); }
-
-int bits_for(unsigned long long n) {   // radix-sort bits of keys in [0, n)
-  int b = 0;
-  while (b < 64 && (1ull << b) < n) ++b;
-  return b > 0 ? b : 1;
-}
 
 size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
 
@@ -127,15 +114,6 @@ __global__ void k_keys(const int32_t* __restrict__ u, const int32_t* __restrict_
   }
 }
 
-// first position in the ascending a[lo, hi) whose value is not below c (hi if none)
-__device__ __forceinline__ int find_col(const int32_t* __restrict__ a, int lo, int hi, int c) {
-  while (lo < hi) {
-    const int mid = (lo + hi) >> 1;
-    if (a[mid] < c) lo = mid + 1; else hi = mid;
-  }
-  return lo;
-}
-
 // entry i of the (u, v) order: keep the last of each equal-key run (the stable sort kept input order), classify it
 // against row u of G, its (v, u) sort key and the block's counts
 __global__ void k_classify(igmc_csr_t G, const int32_t* __restrict__ val, int D, int cap_items,
@@ -152,19 +130,13 @@ __global__ void k_classify(igmc_csr_t G, const int32_t* __restrict__ val, int D,
       const int a = (int)(k / cap_items), b = (int)(k % cap_items);
       uint8_t c = C_NOOP, l = 0;
       if (i == D - 1 || skey[i + 1] != k) {
-        const int x = val[spos[i]];
         int p = -1;
         if (a < G.num_users && b < G.num_items) {
           const int r0 = G.row_ptr[a], r1 = G.row_ptr[a + 1];
           const int q = find_col(G.col_idx, r0, r1, b);
           if (q < r1 && G.col_idx[q] == b) p = q;
         }
-        if (x > 0) {
-          l = (uint8_t)(x - 1);
-          c = p < 0 ? C_INSERT : (G.rating[p] != l ? C_CHANGE : C_NOOP);
-        } else if (p >= 0) {
-          c = C_DELETE;
-        }
+        c = classify(val[spos[i]], p, G.rating, &l);
       }
       cls[i] = c;
       lab[i] = l;
@@ -192,16 +164,6 @@ __global__ void k_gather_col(const int32_t* __restrict__ perm_c, const long long
                              long long* __restrict__ pk_vu) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i <= D; i += gridDim.x * blockDim.x)
     pk_vu[i] = i < D ? pk[perm_c[i]] : 0;
-}
-
-// the run [ds, de) of delta entries of every row (column) that has one; others keep the memset 0 / 0
-__global__ void k_runs(const long long* __restrict__ skey, int D, int stride, int32_t* __restrict__ ds,
-                       int32_t* __restrict__ de) {
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < D; i += gridDim.x * blockDim.x) {
-    const long long r = skey[i] / stride;
-    if (i == 0 || skey[i - 1] / stride != r) ds[r] = i;
-    if (i == D - 1 || skey[i + 1] / stride != r) de[r] = i + 1;
-  }
 }
 
 // new length of every row (column) r < cap: old length (0 at or past the current shape) + the run's net count, 0 past
@@ -244,11 +206,8 @@ __global__ void k_finalize(const long long* __restrict__ ptr_r, int cap_users, i
   H->err = err ? *err : 0;
 }
 
-// ---- apply ---------------------------------------------------------------------------------------------------------
-// One warp per new row (column) r: the old entries [o0, o1) and the delta run [ds, de) (ascending other-side id,
-// only the last entry of an equal-id group is kept) are merged into [n0, n0 + len).  Old entry j goes to
-// n0 + (j - o0) + (inserted - deleted entries of the run with a smaller id) unless it is deleted; an inserted entry
-// to n0 + (old entries with a smaller id) + the same count.
+// ---- apply ----------------------------------------------------------------------------------------------------------
+// One warp per new row (column) r: merge_row of its old entries and its delta run.
 template <bool RATING>
 __global__ void k_merge(const int32_t* __restrict__ ptr, const int32_t* __restrict__ idx,
                         const uint8_t* __restrict__ rating, int n_old, int n_new,
@@ -261,42 +220,8 @@ __global__ void k_merge(const int32_t* __restrict__ ptr, const int32_t* __restri
   const int warps = gridDim.x * (blockDim.x >> 5);
   for (int r = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); r < n_new; r += warps) {
     const int o0 = r < n_old ? ptr[r] : 0, o1 = r < n_old ? ptr[r + 1] : 0;
-    const int d0 = ds[r], d1 = de[r];
-    const long long n0 = ptr_new[r];
-    auto other = [&](int p) { return (int)(skey[p] % stride); };
-    auto clsof = [&](int p) { return perm ? cls[perm[p]] : cls[p]; };
-    if (d0 == d1) {            // untouched row: shifted only
-      for (int j = o0 + lane; j < o1; j += 32) {
-        out_idx[n0 + (j - o0)] = idx[j];
-        if (RATING) out_rating[n0 + (j - o0)] = rating[j];
-      }
-      continue;
-    }
-    const long long base = scan[d0];
-    for (int j = o0 + lane; j < o1; j += 32) {
-      const int c = idx[j];
-      int lo = d0, hi = d1;     // first delta entry with id >= c
-      while (lo < hi) {
-        const int mid = (lo + hi) >> 1;
-        if (other(mid) < c) lo = mid + 1; else hi = mid;
-      }
-      int last = lo;            // the kept (last) entry of the group with id c, if any
-      while (last + 1 < d1 && other(last + 1) == c) ++last;
-      uint8_t k = C_NOOP;
-      if (last < d1 && other(last) == c) k = clsof(last);
-      if (k == C_DELETE) continue;
-      const long long o = n0 + (j - o0) + net(scan[lo] - base);
-      out_idx[o] = c;
-      if (RATING) out_rating[o] = k == C_CHANGE ? lab[last] : rating[j];
-    }
-    for (int p = d0 + lane; p < d1; p += 32) {
-      if (clsof(p) != C_INSERT) continue;
-      const int c = other(p);
-      const int q = find_col(idx, o0, o1, c) - o0;
-      const long long o = n0 + q + net(scan[p] - base);
-      out_idx[o] = c;
-      if (RATING) out_rating[o] = lab[p];
-    }
+    merge_row<RATING>(idx, rating, o0, o1, ds[r], de[r], ptr_new[r], skey, stride, cls, lab, perm, scan, out_idx,
+                      out_rating, lane);
   }
 }
 

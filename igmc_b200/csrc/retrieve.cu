@@ -59,10 +59,13 @@ __device__ __forceinline__ int block_excl_count(bool f, int* wsum, int* total) {
   return r;
 }
 
-__global__ void __launch_bounds__(THREADS)
-k_corated(igmc_csr_t G, const int32_t* __restrict__ users, int U, int m, int exclude_rated, int in_shared,
-          unsigned char* __restrict__ ws, size_t ws_row, int32_t* __restrict__ out_items,
-          int32_t* __restrict__ out_paths, int* err) {
+// SESS: query j is session j of Q (igmc_sessions_t): N(u) is its session row, u = Q.users[j] its real id (a new
+// user, u >= num_users, is in no column of G and is never looked up in w)
+template <bool SESS>
+__device__ __forceinline__ void
+corated(const igmc_csr_t& G, const int32_t* __restrict__ users, int U, int m, int exclude_rated, int in_shared,
+        unsigned char* __restrict__ ws, size_t ws_row, int32_t* __restrict__ out_items, int32_t* __restrict__ out_paths,
+        int* err, const igmc_sessions_t& Q) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   __shared__ int hist[256];
   __shared__ int wsum[WARPS + 1];
@@ -78,8 +81,8 @@ k_corated(igmc_csr_t G, const int32_t* __restrict__ users, int U, int m, int exc
   for (int j = blockIdx.x; j < U; j += gridDim.x) {
     int32_t* oi = out_items + (size_t)j * m;
     int32_t* op = out_paths + (size_t)j * m;
-    const int u = users[j];
-    if (u < 0 || u >= nu) {
+    const int u = SESS ? Q.users[j] : users[j];
+    if (!SESS && (u < 0 || u >= nu)) {
       if (threadIdx.x == 0) igmc_set_err(err, IGMC_ERR_CANDIDATES);
       for (int r = threadIdx.x; r < m; r += THREADS) {
         oi[r] = -1;
@@ -90,9 +93,10 @@ k_corated(igmc_csr_t G, const int32_t* __restrict__ users, int U, int m, int exc
     for (int x = threadIdx.x; x < nu; x += THREADS) w[x] = 0;
     __syncthreads();
     // pass 1: user overlap, a warp per rated item
-    const int r0 = G.row_ptr[u], r1 = G.row_ptr[u + 1];
+    const int32_t* qi = SESS ? Q.col_idx : G.col_idx;
+    const int r0 = SESS ? Q.row_ptr[j] : G.row_ptr[u], r1 = SESS ? Q.row_ptr[j + 1] : G.row_ptr[u + 1];
     for (int e = r0 + warp; e < r1; e += WARPS) {
-      const int i = G.col_idx[e];
+      const int i = qi[e];
       for (int q = G.col_ptr[i] + lane; q < G.col_ptr[i + 1]; q += 32) {
         const int v = G.row_idx[q];
         if (v != u) atomicAdd(&w[v], 1u);
@@ -109,7 +113,7 @@ k_corated(igmc_csr_t G, const int32_t* __restrict__ users, int U, int m, int exc
     }
     __syncthreads();
     if (exclude_rated)
-      for (int e = r0 + threadIdx.x; e < r1; e += THREADS) paths[G.col_idx[e]] = 0;
+      for (int e = r0 + threadIdx.x; e < r1; e += THREADS) paths[qi[e]] = 0;
     // select: threshold T and the number `need` of ties at T to take (ascending item order); every count > T is taken
     unsigned prefix = 0, mask = 0;
     int need = m;
@@ -191,6 +195,20 @@ k_corated(igmc_csr_t G, const int32_t* __restrict__ users, int U, int m, int exc
   }
 }
 
+__global__ void __launch_bounds__(THREADS)
+k_corated(igmc_csr_t G, const int32_t* __restrict__ users, int U, int m, int exclude_rated, int in_shared,
+          unsigned char* __restrict__ ws, size_t ws_row, int32_t* __restrict__ out_items,
+          int32_t* __restrict__ out_paths, int* err) {
+  corated<false>(G, users, U, m, exclude_rated, in_shared, ws, ws_row, out_items, out_paths, err, igmc_sessions_t{});
+}
+
+__global__ void __launch_bounds__(THREADS)
+k_corated_sess(igmc_csr_t G, igmc_sessions_t Q, int m, int exclude_rated, int in_shared,
+               unsigned char* __restrict__ ws, size_t ws_row, int32_t* __restrict__ out_items,
+               int32_t* __restrict__ out_paths, int* err) {
+  corated<true>(G, nullptr, Q.num_sessions, m, exclude_rated, in_shared, ws, ws_row, out_items, out_paths, err, Q);
+}
+
 }  // namespace
 
 extern "C" int igmc_corated_ws_bytes(int num_users, int num_items, int num_query, int m, int64_t* bytes) {
@@ -224,6 +242,31 @@ extern "C" int igmc_corated_items(const igmc_csr_t* G, const int32_t* users, int
   k_corated<<<grid, THREADS, smem, (cudaStream_t)stream>>>(*G, users, num_query, m, exclude_rated ? 1 : 0,
                                                            shared ? 1 : 0, static_cast<unsigned char*>(ws), row, items,
                                                            paths, err);
+  IGMC_CUDA_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" int igmc_corated_sessions(const igmc_csr_t* G, const igmc_sessions_t* S, int m, int exclude_rated,
+                                     void* ws, int64_t ws_bytes, int32_t* items, int32_t* paths, int* err,
+                                     void* stream) {
+  if (!G || !S || S->num_sessions < 0 || m < 1 || m > G->num_items) return -1;
+  const int U = S->num_sessions;
+  if (U == 0) return 0;
+  if (!S->users || !S->row_ptr || !items || !paths) return -1;
+  const int nu = G->num_users, ni = G->num_items;
+  const size_t row = row_bytes(nu, ni, m);
+  const bool shared = fits_shared(nu, ni, m);
+  int grid = U;
+  if (!shared) {
+    grid = U < GLOBAL_CTAS ? U : GLOBAL_CTAS;
+    if (!ws || ws_bytes < (int64_t)grid * (int64_t)row) return -2;
+  }
+  const size_t smem = shared ? row : 0;
+  if (smem > 48 * 1024)
+    cudaFuncSetAttribute(k_corated_sess, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  k_corated_sess<<<grid, THREADS, smem, (cudaStream_t)stream>>>(*G, *S, m, exclude_rated ? 1 : 0, shared ? 1 : 0,
+                                                                static_cast<unsigned char*>(ws), row, items, paths,
+                                                                err);
   IGMC_CUDA_CHECK_LAUNCH();
   return 0;
 }

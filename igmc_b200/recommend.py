@@ -22,6 +22,11 @@ building a dataset of every candidate pair and looping over it in Python.  Here:
   smallest TracIn-CP influence, ``self_influence(model, graph, train)`` -> sum_k eta_k ||grad l_i||^2
   (csrc/influence.cu): a per-graph gradient assembly after the training backward, a split-K GEMM of the conv blocks
   plus the readout's rank-1 factors, and a streaming top-k merge;
+* ``RatingSessions(graph, users, session, items, values)`` -> users described by ratings passed with the query: per
+  session a user id (new ids start from an empty row) and edits to that user's row in ``RatingGraph.update``'s
+  encoding, applied only while that user's own pairs are scored; ``predict_sessions``, ``recommend_sessions`` and
+  ``corated_items_sessions`` score, rank and retrieve for many sessions in one run and leave the graph unchanged.  A
+  session's results are bit for bit those of the graph functions on the graph with that session's edits applied;
 * ``InferenceEngine``: the pipelined, graph-replayed loop behind all of them.  Per step the side stream produces the next
   batch's candidate pairs (``igmc_candidate_pairs``, from a device cursor) and extracts it while the main stream runs
   the eval forward of the current batch (once per checkpoint) and merges its scores into the running per-user top-k
@@ -44,7 +49,8 @@ from .train_eval import replay_step
 from .util_functions import RatingGraph, SubgraphExtractor, _stream_ptr
 
 __all__ = ["predict_pairs", "recommend", "corated_items", "explain_pairs", "Explanation", "attribute_pairs",
-           "Attribution", "pair_gradients", "influence", "self_influence", "Influence", "InferenceEngine"]
+           "Attribution", "pair_gradients", "influence", "self_influence", "Influence", "InferenceEngine",
+           "RatingSessions", "predict_sessions", "recommend_sessions", "corated_items_sessions"]
 
 
 # ---- input validation (host) ----------------------------------------------------------------------------------------
@@ -487,6 +493,168 @@ def edge_grad_scatter_host(edge_ptr, tag, edge_grad, offsets, out, k=0, K=1):
     return out
 
 
+# ---- rating sessions (csrc/session.cu) ------------------------------------------------------------------------------
+def session_rows_host(host, shape, users, session, items, values):
+    """numpy twin of igmc_session_plan + _apply: (row_ptr [S+1], col_idx, rating) of the merged session rows.  Restates
+    the kernels' steps: the base row of every session (the graph row of users[s], empty for a new user), the stable
+    (session, item) order, the last edit of a run kept, classification against the base row and the merge of
+    ``graph_update_host``."""
+    from .util_functions import _merge_side_host
+    users = np.asarray(users, np.int64).reshape(-1)
+    session, items, values = (np.asarray(a, np.int64).reshape(-1) for a in (session, items, values))
+    nu, _ = shape
+    rp, ci, rt = (np.asarray(host[k], np.int64) for k in ("row_ptr", "col_idx", "rating"))
+    S = len(users)
+    base = [np.arange(rp[u], rp[u + 1]) if u < nu else np.zeros(0, np.int64) for u in users]
+    bptr = np.concatenate([[0], np.cumsum([len(b) for b in base])]).astype(np.int64)
+    bpos = np.concatenate(base).astype(np.int64) if S else np.zeros(0, np.int64)
+    bidx, brt = ci[bpos], rt[bpos]
+    if len(session) == 0:                                        # no edits: the base rows
+        return bptr.astype(np.int32), bidx.astype(np.int32), brt.astype(np.uint8)
+    o = np.lexsort((items, session))                             # stable
+    sa, sb, sx = session[o], items[o], values[o]
+    keep = np.r_[(sa[1:] != sa[:-1]) | (sb[1:] != sb[:-1]), True] if len(o) else np.zeros(0, bool)
+    cls = np.zeros(len(o), np.int64)                             # 0 no-op, 1 insert, 2 change, 3 delete
+    lab = np.zeros(len(o), np.int64)
+    for i in np.flatnonzero(keep):
+        a, b, x = sa[i], sb[i], sx[i]
+        row = bidx[bptr[a]:bptr[a + 1]]
+        q = int(np.searchsorted(row, b))
+        p = bptr[a] + q if q < len(row) and row[q] == b else -1
+        if x > 0:
+            lab[i] = x - 1
+            cls[i] = 1 if p < 0 else (2 if brt[p] != x - 1 else 0)
+        elif p >= 0:
+            cls[i] = 3
+    new_rp, new_ci, new_rt = _merge_side_host(bptr, bidx, brt, S, S, sa, sb, cls, lab)
+    return new_rp.astype(np.int32), new_ci.astype(np.int32), new_rt.astype(np.uint8)
+
+
+def _session_inputs(S, num_items, session, items, values):
+    """(session, items, values, D) of the edits: host arrays validated here (IndexError for a session or item id
+    out of range, ValueError for a value outside 0..256 or unequal lengths); int32 device tensors are passed on and
+    checked by the kernel"""
+    arrs = []
+    for name, a in (("session", session), ("items", items), ("values", values)):
+        if torch.is_tensor(a) and a.device.type == "cuda":
+            if a.is_floating_point() or a.is_complex() or a.dtype == torch.bool:
+                raise TypeError("%s must be integers, not %s" % (name, a.dtype))
+            arrs.append(a.reshape(-1))
+            continue
+        a = np.asarray(a.cpu().numpy() if torch.is_tensor(a) else a).reshape(-1)
+        if a.size and not np.issubdtype(a.dtype, np.integer):
+            raise TypeError("%s must be integers, not %s" % (name, a.dtype))
+        arrs.append(a.astype(np.int64))
+    n = [int(a.numel()) if torch.is_tensor(a) else len(a) for a in arrs]
+    if len(set(n)) != 1:
+        raise ValueError("session, items and values must have the same length (%d, %d, %d)" % tuple(n))
+    for a, name, hi in ((arrs[0], "session", S), (arrs[1], "items", num_items)):
+        if not torch.is_tensor(a) and a.size and (a.min() < 0 or a.max() >= hi):
+            bad = int(a.min()) if a.min() < 0 else int(a.max())
+            raise IndexError("%s: id %d out of range [0, %d)" % (name, bad, hi))
+    x = arrs[2]
+    if not torch.is_tensor(x) and x.size and (x.min() < 0 or x.max() > 256):
+        raise ValueError("values must be rating label + 1 (1..256) or 0 (delete), got %d"
+                         % (int(x.min()) if x.min() < 0 else int(x.max())))
+    return arrs[0], arrs[1], arrs[2], n[0]
+
+
+class RatingSessions(object):
+    """Users described by ratings passed with the query, scored without changing the rating graph.
+
+    Session s is user ``users[s]`` with the edits ``(session[i] == s, items[i], values[i])`` applied to that user's
+    row only: ``value`` = rating label + 1 (1..256) inserts or overwrites, 0 deletes (an absent rating: nothing), the
+    last occurrence of (s, item) wins.  Ids below ``graph.num_users`` start from that user's graph row, larger ids are
+    new users and start from an empty row; two sessions may share an id.  Items must exist.  The merged rows are one
+    device CSR of S rows (``row_ptr``, ``col_idx`` ascending, ``rating``), built by csrc/session.cu with one host
+    synchronisation (total length and longest row).  Host arrays are validated here (IndexError for ids, ValueError
+    for values and lengths); int32 device tensors are checked by the kernel (RuntimeError).  The sessions belong to the
+    graph as it was when they were built: using them after ``graph.update`` raises RuntimeError."""
+
+    def __init__(self, graph, users, session=(), items=(), values=()):
+        if not isinstance(graph, RatingGraph):
+            raise TypeError("sessions are built on a RatingGraph")
+        if graph.device is None:
+            raise RuntimeError("igmc_b200 rating sessions run on a CUDA device (there is no CPU path)")
+        self.graph, dev = graph, graph.device
+        if torch.is_tensor(users) and users.device.type == "cuda":
+            u = users.reshape(-1).clamp(-1, 2 ** 31 - 1).to(torch.int32).contiguous()
+        else:
+            u = _host_ids(users, "users", 2 ** 31 - 1)
+            u = torch.from_numpy(u.astype(np.int32)).to(dev)
+        S = int(u.numel())
+        if S < 1:
+            raise ValueError("a RatingSessions holds at least one session")
+        sess, it, val, D = _session_inputs(S, graph.num_items, session, items, values)
+        sess, it, val = (_on_dev_i32(a, dev) for a in (sess, it, val))
+        lib = _lib.load()
+        nbytes = C.c_int64(0)
+        _lib.check(lib.igmc_session_ws_bytes(S, D, graph.num_items, C.byref(nbytes)), "igmc_session_ws_bytes")
+        ws = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=dev)
+        header = torch.zeros(2, dtype=torch.int64, device=dev)
+        err = torch.zeros(1, dtype=torch.int32, device=dev)
+        _lib.check(lib.igmc_session_plan(C.byref(graph._c), u.data_ptr(), S, _lib.ptr(sess), _lib.ptr(it),
+                                         _lib.ptr(val), D, ws.data_ptr(), ws.numel(), header.data_ptr(),
+                                         err.data_ptr(), _stream_ptr()), "igmc_session_plan")
+        hv = torch.cat([header, err.to(torch.int64)]).cpu().numpy()      # the build's one host synchronisation
+        _lib.check_kernel_error(int(hv[2]))
+        self.nnz, self.max_row_deg = int(hv[0]), int(hv[1])
+        if self.nnz > 2 ** 31 - 1:
+            raise ValueError("the session rows hold %d ratings, beyond int32" % self.nnz)
+        self.users = u
+        self.row_ptr = torch.empty(S + 1, dtype=torch.int32, device=dev)
+        self.col_idx = torch.empty(max(self.nnz, 1), dtype=torch.int32, device=dev)
+        self.rating = torch.empty(max(self.nnz, 1), dtype=torch.uint8, device=dev)
+        _lib.check(lib.igmc_session_apply(C.byref(graph._c), u.data_ptr(), S, D, ws.data_ptr(), ws.numel(),
+                                          self.row_ptr.data_ptr(), self.col_idx.data_ptr(), self.rating.data_ptr(),
+                                          _stream_ptr()), "igmc_session_apply")
+        self.num_sessions = S
+        self.version = graph.version
+        self._c = _lib.Sessions(u.data_ptr(), self.row_ptr.data_ptr(), self.col_idx.data_ptr(),
+                                self.rating.data_ptr(), S, self.max_row_deg)
+        # the session rows as a CSR over query slots 0..S-1 (no columns): what the candidate kernels read
+        self._view = _lib.CSR(self.row_ptr.data_ptr(), self.col_idx.data_ptr(), self.rating.data_ptr(), None, None,
+                              S, graph.num_items)
+        self._slots = torch.arange(S, dtype=torch.int32, device=dev)
+
+    def __len__(self):
+        return self.num_sessions
+
+    def check(self, graph=None):
+        """RuntimeError unless the sessions belong to ``graph`` (default: their own) as it is now"""
+        if graph is not None and graph is not self.graph:
+            raise ValueError("the sessions were built on another RatingGraph")
+        if self.graph.version != self.version:
+            raise RuntimeError("the rating graph was updated after these sessions were built: their base rows are "
+                               "gone; build the sessions again")
+
+    def rows(self):
+        """host copies (row_ptr [S+1], col_idx [nnz], rating [nnz]) of the merged rows"""
+        n = self.nnz
+        return (self.row_ptr.cpu().numpy(), self.col_idx[:n].cpu().numpy(), self.rating[:n].cpu().numpy())
+
+
+def _on_dev_i32(a, dev):
+    if torch.is_tensor(a) and a.device.type == "cuda":
+        return (a if a.dtype == torch.int32 else a.clamp(-1, 2 ** 31 - 1).to(torch.int32)).contiguous()
+    return torch.from_numpy(np.clip(np.asarray(a, np.int64), -1, 2 ** 31 - 1).astype(np.int32)).to(dev)
+
+
+def _corated_sessions(lib, sessions, m, exclude_rated, err, ws):
+    """igmc_corated_sessions: (items, paths) [S, m] int32"""
+    g, S, dev = sessions.graph, sessions.num_sessions, sessions.graph.device
+    nbytes = C.c_int64(0)
+    _lib.check(lib.igmc_corated_ws_bytes(g.num_users, g.num_items, S, m, C.byref(nbytes)), "igmc_corated_ws_bytes")
+    if ws.get("ws") is None or ws["ws"].numel() < nbytes.value:
+        ws["ws"] = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=dev)
+    items = torch.empty(S, m, dtype=torch.int32, device=dev)
+    paths = torch.empty(S, m, dtype=torch.int32, device=dev)
+    _lib.check(lib.igmc_corated_sessions(C.byref(g._c), C.byref(sessions._c), m, int(bool(exclude_rated)),
+                                         ws["ws"].data_ptr(), ws["ws"].numel(), items.data_ptr(), paths.data_ptr(),
+                                         err.data_ptr(), _stream_ptr()), "igmc_corated_sessions")
+    return items, paths
+
+
 # ---- the engine -----------------------------------------------------------------------------------------------------
 class InferenceEngine(object):
     """Pipelined, graph-replayed scoring of candidate pairs (module docstring).  ``checkpoints``: state_dict files of
@@ -587,7 +755,7 @@ class InferenceEngine(object):
         Cd.rated_off, Cd.rated_pos = _lib.ptr(run.get("rated_off")), _lib.ptr(run.get("rated_pos"))
         Cd.num_query, Cd.num_cand = U, 0 if cand is None else len(cand)
         Cd.exclude_rated = int(bool(exclude_rated))
-        _lib.check(self.lib.igmc_candidate_plan(C.byref(g._c), C.byref(Cd), self.extractor.err.data_ptr(),
+        _lib.check(self.lib.igmc_candidate_plan(C.byref(self._csr(run)), C.byref(Cd), self.extractor.err.data_ptr(),
                                                 _stream_ptr()), "igmc_candidate_plan")
         Cd.num_pairs = run["P"] = int(run["user_off"][U].item())
         run["Cd"] = Cd
@@ -612,7 +780,7 @@ class InferenceEngine(object):
         Cd = _lib.Candidates()
         Cd.users, Cd.user_off = run["users"].data_ptr(), run["user_off"].data_ptr()
         Cd.num_query, Cd.exclude_rated = U, int(bool(exclude_rated))
-        _lib.check(self.lib.igmc_candidate_lists(C.byref(g._c), C.byref(Cd), rows.data_ptr(), width,
+        _lib.check(self.lib.igmc_candidate_lists(C.byref(self._csr(run)), C.byref(Cd), rows.data_ptr(), width,
                                                  run["lists"].data_ptr(), run["lists_ws"].data_ptr(),
                                                  run["lists_ws"].numel(), err.data_ptr(), _stream_ptr()),
                    "igmc_candidate_lists")
@@ -626,6 +794,90 @@ class InferenceEngine(object):
     def start_pairs(self, users, items):
         """plan a run over the explicit pairs (users[i], items[i]).  Returns their number."""
         return self._start_explicit("pairs", users, items)
+
+    # ---- rating sessions ----------------------------------------------------------------------------------------
+    def _csr(self, run):
+        """the rows the candidate kernels read: the graph's, or a session run's rows as a CSR over its sessions"""
+        return run["sessions"]._view if run.get("sessions") is not None else self.graph._c
+
+    def _check_sessions(self, sessions):
+        if not isinstance(sessions, RatingSessions):
+            raise TypeError("sessions must be a RatingSessions")
+        sessions.check(self.graph)
+        for s in self.slots:
+            if "sess" not in s:
+                s["sess"] = torch.zeros(self.B, dtype=torch.int32, device=self.dev)
+        return sessions
+
+    def start_session_pairs(self, sessions, session, items):
+        """plan a run over the pairs (sessions.users[session[i]], items[i]), each scored with its target user's row
+        taken from session ``session[i]`` (``predict_sessions``).  Returns their number."""
+        sessions = self._check_sessions(sessions)
+        g = self.graph
+        sess = _host_ids(session, "session", sessions.num_sessions)
+        items = _host_ids(items, "items", g.num_items)
+        if len(sess) != len(items):
+            raise ValueError("session and items must have the same length (%d vs %d)" % (len(sess), len(items)))
+        P, dev = len(sess), self.dev
+        run = dict(kind="pairs", P=P, version=g.version, sessions=sessions,
+                   scores=torch.empty(P, dtype=torch.float32, device=dev))
+        self.run = run
+        if P == 0:
+            return 0
+        run["pu"] = torch.from_numpy(sess.astype(np.int32)).to(dev)
+        run["pv"] = torch.from_numpy(items.astype(np.int32)).to(dev)
+        Cd = _lib.Candidates()
+        Cd.pair_u, Cd.pair_v, Cd.num_pairs = run["pu"].data_ptr(), run["pv"].data_ptr(), P
+        run["Cd"] = Cd
+        self._prime()
+        return P
+
+    def start_session_recommend(self, sessions, k, items=None, exclude_rated=True, retrieve=None):
+        """plan a ranking run over the sessions (``recommend_sessions``): query slot s is session s, its candidates and
+        rated items come from its session row.  Arguments as ``start_recommend``'s.  Returns the number of candidate
+        pairs."""
+        k = _check_k(k)
+        sessions = self._check_sessions(sessions)
+        g = self.graph
+        if retrieve is not None and items is not None:
+            raise ValueError("retrieve= chooses the candidates itself: pass it without items=")
+        per_user = retrieve is not None or _is_rows(items)
+        m = None if retrieve is None else _check_m(retrieve, g.num_items)
+        S, dev = sessions.num_sessions, self.dev
+        cand = None if items is None or per_user else np.unique(_host_ids(items, "items", g.num_items))
+        rows = _user_rows(items, S, g.num_items, dev) if per_user and m is None else None
+        run = dict(kind="recommend", U=S, k=k, version=g.version, sessions=sessions,
+                   top_s=torch.full((S, k), -float("inf"), dtype=torch.float32, device=dev),
+                   top_i=torch.full((S, k), -1, dtype=torch.int64, device=dev))
+        self.run = run
+        if (cand is not None and len(cand) == 0) or (rows is not None and rows.shape[1] == 0):
+            run["P"] = 0
+            return 0
+        run["users"] = sessions._slots
+        if per_user:
+            if rows is None:
+                rows, _ = _corated_sessions(self.lib, sessions, m, exclude_rated, self.extractor.err,
+                                            self._retrieve_ws)
+            return self._plan_lists(run, rows, None, exclude_rated)
+        i64 = dict(dtype=torch.int64, device=dev)
+        run["cand"] = None if cand is None else torch.from_numpy(cand.astype(np.int32)).to(dev)
+        run["user_off"] = torch.zeros(S + 1, **i64)
+        if cand is not None and exclude_rated:
+            run["rated_off"] = torch.zeros(S + 1, **i64)
+            run["rated_pos"] = torch.zeros(max(sessions.nnz, 1), dtype=torch.int32, device=dev)
+        Cd = _lib.Candidates()
+        Cd.users, Cd.cand = run["users"].data_ptr(), _lib.ptr(run["cand"])
+        Cd.user_off = run["user_off"].data_ptr()
+        Cd.rated_off, Cd.rated_pos = _lib.ptr(run.get("rated_off")), _lib.ptr(run.get("rated_pos"))
+        Cd.num_query, Cd.num_cand = S, 0 if cand is None else len(cand)
+        Cd.exclude_rated = int(bool(exclude_rated))
+        _lib.check(self.lib.igmc_candidate_plan(C.byref(sessions._view), C.byref(Cd), self.extractor.err.data_ptr(),
+                                                _stream_ptr()), "igmc_candidate_plan")
+        Cd.num_pairs = run["P"] = int(run["user_off"][S].item())
+        run["Cd"] = Cd
+        if run["P"] > 0:
+            self._prime()
+        return run["P"]
 
     def start_explain(self, users, items, m=None):
         """plan an explanation run over the explicit pairs (users[i], items[i]) (``explain_pairs``): the base pass
@@ -871,6 +1123,8 @@ class InferenceEngine(object):
         its buffers, its candidate total and the graph's shape as it was; the extractor follows an updated graph).
         ``total``: the positions of the pass (default: the run's pairs)."""
         run = self.run
+        sessions = run.get("sessions")
+        self.extractor.serve_sessions(sessions.max_row_deg if sessions is not None else 0)
         run["steps"] = ((run["P"] if total is None else total) + self.B - 1) // self.B
         run["done"] = 0
         self.graphs, self.eager_done = {}, set()
@@ -893,12 +1147,19 @@ class InferenceEngine(object):
                                                      s["v"].data_ptr(), s["pid"].data_ptr(), s["tag"].data_ptr(),
                                                      s["j"].data_ptr(), err, _stream_ptr()), "igmc_occlusion_pairs")
         else:
-            _lib.check(self.lib.igmc_candidate_pairs(C.byref(self.graph._c), C.byref(run["Cd"]),
+            _lib.check(self.lib.igmc_candidate_pairs(C.byref(self._csr(run)), C.byref(run["Cd"]),
                                                      self.cursor.data_ptr(), self.B, s["u"].data_ptr(),
                                                      s["v"].data_ptr(), s["pid"].data_ptr(), s["tag"].data_ptr(), err,
                                                      _stream_ptr()), "igmc_candidate_pairs")
+        sessions = run.get("sessions")
+        if sessions is not None:
+            # links_u holds the session: to the session's user id, its pair id and the per-pair session index
+            _lib.check(self.lib.igmc_session_pairs(C.byref(sessions._c), self.graph.num_items, self.B,
+                                                   s["u"].data_ptr(), s["v"].data_ptr(), s["pid"].data_ptr(),
+                                                   s["sess"].data_ptr(), err, _stream_ptr()), "igmc_session_pairs")
         b = self.batches[slot] = self.extractor.extract(pairs=(s["u"], s["v"], None), pair_ids=s["pid"], reuse=True,
-                                                        slot=slot)
+                                                        slot=slot, sessions=sessions,
+                                                        sess=None if sessions is None else s["sess"])
         if occlude:
             _lib.check(self.lib.igmc_occlusion_mask(C.byref(b._lazy["_c"]), self.B, s["tag"].data_ptr(),
                                                     s["j"].data_ptr(), s["keep"].data_ptr(), run["user"].data_ptr(),
@@ -1067,6 +1328,14 @@ class InferenceEngine(object):
 
     def predict_pairs(self, users, items):
         self.start_pairs(users, items)
+        return self.finish()
+
+    def predict_sessions(self, sessions, session, items):
+        self.start_session_pairs(sessions, session, items)
+        return self.finish()
+
+    def recommend_sessions(self, sessions, k, items=None, exclude_rated=True, retrieve=None):
+        self.start_session_recommend(sessions, k, items, exclude_rated, retrieve)
         return self.finish()
 
     def explain_pairs(self, users, items, m=None):
@@ -1292,5 +1561,76 @@ def corated_items(graph, users, m, exclude_rated=True):
     lib = _lib.load()
     err = torch.zeros(1, dtype=torch.int32, device=g.device)
     items, paths = _corated(lib, g, torch.from_numpy(users.astype(np.int32)).to(g.device), m, exclude_rated, err, {})
+    _lib.check_kernel_error(int(err.item()))
+    return items, paths
+
+
+# ---- rating sessions: public API ------------------------------------------------------------------------------------
+def predict_sessions(model, sessions, session, items, *, h=1, sample_ratio=1.0, max_nodes_per_hop=None,
+                     batch_size=256, checkpoints=None, sample_seed=0):
+    """eval-mode scores [P] (fp32, on the model's device) of the pairs (sessions.users[session[i]], items[i]), each
+    with its target user's row taken from session ``session[i]`` (``RatingSessions``) and every other row and column
+    from the graph, which is not changed.  Bit for bit ``predict_pairs`` of the same pair on the graph with that
+    session's edits applied (same kernel plan and batch size); pair ids stay u * num_items + v.  Keywords as
+    ``predict_pairs``'."""
+    if not isinstance(sessions, RatingSessions):
+        raise TypeError("sessions must be a RatingSessions")
+    sessions.check()
+    sess = _host_ids(session, "session", sessions.num_sessions)
+    items = _host_ids(items, "items", sessions.graph.num_items)
+    if len(sess) != len(items):
+        raise ValueError("session and items must have the same length (%d vs %d)" % (len(sess), len(items)))
+    if len(sess) == 0:
+        return torch.zeros(0, dtype=torch.float32, device=model.flat_params.device)
+    eng = InferenceEngine(model, sessions.graph, h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints,
+                          sample_seed)
+    try:
+        return eng.predict_sessions(sessions, sess, items)
+    finally:
+        eng.close()
+
+
+def recommend_sessions(model, sessions, k, *, items=None, exclude_rated=True, retrieve=None, h=1, sample_ratio=1.0,
+                       max_nodes_per_hop=None, batch_size=256, checkpoints=None, sample_seed=0):
+    """per session the ``k`` best candidate items: (top_items [S, k] int64, top_scores [S, k] fp32), row s for
+    session s.  Candidates and order as ``recommend``'s, with the session row as the user's ratings (``exclude_rated``,
+    ``retrieve=M``); a 2-D ``items`` has one row per session.  Row s is bit for bit ``recommend`` for sessions.users[s]
+    on the graph with session s's edits applied (same kernel plan and batch size); the graph is not changed."""
+    k = _check_k(k)
+    if not isinstance(sessions, RatingSessions):
+        raise TypeError("sessions must be a RatingSessions")
+    sessions.check()
+    ni, S = sessions.graph.num_items, sessions.num_sessions
+    if retrieve is not None and items is not None:
+        raise ValueError("retrieve= chooses the candidates itself: pass it without items=")
+    if retrieve is not None:
+        _check_m(retrieve, ni)
+    if _is_rows(items):
+        if torch.is_tensor(items) and items.device.type == "cuda":
+            if items.shape[0] != S:
+                raise ValueError("items has %d rows, one per session is %d" % (items.shape[0], S))
+        else:
+            items = _user_rows(items, S, ni, torch.device("cpu")).numpy()
+    elif items is not None:
+        items = _host_ids(items, "items", ni)
+    eng = InferenceEngine(model, sessions.graph, h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints,
+                          sample_seed)
+    try:
+        return eng.recommend_sessions(sessions, k, items, exclude_rated, retrieve)
+    finally:
+        eng.close()
+
+
+def corated_items_sessions(sessions, m, exclude_rated=True):
+    """``corated_items`` for sessions: per session the ``m`` items with the most bridges to its user, with N(u) the
+    session row (and ``exclude_rated`` dropping its items) and the columns from the graph: (items [S, m], paths
+    [S, m]) int32, row s bit for bit ``corated_items`` for sessions.users[s] on the graph with session s's edits
+    applied.  One host synchronisation (the error word)."""
+    if not isinstance(sessions, RatingSessions):
+        raise TypeError("sessions must be a RatingSessions")
+    sessions.check()
+    m = _check_m(m, sessions.graph.num_items)
+    err = torch.zeros(1, dtype=torch.int32, device=sessions.graph.device)
+    items, paths = _corated_sessions(_lib.load(), sessions, m, exclude_rated, err, {})
     _lib.check_kernel_error(int(err.item()))
     return items, paths

@@ -157,10 +157,12 @@ class RatingGraph(object):
                            self.dev["rating"].data_ptr(), self.dev["col_ptr"].data_ptr(),
                            self.dev["row_idx"].data_ptr(), self.num_users, self.num_items)
 
-    def node_cap(self, max_nodes_per_hop, h=1):
+    def node_cap(self, max_nodes_per_hop, h=1, max_row_deg=None):
         """capacity of one side's node list: target + per hop min(mnph, largest possible fringe) (hop 1: a row or
-        a column of the matrix; later hops: up to the whole side)."""
-        d = max(self.max_row_deg, self.max_col_deg)
+        a column of the matrix; later hops: up to the whole side).  ``max_row_deg``: the longest target row when it
+        may be longer than the graph's (rating sessions)."""
+        d = max(self.max_row_deg if max_row_deg is None else max(self.max_row_deg, int(max_row_deg)),
+                self.max_col_deg)
         side = max(self.num_users, self.num_items)
         if max_nodes_per_hop is not None:
             d = min(d, int(max_nodes_per_hop))
@@ -617,6 +619,7 @@ class SubgraphExtractor(_BatchWriter):
         self.links_v = torch.as_tensor(np.asarray(links_v), dtype=torch.int32).to(dev)
         self.links_label = torch.as_tensor(np.asarray(labels), dtype=torch.int32).to(dev)
         self.class_values = torch.as_tensor(np.asarray(class_values, dtype=np.float32)).to(dev)
+        self.session_row_deg = 0   # the longest rating-session row the extractor serves (0: none)
         self.cap = graph.node_cap(max_nodes_per_hop, self.h)
         self._graph_version = graph.version
         self.feat_dim = 2 * self.h + 2
@@ -626,18 +629,30 @@ class SubgraphExtractor(_BatchWriter):
         self.max_batch = 0
         self._reserve(max_batch)
 
+    def _row_deg(self):
+        """the longest user row a batch can read: the graph's, or a rating session's"""
+        return max(self.graph.max_row_deg, self.session_row_deg)
+
     def _edges_per_graph(self):
         g = self.graph
-        return 2 * min(self.cap * min(self.cap, max(g.max_row_deg, 1)), max(g.nnz, 1))
+        return 2 * min(self.cap * min(self.cap, max(self._row_deg(), 1)), max(g.nnz + self.session_row_deg, 1))
+
+    def serve_sessions(self, row_deg):
+        """size the capacities for target rows of up to ``row_deg`` ratings (a ``RatingSessions``' longest row; 0:
+        the graph's rows only), re-reserving as after a graph update"""
+        if int(row_deg) != self.session_row_deg:
+            self.session_row_deg = int(row_deg)
+            self._graph_version = None
 
     def _sync_graph(self):
-        """after an update of the graph: re-derive ``cap`` and the edge capacity, and re-reserve the workspace if they
-        grew beyond what it holds (a smaller cap uses the larger buffers as they are)"""
+        """after an update of the graph (or of the session rows served): re-derive ``cap`` and the edge capacity, and
+        re-reserve the workspace if they grew beyond what it holds (a smaller cap uses the larger buffers as they
+        are)"""
         g = self.graph
         if g.version == self._graph_version:
             return
         self._graph_version = g.version
-        self.cap = g.node_cap(self._mnph_arg, self.h)
+        self.cap = g.node_cap(self._mnph_arg, self.h, self._row_deg())
         if self.cap > self._ws_cap or self._edges_per_graph() > self._ws_edges:
             self._reserve(self.max_batch, regrow=True)
 
@@ -674,12 +689,14 @@ class SubgraphExtractor(_BatchWriter):
         return B * 2 * self.cap, ecap, ecap
 
     def extract(self, idx=None, pairs=None, pair_ids=None, out=None, inject=None, seed=None, seed_dev=None,
-                reuse=False, slot=0):
+                reuse=False, slot=0, sessions=None, sess=None):
         """Extract + collate.  ``idx``: int64 tensor/array of dataset indices (device tensor preferred),
         or ``pairs=(u, v, label)`` explicit arrays.  ``inject=(nodes_u, nodes_v, n_u, n_v)`` supplies the
         per-graph node lists ([B,cap] int32, target first) instead of sampling (parity tests).
         ``reuse=True`` writes into one cached buffer set per batch size (training loop / CUDA graphs:
         the previous batch of that size is overwritten).  ``seed_dev``: device uint64 overriding the seed.
+        ``sessions`` (a ``RatingSessions``, with ``pairs``) and ``sess`` [B] (int32 device tensor): graph g takes its
+        target user's row from session row sess[g] (igmc_extract_sessions; ``serve_sessions`` first).
         Returns a ``Batch`` whose public tensors are materialised lazily."""
         dev = self.device
         self._sync_graph()
@@ -710,12 +727,28 @@ class SubgraphExtractor(_BatchWriter):
             assert inj_t[0].shape == (B, self.cap) and inj_t[1].shape == (B, self.cap)
             inj = [t.data_ptr() for t in inj_t]
             keep += inj_t
+        if sessions is not None:
+            if inject is not None or pairs is None or sess is None:
+                raise ValueError("session extraction takes pairs= and sess=, and no injected node lists")
+            if sessions.max_row_deg > self.session_row_deg:
+                raise ValueError("the extractor is sized for session rows of up to %d ratings, not %d "
+                                 "(serve_sessions)" % (self.session_row_deg, sessions.max_row_deg))
+            sess = _on_device(sess, torch.int32, dev)
+            keep += [sess, sessions]
+            _lib.check(self.lib.igmc_extract_sessions(C.byref(self.graph._c), C.byref(sessions._c), sess.data_ptr(),
+                                                      C.byref(P), B, self.h, self.mnph, self.sample_ratio,
+                                                      self.seed if seed is None else int(seed), _lib.ptr(seed_dev),
+                                                      self.cap, C.byref(self._ws_c), self.class_values.data_ptr(),
+                                                      int(self.class_values.numel()), int(self._row_deg()),
+                                                      C.byref(o["_c"]), o["err"].data_ptr(), _stream_ptr()),
+                       "igmc_extract_sessions")
+            return self._batch(B, o, keep)
         _lib.check(self.lib.igmc_extract_batch(C.byref(self.graph._c), C.byref(P), B, self.h, self.mnph,
                                                self.sample_ratio, self.seed if seed is None else int(seed),
                                                _lib.ptr(seed_dev), self.cap, inj[0], inj[1], inj[2], inj[3],
                                                C.byref(self._ws_c),
                                                self.class_values.data_ptr(), int(self.class_values.numel()),
-                                               int(self.graph.max_row_deg), C.byref(o["_c"]), o["err"].data_ptr(),
+                                               int(self._row_deg()), C.byref(o["_c"]), o["err"].data_ptr(),
                                                _stream_ptr()), "igmc_extract_batch")
         return self._batch(B, o, keep)
 

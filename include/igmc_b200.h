@@ -641,6 +641,60 @@ int igmc_graph_update_plan(const igmc_csr_t* G, int nnz, int cap_users, int cap_
 int igmc_graph_update_apply(const igmc_csr_t* G, int nnz, int cap_users, int cap_items, int cap_nnz, int D,
                             void* ws, int64_t ws_bytes, int new_nnz, int new_users, int new_items, void* stream);
 
+/* ---- rating sessions (csrc/session.cu, csrc/extract.cu, csrc/retrieve.cu) ----
+ * A session scores one user from a rating row passed with the query, without changing the graph: session s is user
+ * users[s] (>= G.num_users: a new user, starting from an empty row) with edits (s, item, value) applied to that user's
+ * row only, in RatingGraph.update's encoding (value = label + 1 inserts or overwrites, 0 deletes, the last occurrence
+ * of (s, item) wins; items must exist).  Only a pair's target user takes its row from the session; every other row and
+ * column comes from G, so a session pair's subgraph, and its score, are bit-identical to those of the same pair on the
+ * graph with the edits applied to that user. */
+typedef struct {
+  const int32_t* users;     /* [num_sessions] user id of each session (>= 0) */
+  const int32_t* row_ptr;   /* [num_sessions+1] the merged rows */
+  const int32_t* col_idx;   /* [row_ptr[num_sessions]] ascending within a row */
+  const uint8_t* rating;    /* [row_ptr[num_sessions]] rating label */
+  int32_t num_sessions;
+  int32_t max_row_deg;      /* the longest session row */
+} igmc_sessions_t;
+
+/* Bytes of the workspace igmc_session_plan and igmc_session_apply share. */
+int igmc_session_ws_bytes(int num_sessions, int D, int num_items, int64_t* bytes);
+
+/* Validate (session in [0, num_sessions), item in [0, G->num_items), value 0..256, users >= 0, else IGMC_ERR_SESSIONS
+ * in `err`), order the D edits by (session, item) keeping input order in a run, keep the last of each run, classify it
+ * against the session's base row (binary search) and compute the rows' lengths and pointers into the workspace;
+ * header [2] (device int64) = (total length, longest row).  Changes nothing in G. */
+int igmc_session_plan(const igmc_csr_t* G, const int32_t* users, int num_sessions, const int32_t* sess,
+                      const int32_t* items, const int32_t* values, int D, void* ws, int64_t ws_bytes, int64_t* header,
+                      int* err, void* stream);
+
+/* Merge every session row (a warp per session) into col_idx / rating [header[0]] and write row_ptr [num_sessions+1].
+ * Same G, users, num_sessions, D and workspace as the plan, whose error word must be 0. */
+int igmc_session_apply(const igmc_csr_t* G, const int32_t* users, int num_sessions, int D, void* ws, int64_t ws_bytes,
+                       int32_t* row_ptr, int32_t* col_idx, uint8_t* rating, void* stream);
+
+/* After igmc_candidate_pairs ran over the session rows as a CSR view (row_ptr / col_idx / rating of S, num_users =
+ * num_sessions, num_items = G's, query users 0..num_sessions-1 or explicit pairs whose pair_u is the session index):
+ * sess[i] = links_u[i] (the session), links_u[i] = users[sess[i]] and pair_id[i] = links_u[i] * num_items + links_v[i],
+ * the pair id a graph with the edits applied samples the pair with.  tag is left as it is.  A session index out of
+ * range sets IGMC_ERR_CANDIDATES. */
+int igmc_session_pairs(const igmc_sessions_t* S, int num_items, int B, int32_t* links_u, const int32_t* links_v,
+                       int64_t* pair_id, int32_t* sess, int* err, void* stream);
+
+/* igmc_extract_batch in session mode: graph g takes its target user's row from session row sess[g] of S (the hop-1
+ * item fringe, the visited marks of h > 1 and the target user's row scan) and everything else from G.  A session user
+ * id >= G->num_users is never looked up in G's per-user structures.  `max_row_deg`: max(G's longest row, S's). */
+int igmc_extract_sessions(const igmc_csr_t* G, const igmc_sessions_t* S, const int32_t* sess, const igmc_pairs_t* P,
+                          int B, int h, int max_nodes_per_hop, double sample_ratio, uint64_t seed,
+                          const uint64_t* seed_dev, int cap, const igmc_extract_ws_t* W, const float* class_values,
+                          int num_classes, int max_row_deg, const igmc_batch_out_t* O, int* err, void* stream);
+
+/* igmc_corated_items for sessions: query j is session j, its row N(u) the session row (pass 1 and the exclusion of
+ * rated items), u' != u compared with the session's real user id; the columns come from G.  Workspace as
+ * igmc_corated_ws_bytes(G->num_users, G->num_items, num_sessions, m). */
+int igmc_corated_sessions(const igmc_csr_t* G, const igmc_sessions_t* S, int m, int exclude_rated, void* ws,
+                          int64_t ws_bytes, int32_t* items, int32_t* paths, int* err, void* stream);
+
 /* Version / build info: returns the compiled SM arch (90) so the host can refuse stale builds. */
 int igmc_build_info(void);
 
