@@ -48,7 +48,13 @@ U = 2.0 ** -24
 # decay left out or eps inside the square root is off by 2 000 to 16 000 000 u M.
 # wprep (prepared W_r / W_r^T slabs after a fused update; M = sum_b |att| |basis|): largest 2.8, emulation 1.9; a
 # TF32-rounded basis is off by ~10 000, a dropped basis by ~10^7.  Root columns are copies (exact) and padding is 0.
-KAPPA = dict(states=64, pred=0.5, dhid=4, grad=32, edge=1, dstate=4, adam=16, wprep=16)
+# Per-pair gradients (igmc_pair_grad, one graph's conv block against ``backward`` on that graph alone; the 47 cases and
+# 2 K = 3 cases of tests/test_gpu_pair_grad_bounds.py), same H100 and power limit: gradients 8.3 (pyg-2 on plan 2;
+# conv parameters x4: 7.6), inside κ_grad; d hid 0.99.  hid (the head's relu(lin1 feat + b) per unit; M from the
+# magnitude pass of lin1): largest 1.05, so κ_hid = 8.  The numpy emulation of k_pair_grad_raw stays at 1.1; a slip
+# of its indexing or summation (in for inp, att[b R + r], one CTA's rows dropped, d att of the last k only, root from
+# row R - 1, the previous layer's bias) is off by 10^5 to 3 10^7 u M.
+KAPPA = dict(states=64, pred=0.5, dhid=4, grad=32, edge=1, dstate=4, adam=16, wprep=16, hid=8)
 
 
 class Graph:
@@ -319,6 +325,26 @@ def _pad32(t, w):
     return F.pad(t, (0, w - t.shape[1]))
 
 
+def flat_terms(m, grads, mgrads, prefix=""):
+    """(flat offsets, reference, M) of the gradients ``grads`` / ``mgrads`` (by state_dict name) laid out as
+    ``m.flat_grad``, over the layout entries whose name starts with ``prefix`` (padding columns: 0 in both)"""
+    names = {id(p): n for n, p in m.named_parameters()}
+    idx, ref, M = [], [], []
+    for e, (_, _, p) in zip(m._layout, m._named_order()):
+        o, n, s = e[:3]
+        name = names[id(p)]
+        if not name.startswith(prefix):
+            continue
+        full = e[3] if len(e) == 4 else s
+        r, mm = torch.zeros(full, dtype=torch.float64), torch.zeros(full, dtype=torch.float64)
+        r[..., :s[-1]] = grads[name].reshape(s)
+        mm[..., :s[-1]] = mgrads[name].reshape(s)
+        idx.append(torch.arange(o, o + n))
+        ref.append(r.reshape(-1))
+        M.append(mm.reshape(-1))
+    return torch.cat(idx), torch.cat(ref), torch.cat(M)
+
+
 def check_device(m, ob, ws, train, edge_keep=None, arr=0.0, hidden_keep=None, params=None):
     """every quantity of the last forward (eval) or train step of ``m`` on the oracle batch ``ob`` against its fp64
     recomputation; returns {quantity: (largest err / (u M), elements that must be zero but are not, worst index)} and
@@ -346,20 +372,66 @@ def check_device(m, ob, ws, train, edge_keep=None, arr=0.0, hidden_keep=None, pa
         dhid, grads = backward(params, g, saved, aggr, dgcnn, arr)
         mdhid, mgrads = backward(params, g, saved, aggr, dgcnn, arr, mag=True)
         res["dhid"] = ratio(saved["dhid"], dhid, mdhid)
-        names = {id(p): n for n, p in m.named_parameters()}
-        fg = m.flat_grad.double().cpu()
-        got, ref, M = [], [], []
-        for e, (_, _, p) in zip(m._layout, m._named_order()):
-            o, n, s = e[:3]
-            full = e[3] if len(e) == 4 else s
-            name = names[id(p)]
-            r, mm = torch.zeros(full, dtype=torch.float64), torch.zeros(full, dtype=torch.float64)
-            r[..., :s[-1]] = grads[name].reshape(s)
-            mm[..., :s[-1]] = mgrads[name].reshape(s)
-            got.append(fg[o:o + n])
-            ref.append(r.reshape(-1))
-            M.append(mm.reshape(-1))
-        res["grad"] = ratio(torch.cat(got), torch.cat(ref), torch.cat(M))
+        idx, ref, M = flat_terms(m, grads, mgrads)
+        res["grad"] = ratio(m.flat_grad.double().cpu()[idx], ref, M)
+    return res
+
+
+# ---- one graph of a batch: per-pair gradients (csrc/influence.cu) ---------------------------------------------------
+def graph_view(ob, saved, q):
+    """graph ``q`` of the collated batch ``ob`` and of the kernel's saved tensors ``saved`` (``device_saved``, dpred
+    set to the seed the backward ran with): (a one-graph batch dict with its nodes, its edges renumbered from 0 and its
+    edge positions in ``ob`` under "edges", the saved tensors restricted to its state rows, its gscale row and its
+    dpred).  Graphs of a batch share no node and no edge, so every quantity of graph q computed on this view is the
+    one the batch computes for it."""
+    import numpy as np
+    nptr = np.concatenate([[0], np.cumsum(np.bincount(np.asarray(ob["batch"]), minlength=int(ob["num_graphs"])))])
+    lo, hi = int(nptr[q]), int(nptr[q + 1])
+    ei = np.asarray(ob["edge_index"])
+    edges = np.nonzero((ei[1] >= lo) & (ei[1] < hi))[0]
+    sub = dict(x=np.asarray(ob["x"])[lo:hi], edge_index=ei[:, edges] - lo,
+               edge_type=np.asarray(ob["edge_type"])[edges], batch=np.zeros(hi - lo, np.int64), num_graphs=1,
+               nodes=(lo, hi), edges=edges)
+    sv = dict(states=[h[lo:hi] for h in saved["states"]], gscale=saved["gscale"][q:q + 1],
+              dpred=saved["dpred"][q:q + 1])
+    return sub, sv
+
+
+def pair_terms(params, ob, saved, q, aggr):
+    """(reference, M) of graph q's gradient by state_dict name, and of its d hid [128]: ``backward`` (value and
+    magnitude pass, no ARR term) on that graph alone, seeded with its dpred"""
+    sub, sv = graph_view(ob, saved, q)
+    g = Graph(sub)
+    dhid, grads = backward(params, g, sv, aggr, False, 0.0)
+    mdhid, mgrads = backward(params, g, sv, aggr, False, 0.0, mag=True)
+    return grads, mgrads, dhid[0], mdhid[0]
+
+
+def check_pair(m, ob, saved, q, conv, aggr, params=None, dhid=None, hid=None):
+    """ratios of graph q's per-pair gradient: "grad" (the conv block ``conv`` [conv_param_count] against
+    ``pair_terms``), "dhid" (the kernel's d hid row, given), "hid" (the kernel's hid row against lin1 of the graph's
+    saved target states times its gscale, M from the head's magnitude pass) and "branches" (``branch_mismatches`` on
+    the graph).  ``params``: the state_dict the gradient was taken at (default ``m``'s)."""
+    if params is None:
+        params = m.state_dict()
+    params = {k: v.detach().double().cpu().contiguous() for k, v in params.items()}
+    grads, mgrads, rdhid, mdhid = pair_terms(params, ob, saved, q, aggr)
+    idx, ref, M = flat_terms(m, grads, mgrads, "convs.")
+    res = dict(grad=ratio(conv.double().cpu()[idx], ref, M))
+    sub, sv = graph_view(ob, saved, q)
+    g = Graph(sub)
+    res["branches"] = branch_mismatches(params, g, sv, False)
+    if dhid is not None:
+        res["dhid"] = ratio(dhid.double().cpu(), rdhid, mdhid)
+    if hid is not None:
+        _, P, states = _prep(params, sv, False)
+        _, MP, mstates = _prep(params, sv, True)
+        parts, mparts = {}, {}
+        with torch.no_grad():
+            head(torch.cat(states, 1), P, g, sv, False, parts)
+            head(torch.cat(mstates, 1), MP, g, sv, False, mparts)
+        gs = sv["gscale"][0]
+        res["hid"] = ratio(hid.double().cpu(), parts["lin1"][0] * gs, mparts["lin1"][0] * gs.abs())
     return res
 
 

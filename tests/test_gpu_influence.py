@@ -4,7 +4,9 @@ csrc/influence.cu).
 * pair_gradients against fp64 autograd on the extractor's own subgraphs, loss seed and score seed, every parameter
   tensor within 2e-4 of its reference's largest entry: plans 1, 2, 4, plan 0 (R = 13), the L2 plan, pyg-2, NB 2, h = 2,
   multiply_by 2, a cold-start pair, a padded tail and B = 1;
-* on every plan the per-pair loss gradients of a batch, summed and divided by B, are fused_step(ARR=0)'s flat_grad;
+* on every plan the per-pair loss gradients of a batch, summed and divided by B, are fused_step(ARR=0)'s flat_grad
+  per element within 2 KAPPA["grad"] u M of the batch's magnitude pass (each side is within KAPPA["grad"] u M of the
+  same fp64 value); the per-element bounds of each pair's own gradient are in tests/test_gpu_pair_grad_bounds.py;
 * influence and self_influence per element within kappa_infl * 2^-24 * M of fp64 dot products of the kernel's own
   per-pair gradients; the order, top-k truncation, determinism across B / graph replay / runs, checkpoints, no host
   sync in the steady state, graph updates and DGCNN_RS."""
@@ -18,7 +20,10 @@ import torch
 from igmc_b200 import _lib
 from igmc_b200 import recommend as rc
 from igmc_b200.util_functions import RatingGraph, SubgraphExtractor
+from oracle import extract_np
+from tests import error_bounds as eb
 from tests import pyg2_oracle
+from tests.helpers import batch_equal
 from tests.test_gpu_explain import _ds, _model, _pairs, _r13, _subgraph, _with_cold_start
 
 pytestmark = pytest.mark.gpu
@@ -117,13 +122,24 @@ def test_pair_gradients_sum_to_the_train_step(plan):
     b = _train_batch(A, R, u, v, lab, 100, 2, 40)
     assert np.array_equal(b.y.cpu().numpy(), y)
     m.fused_step(b, ARR=0.0)
-    want = m.flat_grad.double().clone()
+    want = m.flat_grad.double().cpu()
+    # M of the batch gradient: the magnitude pass of the step's own saved tensors on the oracle batch of its pairs
+    ni = A.shape[1]
+    ob = extract_np.extract_batch(extract_np.RatingCSR(A), u, v, lab, np.arange(1, R + 1, dtype=np.float32), 1, 1.0,
+                                  100, seed=2, pair_ids=u * ni + v)
+    assert all(batch_equal(b, ob).values())
+    ws = next(w for k, w in m._ws.items() if k[1] == 40 and k[2])
+    saved = eb.device_saved(m, ws, len(ob["x"]), True)
+    params = {k: p.detach().double().cpu() for k, p in m.state_dict().items()}
+    aggr = "mean_per_relation" if m.rgcn == "pyg-2" else "mean_all"
+    _, mgrads = eb.backward(params, eb.Graph(ob), saved, aggr, False, 0.0, mag=True)
+    idx, _, M = eb.flat_terms(m, mgrads, mgrads)
     G = rc.pair_gradients(m, A, u, v, y, max_nodes_per_hop=100, batch_size=40, sample_seed=2)
-    got = G[0].double().sum(0) / 40
-    for n, e in _entries(m).items():
-        w, g = m._pview(want, e), m._pview(got, e)
-        scale = float(w.abs().max())
-        assert float((g - w).abs().max()) <= 1e-5 * scale + 1e-30, (plan, n)
+    got = G[0].double().sum(0).cpu() / 40
+    # each side is within KAPPA["grad"] u M of the same fp64 value (tests/test_influence_host.py pins the identity)
+    r, pad, worst = eb.ratio(got[idx], want[idx], M)
+    print("plan %s: per-pair gradients summed / B against flat_grad, largest err/(u M) %.3f" % (plan, r))
+    assert r <= 2 * eb.KAPPA["grad"] and pad == 0, (plan, r, pad, worst)
 
 
 def _setup(R=5, plan="auto", N=200, T=12, seed=0):
