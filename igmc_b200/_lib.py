@@ -154,6 +154,7 @@ class SortPoolSaved(C.Structure):
 _SIGS = {
     "igmc_extract_batch": [C.POINTER(CSR), C.POINTER(Pairs), C.c_int, C.c_int, C.c_int, C.c_double, C.c_uint64, vp, C.c_int,
                            vp, vp, vp, vp, C.POINTER(ExtractWS), vp, C.c_int, C.c_int, C.POINTER(BatchOut), vp, vp],
+    "igmc_extract_plan": [C.c_int] * 10,
     "igmc_assemble_batch": [C.POINTER(Store), vp, C.c_int, C.POINTER(BatchOut), vp, vp],
     "igmc_batch_ptrs": [vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp],
     "igmc_batch_prepare": [vp, C.c_int64, vp, vp, vp, C.c_int, C.c_int, C.POINTER(Adj), vp, vp],

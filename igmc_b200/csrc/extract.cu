@@ -1093,10 +1093,11 @@ k_assemble(igmc_store_t S, const int64_t* __restrict__ idx, int B, igmc_batch_ou
 namespace {
 
 // h = 1 fast path (one launch) whenever its tables fit: ids in 12 bits, <= 32 rating classes, the user rows of one
-// subgraph within the tile table, two CTAs per SM worth of shared memory, scratch slot >= the edge bound.  Returns
-// the dynamic shared memory of k_extract_fast, 0 when the batch takes the generic path.
-size_t fast_smem(const igmc_csr_t* G, int B, int h, int cap, const igmc_extract_ws_t* W, int num_classes,
-                 int max_row_deg, const igmc_batch_out_t* O) {
+// subgraph within the tile table, two CTAs per SM worth of shared memory, scratch slot >= the edge bound.  `fast`: the
+// workspace has the one-launch flags; `adjacency`: the batch wants the message-passing lists.  Returns the dynamic
+// shared memory of k_extract_fast, 0 when the batch takes the generic path.
+size_t fast_smem(int num_items, int B, int h, int cap, int num_classes, int max_row_deg, int edge_cap, bool fast,
+                 bool adjacency) {
   static int fast_env = -1;
   if (fast_env < 0) {
     const char* e = getenv("IGMC_EXTRACT_FAST");
@@ -1104,10 +1105,10 @@ size_t fast_smem(const igmc_csr_t* G, int B, int h, int cap, const igmc_extract_
   }
   const int R = num_classes;
   const int words = (cap + 31) / 32;
-  const int slot_e = O->edge_cap / B;
-  const size_t smemF = fast_smem_ints(cap, R > 0 ? R : 1, words) * 4 + (((size_t)G->num_items * 2 + 15) & ~(size_t)15);
-  const long long rows_max = (long long)cap * (long long)(max_row_deg > 0 ? max_row_deg : G->num_items);
-  if (fast_env && h == 1 && W->sync && O->adj_in_ptr && R >= 1 && R <= FX_MAXR && cap <= FX_MAXCAP &&
+  const int slot_e = edge_cap / B;
+  const size_t smemF = fast_smem_ints(cap, R > 0 ? R : 1, words) * 4 + (((size_t)num_items * 2 + 15) & ~(size_t)15);
+  const long long rows_max = (long long)cap * (long long)(max_row_deg > 0 ? max_row_deg : num_items);
+  if (fast_env && h == 1 && fast && adjacency && R >= 1 && R <= FX_MAXR && cap <= FX_MAXCAP &&
       rows_max <= (long long)FX_TILE * FX_TCAP && smemF <= 110 * 1024 && slot_e >= 2)
     return smemF;
   return 0;
@@ -1126,20 +1127,43 @@ int generic_threads() {
 }
 
 // the dynamic shared memory of the two generic kernels; false when the item table or the bitmaps do not fit
-bool generic_smem(const igmc_csr_t* G, int h, int cap, size_t* smemA, size_t* smemB) {
-  size_t a = (size_t)cap * sizeof(int) + (size_t)G->num_items * sizeof(uint16_t);
+bool generic_smem(int num_users, int num_items, int h, int cap, size_t* smemA, size_t* smemB) {
+  size_t a = (size_t)cap * sizeof(int) + (size_t)num_items * sizeof(uint16_t);
   if (h > 1) {   // visited / candidate bitmaps + the fringe list of the larger side
-    const size_t wu = (G->num_users + 31) / 32, wv = (G->num_items + 31) / 32;
+    const size_t wu = (num_users + 31) / 32, wv = (num_items + 31) / 32;
     a = ((a + 15) & ~(size_t)15) + (wu + wv + (wu > wv ? wu : wv)) * 4 +
-        (size_t)(G->num_users > G->num_items ? G->num_users : G->num_items) * 4;
+        (size_t)(num_users > num_items ? num_users : num_items) * 4;
     if (a > 220 * 1024) return false;
   }
   *smemA = a;
-  *smemB = 2 * (size_t)cap * sizeof(int) + (size_t)G->num_items * sizeof(uint16_t);
+  *smemB = 2 * (size_t)cap * sizeof(int) + (size_t)num_items * sizeof(uint16_t);
   return *smemB <= 220 * 1024;   // else the item table does not fit in shared memory
 }
 
+// The path a batch takes, decided once for igmc_extract_batch, igmc_extract_sessions and igmc_extract_plan.
+struct ExtractPlan {
+  size_t fast;           // dynamic shared memory of k_extract_fast, 0: the generic kernels
+  size_t smemA, smemB;   // dynamic shared memory of the two generic kernels
+  bool ok;               // false: neither path fits
+};
+ExtractPlan extract_plan(int num_users, int num_items, int B, int h, int cap, int num_classes, int max_row_deg,
+                         int edge_cap, bool fast, bool adjacency) {
+  ExtractPlan p = {fast_smem(num_items, B, h, cap, num_classes, max_row_deg, edge_cap, fast, adjacency), 0, 0, true};
+  if (!p.fast) p.ok = generic_smem(num_users, num_items, h, cap, &p.smemA, &p.smemB);
+  return p;
+}
+
 }  // namespace
+
+extern "C" int igmc_extract_plan(int num_users, int num_items, int B, int h, int cap, int num_classes,
+                                 int max_row_deg, int edge_cap, int fast, int adjacency) {
+  if (B <= 0) return 0;
+  if (cap < 1 || cap > 65534) return -2;
+  if (h < 1 || h > IGMC_MAX_HOP) return -4;
+  const ExtractPlan p = extract_plan(num_users, num_items, B, h, cap, num_classes, max_row_deg, edge_cap, fast != 0,
+                                     adjacency != 0);
+  return p.fast ? (int)p.fast : p.ok ? 0 : -3;
+}
 
 extern "C" int igmc_extract_batch(const igmc_csr_t* G, const igmc_pairs_t* P, int B, int h, int max_nodes_per_hop,
                                   double sample_ratio, uint64_t seed, const uint64_t* seed_dev, int cap,
@@ -1152,7 +1176,9 @@ extern "C" int igmc_extract_batch(const igmc_csr_t* G, const igmc_pairs_t* P, in
   if (h < 1 || h > IGMC_MAX_HOP) return -4;
   if (h > 1 && (inj_nodes_u || !W->hop_off)) return -4;   // injected node lists carry no hop boundaries
   cudaStream_t st = (cudaStream_t)stream;
-  const size_t smemF = fast_smem(G, B, h, cap, W, num_classes, max_row_deg, O);
+  const ExtractPlan pl = extract_plan(G->num_users, G->num_items, B, h, cap, num_classes, max_row_deg, O->edge_cap,
+                                      W->sync != nullptr, O->adj_in_ptr != nullptr);
+  const size_t smemF = pl.fast;
   if (smemF) {
     cudaFuncSetAttribute(k_extract_fast, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemF);
     k_extract_fast<<<B, FX_THREADS, smemF, st>>>(*G, *P, B, max_nodes_per_hop, sample_ratio, seed, seed_dev, cap,
@@ -1162,8 +1188,8 @@ extern "C" int igmc_extract_batch(const igmc_csr_t* G, const igmc_pairs_t* P, in
     return 0;
   }
   const int ex_threads = generic_threads();
-  size_t smemA, smemB;
-  if (!generic_smem(G, h, cap, &smemA, &smemB)) return -3;
+  if (!pl.ok) return -3;
+  const size_t smemA = pl.smemA, smemB = pl.smemB;
   cudaFuncSetAttribute(k_extract_select_count, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemA);
   cudaFuncSetAttribute(k_extract_fill, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemB);
   k_extract_select_count<<<B, ex_threads, smemA, st>>>(*G, *P, B, max_nodes_per_hop, sample_ratio, seed, seed_dev, cap,
@@ -1189,7 +1215,9 @@ extern "C" int igmc_extract_sessions(const igmc_csr_t* G, const igmc_sessions_t*
   if (h > 1 && !W->hop_off) return -4;
   cudaStream_t st = (cudaStream_t)stream;
   const SessArg A = {*S, sess};
-  const size_t smemF = fast_smem(G, B, h, cap, W, num_classes, max_row_deg, O);
+  const ExtractPlan pl = extract_plan(G->num_users, G->num_items, B, h, cap, num_classes, max_row_deg, O->edge_cap,
+                                      W->sync != nullptr, O->adj_in_ptr != nullptr);
+  const size_t smemF = pl.fast;
   if (smemF) {
     cudaFuncSetAttribute(k_extract_fast_sess, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemF);
     k_extract_fast_sess<<<B, FX_THREADS, smemF, st>>>(*G, *P, B, max_nodes_per_hop, sample_ratio, seed, seed_dev, cap,
@@ -1199,8 +1227,8 @@ extern "C" int igmc_extract_sessions(const igmc_csr_t* G, const igmc_sessions_t*
     return 0;
   }
   const int ex_threads = generic_threads();
-  size_t smemA, smemB;
-  if (!generic_smem(G, h, cap, &smemA, &smemB)) return -3;
+  if (!pl.ok) return -3;
+  const size_t smemA = pl.smemA, smemB = pl.smemB;
   cudaFuncSetAttribute(k_extract_select_count_sess, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemA);
   cudaFuncSetAttribute(k_extract_fill_sess, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemB);
   k_extract_select_count_sess<<<B, ex_threads, smemA, st>>>(*G, *P, B, max_nodes_per_hop, sample_ratio, seed,

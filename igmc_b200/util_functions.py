@@ -752,6 +752,17 @@ class SubgraphExtractor(_BatchWriter):
                                                _stream_ptr()), "igmc_extract_batch")
         return self._batch(B, o, keep)
 
+    def plan(self, B):
+        """the path ``extract`` takes for a batch of ``B`` pairs (igmc_extract_plan on this extractor's graph, cap,
+        rating classes, longest row and edge capacity): the dynamic shared memory of the one-launch h = 1 kernel, 0
+        for the generic kernels, < 0 when neither fits.  Sizes the workspace for ``B`` pairs as ``extract`` does."""
+        self._sync_graph()
+        self._reserve(B)
+        g = self.graph
+        return int(self.lib.igmc_extract_plan(g.num_users, g.num_items, int(B), self.h, self.cap,
+                                              int(self.class_values.numel()), int(self._row_deg()),
+                                              self._out_caps(B)[1], int(self.fast), 1))
+
     def node_lists(self, B):
         """(nodes_u [B,cap], nodes_v [B,cap], n_u [B], n_v [B]) of the last extract (host copies)."""
         cap = self.cap

@@ -99,6 +99,13 @@ int igmc_extract_batch(const igmc_csr_t* G, const igmc_pairs_t* P, int B, int h,
                        const igmc_extract_ws_t* W, const float* class_values, int num_classes, int max_row_deg,
                        const igmc_batch_out_t* O, int* err, void* stream);
 
+/* The path igmc_extract_batch and igmc_extract_sessions take for these arguments, without a launch: the dynamic shared
+ * memory of the one-launch h = 1 kernel when the batch takes it, 0 for the generic two-launch kernels, -3 when neither
+ * fits (the item table or the h > 1 bitmaps exceed shared memory; the extraction then returns -3 too), -2 / -4 for a
+ * cap / h out of range.  `fast` = W->sync != NULL, `adjacency` = O->adj_in_ptr != NULL, `edge_cap` = O->edge_cap. */
+int igmc_extract_plan(int num_users, int num_items, int B, int h, int cap, int num_classes, int max_row_deg,
+                      int edge_cap, int fast, int adjacency);
+
 /* Device-resident store of pre-extracted subgraphs: the reference's static `MyDataset` keeps
  * `(data, slices)` = every graph's tensors concatenated WITHOUT node offsets plus per-graph boundaries
  * (util_functions.py:92,108-109; SURVEY A.5b).  Same content here, in compact types, plus the adjacency. */
