@@ -187,6 +187,7 @@ _SIGS = {
     "igmc_candidate_pairs": [C.POINTER(CSR), C.POINTER(Candidates), vp, C.c_int, vp, vp, vp, vp, vp, vp],
     "igmc_topk_merge": [vp, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp, vp],
     "igmc_score_scatter": [vp, C.c_int, C.c_int, vp, vp, vp],
+    "igmc_topk_fits": [C.c_int, C.c_int],
     "igmc_candidate_lists_ws_bytes": [C.c_int, C.c_int, C.POINTER(C.c_int64)],
     "igmc_candidate_lists": [C.POINTER(CSR), C.POINTER(Candidates), vp, C.c_int, vp, vp, C.c_int64, vp, vp],
     "igmc_explain_count": [vp, vp, C.c_int, vp, vp],

@@ -417,8 +417,8 @@ extern "C" int igmc_influence_topk(const float* S, int B, int T, const int64_t* 
   if (B < 0 || T < 0 || k < 1 || k > IGMC_TOPK_MAX) return -20;
   if (B == 0 || T == 0) return 0;
   if (!S || !tag || !pro_value || !pro_index || !con_value || !con_index) return -20;
+  if (!igmc_topk_fits(k, B)) return -20;
   const size_t smem = (size_t)(k + B) * (sizeof(long long) + sizeof(float));
-  if (smem > 227 * 1024) return -20;
   if (smem > 48 * 1024)
     cudaFuncSetAttribute(k_infl_topk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   k_infl_topk<<<T, 256, smem, (cudaStream_t)stream>>>(S, B, T, tag, k, pro_value, pro_index, con_value, con_index);

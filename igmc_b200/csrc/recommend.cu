@@ -24,6 +24,11 @@ constexpr int LIST_THREADS = 256;
 constexpr int PLAN_THREADS = 1024;
 constexpr int PAIR_THREADS = 512;
 constexpr int MERGE_THREADS = 256;
+constexpr int MERGE_HEAD = 16;   // k_topk_merge's dynamic shared memory: the segment-end word, then the lists
+
+// dynamic shared memory of k_topk_merge (the kernel has no static shared memory): the head and (k + B) entries of an
+// int64 id and an fp32 key
+size_t merge_smem(int k, int B) { return MERGE_HEAD + (size_t)(k + B) * (sizeof(long long) + sizeof(float)); }
 
 __device__ __forceinline__ long long warp_incl_scan_ll(long long v, int lane) {
 #pragma unroll
@@ -272,14 +277,14 @@ k_topk_merge(const float* __restrict__ preds, int K, int B, const int64_t* __res
   const int i0 = blockIdx.x;
   const long long slot = tag[i0];
   if (slot < 0 || (i0 > 0 && tag[i0 - 1] == slot)) return;   // not the first entry of a user's segment
-  __shared__ int s_end;
+  int& s_end = *reinterpret_cast<int*>(smem_raw);              // the segment's end, then the lists at MERGE_HEAD
   if (threadIdx.x == 0) s_end = B;
   __syncthreads();
   for (int i = i0 + 1 + threadIdx.x; i < B; i += blockDim.x)
     if (tag[i] != slot) atomicMin(&s_end, i);
   __syncthreads();
   const int m = s_end - i0, n = k + m;
-  long long* I = reinterpret_cast<long long*>(smem_raw);
+  long long* I = reinterpret_cast<long long*>(smem_raw + MERGE_HEAD);
   float* S = reinterpret_cast<float*>(I + n);
   float* ts = top_score + (size_t)slot * k;
   int64_t* ti = top_item + (size_t)slot * k;
@@ -410,11 +415,16 @@ extern "C" int igmc_candidate_pairs(const igmc_csr_t* G, const igmc_candidates_t
   return 0;
 }
 
+extern "C" int igmc_topk_fits(int k, int B) {
+  if (k < 1 || k > IGMC_TOPK_MAX || B < 1) return 0;
+  return merge_smem(k, B) <= 227 * 1024 ? 1 : 0;
+}
+
 extern "C" int igmc_topk_merge(const float* preds, int K, int B, const int64_t* tag, const int32_t* items, int k,
                                float* top_score, int64_t* top_item, void* stream) {
   if (K < 1 || B <= 0 || k < 1 || k > IGMC_TOPK_MAX) return -1;
-  const size_t smem = (size_t)(k + B) * (sizeof(long long) + sizeof(float));
-  if (smem > 227 * 1024) return -2;
+  if (!igmc_topk_fits(k, B)) return -2;
+  const size_t smem = merge_smem(k, B);
   if (smem > 48 * 1024)
     cudaFuncSetAttribute(k_topk_merge, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   k_topk_merge<<<B, MERGE_THREADS, smem, (cudaStream_t)stream>>>(preds, K, B, tag, items, k, top_score, top_item);

@@ -237,8 +237,8 @@ extern "C" int igmc_corated_items(const igmc_csr_t* G, const int32_t* users, int
     if (!ws || ws_bytes < (int64_t)grid * (int64_t)row) return -2;
   }
   const size_t smem = shared ? row : 0;
-  if (smem > 48 * 1024)
-    cudaFuncSetAttribute(k_corated, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  // opted in at every size: the static histogram and scan words count against the default 48 KB as well
+  cudaFuncSetAttribute(k_corated, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   k_corated<<<grid, THREADS, smem, (cudaStream_t)stream>>>(*G, users, num_query, m, exclude_rated ? 1 : 0,
                                                            shared ? 1 : 0, static_cast<unsigned char*>(ws), row, items,
                                                            paths, err);
@@ -262,8 +262,8 @@ extern "C" int igmc_corated_sessions(const igmc_csr_t* G, const igmc_sessions_t*
     if (!ws || ws_bytes < (int64_t)grid * (int64_t)row) return -2;
   }
   const size_t smem = shared ? row : 0;
-  if (smem > 48 * 1024)
-    cudaFuncSetAttribute(k_corated_sess, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  // opted in at every size: the static histogram and scan words count against the default 48 KB as well
+  cudaFuncSetAttribute(k_corated_sess, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   k_corated_sess<<<grid, THREADS, smem, (cudaStream_t)stream>>>(*G, *S, m, exclude_rated ? 1 : 0, shared ? 1 : 0,
                                                                 static_cast<unsigned char*>(ws), row, items, paths,
                                                                 err);

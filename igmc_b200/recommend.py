@@ -129,6 +129,14 @@ def _check_k(k):
     return k
 
 
+def _check_merge_fits(k, batch_size):
+    """ValueError unless the top-k merge (igmc_topk_merge, igmc_influence_topk) can run k kept entries against batches
+    of ``batch_size`` pairs: it holds both in one CTA's shared memory.  A batch size below 1 is the engine's to refuse."""
+    if int(batch_size) >= 1 and not _lib.load().igmc_topk_fits(int(k), int(batch_size)):
+        raise ValueError("k = %d with batch_size = %d does not fit the top-k merge's shared memory (k + batch_size "
+                         "entries in one CTA): lower batch_size or k" % (int(k), int(batch_size)))
+
+
 INFLUENCE_T_MAX = 1024   # test pairs of one influence run: the test-side store is K * T * (conv block + factors) floats
 
 
@@ -721,6 +729,7 @@ class InferenceEngine(object):
         a 2-D [U, width] array of per-user lists (-1 = empty slot); ``retrieve=M``: each user's M items with the most
         bridges (``corated_items``) are its candidates.  Returns the number of candidate pairs."""
         k = _check_k(k)
+        _check_merge_fits(k, self.B)
         g = self.graph
         if retrieve is not None and items is not None:
             raise ValueError("retrieve= chooses the candidates itself: pass it without items=")
@@ -837,6 +846,7 @@ class InferenceEngine(object):
         rated items come from its session row.  Arguments as ``start_recommend``'s.  Returns the number of candidate
         pairs."""
         k = _check_k(k)
+        _check_merge_fits(k, self.B)
         sessions = self._check_sessions(sessions)
         g = self.graph
         if retrieve is not None and items is not None:
@@ -908,6 +918,7 @@ class InferenceEngine(object):
         S[b, t] = sum_k lrs[k] <G_b, G_t> per batch and merges it into each test pair's top-k lists.  Returns the
         number of test pairs."""
         k = _check_influence_k(k)
+        _check_merge_fits(k, self.B)
         _check_per_pair_model(self.model)
         tr = _host_pairs(self.graph.shape, *_split_pairs(train, "train", True), name="train")
         te = _host_pairs(self.graph.shape, *_split_pairs(test, "test", False), name="test")
@@ -1483,6 +1494,7 @@ def influence(model, graph, train, test, k, *, checkpoints=None, lrs=None, h=1, 
     after every number, empty slots -1 / -inf (pro) and -1 / +inf (con).  Conv block by a split-K FFMA GEMM, readout
     block from its rank-1 factors; bit-identical across runs, batch sizes and graph replay.  IGMC only."""
     k = _check_influence_k(k)
+    _check_merge_fits(k, batch_size)
     _check_per_pair_model(model)
     users, items, y = _host_pairs(graph.shape, *_split_pairs(train, "train", True), name="train")
     tu, ti, ty = _host_pairs(graph.shape, *_split_pairs(test, "test", False), name="test")
@@ -1521,6 +1533,7 @@ def recommend(model, graph, users, k, *, items=None, exclude_rated=True, retriev
     descending, then item ascending; a NaN score ranks last; a user with fewer than ``k`` candidates gets item -1 /
     score -inf in the empty slots.  A pair's score does not depend on the candidates it was ranked among."""
     k = _check_k(k)
+    _check_merge_fits(k, batch_size)
     nu, ni = graph.shape
     if retrieve is not None and items is not None:
         raise ValueError("retrieve= chooses the candidates itself: pass it without items=")
@@ -1597,6 +1610,7 @@ def recommend_sessions(model, sessions, k, *, items=None, exclude_rated=True, re
     ``retrieve=M``); a 2-D ``items`` has one row per session.  Row s is bit for bit ``recommend`` for sessions.users[s]
     on the graph with session s's edits applied (same kernel plan and batch size); the graph is not changed."""
     k = _check_k(k)
+    _check_merge_fits(k, batch_size)
     if not isinstance(sessions, RatingSessions):
         raise TypeError("sessions must be a RatingSessions")
     sessions.check()

@@ -475,6 +475,12 @@ int igmc_candidate_pairs(const igmc_csr_t* G, const igmc_candidates_t* Cd, int64
 int igmc_topk_merge(const float* preds, int K, int B, const int64_t* tag, const int32_t* items, int k,
                     float* top_score, int64_t* top_item, void* stream);
 
+/* 1 when a top-k merge of batch size B with k kept entries can launch, else 0: 1 <= k <= IGMC_TOPK_MAX, B >= 1 and the
+ * merge's shared memory, 16 + (k + B) * 12 bytes (a head word, then a running list and the batch as int64 ids and
+ * fp32 keys), within the 227 KB a CTA may take: k + B <= 19 369.  igmc_topk_merge refuses what does not fit with -2,
+ * igmc_influence_topk (whose merge needs no head) with -20: one limit for both. */
+int igmc_topk_fits(int k, int B);
+
 /* Explicit pairs: scores[tag[i]] = the same fp32 checkpoint mean for every i with tag[i] >= 0. */
 int igmc_score_scatter(const float* preds, int K, int B, const int64_t* tag, float* scores, void* stream);
 
