@@ -24,6 +24,9 @@ __device__ __forceinline__ void igmc_set_err(int* err, int code) {
   if (err) atomicCAS(err, 0, code);
 }
 
+// workspace carve-ups: every sub-array starts on a 256-byte boundary
+__host__ __device__ __forceinline__ size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
+
 // ---- "raw" per-CTA gradient rows of the relation-space kernels (csrc/rgcn_rs.cu -> csrc/optim.cu) -------------
 // layer l: [ dW_r : R x inp x 32 | d root : inp x 32 | d bias : 32 ],  inp = in rounded up to 4 (in = in_dim0 for
 // layer 0, 32 after).  The (att, basis) chain rule is linear in dW_r, so it is applied ONCE to the sum over CTAs

@@ -208,8 +208,6 @@ __global__ void k_order_gather(const int32_t* __restrict__ srt, const int64_t* _
   }
 }
 
-size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
-
 // the carve-up of igmc_occlusion_order's workspace: keys in / out [T], positions in / out [T], delta [T], CUB scratch
 struct OrderLayout {
   uint64_t *keys, *keys_out;

@@ -23,8 +23,6 @@ namespace {
 
 constexpr int THREADS = 256;
 
-size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
-
 // the carve-up of the caller's workspace; the same for the size query, the plan and the apply
 struct Layout {
   // per delta entry
@@ -90,11 +88,6 @@ Layout layout(void* base, int D, int cap_users, int cap_items, int cap_nnz, cuda
   L.temp = take(t);
   L.total = off;
   return L;
-}
-
-int grid_for(long long n) {
-  long long g = (n + THREADS - 1) / THREADS;
-  return (int)(g < 1 ? 1 : g > 65535 * 8 ? 65535 * 8 : g);
 }
 
 // ---- plan ----------------------------------------------------------------------------------------------------------
@@ -225,10 +218,6 @@ __global__ void k_merge(const int32_t* __restrict__ ptr, const int32_t* __restri
   }
 }
 
-__global__ void k_store_ptr(const long long* __restrict__ src, int n, int32_t* __restrict__ dst) {
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += gridDim.x * blockDim.x) dst[i] = (int32_t)src[i];
-}
-
 bool caps_ok(const igmc_csr_t* G, int nnz, int cap_users, int cap_items, int cap_nnz) {
   return G && nnz >= 0 && cap_users >= G->num_users && cap_items >= G->num_items && cap_nnz >= nnz &&
          G->num_users >= 0 && G->num_items >= 0 && cap_users >= 1 && cap_items >= 1;
@@ -260,7 +249,7 @@ extern "C" int igmc_graph_update_plan(const igmc_csr_t* G, int nnz, int cap_user
   cudaMemsetAsync(L.col_de, 0, ((size_t)cap_items + 1) * 4, st);
   cudaMemsetAsync(L.pk_uv + D, 0, 8, st);
   const int bits = bits_for((unsigned long long)cap_users * (unsigned long long)cap_items);
-  const int g = grid_for(D);
+  const int g = grid_for(D, THREADS);
   size_t tb = L.temp_bytes;
   k_keys<<<g, THREADS, 0, st>>>(users, items, values, D, cap_users, cap_items, L.key_uv, L.pos, err);
   if (cub::DeviceRadixSort::SortPairs(L.temp, tb, L.key_uv, L.skey_uv, L.pos, L.spos, D, 0, bits, st) != cudaSuccess)
@@ -273,17 +262,17 @@ extern "C" int igmc_graph_update_plan(const igmc_csr_t* G, int nnz, int cap_user
   tb = L.temp_bytes;
   if (cub::DeviceRadixSort::SortPairs(L.temp, tb, L.key_vu, L.skey_vu, L.pos, L.perm_c, D, 0, bits, st) != cudaSuccess)
     return -3;
-  k_gather_col<<<grid_for(D + 1), THREADS, 0, st>>>(L.perm_c, L.pk_uv, D, L.pk_vu);
+  k_gather_col<<<grid_for(D + 1, THREADS), THREADS, 0, st>>>(L.perm_c, L.pk_uv, D, L.pk_vu);
   tb = L.temp_bytes;
   if (cub::DeviceScan::ExclusiveSum(L.temp, tb, L.pk_vu, L.scan_vu, D + 1, st) != cudaSuccess) return -3;
   k_runs<<<g, THREADS, 0, st>>>(L.skey_uv, D, cap_items, L.row_ds, L.row_de);
   k_runs<<<g, THREADS, 0, st>>>(L.skey_vu, D, cap_users, L.col_ds, L.col_de);
-  k_lengths<<<grid_for(cap_users + 1), THREADS, 0, st>>>(G->row_ptr, G->num_users, cap_users, L.skey_uv, D, cap_items,
-                                                         shape_users, L.row_ds, L.row_de, L.scan_uv, L.len_r,
-                                                         &H->num_users, &H->max_row_deg);
-  k_lengths<<<grid_for(cap_items + 1), THREADS, 0, st>>>(G->col_ptr, G->num_items, cap_items, L.skey_vu, D, cap_users,
-                                                         shape_items, L.col_ds, L.col_de, L.scan_vu, L.len_c,
-                                                         &H->num_items, &H->max_col_deg);
+  k_lengths<<<grid_for(cap_users + 1, THREADS), THREADS, 0, st>>>(G->row_ptr, G->num_users, cap_users, L.skey_uv, D,
+                                                                  cap_items, shape_users, L.row_ds, L.row_de,
+                                                                  L.scan_uv, L.len_r, &H->num_users, &H->max_row_deg);
+  k_lengths<<<grid_for(cap_items + 1, THREADS), THREADS, 0, st>>>(G->col_ptr, G->num_items, cap_items, L.skey_vu, D,
+                                                                  cap_users, shape_items, L.col_ds, L.col_de,
+                                                                  L.scan_vu, L.len_c, &H->num_items, &H->max_col_deg);
   tb = L.temp_bytes;
   if (cub::DeviceScan::ExclusiveSum(L.temp, tb, L.len_r, L.ptr_r, cap_users + 1, st) != cudaSuccess) return -3;
   tb = L.temp_bytes;
@@ -303,10 +292,10 @@ extern "C" int igmc_graph_update_apply(const igmc_csr_t* G, int nnz, int cap_use
   cudaStream_t st = (cudaStream_t)stream;
   const Layout L = layout(ws, D, cap_users, cap_items, cap_nnz, st);
   if ((int64_t)L.total > ws_bytes) return -2;
-  k_merge<true><<<grid_for((long long)new_users * 32), THREADS, 0, st>>>(
+  k_merge<true><<<grid_for((long long)new_users * 32, THREADS), THREADS, 0, st>>>(
       G->row_ptr, G->col_idx, G->rating, G->num_users, new_users, L.ptr_r, L.row_ds, L.row_de, L.skey_uv, cap_items,
       L.cls, L.lab, nullptr, L.scan_uv, L.new_col_idx, L.new_rating);
-  k_merge<false><<<grid_for((long long)new_items * 32), THREADS, 0, st>>>(
+  k_merge<false><<<grid_for((long long)new_items * 32, THREADS), THREADS, 0, st>>>(
       G->col_ptr, G->row_idx, nullptr, G->num_items, new_items, L.ptr_c, L.col_ds, L.col_de, L.skey_vu, cap_users,
       L.cls, L.lab, L.perm_c, L.scan_vu, L.new_row_idx, nullptr);
   IGMC_CUDA_CHECK_LAUNCH();
@@ -316,8 +305,8 @@ extern "C" int igmc_graph_update_apply(const igmc_csr_t* G, int nnz, int cap_use
     cudaMemcpyAsync((void*)G->rating, L.new_rating, (size_t)new_nnz, cudaMemcpyDeviceToDevice, st);
     cudaMemcpyAsync((void*)G->row_idx, L.new_row_idx, (size_t)new_nnz * 4, cudaMemcpyDeviceToDevice, st);
   }
-  k_store_ptr<<<grid_for(new_users + 1), THREADS, 0, st>>>(L.ptr_r, new_users, (int32_t*)G->row_ptr);
-  k_store_ptr<<<grid_for(new_items + 1), THREADS, 0, st>>>(L.ptr_c, new_items, (int32_t*)G->col_ptr);
+  k_store_ptr<<<grid_for(new_users + 1, THREADS), THREADS, 0, st>>>(L.ptr_r, new_users, (int32_t*)G->row_ptr);
+  k_store_ptr<<<grid_for(new_items + 1, THREADS), THREADS, 0, st>>>(L.ptr_c, new_items, (int32_t*)G->col_ptr);
   IGMC_CUDA_CHECK_LAUNCH();
   return 0;
 }

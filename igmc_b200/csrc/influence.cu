@@ -14,6 +14,7 @@
 #include <cmath>
 
 #include "common.cuh"
+#include "topk_merge.cuh"
 #include "../../include/igmc_b200.h"
 
 namespace {
@@ -271,17 +272,6 @@ k_infl_finish(int L, int B, int T, int splits, const float* __restrict__ part, c
   if (lane == 0) S[w] = fmaf(eta, s + ro, first ? 0.f : S[w]);
 }
 
-// a ranks before b under key sign * value: key descending, index ascending, NaN after every number, empty slots
-// (index < 0) last
-__device__ __forceinline__ bool infl_before(float as, long long ai, float bs, long long bi, float sign) {
-  if (ai < 0) return false;
-  if (bi < 0) return true;
-  const float ak = sign * as, bk = sign * bs;
-  const bool an = isnan(ak), bn = isnan(bk);
-  if (an || bn) return (an && bn) ? ai < bi : bn;
-  return ak > bk || (ak == bk && ai < bi);
-}
-
 // block t: S[:, t] (index tag[b], padding skipped) merged into the running lists of test pair t by rank counting,
 // proponents (sign +1) then opponents (sign -1)
 __global__ void __launch_bounds__(256)
@@ -306,29 +296,7 @@ k_infl_topk(const float* __restrict__ S, int B, int T, const int64_t* __restrict
       I[k + b] = tag[b];
     }
     __syncthreads();
-    for (int e = threadIdx.x; e < n; e += blockDim.x) {
-      const float ev = V[e];
-      const long long ei = I[e];
-      if (e >= k && ei < 0) continue;
-      int r;
-      if (e < k) {
-        r = e;
-      } else {
-        int lo = 0, hi = k;   // the running list is ranked
-        while (lo < hi) {
-          const int mid = (lo + hi) >> 1;
-          if (infl_before(V[mid], I[mid], ev, ei, sign)) lo = mid + 1; else hi = mid;
-        }
-        r = lo;
-      }
-      if (r >= k) continue;
-      for (int x = k; x < n && r < k; ++x)
-        if (x != e && infl_before(V[x], I[x], ev, ei, sign)) ++r;
-      if (r < k) {
-        tv[r] = ev;
-        ti[r] = ei;
-      }
-    }
+    rank_merge(V, I, k, n, sign, tv, ti);
   }
 }
 
@@ -418,7 +386,7 @@ extern "C" int igmc_influence_topk(const float* S, int B, int T, const int64_t* 
   if (B == 0 || T == 0) return 0;
   if (!S || !tag || !pro_value || !pro_index || !con_value || !con_index) return -20;
   if (!igmc_topk_fits(k, B)) return -20;
-  const size_t smem = (size_t)(k + B) * (sizeof(long long) + sizeof(float));
+  const size_t smem = merge_smem(k, B);
   if (smem > 48 * 1024)
     cudaFuncSetAttribute(k_infl_topk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   k_infl_topk<<<T, 256, smem, (cudaStream_t)stream>>>(S, B, T, tag, k, pro_value, pro_index, con_value, con_index);

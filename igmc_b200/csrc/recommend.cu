@@ -16,6 +16,7 @@
 #include <cub/device/device_segmented_radix_sort.cuh>
 
 #include "common.cuh"
+#include "topk_merge.cuh"
 #include "../../include/igmc_b200.h"
 
 namespace {
@@ -24,11 +25,6 @@ constexpr int LIST_THREADS = 256;
 constexpr int PLAN_THREADS = 1024;
 constexpr int PAIR_THREADS = 512;
 constexpr int MERGE_THREADS = 256;
-constexpr int MERGE_HEAD = 16;   // k_topk_merge's dynamic shared memory: the segment-end word, then the lists
-
-// dynamic shared memory of k_topk_merge (the kernel has no static shared memory): the head and (k + B) entries of an
-// int64 id and an fp32 key
-size_t merge_smem(int k, int B) { return MERGE_HEAD + (size_t)(k + B) * (sizeof(long long) + sizeof(float)); }
 
 __device__ __forceinline__ long long warp_incl_scan_ll(long long v, int lane) {
 #pragma unroll
@@ -260,16 +256,6 @@ __device__ __forceinline__ float ckpt_mean(const float* __restrict__ preds, int 
   return K > 1 ? __fdiv_rn(a, (float)K) : a;
 }
 
-// ranking order: a ranks before b.  Empty slots (item < 0) rank after every candidate, NaN after every number,
-// equal scores (and NaNs among themselves) by ascending item.
-__device__ __forceinline__ bool ranks_before(float as, long long ai, float bs, long long bi) {
-  if (ai < 0) return false;
-  if (bi < 0) return true;
-  const bool an = isnan(as), bn = isnan(bs);
-  if (an || bn) return (an && bn) ? ai < bi : bn;
-  return as > bs || (as == bs && ai < bi);
-}
-
 __global__ void __launch_bounds__(MERGE_THREADS)
 k_topk_merge(const float* __restrict__ preds, int K, int B, const int64_t* __restrict__ tag,
              const int32_t* __restrict__ items, int k, float* __restrict__ top_score, int64_t* __restrict__ top_item) {
@@ -297,29 +283,7 @@ k_topk_merge(const float* __restrict__ preds, int K, int B, const int64_t* __res
     I[k + t] = items[i0 + t];
   }
   __syncthreads();
-  // rank of every element = number of elements ranked before it (distinct items: a permutation of 0..n-1)
-  for (int e = threadIdx.x; e < n; e += blockDim.x) {
-    const float es = S[e];
-    const long long ei = I[e];
-    int r = 0;
-    if (e < k) {
-      r = e;
-    } else {
-      int lo = 0, hi = k;   // the running list is ranked: binary search for the first entry not before e
-      while (lo < hi) {
-        const int mid = (lo + hi) >> 1;
-        if (ranks_before(S[mid], I[mid], es, ei)) lo = mid + 1; else hi = mid;
-      }
-      r = lo;
-    }
-    if (r >= k) continue;
-    for (int x = k; x < n; ++x)
-      if (x != e && ranks_before(S[x], I[x], es, ei)) ++r;
-    if (r < k) {
-      ts[r] = es;
-      ti[r] = ei;
-    }
-  }
+  rank_merge(S, I, k, n, 1.f, ts, ti);
 }
 
 __global__ void __launch_bounds__(MERGE_THREADS)
@@ -342,8 +306,6 @@ extern "C" int igmc_candidate_plan(const igmc_csr_t* G, const igmc_candidates_t*
 }
 
 namespace {
-
-size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
 
 // the carve-up of igmc_candidate_lists' workspace: sorted rows [U * width], segment offsets [U + 1], CUB scratch
 struct ListsLayout {

@@ -21,8 +21,6 @@ constexpr int WARPS = THREADS / 32;
 constexpr int GLOBAL_CTAS = 264;                  // two per H100 SM when the histograms live in global memory
 constexpr size_t SMEM_LIMIT = 200 * 1024;         // dynamic shared memory of the shared-memory regime
 
-__host__ __device__ __forceinline__ size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
-
 __host__ __device__ __forceinline__ int pow2_at_least(int n) {
   int p = 1;
   while (p < n) p <<= 1;

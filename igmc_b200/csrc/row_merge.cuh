@@ -1,6 +1,6 @@
 // Device code shared by the in-place graph update (graph_update.cu) and the rating-session rows (session.cu): the
 // classification of a kept delta entry, the packed (inserted, deleted) counts, the binary search in a sorted row, the
-// per-row runs of a sorted delta and the warp merge of one row with its run.
+// per-row runs of a sorted delta, the warp merge of one row with its run and the int32 store of the row pointers.
 #pragma once
 
 #include "common.cuh"
@@ -14,6 +14,12 @@ __device__ __forceinline__ long long pack_count(uint8_t c) {
   return c == C_INSERT ? (1ll << 32) : c == C_DELETE ? 1ll : 0ll;
 }
 __device__ __forceinline__ long long net(long long p) { return (p >> 32) - (p & 0xffffffffll); }
+
+// blocks of `threads` for a grid-stride loop over n elements: at least 1, at most 65 535 * 8
+inline int grid_for(long long n, int threads) {
+  long long g = (n + threads - 1) / threads;
+  return (int)(g < 1 ? 1 : g > 65535 * 8 ? 65535 * 8 : g);
+}
 
 inline int bits_for(unsigned long long n) {   // radix-sort bits of keys in [0, n)
   int b = 0;
@@ -95,6 +101,11 @@ __device__ __forceinline__ void merge_row(const int32_t* __restrict__ idx, const
     out_idx[o] = c;
     if (RATING) out_rating[o] = lab[p];
   }
+}
+
+// the int64 row pointers [n + 1] of a merge stored as int32
+__global__ void k_store_ptr(const long long* __restrict__ src, int n, int32_t* __restrict__ dst) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += gridDim.x * blockDim.x) dst[i] = (int32_t)src[i];
 }
 
 }  // namespace

@@ -26,8 +26,6 @@ namespace {
 
 constexpr int THREADS = 256;
 
-size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
-
 struct Layout {
   long long *key, *skey, *pk, *scan, *len, *ptr;
   int32_t *pos, *spos, *ds, *de;
@@ -73,11 +71,6 @@ Layout layout(void* base, int S, int D, int num_items, cudaStream_t st) {
   L.temp = take(t);
   L.total = off;
   return L;
-}
-
-int grid_for(long long n) {
-  long long g = (n + THREADS - 1) / THREADS;
-  return (int)(g < 1 ? 1 : g > 65535 * 8 ? 65535 * 8 : g);
 }
 
 // the sort key s * num_items + v of every edit; invalid edits (and invalid user ids) set the error and key 0
@@ -180,10 +173,6 @@ __global__ void k_session_merge(igmc_csr_t G, const int32_t* __restrict__ users,
   }
 }
 
-__global__ void k_session_store_ptr(const long long* __restrict__ src, int n, int32_t* __restrict__ dst) {
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += gridDim.x * blockDim.x) dst[i] = (int32_t)src[i];
-}
-
 // pairs over the session rows: links_u holds the session index; it becomes sess[i], and links_u / pair_id the
 // session user's id and its pair id u * num_items + v
 __global__ void k_session_pairs(const int32_t* __restrict__ users, int S, int num_items, int B,
@@ -223,7 +212,7 @@ extern "C" int igmc_session_plan(const igmc_csr_t* G, const int32_t* users, int 
   cudaMemsetAsync(header, 0, 2 * sizeof(int64_t), st);
   cudaMemsetAsync(L.ds, 0, ((size_t)S + 1) * 4, st);
   cudaMemsetAsync(L.de, 0, ((size_t)S + 1) * 4, st);
-  const int g = grid_for(D > S ? D : S);
+  const int g = grid_for(D > S ? D : S, THREADS);
   k_session_keys<<<g, THREADS, 0, st>>>(users, S, sess, items, values, D, G->num_items, L.key, L.pos, err);
   size_t tb;
   if (D > 0) {
@@ -233,14 +222,14 @@ extern "C" int igmc_session_plan(const igmc_csr_t* G, const int32_t* users, int 
                                         bits_for((unsigned long long)S * (unsigned long long)G->num_items),
                                         st) != cudaSuccess)
       return -3;
-    k_session_classify<<<grid_for(D), THREADS, 0, st>>>(*G, users, values, D, G->num_items, L.skey, L.spos, L.cls,
-                                                        L.lab, L.pk);
+    k_session_classify<<<grid_for(D, THREADS), THREADS, 0, st>>>(*G, users, values, D, G->num_items, L.skey, L.spos,
+                                                                 L.cls, L.lab, L.pk);
     tb = L.temp_bytes;
     if (cub::DeviceScan::ExclusiveSum(L.temp, tb, L.pk, L.scan, D + 1, st) != cudaSuccess) return -3;
-    k_runs<<<grid_for(D), THREADS, 0, st>>>(L.skey, D, G->num_items, L.ds, L.de);
+    k_runs<<<grid_for(D, THREADS), THREADS, 0, st>>>(L.skey, D, G->num_items, L.ds, L.de);
   }
-  k_session_lengths<<<grid_for(S + 1), THREADS, 0, st>>>(*G, users, S, L.ds, L.de, D > 0 ? L.scan : nullptr, L.len,
-                                                         header);
+  k_session_lengths<<<grid_for(S + 1, THREADS), THREADS, 0, st>>>(*G, users, S, L.ds, L.de,
+                                                                  D > 0 ? L.scan : nullptr, L.len, header);
   tb = L.temp_bytes;
   if (cub::DeviceScan::ExclusiveSum(L.temp, tb, L.len, L.ptr, S + 1, st) != cudaSuccess) return -3;
   k_session_total<<<1, 1, 0, st>>>(L.ptr, S, header);
@@ -256,10 +245,10 @@ extern "C" int igmc_session_apply(const igmc_csr_t* G, const int32_t* users, int
   cudaStream_t st = (cudaStream_t)stream;
   const Layout L = layout(ws, S, D, G->num_items, st);
   if ((int64_t)L.total > ws_bytes) return -2;
-  k_session_merge<<<grid_for((long long)S * 32), THREADS, 0, st>>>(*G, users, S, L.ptr, L.ds, L.de, L.skey,
-                                                                    G->num_items, L.cls, L.lab, L.scan, col_idx,
-                                                                    rating);
-  k_session_store_ptr<<<grid_for(S + 1), THREADS, 0, st>>>(L.ptr, S, row_ptr);
+  k_session_merge<<<grid_for((long long)S * 32, THREADS), THREADS, 0, st>>>(*G, users, S, L.ptr, L.ds, L.de, L.skey,
+                                                                             G->num_items, L.cls, L.lab, L.scan,
+                                                                             col_idx, rating);
+  k_store_ptr<<<grid_for(S + 1, THREADS), THREADS, 0, st>>>(L.ptr, S, row_ptr);
   IGMC_CUDA_CHECK_LAUNCH();
   return 0;
 }

@@ -46,7 +46,7 @@ import torch
 
 from . import _lib
 from .train_eval import replay_step
-from .util_functions import RatingGraph, SubgraphExtractor, _stream_ptr
+from .util_functions import RatingGraph, SubgraphExtractor, _cuda_ints, _on_device_i32, _stream_ptr, _update_inputs
 
 __all__ = ["predict_pairs", "recommend", "corated_items", "explain_pairs", "Explanation", "attribute_pairs",
            "Attribution", "pair_gradients", "influence", "self_influence", "Influence", "InferenceEngine",
@@ -75,58 +75,67 @@ def _is_rows(items):
     return items is not None and (items.dim() == 2 if torch.is_tensor(items) else np.ndim(items) == 2)
 
 
-def _user_rows(items, U, num_items, dev):
-    """per-user candidate rows [U, width] as an int32 device tensor.  Host arrays are checked here (IndexError for an
-    id outside [-1, num_items)); integer device tensors are used as they are and checked by the kernel.  ValueError
-    when the row count is not U."""
+def _user_rows(items, U, num_items):
+    """per-user candidate rows [U, width] checked on the host: a host array as int32 (IndexError for an id outside
+    [-1, num_items)); an integer CUDA tensor as it is, checked by the kernel.  ValueError when the row count is not
+    U."""
     if not torch.is_tensor(items):
         items = np.asarray(items)
     if items.shape[0] != U:
-        raise ValueError("items has %d rows, one per query user is %d" % (items.shape[0], U))
-    if torch.is_tensor(items) and items.device.type == "cuda":
-        if items.is_floating_point() or items.is_complex() or items.dtype == torch.bool:
-            raise TypeError("items must be integer ids, not %s" % items.dtype)
-        return items.to(device=dev, dtype=torch.int32).contiguous()
+        raise ValueError("items has %d rows, one per query slot is %d" % (items.shape[0], U))
+    if _cuda_ints(items, "items"):
+        return items
     a = np.asarray(items.cpu().numpy() if torch.is_tensor(items) else items)
     if a.size and not np.issubdtype(a.dtype, np.integer):
-        raise TypeError("items must be integer ids, not %s" % a.dtype)
+        raise TypeError("items must be integers, not %s" % a.dtype)
     a = a.astype(np.int64)
     if a.size and (a.min() < -1 or a.max() >= num_items):
         bad = int(a.min()) if a.min() < -1 else int(a.max())
         raise IndexError("items: id %d out of range [-1, %d)" % (bad, num_items))
-    return torch.from_numpy(a.astype(np.int32)).to(dev)
+    return a.astype(np.int32)
 
 
-def _check_m(m, num_items):
-    m = int(m)
-    if m < 1 or m > num_items:
-        raise ValueError("the number of retrieved items must lie in [1, %d], not %d" % (num_items, m))
-    return m
+def _check_count(n, name, hi, over=NotImplementedError):
+    """``n`` as an int in [1, hi]: ValueError below 1, ``over`` above ``hi``"""
+    n = int(n)
+    if n < 1 or n > hi:
+        raise (ValueError if n < 1 else over)("%s must lie in [1, %d], not %d" % (name, hi, n))
+    return n
 
 
-def _corated(lib, g, users, m, exclude_rated, err, ws):
-    """igmc_corated_items for the int32 device tensor ``users`` on graph ``g``: (items, paths) [U, m] int32.  ``ws``: a
-    dict whose "ws" tensor is grown to the workspace the shape needs"""
-    U, dev = int(users.numel()), g.device
+def _check_top(m):
+    """None, or the count m in [1, IGMC_TOPK_MAX] of ratings an explanation keeps per pair"""
+    return None if m is None else _check_count(m, "m", _lib.TOPK_MAX)
+
+
+def _ranking_inputs(k, batch_size, items, retrieve, U, num_items):
+    """(k, m, cand, rows) of a ranking run over U query slots, checked on the host: m = ``retrieve`` (or None), cand
+    the sorted distinct items of a 1-D ``items`` (or None), rows a 2-D ``items`` as ``_user_rows`` returns it (or
+    None)"""
+    k = _check_count(k, "k", _lib.TOPK_MAX)
+    _check_merge_fits(k, batch_size)
+    if retrieve is not None and items is not None:
+        raise ValueError("retrieve= chooses the candidates itself: pass it without items=")
+    m = None if retrieve is None else _check_count(retrieve, "retrieve", num_items, ValueError)
+    if _is_rows(items):
+        return k, m, None, _user_rows(items, U, num_items)
+    return k, m, None if items is None else np.unique(_host_ids(items, "items", num_items)), None
+
+
+def _corated(lib, g, entry, args, U, m, exclude_rated, err, ws):
+    """the retriever ``entry`` (igmc_corated_items or igmc_corated_sessions, leading arguments ``args``) for U query
+    slots on graph ``g``: (items, paths) [U, m] int32.  ``ws``: a dict whose "ws" tensor is grown to the workspace the
+    shape needs"""
+    dev = g.device
     nbytes = C.c_int64(0)
     _lib.check(lib.igmc_corated_ws_bytes(g.num_users, g.num_items, U, m, C.byref(nbytes)), "igmc_corated_ws_bytes")
     if ws.get("ws") is None or ws["ws"].numel() < nbytes.value:
         ws["ws"] = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=dev)
     items = torch.empty(U, m, dtype=torch.int32, device=dev)
     paths = torch.empty(U, m, dtype=torch.int32, device=dev)
-    _lib.check(lib.igmc_corated_items(C.byref(g._c), users.data_ptr(), U, m, int(bool(exclude_rated)),
-                                      ws["ws"].data_ptr(), ws["ws"].numel(), items.data_ptr(), paths.data_ptr(),
-                                      err.data_ptr(), _stream_ptr()), "igmc_corated_items")
+    _lib.check(getattr(lib, entry)(*args, m, int(bool(exclude_rated)), ws["ws"].data_ptr(), ws["ws"].numel(),
+                                   items.data_ptr(), paths.data_ptr(), err.data_ptr(), _stream_ptr()), entry)
     return items, paths
-
-
-def _check_k(k):
-    k = int(k)
-    if k < 1:
-        raise ValueError("k must be >= 1, not %d" % k)
-    if k > _lib.TOPK_MAX:
-        raise NotImplementedError("the top-k merge kernel keeps at most k = %d items per user" % _lib.TOPK_MAX)
-    return k
 
 
 def _check_merge_fits(k, batch_size):
@@ -152,13 +161,15 @@ def _host_y(y, name, n):
     return y.astype(np.float32)
 
 
-def _host_pairs(shape, users, items, y=None, name="pairs"):
-    """(users, items, y or None) checked on the host: ids in range, matching lengths, finite y"""
+def _host_pairs(shape, users, items, y=None, name="", first="users"):
+    """(users, items, y or None) checked on the host: ids in range of ``shape``, matching lengths, finite y.  ``name``:
+    the argument the pairs came in (train, test), ``first``: what the first array holds"""
+    pre = name + " " if name else ""
     nu, ni = shape
-    users, items = _host_ids(users, name + " users", nu), _host_ids(items, name + " items", ni)
+    users, items = _host_ids(users, pre + first, nu), _host_ids(items, pre + "items", ni)
     if len(users) != len(items):
-        raise ValueError("%s: users and items must have the same length (%d vs %d)" % (name, len(users), len(items)))
-    return users, items, (None if y is None else _host_y(y, name + " y", len(users)))
+        raise ValueError("%s%s and items must have the same length (%d vs %d)" % (pre, first, len(users), len(items)))
+    return users, items, (None if y is None else _host_y(y, pre + "y", len(users)))
 
 
 def _split_pairs(pairs, name, need_y):
@@ -181,37 +192,26 @@ def _check_lrs(lrs, K):
     return lrs
 
 
-def _check_influence_k(k):
-    k = int(k)
-    if k < 1:
-        raise ValueError("k must be >= 1, not %d" % k)
-    if k > _lib.TOPK_MAX:
-        raise NotImplementedError("an influence run keeps at most k = %d training pairs per test pair" % _lib.TOPK_MAX)
-    return k
-
-
 def _check_test_count(T):
     if T > INFLUENCE_T_MAX:
         raise NotImplementedError("an influence run takes at most %d test pairs, not %d: split the test set"
                                   % (INFLUENCE_T_MAX, T))
 
 
+def _influence_inputs(shape, train, test, k, batch_size, lrs, K):
+    """(k, train, test, lrs) of an influence run checked on the host; train and test as ``_host_pairs`` returns them"""
+    k = _check_count(k, "k", _lib.TOPK_MAX)
+    _check_merge_fits(k, batch_size)
+    tr = _host_pairs(shape, *_split_pairs(train, "train", True), name="train")
+    te = _host_pairs(shape, *_split_pairs(test, "test", False), name="test")
+    _check_test_count(len(te[0]))
+    return k, tr, te, _check_lrs(lrs, K)
+
+
 def _check_per_pair_model(model):
     if model._cmodel.readout != 0:
         raise NotImplementedError("per-pair gradients need the IGMC readout: DGCNN_RS's SortPooling readout gradient "
                                   "is summed over the batch")
-
-
-def _check_top(m, name):
-    """None, or a count in [1, IGMC_TOPK_MAX] of entries to keep per pair"""
-    if m is None:
-        return None
-    m = int(m)
-    if m < 1:
-        raise ValueError("%s must be >= 1, not %d" % (name, m))
-    if m > _lib.TOPK_MAX:
-        raise NotImplementedError("an explanation keeps at most %s = %d ratings per pair" % (name, _lib.TOPK_MAX))
-    return m
 
 
 # The result of explain_pairs, device tensors: score [P] fp32 (= predict_pairs), num_edges [P] int32 (the ratings of
@@ -538,35 +538,6 @@ def session_rows_host(host, shape, users, session, items, values):
     return new_rp.astype(np.int32), new_ci.astype(np.int32), new_rt.astype(np.uint8)
 
 
-def _session_inputs(S, num_items, session, items, values):
-    """(session, items, values, D) of the edits: host arrays validated here (IndexError for a session or item id
-    out of range, ValueError for a value outside 0..256 or unequal lengths); int32 device tensors are passed on and
-    checked by the kernel"""
-    arrs = []
-    for name, a in (("session", session), ("items", items), ("values", values)):
-        if torch.is_tensor(a) and a.device.type == "cuda":
-            if a.is_floating_point() or a.is_complex() or a.dtype == torch.bool:
-                raise TypeError("%s must be integers, not %s" % (name, a.dtype))
-            arrs.append(a.reshape(-1))
-            continue
-        a = np.asarray(a.cpu().numpy() if torch.is_tensor(a) else a).reshape(-1)
-        if a.size and not np.issubdtype(a.dtype, np.integer):
-            raise TypeError("%s must be integers, not %s" % (name, a.dtype))
-        arrs.append(a.astype(np.int64))
-    n = [int(a.numel()) if torch.is_tensor(a) else len(a) for a in arrs]
-    if len(set(n)) != 1:
-        raise ValueError("session, items and values must have the same length (%d, %d, %d)" % tuple(n))
-    for a, name, hi in ((arrs[0], "session", S), (arrs[1], "items", num_items)):
-        if not torch.is_tensor(a) and a.size and (a.min() < 0 or a.max() >= hi):
-            bad = int(a.min()) if a.min() < 0 else int(a.max())
-            raise IndexError("%s: id %d out of range [0, %d)" % (name, bad, hi))
-    x = arrs[2]
-    if not torch.is_tensor(x) and x.size and (x.min() < 0 or x.max() > 256):
-        raise ValueError("values must be rating label + 1 (1..256) or 0 (delete), got %d"
-                         % (int(x.min()) if x.min() < 0 else int(x.max())))
-    return arrs[0], arrs[1], arrs[2], n[0]
-
-
 class RatingSessions(object):
     """Users described by ratings passed with the query, scored without changing the rating graph.
 
@@ -593,8 +564,8 @@ class RatingSessions(object):
         S = int(u.numel())
         if S < 1:
             raise ValueError("a RatingSessions holds at least one session")
-        sess, it, val, D = _session_inputs(S, graph.num_items, session, items, values)
-        sess, it, val = (_on_dev_i32(a, dev) for a in (sess, it, val))
+        sess, it, val, D = _update_inputs(session, items, values, S, graph.num_items, ("session", "items", "values"))
+        sess, it, val = (_on_device_i32(a, dev) for a in (sess, it, val))
         lib = _lib.load()
         nbytes = C.c_int64(0)
         _lib.check(lib.igmc_session_ws_bytes(S, D, graph.num_items, C.byref(nbytes)), "igmc_session_ws_bytes")
@@ -642,25 +613,12 @@ class RatingSessions(object):
         return (self.row_ptr.cpu().numpy(), self.col_idx[:n].cpu().numpy(), self.rating[:n].cpu().numpy())
 
 
-def _on_dev_i32(a, dev):
-    if torch.is_tensor(a) and a.device.type == "cuda":
-        return (a if a.dtype == torch.int32 else a.clamp(-1, 2 ** 31 - 1).to(torch.int32)).contiguous()
-    return torch.from_numpy(np.clip(np.asarray(a, np.int64), -1, 2 ** 31 - 1).astype(np.int32)).to(dev)
-
-
-def _corated_sessions(lib, sessions, m, exclude_rated, err, ws):
-    """igmc_corated_sessions: (items, paths) [S, m] int32"""
-    g, S, dev = sessions.graph, sessions.num_sessions, sessions.graph.device
-    nbytes = C.c_int64(0)
-    _lib.check(lib.igmc_corated_ws_bytes(g.num_users, g.num_items, S, m, C.byref(nbytes)), "igmc_corated_ws_bytes")
-    if ws.get("ws") is None or ws["ws"].numel() < nbytes.value:
-        ws["ws"] = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=dev)
-    items = torch.empty(S, m, dtype=torch.int32, device=dev)
-    paths = torch.empty(S, m, dtype=torch.int32, device=dev)
-    _lib.check(lib.igmc_corated_sessions(C.byref(g._c), C.byref(sessions._c), m, int(bool(exclude_rated)),
-                                         ws["ws"].data_ptr(), ws["ws"].numel(), items.data_ptr(), paths.data_ptr(),
-                                         err.data_ptr(), _stream_ptr()), "igmc_corated_sessions")
-    return items, paths
+def _check_sessions(sessions, graph=None):
+    """``sessions`` when it is a RatingSessions of ``graph`` (default: its own) as it is now"""
+    if not isinstance(sessions, RatingSessions):
+        raise TypeError("sessions must be a RatingSessions")
+    sessions.check(graph)
+    return sessions
 
 
 # ---- the engine -----------------------------------------------------------------------------------------------------
@@ -728,80 +686,94 @@ class InferenceEngine(object):
         """plan a ranking run (one host sync: the candidate total).  ``items``: one candidate list for every user, or
         a 2-D [U, width] array of per-user lists (-1 = empty slot); ``retrieve=M``: each user's M items with the most
         bridges (``corated_items``) are its candidates.  Returns the number of candidate pairs."""
-        k = _check_k(k)
-        _check_merge_fits(k, self.B)
         g = self.graph
-        if retrieve is not None and items is not None:
-            raise ValueError("retrieve= chooses the candidates itself: pass it without items=")
-        per_user = retrieve is not None or _is_rows(items)
-        m = None if retrieve is None else _check_m(retrieve, g.num_items)
         users = _host_ids(users, "users", g.num_users)
-        cand = None if items is None or per_user else np.unique(_host_ids(items, "items", g.num_items))
-        U, dev = len(users), self.dev
-        rows = _user_rows(items, U, g.num_items, dev) if per_user and m is None else None
-        run = dict(kind="recommend", U=U, k=k, version=g.version,
+        k, m, cand, rows = _ranking_inputs(k, self.B, items, retrieve, len(users), g.num_items)
+        slots = torch.from_numpy(users.astype(np.int32)).to(self.dev)
+
+        def rated():     # the users' summed row lengths (host row pointers: a copy after an update)
+            rp = g.host["row_ptr"]
+            return int((rp[users + 1] - rp[users]).sum())
+        return self._plan_ranking(slots, k, m, cand, rows, exclude_rated, rated,
+                                  "igmc_corated_items", (C.byref(g._c), slots.data_ptr(), len(users)))
+
+    def start_session_recommend(self, sessions, k, items=None, exclude_rated=True, retrieve=None):
+        """plan a ranking run over the sessions (``recommend_sessions``): query slot s is session s, its candidates and
+        rated items come from its session row.  Arguments as ``start_recommend``'s.  Returns the number of candidate
+        pairs."""
+        sessions = self._session_slots(sessions)
+        k, m, cand, rows = _ranking_inputs(k, self.B, items, retrieve, sessions.num_sessions, self.graph.num_items)
+        return self._plan_ranking(sessions._slots, k, m, cand, rows, exclude_rated, lambda: sessions.nnz,
+                                  "igmc_corated_sessions", (C.byref(self.graph._c), C.byref(sessions._c)), sessions)
+
+    def _plan_ranking(self, slots, k, m, cand, rows, exclude_rated, rated, retriever, args, sessions=None):
+        """the plan of a ranking run over the query slots ``slots`` (int32, on the device) with ``_ranking_inputs``'
+        (k, m, cand, rows): the candidate plan over every item or the list ``cand`` (``rated()``: the slots' summed row
+        lengths, room for their rated positions in the list), or per-slot rows from ``rows`` or from the retriever entry
+        ``retriever`` (leading arguments ``args``).  ``sessions``: the slots are these sessions.  Returns the number of
+        candidate pairs."""
+        U, dev = int(slots.numel()), self.dev
+        run = dict(kind="recommend", U=U, k=k, version=self.graph.version, sessions=sessions, users=slots,
                    top_s=torch.full((U, k), -float("inf"), dtype=torch.float32, device=dev),
                    top_i=torch.full((U, k), -1, dtype=torch.int64, device=dev))
         self.run = run
         if U == 0 or (cand is not None and len(cand) == 0) or (rows is not None and rows.shape[1] == 0):
             run["P"] = 0
             return 0
-        i64 = dict(dtype=torch.int64, device=dev)
-        run["users"] = torch.from_numpy(users.astype(np.int32)).to(dev)
-        if per_user:
-            return self._plan_lists(run, rows, m, exclude_rated)
+        if m is not None:
+            rows, _ = _corated(self.lib, self.graph, retriever, args, U, m, exclude_rated, self.extractor.err,
+                               self._retrieve_ws)
+        if rows is not None:
+            return self._plan_lists(run, rows, exclude_rated)
+        Cd = self._query_candidates(run, exclude_rated)
         run["cand"] = None if cand is None else torch.from_numpy(cand.astype(np.int32)).to(dev)
-        run["user_off"] = torch.zeros(U + 1, **i64)
-        lists = cand is not None and bool(exclude_rated)
-        if lists:
-            rp = g.host["row_ptr"]
-            run["rated_off"] = torch.zeros(U + 1, **i64)
-            run["rated_pos"] = torch.zeros(max(int((rp[users + 1] - rp[users]).sum()), 1), dtype=torch.int32,
-                                           device=dev)
-        Cd = _lib.Candidates()
-        Cd.users, Cd.cand = run["users"].data_ptr(), _lib.ptr(run["cand"])
-        Cd.user_off = run["user_off"].data_ptr()
+        if cand is not None and exclude_rated:
+            run["rated_off"] = torch.zeros(U + 1, dtype=torch.int64, device=dev)
+            run["rated_pos"] = torch.zeros(max(rated(), 1), dtype=torch.int32, device=dev)
+        Cd.cand, Cd.num_cand = _lib.ptr(run["cand"]), 0 if cand is None else len(cand)
         Cd.rated_off, Cd.rated_pos = _lib.ptr(run.get("rated_off")), _lib.ptr(run.get("rated_pos"))
-        Cd.num_query, Cd.num_cand = U, 0 if cand is None else len(cand)
-        Cd.exclude_rated = int(bool(exclude_rated))
         _lib.check(self.lib.igmc_candidate_plan(C.byref(self._csr(run)), C.byref(Cd), self.extractor.err.data_ptr(),
                                                 _stream_ptr()), "igmc_candidate_plan")
-        Cd.num_pairs = run["P"] = int(run["user_off"][U].item())
-        run["Cd"] = Cd
-        if run["P"] > 0:
-            self._prime()
-        return run["P"]
+        return self._planned(run)
 
-    def _plan_lists(self, run, rows, m, exclude_rated):
-        """the plan of a run over per-user candidate rows (``rows``, or the retriever's top ``m`` per user):
+    def _plan_lists(self, run, rows, exclude_rated):
+        """the plan of a run over per-slot candidate rows [U, width] (a host array or a device tensor):
         igmc_candidate_lists compacts them into run["lists"] and user_off"""
-        g, U, dev = self.graph, run["U"], self.dev
-        err = self.extractor.err
-        if rows is None:
-            rows, _ =_corated(self.lib, g, run["users"], m, exclude_rated, err, self._retrieve_ws)
+        U, dev, err = run["U"], self.dev, self.extractor.err
+        rows = run["rows"] = torch.as_tensor(rows, device=dev).to(torch.int32).contiguous()
         width = int(rows.shape[1])
-        run["rows"] = rows
         run["lists"] = torch.empty(max(U * width, 1), dtype=torch.int32, device=dev)
-        run["user_off"] = torch.zeros(U + 1, dtype=torch.int64, device=dev)
         nbytes = C.c_int64(0)
         _lib.check(self.lib.igmc_candidate_lists_ws_bytes(U, width, C.byref(nbytes)), "igmc_candidate_lists_ws_bytes")
         run["lists_ws"] = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=dev)
-        Cd = _lib.Candidates()
-        Cd.users, Cd.user_off = run["users"].data_ptr(), run["user_off"].data_ptr()
-        Cd.num_query, Cd.exclude_rated = U, int(bool(exclude_rated))
+        Cd = self._query_candidates(run, exclude_rated)
         _lib.check(self.lib.igmc_candidate_lists(C.byref(self._csr(run)), C.byref(Cd), rows.data_ptr(), width,
                                                  run["lists"].data_ptr(), run["lists_ws"].data_ptr(),
                                                  run["lists_ws"].numel(), err.data_ptr(), _stream_ptr()),
                    "igmc_candidate_lists")
         Cd.cand, Cd.per_user = run["lists"].data_ptr(), 1
-        Cd.num_pairs = run["P"] = int(run["user_off"][U].item())
-        run["Cd"] = Cd
+        return self._planned(run)
+
+    def _query_candidates(self, run, exclude_rated):
+        """run["Cd"] over the query slots run["users"], with their count prefix run["user_off"] (zeroed)"""
+        U = run["U"]
+        run["user_off"] = torch.zeros(U + 1, dtype=torch.int64, device=self.dev)
+        Cd = run["Cd"] = _lib.Candidates()
+        Cd.users, Cd.user_off, Cd.num_query = run["users"].data_ptr(), run["user_off"].data_ptr(), U
+        Cd.exclude_rated = int(bool(exclude_rated))
+        return Cd
+
+    def _planned(self, run):
+        """after the plan of a ranking run: its pair total (the run's one host sync), the first batch primed.  Returns
+        the total."""
+        run["Cd"].num_pairs = run["P"] = int(run["user_off"][run["U"]].item())
         if run["P"] > 0:
             self._prime()
         return run["P"]
 
     def start_pairs(self, users, items):
         """plan a run over the explicit pairs (users[i], items[i]).  Returns their number."""
+        users, items, _ = _host_pairs(self.graph.shape, users, items)
         return self._start_explicit("pairs", users, items)
 
     # ---- rating sessions ----------------------------------------------------------------------------------------
@@ -809,10 +781,9 @@ class InferenceEngine(object):
         """the rows the candidate kernels read: the graph's, or a session run's rows as a CSR over its sessions"""
         return run["sessions"]._view if run.get("sessions") is not None else self.graph._c
 
-    def _check_sessions(self, sessions):
-        if not isinstance(sessions, RatingSessions):
-            raise TypeError("sessions must be a RatingSessions")
-        sessions.check(self.graph)
+    def _session_slots(self, sessions):
+        """``sessions`` checked against the engine's graph, and the per-slot session index buffers"""
+        _check_sessions(sessions, self.graph)
         for s in self.slots:
             if "sess" not in s:
                 s["sess"] = torch.zeros(self.B, dtype=torch.int32, device=self.dev)
@@ -821,87 +792,25 @@ class InferenceEngine(object):
     def start_session_pairs(self, sessions, session, items):
         """plan a run over the pairs (sessions.users[session[i]], items[i]), each scored with its target user's row
         taken from session ``session[i]`` (``predict_sessions``).  Returns their number."""
-        sessions = self._check_sessions(sessions)
-        g = self.graph
-        sess = _host_ids(session, "session", sessions.num_sessions)
-        items = _host_ids(items, "items", g.num_items)
-        if len(sess) != len(items):
-            raise ValueError("session and items must have the same length (%d vs %d)" % (len(sess), len(items)))
-        P, dev = len(sess), self.dev
-        run = dict(kind="pairs", P=P, version=g.version, sessions=sessions,
-                   scores=torch.empty(P, dtype=torch.float32, device=dev))
-        self.run = run
-        if P == 0:
-            return 0
-        run["pu"] = torch.from_numpy(sess.astype(np.int32)).to(dev)
-        run["pv"] = torch.from_numpy(items.astype(np.int32)).to(dev)
-        Cd = _lib.Candidates()
-        Cd.pair_u, Cd.pair_v, Cd.num_pairs = run["pu"].data_ptr(), run["pv"].data_ptr(), P
-        run["Cd"] = Cd
-        self._prime()
-        return P
-
-    def start_session_recommend(self, sessions, k, items=None, exclude_rated=True, retrieve=None):
-        """plan a ranking run over the sessions (``recommend_sessions``): query slot s is session s, its candidates and
-        rated items come from its session row.  Arguments as ``start_recommend``'s.  Returns the number of candidate
-        pairs."""
-        k = _check_k(k)
-        _check_merge_fits(k, self.B)
-        sessions = self._check_sessions(sessions)
-        g = self.graph
-        if retrieve is not None and items is not None:
-            raise ValueError("retrieve= chooses the candidates itself: pass it without items=")
-        per_user = retrieve is not None or _is_rows(items)
-        m = None if retrieve is None else _check_m(retrieve, g.num_items)
-        S, dev = sessions.num_sessions, self.dev
-        cand = None if items is None or per_user else np.unique(_host_ids(items, "items", g.num_items))
-        rows = _user_rows(items, S, g.num_items, dev) if per_user and m is None else None
-        run = dict(kind="recommend", U=S, k=k, version=g.version, sessions=sessions,
-                   top_s=torch.full((S, k), -float("inf"), dtype=torch.float32, device=dev),
-                   top_i=torch.full((S, k), -1, dtype=torch.int64, device=dev))
-        self.run = run
-        if (cand is not None and len(cand) == 0) or (rows is not None and rows.shape[1] == 0):
-            run["P"] = 0
-            return 0
-        run["users"] = sessions._slots
-        if per_user:
-            if rows is None:
-                rows, _ = _corated_sessions(self.lib, sessions, m, exclude_rated, self.extractor.err,
-                                            self._retrieve_ws)
-            return self._plan_lists(run, rows, None, exclude_rated)
-        i64 = dict(dtype=torch.int64, device=dev)
-        run["cand"] = None if cand is None else torch.from_numpy(cand.astype(np.int32)).to(dev)
-        run["user_off"] = torch.zeros(S + 1, **i64)
-        if cand is not None and exclude_rated:
-            run["rated_off"] = torch.zeros(S + 1, **i64)
-            run["rated_pos"] = torch.zeros(max(sessions.nnz, 1), dtype=torch.int32, device=dev)
-        Cd = _lib.Candidates()
-        Cd.users, Cd.cand = run["users"].data_ptr(), _lib.ptr(run["cand"])
-        Cd.user_off = run["user_off"].data_ptr()
-        Cd.rated_off, Cd.rated_pos = _lib.ptr(run.get("rated_off")), _lib.ptr(run.get("rated_pos"))
-        Cd.num_query, Cd.num_cand = S, 0 if cand is None else len(cand)
-        Cd.exclude_rated = int(bool(exclude_rated))
-        _lib.check(self.lib.igmc_candidate_plan(C.byref(sessions._view), C.byref(Cd), self.extractor.err.data_ptr(),
-                                                _stream_ptr()), "igmc_candidate_plan")
-        Cd.num_pairs = run["P"] = int(run["user_off"][S].item())
-        run["Cd"] = Cd
-        if run["P"] > 0:
-            self._prime()
-        return run["P"]
+        sessions = self._session_slots(sessions)
+        sess, items, _ = _host_pairs((sessions.num_sessions, self.graph.num_items), session, items, first="session")
+        return self._start_explicit("pairs", sess, items, sessions=sessions)
 
     def start_explain(self, users, items, m=None):
         """plan an explanation run over the explicit pairs (users[i], items[i]) (``explain_pairs``): the base pass
         scores them and counts their subgraphs' ratings; once it is done, ``step`` reads the total (the run's one host
         sync) and goes on with the occlusion pass.  ``m``: keep each pair's first m ratings.  Returns the number of
         pairs."""
-        m = _check_top(m, "m")
+        m = _check_top(m)
+        users, items, _ = _host_pairs(self.graph.shape, users, items)
         return self._start_explicit("explain", users, items, m=m, phase="base")
 
     def start_attribute(self, users, items, m=None):
         """plan an attribution run over the explicit pairs (users[i], items[i]) (``attribute_pairs``): the base pass of
         ``start_explain``, then (after the run's one host sync, the rating total) a gradient pass over the same pairs.
         ``m``: keep each pair's first m ratings.  Returns the number of pairs."""
-        m = _check_top(m, "m")
+        m = _check_top(m)
+        users, items, _ = _host_pairs(self.graph.shape, users, items)
         return self._start_explicit("attribute", users, items, m=m, phase="base")
 
     def start_pair_gradients(self, users, items, y=None):
@@ -917,26 +826,16 @@ class InferenceEngine(object):
         every checkpoint's test gradients, then a training pass over ``train`` = (users, items, y) that accumulates
         S[b, t] = sum_k lrs[k] <G_b, G_t> per batch and merges it into each test pair's top-k lists.  Returns the
         number of test pairs."""
-        k = _check_influence_k(k)
-        _check_merge_fits(k, self.B)
         _check_per_pair_model(self.model)
-        tr = _host_pairs(self.graph.shape, *_split_pairs(train, "train", True), name="train")
-        te = _host_pairs(self.graph.shape, *_split_pairs(test, "test", False), name="test")
-        T = len(te[0])
-        _check_test_count(T)
-        lrs = _check_lrs(lrs, self.K)
-        m, dev = self.model._cmodel, self.dev
+        k, tr, te, lrs = _influence_inputs(self.graph.shape, train, test, k, self.B, lrs, self.K)
+        T, m, dev = len(te[0]), self.model._cmodel, self.dev
         f32, i64 = dict(dtype=torch.float32, device=dev), dict(dtype=torch.int64, device=dev)
         FW = self.lib.igmc_pair_factor_count(C.byref(m))
         extra = dict(phase="test", train=tr, lrs=lrs, k=k, T=T, y=self._dev_y(te[2]),
                      tconv=torch.zeros(self.K, T, m.conv_param_count, **f32), tfac=torch.zeros(self.K, T, FW, **f32),
                      pro_i=torch.full((T, k), -1, **i64), pro_v=torch.full((T, k), -float("inf"), **f32),
                      con_i=torch.full((T, k), -1, **i64), con_v=torch.full((T, k), float("inf"), **f32), self_out=None)
-        if T == 0:
-            self.run = dict(kind="influence", P=0, version=self.graph.version, **extra)
-            return 0
-        self._start_explicit("influence", te[0], te[1], **extra)
-        return T
+        return self._start_explicit("influence", te[0], te[1], **extra)
 
     def start_self_influence(self, train, lrs=None):
         """plan a self-influence run (``self_influence``) over ``train`` = (users, items, y).  Returns its size."""
@@ -974,11 +873,7 @@ class InferenceEngine(object):
         if run["P"] == 0:
             run["steps"] = run["done"] = 0
             return False
-        run["pu"] = torch.from_numpy(users.astype(np.int32)).to(self.dev)
-        run["pv"] = torch.from_numpy(items.astype(np.int32)).to(self.dev)
-        Cd = _lib.Candidates()
-        Cd.pair_u, Cd.pair_v, Cd.num_pairs = run["pu"].data_ptr(), run["pv"].data_ptr(), run["P"]
-        run["Cd"] = Cd
+        self._explicit_pairs(run, users, items)
         self._train_buffers()
         self._prime()
         return True
@@ -1032,13 +927,11 @@ class InferenceEngine(object):
                        "igmc_influence_topk")
 
     def _start_explicit(self, kind, users, items, **extra):
-        g = self.graph
-        users = _host_ids(users, "users", g.num_users)
-        items = _host_ids(items, "items", g.num_items)
-        if len(users) != len(items):
-            raise ValueError("users and items must have the same length (%d vs %d)" % (len(users), len(items)))
+        """plan a run over the explicit pairs (users[i], items[i]), host arrays ``_host_pairs`` checked.  Returns their
+        number."""
         P, dev = len(users), self.dev
-        run = dict(kind=kind, P=P, version=g.version, scores=torch.empty(P, dtype=torch.float32, device=dev), **extra)
+        run = dict(kind=kind, P=P, version=self.graph.version, scores=torch.empty(P, dtype=torch.float32, device=dev),
+                   **extra)
         self.run = run
         if kind in ("explain", "attribute"):
             run["num_edges"] = torch.zeros(P, dtype=torch.int32, device=dev)
@@ -1048,13 +941,16 @@ class InferenceEngine(object):
                     s["j"] = torch.zeros(self.B, dtype=torch.int32, device=dev)
         if P == 0:
             return 0
-        run["pu"] = torch.from_numpy(users.astype(np.int32)).to(dev)
-        run["pv"] = torch.from_numpy(items.astype(np.int32)).to(dev)
-        Cd = _lib.Candidates()
-        Cd.pair_u, Cd.pair_v, Cd.num_pairs = run["pu"].data_ptr(), run["pv"].data_ptr(), P
-        run["Cd"] = Cd
+        self._explicit_pairs(run, users, items)
         self._prime()
         return P
+
+    def _explicit_pairs(self, run, users, items):
+        """run["pu"], run["pv"] and run["Cd"]: the explicit pairs (users[i], items[i]) on the device"""
+        run["pu"] = torch.from_numpy(users.astype(np.int32)).to(self.dev)
+        run["pv"] = torch.from_numpy(items.astype(np.int32)).to(self.dev)
+        Cd = run["Cd"] = _lib.Candidates()
+        Cd.pair_u, Cd.pair_v, Cd.num_pairs = run["pu"].data_ptr(), run["pv"].data_ptr(), len(users)
 
     def _rating_total(self, phase):
         """after the base pass of an explanation or attribution run: the offsets of the pairs' ratings, their total T
@@ -1375,22 +1271,35 @@ class InferenceEngine(object):
 
 
 # ---- public API -----------------------------------------------------------------------------------------------------
+def _on_engine(model, graph, call, h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed):
+    """``call(engine)`` on an InferenceEngine of ``model`` and ``graph`` built with the public functions' keywords,
+    closed afterwards"""
+    eng = InferenceEngine(model, graph, h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
+    try:
+        return call(eng)
+    finally:
+        eng.close()
+
+
+def _no_pairs_explained(cls, m, dev):
+    """the Explanation or Attribution (``cls``) of no pairs: [0] / [1] offsets / [0] or [0, m] per-rating tensors"""
+    shape = (0, m) if m else (0,)
+    i32 = dict(dtype=torch.int32, device=dev)
+    return cls(torch.zeros(0, dtype=torch.float32, device=dev), torch.zeros(0, **i32),
+               torch.zeros(1, dtype=torch.int64, device=dev), torch.zeros(shape, **i32), torch.zeros(shape, **i32),
+               torch.zeros(shape, **i32), torch.zeros(shape, dtype=torch.float32, device=dev))
+
+
 def predict_pairs(model, graph, users, items, *, h=1, sample_ratio=1.0, max_nodes_per_hop=None, batch_size=256,
                   checkpoints=None, sample_seed=0):
     """eval-mode scores [P] (fp32, on the model's device) of the pairs (users[i], items[i]); a pair rated in ``graph``
     is scored on its subgraph without the target edge, as in training.  ``checkpoints``: average of the checkpoints'
     scores (fp32 sum in checkpoint order / K)."""
-    nu, ni = graph.shape
-    users, items = _host_ids(users, "users", nu), _host_ids(items, "items", ni)
-    if len(users) != len(items):
-        raise ValueError("users and items must have the same length (%d vs %d)" % (len(users), len(items)))
+    users, items, _ = _host_pairs(graph.shape, users, items)
     if len(users) == 0:
         return torch.zeros(0, dtype=torch.float32, device=model.flat_params.device)
-    eng = InferenceEngine(model, graph, h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
-    try:
-        return eng.predict_pairs(users, items)
-    finally:
-        eng.close()
+    return _on_engine(model, graph, lambda eng: eng.predict_pairs(users, items),
+                      h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
 
 
 def explain_pairs(model, graph, users, items, m=None, *, h=1, sample_ratio=1.0, max_nodes_per_hop=None, batch_size=256,
@@ -1403,24 +1312,12 @@ def explain_pairs(model, graph, users, items, m=None, *, h=1, sample_ratio=1.0, 
     rating's position in the subgraph's edge_index; flat with pair p at [offsets[p], offsets[p+1]) when ``m`` is None,
     else the first ``m`` per pair [P, m], padded with user / item / rating -1 and delta 0.  ``checkpoints``: every score
     is the fp32 checkpoint mean, as in ``predict_pairs``."""
-    nu, ni = graph.shape
-    m = _check_top(m, "m")
-    users, items = _host_ids(users, "users", nu), _host_ids(items, "items", ni)
-    if len(users) != len(items):
-        raise ValueError("users and items must have the same length (%d vs %d)" % (len(users), len(items)))
+    m = _check_top(m)
+    users, items, _ = _host_pairs(graph.shape, users, items)
     if len(users) == 0:
-        dev = model.flat_params.device
-        shape = (0, m) if m else (0,)
-        i32 = dict(dtype=torch.int32, device=dev)
-        return Explanation(torch.zeros(0, dtype=torch.float32, device=dev), torch.zeros(0, **i32),
-                           torch.zeros(1, dtype=torch.int64, device=dev), torch.zeros(shape, **i32),
-                           torch.zeros(shape, **i32), torch.zeros(shape, **i32),
-                           torch.zeros(shape, dtype=torch.float32, device=dev))
-    eng = InferenceEngine(model, graph, h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
-    try:
-        return eng.explain_pairs(users, items, m)
-    finally:
-        eng.close()
+        return _no_pairs_explained(Explanation, m, model.flat_params.device)
+    return _on_engine(model, graph, lambda eng: eng.explain_pairs(users, items, m),
+                      h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
 
 
 def attribute_pairs(model, graph, users, items, m=None, *, h=1, sample_ratio=1.0, max_nodes_per_hop=None,
@@ -1437,24 +1334,12 @@ def attribute_pairs(model, graph, users, items, m=None, *, h=1, sample_ratio=1.0
     by position; the first ``m`` per pair [P, m] padded with -1 / -1 / -1 / 0.  The gradient pass runs the L2 kernel
     plan whatever plan the model uses.  ``checkpoints``: score and grad are fp32 checkpoint means (sum in checkpoint
     order / K)."""
-    nu, ni = graph.shape
-    m = _check_top(m, "m")
-    users, items = _host_ids(users, "users", nu), _host_ids(items, "items", ni)
-    if len(users) != len(items):
-        raise ValueError("users and items must have the same length (%d vs %d)" % (len(users), len(items)))
+    m = _check_top(m)
+    users, items, _ = _host_pairs(graph.shape, users, items)
     if len(users) == 0:
-        dev = model.flat_params.device
-        shape = (0, m) if m else (0,)
-        i32 = dict(dtype=torch.int32, device=dev)
-        return Attribution(torch.zeros(0, dtype=torch.float32, device=dev), torch.zeros(0, **i32),
-                           torch.zeros(1, dtype=torch.int64, device=dev), torch.zeros(shape, **i32),
-                           torch.zeros(shape, **i32), torch.zeros(shape, **i32),
-                           torch.zeros(shape, dtype=torch.float32, device=dev))
-    eng = InferenceEngine(model, graph, h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
-    try:
-        return eng.attribute_pairs(users, items, m)
-    finally:
-        eng.close()
+        return _no_pairs_explained(Attribution, m, model.flat_params.device)
+    return _on_engine(model, graph, lambda eng: eng.attribute_pairs(users, items, m),
+                      h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
 
 
 def pair_gradients(model, graph, users, items, y=None, *, h=1, sample_ratio=1.0, max_nodes_per_hop=None,
@@ -1473,11 +1358,8 @@ def pair_gradients(model, graph, users, items, y=None, *, h=1, sample_ratio=1.0,
     if len(users) == 0:
         K = len(checkpoints) if checkpoints else 1
         return torch.zeros(K, 0, model._cmodel.param_count, dtype=torch.float32, device=model.flat_params.device)
-    eng = InferenceEngine(model, graph, h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
-    try:
-        return eng.pair_gradients(users, items, y)
-    finally:
-        eng.close()
+    return _on_engine(model, graph, lambda eng: eng.pair_gradients(users, items, y),
+                      h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
 
 
 def influence(model, graph, train, test, k, *, checkpoints=None, lrs=None, h=1, sample_ratio=1.0,
@@ -1493,18 +1375,14 @@ def influence(model, graph, train, test, k, *, checkpoints=None, lrs=None, h=1, 
     largest values (pro_*) and the k smallest (con_*) per test pair, index = position in ``train``; ties by index, NaN
     after every number, empty slots -1 / -inf (pro) and -1 / +inf (con).  Conv block by a split-K FFMA GEMM, readout
     block from its rank-1 factors; bit-identical across runs, batch sizes and graph replay.  IGMC only."""
-    k = _check_influence_k(k)
-    _check_merge_fits(k, batch_size)
     _check_per_pair_model(model)
-    users, items, y = _host_pairs(graph.shape, *_split_pairs(train, "train", True), name="train")
-    tu, ti, ty = _host_pairs(graph.shape, *_split_pairs(test, "test", False), name="test")
-    _check_test_count(len(tu))
-    _check_lrs(lrs, len(checkpoints) if checkpoints else 1)
-    eng = InferenceEngine(model, graph, h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
-    try:
-        return eng.influence((users, items, y), (tu, ti, ty), k, lrs)
-    finally:
-        eng.close()
+    k, tr, te, lrs = _influence_inputs(graph.shape, train, test, k, batch_size, lrs,
+                                       len(checkpoints) if checkpoints else 1)
+    if len(te[0]) == 0:
+        dev = model.flat_params.device
+        return Influence(*(torch.zeros(0, k, dtype=t, device=dev) for t in (torch.int64, torch.float32) * 2))
+    return _on_engine(model, graph, lambda eng: eng.influence(tr, te, k, lrs),
+                      h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
 
 
 def self_influence(model, graph, train, *, checkpoints=None, lrs=None, h=1, sample_ratio=1.0, max_nodes_per_hop=None,
@@ -1513,15 +1391,12 @@ def self_influence(model, graph, train, *, checkpoints=None, lrs=None, h=1, samp
     ``train`` = (users, items, y), [N] fp32 on the model's device (``influence``'s definitions).  The usual detector
     of mislabelled training examples: large values first.  IGMC only."""
     _check_per_pair_model(model)
-    users, items, y = _host_pairs(graph.shape, *_split_pairs(train, "train", True), name="train")
-    _check_lrs(lrs, len(checkpoints) if checkpoints else 1)
-    if len(users) == 0:
+    tr = _host_pairs(graph.shape, *_split_pairs(train, "train", True), name="train")
+    lrs = _check_lrs(lrs, len(checkpoints) if checkpoints else 1)
+    if len(tr[0]) == 0:
         return torch.zeros(0, dtype=torch.float32, device=model.flat_params.device)
-    eng = InferenceEngine(model, graph, h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
-    try:
-        return eng.self_influence((users, items, y), lrs)
-    finally:
-        eng.close()
+    return _on_engine(model, graph, lambda eng: eng.self_influence(tr, lrs),
+                      h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
 
 
 def recommend(model, graph, users, k, *, items=None, exclude_rated=True, retrieve=None, h=1, sample_ratio=1.0,
@@ -1532,30 +1407,13 @@ def recommend(model, graph, users, k, *, items=None, exclude_rated=True, retriev
     (``corated_items``), or every item; minus the user's rated items when ``exclude_rated``.  Order: score
     descending, then item ascending; a NaN score ranks last; a user with fewer than ``k`` candidates gets item -1 /
     score -inf in the empty slots.  A pair's score does not depend on the candidates it was ranked among."""
-    k = _check_k(k)
-    _check_merge_fits(k, batch_size)
-    nu, ni = graph.shape
-    if retrieve is not None and items is not None:
-        raise ValueError("retrieve= chooses the candidates itself: pass it without items=")
-    if retrieve is not None:
-        _check_m(retrieve, ni)
-    users = _host_ids(users, "users", nu)
-    if _is_rows(items):
-        if torch.is_tensor(items) and items.device.type == "cuda":
-            if items.shape[0] != len(users):
-                raise ValueError("items has %d rows, one per query user is %d" % (items.shape[0], len(users)))
-        else:
-            items = _user_rows(items, len(users), ni, torch.device("cpu")).numpy()
-    elif items is not None:
-        items = _host_ids(items, "items", ni)
+    users = _host_ids(users, "users", graph.shape[0])
+    k = _ranking_inputs(k, batch_size, items, retrieve, len(users), graph.shape[1])[0]
     if len(users) == 0:
         dev = model.flat_params.device
         return (torch.zeros(0, k, dtype=torch.int64, device=dev), torch.zeros(0, k, dtype=torch.float32, device=dev))
-    eng = InferenceEngine(model, graph, h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
-    try:
-        return eng.recommend(users, k, items, exclude_rated, retrieve)
-    finally:
-        eng.close()
+    return _on_engine(model, graph, lambda eng: eng.recommend(users, k, items, exclude_rated, retrieve),
+                      h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
 
 
 def corated_items(graph, users, m, exclude_rated=True):
@@ -1569,11 +1427,12 @@ def corated_items(graph, users, m, exclude_rated=True):
     g = graph if isinstance(graph, RatingGraph) else RatingGraph(graph)
     if g.device is None:
         raise RuntimeError("igmc_b200 retrieval runs on a CUDA device (there is no CPU path)")
-    m = _check_m(m, g.num_items)
+    m = _check_count(m, "m", g.num_items, ValueError)
     users = _host_ids(users, "users", g.num_users)
-    lib = _lib.load()
     err = torch.zeros(1, dtype=torch.int32, device=g.device)
-    items, paths = _corated(lib, g, torch.from_numpy(users.astype(np.int32)).to(g.device), m, exclude_rated, err, {})
+    du = torch.from_numpy(users.astype(np.int32)).to(g.device)
+    items, paths = _corated(_lib.load(), g, "igmc_corated_items", (C.byref(g._c), du.data_ptr(), len(users)),
+                            len(users), m, exclude_rated, err, {})
     _lib.check_kernel_error(int(err.item()))
     return items, paths
 
@@ -1586,21 +1445,12 @@ def predict_sessions(model, sessions, session, items, *, h=1, sample_ratio=1.0, 
     from the graph, which is not changed.  Bit for bit ``predict_pairs`` of the same pair on the graph with that
     session's edits applied (same kernel plan and batch size); pair ids stay u * num_items + v.  Keywords as
     ``predict_pairs``'."""
-    if not isinstance(sessions, RatingSessions):
-        raise TypeError("sessions must be a RatingSessions")
-    sessions.check()
-    sess = _host_ids(session, "session", sessions.num_sessions)
-    items = _host_ids(items, "items", sessions.graph.num_items)
-    if len(sess) != len(items):
-        raise ValueError("session and items must have the same length (%d vs %d)" % (len(sess), len(items)))
+    sessions = _check_sessions(sessions)
+    sess, items, _ = _host_pairs((sessions.num_sessions, sessions.graph.num_items), session, items, first="session")
     if len(sess) == 0:
         return torch.zeros(0, dtype=torch.float32, device=model.flat_params.device)
-    eng = InferenceEngine(model, sessions.graph, h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints,
-                          sample_seed)
-    try:
-        return eng.predict_sessions(sessions, sess, items)
-    finally:
-        eng.close()
+    return _on_engine(model, sessions.graph, lambda eng: eng.predict_sessions(sessions, sess, items),
+                      h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
 
 
 def recommend_sessions(model, sessions, k, *, items=None, exclude_rated=True, retrieve=None, h=1, sample_ratio=1.0,
@@ -1609,30 +1459,11 @@ def recommend_sessions(model, sessions, k, *, items=None, exclude_rated=True, re
     session s.  Candidates and order as ``recommend``'s, with the session row as the user's ratings (``exclude_rated``,
     ``retrieve=M``); a 2-D ``items`` has one row per session.  Row s is bit for bit ``recommend`` for sessions.users[s]
     on the graph with session s's edits applied (same kernel plan and batch size); the graph is not changed."""
-    k = _check_k(k)
-    _check_merge_fits(k, batch_size)
-    if not isinstance(sessions, RatingSessions):
-        raise TypeError("sessions must be a RatingSessions")
-    sessions.check()
-    ni, S = sessions.graph.num_items, sessions.num_sessions
-    if retrieve is not None and items is not None:
-        raise ValueError("retrieve= chooses the candidates itself: pass it without items=")
-    if retrieve is not None:
-        _check_m(retrieve, ni)
-    if _is_rows(items):
-        if torch.is_tensor(items) and items.device.type == "cuda":
-            if items.shape[0] != S:
-                raise ValueError("items has %d rows, one per session is %d" % (items.shape[0], S))
-        else:
-            items = _user_rows(items, S, ni, torch.device("cpu")).numpy()
-    elif items is not None:
-        items = _host_ids(items, "items", ni)
-    eng = InferenceEngine(model, sessions.graph, h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints,
-                          sample_seed)
-    try:
-        return eng.recommend_sessions(sessions, k, items, exclude_rated, retrieve)
-    finally:
-        eng.close()
+    sessions = _check_sessions(sessions)
+    k = _ranking_inputs(k, batch_size, items, retrieve, sessions.num_sessions, sessions.graph.num_items)[0]
+    return _on_engine(model, sessions.graph,
+                      lambda eng: eng.recommend_sessions(sessions, k, items, exclude_rated, retrieve),
+                      h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
 
 
 def corated_items_sessions(sessions, m, exclude_rated=True):
@@ -1640,11 +1471,11 @@ def corated_items_sessions(sessions, m, exclude_rated=True):
     session row (and ``exclude_rated`` dropping its items) and the columns from the graph: (items [S, m], paths
     [S, m]) int32, row s bit for bit ``corated_items`` for sessions.users[s] on the graph with session s's edits
     applied.  One host synchronisation (the error word)."""
-    if not isinstance(sessions, RatingSessions):
-        raise TypeError("sessions must be a RatingSessions")
-    sessions.check()
-    m = _check_m(m, sessions.graph.num_items)
-    err = torch.zeros(1, dtype=torch.int32, device=sessions.graph.device)
-    items, paths = _corated_sessions(_lib.load(), sessions, m, exclude_rated, err, {})
+    sessions = _check_sessions(sessions)
+    g = sessions.graph
+    m = _check_count(m, "m", g.num_items, ValueError)
+    err = torch.zeros(1, dtype=torch.int32, device=g.device)
+    items, paths = _corated(_lib.load(), g, "igmc_corated_sessions", (C.byref(g._c), C.byref(sessions._c)),
+                            sessions.num_sessions, m, exclude_rated, err, {})
     _lib.check_kernel_error(int(err.item()))
     return items, paths

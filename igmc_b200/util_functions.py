@@ -236,15 +236,23 @@ class RatingGraph(object):
 _TORCH_OF = {np.int32: torch.int32, np.uint8: torch.uint8}
 
 
-def _update_inputs(users, items, values, cap_users, cap_items):
-    """(users, items, values, D) of an update: host arrays validated here (IndexError for an id outside the capacity,
-    ValueError for a value outside 0..256 or unequal lengths); device tensors are passed on unchecked (the kernel
-    checks them)"""
+def _cuda_ints(a, name):
+    """True for a CUDA tensor, which must hold integers (TypeError for a float, complex or bool dtype); False for host
+    data"""
+    if not (torch.is_tensor(a) and a.device.type == "cuda"):
+        return False
+    if a.is_floating_point() or a.is_complex() or a.dtype == torch.bool:
+        raise TypeError("%s must be integers, not %s" % (name, a.dtype))
+    return True
+
+
+def _update_inputs(users, items, values, hi_users, hi_items, names=("users", "items", "values")):
+    """(users, items, values, D) of edits in ``RatingGraph.update``'s encoding, the arrays called ``names``: host arrays
+    validated here (IndexError for an id outside [0, hi_users) / [0, hi_items), ValueError for a value outside 0..256 or
+    unequal lengths); device tensors are passed on unchecked (the kernel checks them)"""
     arrs = []
-    for name, a in (("users", users), ("items", items), ("values", values)):
-        if torch.is_tensor(a) and a.device.type == "cuda":
-            if a.is_floating_point() or a.is_complex() or a.dtype == torch.bool:
-                raise TypeError("%s must be integers, not %s" % (name, a.dtype))
+    for name, a in zip(names, (users, items, values)):
+        if _cuda_ints(a, name):
             arrs.append(a.reshape(-1))
             continue
         a = np.asarray(a.cpu().numpy() if torch.is_tensor(a) else a).reshape(-1)
@@ -253,15 +261,15 @@ def _update_inputs(users, items, values, cap_users, cap_items):
         arrs.append(a.astype(np.int64))
     n = [int(a.numel()) if torch.is_tensor(a) else len(a) for a in arrs]
     if len(set(n)) != 1:
-        raise ValueError("users, items and values must have the same length (%d, %d, %d)" % tuple(n))
-    for a, name, hi in ((arrs[0], "users", cap_users), (arrs[1], "items", cap_items)):
+        raise ValueError("%s, %s and %s must have the same length (%d, %d, %d)" % (names + tuple(n)))
+    for a, name, hi in zip(arrs, names, (hi_users, hi_items)):
         if not torch.is_tensor(a) and a.size and (a.min() < 0 or a.max() >= hi):
             bad = int(a.min()) if a.min() < 0 else int(a.max())
-            raise IndexError("%s: id %d outside the graph's capacity [0, %d)" % (name, bad, hi))
+            raise IndexError("%s: id %d out of range [0, %d)" % (name, bad, hi))
     x = arrs[2]
     if not torch.is_tensor(x) and x.size and (x.min() < 0 or x.max() > 256):
-        raise ValueError("values must be rating label + 1 (1..256) or 0 (delete), got %d"
-                         % (int(x.min()) if x.min() < 0 else int(x.max())))
+        raise ValueError("%s must be rating label + 1 (1..256) or 0 (delete), got %d"
+                         % (names[2], int(x.min()) if x.min() < 0 else int(x.max())))
     return arrs[0], arrs[1], arrs[2], n[0]
 
 

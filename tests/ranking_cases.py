@@ -22,7 +22,7 @@ import scipy.sparse as ssp
 MERGE_THREADS = 256          # csrc/recommend.cu: threads of one k_topk_merge CTA (and of one k_infl_topk CTA)
 SMEM_DEFAULT = 48 * 1024     # dynamic shared memory a launch gets without opting in
 SMEM_MAX = 227 * 1024        # what one CTA may opt in to on sm_90
-MERGE_HEAD = 16              # csrc/recommend.cu: k_topk_merge's segment-end word ahead of its lists
+MERGE_HEAD = 16              # csrc/topk_merge.cuh: the head ahead of the lists (k_topk_merge's segment-end word)
 RETRIEVE_CHUNK = 512         # csrc/retrieve.cu: threads of a k_corated CTA = items per chunk of its tie scan
 RETRIEVE_SMEM = 200 * 1024   # csrc/retrieve.cu: histograms up to this size live in shared memory
 ID_MAX = 2 ** 31 - 1
@@ -325,7 +325,7 @@ def influence_regimes(case):
             B = n + min(3, n) + 2
             if B > MERGE_THREADS:
                 got.add("long_segment")
-            if (k + B) * 12 > SMEM_DEFAULT:
+            if MERGE_HEAD + (k + B) * 12 > SMEM_DEFAULT:
                 got.add("smem_over_48k")
     return got
 

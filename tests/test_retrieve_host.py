@@ -110,7 +110,7 @@ def _fake_model():
     return m
 
 
-def test_validation_of_new_arguments():
+def test_validation_of_rows_and_retrieve():
     nu, ni = 5, 7
     A = _csr(nu, ni, 0.4, 3)
     m = _fake_model()
@@ -136,5 +136,5 @@ def test_validation_of_new_arguments():
     ti, ts = rc.recommend(m, A, np.zeros(0, np.int64), 4, retrieve=2)
     assert ti.shape == (0, 4)
     assert rc._is_rows(np.zeros((2, 3))) and not rc._is_rows([1, 2]) and not rc._is_rows(None)
-    rows = rc._user_rows([[0, -1, 6], [1, 1, 1]], 2, ni, torch.device("cpu"))
-    assert rows.dtype == torch.int32 and rows.tolist() == [[0, -1, 6], [1, 1, 1]]
+    rows = rc._user_rows([[0, -1, 6], [1, 1, 1]], 2, ni)
+    assert rows.dtype == np.int32 and rows.tolist() == [[0, -1, 6], [1, 1, 1]]

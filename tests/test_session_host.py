@@ -96,17 +96,18 @@ def test_row_twin_without_edits_is_the_graph_rows():
     assert rp[4] == rp[3]
 
 
-def test_input_validation():
+def test_edit_validation_through_update_inputs():
     S, ni = 3, 10
+    names = ("session", "items", "values")
     for bad in (([3], [0], [1]), ([-1], [0], [1]), ([0], [10], [1]), ([0], [-1], [1])):
         with pytest.raises(IndexError):
-            rc._session_inputs(S, ni, *bad)
+            rc._update_inputs(*bad, S, ni, names)
     for bad in (([0], [0], [257]), ([0], [0], [-1]), ([0, 1], [0], [1])):
         with pytest.raises(ValueError):
-            rc._session_inputs(S, ni, *bad)
+            rc._update_inputs(*bad, S, ni, names)
     with pytest.raises(TypeError):
-        rc._session_inputs(S, ni, [0.5], [0], [1])
-    s, i, v, D = rc._session_inputs(S, ni, [0, 2], [9, 0], [256, 0])
+        rc._update_inputs([0.5], [0], [1], S, ni, names)
+    s, i, v, D = rc._update_inputs([0, 2], [9, 0], [256, 0], S, ni, names)
     assert D == 2 and list(s) == [0, 2]
 
 
