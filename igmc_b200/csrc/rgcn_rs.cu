@@ -436,64 +436,74 @@ __device__ __forceinline__ void mma_3xtf32_a(float (&d)[4], float (&dsm)[4], con
   mma_tf32(d, ah, bh);
 }
 
-// ---- NP adjacent 16x8 tiles (columns n0 + 8 i) of one 16-row block per warp: the A fragments are loaded and split
-// ONCE for all of them (the tile loops are issue bound: 4 LDS + 8 ALU for A and 2 LDS + 4 ALU + 3 HMMA per tile and
-// k-step; one tile per warp repeated the A part in the four warps of a row block).  Per output element the sums and
-// their order are those of one tile per warp: (d, e) take the even k-steps of the first span, (d2, e2) the odd ones
-// and the second (root) span; e/e2 hold the 3xTF32 cross terms.
+// ---- fragments by ldmatrix: a 16 x 8 fp32 block read as four 8 x 8 b16 matrices (8 rows of 16 bytes each, each row
+// address 16-byte aligned; lanes 8j .. 8j + 7 address the rows of matrix j).  Lane (g, t) = (L >> 2, L & 3) gets word
+// t of row g of matrix j in register j, so
+//   A (rows m of a K-contiguous block): lane L addresses row L & 15, floats 4 (L >> 4) .. +3 -> {a0, a1, a2, a3} of
+//     mma m16n8k8;
+//   B (rows n0 .. n0 + 15 of an n-major, K-contiguous slab): lane L addresses row (L & 7) + 8 (L >> 4), floats
+//     4 ((L >> 3) & 1) .. +3 -> {b0, b1} of the tile n0, then {b0, b1} of the tile n0 + 8 (each pair in adjacent
+//     registers, as the mma takes it).
+// One LDSM replaces four 32-bit LDS.
+__device__ __forceinline__ void ldsm_x4(float (&f)[4], uint32_t addr) {
+  uint32_t r[4];
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr));
+#pragma unroll
+  for (int i = 0; i < 4; ++i) f[i] = __uint_as_float(r[i]);
+}
+
+// ---- two adjacent 16x8 tiles (columns n0, n0 + 8) of one 16-row block per warp: the A fragments are loaded and split
+// ONCE for both (the tile loops are issue bound; one tile per warp repeated the A part in the four warps of a row
+// block), and one ldmatrix.x4 of the B slab gives both tiles' B fragments of a k-step.  Per output element the sums
+// and their order are those of one tile per warp: (d, e) take the even k-steps of the first span, (d2, e2) the odd
+// ones and the second (root) span; e/e2 hold the 3xTF32 cross terms.
 struct TileAcc { float d[4], d2[4], e[4], e2[4]; };
 __device__ __forceinline__ void tile_zero(TileAcc& t) {
 #pragma unroll
   for (int i = 0; i < 4; ++i) { t.d[i] = 0.f; t.d2[i] = 0.f; t.e[i] = 0.f; t.e2[i] = 0.f; }
 }
-// a0p / a1p: rows gq / gq + 8 of the block (+ tq), K-contiguous;  bp: row n0 + gq of the n-major slab (+ tq)
-template <int NP>
-__device__ __forceinline__ void tiles_span(TileAcc (&T)[NP], const float* __restrict__ a0p,
-                                           const float* __restrict__ a1p, const float* __restrict__ bp, int KS, int K) {
+// a: this lane's ldmatrix address in the A block (K-contiguous rows, k = 0);  b: the same in rows n0 .. n0 + 15 of
+// the n-major slab.  K is a multiple of 8.
+__device__ __forceinline__ void tiles_span(TileAcc (&T)[2], uint32_t a, uint32_t b, int K) {
   int k0 = 0;
   for (; k0 + 16 <= K; k0 += 16) {                  // two independent accumulator sets per iteration
-    const float af[4] = {a0p[k0], a1p[k0], a0p[k0 + 4], a1p[k0 + 4]};
-    const float ag[4] = {a0p[k0 + 8], a1p[k0 + 8], a0p[k0 + 12], a1p[k0 + 12]};
+    float af[4], ag[4], bf[4], bg[4];
+    ldsm_x4(af, a + 4 * k0);
+    ldsm_x4(ag, a + 4 * k0 + 32);
+    ldsm_x4(bf, b + 4 * k0);
+    ldsm_x4(bg, b + 4 * k0 + 32);
     uint32_t ah[4], al[4], gh[4], gl[4];
     split_tf32(af, ah, al);
     split_tf32(ag, gh, gl);
 #pragma unroll
-    for (int i = 0; i < NP; ++i) {
-      const float* b = bp + (size_t)i * 8 * KS + k0;
-      const float bf[2] = {b[0], b[4]}, bg[2] = {b[8], b[12]};
-      mma_3xtf32_a(T[i].d, T[i].e, ah, al, bf);
-      mma_3xtf32_a(T[i].d2, T[i].e2, gh, gl, bg);
+    for (int i = 0; i < 2; ++i) {
+      mma_3xtf32_a(T[i].d, T[i].e, ah, al, {bf[2 * i], bf[2 * i + 1]});
+      mma_3xtf32_a(T[i].d2, T[i].e2, gh, gl, {bg[2 * i], bg[2 * i + 1]});
     }
   }
-  for (; k0 < K; k0 += 8) {
-    const float af[4] = {a0p[k0], a1p[k0], a0p[k0 + 4], a1p[k0 + 4]};
+  if (k0 < K) {                                     // 8-K tail (K = 8 mod 16: the 4-wide input layer at R = 5)
+    float af[4], bf[4];
+    ldsm_x4(af, a + 4 * k0);
+    ldsm_x4(bf, b + 4 * k0);
     uint32_t ah[4], al[4];
     split_tf32(af, ah, al);
 #pragma unroll
-    for (int i = 0; i < NP; ++i) {
-      const float* b = bp + (size_t)i * 8 * KS + k0;
-      const float bf[2] = {b[0], b[4]};
-      mma_3xtf32_a(T[i].d, T[i].e, ah, al, bf);
-    }
+    for (int i = 0; i < 2; ++i) mma_3xtf32_a(T[i].d, T[i].e, ah, al, {bf[2 * i], bf[2 * i + 1]});
   }
 }
-// the second span (root / d pre rows), into (d2, e2).  pa / pb: the two 16-row-block rows' element pointers for
-// columns tq and tq + 4 (already swizzled), xa / xb: XOR applied to the k offset (hix swizzle bits 3-4; 0 = linear)
-template <int NP>
-__device__ __forceinline__ void tiles_span2(TileAcc (&T)[NP], const float* __restrict__ p0a, const float* __restrict__ p0b,
-                                            const float* __restrict__ p1a, const float* __restrict__ p1b, int x0, int x1,
-                                            const float* __restrict__ bp, int KS, int K) {
+// the second span (root / d pre rows), into (d2, e2).  a: this lane's ldmatrix address at k = 0 (already swizzled),
+// xs: XOR applied to the k offset (hix swizzle bits 3-4; 0 = linear);  b as in tiles_span
+__device__ __forceinline__ void tiles_span2(TileAcc (&T)[2], uint32_t a, int xs, uint32_t b, int K) {
   for (int k0 = 0; k0 < K; k0 += 8) {
-    const int o0 = k0 ^ x0, o1 = k0 ^ x1;
-    const float af[4] = {p0a[o0], p1a[o1], p0b[o0], p1b[o1]};
+    float af[4], bf[4];
+    ldsm_x4(af, a + 4 * (k0 ^ xs));
+    ldsm_x4(bf, b + 4 * k0);
     uint32_t ah[4], al[4];
     split_tf32(af, ah, al);
 #pragma unroll
-    for (int i = 0; i < NP; ++i) {
-      const float* b = bp + (size_t)i * 8 * KS + k0;
-      const float bf[2] = {b[0], b[4]};
-      mma_3xtf32_a(T[i].d2, T[i].e2, ah, al, bf);
-    }
+    for (int i = 0; i < 2; ++i) mma_3xtf32_a(T[i].d2, T[i].e2, ah, al, {bf[2 * i], bf[2 * i + 1]});
   }
 }
 
@@ -737,18 +747,16 @@ __device__ __forceinline__ bool forward_body(const igmc_model_t& M, const float*
       const int mt = (crow + 15) >> 4;
       for (int item = warp; item < mt * 2; item += nwarps) {   // warp = (16-row block, 16-column half)
         const int m0 = (item >> 1) << 4, nh = (item & 1) << 4;
+        // this lane's ldmatrix row and float offset in the A block and in the B slab (ldsm_x4)
+        const int ar = lane & 15, ac = (lane >> 4) << 2, br = (lane & 7) | ((lane >> 1) & 8), bc = (lane >> 1) & 4;
         TileAcc T[2];
         tile_zero(T[0]); tile_zero(T[1]);
-        const float* a0p = stage + (size_t)(m0 + gq) * SS + tq;
-        const float* bp = Wn + (size_t)(nh + gq) * KS + tq;
-        tiles_span<2>(T, a0p, a0p + 8 * SS, bp, KS, K1p);
+        const uint32_t bs = smem_u32(Wn + (nh + br) * KS + bc);
+        tiles_span(T, smem_u32(stage + (m0 + ar) * SS + ac), bs, K1p);
         const int r0 = c0 + m0 + gq, r1 = r0 + 8;           // rows relative to the own range
-        const int v0 = own.lo + min(r0, n_own - 1), v1 = own.lo + min(r1, n_own - 1);
-        const int sw0 = (v0 & 7) << 2, sw1 = (v1 & 7) << 2;   // hix(): column ^ swizzle, split into its bit 2 and bits 3-4
-        const float* h0 = H + (v0 << 5);
-        const float* h1 = H + (v1 << 5);
-        tiles_span2<2>(T, h0 + (tq | (sw0 & 4)), h0 + (tq | ((sw0 & 4) ^ 4)), h1 + (tq | (sw1 & 4)),
-                       h1 + (tq | ((sw1 & 4) ^ 4)), sw0 & 24, sw1 & 24, bp + K1p, KS, inpp);
+        const int vf = own.lo + min(c0 + m0 + ar, n_own - 1);  // this lane's ldmatrix row of H
+        const int sw = (vf & 7) << 2;                       // hix(): column ^ swizzle, split into its bit 2 and bits 3-4
+        tiles_span2(T, smem_u32(H + (vf << 5) + (ac ^ (sw & 4))), sw & 24, bs + 4 * K1p, inpp);
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
           float d[4];
@@ -1088,15 +1096,13 @@ __device__ __forceinline__ void backward_body(const igmc_model_t& M, const float
         const int mt = (crow + 15) >> 4;
         for (int item = warp; item < mt * 2; item += nwarps) {   // warp = (16-row block, 16-column half)
           const int m0 = (item >> 1) << 4, nh = (item & 1) << 4;
+          const int ar = lane & 15, ac = (lane >> 4) << 2, br = (lane & 7) | ((lane >> 1) & 8), bc = (lane >> 1) & 4;
           TileAcc T[2];
           tile_zero(T[0]); tile_zero(T[1]);
-          const float* a0p = stage + (size_t)(m0 + gq) * SS + tq;
-          const float* bp = Wn + (size_t)(nh + gq) * KS + tq;
-          tiles_span<2>(T, a0p, a0p + 8 * SS, bp, KS, K1p);
+          const uint32_t bs = smem_u32(Wn + (nh + br) * KS + bc);
+          tiles_span(T, smem_u32(stage + (m0 + ar) * SS + ac), bs, K1p);
           const int r0 = c0 + m0 + gq, r1 = r0 + 8;
-          const float* p0 = DP + (size_t)min(r0, own_cap16 - 1) * DPS_ + tq;
-          const float* p1 = DP + (size_t)min(r1, own_cap16 - 1) * DPS_ + tq;
-          tiles_span2<2>(T, p0, p0 + 4, p1, p1 + 4, 0, 0, bp + K1p, KS, HID);
+          tiles_span2(T, smem_u32(DP + min(c0 + m0 + ar, own_cap16 - 1) * DPS_ + ac), 0, bs + 4 * K1p, HID);
 #pragma unroll
           for (int i = 0; i < 2; ++i) {
             float d[4];
