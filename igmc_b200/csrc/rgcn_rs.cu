@@ -8,8 +8,9 @@
 //                                                          edge lists staged in shared memory, software-pipelined
 //   h'[v]      = tanh( 1/deg(v) * sum_r AGG[v,r,:] W_r + h[v] root + bias )    lane = (node, 4 output channels)
 // PR = true (PyG >= 1.6 RGCNConv, igmc_saved_t.rel_inv_deg): 1/|N_r(v)| per relation block in place of 1/deg(v).
-// Node features of the WHOLE subgraph stay in shared memory; CTAs of a cluster exchange their rows through
-// L2 (ld/st.cg) + barrier.cluster once per layer.  Backward = same two passes on the out-lists with W_r^T,
+// Node features of the WHOLE subgraph stay in shared memory; CTAs of a cluster store their rows of every layer into
+// each other's shared memory with st.async, counted on the receiver's mbarrier.  Backward = same two passes on the
+// out-lists with W_r^T,
 // a K=n weight-gradient tile GEMM, and the (att,basis) chain rule applied to the per-CTA dW_r.
 // No float atomics; every reduction has a fixed order (bitwise run-to-run deterministic).
 #include <cooperative_groups.h>
@@ -300,10 +301,21 @@ __device__ __forceinline__ void rel_inv_deg_own(const Lists& Ls, const EdgeKeep&
 // there seven of the eight lanes of a group had nothing to do, now a warp works on 32 segments at a time.
 // PR (backward of the mean per relation): every entry (nbr, type r) is weighed by rinv[nbr*R + r] = 1/|N_r(nbr)|,
 // read through L2 (the table is written by the forward, possibly by a peer CTA of the same launch).
-template <int GL, bool PR = false>
+// RS (forward, staged lists): the run store of a node row whose list is one segment is scaled by the node's degree
+// factor, so that the fold pass only visits rows with extra segments.  The product is the one the fold computed
+// (run sum times the factor, both rounded once); zeroed blocks stay +0.  RS = 1: 1/deg of the segment's row
+// (RunScale::inv[row]), RS = 2 (mean per relation): 1/|N_r(v)| of the run's type r (RunScale::inv[row*R + r], L2).
+// Every other row (extra rows, rows of nodes with extras, RunScale::inv == nullptr) is stored as summed.
+struct RunScale {
+  const float* inv;   // degree factors of the chunk's rows (nullptr: no scaling)
+  const int* ex;      // Lists::ex of the chunk's rows
+  int crow;           // node rows of the chunk (staging rows >= crow are extra rows)
+};
+template <int GL, bool PR = false, int RS = 0>
 __device__ __forceinline__ void gather_segments(const Lists& Ls, const EdgeKeep& K, int sg0, int sg1, int lane,
                                                 const float* __restrict__ feat, float* __restrict__ stage, int SS,
-                                                int inp, int R, int* ticket, const float* rinv = nullptr) {
+                                                int inp, int R, int* ticket, const float* rinv = nullptr,
+                                                RunScale rsc = RunScale{nullptr, nullptr, 0}) {
   const int q = lane & (GL - 1);
   const int fo = 4 * q;
   const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -316,9 +328,18 @@ __device__ __forceinline__ void gather_segments(const Lists& Ls, const EdgeKeep&
     const int sg = valid ? Ls.seg_ord[t] : 0;
     float* rowb = stage;
     int p = 0, p1 = 0;
+    float sc = 1.f;                  // RS = 1: factor of every run of the segment
+    const float* scp = nullptr;      // RS = 2: factors of the row's relation blocks
     if (valid) {
       const int sr = Ls.seg_row[sg];
       rowb = stage + (size_t)(sr & SEG_ROW) * SS;
+      if (RS && rsc.inv) {
+        const int row = sr & SEG_ROW;
+        if (row < rsc.crow && (rsc.ex[row] >> 16) == 0) {
+          if (RS == 1) sc = rsc.inv[row];
+          else scp = rsc.inv + (size_t)row * R;
+        }
+      }
       if (Ls.lst) {
         // every type present gets one plain store of its run below: zero only the blocks of the other types (a
         // lane owns column fo of every block) and the padding behind the last block
@@ -346,6 +367,11 @@ __device__ __forceinline__ void gather_segments(const Lists& Ls, const EdgeKeep&
         acc.x = __fadd_rn(acc.x, (a_).x); acc.y = __fadd_rn(acc.y, (a_).y);                           \
         acc.z = __fadd_rn(acc.z, (a_).z); acc.w = __fadd_rn(acc.w, (a_).w);                           \
         if ((e_) & RUN_END) {                                                                         \
+          if (RS) {                                                                                   \
+            const float s_ = (RS == 2 && scp) ? __ldcg(scp + (int)((e_) >> 24)) : sc;                 \
+            acc = make_float4(__fmul_rn(acc.x, s_), __fmul_rn(acc.y, s_), __fmul_rn(acc.z, s_),       \
+                              __fmul_rn(acc.w, s_));                                                  \
+          }                                                                                           \
           *reinterpret_cast<float4*>(row + (int)((e_) >> 24) * inp) = acc;                            \
           acc = z4;                                                                                   \
         }                                                                                             \
@@ -569,8 +595,41 @@ __device__ __forceinline__ void copy_f4(float* __restrict__ dst, const float* __
 }
 
 // split cluster barrier: work that does not touch peer-written shared memory goes between arrive and wait
-__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
+__device__ __forceinline__ void cluster_arrive_relaxed() { asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory"); }
 __device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
+
+// ---- layer rows to the peer CTAs: every CTA stores its rows straight into the peers' buffers with st.async, which
+// credits the bytes to an mbarrier of the receiving CTA (complete_tx, release at cluster scope).  The receiver arms
+// its barrier with the bytes it expects, (n - n_own) rows x 128 B, and waits for them with acquire at cluster scope:
+// no CTA-wide cluster barrier per layer, and a CTA waits only for the rows it reads.  The byte credit may reach the
+// barrier before it is armed (the phase cannot complete before the receiver's own arrival).
+__device__ __forceinline__ uint32_t mapa_u32(uint32_t a, int rank) {   // shared::cta address -> rank's shared::cluster
+  uint32_t d;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(rank));
+  return d;
+}
+// rank of the (pr + 1)-th other CTA of the cluster (pr + 1 < CL), without a division
+__device__ __forceinline__ int peer_rank(int rank, int pr, int CL) {
+  const int r = rank + pr + 1;
+  return r >= CL ? r - CL : r;
+}
+// v -> the float2 at `dst` and 8 bytes credited to the barrier `bar`, both mapped into CTA `rank` of the cluster
+// (the mapping is derived per store: addresses kept across the layer cost registers in the gather)
+__device__ __forceinline__ void st_async_peer(const float* dst, float2 v, const uint64_t* bar, int rank) {
+  asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.v2.f32 [%0], {%1, %2}, [%3];"
+               ::"r"(mapa_u32(smem_u32(dst), rank)), "f"(v.x), "f"(v.y), "r"(mapa_u32(smem_u32(bar), rank)));
+}
+__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
+  uint32_t ok;
+  do {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}"
+        : "=r"(ok)
+        : "r"(smem_u32(bar)), "r"(parity)
+        : "memory");
+  } while (!ok);
+}
 
 // ------------------------------------------------------------------------------------------------
 // forward
@@ -606,7 +665,8 @@ __device__ __forceinline__ bool forward_body(const igmc_model_t& M, const float*
   uint32_t* lbuf = reinterpret_cast<uint32_t*>(ibuf + a4(list_ints(own_cap)));   // [lcap]
   __shared__ int s_t[2];
   __shared__ int ws[34];
-  __shared__ __align__(8) uint64_t mbar[2];   // [0] list image, [1] weight slab of the current layer (TMA completion)
+  // [0] list image, [1] weight slab of the current layer (TMA completion), [2 + (l & 1)] the peers' rows of layer l
+  __shared__ __align__(8) uint64_t mbar[4];
 
   const int nb = node_ptr[g], n = node_ptr[g + 1] - nb;
   const int eb = edge_ptr[g], m_half = (edge_ptr[g + 1] - eb) >> 1;
@@ -637,11 +697,13 @@ __device__ __forceinline__ bool forward_body(const igmc_model_t& M, const float*
   };
   if (tid == 0) {
     s_t[0] = 0x7fffffff; s_t[1] = 0x7fffffff;
-    mbar_init(&mbar[0], 1);
-    mbar_init(&mbar[1], 1);
+    for (int i = 0; i < 4; ++i) mbar_init(&mbar[i], 1);
     mbar_fence_init();
   }
   __syncthreads();
+  // the peers store into this CTA's buffers and barriers from layer 0's tiles on: its barriers are initialised before
+  // any of them passes the wait in front of the layer loop
+  if (CL > 1) cluster_arrive_relaxed();
   const bool use_img = IMG.tab != nullptr;
   if (use_img && tid == 0) {   // pre-staged lists: header + tables, then the entries, straight into shared memory
     const int32_t* gt = IMG.tab + (size_t)blockIdx.x * IMG.tab_ints;
@@ -681,9 +743,10 @@ __device__ __forceinline__ bool forward_body(const igmc_model_t& M, const float*
   if (tid == 0) ws[33] = 0;   // segment ticket of gather_segments (made visible by the barrier at the top of the layer loop)
   const bool ext = M.readout != 0;   // concat_states only: an external readout (csrc/sortpool.cu) takes over
   const int tu = s_t[0], ti = s_t[1];
-  if (!ext && (tu >= n || ti >= n)) {
+  if (!ext && (tu >= n || ti >= n)) {   // (uniform over the cluster)
     if (tid == 0) igmc_set_err(err, IGMC_ERR_BAD_BATCH);
     mbar_wait(&mbar[1], 0);   // do not exit under an in-flight bulk copy
+    if (CL > 1) cluster_wait();
     return false;
   }
   if (S.prof && tid == 0) {   // debug: staging facts
@@ -692,22 +755,38 @@ __device__ __forceinline__ bool forward_body(const igmc_model_t& M, const float*
     pp[59] = chunk; pp[58] = n_own;
   }
   const int gq = lane >> 2, tq = lane & 3;
+  // the peers' barriers are initialised (arrive after this CTA's initialisation above)
+  if (CL > 1) cluster_wait();
   IGMC_STAMP(1);
+  // Layer l's rows travel to the peers by st.async on their barrier mbar[2 + (l & 1)] (phase (l >> 1) & 1); every CTA
+  // waits on its own barrier for the (n - n_own) rows of the peers at the end of the layer.  Write-after-read: a peer
+  // stores only rows it owns, into the buffer this CTA gathers layer l - 1 from; it reaches layer l's tiles only after
+  // it has received all of this CTA's layer l - 1 rows, which are pushed by the tiles of the last chunk, after every
+  // gather of layer l - 1 (release of the byte credit, acquire of the peer's wait).  The same argument orders a
+  // barrier's uses: layer l + 2's bytes can reach it only after this CTA's layer l + 1 gather, behind its layer l wait.
+  // Nothing is stored into this CTA after its last layer's wait has seen every byte: it may exit (or re-carve its
+  // shared memory for the backward) from there.
   for (int l = 0; l < L; ++l) {
     const int inp = l == 0 ? in0p : HID;
     const int K1 = R * inp, K1p = a8(K1), inpp = a8(inp), SS = K1p + 4, KS = K1p + inpp + 4;
+    uint64_t* xbar = &mbar[2 + (l & 1)];
+    if (CL > 1 && tid == 0) mbar_expect_tx(xbar, (uint32_t)(n - n_own) * 128u);
     __syncthreads();
     IGMC_STAMP(2 + 6 * l);
-    float* peerH[3];   // this layer's output buffer in the other CTAs of the cluster (mapped once, not per tile)
-#pragma unroll
-    for (int pr = 0; pr < 3; ++pr) peerH[pr] = pr + 1 < CL ? cluster.map_shared_rank(Hn, (rank + pr + 1) % CL) : Hn;
+    // staged lists: the gather stores the rows of one-segment nodes already scaled by their degree factor, the fold
+    // below only adds the extra rows of long lists.  Unstaged lists (gathered by read-modify-write) and layer 0 with a
+    // saved aggregate over several chunks (written by the fold) keep the fold over every row.
+    const bool run_scale = Ls.lst != nullptr && !(S.zsave && l == 0 && n_own > chunk);
     for (int c0 = 0; c0 < n_own; c0 += chunk) {
       const int crow = min(chunk, n_own - c0);
       // ---- aggregate: one 8-lane group per list segment ----
 #define IGMC_STAMP_T(t_, i_) do { if (S.prof && l == 1 && threadIdx.x == (t_)) S.prof[(size_t)blockIdx.x * 64 + (i_)] = clock64(); } while (0)
       IGMC_STAMP_T(0, 39); IGMC_STAMP_T(992, 49);
-      if (inp == 4) gather_segments<1>(Ls, K, Ls.segbase[c0], Ls.segbase[c0 + crow], lane, H, stage, SS, inp, R, &ws[33]);
-      else gather_segments<8>(Ls, K, Ls.segbase[c0], Ls.segbase[c0 + crow], lane, H, stage, SS, inp, R, &ws[33]);
+      const RunScale rsc{run_scale ? (PR ? rinv + (size_t)(own.lo + c0) * R : invdeg + own.lo + c0) : nullptr,
+                         Ls.ex + c0, crow};
+      const int sg0 = Ls.segbase[c0], sg1 = Ls.segbase[c0 + crow];
+      if (inp == 4) gather_segments<1, false, PR ? 2 : 1>(Ls, K, sg0, sg1, lane, H, stage, SS, inp, R, &ws[33], nullptr, rsc);
+      else gather_segments<8, false, PR ? 2 : 1>(Ls, K, sg0, sg1, lane, H, stage, SS, inp, R, &ws[33], nullptr, rsc);
       IGMC_STAMP_T(0, 40); IGMC_STAMP_T(992, 43); IGMC_STAMP_T(480, 46);
       if (l == 0) IGMC_STAMP(32);
       __syncthreads();
@@ -716,7 +795,7 @@ __device__ __forceinline__ bool forward_body(const igmc_model_t& M, const float*
       IGMC_STAMP_T(0, 41); IGMC_STAMP_T(992, 44);
       // ---- fold the extra segments of long lists into their node row, scale by 1/deg (PR: the relation block by
       //      1/|N_r(v)|), keep a copy for backward ----
-      {
+      if (!run_scale) {
         const int kq = K1 >> 2, SS4 = SS >> 2;
         float4* st4 = reinterpret_cast<float4*>(stage);
         // flat over (row, float4): independent iterations; (r, k4) advance by NT = dr * kq + dk without a division
@@ -734,13 +813,31 @@ __device__ __forceinline__ bool forward_body(const igmc_model_t& M, const float*
           }
           t.x *= id2; t.y *= id2; t.z *= id2; t.w *= id2;
           st4[(size_t)r * SS4 + k4] = t;
-          if (S.zsave && l == 0 && n_own > chunk)   // (one chunk: copied out below, in the cluster-barrier window)
+          if (S.zsave && l == 0 && n_own > chunk)   // (one chunk: copied out below, at the end of the layer)
             reinterpret_cast<float4*>(S.zsave + (size_t)(nb + v) * (size_t)K1)[k4] = t;
+        }
+      } else if (sg1 - sg0 > crow) {   // the chunk has extra segments (uniform: from the segment table)
+        const int kq = K1 >> 2, SS4 = SS >> 2;
+        float4* st4 = reinterpret_cast<float4*>(stage);
+        for (int r = warp; r < crow; r += nwarps) {
+          const int e = Ls.ex[c0 + r], x0 = e & 0xffff, nex = e >> 16;
+          if (nex == 0) continue;
+          const int v = own.lo + c0 + r;
+          for (int k4 = lane; k4 < kq; k4 += 32) {
+            const float id2 = PR ? __ldcg(rinv + (size_t)v * R + k4 / (inp >> 2)) : invdeg[v];
+            float4 t = st4[(size_t)r * SS4 + k4];
+            for (int j = 0; j < nex; ++j) {
+              const float4 u = st4[(size_t)(crow + x0 + j) * SS4 + k4];
+              t.x += u.x; t.y += u.y; t.z += u.z; t.w += u.w;
+            }
+            t.x *= id2; t.y *= id2; t.z *= id2; t.w *= id2;
+            st4[(size_t)r * SS4 + k4] = t;
+          }
         }
       }
       IGMC_STAMP_T(0, 42); IGMC_STAMP_T(992, 45);
       IGMC_STAMP(3 + 6 * l);
-      __syncthreads();
+      if (!run_scale || sg1 - sg0 > crow) __syncthreads();
       IGMC_STAMP(4 + 6 * l);
       // ---- dense transform on tensor cores: out[16x8 tiles] = [AGG' | h] . [W_r ; root] ----
       if (c0 == 0) mbar_wait(&mbar[1], (uint32_t)(l & 1));   // this layer's weight slab has landed
@@ -773,8 +870,8 @@ __device__ __forceinline__ bool forward_body(const igmc_model_t& M, const float*
               const int off = hix(v, cc);
               *reinterpret_cast<float2*>(Hn + off) = o;
 #pragma unroll
-              for (int pr = 0; pr < 3; ++pr)   // push the row slice to the other CTAs of the cluster (DSMEM)
-                if (pr + 1 < CL) *reinterpret_cast<float2*>(peerH[pr] + off) = o;
+              for (int pr = 0; pr < 3; ++pr)   // push the row slice to the other CTAs of the cluster
+                if (pr + 1 < CL) st_async_peer(Hn + off, o, xbar, peer_rank(rank, pr, CL));
             }
           }
         }
@@ -784,8 +881,8 @@ __device__ __forceinline__ bool forward_body(const igmc_model_t& M, const float*
     }
     IGMC_STAMP(6 + 6 * l);
     if (n_own == 0) mbar_wait(&mbar[1], (uint32_t)(l & 1));   // keep the barrier phases in step (no tiles ran)
-    // the next layer's weights do not depend on the peers: load them while the row pushes of the cluster land
-    if (CL > 1) cluster_arrive();
+    // the next layer's weights do not depend on the peers (every read of Wn is behind the barrier above): load them
+    // while the peers' rows land
     if (l + 1 < L) load_weights(l + 1);
     if (S.zsave && l == 0 && n_own <= chunk) {
       // layer 0's scaled aggregate for the backward (layers >= 1: the backward takes its weight gradients from its own
@@ -800,16 +897,16 @@ __device__ __forceinline__ bool forward_body(const igmc_model_t& M, const float*
       }
       IGMC_STAMP(34);
     }
-    if (CL > 1) cluster_wait();
-    IGMC_STAMP(7 + 6 * l);
     float* t = H; H = Hn; Hn = t;
-    // concat_states of the own rows -> global, issued after the barrier (whose release fence would otherwise wait
-    // for these stores) and overlapping the next layer's gather; one coalesced 128 B row per 8 threads
+    // concat_states of the own rows -> global (local rows: no need to wait for the peers), overlapping the next
+    // layer's gather; one coalesced 128 B row per 8 threads
     for (int idx = tid; idx < n_own * 8; idx += NT) {
       const int v = own.lo + (idx >> 3), c4 = (idx & 7) << 2;
       __stcg(reinterpret_cast<float4*>(S.states + (size_t)(nb + v) * CW + l * HID + c4),
              *reinterpret_cast<const float4*>(H + hix(v, c4)));
     }
+    if (CL > 1) mbar_wait_cluster(xbar, (uint32_t)((l >> 1) & 1));   // the peers' rows of layer l have landed
+    IGMC_STAMP(7 + 6 * l);
     // concat_states rows of the two target nodes (models.py:203-207), all rows are local now
     if (rank == 0 && !ext && tid < 2 * HID) {
       const int node = tid < HID ? tu : ti, c = tid & 31;
@@ -911,7 +1008,8 @@ __device__ __forceinline__ void backward_body(const igmc_model_t& M, const float
   int* ibuf = reinterpret_cast<int*>(dhid_s + L1O) + IMG_HDR;   // [header |] list offsets + segment table
   uint32_t* lbuf = reinterpret_cast<uint32_t*>(ibuf + a4(list_ints(own_cap)));   // [lcap]
   __shared__ int ws[34];
-  __shared__ __align__(8) uint64_t mbar[3];   // TMA completion: [0] list image, [1] weight slab, [2] h_{l-1} rows
+  // TMA completion: [0] list image, [1] weight slab, [2] h_{l-1} rows;  [3 + (l & 1)] the peers' rows of d h_{l-1}
+  __shared__ __align__(8) uint64_t mbar[5];
 
   const int nb = node_ptr[g], n = node_ptr[g + 1] - nb;
   const int eb = edge_ptr[g], m_half = (edge_ptr[g + 1] - eb) >> 1;
@@ -927,12 +1025,11 @@ __device__ __forceinline__ void backward_body(const igmc_model_t& M, const float
   float* gp = gpart + ((size_t)g * CL + rank) * (size_t)igmc_raw_count(R, in0, L);
   pdl_trigger();   // the gradient-assembly kernel behind this one may be scheduled as SMs free up
   if (tid == 0) {
-    mbar_init(&mbar[0], 1);
-    mbar_init(&mbar[1], 1);
-    mbar_init(&mbar[2], 1);
+    for (int i = 0; i < 5; ++i) mbar_init(&mbar[i], 1);
     mbar_fence_init();
   }
   __syncthreads();
+  if (CL > 1) cluster_arrive_relaxed();   // (waited for in front of the layer loop, before the first push)
   uint32_t wuse = 0, huse = 0;   // completed-phase counters of mbar[1] / mbar[2] (uniform over the block)
   // per-layer operand that does not depend on the peers: the [W_r^T ; root^T] slab of the data gradient (one bulk
   // copy by one thread; waited for right before the tiles).  Callers guarantee that nobody still reads Wn.
@@ -1012,7 +1109,13 @@ __device__ __forceinline__ void backward_body(const igmc_model_t& M, const float
   __syncthreads();
 
   const int gq = lane >> 2, tq = lane & 3;
+  if (CL > 1) cluster_wait();   // the peers' barriers are initialised
   IGMC_STAMP(1);
+  // d h_{l-1} travels as the forward's layer rows do (st.async on the receiver's barrier mbar[3 + (l & 1)], phase
+  // ((L - 1 - l) >> 1) & 1, waited for at the end of layer l; layer 0 exchanges nothing).  Write-after-read: a peer
+  // stores its own rows of d h_{l-1} into the buffer this CTA gathered layer l + 1 from, and only after it has received
+  // all of this CTA's d h_l rows, pushed by the tiles of this CTA's last layer l + 1 chunk, behind every read of that
+  // buffer (step (0) and the gathers).  After its layer 1 wait nothing is stored into this CTA any more.
   for (int l = L - 1; l >= 0; --l) {
     const int in = l == 0 ? in0 : HID, inp = l == 0 ? in0p : HID;
     const int K1 = R * inp, K1p = a8(K1), inpp = a8(inp), KRp = K1p + inpp;
@@ -1020,9 +1123,8 @@ __device__ __forceinline__ void backward_body(const igmc_model_t& M, const float
     float* DPS = (l & 1) ? DH1 : DH0;                    // d h_l on entry, dpre/deg after step (0)
     float* DHn = (l & 1) ? DH0 : DH1;                    // d h_{l-1} (written here and by the peers)
     float* gpl = gp + igmc_raw_off(R, in0, l);           // this layer's block of the raw partial row
-    float* peerD[3];   // d h_{l-1} in the other CTAs of the cluster (mapped once per layer, not per tile)
-#pragma unroll
-    for (int pr = 0; pr < 3; ++pr) peerD[pr] = pr + 1 < CL ? cluster.map_shared_rank(DHn, (rank + pr + 1) % CL) : DHn;
+    uint64_t* xbar = &mbar[3 + (l & 1)];
+    if (CL > 1 && l > 0 && tid == 0) mbar_expect_tx(xbar, (uint32_t)(n - n_own) * 128u);
     // (0) d pre = d h (1 - h^2);  DPS = d pre / deg (gather source), DP = d pre of the own rows (padded with zeros)
     for (int idx = tid; idx < n * 8; idx += NT) {
       const int v = idx >> 3, c4 = (idx & 7) * 4;
@@ -1050,7 +1152,6 @@ __device__ __forceinline__ void backward_body(const igmc_model_t& M, const float
     if (l > 0) {
       const int SS = K1p + 4, KS = KRp + 4;
       const int NTN = (R + 1) * 4;                        // 8-column tiles of [dW_r ... | d root]
-      bool arrived = false;
       for (int c0 = 0; c0 < n_own; c0 += chunk) {
         const int crow = min(chunk, n_own - c0);
         // h_{l-1} of the chunk's rows -> Hs, one 128 B bulk copy per row issued by warp 0 (lands under the gather)
@@ -1125,15 +1226,13 @@ __device__ __forceinline__ void backward_body(const igmc_model_t& M, const float
                 *reinterpret_cast<float2*>(DHn + off) = o;
 #pragma unroll
                 for (int pr = 0; pr < 3; ++pr)
-                  if (pr + 1 < CL) *reinterpret_cast<float2*>(peerD[pr] + off) = o;
+                  if (pr + 1 < CL) st_async_peer(DHn + off, o, xbar, peer_rank(rank, pr, CL));
               }
             }
           }
         }
         IGMC_STAMP(sb + 1);
-        // the last chunk's pushes of d h_{l-1} are issued: arrive now, wait at the end of the layer - the
-        // weight-gradient tiles below touch neither peer memory nor the buffer the peers are writing (DHn)
-        if (CL > 1 && c0 + chunk >= n_own) { cluster_arrive(); arrived = true; }
+        // the weight-gradient tiles below touch neither peer memory nor the buffer the peers are writing (DHn)
         // (2) weight gradients over the chunk's rows:  D[k][(r,j) | j'] += sum_u h_{l-1}[u][k] [Q[u] | dpre[u]]
         //     M = 32 (k, two 16-row tiles), N = (R+1)*32, K = crow nodes; warp = (m tile, every (nwarps/2)-th n tile)
         mbar_wait(&mbar[2], huse & 1u); ++huse;            // the chunk's h_{l-1} rows have landed
@@ -1195,7 +1294,6 @@ __device__ __forceinline__ void backward_body(const igmc_model_t& M, const float
         mbar_wait(&mbar[1], wuse & 1u); ++wuse;
         for (int i = tid; i < (R + 1) * HID * HID; i += NT) gpl[i] = 0.f;
       }
-      if (CL > 1 && !arrived) cluster_arrive();
     } else {
       // layer 0: dW[kk][j] = sum_v A[v][kk] dpre[v][j],  A[v] = [ AGG'[v,r,k] (saved, 1/deg-scaled) | x[v,k] one-hot ]
       //          M = KRp rows, N = 32, K = own nodes
@@ -1271,7 +1369,7 @@ __device__ __forceinline__ void backward_body(const igmc_model_t& M, const float
     // (3) every CTA's DH holds d h_{l-1} of all nodes once the pushes have landed; the next layer's weight slab is
     //     requested while they do (every read of Wn is behind the barrier above)
     if (l > 1) load_weights(l - 1);
-    if (CL > 1 && l > 0) cluster_wait();   // nothing is exchanged after layer 0
+    if (CL > 1 && l > 0) mbar_wait_cluster(xbar, (uint32_t)(((L - 1 - l) >> 1) & 1));   // (layer 0 exchanges nothing)
     IGMC_STAMP(sb + 4);
   }
   IGMC_WALL(54);
