@@ -51,7 +51,7 @@ __device__ void build_lists(const int64_t* __restrict__ key_row, const int64_t* 
                             int32_t* __restrict__ ptr_out, uint32_t* __restrict__ adj_out,
                             int32_t* __restrict__ eid_out, uint64_t* __restrict__ tmp, int* cnt, int* fill,
                             int* ws, int* err) {
-  const int tid = threadIdx.x, nt = blockDim.x, lane = tid & 31, warp = tid >> 5, nwarps = nt >> 5;
+  const int tid = threadIdx.x, nt = blockDim.x, warp = tid >> 5, nwarps = nt >> 5;
   for (int v = tid; v <= n; v += nt) cnt[v] = 0;
   __syncthreads();
   for (int e = tid; e < ne; e += nt) {
@@ -60,36 +60,25 @@ __device__ void build_lists(const int64_t* __restrict__ key_row, const int64_t* 
     atomicAdd(&cnt[(int)k], 1);
   }
   __syncthreads();
-  int running = 0;
-  for (int base = 0; base < n; base += nt) {
-    const int v = base + tid;
-    const int c = v < n ? cnt[v] : 0;
-    int tot;
-    const int ex = block_excl_scan_i(c, ws, &tot);
-    if (v < n) { fill[v] = running + ex; ptr_out[nb + v] = eb + running + ex; }
-    running += tot;
-  }
+  block_scan_chunks(
+      n, ws, [&](int v) { return cnt[v]; },
+      [&](int v, int ex) {
+        fill[v] = ex;
+        ptr_out[nb + v] = eb + ex;
+      });
   __syncthreads();
   // unordered placement; fill[v] ends at the list end
   for (int e = tid; e < ne; e += nt) {
     const int64_t k = key_row[eb + e] - nb, o = nbr_row[eb + e] - nb;
     if (k < 0 || k >= n || o < 0 || o >= n) continue;
     const int slot = atomicAdd(&fill[(int)k], 1);
-    const uint64_t ty = (uint64_t)(edge_type[eb + e] & 0xff);
-    tmp[eb + slot] = (ty << 48) | ((uint64_t)o << 32) | (uint64_t)(uint32_t)e;  // (type, nbr, edge) order
+    tmp[eb + slot] = list_key((uint32_t)(edge_type[eb + e] & 0xff), (uint32_t)o, (uint32_t)e);
   }
   __syncthreads();
-  // deterministic order: rank-sort every list by its 64-bit key (lists are short: mean degree ~20)
+  // deterministic order: rank-sort every list by its key (lists are short: mean degree ~20)
   for (int v = warp; v < n; v += nwarps) {
-    const int end = fill[v], k = cnt[v], beg = end - k;
-    for (int i = lane; i < k; i += 32) {
-      const uint64_t key = tmp[eb + beg + i];
-      int rank = 0;
-      for (int q = 0; q < k; ++q) rank += (tmp[eb + beg + q] < key) ? 1 : 0;
-      const uint32_t nbr = (uint32_t)((key >> 32) & 0xffff), ty = (uint32_t)(key >> 48);
-      adj_out[eb + beg + rank] = nbr | (ty << 16);
-      eid_out[eb + beg + rank] = eb + (int)(uint32_t)(key & 0xffffffffu);
-    }
+    const int k = cnt[v], beg = eb + fill[v] - k;
+    rank_sort_list(tmp + beg, k, adj_out + beg, eid_out + beg, eb);
   }
   __syncthreads();
 }

@@ -102,6 +102,22 @@ __device__ __forceinline__ int block_excl_scan_i(int v, int* ws, int* total) {
   return excl;
 }
 
+// Block-wide exclusive scan of in(k), k < n, in chunks of one value per thread: out(k, prefix) for every k < n, called
+// by the thread that called in(k).  Returns the total.  Every thread of the block calls it.
+template <class In, class Out>
+__device__ __forceinline__ int block_scan_chunks(int n, int* ws, In in, Out out) {
+  int running = 0;
+  for (int base = 0; base < n; base += blockDim.x) {
+    const int k = base + threadIdx.x;
+    const int v = k < n ? in(k) : 0;
+    int tot;
+    const int ex = block_excl_scan_i(v, ws, &tot);
+    if (k < n) out(k, running + ex);
+    running += tot;
+  }
+  return running;
+}
+
 __device__ __forceinline__ int block_sum_i(int v, int* ws) {
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
   v = warp_sum_i(v);
@@ -117,6 +133,24 @@ __device__ __forceinline__ int block_sum_i(int v, int* ws) {
   s = ws[32];
   __syncthreads();
   return s;
+}
+
+// ---- message-passing list entries (igmc_adj_t: neighbour | type << 16 and an edge id), built by the extractor and
+// by igmc_batch_prepare.  A list is sorted by (type, neighbour, edge id): the order of this 64-bit key.
+__device__ __forceinline__ uint64_t list_key(uint32_t type, uint32_t nbr, uint32_t eid) {
+  return ((uint64_t)type << 56) | ((uint64_t)nbr << 32) | (uint64_t)eid;
+}
+// Warp-wide rank sort of the k keys at key[0..k) (lists are short): the entry of rank r goes to adj[r] / eid[r], its
+// edge id offset by eid_base.
+__device__ __forceinline__ void rank_sort_list(const uint64_t* __restrict__ key, int k, uint32_t* __restrict__ adj,
+                                               int32_t* __restrict__ eid, int eid_base) {
+  for (int i = threadIdx.x & 31; i < k; i += 32) {
+    const uint64_t x = key[i];
+    int rank = 0;
+    for (int q = 0; q < k; ++q) rank += (key[q] < x) ? 1 : 0;
+    adj[rank] = (uint32_t)((x >> 32) & 0xffffu) | ((uint32_t)(x >> 56) << 16);
+    eid[rank] = eid_base + (int32_t)(uint32_t)(x & 0xffffffffu);
+  }
 }
 
 // ---- async-proxy bulk copies (TMA, 1-D) + mbarrier completion --------------------------------------

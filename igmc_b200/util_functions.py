@@ -743,21 +743,15 @@ class SubgraphExtractor(_BatchWriter):
                                  "(serve_sessions)" % (self.session_row_deg, sessions.max_row_deg))
             sess = _on_device(sess, torch.int32, dev)
             keep += [sess, sessions]
+        head = (C.byref(P), B, self.h, self.mnph, self.sample_ratio, self.seed if seed is None else int(seed),
+                _lib.ptr(seed_dev), self.cap)
+        tail = (C.byref(self._ws_c), self.class_values.data_ptr(), int(self.class_values.numel()),
+                int(self._row_deg()), C.byref(o["_c"]), o["err"].data_ptr(), _stream_ptr())
+        if sessions is not None:
             _lib.check(self.lib.igmc_extract_sessions(C.byref(self.graph._c), C.byref(sessions._c), sess.data_ptr(),
-                                                      C.byref(P), B, self.h, self.mnph, self.sample_ratio,
-                                                      self.seed if seed is None else int(seed), _lib.ptr(seed_dev),
-                                                      self.cap, C.byref(self._ws_c), self.class_values.data_ptr(),
-                                                      int(self.class_values.numel()), int(self._row_deg()),
-                                                      C.byref(o["_c"]), o["err"].data_ptr(), _stream_ptr()),
-                       "igmc_extract_sessions")
-            return self._batch(B, o, keep)
-        _lib.check(self.lib.igmc_extract_batch(C.byref(self.graph._c), C.byref(P), B, self.h, self.mnph,
-                                               self.sample_ratio, self.seed if seed is None else int(seed),
-                                               _lib.ptr(seed_dev), self.cap, inj[0], inj[1], inj[2], inj[3],
-                                               C.byref(self._ws_c),
-                                               self.class_values.data_ptr(), int(self.class_values.numel()),
-                                               int(self._row_deg()), C.byref(o["_c"]), o["err"].data_ptr(),
-                                               _stream_ptr()), "igmc_extract_batch")
+                                                      *head, *tail), "igmc_extract_sessions")
+        else:
+            _lib.check(self.lib.igmc_extract_batch(C.byref(self.graph._c), *head, *inj, *tail), "igmc_extract_batch")
         return self._batch(B, o, keep)
 
     def plan(self, B):

@@ -64,10 +64,20 @@ def test_forward_on_extracted_batch_matches_foreign_batch():
     m.eval()
     ds = MyDynamicDataset(None, A, (u, v), lab, 1, 1.0, 30, None, None, cv, seed=5)
     b = ds.extract_batch(np.arange(16))
+    fb = _gpu_batch(ob)
     with torch.no_grad():
         p1 = m(b).clone()
-        p2 = m(_gpu_batch(ob)).clone()
+        p2 = m(fb).clone()
     assert torch.equal(p1, p2)
+    # both producers sort every in-list by (type, neighbour, edge id): over the same canonical edges, the foreign
+    # batch's igmc_batch_prepare lists equal the extractor's element by element
+    N, E = ob["x"].shape[0], ob["edge_index"].shape[1]
+    assert torch.equal(b.edge_index.cpu(), torch.as_tensor(ob["edge_index"], dtype=torch.int64))
+    assert torch.equal(b.edge_type.cpu(), torch.as_tensor(ob["edge_type"], dtype=torch.int64))
+    got, want = b.adjacency()[1], fb.adjacency()[1]
+    assert torch.equal(got["adj_in_ptr"][:N + 1], want["in_ptr"][:N + 1])
+    assert torch.equal(got["adj_in"][:E], want["in_adj"][:E])
+    assert torch.equal(got["adj_eid"][:E], want["in_eid"][:E])
 
 
 @pytest.mark.parametrize("R,NB,symmetric,plan", [(5, 4, True, 0), (5, 4, True, 1), (5, 4, True, 2), (5, 4, True, 3), (5, 4, True, 4),
