@@ -185,6 +185,7 @@ _SIGS = {
     "igmc_gate_wait": [vp, C.c_int, C.c_int, vp],
     "igmc_candidate_plan": [C.POINTER(CSR), C.POINTER(Candidates), vp, vp],
     "igmc_candidate_pairs": [C.POINTER(CSR), C.POINTER(Candidates), vp, C.c_int, vp, vp, vp, vp, vp, vp],
+    "igmc_item_query_pairs": [C.c_int, C.c_int, vp, vp, vp, vp, vp],
     "igmc_topk_merge": [vp, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp, vp],
     "igmc_score_scatter": [vp, C.c_int, C.c_int, vp, vp, vp],
     "igmc_topk_fits": [C.c_int, C.c_int],
@@ -210,6 +211,7 @@ _SIGS = {
     "igmc_influence_topk": [vp, C.c_int, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp],
     "igmc_corated_ws_bytes":[C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int64)],
     "igmc_corated_items": [C.POINTER(CSR), vp, C.c_int, C.c_int, C.c_int, vp, C.c_int64, vp, vp, vp, vp],
+    "igmc_corated_users": [C.POINTER(CSR), vp, C.c_int, C.c_int, C.c_int, vp, C.c_int64, vp, vp, vp, vp],
     "igmc_graph_update_ws_bytes": [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int64)],
     "igmc_graph_update_plan": [C.POINTER(CSR), C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, C.c_int, C.c_int,
                                C.c_int, vp, C.c_int64, vp, vp, vp],

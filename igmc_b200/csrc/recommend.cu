@@ -11,6 +11,8 @@
 //   k_topk_merge       one CTA per per-user segment of the batch: fp32 checkpoint mean + merge into the running
 //                      [U, k] (score, item) list
 //   k_score_scatter    explicit pairs: the fp32 checkpoint mean stored at the pair's index
+//   k_item_query_pairs item-side runs (query items, candidate users): the candidate kernels run on the transposed view
+//                      of the graph, and this post-pass turns their (item, user) pairs back into (user, item) ones
 // No float atomics: the ranking order (score descending, item ascending, NaN last, empty slots after everything) is a
 // strict total order on distinct items, so the top-k of a user does not depend on where batch boundaries fall.
 #include <cub/device/device_segmented_radix_sort.cuh>
@@ -295,6 +297,24 @@ k_score_scatter(const float* __restrict__ preds, int K, int B, const int64_t* __
   if (t >= 0) scores[t] = ckpt_mean(preds, K, B, i);
 }
 
+// pairs igmc_candidate_pairs wrote over the transposed view (links_u = the query item, links_v = the candidate user):
+// swapped back, with the pair id (user, item) samples its subgraph with
+__global__ void __launch_bounds__(LIST_THREADS)
+k_item_query_pairs(int num_items, int B, int32_t* __restrict__ links_u, int32_t* __restrict__ links_v,
+                   int64_t* __restrict__ pair_id, int* err) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < B; i += gridDim.x * blockDim.x) {
+    int v = links_u[i], u = links_v[i];
+    if (v < 0 || v >= num_items || u < 0) {
+      igmc_set_err(err, IGMC_ERR_CANDIDATES);
+      u = 0;
+      v = 0;
+    }
+    links_u[i] = u;
+    links_v[i] = v;
+    pair_id[i] = (int64_t)u * num_items + v;
+  }
+}
+
 }  // namespace
 
 extern "C" int igmc_candidate_plan(const igmc_csr_t* G, const igmc_candidates_t* Cd, int* err, void* stream) {
@@ -373,6 +393,15 @@ extern "C" int igmc_candidate_pairs(const igmc_csr_t* G, const igmc_candidates_t
   if (Cd->per_user && (!Cd->users || !Cd->cand)) return -1;
   k_candidate_pairs<<<1, PAIR_THREADS, 0, (cudaStream_t)stream>>>(*G, *Cd, cursor, B, links_u, links_v, pair_id, tag,
                                                                    err);
+  IGMC_CUDA_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" int igmc_item_query_pairs(int num_items, int B, int32_t* links_u, int32_t* links_v, int64_t* pair_id,
+                                     int* err, void* stream) {
+  if (num_items < 1 || B <= 0 || !links_u || !links_v || !pair_id) return -1;
+  k_item_query_pairs<<<(B + LIST_THREADS - 1) / LIST_THREADS, LIST_THREADS, 0, (cudaStream_t)stream>>>(
+      num_items, B, links_u, links_v, pair_id, err);
   IGMC_CUDA_CHECK_LAUNCH();
   return 0;
 }

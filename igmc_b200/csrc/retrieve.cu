@@ -11,6 +11,12 @@
 //   select         radix select of the M-th largest count (8 bits a pass), ties at the threshold in ascending item
 //                  order, then a bitonic sort of the chosen (~paths, item) keys: paths descending, item ascending
 // Integer arithmetic only and every output has one writer: two runs are bit-identical.
+//
+// Item side (igmc_b200/recommend.py: corated_users): the same body runs on the transposed view T (T's rows are G's
+// columns), query v an item, with the count C[u][v] = (B B^T B)[u][v] - deg(u) B[u][v] of corated_items:
+//   pass 1 (push)  w[i] += 1 for every u' in col(v), i in row(u') - no exclusion, so w[v] = deg(v)
+//   pass 2 (pull)  paths[u] = sum over i in row(u) of w[i], minus deg(u) when row(u) holds v (the u' = u term)
+// The user-side exclusion u' != u is not the item-side i != v: on a rated pair they differ by (deg(v) - deg(u)).
 #include "common.cuh"
 #include "../../include/igmc_b200.h"
 
@@ -57,13 +63,18 @@ __device__ __forceinline__ int block_excl_count(bool f, int* wsum, int* total) {
   return r;
 }
 
-// SESS: query j is session j of Q (igmc_sessions_t): N(u) is its session row, u = Q.users[j] its real id (a new
-// user, u >= num_users, is in no column of G and is never looked up in w)
-template <bool SESS>
+// MODE_USER: query j is user users[j] of G.  MODE_SESS: query j is session j of Q (igmc_sessions_t): N(u) is its
+// session row, u = Q.users[j] its real id (a new user, u >= num_users, is in no column of G and is never looked up in
+// w).  MODE_ITEM: G is the transposed view and query j is item users[j]; "users" of the body are items and "items"
+// users (pass 1 keeps i = v, pass 2 takes out the u' = u term).
+enum { MODE_USER, MODE_SESS, MODE_ITEM };
+
+template <int MODE>
 __device__ __forceinline__ void
 corated(const igmc_csr_t& G, const int32_t* __restrict__ users, int U, int m, int exclude_rated, int in_shared,
         unsigned char* __restrict__ ws, size_t ws_row, int32_t* __restrict__ out_items, int32_t* __restrict__ out_paths,
         int* err, const igmc_sessions_t& Q) {
+  constexpr bool SESS = MODE == MODE_SESS;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   __shared__ int hist[256];
   __shared__ int wsum[WARPS + 1];
@@ -97,14 +108,19 @@ corated(const igmc_csr_t& G, const int32_t* __restrict__ users, int U, int m, in
       const int i = qi[e];
       for (int q = G.col_ptr[i] + lane; q < G.col_ptr[i + 1]; q += 32) {
         const int v = G.row_idx[q];
-        if (v != u) atomicAdd(&w[v], 1u);
+        if (MODE == MODE_ITEM || v != u) atomicAdd(&w[v], 1u);
       }
     }
     __syncthreads();
     // pass 2: item scores, a warp per item
     for (int v = warp; v < ni; v += WARPS) {
       unsigned s = 0;
-      for (int q = G.col_ptr[v] + lane; q < G.col_ptr[v + 1]; q += 32) s += w[G.row_idx[q]];
+      for (int q = G.col_ptr[v] + lane; q < G.col_ptr[v + 1]; q += 32) {
+        const int x = G.row_idx[q];
+        s += w[x];
+        // item side (v a user, u the query item): when v rated u, the u' = v term - deg(v) paths through v - comes out
+        if (MODE == MODE_ITEM && x == u) s -= (unsigned)(G.col_ptr[v + 1] - G.col_ptr[v]);
+      }
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(IGMC_FULL, s, o);
       if (lane == 0) paths[v] = s;
@@ -197,14 +213,38 @@ __global__ void __launch_bounds__(THREADS)
 k_corated(igmc_csr_t G, const int32_t* __restrict__ users, int U, int m, int exclude_rated, int in_shared,
           unsigned char* __restrict__ ws, size_t ws_row, int32_t* __restrict__ out_items,
           int32_t* __restrict__ out_paths, int* err) {
-  corated<false>(G, users, U, m, exclude_rated, in_shared, ws, ws_row, out_items, out_paths, err, igmc_sessions_t{});
+  corated<MODE_USER>(G, users, U, m, exclude_rated, in_shared, ws, ws_row, out_items, out_paths, err,
+                     igmc_sessions_t{});
+}
+
+__global__ void __launch_bounds__(THREADS)
+k_corated_users(igmc_csr_t T, const int32_t* __restrict__ items, int I, int m, int exclude_rated, int in_shared,
+                unsigned char* __restrict__ ws, size_t ws_row, int32_t* __restrict__ out_users,
+                int32_t* __restrict__ out_paths, int* err) {
+  corated<MODE_ITEM>(T, items, I, m, exclude_rated, in_shared, ws, ws_row, out_users, out_paths, err,
+                     igmc_sessions_t{});
 }
 
 __global__ void __launch_bounds__(THREADS)
 k_corated_sess(igmc_csr_t G, igmc_sessions_t Q, int m, int exclude_rated, int in_shared,
                unsigned char* __restrict__ ws, size_t ws_row, int32_t* __restrict__ out_items,
                int32_t* __restrict__ out_paths, int* err) {
-  corated<true>(G, nullptr, Q.num_sessions, m, exclude_rated, in_shared, ws, ws_row, out_items, out_paths, err, Q);
+  corated<MODE_SESS>(G, nullptr, Q.num_sessions, m, exclude_rated, in_shared, ws, ws_row, out_items, out_paths, err,
+                     Q);
+}
+
+// the launch shape of U queries on G: the histogram row, whether it fits in shared memory and the grid; -2 when the
+// global-memory regime has no workspace of grid rows
+int launch_shape(const igmc_csr_t& G, int U, int m, const void* ws, int64_t ws_bytes, size_t* row, bool* shared,
+                 int* grid) {
+  *row = row_bytes(G.num_users, G.num_items, m);
+  *shared = fits_shared(G.num_users, G.num_items, m);
+  *grid = U;
+  if (!*shared) {
+    *grid = U < GLOBAL_CTAS ? U : GLOBAL_CTAS;
+    if (!ws || ws_bytes < (int64_t)*grid * (int64_t)*row) return -2;
+  }
+  return 0;
 }
 
 }  // namespace
@@ -226,14 +266,10 @@ extern "C" int igmc_corated_items(const igmc_csr_t* G, const int32_t* users, int
   if (!G || num_query < 0 || m < 1 || m > G->num_items) return -1;
   if (num_query == 0) return 0;
   if (!users || !items || !paths) return -1;
-  const int nu = G->num_users, ni = G->num_items;
-  const size_t row = row_bytes(nu, ni, m);
-  const bool shared = fits_shared(nu, ni, m);
-  int grid = num_query;
-  if (!shared) {
-    grid = num_query < GLOBAL_CTAS ? num_query : GLOBAL_CTAS;
-    if (!ws || ws_bytes < (int64_t)grid * (int64_t)row) return -2;
-  }
+  size_t row;
+  bool shared;
+  int grid;
+  if (launch_shape(*G, num_query, m, ws, ws_bytes, &row, &shared, &grid)) return -2;
   const size_t smem = shared ? row : 0;
   // opted in at every size: the static histogram and scan words count against the default 48 KB as well
   cudaFuncSetAttribute(k_corated, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -251,20 +287,36 @@ extern "C" int igmc_corated_sessions(const igmc_csr_t* G, const igmc_sessions_t*
   const int U = S->num_sessions;
   if (U == 0) return 0;
   if (!S->users || !S->row_ptr || !items || !paths) return -1;
-  const int nu = G->num_users, ni = G->num_items;
-  const size_t row = row_bytes(nu, ni, m);
-  const bool shared = fits_shared(nu, ni, m);
-  int grid = U;
-  if (!shared) {
-    grid = U < GLOBAL_CTAS ? U : GLOBAL_CTAS;
-    if (!ws || ws_bytes < (int64_t)grid * (int64_t)row) return -2;
-  }
+  size_t row;
+  bool shared;
+  int grid;
+  if (launch_shape(*G, U, m, ws, ws_bytes, &row, &shared, &grid)) return -2;
   const size_t smem = shared ? row : 0;
   // opted in at every size: the static histogram and scan words count against the default 48 KB as well
   cudaFuncSetAttribute(k_corated_sess, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   k_corated_sess<<<grid, THREADS, smem, (cudaStream_t)stream>>>(*G, *S, m, exclude_rated ? 1 : 0, shared ? 1 : 0,
                                                                 static_cast<unsigned char*>(ws), row, items, paths,
                                                                 err);
+  IGMC_CUDA_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" int igmc_corated_users(const igmc_csr_t* T, const int32_t* items, int num_query, int m, int exclude_rated,
+                                  void* ws, int64_t ws_bytes, int32_t* users, int32_t* paths, int* err,
+                                  void* stream) {
+  if (!T || num_query < 0 || m < 1 || m > T->num_items) return -1;
+  if (num_query == 0) return 0;
+  if (!items || !users || !paths) return -1;
+  size_t row;
+  bool shared;
+  int grid;
+  if (launch_shape(*T, num_query, m, ws, ws_bytes, &row, &shared, &grid)) return -2;
+  const size_t smem = shared ? row : 0;
+  // opted in at every size: the static histogram and scan words count against the default 48 KB as well
+  cudaFuncSetAttribute(k_corated_users, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  k_corated_users<<<grid, THREADS, smem, (cudaStream_t)stream>>>(*T, items, num_query, m, exclude_rated ? 1 : 0,
+                                                                 shared ? 1 : 0, static_cast<unsigned char*>(ws), row,
+                                                                 users, paths, err);
   IGMC_CUDA_CHECK_LAUNCH();
   return 0;
 }

@@ -11,6 +11,11 @@ building a dataset of every candidate pair and looping over it in Python.  Here:
   last; missing slots hold item -1 and score -inf;
 * ``corated_items(graph, users, m)`` -> per query user the ``m`` items with the most bridges (3-paths u - i - u' - v,
   ``igmc_corated_items``): the cheap first stage that proposes each user's candidates for the model to rank;
+* ``recommend_users(model, graph, items, k)`` and ``corated_users(graph, items, m)`` ask the same from the item's side:
+  per query item the ``k`` best users (the audience of a new or promoted item) and the ``m`` users with the most
+  bridges to it.  The candidate kernels run on the graph's transposed view (``RatingGraph._ct``) and
+  ``igmc_item_query_pairs`` turns their pairs back into (user, item); every score is ``predict_pairs``' score of the
+  pair;
 * ``explain_pairs(model, graph, users, items, m)`` -> per pair its score and, for every rating in its enclosing
   subgraph, the score change from removing that rating (csrc/explain.cu): a base pass of the pairs, then an occlusion
   pass over (pair, rating) positions whose batches carry an edge mask into a training-mode forward without dropout;
@@ -50,7 +55,8 @@ from .util_functions import RatingGraph, SubgraphExtractor, _cuda_ints, _on_devi
 
 __all__ = ["predict_pairs", "recommend", "corated_items", "explain_pairs", "Explanation", "attribute_pairs",
            "Attribution", "pair_gradients", "influence", "self_influence", "Influence", "InferenceEngine",
-           "RatingSessions", "predict_sessions", "recommend_sessions", "corated_items_sessions"]
+           "RatingSessions", "predict_sessions", "recommend_sessions", "corated_items_sessions", "recommend_users",
+           "corated_users"]
 
 
 # ---- input validation (host) ----------------------------------------------------------------------------------------
@@ -75,23 +81,23 @@ def _is_rows(items):
     return items is not None and (items.dim() == 2 if torch.is_tensor(items) else np.ndim(items) == 2)
 
 
-def _user_rows(items, U, num_items):
+def _user_rows(items, U, num_items, name="items"):
     """per-user candidate rows [U, width] checked on the host: a host array as int32 (IndexError for an id outside
     [-1, num_items)); an integer CUDA tensor as it is, checked by the kernel.  ValueError when the row count is not
-    U."""
+    U.  ``name``: the argument the rows came in (item-side runs: per-item rows of users)."""
     if not torch.is_tensor(items):
         items = np.asarray(items)
     if items.shape[0] != U:
-        raise ValueError("items has %d rows, one per query slot is %d" % (items.shape[0], U))
-    if _cuda_ints(items, "items"):
+        raise ValueError("%s has %d rows, one per query slot is %d" % (name, items.shape[0], U))
+    if _cuda_ints(items, name):
         return items
     a = np.asarray(items.cpu().numpy() if torch.is_tensor(items) else items)
     if a.size and not np.issubdtype(a.dtype, np.integer):
-        raise TypeError("items must be integers, not %s" % a.dtype)
+        raise TypeError("%s must be integers, not %s" % (name, a.dtype))
     a = a.astype(np.int64)
     if a.size and (a.min() < -1 or a.max() >= num_items):
         bad = int(a.min()) if a.min() < -1 else int(a.max())
-        raise IndexError("items: id %d out of range [-1, %d)" % (bad, num_items))
+        raise IndexError("%s: id %d out of range [-1, %d)" % (name, bad, num_items))
     return a.astype(np.int32)
 
 
@@ -108,27 +114,28 @@ def _check_top(m):
     return None if m is None else _check_count(m, "m", _lib.TOPK_MAX)
 
 
-def _ranking_inputs(k, batch_size, items, retrieve, U, num_items):
+def _ranking_inputs(k, batch_size, items, retrieve, U, num_items, name="items"):
     """(k, m, cand, rows) of a ranking run over U query slots, checked on the host: m = ``retrieve`` (or None), cand
     the sorted distinct items of a 1-D ``items`` (or None), rows a 2-D ``items`` as ``_user_rows`` returns it (or
-    None)"""
+    None).  Item-side runs pass the candidate users as ``items``, num_users as ``num_items`` and ``name`` = "users"."""
     k = _check_count(k, "k", _lib.TOPK_MAX)
     _check_merge_fits(k, batch_size)
     if retrieve is not None and items is not None:
-        raise ValueError("retrieve= chooses the candidates itself: pass it without items=")
+        raise ValueError("retrieve= chooses the candidates itself: pass it without %s=" % name)
     m = None if retrieve is None else _check_count(retrieve, "retrieve", num_items, ValueError)
     if _is_rows(items):
-        return k, m, None, _user_rows(items, U, num_items)
-    return k, m, None if items is None else np.unique(_host_ids(items, "items", num_items)), None
+        return k, m, None, _user_rows(items, U, num_items, name)
+    return k, m, None if items is None else np.unique(_host_ids(items, name, num_items)), None
 
 
-def _corated(lib, g, entry, args, U, m, exclude_rated, err, ws):
-    """the retriever ``entry`` (igmc_corated_items or igmc_corated_sessions, leading arguments ``args``) for U query
-    slots on graph ``g``: (items, paths) [U, m] int32.  ``ws``: a dict whose "ws" tensor is grown to the workspace the
+def _corated(lib, shape, entry, args, U, m, exclude_rated, err, ws):
+    """the retriever ``entry`` (igmc_corated_items, igmc_corated_sessions or igmc_corated_users, leading arguments
+    ``args``) for U query slots on a graph of ``shape`` (num_users, num_items; the item side: the transposed shape):
+    (ids, paths) [U, m] int32 on ``err``'s device.  ``ws``: a dict whose "ws" tensor is grown to the workspace the
     shape needs"""
-    dev = g.device
+    dev = err.device
     nbytes = C.c_int64(0)
-    _lib.check(lib.igmc_corated_ws_bytes(g.num_users, g.num_items, U, m, C.byref(nbytes)), "igmc_corated_ws_bytes")
+    _lib.check(lib.igmc_corated_ws_bytes(shape[0], shape[1], U, m, C.byref(nbytes)), "igmc_corated_ws_bytes")
     if ws.get("ws") is None or ws["ws"].numel() < nbytes.value:
         ws["ws"] = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=dev)
     items = torch.empty(U, m, dtype=torch.int32, device=dev)
@@ -394,6 +401,37 @@ def corated_host(row_ptr, col_idx, num_users, num_items, users, m, exclude_rated
     return items, paths
 
 
+def corated_users_host(row_ptr, col_idx, num_users, num_items, items, m, exclude_rated=True):
+    """twin of igmc_corated_users: per query item v the ``m`` users with the most bridges, C[u][v] = (B B^T B)[u][v]
+    - deg(u) B[u][v] (``corated_host``'s count of v for u), ordered by count descending then user ascending, users
+    without a bridge dropped, ``exclude_rated`` dropping v's raters; (users [I, m], paths [I, m]) int32 padded with
+    -1 / 0"""
+    import scipy.sparse as ssp
+    items = np.asarray(items, np.int64).reshape(-1)
+    rp = np.asarray(row_ptr, np.int64)
+    nnz = int(rp[num_users])
+    Bm = ssp.csr_matrix((np.ones(nnz, np.int64), np.asarray(col_idx[:nnz], np.int64), rp[:num_users + 1]),
+                        shape=(num_users, num_items))
+    Bv = Bm[:, items].toarray()                              # [nu, I]
+    P = np.asarray((Bm @ (Bm.T @ ssp.csr_matrix(Bv))).toarray(), np.int64) - np.diff(rp)[:num_users, None] * Bv
+    if exclude_rated:
+        P[Bv > 0] = 0
+    users = np.full((len(items), m), -1, np.int32)
+    paths = np.zeros((len(items), m), np.int32)
+    for j in range(len(items)):
+        o = np.argsort(-P[:, j], kind="stable")[:m]         # count descending, then user ascending
+        o = o[P[o, j] > 0]
+        users[j, :len(o)], paths[j, :len(o)] = o, P[o, j]
+    return users, paths
+
+
+def item_query_pairs_host(num_items, links_u, links_v):
+    """twin of igmc_item_query_pairs: the (item, user) pairs of a run over the transposed view as (links_u = users,
+    links_v = items, pair_id = u * num_items + v)"""
+    u, v = np.asarray(links_v, np.int64), np.asarray(links_u, np.int64)
+    return u, v, u * num_items + v
+
+
 def candidate_lists_host(row_ptr, col_idx, num_items, users, rows, exclude_rated=True):
     """twin of igmc_candidate_lists: (user_off [U+1] int64, lists) - per query slot its row sorted, deduplicated, -1
     slots dropped and (exclude_rated) the user's rated items removed"""
@@ -629,6 +667,7 @@ class InferenceEngine(object):
 
         eng = InferenceEngine(model, graph, batch_size=256)
         eng.start_recommend(users, k)          # or start_pairs(users, items) / start_explain / start_attribute(users, items, m)
+                                               # or start_recommend_users(items, k): per item its best users
         while eng.step():
             pass
         top_items, top_scores = eng.finish()   # (predict: scores; explain: an Explanation; attribute: an Attribution)
@@ -706,14 +745,32 @@ class InferenceEngine(object):
         return self._plan_ranking(sessions._slots, k, m, cand, rows, exclude_rated, lambda: sessions.nnz,
                                   "igmc_corated_sessions", (C.byref(self.graph._c), C.byref(sessions._c)), sessions)
 
-    def _plan_ranking(self, slots, k, m, cand, rows, exclude_rated, rated, retriever, args, sessions=None):
+    def start_recommend_users(self, items, k, users=None, exclude_rated=True, retrieve=None):
+        """plan an item-side ranking run (``recommend_users``): per query item its best users.  ``users``: one
+        candidate list for every item, or a 2-D [I, width] array of per-item lists (-1 = empty slot); ``retrieve=M``:
+        each item's M users with the most bridges (``corated_users``).  The candidate kernels run on the graph's
+        transposed view.  Returns the number of candidate pairs."""
+        g = self.graph
+        items = _host_ids(items, "items", g.num_items)
+        k, m, cand, rows = _ranking_inputs(k, self.B, users, retrieve, len(items), g.num_users, "users")
+        slots = torch.from_numpy(items.astype(np.int32)).to(self.dev)
+
+        def rated():     # the items' summed column lengths (host column pointers: a copy after an update)
+            cp = g.host["col_ptr"]
+            return int((cp[items + 1] - cp[items]).sum())
+        return self._plan_ranking(slots, k, m, cand, rows, exclude_rated, rated,
+                                  "igmc_corated_users", (C.byref(g._ct), slots.data_ptr(), len(items)), by_item=True)
+
+    def _plan_ranking(self, slots, k, m, cand, rows, exclude_rated, rated, retriever, args, sessions=None,
+                      by_item=False):
         """the plan of a ranking run over the query slots ``slots`` (int32, on the device) with ``_ranking_inputs``'
         (k, m, cand, rows): the candidate plan over every item or the list ``cand`` (``rated()``: the slots' summed row
         lengths, room for their rated positions in the list), or per-slot rows from ``rows`` or from the retriever entry
-        ``retriever`` (leading arguments ``args``).  ``sessions``: the slots are these sessions.  Returns the number of
-        candidate pairs."""
-        U, dev = int(slots.numel()), self.dev
-        run = dict(kind="recommend", U=U, k=k, version=self.graph.version, sessions=sessions, users=slots,
+        ``retriever`` (leading arguments ``args``).  ``sessions``: the slots are these sessions.  ``by_item``: the
+        slots are items and the candidates users - the plan runs on the graph's transposed view, whose rows are the
+        items' columns.  Returns the number of candidate pairs."""
+        U, dev, g = int(slots.numel()), self.dev, self.graph
+        run = dict(kind="recommend", U=U, k=k, version=g.version, sessions=sessions, users=slots, by_item=by_item,
                    top_s=torch.full((U, k), -float("inf"), dtype=torch.float32, device=dev),
                    top_i=torch.full((U, k), -1, dtype=torch.int64, device=dev))
         self.run = run
@@ -721,8 +778,8 @@ class InferenceEngine(object):
             run["P"] = 0
             return 0
         if m is not None:
-            rows, _ = _corated(self.lib, self.graph, retriever, args, U, m, exclude_rated, self.extractor.err,
-                               self._retrieve_ws)
+            rows, _ = _corated(self.lib, g.shape[::-1] if by_item else g.shape, retriever, args, U, m, exclude_rated,
+                               self.extractor.err, self._retrieve_ws)
         if rows is not None:
             return self._plan_lists(run, rows, exclude_rated)
         Cd = self._query_candidates(run, exclude_rated)
@@ -778,7 +835,10 @@ class InferenceEngine(object):
 
     # ---- rating sessions ----------------------------------------------------------------------------------------
     def _csr(self, run):
-        """the rows the candidate kernels read: the graph's, or a session run's rows as a CSR over its sessions"""
+        """the rows the candidate kernels read: the graph's, its transposed view on an item-side run, or a session
+        run's rows as a CSR over its sessions"""
+        if run.get("by_item"):
+            return self.graph._ct
         return run["sessions"]._view if run.get("sessions") is not None else self.graph._c
 
     def _session_slots(self, sessions):
@@ -1058,6 +1118,11 @@ class InferenceEngine(object):
                                                      self.cursor.data_ptr(), self.B, s["u"].data_ptr(),
                                                      s["v"].data_ptr(), s["pid"].data_ptr(), s["tag"].data_ptr(), err,
                                                      _stream_ptr()), "igmc_candidate_pairs")
+        if run.get("by_item"):
+            # pairs over the transposed view are (item, user): back to (user, item) and the pair's own pair id
+            _lib.check(self.lib.igmc_item_query_pairs(self.graph.num_items, self.B, s["u"].data_ptr(),
+                                                      s["v"].data_ptr(), s["pid"].data_ptr(), err, _stream_ptr()),
+                       "igmc_item_query_pairs")
         sessions = run.get("sessions")
         if sessions is not None:
             # links_u holds the session: to the session's user id, its pair id and the per-pair session index
@@ -1109,8 +1174,9 @@ class InferenceEngine(object):
                 self.preds[j].copy_(pred)
                 preds = self.preds
         if run["kind"] == "recommend":
+            ranked = s["u"] if run.get("by_item") else s["v"]      # the candidates: users on an item-side run
             _lib.check(self.lib.igmc_topk_merge(preds.data_ptr(), self.K, self.B, s["tag"].data_ptr(),
-                                                s["v"].data_ptr(), run["k"], run["top_s"].data_ptr(),
+                                                ranked.data_ptr(), run["k"], run["top_s"].data_ptr(),
                                                 run["top_i"].data_ptr(), _stream_ptr()), "igmc_topk_merge")
         else:
             out = run["occ"] if occlude else run["scores"]
@@ -1231,6 +1297,10 @@ class InferenceEngine(object):
 
     def recommend(self, users, k, items=None, exclude_rated=True, retrieve=None):
         self.start_recommend(users, k, items, exclude_rated, retrieve)
+        return self.finish()
+
+    def recommend_users(self, items, k, users=None, exclude_rated=True, retrieve=None):
+        self.start_recommend_users(items, k, users, exclude_rated, retrieve)
         return self.finish()
 
     def predict_pairs(self, users, items):
@@ -1431,10 +1501,50 @@ def corated_items(graph, users, m, exclude_rated=True):
     users = _host_ids(users, "users", g.num_users)
     err = torch.zeros(1, dtype=torch.int32, device=g.device)
     du = torch.from_numpy(users.astype(np.int32)).to(g.device)
-    items, paths = _corated(_lib.load(), g, "igmc_corated_items", (C.byref(g._c), du.data_ptr(), len(users)),
+    items, paths = _corated(_lib.load(), g.shape, "igmc_corated_items", (C.byref(g._c), du.data_ptr(), len(users)),
                             len(users), m, exclude_rated, err, {})
     _lib.check_kernel_error(int(err.item()))
     return items, paths
+
+
+def recommend_users(model, graph, items, k, *, users=None, exclude_rated=True, retrieve=None, h=1, sample_ratio=1.0,
+                    max_nodes_per_hop=None, batch_size=256, checkpoints=None, sample_seed=0):
+    """for every query item the ``k`` best candidate users - the audience of a new or promoted item: (top_users [I, k]
+    int64, top_scores [I, k] fp32), on the model's device.  Candidates: ``users`` (sorted, deduplicated), a 2-D
+    ``users`` [I, width] of per-item lists (-1 = empty slot), the item's ``retrieve`` users with the most bridges
+    (``corated_users``), or every user; minus the item's raters when ``exclude_rated``.  Order: score descending, then
+    user ascending; a NaN score ranks last; an item with fewer than ``k`` candidates gets user -1 / score -inf in the
+    empty slots.  A pair's score is ``predict_pairs``' score of (u, v) bit for bit at the same batch size and kernel
+    plan (pair id u * num_items + v): the lists filter those scores and compute nothing new.  An item added with
+    ``graph.update`` and a few ratings is ranked against every user without retraining."""
+    items = _host_ids(items, "items", graph.shape[1])
+    k = _ranking_inputs(k, batch_size, users, retrieve, len(items), graph.shape[0], "users")[0]
+    if len(items) == 0:
+        dev = model.flat_params.device
+        return (torch.zeros(0, k, dtype=torch.int64, device=dev), torch.zeros(0, k, dtype=torch.float32, device=dev))
+    return _on_engine(model, graph, lambda eng: eng.recommend_users(items, k, users, exclude_rated, retrieve),
+                      h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
+
+
+def corated_users(graph, items, m, exclude_rated=True):
+    """per query item the ``m`` users with the most bridges to it: (users [I, m], paths [I, m]) int32 on the graph's
+    device.  The count for user u is exactly the count ``corated_items`` gives item v for u, C[u][v] = (B B^T B)[u][v]
+    - deg(u) B[u][v] (B the 0/1 rating matrix): the 3-paths u - i - u' - v with u' != u.  Ordered by count descending,
+    then user ascending; users without a bridge are never returned, the rest of a row is user -1 / paths 0;
+    ``exclude_rated`` drops the item's raters.  Exact integer counts: runs are bit-identical.  ``graph``: a RatingGraph
+    or a rating matrix (copied to the current CUDA device).  One host synchronisation (the error word)."""
+    g = graph if isinstance(graph, RatingGraph) else RatingGraph(graph)
+    m = _check_count(m, "m", g.num_users, ValueError)
+    items = _host_ids(items, "items", g.num_items)
+    if g.device is None:
+        raise RuntimeError("igmc_b200 retrieval runs on a CUDA device (there is no CPU path)")
+    err = torch.zeros(1, dtype=torch.int32, device=g.device)
+    dv = torch.from_numpy(items.astype(np.int32)).to(g.device)
+    users, paths = _corated(_lib.load(), g.shape[::-1], "igmc_corated_users", (C.byref(g._ct), dv.data_ptr(),
+                                                                                len(items)),
+                            len(items), m, exclude_rated, err, {})
+    _lib.check_kernel_error(int(err.item()))
+    return users, paths
 
 
 # ---- rating sessions: public API ------------------------------------------------------------------------------------
@@ -1475,7 +1585,7 @@ def corated_items_sessions(sessions, m, exclude_rated=True):
     g = sessions.graph
     m = _check_count(m, "m", g.num_items, ValueError)
     err = torch.zeros(1, dtype=torch.int32, device=g.device)
-    items, paths = _corated(_lib.load(), g, "igmc_corated_sessions", (C.byref(g._c), C.byref(sessions._c)),
+    items, paths = _corated(_lib.load(), g.shape, "igmc_corated_sessions", (C.byref(g._c), C.byref(sessions._c)),
                             sessions.num_sessions, m, exclude_rated, err, {})
     _lib.check_kernel_error(int(err.item()))
     return items, paths

@@ -153,9 +153,13 @@ class RatingGraph(object):
         return self
 
     def _make_c(self):
-        self._c = _lib.CSR(self.dev["row_ptr"].data_ptr(), self.dev["col_idx"].data_ptr(),
-                           self.dev["rating"].data_ptr(), self.dev["col_ptr"].data_ptr(),
-                           self.dev["row_idx"].data_ptr(), self.num_users, self.num_items)
+        d = self.dev
+        self._c = _lib.CSR(d["row_ptr"].data_ptr(), d["col_idx"].data_ptr(), d["rating"].data_ptr(),
+                           d["col_ptr"].data_ptr(), d["row_idx"].data_ptr(), self.num_users, self.num_items)
+        # the transposed view: rows are items, columns users (no ratings: they are not in column order).  What the
+        # candidate kernels and the retriever read on item-side runs (include/igmc_b200.h: igmc_item_query_pairs)
+        self._ct = _lib.CSR(d["col_ptr"].data_ptr(), d["row_idx"].data_ptr(), None, d["row_ptr"].data_ptr(),
+                            d["col_idx"].data_ptr(), self.num_items, self.num_users)
 
     def node_cap(self, max_nodes_per_hop, h=1, max_row_deg=None):
         """capacity of one side's node list: target + per hop min(mnph, largest possible fringe) (hop 1: a row or

@@ -467,6 +467,19 @@ int igmc_candidate_lists(const igmc_csr_t* G, const igmc_candidates_t* Cd, const
 int igmc_candidate_pairs(const igmc_csr_t* G, const igmc_candidates_t* Cd, int64_t* cursor, int B,
                          int32_t* links_u, int32_t* links_v, int64_t* pair_id, int64_t* tag, int* err, void* stream);
 
+/* Item-side runs (recommend_users: per query item its best candidate users) run the three candidate kernels above on the
+ * transposed view of G: an igmc_csr_t with row_ptr = G.col_ptr, col_idx = G.row_idx, col_ptr = G.row_ptr, row_idx =
+ * G.col_idx, num_users = G.num_items, num_items = G.num_users and rating = NULL (G's ratings are not in column order).
+ * igmc_candidate_plan, igmc_candidate_lists and igmc_candidate_pairs read only row_ptr, col_idx, num_users and
+ * num_items of the igmc_csr_t they are given and never read rating, so they take such a view as it is: the query slots
+ * are items, the candidates users and a slot's rated entries its raters.  Their pairs come out as (item, user);
+ * igmc_item_query_pairs, run after igmc_candidate_pairs on the same batch, swaps links_u / links_v back to (user, item)
+ * and rewrites pair_id = u * num_items + v (int64; num_items = G's), the pair id predict_pairs samples the pair with.
+ * tag is left as it is; the tail (tag -1, the last pair repeated) is swapped like every other slot.  An item id outside
+ * [0, num_items) or a negative user id sets IGMC_ERR_CANDIDATES (the pair becomes (0, 0)). */
+int igmc_item_query_pairs(int num_items, int B, int32_t* links_u, int32_t* links_v, int64_t* pair_id, int* err,
+                          void* stream);
+
 /* Streaming top-k: s = (preds[0][i] + ... + preds[K-1][i]) / K in fp32, summed in checkpoint order (preds row stride B),
  * then every contiguous run of equal tag (one query user's candidates in this batch; tag -1 = padding) is merged into
  * that user's running list top_score / top_item [*, k] (ranked: score descending, then item ascending; NaN after every
@@ -616,6 +629,19 @@ int igmc_influence_topk(const float* S, int B, int T, const int64_t* tag, int k,
 int igmc_corated_ws_bytes(int num_users, int num_items, int num_query, int m, int64_t* bytes);
 int igmc_corated_items(const igmc_csr_t* G, const int32_t* users, int num_query, int m, int exclude_rated, void* ws,
                        int64_t ws_bytes, int32_t* items, int32_t* paths, int* err, void* stream);
+
+/* The item side of the same count: per query item v the m users u with the largest
+ *   C[u][v] = (B B^T B)[u][v] - deg(u) * B[u][v]      (B the 0/1 rating matrix)
+ * which is exactly the paths[v] igmc_corated_items gives user u.  `T` is the transposed view of G (see
+ * igmc_item_query_pairs; rating is not read).  One CTA per item: pass 1 pushes w[i] += 1 for every rater u' of v and
+ * every item i of u' (i = v included: w[v] = deg(v)), pass 2 pulls paths[u] = sum over i in row(u) of w[i], minus
+ * deg(u) when row(u) holds v; then igmc_corated_items' select and sort.  users [num_query, m] / paths [num_query, m]
+ * int32: paths descending, then user ascending; users without a bridge are never returned, the rest of a row is user -1
+ * / paths 0; exclude_rated drops the item's raters.  Workspace igmc_corated_ws_bytes(G->num_items, G->num_users,
+ * num_query, m) (T's shape).  Integer arithmetic, one writer per output: bit-identical across runs.  Item ids outside G
+ * set IGMC_ERR_CANDIDATES (their row is padding).  1 <= m <= G->num_users. */
+int igmc_corated_users(const igmc_csr_t* T, const int32_t* items, int num_query, int m, int exclude_rated, void* ws,
+                       int64_t ws_bytes, int32_t* users, int32_t* paths, int* err, void* stream);
 
 /* ---- in-place update of the rating graph (csrc/graph_update.cu) ----
  * The reference can only change its rating matrix by rebuilding everything from a new scipy matrix.  Here a delta of D
