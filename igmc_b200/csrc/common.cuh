@@ -118,6 +118,19 @@ __device__ __forceinline__ int block_scan_chunks(int n, int* ws, In in, Out out)
   return running;
 }
 
+// Sum of one float per thread of a 256-thread block in a fixed order; `red` is 8 floats of shared scratch.  Starts
+// with a barrier, so consecutive calls may share red; it does not end with one.
+__device__ __forceinline__ float block_sum_f256(float v, float* red) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  v = warp_sum_f(v);
+  __syncthreads();
+  if (lane == 0) red[warp] = v;
+  __syncthreads();
+  float s = 0.f;
+  for (int w = 0; w < 8; ++w) s += red[w];
+  return s;
+}
+
 __device__ __forceinline__ int block_sum_i(int v, int* ws) {
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
   v = warp_sum_i(v);

@@ -13,9 +13,8 @@
 // tiles: runs are bit-identical across batch sizes, graph replay and repetitions.
 #include <cmath>
 
-#include "common.cuh"
+#include "lists.cuh"
 #include "topk_merge.cuh"
-#include "../../include/igmc_b200.h"
 
 namespace {
 
@@ -136,17 +135,11 @@ k_pair_readout(igmc_model_t M, const float* __restrict__ dhid, const float* __re
   if (out) {
     const int p = PC + q;
     if (p < M.param_count) {
-      float s = 0.f;
-      if (p >= M.off_lin1_w && p < M.off_lin1_w + L1O * F) {
-        const int r = p - M.off_lin1_w, oo = r / F, i = r - oo * F;
-        s = dhid[(size_t)g * L1O + oo] * feat[(size_t)g * F + i];
-      } else if (p >= M.off_lin1_b && p < M.off_lin1_b + L1O) {
-        s = dhid[(size_t)g * L1O + p - M.off_lin1_b];
-      } else if (p >= M.off_lin2_w && p < M.off_lin2_w + L1O) {
-        s = dpred[g] * hid[(size_t)g * L1O + p - M.off_lin2_w];
-      } else if (p == M.off_lin2_b) {
-        s = dpred[g];
-      }
+      float s = 0.f;   // graph g's term alone (a product, not an fmaf onto +0: a -0 term stays -0)
+      readout_param_grad(
+          M, p, F, dhid, feat, hid, dpred,
+          [&](const float* x, int sx, const float* y, int sy) { s = x[(size_t)g * sx] * y[(size_t)g * sy]; },
+          [&](const float* x, int sx) { s = x[(size_t)g * sx]; });
       out[(size_t)row * ld + p] = real ? s : 0.f;
     }
   }
@@ -159,17 +152,6 @@ k_pair_readout(igmc_model_t M, const float* __restrict__ dhid, const float* __re
     else v = dpred[g];
     fac[(size_t)row * FW + q] = real ? v : 0.f;
   }
-}
-
-__device__ __forceinline__ float block_sum_256(float v, float* red) {   // fixed order; ends with a barrier
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  v = warp_sum_f(v);
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  float s = 0.f;
-  for (int w = 0; w < 8; ++w) s += red[w];
-  __syncthreads();
-  return s;
 }
 
 // the readout's share of <G_a, G_b> from two factor rows (lin1: rank-1 dhid (x) feat, plus its bias; lin2: dpred hid,
@@ -206,7 +188,7 @@ k_self_influence(int PC, int L, const float* __restrict__ conv, const float* __r
     const float ro = readout_dot(f, f, 2 * HID * L, threadIdx.x);
     if (threadIdx.x == 0) s_ro = ro;
   }
-  const float c = block_sum_256(s, red);
+  const float c = block_sum_f256(s, red);
   if (threadIdx.x == 0) self_out[t] = fmaf(eta, c + s_ro, self_out[t]);
 }
 

@@ -1,8 +1,11 @@
 // Device pieces shared by the model kernels: csrc/rgcn.cu (plan 0), csrc/rgcn_l2.cu (L2 plan), csrc/rgcn_rs.cu
-// (relation-space / cluster plans) and csrc/sortpool.cu (DGCNN_RS readout).
+// (relation-space / cluster plans) and csrc/sortpool.cu (DGCNN_RS readout), and by the gradient kernels.
 //   - the step's dropout draws: edge dropout (EdgeKeep) and the hidden dropout before lin2 (hidden_scale)
 //   - a warp-wide walk over one node's (type, neighbour)-sorted list and the type-run segment reduce on it
-//   - the readout head: lin1 / ReLU / dropout / save, lin2 / loss, and their backward (d hid, d feat)
+//   - the readout head: lin1 / ReLU / dropout / save, lin2 / loss, their backward (d hid, d feat) and the lin1 / lin2
+//     parameter gradients from the saved factors (csrc/optim.cu, csrc/influence.cu too)
+//   - W_r from att and basis, the adjacent-rating regulariser's d W_r, and the per-step weight preparation (the wprep
+//     slab layout) of the cluster plans (csrc/optim.cu too)
 //   - the basis-space weight staging and weight-gradient row store of plan 0 and the L2 plan
 // Each is one computation in one place: a kernel that calls it computes bit-for-bit what the others do.
 #pragma once
@@ -234,6 +237,136 @@ __device__ __forceinline__ void readout_dfeat_part(const Model& M, const float* 
 #pragma unroll 32   // independent L2 loads in flight (latency bound)
     for (int o = part; o < IGMC_LIN1_OUT; o += parts) s = fmaf(__ldg(W1 + (size_t)o * F + i), dhid_s[o], s);
     out[part * F + i] = s;
+  }
+}
+
+// The gradient of readout parameter p as a function of the saved factors of the graphs (dhid [g][128], feat [g][F],
+// hid [g][128], dpred [g]):
+//   lin1.weight[o][i]: sum_g dhid[g][o] feat[g][i]      lin1.bias[o]: sum_g dhid[g][o]
+//   lin2.weight[o]:    sum_g dpred[g] hid[g][o]         lin2.bias:    sum_g dpred[g]
+// Calls prod(x, sx, y, sy) for a product term x[g * sx] * y[g * sy] or one(x, sx) for a single factor x[g * sx], and
+// returns false (calling neither) when p is not a lin1 / lin2 entry.
+template <class Model, class Prod, class One>
+__device__ __forceinline__ bool readout_param_grad(const Model& M, int p, int F, const float* dhid, const float* feat,
+                                                   const float* hid, const float* dpred, Prod&& prod, One&& one) {
+  constexpr int L1O = IGMC_LIN1_OUT;
+  if (p >= M.off_lin1_w && p < M.off_lin1_w + L1O * F) {
+    const int q = p - M.off_lin1_w, o = q / F, i = q - o * F;
+    prod(dhid + o, L1O, feat + i, F);
+  } else if (p >= M.off_lin1_b && p < M.off_lin1_b + L1O) {
+    one(dhid + (p - M.off_lin1_b), L1O);
+  } else if (p >= M.off_lin2_w && p < M.off_lin2_w + L1O) {
+    prod(dpred, 1, hid + (p - M.off_lin2_w), L1O);
+  } else if (p == M.off_lin2_b) {
+    one(dpred, 1);
+  } else {
+    return false;
+  }
+  return true;
+}
+
+// readout_param_grad summed over the batch's B graphs in ascending g into s (which starts at +0)
+template <class Model>
+__device__ __forceinline__ bool readout_param_grad_sum(const Model& M, int p, int F, int B, const float* dhid,
+                                                       const float* feat, const float* hid, const float* dpred,
+                                                       float& s) {
+  return readout_param_grad(
+      M, p, F, dhid, feat, hid, dpred,
+      [&](const float* x, int sx, const float* y, int sy) {
+#pragma unroll 25   // 50 independent L2 loads in flight (latency bound)
+        for (int g = 0; g < B; ++g) s = fmaf(x[(size_t)g * sx], y[(size_t)g * sy], s);
+      },
+      [&](const float* x, int sx) {
+#pragma unroll 25
+        for (int g = 0; g < B; ++g) s += x[(size_t)g * sx];
+      });
+}
+
+// ---- per-step weight preparation (csrc/rgcn_rs.cu consumes it) ---------------------------------------------------
+// W_r[k][j] = sum_b att[r,b] basis[b][k][j] as one fmaf chain over ascending b; att(b) and basis(b) read the two
+// factors of term b, all of them before the first fmaf
+template <class Att, class Basis>
+__device__ __forceinline__ float compose_w(int NB, Att&& att, Basis&& basis) {
+  float av[IGMC_MAX_BASES], bv[IGMC_MAX_BASES];
+#pragma unroll
+  for (int b = 0; b < IGMC_MAX_BASES; ++b) {
+    av[b] = b < NB ? att(b) : 0.f;
+    bv[b] = b < NB ? basis(b) : 0.f;
+  }
+  float w = 0.f;
+#pragma unroll
+  for (int b = 0; b < IGMC_MAX_BASES; ++b)
+    if (b < NB) w = fmaf(av[b], bv[b], w);
+  return w;
+}
+
+// d reg / d W_r at one entry of the adjacent-rating regulariser reg = sum_{r<R-1} ||W_{r+1} - W_r||^2:
+// 2 (W_r - W_{r-1}) [r > 0] - 2 (W_{r+1} - W_r) [r < R-1], W(r) giving the entry of W_r.  `pair` (optional) receives
+// (W_{r+1} - W_r)^2, the entry's share of the pair (r, r+1) (+0 for r = R-1).
+template <class W>
+__device__ __forceinline__ float arr_dw(W&& w, int R, int r, float* pair) {
+  const float w0 = w(r);
+  float dw = 0.f, d = 0.f;
+  if (r > 0) dw += 2.f * (w0 - w(r - 1));
+  if (r < R - 1) {
+    d = w(r + 1) - w0;
+    dw -= 2.f * d;
+  }
+  if (pair) *pair = d * d;
+  return dw;
+}
+
+// Prepared weights: slab(l, dir) = Bn[n][KS] (n = output channel, 32 rows):
+//   dir 0 (forward, B of  [AGG | h] . [W_r ; root]):   Bn[n][r*inp+k] = W_r[k][n],  Bn[n][K1p+k] = root[k][n]
+//   dir 1 (backward, B of [Q | dpre] . [W_r^T ; root^T], layers >= 1):  Bn[k][r*32+j] = W_r[k][j],  Bn[k][R*32+j] = root[k][j]
+// Rows are n-major / K-contiguous so the mma B fragments load conflict-free.  Row geometry of a layer whose input width
+// rounded up to 4 is inp: the relation columns [0, K1 = R * inp) padded to K1p, the root columns [K1p, K1p + inp) padded
+// to inpp, 4 more floats: KS per row.
+__host__ __device__ __forceinline__ int a8(int x) { return (x + 7) & ~7; }
+struct WprepRow {
+  int K1, K1p, inpp;
+  __host__ __device__ __forceinline__ int KS() const { return K1p + inpp + 4; }
+};
+__host__ __device__ __forceinline__ WprepRow wprep_row(int R, int inp) {
+  WprepRow g;
+  g.K1 = R * inp;
+  g.K1p = a8(g.K1);
+  g.inpp = a8(inp);
+  return g;
+}
+// floats of one slab: 32 rows of a 32-wide layer's KS = (R + 1) * 32 + 4 (the widest; a slab of layer 0 uses a
+// prefix).  Twin: igmc_b200/models.py IGMC._wprep_buf.
+__host__ __device__ __forceinline__ size_t wprep_slab(int R) {
+  return (size_t)IGMC_HIDDEN * ((size_t)(R + 1) * IGMC_HIDDEN + 4);
+}
+
+// Row n of slab (l, dir) from the parameters, a 256-thread block striding over its KS floats.  params are read through
+// L2 (__ldcg): the update kernel calls this on parameters other blocks of the same launch have just written.
+__device__ __forceinline__ void wprep_write_row(const igmc_model_t& M, const float* params, float* wprep, int l,
+                                                int dir, int n) {
+  constexpr int HID = IGMC_HIDDEN;
+  const int R = M.num_relations, NB = M.num_bases;
+  const int in = l == 0 ? M.in_dim0 : HID, inp = a4(in);
+  const WprepRow G = wprep_row(R, inp);
+  const float* bs = params + M.off_basis[l];
+  const float* at = params + M.off_att[l];
+  const float* rt = params + M.off_root[l];
+  float* out = wprep + ((size_t)l * 2 + dir) * wprep_slab(R) + (size_t)n * G.KS();
+  for (int kk = threadIdx.x; kk < G.KS(); kk += 256) {
+    float w = 0.f;
+    if (kk < G.K1) {
+      const int r = kk / inp, q = kk - r * inp;
+      if (q < in) {
+        // dir 0: W_r[k=q][n] ; dir 1: W_r[k=n][j=q]
+        const int k = dir == 0 ? q : n, j = dir == 0 ? n : q;
+        w = compose_w(NB, [&](int b) { return __ldcg(at + r * NB + b); },
+                      [&](int b) { return __ldcg(bs + (b * in + k) * HID + j); });
+      }
+    } else if (kk >= G.K1p && kk < G.K1p + inp) {
+      const int q = kk - G.K1p;
+      if (q < in) w = dir == 0 ? __ldcg(rt + q * HID + n) : __ldcg(rt + n * HID + q);
+    }
+    out[kk] = w;
   }
 }
 

@@ -7,42 +7,20 @@
 #include <cstdlib>
 #include <cstring>
 
-#include "common.cuh"
-#include "../../include/igmc_b200.h"
+#include "lists.cuh"
 
 namespace {
 
 constexpr int HID = IGMC_HIDDEN;
-constexpr int L1O = IGMC_LIN1_OUT;
 
-// dW_r[kj] of the adjacent-rating regulariser for one (layer, kj):  reg = sum_{r<R-1} ||W_{r+1}-W_r||^2,
-// W_r = sum_b att[r,b] basis[b];  d reg / d W_r = 2 (W_r - W_{r-1}) [r>0] - 2 (W_{r+1} - W_r) [r<R-1].
-// `pair` (optional) receives (W_{r+1}[kj]-W_r[kj])^2, the contribution of the pair (r, r+1) to reg.
-__device__ __forceinline__ float arr_dw(const float* __restrict__ att, const float* __restrict__ bs, int NB, int KJ,
-                                        int R, int r, int kj, float* pair) {
-  float wm = 0.f, w0 = 0.f, wp = 0.f;
-  for (int b = 0; b < NB; ++b) {
-    const float bv = bs[b * KJ + kj];
-    w0 = fmaf(att[r * NB + b], bv, w0);
-    if (r > 0) wm = fmaf(att[(r - 1) * NB + b], bv, wm);
-    if (r < R - 1) wp = fmaf(att[(r + 1) * NB + b], bv, wp);
-  }
-  float dw = 0.f;
-  if (r > 0) dw += 2.f * (w0 - wm);
-  if (r < R - 1) dw -= 2.f * (wp - w0);
-  if (pair) *pair = r < R - 1 ? (wp - w0) * (wp - w0) : 0.f;
-  return dw;
-}
-
-__device__ __forceinline__ float block_sum_f256(float v, float* red) {   // 256-thread block, fixed order
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  v = warp_sum_f(v);
-  __syncthreads();
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  float s = 0.f;
-  for (int w = 0; w < 8; ++w) s += red[w];
-  return s;
+// dW_r[kj] of the adjacent-rating regulariser for one (layer, kj), W_r composed from att and the basis bs (stride KJ
+// between bases)
+__device__ __forceinline__ float arr_dw_kj(const float* __restrict__ att, const float* __restrict__ bs, int NB, int KJ,
+                                           int R, int r, int kj, float* pair) {
+  const auto w = [&](int rr) {
+    return compose_w(NB, [&](int b) { return att[rr * NB + b]; }, [&](int b) { return bs[b * KJ + kj]; });
+  };
+  return arr_dw(w, R, r, pair);
 }
 
 // Blocks [0, PB): one thread per parameter.
@@ -75,7 +53,7 @@ k_grad_reduce(igmc_model_t M, const float* __restrict__ params, int B, int rows,
               const float* att = params + M.off_att[l];
               float t = 0.f;
               for (int r = 0; r < R; ++r)
-                t = fmaf(att[r * NB + b], arr_dw(att, params + M.off_basis[l], NB, KJ, R, r, kj, nullptr), t);
+                t = fmaf(att[r * NB + b], arr_dw_kj(att, params + M.off_basis[l], NB, KJ, R, r, kj, nullptr), t);
               s = fmaf(arr, t, s);
             }
             const int qa = p - M.off_att[l];
@@ -84,17 +62,8 @@ k_grad_reduce(igmc_model_t M, const float* __restrict__ params, int B, int rows,
         }
       } else if (M.readout != 0) {
         skip = true;   // readout parameters belong to the external readout's gradient kernel
-      } else if (p >= M.off_lin1_w && p < M.off_lin1_w + L1O * F) {
-        const int q = p - M.off_lin1_w, o = q / F, i = q - o * F;      // lin1.weight[o][i]
-        for (int g = 0; g < B; ++g) s = fmaf(dhid[(size_t)g * L1O + o], feat[(size_t)g * F + i], s);
-      } else if (p >= M.off_lin1_b && p < M.off_lin1_b + L1O) {
-        const int o = p - M.off_lin1_b;
-        for (int g = 0; g < B; ++g) s += dhid[(size_t)g * L1O + o];
-      } else if (p >= M.off_lin2_w && p < M.off_lin2_w + L1O) {
-        const int o = p - M.off_lin2_w;
-        for (int g = 0; g < B; ++g) s = fmaf(dpred[g], hid[(size_t)g * L1O + o], s);
-      } else if (p == M.off_lin2_b) {
-        for (int g = 0; g < B; ++g) s += dpred[g];
+      } else {
+        readout_param_grad_sum(M, p, F, B, dhid, feat, hid, dpred, s);
       }
       if (!skip) grad[p] = s * grad_scale;
     }
@@ -122,7 +91,7 @@ k_grad_reduce(igmc_model_t M, const float* __restrict__ params, int B, int rows,
   float pair_sum = 0.f;
   for (int kj = tid; kj < KJ; kj += 256) {
     float pr;
-    dw[kj] = arr_dw(att, bs, NB, KJ, R, r, kj, &pr);
+    dw[kj] = arr_dw_kj(att, bs, NB, KJ, R, r, kj, &pr);
     pair_sum += pr;
   }
   __syncthreads();
@@ -236,27 +205,7 @@ __device__ __forceinline__ void reduce_raw_block(const igmc_model_t& M, const fl
     const int p = M.conv_param_count + ((int)blockIdx.x - NA) * 256 + tid;
     if (p >= M.param_count) return;
     float s = 0.f;
-    bool write = false;
-    if (p >= M.off_lin1_w && p < M.off_lin1_w + L1O * F) {
-      const int q = p - M.off_lin1_w, o = q / F, i = q - o * F;      // lin1.weight[o][i]
-#pragma unroll 25   // 50 independent L2 loads in flight (latency bound)
-      for (int g = 0; g < B; ++g) s = fmaf(dhid[(size_t)g * L1O + o], feat[(size_t)g * F + i], s);
-      write = true;
-    } else if (p >= M.off_lin1_b && p < M.off_lin1_b + L1O) {
-      const int o = p - M.off_lin1_b;
-#pragma unroll 25
-      for (int g = 0; g < B; ++g) s += dhid[(size_t)g * L1O + o];
-      write = true;
-    } else if (p >= M.off_lin2_w && p < M.off_lin2_w + L1O) {
-      const int o = p - M.off_lin2_w;
-#pragma unroll 25
-      for (int g = 0; g < B; ++g) s = fmaf(dpred[g], hid[(size_t)g * L1O + o], s);
-      write = true;
-    } else if (p == M.off_lin2_b) {
-      for (int g = 0; g < B; ++g) s += dpred[g];
-      write = true;
-    }
-    if (write) grad[p] = s * grad_scale;
+    if (readout_param_grad_sum(M, p, F, B, dhid, feat, hid, dpred, s)) grad[p] = s * grad_scale;
     return;
   }
   // ---- block (l, k): row k of dW_0..dW_{R-1} and of d root; block (l, 0) also d bias ----
@@ -293,9 +242,7 @@ __device__ __forceinline__ void reduce_raw_block(const igmc_model_t& M, const fl
     for (int w = 0; w < 8; ++w) s += ps[c][w][j];
     if (c < R) {
       dWs[c][j] = s;
-      float wv = 0.f;
-      for (int b = 0; b < NB; ++b) wv = fmaf(att[c * NB + b], bs[b][j], wv);
-      Wc[c][j] = wv;
+      Wc[c][j] = compose_w(NB, [&](int b) { return att[c * NB + b]; }, [&](int b) { return bs[b][j]; });
     } else if (c == R) {
       grad[M.off_root[l] + k * HID + j] = s * grad_scale;
     } else {
@@ -307,14 +254,9 @@ __device__ __forceinline__ void reduce_raw_block(const igmc_model_t& M, const fl
   if (arr != 0.f) {
     for (int t = tid; t < R * HID; t += 256) {
       const int r = t >> 5, j = t & 31;
-      const float w0 = Wc[r][j];
-      float dw = 0.f;
-      if (r > 0) dw += 2.f * (w0 - Wc[r - 1][j]);
-      if (r < R - 1) {
-        const float dd = Wc[r + 1][j] - w0;
-        dw -= 2.f * dd;
-        pair_sum += dd * dd;
-      }
+      float pr;
+      const float dw = arr_dw([&](int rr) { return Wc[rr][j]; }, R, r, &pr);
+      pair_sum += pr;
       dWs[r][j] = fmaf(arr, dw, dWs[r][j]);
     }
   }
@@ -410,6 +352,26 @@ k_grad_reduce_raw(igmc_model_t M, const float* __restrict__ params, int B, int r
                          loss_out, reg_ws);
 }
 
+// ---- torch.optim.Adam (torch 1.4 semantics) --------------------------------------------------------------------
+// bias correction 1 - beta^step, in double from log beta (computed on the host)
+__device__ __forceinline__ float adam_bias_correction(int64_t step, double log_beta) {
+  return (float)(1.0 - exp((double)step * log_beta));
+}
+
+// one element: gradient g (already scaled), weight decay, moments m / v, parameter p
+__device__ __forceinline__ void adam_update(float* __restrict__ params, float* __restrict__ m, float* __restrict__ v,
+                                            int i, float g, float lr, float b1, float b2, float bc1, float bc2,
+                                            float eps, float wd) {
+  const float p = params[i];
+  if (wd != 0.f) g = fmaf(wd, p, g);
+  const float mi = b1 * m[i] + (1.f - b1) * g;
+  const float vi = b2 * v[i] + (1.f - b2) * g * g;
+  m[i] = mi;
+  v[i] = vi;
+  const float denom = sqrtf(vi) / sqrtf(bc2) + eps;
+  params[i] = p - (lr / bc1) * (mi / denom);
+}
+
 // ---- system-scope flags for the peer exchange ----------------------------------------------------------------
 __device__ __forceinline__ void st_release_sys(int* p, int v) {
   asm volatile("st.release.sys.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
@@ -463,10 +425,8 @@ k_reduce_allreduce_adam(igmc_model_t M, float* __restrict__ params, int B, int r
   const int t = (int)t64;
   const int64_t step_i = step_count[0] + 1;
   __shared__ float s_bc[2];
-  if (tid >= 254) {   // bias corrections 1 - beta^step (double, off the critical path: before the gradient assembly)
-    const double step = (double)step_i;
-    s_bc[tid - 254] = (float)(1.0 - exp(step * (tid == 255 ? log_b2 : log_b1)));
-  }
+  if (tid >= 254)   // bias corrections (off the critical path: before the gradient assembly)
+    s_bc[tid - 254] = adam_bias_correction(step_i, tid == 255 ? log_b2 : log_b1);
   float* gl = C.grad[C.rank] + (size_t)(t & 1) * C.stride;
   reduce_raw_block<false>(M, params, B, rows, NA, gpart, dhid, feat, hid, dpred, sqerr, loss_scale, arr, 1.0f, gl,
                           loss_out, reg_ws);
@@ -507,15 +467,7 @@ k_reduce_allreduce_adam(igmc_model_t M, float* __restrict__ params, int B, int r
 #pragma unroll
     for (int r = 0; r < IGMC_MAX_RANKS; ++r) g += gv[r];   // rank order; absent ranks add +0
     if (grad_copy) grad_copy[i] = g;
-    g *= grad_mul;
-    const float p = params[i];
-    if (wd != 0.f) g = fmaf(wd, p, g);
-    const float mi = b1 * exp_avg[i] + (1.f - b1) * g;
-    const float vi = b2 * exp_avg_sq[i] + (1.f - b2) * g * g;
-    exp_avg[i] = mi;
-    exp_avg_sq[i] = vi;
-    const float denom = sqrtf(vi) / sqrtf(bc2) + eps;
-    params[i] = p - (lr / bc1) * (mi / denom);
+    adam_update(params, exp_avg, exp_avg_sq, i, g * grad_mul, lr, b1, b2, bc1, bc2, eps, wd);
   }
   if (blockIdx.x == 0 && tid < 32 && loss_out) {
     // the step's loss, off the critical path (every layer's regulariser value is complete behind the grid barrier)
@@ -545,44 +497,12 @@ k_reduce_allreduce_adam(igmc_model_t M, float* __restrict__ params, int B, int r
   }
   if (!wprep) return;
   __syncthreads();
-  // ---- phase 4: W_r = sum_b att[r,b] basis[b] and its transpose for the NEXT step's kernels (what
-  //      igmc_prep_weights launches; same layout: slab(l, dir) = 32 rows of KS floats) ----
-  {
-    const int R = M.num_relations, NB = M.num_bases;
-    const size_t slab = (size_t)HID * ((size_t)(R + 1) * HID + 4);
-    // rows of slab (0, 1) do not exist (layer 0 has no data gradient): active row a -> row a (a < 32) / a + 32
-    for (int a = blockIdx.x; a < (M.num_layers * 2 - 1) * 32; a += gridDim.x) {
-      const int row = a < 32 ? a : a + 32;
-      const int n = row & 31, ld = row >> 5, l = ld >> 1, dir = ld & 1;
-      const int in = l == 0 ? M.in_dim0 : HID, inp = (in + 3) & ~3;
-      const int K1 = R * inp, K1p = (K1 + 7) & ~7, inpp = (inp + 7) & ~7, KS = K1p + inpp + 4;
-      const float* bs = params + M.off_basis[l];
-      const float* at = params + M.off_att[l];
-      const float* rt = params + M.off_root[l];
-      float* out = wprep + ((size_t)l * 2 + dir) * slab + (size_t)n * KS;
-      for (int kk = tid; kk < KS; kk += 256) {
-        float w = 0.f;
-        if (kk < K1) {
-          const int r = kk / inp, q = kk - r * inp;
-          if (q < in) {
-            const int k = dir == 0 ? q : n, j = dir == 0 ? n : q;
-            float av[IGMC_MAX_BASES], bv[IGMC_MAX_BASES];
-#pragma unroll
-            for (int b = 0; b < IGMC_MAX_BASES; ++b) {   // all loads in flight before the first fma
-              av[b] = b < NB ? __ldcg(at + r * NB + b) : 0.f;
-              bv[b] = b < NB ? __ldcg(bs + (b * in + k) * HID + j) : 0.f;
-            }
-#pragma unroll
-            for (int b = 0; b < IGMC_MAX_BASES; ++b)
-              if (b < NB) w = fmaf(av[b], bv[b], w);
-          }
-        } else if (kk >= K1p && kk < K1p + inp) {
-          const int q = kk - K1p;
-          if (q < in) w = dir == 0 ? __ldcg(rt + q * HID + n) : __ldcg(rt + n * HID + q);
-        }
-        out[kk] = w;
-      }
-    }
+  // ---- phase 4: the prepared weights of the NEXT step's kernels (what igmc_prep_weights launches).  Rows of slab
+  //      (0, 1) do not exist (layer 0 has no data gradient): active row a -> row a (a < 32) / a + 32 ----
+  for (int a = blockIdx.x; a < (M.num_layers * 2 - 1) * 32; a += gridDim.x) {
+    const int row = a < 32 ? a : a + 32;
+    const int ld = row >> 5;
+    wprep_write_row(M, params, wprep, ld >> 1, ld & 1, row & 31);
   }
 }
 
@@ -596,24 +516,11 @@ __global__ void k_adam(float* __restrict__ params, const float* __restrict__ gra
   if (i == 0 && loss_acc) loss_acc[0] += loss_in[0] * loss_weight;   // epoch loss bookkeeping (train_eval.py:176)
   const int64_t step_i = step_count[0] + 1;
   __shared__ float s_bc[2];
-  if (threadIdx.x < 2) {   // bias corrections 1 - beta^step in double, once per block (log beta comes from the host)
-    const double step = (double)step_i;
-    s_bc[threadIdx.x] = (float)(1.0 - exp(step * (threadIdx.x ? log_b2 : log_b1)));
-  }
+  if (threadIdx.x < 2)   // bias corrections, once per block
+    s_bc[threadIdx.x] = adam_bias_correction(step_i, threadIdx.x ? log_b2 : log_b1);
   __syncthreads();
-  if (i < n) {
-    const float lr = lr_dev ? *lr_dev : lr_val;
-    const float bc1 = s_bc[0], bc2 = s_bc[1];
-    float g = grad[i] * grad_mul;
-    const float p = params[i];
-    if (wd != 0.f) g = fmaf(wd, p, g);
-    const float mi = b1 * m[i] + (1.f - b1) * g;
-    const float vi = b2 * v[i] + (1.f - b2) * g * g;
-    m[i] = mi;
-    v[i] = vi;
-    const float denom = sqrtf(vi) / sqrtf(bc2) + eps;
-    params[i] = p - (lr / bc1) * (mi / denom);
-  }
+  if (i < n)
+    adam_update(params, m, v, i, grad[i] * grad_mul, lr_dev ? *lr_dev : lr_val, b1, b2, s_bc[0], s_bc[1], eps, wd);
   __syncthreads();   // every thread of the block has read step_count
   if (threadIdx.x == 0) {
     __threadfence();

@@ -533,7 +533,6 @@ __device__ __forceinline__ void tiles_span2(TileAcc (&T)[2], uint32_t a, int xs,
   }
 }
 
-__host__ __device__ __forceinline__ int a8(int x) { return (x + 7) & ~7; }
 __host__ __device__ __forceinline__ int a16(int x) { return (x + 15) & ~15; }
 
 struct Split { int lo, hi; };
@@ -551,41 +550,13 @@ __host__ __device__ __forceinline__ int own_cap_of(int n_cap, int CL) { return (
 #define IGMC_WALL(i_) do { if (S.prof && threadIdx.x == 0) { S.prof[(size_t)blockIdx.x * 64 + (i_)] = igmc_globaltimer(); \
                                                               S.prof[(size_t)blockIdx.x * 64 + ((i_) < 53 ? 52 : 55)] = igmc_smid(); } } while (0)
 
-// ------------------------------------------------------------------------------------------------
-// per-step weight preparation.  slab(l, dir) = Bn[n][KS]  (n = output channel, KS = Ktot + 4):
-//   dir 0 (forward, B of  [AGG | h] . [W_r ; root]):   Bn[n][r*inp+k] = W_r[k][n],  Bn[n][K1p+k] = root[k][n]
-//   dir 1 (backward, B of [Q | dpre] . [W_r^T ; root^T], layers >= 1):  Bn[k][r*32+j] = W_r[k][j],  Bn[k][R*32+j] = root[k][j]
-// W_r = sum_b att[r,b] basis[b];  rows are n-major / K-contiguous so the mma B fragments load conflict-free.
-// ------------------------------------------------------------------------------------------------
-__host__ __device__ __forceinline__ size_t wprep_slab(int R) { return (size_t)HID * ((size_t)(R + 1) * HID + 4); }
-
-// grid = L * 2 * 32 blocks: block (l, dir, n) writes row n of slab (l, dir); one thread per K position.
+// per-step weight preparation (layout: wprep_slab in csrc/lists.cuh).  grid = L * 2 * 32 blocks: block (l, dir, n)
+// writes row n of slab (l, dir); one thread per K position.
 __global__ void __launch_bounds__(256)
 k_prep_weights(igmc_model_t M, const float* __restrict__ params, float* __restrict__ wprep) {
   const int n = blockIdx.x & 31, ld = blockIdx.x >> 5, l = ld >> 1, dir = ld & 1;
-  const int R = M.num_relations, NB = M.num_bases;
-  const int in = l == 0 ? M.in_dim0 : HID, inp = a4(in);
-  const int K1 = R * inp, K1p = a8(K1), inpp = a8(inp), KS = K1p + inpp + 4;
   if (dir == 1 && l == 0) return;
-  const float* bs = params + M.off_basis[l];
-  const float* at = params + M.off_att[l];
-  const float* rt = params + M.off_root[l];
-  float* out = wprep + ((size_t)l * 2 + dir) * wprep_slab(R) + (size_t)n * KS;
-  for (int kk = threadIdx.x; kk < KS; kk += 256) {
-    float w = 0.f;
-    if (kk < K1) {
-      const int r = kk / inp, q = kk - r * inp;
-      if (q < in) {
-        // dir 0: W_r[k=q][n] ; dir 1: W_r[k=n][j=q]
-        const int k = dir == 0 ? q : n, j = dir == 0 ? n : q;
-        for (int b = 0; b < NB; ++b) w = fmaf(__ldg(at + r * NB + b), __ldg(bs + (b * in + k) * HID + j), w);
-      }
-    } else if (kk >= K1p && kk < K1p + inp) {
-      const int q = kk - K1p;
-      if (q < in) w = dir == 0 ? __ldg(rt + q * HID + n) : __ldg(rt + n * HID + q);
-    }
-    out[kk] = w;
-  }
+  wprep_write_row(M, params, wprep, l, dir, n);
 }
 
 __device__ __forceinline__ void copy_f4(float* __restrict__ dst, const float* __restrict__ src, int nfloats) {
@@ -686,8 +657,7 @@ __device__ __forceinline__ bool forward_body(const igmc_model_t& M, const float*
   // thread; every thread waits on mbar[1] (phase = layer parity) right before the layer's tensor-core tiles, so the
   // copy runs under the gather.  Callers guarantee (barrier) that nobody still reads Wn.
   auto load_weights = [&](int l) {
-    const int inp = l == 0 ? in0p : HID;
-    const int KS = a8(R * inp) + a8(inp) + 4;
+    const int KS = wprep_row(R, l == 0 ? in0p : HID).KS();
     if (tid == 0) {
       fence_proxy_async();
       mbar_expect_tx(&mbar[1], (uint32_t)(HID * KS * 4));
@@ -768,7 +738,8 @@ __device__ __forceinline__ bool forward_body(const igmc_model_t& M, const float*
   // shared memory for the backward) from there.
   for (int l = 0; l < L; ++l) {
     const int inp = l == 0 ? in0p : HID;
-    const int K1 = R * inp, K1p = a8(K1), inpp = a8(inp), SS = K1p + 4, KS = K1p + inpp + 4;
+    const WprepRow wr = wprep_row(R, inp);
+    const int K1 = wr.K1, K1p = wr.K1p, inpp = wr.inpp, SS = K1p + 4, KS = wr.KS();
     uint64_t* xbar = &mbar[2 + (l & 1)];
     if (CL > 1 && tid == 0) mbar_expect_tx(xbar, (uint32_t)(n - n_own) * 128u);
     __syncthreads();
@@ -1035,7 +1006,7 @@ __device__ __forceinline__ void backward_body(const igmc_model_t& M, const float
   // copy by one thread; waited for right before the tiles).  Callers guarantee that nobody still reads Wn.
   auto load_weights = [&](int l) {
     if (tid == 0) {
-      const uint32_t bytes = (uint32_t)(HID * ((R + 1) * HID + 4) * 4);
+      const uint32_t bytes = (uint32_t)(wprep_slab(R) * 4);
       fence_proxy_async();
       mbar_expect_tx(&mbar[1], bytes);
       bulk_g2s(Wn, S.wprep + ((size_t)l * 2 + 1) * wprep_slab(R), bytes, &mbar[1]);
@@ -1118,7 +1089,8 @@ __device__ __forceinline__ void backward_body(const igmc_model_t& M, const float
   // buffer (step (0) and the gathers).  After its layer 1 wait nothing is stored into this CTA any more.
   for (int l = L - 1; l >= 0; --l) {
     const int in = l == 0 ? in0 : HID, inp = l == 0 ? in0p : HID;
-    const int K1 = R * inp, K1p = a8(K1), inpp = a8(inp), KRp = K1p + inpp;
+    const WprepRow wr = wprep_row(R, inp);
+    const int K1 = wr.K1, K1p = wr.K1p, KRp = K1p + wr.inpp;
     const int sb = 2 + 8 * (L - 1 - l);
     float* DPS = (l & 1) ? DH1 : DH0;                    // d h_l on entry, dpre/deg after step (0)
     float* DHn = (l & 1) ? DH0 : DH1;                    // d h_{l-1} (written here and by the peers)
@@ -1150,7 +1122,7 @@ __device__ __forceinline__ void backward_body(const igmc_model_t& M, const float
     }
 
     if (l > 0) {
-      const int SS = K1p + 4, KS = KRp + 4;
+      const int SS = K1p + 4, KS = wr.KS();
       const int NTN = (R + 1) * 4;                        // 8-column tiles of [dW_r ... | d root]
       for (int c0 = 0; c0 < n_own; c0 += chunk) {
         const int crow = min(chunk, n_own - c0);
@@ -1452,15 +1424,15 @@ k_stage_lists(const int32_t* __restrict__ node_ptr, const int32_t* __restrict__ 
 }
 
 size_t fwd_base_fl(int n_cap, int R, int L, int CL) {   // everything except the stage rows and the list buffer
-  const size_t KSmax = (size_t)(R + 1) * HID + 4, F = 2 * HID * L;
+  const size_t F = 2 * HID * L;
   const size_t own_cap = (size_t)own_cap_of(n_cap, CL);
-  return 2 * (size_t)n_cap * HID + HID * KSmax + HID + a4(n_cap) + a4((int)F) + L1O + img_ints((int)own_cap) +
+  return 2 * (size_t)n_cap * HID + wprep_slab(R) + HID + a4(n_cap) + a4((int)F) + L1O + img_ints((int)own_cap) +
          (size_t)XR * ((size_t)R * HID + 4);
 }
 size_t bwd_base_fl(int n_cap, int R, int L, int CL) {   // everything except the (stage + Hs) rows and the list buffer
-  const size_t KSmax = (size_t)(R + 1) * HID + 4, F = 2 * HID * L;
+  const size_t F = 2 * HID * L;
   const size_t own_cap = (size_t)own_cap_of(n_cap, CL), own_cap16 = (size_t)a16((int)own_cap);
-  return 2 * (size_t)n_cap * HID + own_cap16 * DPS_ + HID * KSmax + a4(n_cap) + a4((int)F) + L1O +
+  return 2 * (size_t)n_cap * HID + own_cap16 * DPS_ + wprep_slab(R) + a4(n_cap) + a4((int)F) + L1O +
          img_ints((int)own_cap) + (size_t)XR * ((size_t)R * HID + 4);
 }
 

@@ -304,17 +304,8 @@ k_sortpool_grad(igmc_sortpool_t P, int B, igmc_sortpool_saved_t S, const float* 
   float s = 0.f;
   if (q >= 0) {
     for (int g = 0; g < B; ++g) s += S.gpart[(size_t)g * GP + q];
-  } else if (p >= P.off_lin1_w && p < P.off_lin1_w + L1O * P.dense_dim) {
-    const int r = p - P.off_lin1_w, o = r / P.dense_dim, i = r - o * P.dense_dim;
-    for (int g = 0; g < B; ++g) s = fmaf(S.dhid[(size_t)g * L1O + o], S.flat[(size_t)g * P.dense_dim + i], s);
-  } else if (p >= P.off_lin1_b && p < P.off_lin1_b + L1O) {
-    const int o = p - P.off_lin1_b;
-    for (int g = 0; g < B; ++g) s += S.dhid[(size_t)g * L1O + o];
-  } else if (p >= P.off_lin2_w && p < P.off_lin2_w + L1O) {
-    const int o = p - P.off_lin2_w;
-    for (int g = 0; g < B; ++g) s = fmaf(dpred[g], S.hid[(size_t)g * L1O + o], s);
-  } else if (p == P.off_lin2_b) {
-    for (int g = 0; g < B; ++g) s += dpred[g];
+  } else {
+    readout_param_grad_sum(P, p, P.dense_dim, B, S.dhid, S.flat, S.hid, dpred, s);
   }
   grad[p] = s * grad_scale;   // alignment padding between parameters gets 0
 }

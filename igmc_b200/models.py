@@ -493,6 +493,7 @@ class IGMC(nn.Module):
 
     def _wprep_buf(self):
         if self._wprep is None or self._wprep.device != self.flat_params.device:
+            # two slabs per layer of wprep_slab(R) floats each (csrc/lists.cuh)
             n = len(self.convs) * 2 * HID * ((self.num_relations + 1) * HID + 4)
             self._wprep = torch.zeros(n, dtype=torch.float32, device=self.flat_params.device)
         return self._wprep
@@ -587,14 +588,20 @@ class IGMC(nn.Module):
     def forward_backward(self, batch, global_num_graphs=None, edge_keep=None, hidden_keep=None, seed_dev=None):
         """prep + forward + loss + backward of one training step WITHOUT the gradient assembly: leaves the raw partial
         rows / readout factors in the workspace for ``FusedAdam.reduce_update`` (or ``_launch_grad_reduce``)."""
+        return self._train_launches(batch, global_num_graphs, edge_keep, hidden_keep, seed_dev, one_launch=True)[0]
+
+    def _train_launches(self, batch, global_num_graphs, edge_keep, hidden_keep, seed_dev, one_launch):
+        """the step's forward + loss + backward launches; ``one_launch`` allows igmc_forward_backward where the plan
+        has it.  Returns (saved, G)."""
         self._step += 1
         drop = self.make_dropout(True, edge_keep, hidden_keep, seed_dev=seed_dev)
         G = batch.num_graphs if global_num_graphs is None else int(global_num_graphs)
-        if self._cmodel.readout == 0 and _lib.is_rs(self._plan(batch)) and os.environ.get("IGMC_FUSED_FB", "1") != "0":
-            return self._launch_train(batch, drop, batch.y, 1.0 / G)
+        if one_launch and self._cmodel.readout == 0 and _lib.is_rs(self._plan(batch)) \
+                and os.environ.get("IGMC_FUSED_FB", "1") != "0":
+            return self._launch_train(batch, drop, batch.y, 1.0 / G), G
         out, saved = self._launch_forward(batch, True, drop, y=batch.y, loss_scale=1.0 / G)
         self._launch_backward(batch, drop, saved, saved["ws"]["dpred"])
-        return saved
+        return saved, G
 
     def _launch_train(self, batch, drop, y, loss_scale):
         """forward + loss + backward as ONE launch (igmc_forward_backward): cluster plans, IGMC readout."""
@@ -639,11 +646,7 @@ class IGMC(nn.Module):
         NCCL SUM of flat_grad is the gradient of the global-batch mean).  Returns the device scalar
         ``sum_g (out_g-y_g)^2 / global_num_graphs + ARR*reg``.
         """
-        self._step += 1
-        drop = self.make_dropout(True, edge_keep, hidden_keep, seed_dev=seed_dev)
-        G = batch.num_graphs if global_num_graphs is None else int(global_num_graphs)
-        out, saved = self._launch_forward(batch, True, drop, y=batch.y, loss_scale=1.0 / G)
-        self._launch_backward(batch, drop, saved, saved["ws"]["dpred"])
+        saved, G = self._train_launches(batch, global_num_graphs, edge_keep, hidden_keep, seed_dev, one_launch=False)
         self._launch_grad_reduce(batch, saved, loss_scale=1.0 / G, arr=ARR, with_loss=True)
         return saved["ws"]["loss"]
 

@@ -183,18 +183,23 @@ class TrainEngine(object):
                 rows = nb * ws["cluster"]
             else:   # no graph of a short tail batch on this rank: it still takes part in the exchange (zero rows)
                 ws, rows = self._last_ws, 0
-            loss = self.opt.reduce_update(self.exchange, ws, nb, rows, 1.0 / max(G, 1), self.arr_local,
-                                          lr_dev=self.lr_dev, loss_acc=self.loss_acc, loss_weight=float(G),
-                                          loss_ring=self.loss_ring_view if self.zero_copy else None)
+            self.last_loss = self.opt.reduce_update(self.exchange, ws, nb, rows, 1.0 / max(G, 1), self.arr_local,
+                                                    lr_dev=self.lr_dev, loss_acc=self.loss_acc, loss_weight=float(G),
+                                                    loss_ring=self.loss_ring_view if self.zero_copy else None)
         else:
-            if nb > 0:
-                loss = m.fused_step(batch, ARR=self.arr_local, global_num_graphs=G, seed_dev=seed_dev)
-            else:
-                m.flat_grad.zero_()
-                loss = torch.zeros(1, dtype=torch.float32, device=self.dev)
-            if self.world > 1:
-                dist.all_reduce(m.flat_grad)
-            self.opt.step(grad_mul=1.0, lr_dev=self.lr_dev, loss_in=loss, loss_acc=self.loss_acc, loss_weight=float(G))
+            self._separate_step(batch, nb, G, seed_dev)
+
+    def _separate_step(self, batch, nb, G, seed_dev=None):
+        """gradient assembly (``fused_step``) -> NCCL all-reduce -> Adam, as separate launches"""
+        m = self.model
+        if nb > 0:
+            loss = m.fused_step(batch, ARR=self.arr_local, global_num_graphs=G, seed_dev=seed_dev)
+        else:
+            m.flat_grad.zero_()
+            loss = torch.zeros(1, dtype=torch.float32, device=self.dev)
+        if self.world > 1:
+            dist.all_reduce(m.flat_grad)
+        self.opt.step(grad_mul=1.0, lr_dev=self.lr_dev, loss_in=loss, loss_acc=self.loss_acc, loss_weight=float(G))
         self.last_loss = loss
 
     def _launch(self, nb, G):
@@ -207,11 +212,7 @@ class TrainEngine(object):
 
     def _launch_static(self, idx, G):
         batch = self.dataset.extract_batch(idx)
-        loss = self.model.fused_step(batch, ARR=self.arr_local, global_num_graphs=G)
-        if self.world > 1:
-            dist.all_reduce(self.model.flat_grad)
-        self.opt.step(grad_mul=1.0, lr_dev=self.lr_dev, loss_in=loss, loss_acc=self.loss_acc, loss_weight=float(G))
-        self.last_loss = loss
+        self._separate_step(batch, batch.num_graphs, G)
 
     def stage(self, idx, epoch, G):
         """fill the next pinned slot with this step's inputs and enqueue its H2D copy."""
