@@ -200,6 +200,9 @@ _SIGS = {
     "igmc_edge_grad": [C.POINTER(Model), vp, vp, vp, vp, C.POINTER(Adj), C.c_int, C.c_int, C.POINTER(Dropout),
                        C.POINTER(Saved), vp, vp, C.c_int, vp, vp],
     "igmc_edge_grad_scatter": [C.POINTER(BatchOut), C.c_int, vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp],
+    "igmc_explain_node_count": [vp, vp, C.c_int, vp, vp],
+    "igmc_node_occlusion_mask": [C.POINTER(BatchOut), C.c_int, vp, vp, vp, vp, vp, vp, vp, vp],
+    "igmc_node_grad_scatter": [C.POINTER(BatchOut), C.c_int, vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp],
     "igmc_pair_factor_count": [C.POINTER(Model)],
     "igmc_pair_seed": [vp, vp, vp, C.c_int, C.c_float, vp, vp],
     "igmc_pair_grad": [C.POINTER(Model), vp, C.c_int, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, C.c_int, vp, C.c_int,

@@ -17,8 +17,14 @@
 // Attribution (attribute_pairs) reuses the count, offsets and order: its gradient pass extracts the P pairs again and
 // k_edge_grad_scatter sums each rating's two directed-edge gradients of igmc_edge_grad (csrc/rgcn_l2.cu) into its
 // position; igmc_occlusion_order then orders those values as they are (score = NULL).
+// Node explanations (explain_nodes / attribute_nodes) run the same passes with a pair's non-target nodes as positions:
+//   k_node_count          after a base batch's extraction: num_nodes[tag] = the graph's node count - 2
+//   k_node_occlusion_mask an occlusion batch's edge_keep drops every rating of the node at position j
+//                         (k_occlusion_pairs' edge_j is the node position) and records its id, label and rating count
+//   k_node_grad_scatter   the sum of each node's ratings' igmc_edge_grad values, in its in-list order, at its position
 #include <algorithm>
 
+#include <cub/block/block_reduce.cuh>
 #include <cub/block/block_scan.cuh>
 #include <cub/device/device_segmented_radix_sort.cuh>
 
@@ -159,6 +165,115 @@ k_edge_grad_scatter(const int32_t* __restrict__ edge_ptr, const int64_t* __restr
   }
 }
 
+// ---- node explanations (explain_nodes / attribute_nodes) ----
+// A pair's positions are the non-target nodes of its subgraph (node_label >= 2) in node order: position j is the j-th.
+
+__global__ void k_node_count(const int32_t* __restrict__ node_ptr, const int64_t* __restrict__ tag, int B,
+                             int32_t* __restrict__ num_nodes) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B) return;
+  const long long t = tag[i];
+  if (t >= 0) num_nodes[t] = max(node_ptr[i + 1] - node_ptr[i] - 2, 0);
+}
+
+// f(n, j) for every non-target node n of the nodes [n0, n1), j its position; one chunk of MASK_THREADS nodes at a time.
+// Every thread of the CTA must call it.
+template <class F>
+__device__ __forceinline__ void foreach_position(const uint8_t* __restrict__ node_label, int n0, int n1, F f) {
+  using Scan = cub::BlockScan<int, MASK_THREADS>;
+  __shared__ typename Scan::TempStorage tmp;
+  int carry = 0;
+  for (int base = n0; base < n1; base += MASK_THREADS) {
+    const int n = base + threadIdx.x;
+    const int flag = n < n1 && node_label[n] >= 2;
+    int ex, tot;
+    Scan(tmp).ExclusiveSum(flag, ex, tot);
+    if (flag) f(n, carry + ex);
+    carry += tot;
+    __syncthreads();   // tmp is reused by the next chunk
+  }
+}
+
+// graph i of an extracted occlusion batch: edge_keep of its edges (0 on every directed edge with node p = position j
+// as an endpoint: both copies of each of p's ratings) and p's global id, label and rating count at position c
+__global__ void __launch_bounds__(MASK_THREADS)
+k_node_occlusion_mask(const int32_t* __restrict__ node_ptr, const int32_t* __restrict__ edge_ptr,
+                      const int64_t* __restrict__ edge_index, long long row_stride,
+                      const uint8_t* __restrict__ node_label, const int32_t* __restrict__ node_gid,
+                      const int64_t* __restrict__ tag, const int32_t* __restrict__ node_j,
+                      uint8_t* __restrict__ edge_keep, int32_t* __restrict__ out_node, int32_t* __restrict__ out_label,
+                      int32_t* __restrict__ out_ratings, int* err) {
+  using Reduce = cub::BlockReduce<int, MASK_THREADS>;
+  __shared__ typename Reduce::TempStorage rtmp;
+  __shared__ int s_p;
+  const int i = blockIdx.x;
+  const int e0 = edge_ptr[i], e1 = edge_ptr[i + 1];
+  const long long c = tag[i];
+  const int j = node_j[i];
+  if (threadIdx.x == 0) s_p = -1;
+  __syncthreads();
+  if (c >= 0) foreach_position(node_label, node_ptr[i], node_ptr[i + 1], [&](int n, int jn) { if (jn == j) s_p = n; });
+  __syncthreads();
+  const int p = s_p;
+  if (c >= 0 && p < 0 && threadIdx.x == 0) igmc_set_err(err, IGMC_ERR_CANDIDATES);   // not the base pass's subgraph
+  int hits = 0;
+  for (int e = e0 + threadIdx.x; e < e1; e += blockDim.x) {
+    const bool hit = p >= 0 && (edge_index[e] == p || edge_index[row_stride + e] == p);
+    edge_keep[e] = hit ? 0 : 1;
+    hits += hit;
+  }
+  const int total = Reduce(rtmp).Sum(hits);   // thread 0: two directed edges per rating
+  if (p >= 0 && threadIdx.x == 0) {
+    out_node[c] = node_gid[p];
+    out_label[c] = node_label[p];
+    out_ratings[c] = total >> 1;
+  }
+}
+
+// graph i of an attribution batch with tag q >= 0: node n at position j gets the sum, in n's in-list order, of its
+// ratings' values edge_grad[a] + edge_grad[a + m] (a the rating's user -> item edge); out[offsets[q] + j] =
+// (checkpoint k = 0 ? 0 : out) + that sum, divided by K after the last checkpoint k = K - 1
+__global__ void __launch_bounds__(MASK_THREADS)
+k_node_grad_scatter(const int32_t* __restrict__ node_ptr, const int32_t* __restrict__ edge_ptr,
+                    const uint8_t* __restrict__ node_label, const int32_t* __restrict__ node_gid,
+                    const int32_t* __restrict__ in_ptr, const int32_t* __restrict__ in_eid,
+                    const int64_t* __restrict__ tag, const float* __restrict__ edge_grad,
+                    const int64_t* __restrict__ offsets, int k, int K, float* __restrict__ out,
+                    int32_t* __restrict__ out_node, int32_t* __restrict__ out_label, int32_t* __restrict__ out_ratings,
+                    int* err) {
+  const int i = blockIdx.x;
+  const long long q = tag[i];
+  if (q < 0) return;
+  const int n0 = node_ptr[i], n1 = node_ptr[i + 1], e0 = edge_ptr[i], m = (edge_ptr[i + 1] - e0) >> 1;
+  const long long o = offsets[q], cnt = offsets[q + 1] - o;
+  if (cnt != max(n1 - n0 - 2, 0)) {   // the subgraph is not the one the base pass counted
+    if (threadIdx.x == 0) igmc_set_err(err, IGMC_ERR_CANDIDATES);
+    return;
+  }
+  foreach_position(node_label, n0, n1, [&](int n, int j) {
+    if (j >= cnt) {   // more non-target nodes than nodes - 2: labels unlike an extracted subgraph's
+      igmc_set_err(err, IGMC_ERR_CANDIDATES);
+      return;
+    }
+    const int a0 = in_ptr[n], a1 = in_ptr[n + 1];
+    float v = 0.f;
+    for (int a = a0; a < a1; ++a) {
+      const int e = in_eid[a];
+      const int r = e - e0 < m ? e : e - m;
+      const float g = edge_grad[r] + edge_grad[r + m];
+      v = a == a0 ? g : v + g;
+    }
+    if (k > 0) v = out[o + j] + v;
+    if (k == K - 1) v = v / (float)K;
+    out[o + j] = v;
+    if (k == 0) {
+      out_node[o + j] = node_gid[n];
+      out_label[o + j] = node_label[n];
+      out_ratings[o + j] = a1 - a0;
+    }
+  });
+}
+
 // |delta| descending, NaN after every number: an ascending key on ~o, o = 0 for NaN, else the bits of |delta| + 1
 // (the bits of a non-negative float ascend with its value; +0 and -0 are one value)
 __device__ __forceinline__ uint32_t orderable_abs(float d) {
@@ -289,6 +404,40 @@ extern "C" int igmc_edge_grad_scatter(const igmc_batch_out_t* O, int B, const in
   k_edge_grad_scatter<<<B, MASK_THREADS, 0, (cudaStream_t)stream>>>(O->edge_ptr, O->edge_index, O->edge_cap,
                                                                      O->edge_type, O->node_gid, tag, edge_grad, offsets,
                                                                      k, K, out, user, item, rating, err);
+  IGMC_CUDA_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" int igmc_explain_node_count(const int32_t* node_ptr, const int64_t* tag, int B, int32_t* num_nodes,
+                                       void* stream) {
+  if (!node_ptr || !tag || !num_nodes || B <= 0) return -1;
+  k_node_count<<<(B + 255) / 256, 256, 0, (cudaStream_t)stream>>>(node_ptr, tag, B, num_nodes);
+  IGMC_CUDA_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" int igmc_node_occlusion_mask(const igmc_batch_out_t* O, int B, const int64_t* tag, const int32_t* node_j,
+                                        uint8_t* edge_keep, int32_t* node, int32_t* label, int32_t* ratings, int* err,
+                                        void* stream) {
+  if (!O || !O->node_ptr || !O->edge_ptr || !O->edge_index || !O->node_label || !O->node_gid || B <= 0) return -1;
+  if (!tag || !node_j || !edge_keep || !node || !label || !ratings) return -1;
+  k_node_occlusion_mask<<<B, MASK_THREADS, 0, (cudaStream_t)stream>>>(O->node_ptr, O->edge_ptr, O->edge_index,
+                                                                       O->edge_cap, O->node_label, O->node_gid, tag,
+                                                                       node_j, edge_keep, node, label, ratings, err);
+  IGMC_CUDA_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" int igmc_node_grad_scatter(const igmc_batch_out_t* O, int B, const int64_t* tag, const float* edge_grad,
+                                      const int64_t* offsets, int k, int K, float* out, int32_t* node, int32_t* label,
+                                      int32_t* ratings, int* err, void* stream) {
+  if (!O || !O->node_ptr || !O->edge_ptr || !O->node_label || !O->node_gid || !O->adj_in_ptr || !O->adj_eid || B <= 0)
+    return -1;
+  if (!tag || !edge_grad || !offsets || !out || !node || !label || !ratings || K < 1 || k < 0 || k >= K) return -1;
+  k_node_grad_scatter<<<B, MASK_THREADS, 0, (cudaStream_t)stream>>>(O->node_ptr, O->edge_ptr, O->node_label,
+                                                                     O->node_gid, O->adj_in_ptr, O->adj_eid, tag,
+                                                                     edge_grad, offsets, k, K, out, node, label,
+                                                                     ratings, err);
   IGMC_CUDA_CHECK_LAUNCH();
   return 0;
 }

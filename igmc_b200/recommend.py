@@ -22,6 +22,10 @@ building a dataset of every candidate pair and looping over it in Python.  Here:
 * ``attribute_pairs(model, graph, users, items, m)`` -> the same layout with, per rating, the score's gradient with
   respect to a weight on that rating (igmc_edge_grad): the same base pass, then one gradient pass over the P pairs, each
   an L2-plan eval forward and one backward whose list walk writes every edge's term;
+* ``explain_nodes`` / ``attribute_nodes(model, graph, users, items, m)`` -> the same two answers per node of the
+  enclosing subgraph (its users and items other than the two targets): the score change from removing every rating of
+  the node, and the score's gradient with respect to a gate on all of them.  The passes are the two above with the
+  pair's nodes as positions;
 * ``pair_gradients(model, graph, users, items, y)`` -> per-example gradients [K, P, param_count] of each pair's squared
   error (or score), ``influence(model, graph, train, test, k)`` -> per test pair the k training pairs of largest and
   smallest TracIn-CP influence, ``self_influence(model, graph, train)`` -> sum_k eta_k ||grad l_i||^2
@@ -56,7 +60,7 @@ from .util_functions import RatingGraph, SubgraphExtractor, _cuda_ints, _on_devi
 __all__ = ["predict_pairs", "recommend", "corated_items", "explain_pairs", "Explanation", "attribute_pairs",
            "Attribution", "pair_gradients", "influence", "self_influence", "Influence", "InferenceEngine",
            "RatingSessions", "predict_sessions", "recommend_sessions", "corated_items_sessions", "recommend_users",
-           "corated_users"]
+           "corated_users", "explain_nodes", "NodeExplanation", "attribute_nodes", "NodeAttribution"]
 
 
 # ---- input validation (host) ----------------------------------------------------------------------------------------
@@ -230,6 +234,21 @@ Explanation = collections.namedtuple("Explanation", "score num_edges offsets use
 # The result of attribute_pairs: Explanation's layout and order with grad (d score / d m_e, the rating's weight m_e at
 # m = 1) in place of delta.  -grad is the first-order estimate of explain_pairs' delta.
 Attribution = collections.namedtuple("Attribution", "score num_edges offsets user item rating grad")
+
+# The result of explain_nodes: score [P] fp32 (= predict_pairs), num_nodes [P] int32 (the non-target nodes of each
+# pair's subgraph), offsets [P+1] int64 and, per node, node (its global user or item id) / label (its node_label: even
+# a user, odd an item, 2h or 2h+1 at distance h) / ratings (its ratings in the subgraph) int32 and delta fp32 (score
+# with every rating of the node removed - score): flat or [P, m] padded with -1 / -1 / 0 / 0.
+NodeExplanation = collections.namedtuple("NodeExplanation", "score num_nodes offsets node label ratings delta")
+
+# The result of attribute_nodes: NodeExplanation's layout and order with grad (d score / d g_n at g = 1, g_n a gate on
+# the weight of each of the node's ratings: the sum of attribute_pairs' grad over them) in place of delta.
+NodeAttribution = collections.namedtuple("NodeAttribution", "score num_nodes offsets node label ratings grad")
+
+# the runs that explain a pair by its nodes, and the result of each explanation or attribution run
+_NODE_KINDS = ("explain_nodes", "attribute_nodes")
+_EXPLAIN_RESULTS = dict(explain=Explanation, attribute=Attribution, explain_nodes=NodeExplanation,
+                        attribute_nodes=NodeAttribution)
 
 # The result of influence: per test pair the k training pairs with the largest influence (pro_*, value descending) and
 # the k with the smallest (con_*, value ascending), [T, k] device tensors; index = position in the training list
@@ -539,6 +558,70 @@ def edge_grad_scatter_host(edge_ptr, tag, edge_grad, offsets, out, k=0, K=1):
     return out
 
 
+def node_positions_host(node_label, n0, n1):
+    """the nodes at positions 0, 1, ... of the graph with nodes [n0, n1): its nodes with node_label >= 2, in order"""
+    return n0 + np.flatnonzero(np.asarray(node_label)[n0:n1] >= 2)
+
+
+def node_count_host(node_ptr, tag, num_nodes):
+    """twin of igmc_explain_node_count: num_nodes[tag[g]] = max(N_g - 2, 0) for every graph g with tag >= 0;
+    ``num_nodes`` is updated in place and returned"""
+    node_ptr = np.asarray(node_ptr, np.int64)
+    for g in range(len(node_ptr) - 1):
+        if tag[g] >= 0:
+            num_nodes[tag[g]] = max(int(node_ptr[g + 1] - node_ptr[g]) - 2, 0)
+    return num_nodes
+
+
+def node_occlusion_mask_host(node_ptr, edge_ptr, src, dst, node_label, node_gid, tag, node_j):
+    """twin of igmc_node_occlusion_mask: (edge_keep [edge_ptr[B]], and per graph the dropped node's global id, label
+    and rating count, -1 / -1 / -1 where nothing is dropped).  Graph g with tag >= 0 drops every directed edge with its
+    node at position node_j[g] as src or dst (``src`` / ``dst``: edge_index rows, batch node ids)"""
+    node_ptr, edge_ptr = np.asarray(node_ptr, np.int64), np.asarray(edge_ptr, np.int64)
+    src, dst = np.asarray(src, np.int64), np.asarray(dst, np.int64)
+    B = len(node_ptr) - 1
+    keep = np.ones(int(edge_ptr[-1]), np.uint8)
+    rec = np.full((3, B), -1, np.int64)
+    for g in range(B):
+        pos = node_positions_host(node_label, int(node_ptr[g]), int(node_ptr[g + 1]))
+        if tag[g] < 0 or not 0 <= node_j[g] < len(pos):
+            continue
+        p = int(pos[node_j[g]])
+        e = np.arange(edge_ptr[g], edge_ptr[g + 1])
+        hit = e[(src[e] == p) | (dst[e] == p)]
+        keep[hit] = 0
+        rec[:, g] = (node_gid[p], node_label[p], len(hit) // 2)
+    return keep, rec
+
+
+def node_grad_scatter_host(node_ptr, edge_ptr, node_label, in_ptr, in_eid, tag, edge_grad, offsets, out, k=0, K=1):
+    """twin of igmc_node_grad_scatter's values for checkpoint ``k`` of ``K``: graph g with tag q >= 0 writes, for its
+    node n at position j, the fp32 sum over n's in-list in_eid[in_ptr[n]:in_ptr[n+1]] in list order (the first value
+    as it is, then each next one added) of the rating values edge_grad[a] + edge_grad[a + E_g/2] (a the rating's
+    user -> item edge) to out[offsets[q] + j] (k = 0), or adds it (k > 0), then divides by K (k = K - 1).  ``out`` [T]
+    is updated in place and returned"""
+    node_ptr, edge_ptr, offsets = (np.asarray(a, np.int64) for a in (node_ptr, edge_ptr, offsets))
+    edge_grad = np.asarray(edge_grad, np.float32)
+    for g in range(len(node_ptr) - 1):
+        q = int(tag[g])
+        if q < 0:
+            continue
+        e0, m = int(edge_ptr[g]), int(edge_ptr[g + 1] - edge_ptr[g]) // 2
+        o = int(offsets[q])
+        for j, n in enumerate(node_positions_host(node_label, int(node_ptr[g]), int(node_ptr[g + 1]))):
+            v = np.float32(0)
+            for t, e in enumerate(in_eid[in_ptr[n]:in_ptr[n + 1]]):
+                a = int(e) if int(e) - e0 < m else int(e) - m
+                r = np.float32(edge_grad[a] + edge_grad[a + m])
+                v = r if t == 0 else np.float32(v + r)
+            if k > 0:
+                v = np.float32(out[o + j] + v)
+            if k == K - 1:
+                v = np.float32(v / np.float32(K))
+            out[o + j] = v
+    return out
+
+
 # ---- rating sessions (csrc/session.cu) ------------------------------------------------------------------------------
 def session_rows_host(host, shape, users, session, items, values):
     """numpy twin of igmc_session_plan + _apply: (row_ptr [S+1], col_idx, rating) of the merged session rows.  Restates
@@ -668,6 +751,7 @@ class InferenceEngine(object):
         eng = InferenceEngine(model, graph, batch_size=256)
         eng.start_recommend(users, k)          # or start_pairs(users, items) / start_explain / start_attribute(users, items, m)
                                                # or start_recommend_users(items, k): per item its best users
+                                               # or start_explain_nodes / start_attribute_nodes(users, items, m)
         while eng.step():
             pass
         top_items, top_scores = eng.finish()   # (predict: scores; explain: an Explanation; attribute: an Attribution)
@@ -873,6 +957,20 @@ class InferenceEngine(object):
         users, items, _ = _host_pairs(self.graph.shape, users, items)
         return self._start_explicit("attribute", users, items, m=m, phase="base")
 
+    def start_explain_nodes(self, users, items, m=None):
+        """plan a node explanation run (``explain_nodes``): ``start_explain``'s two passes with the non-target nodes
+        of each pair's subgraph as positions; the base pass counts them.  Returns the number of pairs."""
+        m = _check_top(m)
+        users, items, _ = _host_pairs(self.graph.shape, users, items)
+        return self._start_explicit("explain_nodes", users, items, m=m, phase="base")
+
+    def start_attribute_nodes(self, users, items, m=None):
+        """plan a node attribution run (``attribute_nodes``): ``start_attribute``'s two passes, each node's gradient
+        the sum of its ratings' gradients.  Returns the number of pairs."""
+        m = _check_top(m)
+        users, items, _ = _host_pairs(self.graph.shape, users, items)
+        return self._start_explicit("attribute_nodes", users, items, m=m, phase="base")
+
     def start_pair_gradients(self, users, items, y=None):
         """plan a per-pair gradient run (``pair_gradients``) over the explicit pairs: per checkpoint the gradient of
         l_i = (f_i - y_i)^2 (``y`` given) or of the score f_i into run["out"] [K, P, param_count].  Returns P."""
@@ -993,11 +1091,12 @@ class InferenceEngine(object):
         run = dict(kind=kind, P=P, version=self.graph.version, scores=torch.empty(P, dtype=torch.float32, device=dev),
                    **extra)
         self.run = run
-        if kind in ("explain", "attribute"):
+        if kind in _EXPLAIN_RESULTS:
+            # the positions per pair: its ratings, or its non-target nodes on a node run
             run["num_edges"] = torch.zeros(P, dtype=torch.int32, device=dev)
             run["offsets"] = torch.zeros(P + 1, dtype=torch.int64, device=dev)
             for s in self.slots:
-                if kind == "explain" and "j" not in s:
+                if kind in ("explain", "explain_nodes") and "j" not in s:
                     s["j"] = torch.zeros(self.B, dtype=torch.int32, device=dev)
         if P == 0:
             return 0
@@ -1132,14 +1231,16 @@ class InferenceEngine(object):
         b = self.batches[slot] = self.extractor.extract(pairs=(s["u"], s["v"], None), pair_ids=s["pid"], reuse=True,
                                                         slot=slot, sessions=sessions,
                                                         sess=None if sessions is None else s["sess"])
+        nodes = run["kind"] in _NODE_KINDS
         if occlude:
-            _lib.check(self.lib.igmc_occlusion_mask(C.byref(b._lazy["_c"]), self.B, s["tag"].data_ptr(),
-                                                    s["j"].data_ptr(), s["keep"].data_ptr(), run["user"].data_ptr(),
-                                                    run["item"].data_ptr(), run["rating"].data_ptr(), err,
-                                                    _stream_ptr()), "igmc_occlusion_mask")
+            mask = "igmc_node_occlusion_mask" if nodes else "igmc_occlusion_mask"
+            _lib.check(getattr(self.lib, mask)(C.byref(b._lazy["_c"]), self.B, s["tag"].data_ptr(), s["j"].data_ptr(),
+                                               s["keep"].data_ptr(), run["user"].data_ptr(), run["item"].data_ptr(),
+                                               run["rating"].data_ptr(), err, _stream_ptr()), mask)
         elif run.get("phase") == "base":
-            _lib.check(self.lib.igmc_explain_count(b._priv["edge_ptr"].data_ptr(), s["tag"].data_ptr(), self.B,
-                                                   run["num_edges"].data_ptr(), _stream_ptr()), "igmc_explain_count")
+            count, ptr = ("igmc_explain_node_count", "node_ptr") if nodes else ("igmc_explain_count", "edge_ptr")
+            _lib.check(getattr(self.lib, count)(b._priv[ptr].data_ptr(), s["tag"].data_ptr(), self.B,
+                                                run["num_edges"].data_ptr(), _stream_ptr()), count)
 
     @contextlib.contextmanager
     def _params(self, j):
@@ -1211,11 +1312,11 @@ class InferenceEngine(object):
                                                    C.byref(d), C.byref(S), gw["seed"].data_ptr(),
                                                    gw["edge_grad"].data_ptr(), ws["cluster"], b._err.data_ptr(), st),
                            "igmc_edge_grad")
-            _lib.check(self.lib.igmc_edge_grad_scatter(C.byref(b._lazy["_c"]), self.B, s["tag"].data_ptr(),
-                                                       gw["edge_grad"].data_ptr(), run["offsets"].data_ptr(), j,
-                                                       self.K, run["occ"].data_ptr(), run["user"].data_ptr(),
-                                                       run["item"].data_ptr(), run["rating"].data_ptr(),
-                                                       self.extractor.err.data_ptr(), st), "igmc_edge_grad_scatter")
+            scatter = "igmc_node_grad_scatter" if run["kind"] in _NODE_KINDS else "igmc_edge_grad_scatter"
+            _lib.check(getattr(self.lib, scatter)(C.byref(b._lazy["_c"]), self.B, s["tag"].data_ptr(),
+                                                  gw["edge_grad"].data_ptr(), run["offsets"].data_ptr(), j, self.K,
+                                                  run["occ"].data_ptr(), run["user"].data_ptr(), run["item"].data_ptr(),
+                                                  run["rating"].data_ptr(), self.extractor.err.data_ptr(), st), scatter)
 
     def _launch(self, slot):
         main = torch.cuda.current_stream()
@@ -1246,7 +1347,7 @@ class InferenceEngine(object):
             return self._start_train_pass()
         if run.get("phase") != "base":
             return False
-        return self._start_occlusion() if run["kind"] == "explain" else self._start_gradient()
+        return self._start_occlusion() if run["kind"] in ("explain", "explain_nodes") else self._start_gradient()
 
     def finish(self):
         """wait for the run, check the error word (one host sync) and return (top_items [U, k] int64, top_scores
@@ -1263,7 +1364,7 @@ class InferenceEngine(object):
         self.run = None
         if run["kind"] == "recommend":
             return run["top_i"], run["top_s"]
-        if run["kind"] in ("explain", "attribute"):
+        if run["kind"] in _EXPLAIN_RESULTS:
             return self._order(run)
         if run["kind"] == "pair_gradients":
             return run["out"]
@@ -1285,15 +1386,18 @@ class InferenceEngine(object):
         nbytes = C.c_int64(0)
         _lib.check(self.lib.igmc_occlusion_order_ws_bytes(P, T, C.byref(nbytes)), "igmc_occlusion_order_ws_bytes")
         ws = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=dev)
-        explain = run["kind"] == "explain"
-        _lib.check(self.lib.igmc_occlusion_order(run["scores"].data_ptr() if explain else None, run["occ"].data_ptr(),
-                                                 run["offsets"].data_ptr(), P, T, run["user"].data_ptr(),
-                                                 run["item"].data_ptr(), run["rating"].data_ptr(), m or 0,
-                                                 ws.data_ptr(), ws.numel(), out["user"].data_ptr(),
-                                                 out["item"].data_ptr(), out["rating"].data_ptr(),
-                                                 out["delta"].data_ptr(), _stream_ptr()), "igmc_occlusion_order")
-        return (Explanation if explain else Attribution)(run["scores"], run["num_edges"], run["offsets"], out["user"],
-                                                         out["item"], out["rating"], out["delta"])
+        occlusion = run["kind"] in ("explain", "explain_nodes")
+        _lib.check(self.lib.igmc_occlusion_order(run["scores"].data_ptr() if occlusion else None,
+                                                 run["occ"].data_ptr(), run["offsets"].data_ptr(), P, T,
+                                                 run["user"].data_ptr(), run["item"].data_ptr(),
+                                                 run["rating"].data_ptr(), m or 0, ws.data_ptr(), ws.numel(),
+                                                 out["user"].data_ptr(), out["item"].data_ptr(),
+                                                 out["rating"].data_ptr(), out["delta"].data_ptr(), _stream_ptr()),
+                   "igmc_occlusion_order")
+        if m and run["kind"] in _NODE_KINDS:
+            out["rating"].masked_fill_(out["user"] < 0, 0)      # a padded node has no ratings
+        return _EXPLAIN_RESULTS[run["kind"]](run["scores"], run["num_edges"], run["offsets"], out["user"],
+                                             out["item"], out["rating"], out["delta"])
 
     def recommend(self, users, k, items=None, exclude_rated=True, retrieve=None):
         self.start_recommend(users, k, items, exclude_rated, retrieve)
@@ -1321,6 +1425,14 @@ class InferenceEngine(object):
 
     def attribute_pairs(self, users, items, m=None):
         self.start_attribute(users, items, m)
+        return self.finish()
+
+    def explain_nodes(self, users, items, m=None):
+        self.start_explain_nodes(users, items, m)
+        return self.finish()
+
+    def attribute_nodes(self, users, items, m=None):
+        self.start_attribute_nodes(users, items, m)
         return self.finish()
 
     def pair_gradients(self, users, items, y=None):
@@ -1409,6 +1521,42 @@ def attribute_pairs(model, graph, users, items, m=None, *, h=1, sample_ratio=1.0
     if len(users) == 0:
         return _no_pairs_explained(Attribution, m, model.flat_params.device)
     return _on_engine(model, graph, lambda eng: eng.attribute_pairs(users, items, m),
+                      h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
+
+
+def explain_nodes(model, graph, users, items, m=None, *, h=1, sample_ratio=1.0, max_nodes_per_hop=None, batch_size=256,
+                  checkpoints=None, sample_seed=0):
+    """why each pair (users[i], items[i]) got its score, one node at a time: for every node of the pair's enclosing
+    subgraph other than its two targets (the users and items with node_label >= 2, in the subgraph's node order),
+    delta = the score of that subgraph with every rating of the node removed (both directed edges; same nodes, labels
+    and sampling) - the pair's score.  For IGMC an isolated node sends no message, so this is the node removed;
+    DGCNN_RS still sorts it into its SortPooling.  Returns a ``NodeExplanation`` of device tensors: score [P] (bit for
+    bit ``predict_pairs``), num_nodes [P], offsets [P+1] and per node node (global user or item id) / label
+    (node_label) / ratings (its ratings in the subgraph) / delta, ordered within a pair by |delta| descending, NaN
+    after every number, ties by position; flat with pair p at [offsets[p], offsets[p+1]) when ``m`` is None, else the
+    first ``m`` per pair [P, m], padded with node / label -1 and ratings / delta 0.  A pair whose subgraph holds only
+    its targets (a cold-start pair) has no entries.  ``checkpoints``: every score is the fp32 checkpoint mean."""
+    m = _check_top(m)
+    users, items, _ = _host_pairs(graph.shape, users, items)
+    if len(users) == 0:
+        return _no_pairs_explained(NodeExplanation, m, model.flat_params.device)
+    return _on_engine(model, graph, lambda eng: eng.explain_nodes(users, items, m),
+                      h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
+
+
+def attribute_nodes(model, graph, users, items, m=None, *, h=1, sample_ratio=1.0, max_nodes_per_hop=None,
+                    batch_size=256, checkpoints=None, sample_seed=0):
+    """why each pair (users[i], items[i]) got its score, one node at a time and to first order: every non-target node
+    n of the pair's enclosing subgraph gets a gate g_n that multiplies the weight m_e (``attribute_pairs``) of each of
+    its ratings; grad = d score / d g_n at g = 1 = the sum of ``attribute_pairs``' grad over n's ratings, summed in n's
+    in-list order (its ratings sorted by (label, neighbour)).  -grad estimates ``explain_nodes``' delta.  Returns a
+    ``NodeAttribution`` in ``NodeExplanation``'s layout and order with grad in place of delta.  The gradient pass runs
+    the L2 kernel plan whatever plan the model uses.  ``checkpoints``: score and grad are fp32 checkpoint means."""
+    m = _check_top(m)
+    users, items, _ = _host_pairs(graph.shape, users, items)
+    if len(users) == 0:
+        return _no_pairs_explained(NodeAttribution, m, model.flat_params.device)
+    return _on_engine(model, graph, lambda eng: eng.attribute_nodes(users, items, m),
                       h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
 
 

@@ -568,6 +568,40 @@ int igmc_edge_grad_scatter(const igmc_batch_out_t* O, int B, const int64_t* tag,
                            const int64_t* offsets, int k, int K, float* out, int32_t* user, int32_t* item,
                            int32_t* rating, int* err, void* stream);
 
+/* ---- node explanations (csrc/explain.cu) ----
+ * The explanation and attribution passes above with a pair's non-target nodes as positions: position j of graph g is
+ * its j-th node with node_label >= 2 in node order (N_g - 2 positions for an extracted subgraph; the two targets are
+ * not explained).  Occlusion drops every rating incident to the node (both directed edges; nodes, labels and sampling
+ * unchanged), so an IGMC node sends no message: the node removed.  DGCNN_RS still sorts the isolated node into its
+ * SortPooling.  The gradient of a node is d score / d g_n at g = 1 for a gate g_n on the weight m_e of each of its
+ * ratings: the sum of those ratings' igmc_edge_grad_scatter values. */
+
+/* After the extraction of a base batch: num_nodes[tag[i]] = max(node_ptr[i+1] - node_ptr[i] - 2, 0) for every i with
+ * tag[i] >= 0.  igmc_explain_offsets scans the counts and igmc_occlusion_pairs maps the positions unchanged (its
+ * edge_j is the node position j). */
+int igmc_explain_node_count(const int32_t* node_ptr, const int64_t* tag, int B, int32_t* num_nodes, void* stream);
+
+/* For the batch O of B graphs extracted from igmc_occlusion_pairs' output: edge_keep [O->edge_ptr[B]] is 1 except, in
+ * every graph with tag >= 0, 0 on each directed edge with node p as source or target (both copies of each rating of
+ * p), p = the graph's node at position node_j; and node / label / ratings [T] at position tag = p's global id
+ * (node_gid), its node_label and its number of ratings in the subgraph.  One CTA per graph.  A position outside the
+ * graph's nodes sets IGMC_ERR_CANDIDATES, drops nothing and records nothing. */
+int igmc_node_occlusion_mask(const igmc_batch_out_t* O, int B, const int64_t* tag, const int32_t* node_j,
+                             uint8_t* edge_keep, int32_t* node, int32_t* label, int32_t* ratings, int* err,
+                             void* stream);
+
+/* One CTA per graph i of the batch O (adjacency required) with tag[i] = q >= 0: for the node n at position j,
+ * out[offsets[q] + j] = the fp32 sum over n's in-list entries adj_in_ptr[n] .. adj_in_ptr[n+1] (one per rating of n)
+ * in list order, the first entry's value taken as it is, each later one added, of the rating's value
+ * edge_grad[a] + edge_grad[a + E_i/2] (a = the rating's user -> item edge, e0 <= a < e0 + E_i/2); +0 without
+ * entries.  Accumulated over checkpoints as igmc_edge_grad_scatter does: k = 0 stores, k > 0 adds in k order,
+ * k = K - 1 divides by K.  At k = 0 also node / label / ratings [T] as igmc_node_occlusion_mask records them (ratings =
+ * the in-list length).  A graph whose node count is not its base-pass count sets IGMC_ERR_CANDIDATES and writes
+ * nothing. */
+int igmc_node_grad_scatter(const igmc_batch_out_t* O, int B, const int64_t* tag, const float* edge_grad,
+                           const int64_t* offsets, int k, int K, float* out, int32_t* node, int32_t* label,
+                           int32_t* ratings, int* err, void* stream);
+
 /* ---- per-pair gradients and training-data influence (csrc/influence.cu) ----
  * TracIn-CP (Pruthi et al., NeurIPS 2020): influence(i, t) = sum_k eta_k <grad l_i(theta_k), grad q_t(theta_k)> over
  * checkpoints k, self_influence(i) = sum_k eta_k ||grad l_i(theta_k)||^2, with l_i = (f_i - y_i)^2 of ONE pair (no batch
