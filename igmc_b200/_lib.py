@@ -27,6 +27,7 @@ ERR_NAMES = {
     7: "inference candidates: a user / item id outside the rating matrix or an inconsistent candidate plan",
     8: "graph update: a user / item id outside the graph's capacity or a value outside 0..256",
     9: "rating sessions: a session / item id out of range, a negative user id or a value outside 0..256",
+    10: "online training draw: the rating graph has no ratings",
 }
 
 TOPK_MAX = 256       # IGMC_TOPK_MAX
@@ -228,6 +229,9 @@ _SIGS = {
                               C.c_double, C.c_uint64, vp, C.c_int, C.POINTER(ExtractWS), vp, C.c_int, C.c_int,
                               C.POINTER(BatchOut), vp, vp],
     "igmc_corated_sessions": [C.POINTER(CSR), C.POINTER(Sessions), C.c_int, C.c_int, vp, C.c_int64, vp, vp, vp, vp],
+    "igmc_online_draw": [C.POINTER(CSR), vp, vp, C.c_int, vp, C.c_int64, vp, C.c_int, C.c_uint64, C.c_uint64, C.c_int,
+                         vp, vp, vp, vp, vp, vp, vp],
+    "igmc_online_recent_append": [vp, vp, vp, C.c_int, vp, vp, C.c_int, vp, vp, vp],
     "igmc_build_info": [],
     "igmc_model_plan": [C.POINTER(Model), C.c_int, C.c_int, C.c_int],
     "igmc_sortpool_plan": [C.POINTER(SortPool), C.c_int, C.c_int],

@@ -415,7 +415,9 @@ class IGMC(nn.Module):
             return None
         lib = _lib.load()
         p = batch._priv
-        key = (p["node_cap"], batch.num_graphs, bool(training), cl, int(slot))
+        # (an image is laid out for n_cap, which an extractor that follows graph updates may lower inside buffers of the
+        # same node_cap, and for the list capacity of list_hint, which a later plan for larger subgraphs may set)
+        key = (p["node_cap"], p["n_cap"], batch.num_graphs, bool(training), cl, int(slot), self._cmodel.list_hint)
         cache = self.__dict__.setdefault("_stage_ws", {})
         st = cache.get(key)
         if st is None:

@@ -13,9 +13,11 @@ What changed underneath (SURVEY.md §3.2 / §7):
   slice of every global batch; the only collective is one all-reduce(SUM) of the flat gradient
   (49 k floats) per step, plus one scalar all-reduce per epoch for the reported loss / RMSE.
 """
+import ctypes as C
 import math
 import os
 import time
+import types
 
 import numpy as np
 import torch
@@ -23,6 +25,7 @@ import torch
 from . import _lib
 from .models import FusedAdam, splitmix64
 from .util_functions import DevView, MyDynamicDataset  # noqa: F401  (re-export, Main.py star-imports)
+from .util_functions import RatingGraph, SubgraphExtractor, _on_device_i32, _stream_ptr, _update_inputs
 
 try:
     import torch.distributed as dist
@@ -183,6 +186,7 @@ class TrainEngine(object):
                 rows = nb * ws["cluster"]
             else:   # no graph of a short tail batch on this rank: it still takes part in the exchange (zero rows)
                 ws, rows = self._last_ws, 0
+            self._before_update()
             self.last_loss = self.opt.reduce_update(self.exchange, ws, nb, rows, 1.0 / max(G, 1), self.arr_local,
                                                     lr_dev=self.lr_dev, loss_acc=self.loss_acc, loss_weight=float(G),
                                                     loss_ring=self.loss_ring_view if self.zero_copy else None)
@@ -199,8 +203,13 @@ class TrainEngine(object):
             loss = torch.zeros(1, dtype=torch.float32, device=self.dev)
         if self.world > 1:
             dist.all_reduce(m.flat_grad)
+        self._before_update()
         self.opt.step(grad_mul=1.0, lr_dev=self.lr_dev, loss_in=loss, loss_acc=self.loss_acc, loss_weight=float(G))
         self.last_loss = loss
+
+    def _before_update(self):
+        """launches that must be ordered before the step's update kernel, which writes the parameters and the Adam step
+        counter (none here; ``OnlineTrainer`` waits for its draw, which reads the counter)"""
 
     def _launch(self, nb, G):
         B = self.B
@@ -290,12 +299,19 @@ class TrainEngine(object):
         """extract the ``nb`` indices of step inputs ``buf`` into batch slot ``slot`` and stage its edge lists with the
         dropout draws of the step that trains on it (seed at buf[B + 3])"""
         B = self.B
-        self.batches[slot] = self.dataset.extractor.extract(idx=buf[:nb], seed_dev=buf[B:B + 1], reuse=True, slot=slot)
-        self.model.stage_batch(self.batches[slot], True, self.model.make_dropout(True, seed_dev=buf[B + 3:B + 4]),
-                               slot=slot)
+        self._stage(slot, self.dataset.extractor.extract(idx=buf[:nb], seed_dev=buf[B:B + 1], reuse=True, slot=slot),
+                    buf[B + 3:B + 4])
 
-    def _launch_pipe(self, nb, G, slot, nb_next, buf=None):
+    def _stage(self, slot, batch, drop_seed_dev):
+        """batch slot ``slot`` <- ``batch``, its list images staged with the dropout seed (device) of the step that
+        trains on it"""
+        self.batches[slot] = batch
+        self.model.stage_batch(batch, True, self.model.make_dropout(True, seed_dev=drop_seed_dev), slot=slot)
+
+    def _launch_pipe(self, nb, G, slot, nb_next, buf=None, seed_dev=None):
+        """``seed_dev``: the dropout seed (device) of this step, default the one in the step inputs ``buf``"""
         buf = self.stepbuf_dev if buf is None else buf
+        seed_dev = buf[self.B + 1:self.B + 2] if seed_dev is None else seed_dev
         main = torch.cuda.current_stream()
         if nb_next > 0:
             self.side.wait_stream(main)
@@ -307,7 +323,7 @@ class TrainEngine(object):
                     # they pack two per SM on the SMs that are left.
                     self.model.gate_wait(self.batches[slot])
                 self._extract(slot ^ 1, nb_next, buf)
-        self._model_step(self.batches[slot] if nb > 0 else None, nb, G, buf[self.B + 1:self.B + 2])
+        self._model_step(self.batches[slot] if nb > 0 else None, nb, G, seed_dev)
         if nb_next > 0:
             main.wait_stream(self.side)
 
@@ -370,6 +386,223 @@ class TrainEngine(object):
 
     def check(self):
         _check_dataset(self.dataset)
+
+
+_M64 = (1 << 64) - 1
+_DRAW_HOP_TAG = 7    # csrc/online.cu: sample_state's hop slot of the draw keys
+
+
+def _splitmix64_np(x):
+    """splitmix64 on uint64 arrays (csrc/common.cuh), wrapping mod 2^64"""
+    x = np.asarray(x, dtype=np.uint64)
+    with np.errstate(over="ignore"):
+        x = x + np.uint64(0x9E3779B97F4A7C15)
+        x = (x ^ (x >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+        x = (x ^ (x >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+        return x ^ (x >> np.uint64(31))
+
+
+def _draw_keys(seed, B, rnd):
+    """sample_state(seed, j, rnd, 7) of slots j < B (csrc/common.cuh, csrc/online.cu: draw_key)"""
+    tag = np.arange(B, dtype=np.uint64) * np.uint64(16) + np.uint64(2 * _DRAW_HOP_TAG + rnd)
+    return _splitmix64_np(np.uint64(int(seed) & _M64) ^ _splitmix64_np(tag))
+
+
+def recent_threshold(recent_fraction):
+    """round(recent_fraction * 2^32): a slot draws from the recent window when the top 32 bits of its key fall below"""
+    return int(round(float(recent_fraction) * 4294967296.0))
+
+
+def recent_append_host(ring_u, ring_v, total, users, items, values):
+    """numpy twin of igmc_online_recent_append: the (user, item) of the entries with value > 0 appended at slot
+    (total + rank) % capacity, in input order.  Returns (ring_u, ring_v, total) (new arrays)."""
+    u, v, x = (np.asarray(a, dtype=np.int64).reshape(-1) for a in (users, items, values))
+    keep = (u >= 0) & (v >= 0) & (x > 0) & (x <= 256)
+    u, v = u[keep], v[keep]
+    ring_u, ring_v = np.array(ring_u, dtype=np.int32), np.array(ring_v, dtype=np.int32)
+    first = max(len(u) - len(ring_u), 0)
+    slots = (int(total) + np.arange(first, len(u))) % len(ring_u)
+    ring_u[slots], ring_v[slots] = u[first:], v[first:]
+    return ring_u, ring_v, int(total) + len(u)
+
+
+def online_draw_host(row_ptr, col_idx, rating, num_items, ring_u, ring_v, total, recent_thresh, step, sample_seed,
+                     drop_seed, B):
+    """numpy twin of igmc_online_draw for step ``step`` (= the step counter + step_ahead) on the host arrays of a graph
+    (row_ptr [num_users + 1]).  Returns (users, items, labels, pair_ids, seeds [3] uint64, from_window [B] bool)."""
+    row_ptr = np.asarray(row_ptr, dtype=np.int64)
+    num_users, nnz = len(row_ptr) - 1, int(row_ptr[-1])
+    s = int(step)
+    seed = int(_splitmix64_np(np.uint64((int(sample_seed) + s) & _M64)))
+    seeds = _splitmix64_np(np.array([(int(drop_seed) + s) & _M64, (int(drop_seed) + s + 1) & _M64], dtype=np.uint64))
+    seeds = np.concatenate([np.array([seed], dtype=np.uint64), seeds])
+    W = min(int(total), len(ring_u))
+    key = _draw_keys(seed, B, 0)
+    pos = np.full(B, -1, dtype=np.int64)
+    u = np.zeros(B, dtype=np.int64)
+    v = np.zeros(B, dtype=np.int64)
+    win = (key >> np.uint64(32)).astype(np.int64) < int(recent_thresh) if W > 0 else np.zeros(B, dtype=bool)
+    for j in np.flatnonzero(win):
+        e = (int(key[j]) & 0xFFFFFFFF) * W >> 32
+        a, b = int(ring_u[e]), int(ring_v[e])
+        if 0 <= a < num_users and 0 <= b < num_items:
+            lo, hi = row_ptr[a], row_ptr[a + 1]
+            k = lo + np.searchsorted(col_idx[lo:hi], b)
+            if k < hi and col_idx[k] == b:
+                u[j], v[j], pos[j] = a, b, k
+    fall = pos < 0
+    h = _draw_keys(seed, B, 1)
+    # floor(h * nnz / 2^64) in two 32-bit halves (nnz < 2^31: no partial product overflows)
+    hi32, lo32 = (h >> np.uint64(32)).astype(np.uint64), (h & np.uint64(0xFFFFFFFF)).astype(np.uint64)
+    with np.errstate(over="ignore"):
+        p = ((hi32 * np.uint64(nnz) + ((lo32 * np.uint64(nnz)) >> np.uint64(32))) >> np.uint64(32)).astype(np.int64)
+    uu = np.searchsorted(row_ptr, p, side="right") - 1
+    u[fall], pos[fall] = uu[fall], p[fall]
+    v[fall] = np.asarray(col_idx)[p[fall]]
+    lab = np.asarray(rating)[pos].astype(np.int64)
+    return u, v, lab, u * int(num_items) + v, seeds, ~fall
+
+
+class OnlineTrainer(TrainEngine):
+    """Fine-tunes a trained model on its ``RatingGraph`` as ratings arrive (DESIGN §15).
+
+        tr = OnlineTrainer(model, graph, optimizer, batch_size=50, ARR=0.001, h=1, max_nodes_per_hop=100)
+        tr.update(users, items, values)   # graph.update(...) + the rated entries appended to the recent window
+        loss = tr.train(steps=20)         # mean training loss over the steps (one host sync)
+
+    A step is ``TrainEngine``'s pipelined, graph-replayed step (``_launch_pipe``: the fused update kernel, or fused_step
+    + Adam where the plan has no raw rows) with no host inputs: the pairs of the next step are drawn on the device
+    (igmc_online_draw) beside this one, a ``recent_fraction`` share of them from a ring of the last ``recent_capacity``
+    rated pairs of ``update`` (a pair appended twice is drawn with twice the weight), the rest uniformly from the
+    graph's ratings, each labelled as the graph holds it when drawn.  The step number is the optimizer's device Adam
+    step counter, so the dropout stream continues the one a ``train_multiple_epochs`` run left.  Parameters are updated
+    in place.  ``train`` starts over on a graph that changed since the captured steps were built: captured graphs
+    dropped, the extractor's capacities re-derived (workspace re-reserved), the model planned for the new batches, the
+    first batch drawn again.  One process only."""
+
+    def __init__(self, model, graph, optimizer, batch_size=50, ARR=0.001, h=1, max_nodes_per_hop=100,
+                 class_values=None, recent_fraction=0.5, recent_capacity=65536, sample_seed=0, use_graph=True):
+        dev = model.flat_params.device
+        if dev.type != "cuda":
+            raise RuntimeError("igmc_b200 training needs the model on a CUDA device (there is no CPU path)")
+        if _dist_info()[1] > 1:
+            raise NotImplementedError("online training runs in one process: graph updates are not replicated across "
+                                      "ranks")
+        if not isinstance(graph, RatingGraph):
+            raise TypeError("graph must be a RatingGraph (the trainer follows its updates)")
+        if int(batch_size) < 1:
+            raise ValueError("batch_size must be >= 1")
+        if not 0.0 <= float(recent_fraction) <= 1.0:
+            raise ValueError("recent_fraction must lie in [0, 1], got %r" % (recent_fraction,))
+        if int(recent_capacity) < 1:
+            raise ValueError("recent_capacity must be >= 1")
+        if model.num_features != 2 * int(h) + 2:
+            raise ValueError("the model takes %d node features, hop %d extraction gives %d"
+                             % (model.num_features, int(h), 2 * int(h) + 2))
+        _check_ratings(graph)
+        if graph.device is None or graph.device != dev:
+            graph.to(dev)
+        cv = np.arange(1, model.num_relations + 1, dtype=np.float32) if class_values is None else class_values
+        ex = SubgraphExtractor(graph, [0], [0], [0], cv, h, 1.0, max_nodes_per_hop, max_batch=int(batch_size),
+                               seed=sample_seed)
+        super().__init__(types.SimpleNamespace(graph=graph, extractor=ex), model, optimizer, batch_size, ARR,
+                         use_graph, sample_seed)
+        self.lib, self.graph = _lib.load(), graph
+        self.recent_fraction = float(recent_fraction)
+        i32, i64 = dict(dtype=torch.int32, device=dev), dict(dtype=torch.int64, device=dev)
+        # the recent window: a ring of (user, item) and the count of pairs ever appended
+        self.recent_u, self.recent_v = torch.zeros(int(recent_capacity), **i32), torch.zeros(int(recent_capacity), **i32)
+        self.recent_total = torch.zeros(1, **i64)
+        # per batch slot: the drawn pairs igmc_extract_batch reads (idx = NULL) and the step's three seeds
+        self.draws = [dict(u=torch.zeros(self.B, **i32), v=torch.zeros(self.B, **i32), label=torch.zeros(self.B, **i32),
+                           pid=torch.zeros(self.B, **i64), seeds=torch.zeros(3, **i64)) for _ in range(2)]
+        self.drawn = torch.cuda.Event()
+        self.side = torch.cuda.Stream(dev)
+        self.batches = [None, None]
+        self.slot = 0
+        self._version = None     # graph version of the captured steps and the drawn batch (None: nothing drawn yet)
+
+    def update(self, users, items, values, shape=None):
+        """``graph.update(users, items, values, shape)`` (its validation and counts), then the (user, item) of every
+        entry with value > 0 appended to the recent window"""
+        counts = self.graph.update(users, items, values, shape)
+        cu, ci, _ = self.graph.capacity
+        u, v, x, D = _update_inputs(users, items, values, cu, ci)
+        if D:
+            u, v, x = (_on_device_i32(a, self.dev) for a in (u, v, x))
+            _lib.check(self.lib.igmc_online_recent_append(u.data_ptr(), v.data_ptr(), x.data_ptr(), D,
+                                                          self.recent_u.data_ptr(), self.recent_v.data_ptr(),
+                                                          self.recent_u.numel(), self.recent_total.data_ptr(),
+                                                          self.dataset.extractor.err.data_ptr(), _stream_ptr()),
+                       "igmc_online_recent_append")
+        return counts
+
+    def train(self, steps):
+        """``steps`` optimisation steps on the graph as it is now; returns their mean training loss (one host sync)"""
+        steps = int(steps)
+        if steps < 1:
+            raise ValueError("steps must be >= 1")
+        _check_ratings(self.graph)
+        self.model.train()
+        self.sync_lr()
+        if self._version != self.graph.version:
+            self._prime()
+        else:
+            # the drawn batch's list images live in the model's stage cache, which another engine training this model
+            # may have overwritten since the last call: build them again (the same images: batch and seed are the same)
+            self._stage(self.slot, self.batches[self.slot], self.draws[self.slot]["seeds"][2:3])
+        if self.fused_update and self.model.fused_update_ok(self.batches[self.slot]):
+            # W_r / W_r^T of the parameters as they are now (an eval forward or a loaded state may have left them
+            # unprepared): the captured steps of the fused update kernel never prepare them, its update does
+            self.model.prep_weights(mark=True)
+        self.loss_acc.zero_()
+        for _ in range(steps):
+            slot = self.slot
+            self.steps += 1
+            self._replay(slot, lambda: self._launch_pipe(self.B, self.B, slot, self.B,
+                                                         seed_dev=self.draws[slot]["seeds"][2:3]))
+            self._updates += 1
+            self.slot ^= 1
+        loss = float(self.loss_acc.item()) / (steps * self.B)
+        self.check()
+        return loss
+
+    def _prime(self):
+        """start over on the graph as it is: drop the captured steps (they hold its old shape and the extractor's old
+        buffers), then draw, extract and stage the first batch (the extractor re-derives its capacities, the model
+        plans for the batch's shape)"""
+        torch.cuda.current_stream().synchronize()     # no replay still reads what is dropped
+        self.graphs.clear()
+        self.graph_loss.clear()
+        self.eager_done.clear()
+        self._version = self.graph.version
+        self.slot = 0
+        self._extract(0, self.B, None, ahead=0)
+
+    def _extract(self, slot, nb, buf=None, ahead=1):
+        """draw the pairs of batch slot ``slot`` (step counter + ``ahead``: 1 beside the step that will increment it),
+        extract them and stage their list images with the dropout seed of the step that trains on them"""
+        d, g = self.draws[slot], self.graph
+        _lib.check(self.lib.igmc_online_draw(C.byref(g._c), self.recent_u.data_ptr(), self.recent_v.data_ptr(),
+                                             self.recent_u.numel(), self.recent_total.data_ptr(),
+                                             recent_threshold(self.recent_fraction), self.opt.step_count.data_ptr(),
+                                             int(ahead), self.sample_seed & _M64, self.model.drop_seed & _M64, self.B,
+                                             d["u"].data_ptr(), d["v"].data_ptr(), d["label"].data_ptr(),
+                                             d["pid"].data_ptr(), d["seeds"].data_ptr(),
+                                             self.dataset.extractor.err.data_ptr(), _stream_ptr()), "igmc_online_draw")
+        self.drawn.record()
+        b = self.dataset.extractor.extract(pairs=(d["u"], d["v"], d["label"]), pair_ids=d["pid"],
+                                           seed_dev=d["seeds"][0:1], reuse=True, slot=slot)
+        self._stage(slot, b, d["seeds"][2:3])
+
+    def _before_update(self):
+        # the draw beside this step reads the step counter the update kernel increments
+        torch.cuda.current_stream().wait_event(self.drawn)
+
+
+def _check_ratings(graph):
+    if graph.nnz == 0:
+        raise ValueError("the rating graph has no ratings to train on")
 
 
 def train_multiple_epochs(train_dataset, test_dataset, model, epochs, batch_size, lr, lr_decay_factor,

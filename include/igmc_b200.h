@@ -768,6 +768,36 @@ int igmc_extract_sessions(const igmc_csr_t* G, const igmc_sessions_t* S, const i
 int igmc_corated_sessions(const igmc_csr_t* G, const igmc_sessions_t* S, int m, int exclude_rated, void* ws,
                           int64_t ws_bytes, int32_t* items, int32_t* paths, int* err, void* stream);
 
+/* ---- online fine-tuning (csrc/online.cu; igmc_b200/train_eval.py: OnlineTrainer) ----
+ * A trainer that follows graph updates draws each step's training pairs from G itself, a share of them from a ring of
+ * recently rated pairs.  The ring holds `capacity` (user, item) pairs in ring_u / ring_v; `total` (device int64) counts
+ * the pairs ever appended, so the window is its first W = min(total, capacity) slots.  Labels are never stored: a
+ * window pair is looked up in G when it is drawn, so a later overwrite or delete is respected.
+ *
+ * igmc_online_recent_append appends the (users[i], items[i]) of every entry with values[i] > 0 of a delta (RatingGraph
+ * update encoding) in input order at slot (total + rank) % capacity, the newest over the oldest, then total += their
+ * count.  One CTA.  A negative id or a value outside 0..256 sets IGMC_ERR_GRAPH_UPDATE and the entry is skipped. */
+int igmc_online_recent_append(const int32_t* users, const int32_t* items, const int32_t* values, int D, int32_t* ring_u,
+                              int32_t* ring_v, int capacity, int64_t* total, int* err, void* stream);
+
+/* One step's B training pairs for igmc_extract_batch (idx = NULL): links_u / links_v / label / pair_id [B] and seeds [3].
+ * The step s = step_count[0] + step_ahead (step_count: the optimizer's device Adam step counter; step_ahead 1 when the
+ * draw runs beside the step that will increment it, 0 otherwise), and
+ *   seeds[0] = splitmix64(sample_seed + s)   the extraction sample seed, and the seed of the pair keys below
+ *   seeds[1] = splitmix64(drop_seed + s)     the dropout seed of step s
+ *   seeds[2] = splitmix64(drop_seed + s + 1) the dropout seed of step s + 1, the step that trains on these pairs
+ * Slot j: key = sample_state(seeds[0], j, 0, 7) (csrc/common.cuh; hop slot 7 is never used by extraction).  When W > 0
+ * and key >> 32 < recent_thresh (= round(recent_fraction * 2^32), 0..2^32) the pair is window entry
+ * ((key & 0xffffffff) * W) >> 32, labelled by a binary search of its user's row; a window pair G does not hold (deleted,
+ * or ids outside G) falls through.  Otherwise p = (h * nnz) >> 64 with h = sample_state(seeds[0], j, 1, 7) and nnz =
+ * row_ptr[num_users]: user upper_bound(row_ptr[0..num_users], p) - 1, item col_idx[p], label rating[p].  pair_id = u *
+ * num_items + v.  A graph without ratings sets IGMC_ERR_ONLINE (pairs (0, 0)).  Reads only device state: one captured
+ * CUDA graph serves every step while G's shape stays. */
+int igmc_online_draw(const igmc_csr_t* G, const int32_t* ring_u, const int32_t* ring_v, int capacity,
+                     const int64_t* total, int64_t recent_thresh, const int64_t* step_count, int step_ahead,
+                     uint64_t sample_seed, uint64_t drop_seed, int B, int32_t* links_u, int32_t* links_v, int32_t* label,
+                     int64_t* pair_id, uint64_t* seeds, int* err, void* stream);
+
 /* Version / build info: returns the compiled SM arch (90) so the host can refuse stale builds. */
 int igmc_build_info(void);
 
