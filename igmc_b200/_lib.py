@@ -31,6 +31,7 @@ ERR_NAMES = {
 }
 
 TOPK_MAX = 256       # IGMC_TOPK_MAX
+DRAWS_MAX = 256      # IGMC_DRAWS_MAX
 
 # Kernel plan values (igmc_model_plan): 0 generic kernels, 1..4 relation-space cluster kernels (CTAs per subgraph),
 # PLAN_L2_BASE + c (c = 1, 2, 4, 8) the L2 plan with c CTAs per subgraph (IGMC_PLAN_L2 in include/igmc_b200.h).
@@ -232,6 +233,9 @@ _SIGS = {
     "igmc_online_draw": [C.POINTER(CSR), vp, vp, C.c_int, vp, C.c_int64, vp, C.c_int, C.c_uint64, C.c_uint64, C.c_int,
                          vp, vp, vp, vp, vp, vp, vp],
     "igmc_online_recent_append": [vp, vp, vp, C.c_int, vp, vp, C.c_int, vp, vp, vp],
+    "igmc_draws_expand": [C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp],
+    "igmc_draws_mask": [C.POINTER(BatchOut), C.c_int, vp, vp, vp, C.c_float, C.c_uint64, vp, vp, vp],
+    "igmc_draws_stats": [vp, C.c_int, C.c_int, C.c_int, vp, C.c_double, vp, vp, vp, vp, vp],
     "igmc_build_info": [],
     "igmc_model_plan": [C.POINTER(Model), C.c_int, C.c_int, C.c_int],
     "igmc_sortpool_plan": [C.POINTER(SortPool), C.c_int, C.c_int],

@@ -62,6 +62,13 @@ __host__ __device__ __forceinline__ bool edge_keep(uint64_t seed, uint32_t eid, 
   return (uint32_t)(splitmix64(seed + (uint64_t)eid) >> 32) >= thresh;
 }
 
+// fp32 mean of the K checkpoint predictions of batch entry i (preds row stride B), summed in checkpoint order
+__device__ __forceinline__ float ckpt_mean(const float* __restrict__ preds, int K, int B, int i) {
+  float a = preds[i];
+  for (int q = 1; q < K; ++q) a = __fadd_rn(a, preds[(size_t)q * B + i]);
+  return K > 1 ? __fdiv_rn(a, (float)K) : a;
+}
+
 // ---- warp / block primitives -----------------------------------------------------------------
 __device__ __forceinline__ int warp_sum_i(int v) {
 #pragma unroll

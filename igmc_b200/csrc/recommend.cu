@@ -251,13 +251,6 @@ k_candidate_pairs(igmc_csr_t G, igmc_candidates_t Cd, int64_t* __restrict__ curs
   if (threadIdx.x == 0) *cursor = pos + B;
 }
 
-// fp32 mean of the K checkpoint predictions of batch entry i, summed in checkpoint order
-__device__ __forceinline__ float ckpt_mean(const float* __restrict__ preds, int K, int B, int i) {
-  float a = preds[i];
-  for (int q = 1; q < K; ++q) a = __fadd_rn(a, preds[(size_t)q * B + i]);
-  return K > 1 ? __fdiv_rn(a, (float)K) : a;
-}
-
 __global__ void __launch_bounds__(MERGE_THREADS)
 k_topk_merge(const float* __restrict__ preds, int K, int B, const int64_t* __restrict__ tag,
              const int32_t* __restrict__ items, int k, float* __restrict__ top_score, int64_t* __restrict__ top_item) {

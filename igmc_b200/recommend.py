@@ -36,6 +36,10 @@ building a dataset of every candidate pair and looping over it in Python.  Here:
   encoding, applied only while that user's own pairs are scored; ``predict_sessions``, ``recommend_sessions`` and
   ``corated_items_sessions`` score, rank and retrieve for many sessions in one run and leave the graph unchanged.  A
   session's results are bit for bit those of the graph functions on the graph with that session's edits applied;
+* ``predict_draws(model, graph, users, items, draws)`` -> per pair S Monte-Carlo-dropout draws of its score (the
+  training-mode forward under the model's own edge and hidden dropout, masks keyed by the pair id and the draw index)
+  and their mean and std (csrc/draws.cu); ``recommend``, ``recommend_users`` and ``recommend_sessions`` with
+  ``draws=S`` rank by mean + beta * std over S draws (Thompson sampling at S = 1, UCB for beta > 0);
 * ``InferenceEngine``: the pipelined, graph-replayed loop behind all of them.  Per step the side stream produces the next
   batch's candidate pairs (``igmc_candidate_pairs``, from a device cursor) and extracts it while the main stream runs
   the eval forward of the current batch (once per checkpoint) and merges its scores into the running per-user top-k
@@ -60,7 +64,8 @@ from .util_functions import RatingGraph, SubgraphExtractor, _cuda_ints, _on_devi
 __all__ = ["predict_pairs", "recommend", "corated_items", "explain_pairs", "Explanation", "attribute_pairs",
            "Attribution", "pair_gradients", "influence", "self_influence", "Influence", "InferenceEngine",
            "RatingSessions", "predict_sessions", "recommend_sessions", "corated_items_sessions", "recommend_users",
-           "corated_users", "explain_nodes", "NodeExplanation", "attribute_nodes", "NodeAttribution"]
+           "corated_users", "explain_nodes", "NodeExplanation", "attribute_nodes", "NodeAttribution", "predict_draws",
+           "Draws"]
 
 
 # ---- input validation (host) ----------------------------------------------------------------------------------------
@@ -622,6 +627,110 @@ def node_grad_scatter_host(node_ptr, edge_ptr, node_label, in_ptr, in_eid, tag, 
     return out
 
 
+# ---- Monte-Carlo-dropout draws (csrc/draws.cu) ----------------------------------------------------------------------
+# The result of predict_draws, device tensors: value [P, S] fp32 (draw s of pair p), mean [P] and std [P] fp32 (the
+# unbiased standard deviation over the S draws, 0 when S = 1).
+Draws = collections.namedtuple("Draws", "value mean std")
+
+DRAWS_HOP_TAG = 4    # sample_state's hop slot of the draw streams: side 0 the edges, side 1 the hidden units
+
+
+def _check_draw_seed(draw_seed):
+    if isinstance(draw_seed, (bool, np.bool_)) or not isinstance(draw_seed, (int, np.integer)):
+        raise TypeError("draw_seed must be an integer, not %s" % type(draw_seed).__name__)
+    if not 0 <= int(draw_seed) < 2 ** 64:
+        raise ValueError("draw_seed must lie in [0, 2^64), not %d" % int(draw_seed))
+    return int(draw_seed)
+
+
+def _draw_inputs(draws, beta, draw_seed, batch_size):
+    """None (``draws`` None: the eval scores) or dict(S, beta, draw_seed) of a run over draws, checked on the host:
+    ValueError for draws < 1, draws > batch_size (all draws of a pair share one batch), a non-finite beta, or beta
+    without draws; NotImplementedError above IGMC_DRAWS_MAX"""
+    beta = float(beta)
+    if not np.isfinite(beta):
+        raise ValueError("beta must be finite, not %r" % beta)
+    seed = _check_draw_seed(draw_seed)
+    if draws is None:
+        if beta != 0.0:
+            raise ValueError("beta= ranks by mean + beta * std over draws: pass draws= as well")
+        return None
+    S = _check_count(draws, "draws", _lib.DRAWS_MAX)
+    if S > int(batch_size):
+        raise ValueError("draws = %d exceed batch_size = %d: every draw of a pair runs in one batch" % (S, batch_size))
+    return dict(S=S, beta=beta, draw_seed=seed)
+
+
+def draws_expand_host(S, B, pair_u, pair_v, pair_pid, pair_tag):
+    """twin of igmc_draws_expand: (links_u, links_v, pair_id, tag, draw) [B] of the G = B // S pairs, S consecutive
+    draws each; positions G*S..B-1 copy pair 0 with tag -1 and draw 0"""
+    G = B // S
+    i = np.arange(B)
+    real = i < G * S
+    g = np.where(real, i // S, 0)
+    return (np.asarray(pair_u, np.int32)[g], np.asarray(pair_v, np.int32)[g], np.asarray(pair_pid, np.int64)[g],
+            np.where(real, np.asarray(pair_tag, np.int64)[g], -1), np.where(real, i - g * S, 0).astype(np.int32))
+
+
+def draw_states_host(draw_seed, pair_id, draw, side):
+    """the stream state of each draw: splitmix64(sample_state(draw_seed, pair_id, side, DRAWS_HOP_TAG) + draw), uint64"""
+    from oracle.extract_np import splitmix64
+    with np.errstate(over="ignore"):
+        tag = np.asarray(pair_id, np.int64).astype(np.uint64) * np.uint64(16) + np.uint64(DRAWS_HOP_TAG * 2 + side)
+        state = splitmix64(np.uint64(int(draw_seed)) ^ splitmix64(tag))
+        return splitmix64(state + np.asarray(draw, np.int64).astype(np.uint32).astype(np.uint64))
+
+
+def draws_mask_host(edge_ptr, pair_id, tag, draw, adj_dropout, draw_seed):
+    """twin of igmc_draws_mask: (edge_keep [edge_ptr[B]], hidden_keep [B * 128]) uint8.  Directed edge e of graph g is
+    kept iff the high 32 bits of splitmix64(edge state + (e - edge_ptr[g])) reach keep_thresh(adj_dropout), hidden unit
+    o iff those of splitmix64(hidden state + o) reach keep_thresh(0.5); a graph with tag < 0 keeps everything"""
+    from oracle.extract_np import splitmix64
+    from .models import _keep_threshold
+    edge_ptr = np.asarray(edge_ptr, np.int64)
+    B = len(edge_ptr) - 1
+    pad = np.asarray(tag, np.int64) < 0
+    se, sh = draw_states_host(draw_seed, pair_id, draw, 0), draw_states_host(draw_seed, pair_id, draw, 1)
+    g = np.repeat(np.arange(B), np.diff(edge_ptr))
+    local = (np.arange(edge_ptr[0], edge_ptr[-1]) - edge_ptr[g]).astype(np.uint64)
+    keep = np.ones(int(edge_ptr[-1]), np.uint8)
+    with np.errstate(over="ignore"):
+        ek = (splitmix64(se[g] + local) >> np.uint64(32)) >= np.uint64(_keep_threshold(adj_dropout))
+        hk = (splitmix64(sh[:, None] + np.arange(_lib.LIN1_OUT, dtype=np.uint64)[None]) >> np.uint64(32)) >= \
+            np.uint64(_keep_threshold(0.5))
+    keep[edge_ptr[0]:] = ek | pad[g]
+    return keep, (hk | pad[:, None]).reshape(-1).astype(np.uint8)
+
+
+def draws_stats_host(preds, K, B, S, beta=0.0):
+    """twin of igmc_draws_stats over one batch: (x [G, S], mean [G], std [G], key [G]) fp32 of its G = B // S pairs; x
+    the fp32 checkpoint means, the statistics in fp64 in draw order (Python floats: no fma), each rounded once"""
+    import math
+    preds = np.asarray(preds, np.float32).reshape(K, B)
+    x = preds[0].copy()
+    for q in range(1, K):
+        x = (x + preds[q]).astype(np.float32)
+    if K > 1:
+        x = (x / np.float32(K)).astype(np.float32)
+    G = B // S
+    x = x[:G * S].reshape(G, S)
+    out = np.zeros((3, G), np.float64)
+    for g in range(G):
+        total = 0.0
+        for v in x[g]:
+            total += float(v)
+        mean, sd = total / S, 0.0
+        if S > 1:
+            ss = 0.0
+            for v in x[g]:
+                d = float(v) - mean
+                ss += d * d
+            sd = math.sqrt(ss / (S - 1))
+        out[:, g] = (mean, sd, mean + float(beta) * sd)
+    mean, sd, key = out.astype(np.float32)
+    return x, mean, sd, key
+
+
 # ---- rating sessions (csrc/session.cu) ------------------------------------------------------------------------------
 def session_rows_host(host, shape, users, session, items, values):
     """numpy twin of igmc_session_plan + _apply: (row_ptr [S+1], col_idx, rating) of the merged session rows.  Restates
@@ -752,6 +861,7 @@ class InferenceEngine(object):
         eng.start_recommend(users, k)          # or start_pairs(users, items) / start_explain / start_attribute(users, items, m)
                                                # or start_recommend_users(items, k): per item its best users
                                                # or start_explain_nodes / start_attribute_nodes(users, items, m)
+                                               # or start_draws(users, items, S): S dropout draws per pair
         while eng.step():
             pass
         top_items, top_scores = eng.finish()   # (predict: scores; explain: an Explanation; attribute: an Attribution)
@@ -805,11 +915,14 @@ class InferenceEngine(object):
         self._grad_plans = {}        # the model's plan cache while a gradient pass forces the L2 plan
 
     # ---- one run: plan, prime, steps, finish --------------------------------------------------------------------
-    def start_recommend(self, users, k, items=None, exclude_rated=True, retrieve=None):
+    def start_recommend(self, users, k, items=None, exclude_rated=True, retrieve=None, draws=None, beta=0.0,
+                        draw_seed=0):
         """plan a ranking run (one host sync: the candidate total).  ``items``: one candidate list for every user, or
         a 2-D [U, width] array of per-user lists (-1 = empty slot); ``retrieve=M``: each user's M items with the most
-        bridges (``corated_items``) are its candidates.  Returns the number of candidate pairs."""
+        bridges (``corated_items``) are its candidates.  ``draws=S``: rank by mean + beta * std over S draws
+        (``recommend``).  Returns the number of candidate pairs."""
         g = self.graph
+        d = _draw_inputs(draws, beta, draw_seed, self.B)
         users = _host_ids(users, "users", g.num_users)
         k, m, cand, rows = _ranking_inputs(k, self.B, items, retrieve, len(users), g.num_items)
         slots = torch.from_numpy(users.astype(np.int32)).to(self.dev)
@@ -818,23 +931,29 @@ class InferenceEngine(object):
             rp = g.host["row_ptr"]
             return int((rp[users + 1] - rp[users]).sum())
         return self._plan_ranking(slots, k, m, cand, rows, exclude_rated, rated,
-                                  "igmc_corated_items", (C.byref(g._c), slots.data_ptr(), len(users)))
+                                  "igmc_corated_items", (C.byref(g._c), slots.data_ptr(), len(users)), draws=d)
 
-    def start_session_recommend(self, sessions, k, items=None, exclude_rated=True, retrieve=None):
+    def start_session_recommend(self, sessions, k, items=None, exclude_rated=True, retrieve=None, draws=None,
+                                beta=0.0, draw_seed=0):
         """plan a ranking run over the sessions (``recommend_sessions``): query slot s is session s, its candidates and
         rated items come from its session row.  Arguments as ``start_recommend``'s.  Returns the number of candidate
         pairs."""
+        d = _draw_inputs(draws, beta, draw_seed, self.B)
         sessions = self._session_slots(sessions)
         k, m, cand, rows = _ranking_inputs(k, self.B, items, retrieve, sessions.num_sessions, self.graph.num_items)
         return self._plan_ranking(sessions._slots, k, m, cand, rows, exclude_rated, lambda: sessions.nnz,
-                                  "igmc_corated_sessions", (C.byref(self.graph._c), C.byref(sessions._c)), sessions)
+                                  "igmc_corated_sessions", (C.byref(self.graph._c), C.byref(sessions._c)), sessions,
+                                  draws=d)
 
-    def start_recommend_users(self, items, k, users=None, exclude_rated=True, retrieve=None):
+    def start_recommend_users(self, items, k, users=None, exclude_rated=True, retrieve=None, draws=None, beta=0.0,
+                              draw_seed=0):
         """plan an item-side ranking run (``recommend_users``): per query item its best users.  ``users``: one
         candidate list for every item, or a 2-D [I, width] array of per-item lists (-1 = empty slot); ``retrieve=M``:
         each item's M users with the most bridges (``corated_users``).  The candidate kernels run on the graph's
-        transposed view.  Returns the number of candidate pairs."""
+        transposed view.  ``draws`` / ``beta`` / ``draw_seed`` as ``start_recommend``'s.  Returns the number of
+        candidate pairs."""
         g = self.graph
+        d = _draw_inputs(draws, beta, draw_seed, self.B)
         items = _host_ids(items, "items", g.num_items)
         k, m, cand, rows = _ranking_inputs(k, self.B, users, retrieve, len(items), g.num_users, "users")
         slots = torch.from_numpy(items.astype(np.int32)).to(self.dev)
@@ -843,20 +962,22 @@ class InferenceEngine(object):
             cp = g.host["col_ptr"]
             return int((cp[items + 1] - cp[items]).sum())
         return self._plan_ranking(slots, k, m, cand, rows, exclude_rated, rated,
-                                  "igmc_corated_users", (C.byref(g._ct), slots.data_ptr(), len(items)), by_item=True)
+                                  "igmc_corated_users", (C.byref(g._ct), slots.data_ptr(), len(items)), by_item=True,
+                                  draws=d)
 
     def _plan_ranking(self, slots, k, m, cand, rows, exclude_rated, rated, retriever, args, sessions=None,
-                      by_item=False):
+                      by_item=False, draws=None):
         """the plan of a ranking run over the query slots ``slots`` (int32, on the device) with ``_ranking_inputs``'
         (k, m, cand, rows): the candidate plan over every item or the list ``cand`` (``rated()``: the slots' summed row
         lengths, room for their rated positions in the list), or per-slot rows from ``rows`` or from the retriever entry
         ``retriever`` (leading arguments ``args``).  ``sessions``: the slots are these sessions.  ``by_item``: the
         slots are items and the candidates users - the plan runs on the graph's transposed view, whose rows are the
-        items' columns.  Returns the number of candidate pairs."""
+        items' columns.  ``draws``: ``_draw_inputs``' dict of a run ranked by draws.  Returns the number of candidate
+        pairs."""
         U, dev, g = int(slots.numel()), self.dev, self.graph
         run = dict(kind="recommend", U=U, k=k, version=g.version, sessions=sessions, users=slots, by_item=by_item,
                    top_s=torch.full((U, k), -float("inf"), dtype=torch.float32, device=dev),
-                   top_i=torch.full((U, k), -1, dtype=torch.int64, device=dev))
+                   top_i=torch.full((U, k), -1, dtype=torch.int64, device=dev), **self._draw_run(draws))
         self.run = run
         if U == 0 or (cand is not None and len(cand) == 0) or (rows is not None and rows.shape[1] == 0):
             run["P"] = 0
@@ -916,6 +1037,40 @@ class InferenceEngine(object):
         """plan a run over the explicit pairs (users[i], items[i]).  Returns their number."""
         users, items, _ = _host_pairs(self.graph.shape, users, items)
         return self._start_explicit("pairs", users, items)
+
+    def start_draws(self, users, items, draws, draw_seed=0):
+        """plan a run of ``draws`` Monte-Carlo-dropout draws of each explicit pair (users[i], items[i])
+        (``predict_draws``).  Returns the number of pairs."""
+        d = _draw_inputs(draws, 0.0, draw_seed, self.B)
+        users, items, _ = _host_pairs(self.graph.shape, users, items)
+        P, S, f32 = len(users), d["S"], dict(dtype=torch.float32, device=self.dev)
+        return self._start_explicit("draws", users, items, value=torch.empty(P, S, **f32),
+                                    mean=torch.empty(P, **f32), std=torch.empty(P, **f32), **self._draw_run(d))
+
+    def _draw_run(self, d):
+        """the run fields of a run over draws (``_draw_inputs``' dict d, or None: none), the slots' draw buffers
+        allocated: per slot the G pairs of a batch before their expansion, the draw index and the hidden mask"""
+        if d is None:
+            return {}
+        i32, i64 = dict(dtype=torch.int32, device=self.dev), dict(dtype=torch.int64, device=self.dev)
+        for s in self.slots:
+            if "draw" not in s:
+                s.update(gu=torch.zeros(self.B, **i32), gv=torch.zeros(self.B, **i32), gpid=torch.zeros(self.B, **i64),
+                         gtag=torch.zeros(self.B, **i64), draw=torch.zeros(self.B, **i32),
+                         hkeep=torch.ones(self.B * _lib.LIN1_OUT, dtype=torch.uint8, device=self.dev))
+        return dict(d, G=self.B // d["S"], keys=torch.empty(self.B, dtype=torch.float32, device=self.dev))
+
+    def _draw_masks(self):
+        """each slot's edge mask sized for the extractor's batch edge capacity, and its dropout descriptor: the
+        training-mode forward with both rates 0 and the slot's injected edge and hidden masks"""
+        self.extractor._sync_graph()
+        ecap = self.extractor._out_caps(self.B)[1]
+        for s in self.slots:
+            if s.get("keep") is None or s["keep"].numel() < ecap:
+                s["keep"] = torch.ones(ecap, dtype=torch.uint8, device=self.dev)
+            d = self.model.make_dropout(False)[0]
+            d.edge_keep, d.hidden_keep = s["keep"].data_ptr(), s["hkeep"].data_ptr()
+            s["drop"] = (d, [s["keep"], s["hkeep"]])
 
     # ---- rating sessions ----------------------------------------------------------------------------------------
     def _csr(self, run):
@@ -1191,7 +1346,10 @@ class InferenceEngine(object):
         run = self.run
         sessions = run.get("sessions")
         self.extractor.serve_sessions(sessions.max_row_deg if sessions is not None else 0)
-        run["steps"] = ((run["P"] if total is None else total) + self.B - 1) // self.B
+        per = run.get("G", self.B)      # pairs per batch: G on a run over draws
+        run["steps"] = ((run["P"] if total is None else total) + per - 1) // per
+        if run.get("S"):
+            self._draw_masks()
         run["done"] = 0
         self.graphs, self.eager_done = {}, set()
         self.cursor.zero_()
@@ -1212,6 +1370,16 @@ class InferenceEngine(object):
                                                      self.cursor.data_ptr(), self.B, s["u"].data_ptr(),
                                                      s["v"].data_ptr(), s["pid"].data_ptr(), s["tag"].data_ptr(),
                                                      s["j"].data_ptr(), err, _stream_ptr()), "igmc_occlusion_pairs")
+        elif run.get("S"):
+            # G pairs, then S consecutive draws of each over the B positions
+            _lib.check(self.lib.igmc_candidate_pairs(C.byref(self._csr(run)), C.byref(run["Cd"]),
+                                                     self.cursor.data_ptr(), run["G"], s["gu"].data_ptr(),
+                                                     s["gv"].data_ptr(), s["gpid"].data_ptr(), s["gtag"].data_ptr(),
+                                                     err, _stream_ptr()), "igmc_candidate_pairs")
+            _lib.check(self.lib.igmc_draws_expand(run["S"], self.B, s["gu"].data_ptr(), s["gv"].data_ptr(),
+                                                  s["gpid"].data_ptr(), s["gtag"].data_ptr(), s["u"].data_ptr(),
+                                                  s["v"].data_ptr(), s["pid"].data_ptr(), s["tag"].data_ptr(),
+                                                  s["draw"].data_ptr(), _stream_ptr()), "igmc_draws_expand")
         else:
             _lib.check(self.lib.igmc_candidate_pairs(C.byref(self._csr(run)), C.byref(run["Cd"]),
                                                      self.cursor.data_ptr(), self.B, s["u"].data_ptr(),
@@ -1237,6 +1405,12 @@ class InferenceEngine(object):
             _lib.check(getattr(self.lib, mask)(C.byref(b._lazy["_c"]), self.B, s["tag"].data_ptr(), s["j"].data_ptr(),
                                                s["keep"].data_ptr(), run["user"].data_ptr(), run["item"].data_ptr(),
                                                run["rating"].data_ptr(), err, _stream_ptr()), mask)
+        elif run.get("S"):
+            # the masks are keyed by the final (user, item) pair id: after the mapping kernels above
+            _lib.check(self.lib.igmc_draws_mask(C.byref(b._lazy["_c"]), self.B, s["pid"].data_ptr(),
+                                                s["tag"].data_ptr(), s["draw"].data_ptr(), float(self.model.adj_dropout),
+                                                run["draw_seed"], s["keep"].data_ptr(), s["hkeep"].data_ptr(),
+                                                _stream_ptr()), "igmc_draws_mask")
         elif run.get("phase") == "base":
             count, ptr = ("igmc_explain_node_count", "node_ptr") if nodes else ("igmc_explain_count", "edge_ptr")
             _lib.check(getattr(self.lib, count)(b._priv[ptr].data_ptr(), s["tag"].data_ptr(), self.B,
@@ -1264,7 +1438,7 @@ class InferenceEngine(object):
         if run.get("phase") in ("pgrad", "test", "train"):
             return self._pair_grad_step(slot)
         occlude = run.get("phase") == "occlude"
-        training, drop = (True, s["drop"]) if occlude else (False, self.drop)
+        training, drop = (True, s["drop"]) if occlude or run.get("S") else (False, self.drop)
         preds = None
         for j in range(self.K):
             with self._params(j):
@@ -1274,6 +1448,8 @@ class InferenceEngine(object):
             else:
                 self.preds[j].copy_(pred)
                 preds = self.preds
+        if run.get("S"):
+            return self._draw_stats(preds, s)
         if run["kind"] == "recommend":
             ranked = s["u"] if run.get("by_item") else s["v"]      # the candidates: users on an item-side run
             _lib.check(self.lib.igmc_topk_merge(preds.data_ptr(), self.K, self.B, s["tag"].data_ptr(),
@@ -1283,6 +1459,20 @@ class InferenceEngine(object):
             out = run["occ"] if occlude else run["scores"]
             _lib.check(self.lib.igmc_score_scatter(preds.data_ptr(), self.K, self.B, s["tag"].data_ptr(),
                                                    out.data_ptr(), _stream_ptr()), "igmc_score_scatter")
+
+    def _draw_stats(self, preds, s):
+        """a batch of draws: per pair its statistics scattered to the run's outputs, or (ranking) its key
+        mean + beta * std merged into the running top-k lists over the batch's G pairs"""
+        run, st = self.run, _stream_ptr()
+        rank = run["kind"] == "recommend"
+        outs = (None, None, None, run["keys"]) if rank else (run["value"], run["mean"], run["std"], None)
+        _lib.check(self.lib.igmc_draws_stats(preds.data_ptr(), self.K, self.B, run["S"], s["tag"].data_ptr(),
+                                             run["beta"], *(_lib.ptr(t) for t in outs), st), "igmc_draws_stats")
+        if rank:
+            # the candidates before the mapping kernels: items, or users on an item-side run
+            _lib.check(self.lib.igmc_topk_merge(run["keys"].data_ptr(), 1, run["G"], s["gtag"].data_ptr(),
+                                                s["gv"].data_ptr(), run["k"], run["top_s"].data_ptr(),
+                                                run["top_i"].data_ptr(), st), "igmc_topk_merge")
 
     def _gradient(self, slot):
         """per parameter set: the eval forward of batch ``slot`` on the L2 plan, (DGCNN_RS) the SortPooling backward
@@ -1372,6 +1562,8 @@ class InferenceEngine(object):
             return Influence(run["pro_i"], run["pro_v"], run["con_i"], run["con_v"])
         if run["kind"] == "self_influence":
             return run["self_out"]
+        if run["kind"] == "draws":
+            return Draws(run["value"], run["mean"], run["std"])
         return run["scores"]
 
     def _order(self, run):
@@ -1399,24 +1591,30 @@ class InferenceEngine(object):
         return _EXPLAIN_RESULTS[run["kind"]](run["scores"], run["num_edges"], run["offsets"], out["user"],
                                              out["item"], out["rating"], out["delta"])
 
-    def recommend(self, users, k, items=None, exclude_rated=True, retrieve=None):
-        self.start_recommend(users, k, items, exclude_rated, retrieve)
+    def recommend(self, users, k, items=None, exclude_rated=True, retrieve=None, draws=None, beta=0.0, draw_seed=0):
+        self.start_recommend(users, k, items, exclude_rated, retrieve, draws, beta, draw_seed)
         return self.finish()
 
-    def recommend_users(self, items, k, users=None, exclude_rated=True, retrieve=None):
-        self.start_recommend_users(items, k, users, exclude_rated, retrieve)
+    def recommend_users(self, items, k, users=None, exclude_rated=True, retrieve=None, draws=None, beta=0.0,
+                        draw_seed=0):
+        self.start_recommend_users(items, k, users, exclude_rated, retrieve, draws, beta, draw_seed)
         return self.finish()
 
     def predict_pairs(self, users, items):
         self.start_pairs(users, items)
         return self.finish()
 
+    def predict_draws(self, users, items, draws, draw_seed=0):
+        self.start_draws(users, items, draws, draw_seed)
+        return self.finish()
+
     def predict_sessions(self, sessions, session, items):
         self.start_session_pairs(sessions, session, items)
         return self.finish()
 
-    def recommend_sessions(self, sessions, k, items=None, exclude_rated=True, retrieve=None):
-        self.start_session_recommend(sessions, k, items, exclude_rated, retrieve)
+    def recommend_sessions(self, sessions, k, items=None, exclude_rated=True, retrieve=None, draws=None, beta=0.0,
+                           draw_seed=0):
+        self.start_session_recommend(sessions, k, items, exclude_rated, retrieve, draws, beta, draw_seed)
         return self.finish()
 
     def explain_pairs(self, users, items, m=None):
@@ -1481,6 +1679,26 @@ def predict_pairs(model, graph, users, items, *, h=1, sample_ratio=1.0, max_node
     if len(users) == 0:
         return torch.zeros(0, dtype=torch.float32, device=model.flat_params.device)
     return _on_engine(model, graph, lambda eng: eng.predict_pairs(users, items),
+                      h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
+
+
+def predict_draws(model, graph, users, items, draws, *, draw_seed=0, h=1, sample_ratio=1.0, max_nodes_per_hop=None,
+                  batch_size=256, checkpoints=None, sample_seed=0):
+    """``draws`` Monte-Carlo-dropout draws of the score of each pair (users[i], items[i]) and their statistics: a
+    ``Draws`` of value [P, S], mean [P] and std [P] fp32 on the model's device.  Draw s of a pair is the training-mode
+    forward of the subgraph ``predict_pairs`` scores, with each directed edge kept with probability 1 - adj_dropout
+    and each of the 128 hidden units before lin2 kept with probability 0.5 (and scaled by 2), IGMC and DGCNN_RS alike:
+    the dropout the model was trained with.  The masks are counter hashes of (draw_seed, u * num_items + v, s, the
+    edge's offset in its subgraph or the unit's index), so a draw depends on the parameters, the graph, the pair, s and
+    draw_seed only: not on the batch size, the batch position or the other pairs of the run.  ``checkpoints``: a draw
+    is the fp32 checkpoint mean under the same masks.  mean and std (unbiased, 0 for S = 1) are taken in fp64 in draw
+    order and rounded once; a NaN draw makes both NaN.  1 <= draws <= min(batch_size, IGMC_DRAWS_MAX = 256)."""
+    d = _draw_inputs(draws, 0.0, draw_seed, batch_size)
+    users, items, _ = _host_pairs(graph.shape, users, items)
+    if len(users) == 0:
+        dev = model.flat_params.device
+        return Draws(*(torch.zeros(shape, dtype=torch.float32, device=dev) for shape in ((0, d["S"]), (0,), (0,))))
+    return _on_engine(model, graph, lambda eng: eng.predict_draws(users, items, d["S"], d["draw_seed"]),
                       h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
 
 
@@ -1617,20 +1835,26 @@ def self_influence(model, graph, train, *, checkpoints=None, lrs=None, h=1, samp
                       h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
 
 
-def recommend(model, graph, users, k, *, items=None, exclude_rated=True, retrieve=None, h=1, sample_ratio=1.0,
-              max_nodes_per_hop=None, batch_size=256, checkpoints=None, sample_seed=0):
+def recommend(model, graph, users, k, *, items=None, exclude_rated=True, retrieve=None, draws=None, beta=0.0,
+              draw_seed=0, h=1, sample_ratio=1.0, max_nodes_per_hop=None, batch_size=256, checkpoints=None,
+              sample_seed=0):
     """for every query user the ``k`` best candidate items: (top_items [U, k] int64, top_scores [U, k] fp32), on the
     model's device.  Candidates: ``items`` (sorted, deduplicated), a 2-D ``items`` [U, width] of per-user lists (-1 =
     empty slot; each row sorted and deduplicated), the user's ``retrieve`` items with the most bridges
     (``corated_items``), or every item; minus the user's rated items when ``exclude_rated``.  Order: score
     descending, then item ascending; a NaN score ranks last; a user with fewer than ``k`` candidates gets item -1 /
-    score -inf in the empty slots.  A pair's score does not depend on the candidates it was ranked among."""
+    score -inf in the empty slots.  A pair's score does not depend on the candidates it was ranked among.
+    ``draws=S``: every candidate is ranked by its key mean + beta * std over S draws (``predict_draws``, seeded by
+    ``draw_seed``), and the returned scores are those keys: S = 1 is Thompson sampling (std = 0), beta > 0 UCB and
+    beta < 0 a risk-averse ranking.  ``draws=None`` ranks by the eval score."""
+    d = _draw_inputs(draws, beta, draw_seed, batch_size)
     users = _host_ids(users, "users", graph.shape[0])
     k = _ranking_inputs(k, batch_size, items, retrieve, len(users), graph.shape[1])[0]
     if len(users) == 0:
         dev = model.flat_params.device
         return (torch.zeros(0, k, dtype=torch.int64, device=dev), torch.zeros(0, k, dtype=torch.float32, device=dev))
-    return _on_engine(model, graph, lambda eng: eng.recommend(users, k, items, exclude_rated, retrieve),
+    return _on_engine(model, graph, lambda eng: eng.recommend(users, k, items, exclude_rated, retrieve, draws, beta,
+                                                              draw_seed),
                       h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
 
 
@@ -1655,8 +1879,9 @@ def corated_items(graph, users, m, exclude_rated=True):
     return items, paths
 
 
-def recommend_users(model, graph, items, k, *, users=None, exclude_rated=True, retrieve=None, h=1, sample_ratio=1.0,
-                    max_nodes_per_hop=None, batch_size=256, checkpoints=None, sample_seed=0):
+def recommend_users(model, graph, items, k, *, users=None, exclude_rated=True, retrieve=None, draws=None, beta=0.0,
+                    draw_seed=0, h=1, sample_ratio=1.0, max_nodes_per_hop=None, batch_size=256, checkpoints=None,
+                    sample_seed=0):
     """for every query item the ``k`` best candidate users - the audience of a new or promoted item: (top_users [I, k]
     int64, top_scores [I, k] fp32), on the model's device.  Candidates: ``users`` (sorted, deduplicated), a 2-D
     ``users`` [I, width] of per-item lists (-1 = empty slot), the item's ``retrieve`` users with the most bridges
@@ -1664,13 +1889,16 @@ def recommend_users(model, graph, items, k, *, users=None, exclude_rated=True, r
     user ascending; a NaN score ranks last; an item with fewer than ``k`` candidates gets user -1 / score -inf in the
     empty slots.  A pair's score is ``predict_pairs``' score of (u, v) bit for bit at the same batch size and kernel
     plan (pair id u * num_items + v): the lists filter those scores and compute nothing new.  An item added with
-    ``graph.update`` and a few ratings is ranked against every user without retraining."""
+    ``graph.update`` and a few ratings is ranked against every user without retraining.  ``draws`` / ``beta`` /
+    ``draw_seed``: ranked by mean + beta * std over draws, as in ``recommend``."""
+    _draw_inputs(draws, beta, draw_seed, batch_size)
     items = _host_ids(items, "items", graph.shape[1])
     k = _ranking_inputs(k, batch_size, users, retrieve, len(items), graph.shape[0], "users")[0]
     if len(items) == 0:
         dev = model.flat_params.device
         return (torch.zeros(0, k, dtype=torch.int64, device=dev), torch.zeros(0, k, dtype=torch.float32, device=dev))
-    return _on_engine(model, graph, lambda eng: eng.recommend_users(items, k, users, exclude_rated, retrieve),
+    return _on_engine(model, graph, lambda eng: eng.recommend_users(items, k, users, exclude_rated, retrieve, draws,
+                                                                    beta, draw_seed),
                       h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
 
 
@@ -1711,16 +1939,20 @@ def predict_sessions(model, sessions, session, items, *, h=1, sample_ratio=1.0, 
                       h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
 
 
-def recommend_sessions(model, sessions, k, *, items=None, exclude_rated=True, retrieve=None, h=1, sample_ratio=1.0,
-                       max_nodes_per_hop=None, batch_size=256, checkpoints=None, sample_seed=0):
+def recommend_sessions(model, sessions, k, *, items=None, exclude_rated=True, retrieve=None, draws=None, beta=0.0,
+                       draw_seed=0, h=1, sample_ratio=1.0, max_nodes_per_hop=None, batch_size=256, checkpoints=None,
+                       sample_seed=0):
     """per session the ``k`` best candidate items: (top_items [S, k] int64, top_scores [S, k] fp32), row s for
     session s.  Candidates and order as ``recommend``'s, with the session row as the user's ratings (``exclude_rated``,
     ``retrieve=M``); a 2-D ``items`` has one row per session.  Row s is bit for bit ``recommend`` for sessions.users[s]
-    on the graph with session s's edits applied (same kernel plan and batch size); the graph is not changed."""
+    on the graph with session s's edits applied (same kernel plan and batch size); the graph is not changed.
+    ``draws`` / ``beta`` / ``draw_seed``: ranked by mean + beta * std over draws, as in ``recommend``."""
+    _draw_inputs(draws, beta, draw_seed, batch_size)
     sessions = _check_sessions(sessions)
     k = _ranking_inputs(k, batch_size, items, retrieve, sessions.num_sessions, sessions.graph.num_items)[0]
     return _on_engine(model, sessions.graph,
-                      lambda eng: eng.recommend_sessions(sessions, k, items, exclude_rated, retrieve),
+                      lambda eng: eng.recommend_sessions(sessions, k, items, exclude_rated, retrieve, draws, beta,
+                                                         draw_seed),
                       h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
 
 

@@ -798,6 +798,41 @@ int igmc_online_draw(const igmc_csr_t* G, const int32_t* ring_u, const int32_t* 
                      uint64_t sample_seed, uint64_t drop_seed, int B, int32_t* links_u, int32_t* links_v, int32_t* label,
                      int64_t* pair_id, uint64_t* seeds, int* err, void* stream);
 
+/* ---- Monte-Carlo-dropout draws (csrc/draws.cu; igmc_b200/recommend.py: predict_draws, recommend(draws=S)) ----
+ * Draw s of pair (u, v) is a training-mode forward of the pair's enclosing subgraph with injected masks: each directed
+ * edge kept with probability 1 - adj_dropout (the model's rate), each of the 128 hidden units before lin2 kept with
+ * probability 0.5 and scaled by 2 (an injected hidden_keep stands for p = 0.5).  With pid = u * num_items + v, the
+ * masks of draw s are counter hashes
+ *   edges:  edge_keep(splitmix64(sample_state(draw_seed, pid, 0, 4) + s), e - edge_ptr[g], keep_thresh(adj_dropout))
+ *   hidden: edge_keep(splitmix64(sample_state(draw_seed, pid, 1, 4) + s), o, keep_thresh(0.5))
+ * (csrc/common.cuh, csrc/lists.cuh; hop slot 4 is used by neither extraction, hops 1..3, nor the online draw, hop 7).
+ * A draw depends on (parameters, graph, pair, s, draw_seed) only, never on a batch position.  A batch of B graphs holds
+ * G = B / S pairs times S consecutive draws, pair major; graphs G*S..B-1 are padding (tag -1).  The pair stream
+ * (igmc_candidate_pairs) runs with G slots per batch.  1 <= S <= IGMC_DRAWS_MAX and S <= B. */
+#define IGMC_DRAWS_MAX 256
+
+/* Position i < G*S of the batch: pair g = i / S of the G pairs pair_u / pair_v / pair_pid / pair_tag, draw i - g*S;
+ * positions G*S..B-1 copy pair 0 with tag -1 and draw 0.  Writes links_u / links_v / pair_id / tag / draw [B] for the
+ * mapping kernels (igmc_item_query_pairs, igmc_session_pairs), which run next on all B positions, and for
+ * igmc_extract_batch (idx = NULL). */
+int igmc_draws_expand(int S, int B, const int32_t* pair_u, const int32_t* pair_v, const int64_t* pair_pid,
+                      const int64_t* pair_tag, int32_t* links_u, int32_t* links_v, int64_t* pair_id, int64_t* tag,
+                      int32_t* draw, void* stream);
+
+/* For the batch O of B graphs extracted from those positions: edge_keep [O->edge_ptr[B]] and hidden_keep [B * 128] of
+ * graph g from pair_id[g] and draw[g] by the hashes above; a graph with tag < 0 keeps everything.  One CTA per graph.
+ * 0 <= adj_dropout <= 1 (else -2). */
+int igmc_draws_mask(const igmc_batch_out_t* O, int B, const int64_t* pair_id, const int64_t* tag, const int32_t* draw,
+                    float adj_dropout, uint64_t draw_seed, uint8_t* edge_keep, uint8_t* hidden_keep, void* stream);
+
+/* Per pair g < G = B / S of the batch: its draws x_s = the fp32 checkpoint mean of preds[.][g*S + s] (as
+ * igmc_topk_merge / igmc_score_scatter take it), then in fp64, in draw order and without fma contraction: mean = sum /
+ * S, std = sqrt(sum (x_s - mean)^2 / (S - 1)) (0 when S = 1) and key = mean + beta * std, each rounded once to fp32.
+ * A NaN draw makes all three NaN.  key != NULL: key [G] for every pair (igmc_topk_merge with K = 1 and B = G then
+ * consumes it).  Otherwise, for t = tag[g*S] >= 0: value[t * S + s] = x_s, mean[t], std[t].  beta finite (else -2). */
+int igmc_draws_stats(const float* preds, int K, int B, int S, const int64_t* tag, double beta, float* value,
+                     float* mean, float* std, float* key, void* stream);
+
 /* Version / build info: returns the compiled SM arch (90) so the host can refuse stale builds. */
 int igmc_build_info(void);
 
