@@ -32,6 +32,7 @@ ERR_NAMES = {
 
 TOPK_MAX = 256       # IGMC_TOPK_MAX
 DRAWS_MAX = 256      # IGMC_DRAWS_MAX
+COUNTERFACTUAL_MAX = 256   # IGMC_COUNTERFACTUAL_MAX
 
 # Kernel plan values (igmc_model_plan): 0 generic kernels, 1..4 relation-space cluster kernels (CTAs per subgraph),
 # PLAN_L2_BASE + c (c = 1, 2, 4, 8) the L2 plan with c CTAs per subgraph (IGMC_PLAN_L2 in include/igmc_b200.h).
@@ -127,6 +128,11 @@ class Candidates(C.Structure):
 class Sessions(C.Structure):
     _fields_ = [("users", vp), ("row_ptr", vp), ("col_idx", vp), ("rating", vp), ("num_sessions", C.c_int32),
                 ("max_row_deg", C.c_int32)]
+
+
+class Counterfactual(C.Structure):
+    _fields_ = [("users", vp), ("items", vp), ("rivals", vp), ("size", vp), ("removed", vp), ("num_query", C.c_int32),
+                ("max_removals", C.c_int32)]
 
 
 GRAPH_UPDATE_HEADER = ("nnz", "num_users", "num_items", "max_row_deg", "max_col_deg", "inserted", "changed",
@@ -236,6 +242,10 @@ _SIGS = {
     "igmc_draws_expand": [C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp],
     "igmc_draws_mask": [C.POINTER(BatchOut), C.c_int, vp, vp, vp, C.c_float, C.c_uint64, vp, vp, vp],
     "igmc_draws_stats": [vp, C.c_int, C.c_int, C.c_int, vp, C.c_double, vp, vp, vp, vp, vp],
+    "igmc_counterfactual_pairs": [C.POINTER(CSR), C.POINTER(Counterfactual), vp, C.c_int, vp, C.c_int, vp, vp, vp, vp,
+                                  vp, vp, vp, vp, C.c_int, vp, vp, vp],
+    "igmc_counterfactual_select": [C.POINTER(CSR), C.POINTER(Counterfactual), vp, vp, C.c_int, vp, vp, vp, vp, vp, vp,
+                                   vp, vp],
     "igmc_build_info": [],
     "igmc_model_plan": [C.POINTER(Model), C.c_int, C.c_int, C.c_int],
     "igmc_sortpool_plan": [C.POINTER(SortPool), C.c_int, C.c_int],

@@ -69,6 +69,28 @@ __device__ __forceinline__ float ckpt_mean(const float* __restrict__ preds, int 
   return K > 1 ? __fdiv_rn(a, (float)K) : a;
 }
 
+// Rank-skip search over ascending excluded positions r[0..n): the number t of them with r[q] - q <= c, so that the c-th
+// position not in r is c + t (r[q] - q counts the positions below r[q] that are not excluded, non-decreasing in q)
+__device__ __forceinline__ long long rank_skip(const int32_t* __restrict__ r, long long n, long long c) {
+  long long a = 0, b = n;
+  while (a < b) {
+    const long long mid = (a + b) >> 1;
+    if ((long long)r[mid] - mid <= c) a = mid + 1; else b = mid;
+  }
+  return a;
+}
+
+// the pair that owns position c of a run of per-pair positions: the last q in [0, P) with offsets[q] <= c (pairs
+// without positions share their offset with the next pair and own none)
+__device__ __forceinline__ int owner(const int64_t* __restrict__ offsets, int P, long long c) {
+  int lo = 0, hi = P;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (offsets[mid] <= c) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
 // ---- warp / block primitives -----------------------------------------------------------------
 __device__ __forceinline__ int warp_sum_i(int v) {
 #pragma unroll

@@ -63,17 +63,6 @@ k_explain_offsets(const int32_t* __restrict__ num_edges, long long P, int64_t* _
   if (threadIdx.x == 0) offsets[P] = carry;
 }
 
-// the pair that owns position c: the last q in [0, P) with offsets[q] <= c (pairs without edges share their offset
-// with the next pair and own no position)
-__device__ __forceinline__ int owner(const int64_t* __restrict__ offsets, int P, long long c) {
-  int lo = 0, hi = P;
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (offsets[mid] <= c) lo = mid; else hi = mid;
-  }
-  return lo;
-}
-
 __global__ void __launch_bounds__(PAIR_THREADS)
 k_occlusion_pairs(igmc_csr_t G, const int32_t* __restrict__ pair_u, const int32_t* __restrict__ pair_v,
                   const int64_t* __restrict__ offsets, int P, int64_t* __restrict__ cursor, int B,

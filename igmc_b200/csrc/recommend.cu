@@ -211,8 +211,7 @@ k_candidate_pairs(igmc_csr_t G, igmc_candidates_t Cd, int64_t* __restrict__ curs
       if (Cd.per_user) {
         p = Cd.user_off[lo] + c;    // the user's own list in cand; its rated items are already gone
       } else if (Cd.exclude_rated) {
-        // candidate rank c -> list position c + t, t = number of rated positions r_q with r_q - q <= c (r_q - q counts
-        // the unrated positions below r_q, non-decreasing in q)
+        // candidate rank c -> list position c + t, t = number of rated positions r_q with r_q - q <= c
         const int32_t* r;
         long long n;
         if (Cd.cand) {
@@ -222,12 +221,7 @@ k_candidate_pairs(igmc_csr_t G, igmc_candidates_t Cd, int64_t* __restrict__ curs
           r = G.col_idx + G.row_ptr[u];
           n = G.row_ptr[u + 1] - G.row_ptr[u];
         }
-        long long a = 0, b = n;
-        while (a < b) {
-          const long long mid = (a + b) >> 1;
-          if ((long long)r[mid] - mid <= c) a = mid + 1; else b = mid;
-        }
-        p = c + a;
+        p = c + rank_skip(r, n, c);
       }
       const long long lim = Cd.per_user ? P : Cd.cand ? Cd.num_cand : G.num_items;
       if (p < 0 || p >= lim) {

@@ -40,6 +40,10 @@ building a dataset of every candidate pair and looping over it in Python.  Here:
   training-mode forward under the model's own edge and hidden dropout, masks keyed by the pair id and the draw index)
   and their mean and std (csrc/draws.cu); ``recommend``, ``recommend_users`` and ``recommend_sessions`` with
   ``draws=S`` rank by mean + beta * std over S draws (Thompson sampling at S = 1, UCB for beta > 0);
+* ``counterfactual(model, graph, users, items, rivals, max_removals)`` -> per query (u, X, Y) the ratings of u whose
+  removal together puts X behind the rival Y, found greedily with every candidate scored exactly (csrc/counterfactual.cu):
+  a base pass, then per step one pass over every remaining rating of every active query, each trial extracted in
+  session mode with the user's row without its removals;
 * ``InferenceEngine``: the pipelined, graph-replayed loop behind all of them.  Per step the side stream produces the next
   batch's candidate pairs (``igmc_candidate_pairs``, from a device cursor) and extracts it while the main stream runs
   the eval forward of the current batch (once per checkpoint) and merges its scores into the running per-user top-k
@@ -65,7 +69,7 @@ __all__ = ["predict_pairs", "recommend", "corated_items", "explain_pairs", "Expl
            "Attribution", "pair_gradients", "influence", "self_influence", "Influence", "InferenceEngine",
            "RatingSessions", "predict_sessions", "recommend_sessions", "corated_items_sessions", "recommend_users",
            "corated_users", "explain_nodes", "NodeExplanation", "attribute_nodes", "NodeAttribution", "predict_draws",
-           "Draws"]
+           "Draws", "counterfactual", "Counterfactual"]
 
 
 # ---- input validation (host) ----------------------------------------------------------------------------------------
@@ -851,6 +855,162 @@ def _check_sessions(sessions, graph=None):
     return sessions
 
 
+# ---- counterfactual explanations (csrc/counterfactual.cu) -----------------------------------------------------------
+# The result of counterfactual, per query (u, X, Y): found [Q] bool (X ends behind Y), size [Q] int32 (|R|), items and
+# ratings [Q, max_removals] int32 (the removed items in greedy order and their labels, -1 past size), score and
+# rival_score [Q, max_removals + 1] fp32 (s(u, X) and s(u, Y) before any removal and after each, NaN past size).
+Counterfactual = collections.namedtuple("Counterfactual", "found size items ratings score rival_score")
+
+
+def _counterfactual_inputs(shape, users, items, rivals, max_removals):
+    """(users, items, rivals, max_removals) of a counterfactual run checked on the host: ids in range (IndexError),
+    equal lengths, items[q] != rivals[q] and max_removals >= 1 (ValueError), max_removals <= IGMC_COUNTERFACTUAL_MAX
+    (NotImplementedError)"""
+    M = _check_count(max_removals, "max_removals", _lib.COUNTERFACTUAL_MAX)
+    users, items, _ = _host_pairs(shape, users, items)
+    rivals = _host_ids(rivals, "rivals", shape[1])
+    if len(rivals) != len(items):
+        raise ValueError("items and rivals must have the same length (%d vs %d)" % (len(items), len(rivals)))
+    if np.any(items == rivals):
+        q = int(np.flatnonzero(items == rivals)[0])
+        raise ValueError("query %d names item %d as its own rival" % (q, int(items[q])))
+    return users, items, rivals, M
+
+
+def _no_counterfactual(Q, M, dev):
+    """the Counterfactual of Q queries before any pass: nothing found, nothing removed"""
+    i32 = dict(dtype=torch.int32, device=dev)
+    nan = dict(fill_value=float("nan"), dtype=torch.float32, device=dev)
+    return Counterfactual(torch.zeros(Q, dtype=torch.bool, device=dev), torch.zeros(Q, **i32),
+                          torch.full((Q, M), -1, **i32), torch.full((Q, M), -1, **i32), torch.full((Q, M + 1), **nan),
+                          torch.full((Q, M + 1), **nan))
+
+
+def counterfactual_pairs_host(row_ptr, col_idx, rating, num_items, users, items, rivals, removed, size, offsets, step,
+                              pos, B):
+    """twin of igmc_counterfactual_pairs for positions [pos, pos + B): ((links_u, links_v, pair_id, tag) [4, B] int64,
+    (row_users [B], row_ptr [B+1], row_col, row_rating)).  ``removed`` [Q, M]: R ascending in its first size[q]
+    entries"""
+    offsets = np.asarray(offsets, np.int64)
+    Q, P2 = len(offsets) - 1, 2 * int(offsets[-1])
+    out = np.zeros((4, B), np.int64)
+    cols, rats = [], []
+    for i in range(B):
+        p = pos + i
+        real = p < P2
+        if not real:
+            p = P2 - 1
+        trial = p >> 1
+        q = min(int(np.searchsorted(offsets, trial, side="right")) - 1, Q - 1)    # the last q with offsets[q] <= trial
+        u, v = int(users[q]), int(rivals[q] if p & 1 else items[q])
+        r0, deg = int(row_ptr[u]), int(row_ptr[u + 1] - row_ptr[u])
+        keep = np.ones(deg, bool)
+        keep[np.asarray(removed[q][:size[q]], np.int64)] = False
+        if step > 0:
+            keep[np.flatnonzero(keep)[trial - offsets[q]]] = False       # the candidate: the c-th position not in R
+        cols.append(np.asarray(col_idx, np.int32)[r0 + np.flatnonzero(keep)])
+        rats.append(np.asarray(rating, np.uint8)[r0 + np.flatnonzero(keep)])
+        out[:, i] = (u, v, u * num_items + v, p if real else -1)
+    rp = np.concatenate([[0], np.cumsum([len(c) for c in cols])]).astype(np.int32)
+    return out, (out[0].astype(np.int32), rp, np.concatenate(cols).astype(np.int32),
+                 np.concatenate(rats).astype(np.uint8))
+
+
+def counterfactual_select_host(row_ptr, col_idx, rating, users, items, rivals, offsets, scores, step, state):
+    """twin of igmc_counterfactual_select: ``state`` a dict of numpy arrays removed [Q, M] (ascending in its first
+    size[q] entries), size [Q], count [Q], found [Q], items / ratings [Q, M], score / rival_score [Q, M + 1], updated in
+    place.  ``scores`` [2T]: side s of trial t at 2t + s"""
+    offsets = np.asarray(offsets, np.int64)
+    scores = np.asarray(scores, np.float32)
+    M = state["removed"].shape[1]
+    for q in range(len(offsets) - 1):
+        o, n = int(offsets[q]), int(offsets[q + 1] - offsets[q])
+        if n == 0:
+            state["count"][q] = 0
+            continue
+        u, X, Y = int(users[q]), int(items[q]), int(rivals[q])
+        r0, deg, t = int(row_ptr[u]), int(row_ptr[u + 1] - row_ptr[u]), int(state["size"][q])
+        sx, sy = scores[2 * o:2 * (o + n):2], scores[2 * o + 1:2 * (o + n):2]
+        if step == 0:
+            state["score"][q, 0], state["rival_score"][q, 0] = sx[0], sy[0]
+            behind = _before(sy[0], Y, sx[0], X)
+            state["found"][q] = behind
+            state["count"][q] = 0 if behind else deg
+            continue
+        free = np.setdiff1d(np.arange(deg), state["removed"][q, :t])       # the candidates, ascending
+        flip = np.array([_before(b, Y, a, X) for a, b in zip(sx, sy)], bool)
+        margin = (sx - sy).astype(np.float32)
+        item = np.asarray(col_idx, np.int64)[r0 + free]
+        c = int(np.lexsort((item, np.where(np.isnan(margin), 0, margin), np.isnan(margin), ~flip))[0])
+        pos = int(free[c])
+        state["removed"][q, :t + 1] = np.sort(np.r_[state["removed"][q, :t], pos])
+        state["items"][q, t], state["ratings"][q, t] = item[c], int(rating[r0 + pos])
+        state["score"][q, t + 1], state["rival_score"][q, t + 1] = sx[c], sy[c]
+        state["size"][q] = t + 1
+        state["found"][q] = flip[c]
+        state["count"][q] = 0 if (flip[c] or t + 1 == M or deg == t + 1) else deg - t - 1
+    return state
+
+
+def counterfactual_host(row_ptr, col_idx, rating, users, items, rivals, max_removals, scorer):
+    """``counterfactual``'s greedy search restated on the host, one ``scorer`` call per step: scorer(users, deleted,
+    targets) -> fp32 [n], the score of (users[i], targets[i]) with users[i]'s ratings of the items deleted[i] (a list)
+    removed.  Returns a ``Counterfactual`` of numpy arrays."""
+    users, items, rivals = (np.asarray(a, np.int64).reshape(-1) for a in (users, items, rivals))
+    Q, M = len(users), int(max_removals)
+    col_idx = np.asarray(col_idx, np.int64)
+    found, size = np.zeros(Q, bool), np.zeros(Q, np.int32)
+    out_i, out_r = np.full((Q, M), -1, np.int32), np.full((Q, M), -1, np.int32)
+    score, rival = np.full((Q, M + 1), np.nan, np.float32), np.full((Q, M + 1), np.nan, np.float32)
+    R = [[] for _ in range(Q)]               # removed row positions, in greedy order
+    s = np.asarray(scorer(np.r_[users, users], [[]] * (2 * Q), np.r_[items, rivals]), np.float32)
+    score[:, 0], rival[:, 0] = s[:Q], s[Q:]
+    found[:] = [_before(s[Q + q], rivals[q], s[q], items[q]) for q in range(Q)]
+    deg = np.asarray(row_ptr, np.int64)[users + 1] - np.asarray(row_ptr, np.int64)[users]
+    active = [q for q in range(Q) if not found[q] and deg[q] > 0]
+    while active:
+        trials = []                          # (q, candidate position, deleted items)
+        for q in active:
+            r0 = int(row_ptr[users[q]])
+            for pos in range(int(deg[q])):
+                if pos not in R[q]:
+                    trials.append((q, pos, list(col_idx[r0 + np.array(R[q] + [pos], np.int64)])))
+        n = len(trials)
+        tu = np.array([users[q] for q, _, _ in trials] * 2, np.int64)
+        tt = np.r_[[items[q] for q, _, _ in trials], [rivals[q] for q, _, _ in trials]].astype(np.int64)
+        s = np.asarray(scorer(tu, [d for _, _, d in trials] * 2, tt), np.float32)
+        best = {}
+        for k, (q, pos, d) in enumerate(trials):
+            sx, sy = s[k], s[n + k]
+            m = np.float32(sx - sy)
+            key = (not _before(sy, rivals[q], sx, items[q]), bool(np.isnan(m)), 0.0 if np.isnan(m) else float(m),
+                   int(d[-1]))
+            if q not in best or key < best[q][0]:
+                best[q] = (key, pos, sx, sy)
+        for q in active:
+            key, pos, sx, sy = best[q]
+            t = len(R[q])
+            r0 = int(row_ptr[users[q]])
+            R[q].append(pos)
+            out_i[q, t], out_r[q, t] = col_idx[r0 + pos], int(rating[r0 + pos])
+            score[q, t + 1], rival[q, t + 1] = sx, sy
+            size[q], found[q] = t + 1, not key[0]
+        active = [q for q in active if not found[q] and size[q] < M and size[q] < deg[q]]
+    return Counterfactual(found, size, out_i, out_r, score, rival)
+
+
+class _TrialRows(object):
+    """one batch slot's trial rows of a counterfactual pass, and their igmc_sessions_t (``_c``): what
+    ``SubgraphExtractor.extract`` takes as ``sessions``"""
+
+    def __init__(self, users, row_ptr, col_idx, rating):
+        self.users, self.row_ptr, self.col_idx, self.rating = users, row_ptr, col_idx, rating
+        self.cap = int(col_idx.numel())
+        self.max_row_deg = 0
+        self._c = _lib.Sessions(users.data_ptr(), row_ptr.data_ptr(), col_idx.data_ptr(), rating.data_ptr(),
+                                int(users.numel()), 0)
+
+
 # ---- the engine -----------------------------------------------------------------------------------------------------
 class InferenceEngine(object):
     """Pipelined, graph-replayed scoring of candidate pairs (module docstring).  ``checkpoints``: state_dict files of
@@ -862,9 +1022,11 @@ class InferenceEngine(object):
                                                # or start_recommend_users(items, k): per item its best users
                                                # or start_explain_nodes / start_attribute_nodes(users, items, m)
                                                # or start_draws(users, items, S): S dropout draws per pair
+                                               # or start_counterfactual(users, items, rivals, max_removals)
         while eng.step():
             pass
-        top_items, top_scores = eng.finish()   # (predict: scores; explain: an Explanation; attribute: an Attribution)
+        top_items, top_scores = eng.finish()   # (predict: scores; explain: an Explanation; attribute: an Attribution;
+                                               # counterfactual: a Counterfactual)
 
     An engine serves across updates of its ``RatingGraph`` (``graph.update``) between runs; an update during a run
     makes its next ``step`` raise RuntimeError.
@@ -1126,6 +1288,75 @@ class InferenceEngine(object):
         users, items, _ = _host_pairs(self.graph.shape, users, items)
         return self._start_explicit("attribute_nodes", users, items, m=m, phase="base")
 
+    def start_counterfactual(self, users, items, rivals, max_removals=10):
+        """plan a counterfactual run (``counterfactual``) over the queries (users[q], items[q], rivals[q]): a base pass
+        scores each query's two pairs, then every trial pass scores each active query's trials (its row without R and
+        without one more position, the pairs (u, X) and (u, Y)) and igmc_counterfactual_select appends the best one
+        to R.  Each pass ends in one host sync (its trial total).  Returns the number of queries."""
+        g, dev = self.graph, self.dev
+        users, items, rivals, M = _counterfactual_inputs(g.shape, users, items, rivals, max_removals)
+        Q = len(users)
+        run = dict(kind="counterfactual", P=Q, version=g.version, M=M, step=0, row_deg=g.max_row_deg,
+                   out=_no_counterfactual(Q, M, dev), removed=torch.zeros(Q, M, dtype=torch.int32, device=dev),
+                   count=torch.ones(Q, dtype=torch.int32, device=dev),
+                   offsets=torch.zeros(Q + 1, dtype=torch.int64, device=dev))
+        self.run = run
+        if Q == 0:
+            return 0
+        run["pu"], run["px"], run["py"] = (torch.from_numpy(a.astype(np.int32)).to(dev) for a in (users, items, rivals))
+        run["Qd"] = _lib.Counterfactual(run["pu"].data_ptr(), run["px"].data_ptr(), run["py"].data_ptr(),
+                                        run["out"].size.data_ptr(), run["removed"].data_ptr(), Q, M)
+        self._trial_rows()
+        self._trial_pass()
+        return Q
+
+    def _trial_rows(self):
+        """each slot's trial rows: B rows of up to the graph's longest row, as the session rows igmc_extract_sessions
+        reads (session g of slot g is its trial row)"""
+        L = max(self.graph.max_row_deg, 1)
+        if self.B * L > 2 ** 31 - 1:
+            raise NotImplementedError("batch_size * the longest rating row = %d trial-row entries, beyond int32"
+                                      % (self.B * L))
+        i32 = dict(dtype=torch.int32, device=self.dev)
+        for s in self.slots:
+            t = s.get("trial")
+            if t is None or t.cap < self.B * L:
+                t = s["trial"] = _TrialRows(torch.zeros(self.B, **i32), torch.zeros(self.B + 1, **i32),
+                                            torch.zeros(self.B * L, **i32),
+                                            torch.zeros(self.B * L, dtype=torch.uint8, device=self.dev))
+            if "sess" not in s:
+                s["sess"] = torch.zeros(self.B, **i32)
+            t.max_row_deg = self.graph.max_row_deg
+            t._c.max_row_deg = t.max_row_deg
+
+    def _trial_pass(self):
+        """the next pass of a counterfactual run: the offsets of the queries' trial counts, their total T (the pass's
+        host sync) and its 2T positions primed.  Returns True when it has trials."""
+        run = self.run
+        _lib.check(self.lib.igmc_explain_offsets(run["count"].data_ptr(), run["P"], run["offsets"].data_ptr(),
+                                                 _stream_ptr()), "igmc_explain_offsets")
+        T = int(run["offsets"][run["P"]].item())
+        if T == 0:
+            run["steps"] = run["done"] = 0
+            return False
+        run["scores"] = torch.empty(2 * T, dtype=torch.float32, device=self.dev)
+        self._prime(2 * T)
+        return True
+
+    def _select_trials(self):
+        """after a pass of a counterfactual run: each query's best trial appended (igmc_counterfactual_select), then
+        the next pass.  Returns True when it has trials."""
+        run, out = self.run, self.run["out"]
+        _lib.check(self.lib.igmc_counterfactual_select(C.byref(self.graph._c), C.byref(run["Qd"]),
+                                                       run["offsets"].data_ptr(), run["scores"].data_ptr(),
+                                                       run["step"], run["count"].data_ptr(), out.found.data_ptr(),
+                                                       out.items.data_ptr(), out.ratings.data_ptr(),
+                                                       out.score.data_ptr(), out.rival_score.data_ptr(),
+                                                       self.extractor.err.data_ptr(), _stream_ptr()),
+                   "igmc_counterfactual_select")
+        run["step"] += 1
+        return self._trial_pass()
+
     def start_pair_gradients(self, users, items, y=None):
         """plan a per-pair gradient run (``pair_gradients``) over the explicit pairs: per checkpoint the gradient of
         l_i = (f_i - y_i)^2 (``y`` given) or of the score f_i into run["out"] [K, P, param_count].  Returns P."""
@@ -1345,7 +1576,9 @@ class InferenceEngine(object):
         ``total``: the positions of the pass (default: the run's pairs)."""
         run = self.run
         sessions = run.get("sessions")
-        self.extractor.serve_sessions(sessions.max_row_deg if sessions is not None else 0)
+        # session rows served: a session run's, or the trial rows of a counterfactual run (never longer than the
+        # graph's rows)
+        self.extractor.serve_sessions(sessions.max_row_deg if sessions is not None else run.get("row_deg", 0))
         per = run.get("G", self.B)      # pairs per batch: G on a run over draws
         run["steps"] = ((run["P"] if total is None else total) + per - 1) // per
         if run.get("S"):
@@ -1364,7 +1597,18 @@ class InferenceEngine(object):
         """candidate pairs of the next B positions (device cursor) + their extraction into batch slot ``slot``"""
         s, run, err = self.slots[slot], self.run, self.extractor.err.data_ptr()
         occlude = run.get("phase") == "occlude"
-        if occlude:
+        sessions = run.get("sessions")
+        if run["kind"] == "counterfactual":
+            # the trials' pairs, and per slot its trial row as session g, extracted in session mode
+            t = sessions = s["trial"]
+            _lib.check(self.lib.igmc_counterfactual_pairs(C.byref(self.graph._c), C.byref(run["Qd"]),
+                                                          run["offsets"].data_ptr(), run["step"], self.cursor.data_ptr(),
+                                                          self.B, s["u"].data_ptr(), s["v"].data_ptr(),
+                                                          s["pid"].data_ptr(), s["tag"].data_ptr(), t.users.data_ptr(),
+                                                          t.row_ptr.data_ptr(), t.col_idx.data_ptr(),
+                                                          t.rating.data_ptr(), t.cap, s["sess"].data_ptr(), err,
+                                                          _stream_ptr()), "igmc_counterfactual_pairs")
+        elif occlude:
             _lib.check(self.lib.igmc_occlusion_pairs(C.byref(self.graph._c), run["pu"].data_ptr(),
                                                      run["pv"].data_ptr(), run["offsets"].data_ptr(), run["P"],
                                                      self.cursor.data_ptr(), self.B, s["u"].data_ptr(),
@@ -1390,8 +1634,7 @@ class InferenceEngine(object):
             _lib.check(self.lib.igmc_item_query_pairs(self.graph.num_items, self.B, s["u"].data_ptr(),
                                                       s["v"].data_ptr(), s["pid"].data_ptr(), err, _stream_ptr()),
                        "igmc_item_query_pairs")
-        sessions = run.get("sessions")
-        if sessions is not None:
+        if run.get("sessions") is not None:
             # links_u holds the session: to the session's user id, its pair id and the per-pair session index
             _lib.check(self.lib.igmc_session_pairs(C.byref(sessions._c), self.graph.num_items, self.B,
                                                    s["u"].data_ptr(), s["v"].data_ptr(), s["pid"].data_ptr(),
@@ -1533,6 +1776,8 @@ class InferenceEngine(object):
         run["done"] += 1
         if run["done"] < run["steps"]:
             return True
+        if run["kind"] == "counterfactual":
+            return self._select_trials()
         if run.get("phase") == "test":
             return self._start_train_pass()
         if run.get("phase") != "base":
@@ -1564,6 +1809,8 @@ class InferenceEngine(object):
             return run["self_out"]
         if run["kind"] == "draws":
             return Draws(run["value"], run["mean"], run["std"])
+        if run["kind"] == "counterfactual":
+            return run["out"]
         return run["scores"]
 
     def _order(self, run):
@@ -1627,6 +1874,10 @@ class InferenceEngine(object):
 
     def explain_nodes(self, users, items, m=None):
         self.start_explain_nodes(users, items, m)
+        return self.finish()
+
+    def counterfactual(self, users, items, rivals, max_removals=10):
+        self.start_counterfactual(users, items, rivals, max_removals)
         return self.finish()
 
     def attribute_nodes(self, users, items, m=None):
@@ -1775,6 +2026,30 @@ def attribute_nodes(model, graph, users, items, m=None, *, h=1, sample_ratio=1.0
     if len(users) == 0:
         return _no_pairs_explained(NodeAttribution, m, model.flat_params.device)
     return _on_engine(model, graph, lambda eng: eng.attribute_nodes(users, items, m),
+                      h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
+
+
+def counterfactual(model, graph, users, items, rivals, max_removals=10, *, h=1, sample_ratio=1.0,
+                   max_nodes_per_hop=None, batch_size=256, checkpoints=None, sample_seed=0):
+    """which of user u's own ratings, removed together, put item X behind the rival item Y: per query (users[q],
+    items[q], rivals[q]) a greedy search over u's ratings with every candidate scored exactly.  s_R(u, v) is the eval
+    score of (u, v) on the graph with u's ratings of the items in R deleted (``predict_sessions`` on a session of u
+    that deletes R: same pair id, sample_seed and checkpoint mean); "X ahead of Y" is ``recommend``'s order (score
+    descending, item ascending, NaN last).  From R = {}: if X is not ahead of Y the answer has size 0.  Otherwise each
+    step scores the trial R + {i} for every item i of u's row not in R and adds the first by (trials that put X
+    behind Y first, then the margin s(u,X) - s(u,Y) (fp32) ascending with NaN after every number, then item
+    ascending).  The search stops when X is behind Y (found), when |R| = ``max_removals`` or when u's row has no item
+    left (not found; the path taken is still reported).  u's ratings of X and Y are candidates like any other; a pair's
+    own rating is never in its own subgraph, as in ``predict_pairs``.  Returns a ``Counterfactual`` of device
+    tensors: found [Q] bool, size [Q] int32, items / ratings [Q, max_removals] int32 (the removed items in greedy order
+    and their labels, -1 past size), score / rival_score [Q, max_removals + 1] fp32 (s(u, X) / s(u, Y) before any
+    removal and after each, NaN past size).  The results do not depend on batch_size, graph replay or the other
+    queries.  A step costs 2 (deg(u) - |R|) forwards per query; 1 <= max_removals <= IGMC_COUNTERFACTUAL_MAX = 256.
+    The graph is not changed."""
+    users, items, rivals, M = _counterfactual_inputs(graph.shape, users, items, rivals, max_removals)
+    if len(users) == 0:
+        return _no_counterfactual(0, M, model.flat_params.device)
+    return _on_engine(model, graph, lambda eng: eng.counterfactual(users, items, rivals, M),
                       h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
 
 

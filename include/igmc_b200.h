@@ -833,6 +833,49 @@ int igmc_draws_mask(const igmc_batch_out_t* O, int B, const int64_t* pair_id, co
 int igmc_draws_stats(const float* preds, int K, int B, int S, const int64_t* tag, double beta, float* value,
                      float* mean, float* std, float* key, void* stream);
 
+/* ---- counterfactual explanations (csrc/counterfactual.cu; igmc_b200/recommend.py: counterfactual) ----
+ * Query q = (u, X, Y): which of u's own ratings, removed together, put item X behind the rival Y in recommend's order
+ * (score descending, item ascending, NaN last)?  s_R(u, v) is the eval score of (u, v) on the graph with u's ratings at
+ * the row positions R deleted: the pair extracted in session mode (igmc_extract_sessions) with u's row without R as the
+ * target row, pair id u * num_items + v.  Greedy search from R = {}: pass 0 scores (u, X) and (u, Y) once; each later
+ * pass scores every trial R + {i}, i a position of u's row not in R, and keeps the first trial by (X behind Y first,
+ * then margin s(u,X) - s(u,Y) ascending with NaN after every number, then item ascending).  The search stops when X is
+ * behind Y, when |R| = max_removals or when u's row has no position left.  A pass covers 2T positions, T = offsets[Q]
+ * its trials (igmc_explain_offsets over count): position p is side p & 1 (0: X, 1: Y) of trial p >> 1. */
+#define IGMC_COUNTERFACTUAL_MAX 256
+typedef struct {
+  const int32_t* users;     /* [num_query] u */
+  const int32_t* items;     /* [num_query] X */
+  const int32_t* rivals;    /* [num_query] Y */
+  int32_t* size;            /* [num_query] |R| (0 before pass 1) */
+  int32_t* removed;         /* [num_query, max_removals] R as positions in u's row, ascending */
+  int32_t num_query, max_removals;
+} igmc_counterfactual_t;
+
+/* The pairs of positions [*cursor, *cursor + B), then *cursor += B (the igmc_candidate_pairs of a pass): position p
+ * belongs to trial p >> 1 of query q (the last q with offsets[q] <= p >> 1), whose candidate (step > 0) is c = (p >> 1)
+ * - offsets[q], the c-th position of u's row not in R.  Writes links_u = u, links_v = X or Y, pair_id = u * num_items +
+ * links_v, tag = p (positions past 2T repeat the last one with tag -1), and per slot g its trial row as the session
+ * rows igmc_extract_sessions reads with sess[g] = g: row_users[g] = u, row_ptr [B+1], and at [row_ptr[g],
+ * row_ptr[g+1]) u's graph row without R and (step > 0) without the candidate, ascending, into row_col / row_rating
+ * (row_cap entries; at most B * the longest graph row are needed).  Two launches.  Ids outside G, a candidate past the
+ * row or rows beyond row_cap set IGMC_ERR_CANDIDATES. */
+int igmc_counterfactual_pairs(const igmc_csr_t* G, const igmc_counterfactual_t* Q, const int64_t* offsets, int step,
+                              int64_t* cursor, int B, int32_t* links_u, int32_t* links_v, int64_t* pair_id,
+                              int64_t* tag, int32_t* row_users, int32_t* row_ptr, int32_t* row_col,
+                              uint8_t* row_rating, int row_cap, int32_t* sess, int* err, void* stream);
+
+/* One CTA per query q with trials in this pass (offsets[q+1] > offsets[q]), after the pass's scores are in
+ * trial_scores [2T] (igmc_score_scatter by tag).  step 0: score / rival_score [q, 0] = the trial's two scores, found[q]
+ * = X not ahead of Y.  step > 0: the query's first trial in the order above (a fixed-order block reduction) is
+ * appended: its position joins removed, its item and label go to out_item / out_rating [q, size], its scores to
+ * score / rival_score [q, size + 1], size += 1 and found[q] = X behind Y under it.  count[q] is the next pass's trial
+ * count: deg(u) - size, or 0 once found, size = max_removals or the row has no position left; 0 for a query without
+ * trials. */
+int igmc_counterfactual_select(const igmc_csr_t* G, const igmc_counterfactual_t* Q, const int64_t* offsets,
+                               const float* trial_scores, int step, int32_t* count, uint8_t* found, int32_t* out_item,
+                               int32_t* out_rating, float* score, float* rival_score, int* err, void* stream);
+
 /* Version / build info: returns the compiled SM arch (90) so the host can refuse stale builds. */
 int igmc_build_info(void);
 
