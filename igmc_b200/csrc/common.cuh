@@ -56,10 +56,13 @@ __host__ __device__ __forceinline__ uint32_t sample_key(uint64_t state, int node
   return (uint32_t)(splitmix64(state + (uint64_t)(uint32_t)node) >> 32);
 }
 
-// edge-dropout draw for directed edge `eid` of the current step: keep iff hash >= thresh
-// (thresh = p * 2^32).  Twin: igmc_b200/models.py::edge_keep_reference.
+// edge-dropout draw for directed edge `eid` of the current step: keep iff hash >= thresh (thresh = p * 2^32,
+// keep_thresh in csrc/lists.cuh).  thresh 0xFFFFFFFF is p >= 1 (an fp32 p < 1 gives at most 2^32 - 256) and keeps
+// nothing: the hash is clamped to 0xFFFFFFFE, which changes no compare against a smaller threshold (a separate test of
+// thresh would add spills to the train kernels; the clamp adds none).  Twin: igmc_b200/models.py::edge_keep_reference.
 __host__ __device__ __forceinline__ bool edge_keep(uint64_t seed, uint32_t eid, uint32_t thresh) {
-  return (uint32_t)(splitmix64(seed + (uint64_t)eid) >> 32) >= thresh;
+  const uint32_t h = (uint32_t)(splitmix64(seed + (uint64_t)eid) >> 32);
+  return (h < 0xFFFFFFFEu ? h : 0xFFFFFFFEu) >= thresh;
 }
 
 // fp32 mean of the K checkpoint predictions of batch entry i (preds row stride B), summed in checkpoint order

@@ -23,7 +23,8 @@ __host__ __device__ __forceinline__ int a4(int x) { return (x + 3) & ~3; }
 // ---- dropout draws of the step ---------------------------------------------------------------------------------
 constexpr uint32_t DROPPED = 0xFFFFFFFFu;
 
-// keep threshold p * 2^32 of a hash draw (p >= 1 drops everything).  Twin: igmc_b200/models.py::_keep_threshold.
+// keep threshold p * 2^32 of a hash draw, 0xFFFFFFFF for p >= 1, which edge_keep reads as "drop everything".  Twin:
+// igmc_b200/models.py::_keep_threshold.
 __device__ __forceinline__ uint32_t keep_thresh(float p) {
   const double t = (double)p * 4294967296.0;
   return t >= 4294967295.0 ? 0xFFFFFFFFu : (uint32_t)t;
@@ -49,8 +50,8 @@ __device__ __forceinline__ EdgeKeep make_keep(const igmc_dropout_t& D, int train
 }
 
 // F.dropout before lin2 (models.py:212): factor of unit o of graph g, 0 or 1/(1-p) in training, else 1.  The draw is
-// an edge_keep draw of index g*128 + o on the step seed ^ 0x5bd1e995a5a5a5a5 (twin: models.py::hidden_keep_reference);
-// an injected D.hidden_keep mask stands for p = 0.5.
+// an edge_keep draw of index g*128 + o on the step seed ^ 0x5bd1e995a5a5a5a5 (twin: models.py::hidden_keep_reference),
+// so p >= 1 keeps no unit and every factor is 0; an injected D.hidden_keep mask stands for p = 0.5.
 __device__ __forceinline__ float hidden_scale(const igmc_dropout_t& D, uint64_t seed, int training, int g, int o) {
   float scale = 1.f;
   if (training && (D.hidden_dropout > 0.f || D.hidden_keep)) {

@@ -38,9 +38,11 @@ def splitmix64(x):
 
 
 def _keep_threshold(p):
-    """Host twin of ``keep_thresh`` in csrc/lists.cuh: a draw keeps its unit iff hash >= p * 2^32 (clamped)."""
+    """Host twin of ``keep_thresh`` in csrc/lists.cuh and ``edge_keep``'s reading of it: a draw keeps its unit iff its
+    high 32 bits >= the returned p * 2^32, which is 2^32 (nothing kept) for p >= 1."""
     import numpy as np
-    return min(int(float(np.float32(p)) * 4294967296.0), 0xFFFFFFFF)   # the kernel sees p as fp32
+    t = float(np.float32(p)) * 4294967296.0   # the kernel sees p as fp32
+    return 1 << 32 if t >= 4294967295.0 else int(t)
 
 
 def edge_keep_reference(seed, num_edges, p):

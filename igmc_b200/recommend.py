@@ -687,8 +687,9 @@ def draw_states_host(draw_seed, pair_id, draw, side):
 
 def draws_mask_host(edge_ptr, pair_id, tag, draw, adj_dropout, draw_seed):
     """twin of igmc_draws_mask: (edge_keep [edge_ptr[B]], hidden_keep [B * 128]) uint8.  Directed edge e of graph g is
-    kept iff the high 32 bits of splitmix64(edge state + (e - edge_ptr[g])) reach keep_thresh(adj_dropout), hidden unit
-    o iff those of splitmix64(hidden state + o) reach keep_thresh(0.5); a graph with tag < 0 keeps everything"""
+    kept iff the high 32 bits of splitmix64(edge state + (e - edge_ptr[g])) reach keep_thresh(adj_dropout) (none at
+    adj_dropout = 1), hidden unit o iff those of splitmix64(hidden state + o) reach keep_thresh(0.5); a graph with tag
+    < 0 keeps everything"""
     from oracle.extract_np import splitmix64
     from .models import _keep_threshold
     edge_ptr = np.asarray(edge_ptr, np.int64)

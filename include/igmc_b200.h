@@ -806,6 +806,8 @@ int igmc_online_draw(const igmc_csr_t* G, const int32_t* ring_u, const int32_t* 
  *   edges:  edge_keep(splitmix64(sample_state(draw_seed, pid, 0, 4) + s), e - edge_ptr[g], keep_thresh(adj_dropout))
  *   hidden: edge_keep(splitmix64(sample_state(draw_seed, pid, 1, 4) + s), o, keep_thresh(0.5))
  * (csrc/common.cuh, csrc/lists.cuh; hop slot 4 is used by neither extraction, hops 1..3, nor the online draw, hop 7).
+ * edge_keep keeps iff the hash's high 32 bits reach the threshold, except that keep_thresh(1) = 0xFFFFFFFF keeps
+ * nothing: at adj_dropout = 1 every edge is dropped, as the probability 1 - adj_dropout says.
  * A draw depends on (parameters, graph, pair, s, draw_seed) only, never on a batch position.  A batch of B graphs holds
  * G = B / S pairs times S consecutive draws, pair major; graphs G*S..B-1 are padding (tag -1).  The pair stream
  * (igmc_candidate_pairs) runs with G slots per batch.  1 <= S <= IGMC_DRAWS_MAX and S <= B. */
