@@ -28,6 +28,8 @@ ERR_NAMES = {
     8: "graph update: a user / item id outside the graph's capacity or a value outside 0..256",
     9: "rating sessions: a session / item id out of range, a negative user id or a value outside 0..256",
     10: "online training draw: the rating graph has no ratings",
+    11: "extraction: a rating label or a pair label outside 0..num_classes-1 (more ratings than class_values / "
+        "the model's relations)",
 }
 
 TOPK_MAX = 256       # IGMC_TOPK_MAX

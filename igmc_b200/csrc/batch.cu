@@ -12,7 +12,9 @@ namespace {
 
 constexpr int BP_THREADS = 1024;
 
-// node_ptr[b] = first node with batch >= b ; edge_ptr[b] = first edge whose source lies in graph >= b
+// node_ptr[b] = first node with batch >= b ; edge_ptr[b] = first edge whose source lies in graph >= b.  A batch id
+// outside [0, B) or below its predecessor, and an edge source outside [0, N) or in a graph before its predecessor's,
+// set IGMC_ERR_BAD_BATCH (node_ptr / edge_ptr are then undefined).
 __global__ void k_batch_ptrs(const int64_t* __restrict__ batch, const int64_t* __restrict__ edge_src,
                              int N, int E, int B, int32_t* __restrict__ node_ptr,
                              int32_t* __restrict__ edge_ptr, int* err) {
@@ -20,7 +22,7 @@ __global__ void k_batch_ptrs(const int64_t* __restrict__ batch, const int64_t* _
   if (t < N) {
     const int64_t cur = batch[t];
     const int64_t prev = t == 0 ? -1 : batch[t - 1];
-    if (cur < prev || cur >= B) igmc_set_err(err, IGMC_ERR_BAD_BATCH);
+    if (cur < 0 || cur < prev || cur >= B) igmc_set_err(err, IGMC_ERR_BAD_BATCH);
     for (int64_t b = prev + 1; b <= cur && b < B; ++b) node_ptr[b] = t;
     if (t == N - 1)
       for (int64_t b = cur + 1; b <= B; ++b) node_ptr[b] = N;
@@ -45,7 +47,12 @@ __global__ void k_batch_ptrs(const int64_t* __restrict__ batch, const int64_t* _
 }
 
 // One direction of the adjacency of graph g.  key: node whose list the edge joins (dst for
-// incoming), nbr: the other endpoint.
+// incoming), nbr: the other endpoint.  An edge with an endpoint outside the graph or a type outside 0..255 (the 8-bit
+// type field of a list entry) sets IGMC_ERR_BAD_BATCH and joins no list.
+__device__ __forceinline__ bool edge_ok(int64_t k, int64_t o, int64_t type, int n) {
+  return k >= 0 && k < n && o >= 0 && o < n && type >= 0 && type <= 255;
+}
+
 __device__ void build_lists(const int64_t* __restrict__ key_row, const int64_t* __restrict__ nbr_row,
                             const int64_t* __restrict__ edge_type, int nb, int n, int eb, int ne,
                             int32_t* __restrict__ ptr_out, uint32_t* __restrict__ adj_out,
@@ -56,7 +63,7 @@ __device__ void build_lists(const int64_t* __restrict__ key_row, const int64_t* 
   __syncthreads();
   for (int e = tid; e < ne; e += nt) {
     const int64_t k = key_row[eb + e] - nb, o = nbr_row[eb + e] - nb;
-    if (k < 0 || k >= n || o < 0 || o >= n) { igmc_set_err(err, IGMC_ERR_BAD_BATCH); continue; }
+    if (!edge_ok(k, o, edge_type[eb + e], n)) { igmc_set_err(err, IGMC_ERR_BAD_BATCH); continue; }
     atomicAdd(&cnt[(int)k], 1);
   }
   __syncthreads();
@@ -69,10 +76,10 @@ __device__ void build_lists(const int64_t* __restrict__ key_row, const int64_t* 
   __syncthreads();
   // unordered placement; fill[v] ends at the list end
   for (int e = tid; e < ne; e += nt) {
-    const int64_t k = key_row[eb + e] - nb, o = nbr_row[eb + e] - nb;
-    if (k < 0 || k >= n || o < 0 || o >= n) continue;
+    const int64_t k = key_row[eb + e] - nb, o = nbr_row[eb + e] - nb, type = edge_type[eb + e];
+    if (!edge_ok(k, o, type, n)) continue;
     const int slot = atomicAdd(&fill[(int)k], 1);
-    tmp[eb + slot] = list_key((uint32_t)(edge_type[eb + e] & 0xff), (uint32_t)o, (uint32_t)e);
+    tmp[eb + slot] = list_key((uint32_t)type, (uint32_t)o, (uint32_t)e);
   }
   __syncthreads();
   // deterministic order: rank-sort every list by its key (lists are short: mean degree ~20)

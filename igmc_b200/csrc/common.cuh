@@ -19,6 +19,7 @@ enum {
   IGMC_ERR_GRAPH_UPDATE = 8,  // graph update: an id outside the capacity or a value outside 0..256
   IGMC_ERR_SESSIONS = 9,    // rating sessions: a session / item id out of range, a negative user or a value outside 0..256
   IGMC_ERR_ONLINE = 10,     // online training draw: the rating graph has no ratings
+  IGMC_ERR_LABEL = 11,      // extraction: a stored rating label or a pair label outside 0..num_classes-1
 };
 
 __device__ __forceinline__ void igmc_set_err(int* err, int code) {

@@ -188,6 +188,15 @@ __device__ __forceinline__ void resolve_pair(const igmc_pairs_t& P, int g, int* 
   *pid = P.pair_id ? P.pair_id[g] : src;
 }
 
+// A rating label (stored, or the pair's) as an index of class_values and of the model's relations: outside 0..R-1 it
+// sets IGMC_ERR_LABEL (when `who` is 0: callers pass their thread index to flag once per CTA) and reads as 0, so that
+// no later kernel indexes a relation table past R.
+__device__ __forceinline__ int checked_label(int lab, int R, int who, int* err) {
+  if ((unsigned)lab < (unsigned)R) return lab;
+  if (who == 0) igmc_set_err(err, IGMC_ERR_LABEL);
+  return 0;
+}
+
 // Session mode (igmc_extract_sessions, SESS = true): graph g takes its target user's row from session row sess[g];
 // every other row and column comes from G.  Plain mode passes an empty SessArg and never reads it.
 struct SessArg {
@@ -431,7 +440,7 @@ k_extract_fill(igmc_csr_t G, igmc_pairs_t P, int B, int cap,
                const int32_t* __restrict__ n_u, const int32_t* __restrict__ n_v,
                const int32_t* __restrict__ row_cnt, const int32_t* __restrict__ m_cnt,
                const int32_t* __restrict__ col_cnt, int h, const int32_t* __restrict__ hop_off,
-               const float* __restrict__ class_values, igmc_batch_out_t O, int* err, SessArg A) {
+               const float* __restrict__ class_values, int R, igmc_batch_out_t O, int* err, SessArg A) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   int* rowoff = reinterpret_cast<int*>(smem_raw);                 // [cap]
   int* colfill = rowoff + cap;                                    // [cap] running fill pointer of the item lists
@@ -449,6 +458,7 @@ k_extract_fill(igmc_csr_t G, igmc_pairs_t P, int B, int cap,
   int i, j, lab;
   int64_t pid;
   resolve_pair(P, g, &i, &j, &lab, &pid);
+  lab = checked_label(lab, R, tid, err);
   if (tid == 0) {
     O.y[g] = class_values[lab];
     O.graph_nu[g] = nu;
@@ -542,7 +552,7 @@ k_extract_fill(igmc_csr_t G, igmc_pairs_t P, int B, int cap,
       }
       if (match) {
         const int rank = isj ? 0 : (h > 1 ? jfirst + hrank : jfirst + seen + __popc(bal & lt_mask));
-        const int64_t r = rt[p];
+        const int64_t r = checked_label(rt[p], R, 0, err);
         const size_t e1 = (size_t)2 * Mbase + base + rank, e2 = e1 + m;
         const int64_t un = Nbase + a, vn = Nbase + nu + b;
         ei0[e1] = un; ei1[e1] = vn; O.edge_type[e1] = r;
@@ -676,6 +686,7 @@ k_extract_fast(igmc_csr_t G, igmc_pairs_t P, int B, int mnph, double ratio, uint
   int i, j, lab;
   int64_t pid;
   resolve_pair(P, g, &i, &j, &lab, &pid);
+  lab = checked_label(lab, R, tid, err);
   const UserRows<SESS> rows = user_rows<SESS>(G, A, g);
   int32_t* gu = W.nodes_u + (size_t)g * cap;
   int32_t* gv = W.nodes_v + (size_t)g * cap;
@@ -745,7 +756,7 @@ k_extract_fast(igmc_csr_t G, igmc_pairs_t P, int B, int mnph, double ratio, uint
         uint32_t r = 0;
         if (match) {
           r = rat[u];
-          if ((int)r >= R) { igmc_set_err(err, IGMC_ERR_BAD_BATCH); r = 0; }   // label outside class_values
+          r = checked_label((int)r, R, 0, err);
           atomicAdd(&S.rowcnt[ar[u]], 1);
           atomicOr(&S.bm[((size_t)b * R + r) * words + (ar[u] >> 5)], 1u << (ar[u] & 31));
           if (b == 0) S.hj[ar[u]] = 1 | (int)(r << 8);
@@ -1064,7 +1075,7 @@ int launch_extract(const ExtractArgs& X, int max_row_deg, cudaStream_t st) {
   IGMC_CUDA_CHECK_LAUNCH();
   k_extract_fill<SESS><<<X.B, threads, pl.smemB, st>>>(X.G, X.P, X.B, X.cap, W.nodes_u, W.nodes_v, W.n_u, W.n_v,
                                                         W.row_cnt, W.m_cnt, W.col_cnt, X.h, W.hop_off, X.class_values,
-                                                        X.O, X.err, X.A);
+                                                        X.R, X.O, X.err, X.A);
   IGMC_CUDA_CHECK_LAUNCH();
   return 0;
 }

@@ -411,6 +411,7 @@ class IGMC(nn.Module):
         """Build the list images of ``batch`` for the forward (and, when training, backward) kernel of its plan and
         attach them to the batch.  ``drop`` must be the dropout descriptor the step will use (same seed source).
         No-op for the generic and L2 plans."""
+        self._check_types(batch)
         cl = self._plan(batch)
         if not _lib.is_rs(cl):
             batch._stage = None
@@ -570,6 +571,16 @@ class IGMC(nn.Module):
                                         _stream_ptr()), "igmc_grad_reduce")
 
     # ---- public API ------------------------------------------------------------------------------------------
+    def _check_types(self, batch):
+        """IndexError unless every edge type of a foreign batch lies in [0, num_relations): the kernels index the
+        relation tables with it (PyG's RGCNConv fails in index_select).  Foreign batches and batches assembled from a
+        StaticStore carry the range; extracted batches are checked by the extractor (IGMC_ERR_LABEL)."""
+        tr = batch._priv.get("type_range")
+        if tr is not None and (tr[0] < 0 or tr[1] >= self.num_relations):
+            bad = tr[0] if tr[0] < 0 else tr[1]
+            raise IndexError("edge type %d outside the model's %d relations (types must lie in [0, %d))"
+                             % (bad, self.num_relations, self.num_relations))
+
     def _as_batch(self, data):
         if isinstance(data, Batch):
             return data
@@ -580,6 +591,7 @@ class IGMC(nn.Module):
 
     def forward(self, data, edge_keep=None, hidden_keep=None):
         batch = self._as_batch(data)
+        self._check_types(batch)
         drop = self.make_dropout(self.training, edge_keep, hidden_keep)
         need_grad = torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())
         if need_grad:
@@ -597,6 +609,7 @@ class IGMC(nn.Module):
     def _train_launches(self, batch, global_num_graphs, edge_keep, hidden_keep, seed_dev, one_launch):
         """the step's forward + loss + backward launches; ``one_launch`` allows igmc_forward_backward where the plan
         has it.  Returns (saved, G)."""
+        self._check_types(batch)
         self._step += 1
         drop = self.make_dropout(True, edge_keep, hidden_keep, seed_dev=seed_dev)
         G = batch.num_graphs if global_num_graphs is None else int(global_num_graphs)

@@ -113,6 +113,11 @@ class TrainEngine(object):
     LOSS_RING = 1024          # per-step losses the host can read back late (power of two)
 
     def __init__(self, dataset, model, optimizer, batch_size, ARR=0.0, use_graph=True, sample_seed=0):
+        cv = getattr(getattr(dataset, "extractor", None), "class_values", None)
+        if cv is not None and len(cv) > model.num_relations:
+            # a rating label is an edge type: labels past the model's relations would index its tables out of range
+            raise ValueError("%d class values for a model of %d relations: the rating labels must be edge types "
+                             "[0, %d)" % (len(cv), model.num_relations, model.num_relations))
         self.dataset, self.model, self.opt = dataset, model, optimizer
         self.B, self.ARR = int(batch_size), float(ARR)
         self.rank, self.world = _dist_info()

@@ -462,7 +462,9 @@ class Batch(Data):
     # ---- foreign batches (PyG-collated tensors from anywhere) ------------------------------------
     @staticmethod
     def from_arrays(x, edge_index, edge_type, batch, y, num_graphs=None, device=None):
-        """Wrap already-collated arrays (e.g. the oracle's) and derive graph offsets on the GPU."""
+        """Wrap already-collated arrays (e.g. the oracle's) and derive graph offsets on the GPU.  Records the range of
+        the edge types (``_priv["type_range"]``, None without edges), which the models compare with their relation
+        count before they launch anything on the batch."""
         device = _require_cuda(device)
         lib = _lib.load()
         x = torch.as_tensor(x, dtype=torch.float32).to(device).contiguous()
@@ -482,10 +484,15 @@ class Batch(Data):
         _lib.check(lib.igmc_batch_ptrs(batch.data_ptr() if N else None, src.data_ptr(), N, E, B,
                                        node_ptr.data_ptr(), edge_ptr.data_ptr(), err.data_ptr(), _stream_ptr()),
                    "igmc_batch_ptrs")
-        n_max = int((node_ptr[1:] - node_ptr[:-1]).max().item()) if B else 0
+        # the largest graph and the edge-type range in one device-to-host copy
+        zero = torch.zeros(1, dtype=torch.int64, device=device)
+        stats = torch.cat([(node_ptr[1:] - node_ptr[:-1]).max().long().view(1) if B else zero,
+                           edge_type.min().view(1) if E else zero, edge_type.max().view(1) if E else zero]).tolist()
+        n_max = stats[0]
         b._err = err
         b._priv = dict(node_label=lab, node_ptr=node_ptr, edge_ptr=edge_ptr, node_cap=max(N, 1),
-                       edge_cap=max(E, 1), n_cap=max(n_max, 2), symmetric=0, edge_row_stride=E)
+                       edge_cap=max(E, 1), n_cap=max(n_max, 2), symmetric=0, edge_row_stride=E,
+                       type_range=(stats[1], stats[2]) if E else None)
         b.__dict__["node_label"] = lab
         b.check()
         return b
@@ -916,6 +923,9 @@ class StaticStore(_BatchWriter):
         ei, et = edge_index.to(dev).long(), edge_type.to(dev).long()
         noff, eoff = node_off.to(dev).long(), edge_off.to(dev).long()
         G = int(y.numel())
+        if et.numel() and (int(et.min()) < 0 or int(et.max()) > 255):
+            raise ValueError("edge types must lie in 0..255 (the stored type is one byte), got %d..%d"
+                             % (int(et.min()), int(et.max())))
         if int(x.shape[1]) != self.feat_dim:
             raise ValueError("cached node features have width %d, expected %d (hop mismatch)" % (x.shape[1], feat_dim))
         ncnt, ecnt = noff[1:] - noff[:-1], eoff[1:] - eoff[:-1]
@@ -972,6 +982,10 @@ class StaticStore(_BatchWriter):
         self.num_graphs = num_graphs
         self.max_n = int(cat["ncnt"].max()) if num_graphs else 2
         self.max_e = int(cat["ecnt"].max()) if num_graphs else 2
+        et = cat["edge_type"]
+        # every batch assembled from the store carries the store's edge-type range: the models compare it with their
+        # relation count before they launch (Batch.from_arrays records the same for foreign batches)
+        self.type_range = tuple(torch.stack([et.min(), et.max()]).long().tolist()) if et.numel() else None
         self.cap = (self.max_n + 1) // 2 + 1          # n_cap = 2*cap >= max_n (the model plans by 2*cap)
         self.err = torch.zeros(1, dtype=torch.int32, device=dev)
         self._c = _lib.Store(self.node_off.data_ptr(), self.edge_off.data_ptr(),
@@ -989,7 +1003,9 @@ class StaticStore(_BatchWriter):
         o = self._alloc_out(B, reuse, slot)
         _lib.check(self.lib.igmc_assemble_batch(C.byref(self._c), idx.data_ptr(), B, C.byref(o["_c"]),
                                                 self.err.data_ptr(), _stream_ptr()), "igmc_assemble_batch")
-        return self._batch(B, o, [idx])
+        b = self._batch(B, o, [idx])
+        b._priv["type_range"] = self.type_range
+        return b
 
 
 class MyDataset(MyDynamicDataset):

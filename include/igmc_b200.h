@@ -30,7 +30,7 @@ extern "C" {
 typedef struct {
   const int32_t* row_ptr;   /* [num_users+1] */
   const int32_t* col_idx;   /* [nnz] ascending within a row */
-  const uint8_t* rating;    /* [nnz] rating label 0..R-1 */
+  const uint8_t* rating;    /* [nnz] rating label 0..R-1 (the extractors flag IGMC_ERR_LABEL on a label >= R) */
   const int32_t* col_ptr;   /* [num_items+1] */
   const int32_t* row_idx;   /* [nnz] ascending within a column */
   int32_t num_users, num_items;
@@ -91,7 +91,8 @@ typedef struct {
  * node lists [B*cap] (test hook: the reference's own random.sample draw; h = 1 only).  `seed_dev` (optional, device) overrides `seed` so that a
  * captured CUDA graph can be replayed with a fresh sampling stream every step.
  * `num_classes` = len(class_values), `max_row_deg` = the longest user row of G (0 = unknown): with W->sync set they
- * let h = 1 batches take the one-launch path (single balanced row scan, look-back offsets; same outputs bit for bit). */
+ * let h = 1 batches take the one-launch path (single balanced row scan, look-back offsets; same outputs bit for bit).
+ * A stored rating label or a pair label outside 0..num_classes-1 sets IGMC_ERR_LABEL and is written as 0. */
 int igmc_extract_batch(const igmc_csr_t* G, const igmc_pairs_t* P, int B, int h, int max_nodes_per_hop,
                        double sample_ratio, uint64_t seed, const uint64_t* seed_dev, int cap,
                        const int32_t* inj_nodes_u, const int32_t* inj_nodes_v,
@@ -131,7 +132,9 @@ int igmc_assemble_batch(const igmc_store_t* S, const int64_t* idx, int B, const 
                         void* stream);
 
 /* Graph offsets of a foreign (PyG-collated) batch: node_ptr from `batch`, edge_ptr from the graph
- * of each edge's source.  Replaces what Batch.from_data_list knows implicitly. */
+ * of each edge's source.  Replaces what Batch.from_data_list knows implicitly.  Sets IGMC_ERR_BAD_BATCH when a batch
+ * id lies outside [0, B) or below the previous node's, or an edge's source lies outside [0, N) or in a graph before
+ * the previous edge's; node_ptr and edge_ptr are then undefined (do not pass them to igmc_batch_prepare). */
 int igmc_batch_ptrs(const int64_t* batch, const int64_t* edge_src, int N, int E, int B,
                     int32_t* node_ptr, int32_t* edge_ptr, int* err, void* stream);
 
@@ -151,6 +154,11 @@ typedef struct {
   int32_t symmetric;
 } igmc_adj_t;
 
+/* One CTA per graph, with 2 (n_cap + 1) ints of shared memory: returns -3 when that exceeds 200 KB.  A graph of more
+ * than min(n_cap, 65535) nodes sets IGMC_ERR_SMEM_NODES and gets no lists.  An edge with an endpoint outside its
+ * source's graph, or a type outside 0..255, sets IGMC_ERR_BAD_BATCH and joins no list (the lists of that graph then
+ * leave slots unwritten).  The entry point does not know the model's relation count: types in [R, 256) are the
+ * caller's to refuse (Batch.from_arrays records the type range; the models raise before any launch). */
 int igmc_batch_prepare(const int64_t* edge_index, int64_t edge_row_stride, const int64_t* edge_type,
                        const int32_t* node_ptr, const int32_t* edge_ptr, int B, int n_cap,
                        const igmc_adj_t* A, int* err, void* stream);
