@@ -248,6 +248,9 @@ _SIGS = {
                                   vp, vp, vp, vp, C.c_int, vp, vp, vp],
     "igmc_counterfactual_select": [C.POINTER(CSR), C.POINTER(Counterfactual), vp, vp, C.c_int, vp, vp, vp, vp, vp, vp,
                                    vp, vp],
+    "igmc_elicit_pairs": [C.POINTER(Sessions), C.c_int, C.c_int, vp, C.c_int, C.c_int, vp, vp, vp, C.c_int, vp, vp, vp,
+                          vp, vp, vp, vp, vp, C.c_int, vp, vp, vp],
+    "igmc_elicit_stats": [vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp],
     "igmc_build_info": [],
     "igmc_model_plan": [C.POINTER(Model), C.c_int, C.c_int, C.c_int],
     "igmc_sortpool_plan": [C.POINTER(SortPool), C.c_int, C.c_int],

@@ -44,6 +44,11 @@ building a dataset of every candidate pair and looping over it in Python.  Here:
   removal together puts X behind the rival Y, found greedily with every candidate scored exactly (csrc/counterfactual.cu):
   a base pass, then per step one pass over every remaining rating of every active query, each trial extracted in
   session mode with the user's row without its removals;
+* ``elicit(model, sessions, n, targets)`` -> per session the ``n`` items it should be asked to rate: every answer to
+  every question scored exactly (the session's row plus the hypothetical rating, extracted in session mode), ranked by
+  the mean over ``targets`` of how far the answers move each target's score (csrc/elicit.cu);
+  ``question_impact(model, sessions, session, questions, targets)`` -> that impact and the mean target score under
+  each answer for explicit (session, question) units;
 * ``InferenceEngine``: the pipelined, graph-replayed loop behind all of them.  Per step the side stream produces the next
   batch's candidate pairs (``igmc_candidate_pairs``, from a device cursor) and extracts it while the main stream runs
   the eval forward of the current batch (once per checkpoint) and merges its scores into the running per-user top-k
@@ -69,7 +74,7 @@ __all__ = ["predict_pairs", "recommend", "corated_items", "explain_pairs", "Expl
            "Attribution", "pair_gradients", "influence", "self_influence", "Influence", "InferenceEngine",
            "RatingSessions", "predict_sessions", "recommend_sessions", "corated_items_sessions", "recommend_users",
            "corated_users", "explain_nodes", "NodeExplanation", "attribute_nodes", "NodeAttribution", "predict_draws",
-           "Draws", "counterfactual", "Counterfactual"]
+           "Draws", "counterfactual", "Counterfactual", "elicit", "question_impact", "QuestionImpact"]
 
 
 # ---- input validation (host) ----------------------------------------------------------------------------------------
@@ -707,16 +712,22 @@ def draws_mask_host(edge_ptr, pair_id, tag, draw, adj_dropout, draw_seed):
     return keep, (hk | pad[:, None]).reshape(-1).astype(np.uint8)
 
 
-def draws_stats_host(preds, K, B, S, beta=0.0):
-    """twin of igmc_draws_stats over one batch: (x [G, S], mean [G], std [G], key [G]) fp32 of its G = B // S pairs; x
-    the fp32 checkpoint means, the statistics in fp64 in draw order (Python floats: no fma), each rounded once"""
-    import math
+def _ckpt_mean_host(preds, K, B):
+    """the fp32 checkpoint mean [B] of preds [K, B] (ckpt_mean in csrc/common.cuh): fp32 sum in checkpoint order / K"""
     preds = np.asarray(preds, np.float32).reshape(K, B)
     x = preds[0].copy()
     for q in range(1, K):
         x = (x + preds[q]).astype(np.float32)
     if K > 1:
         x = (x / np.float32(K)).astype(np.float32)
+    return x
+
+
+def draws_stats_host(preds, K, B, S, beta=0.0):
+    """twin of igmc_draws_stats over one batch: (x [G, S], mean [G], std [G], key [G]) fp32 of its G = B // S pairs; x
+    the fp32 checkpoint means, the statistics in fp64 in draw order (Python floats: no fma), each rounded once"""
+    import math
+    x = _ckpt_mean_host(preds, K, B)
     G = B // S
     x = x[:G * S].reshape(G, S)
     out = np.zeros((3, G), np.float64)
@@ -1000,9 +1011,162 @@ def counterfactual_host(row_ptr, col_idx, rating, users, items, rivals, max_remo
     return Counterfactual(found, size, out_i, out_r, score, rival)
 
 
+# ---- question impact for rating sessions (csrc/elicit.cu) -----------------------------------------------------------
+# The result of question_impact, per unit (session, question): impact [P] fp32 (the mean over the targets of the range
+# of their scores over the answers) and answer_mean [P, A] fp32 (per answer the mean score of the targets).
+QuestionImpact = collections.namedtuple("QuestionImpact", "impact answer_mean")
+
+
+def _target_rows(targets):
+    """``targets`` as a 2-D int64 array: one row (a 1-D list shared by every session) or one row per session"""
+    t = np.asarray(targets, np.int64)
+    return t.reshape(1, -1) if t.ndim == 1 else t
+
+
+def _elicit_targets(targets, S, num_items, A, batch_size, queried):
+    """(targets int32 [1, W] or [S, W], per_session) of a question-impact run over S sessions, checked on the host:
+    IndexError for ids outside [0, num_items) (a 2-D array: [-1, num_items)), ValueError for a 2-D array without one
+    row per session, no target slot, a session of ``queried`` whose row has no entry, or A * W > batch_size (every
+    score of a question runs in one batch)"""
+    if torch.is_tensor(targets):
+        targets = targets.detach().cpu().numpy()
+    per = _is_rows(targets)
+    t = _user_rows(targets, S, num_items, "targets") if per else _host_ids(targets, "targets", num_items)
+    t = _target_rows(t)
+    W = t.shape[1]
+    if W == 0:
+        raise ValueError("targets is empty: a question is scored by its effect on at least one target")
+    if per:
+        bare = np.flatnonzero((t[np.asarray(queried, np.int64)] < 0).all(axis=1))
+        if len(bare):
+            raise ValueError("session %d has no target: its row of targets holds only -1"
+                             % int(np.asarray(queried)[bare[0]]))
+    if A * W > int(batch_size):
+        raise ValueError("the %d answers x %d target slots of a question exceed batch_size = %d: every score of a "
+                         "question runs in one batch; raise batch_size" % (A, W, int(batch_size)))
+    return t.astype(np.int32), int(per)
+
+
+def _question_units(sessions, session, questions):
+    """(session, questions) host int64 vectors of explicit units: ids in range (IndexError), equal lengths"""
+    sess = _host_ids(session, "session", sessions.num_sessions)
+    q = _host_ids(questions, "questions", sessions.graph.num_items)
+    if len(sess) != len(q):
+        raise ValueError("session and questions must have the same length (%d vs %d)" % (len(sess), len(q)))
+    return sess, q
+
+
+def elicit_pairs_host(row_ptr, col_idx, rating, users, num_items, A, targets, unit_s, unit_q, unit_tag, B):
+    """twin of igmc_elicit_pairs: ((links_u, links_v, pair_id, tag) [4, B] int64, sess [B] int32, (row_users [G*A],
+    row_ptr [G*A+1], row_col, row_rating)).  ``row_ptr`` / ``col_idx`` / ``rating``: the session rows, ``users`` the
+    sessions' user ids, ``targets`` one list [W] or a row per session [S, W] (-1 = empty slot)"""
+    t2 = _target_rows(targets)
+    W = t2.shape[1]
+    U = A * W
+    G = B // U
+    out = np.zeros((4, B), np.int64)
+    sess = np.zeros(B, np.int32)
+    for i in range(B):
+        real = i < G * U
+        g, a = (i // U, (i % U) // W) if real else (0, 0)
+        s, q = int(unit_s[g]), int(unit_q[g])
+        t = int(t2[s if len(t2) > 1 else 0, i % W]) if real else -1
+        u = int(users[s])
+        v = t if t >= 0 else q
+        out[:, i] = (u, v, u * num_items + v, int(unit_tag[g]) if t >= 0 else -1)
+        sess[i] = g * A + a
+    ru, cols, rats = [], [], []
+    for r in range(G * A):
+        g, a = divmod(r, A)
+        s, q = int(unit_s[g]), int(unit_q[g])
+        row = np.asarray(col_idx[row_ptr[s]:row_ptr[s + 1]], np.int64)
+        p = int(np.searchsorted(row, q))
+        ru.append(int(users[s]))
+        cols.append(np.insert(row, p, q))
+        rats.append(np.insert(np.asarray(rating[row_ptr[s]:row_ptr[s + 1]], np.int64), p, a))
+    rp = np.concatenate([[0], np.cumsum([len(c) for c in cols])]).astype(np.int32)
+    cat = lambda xs, dt: (np.concatenate(xs) if xs else np.zeros(0)).astype(dt)   # noqa: E731
+    return out, sess, (np.asarray(ru, np.int32), rp, cat(cols, np.int32), cat(rats, np.uint8))
+
+
+def _impact_of(x):
+    """impact and answer means of one question from its scores x [A][n] (fp32, real targets in slot order): in fp64
+    (Python floats: no fma) in slot order, each rounded once; a NaN score makes the impact NaN"""
+    A, n = len(x), len(x[0])
+    total, nan = 0.0, False
+    for w in range(n):
+        col = [float(x[a][w]) for a in range(A)]
+        nan = nan or any(np.isnan(col))
+        total += max(col) - min(col)
+    means = []
+    for a in range(A):
+        m = 0.0
+        for w in range(n):
+            m += float(x[a][w])
+        means.append(m / n)
+    return np.float32(np.nan if nan else total / n), np.asarray(means).astype(np.float32)
+
+
+def elicit_stats_host(preds, K, B, A, W, tag):
+    """twin of igmc_elicit_stats over one batch: (impact [G], answer_mean [G, A], unit tag [G]) of its G = B // (A * W)
+    units; a unit without real slots has impact 0, answer_mean NaN and tag -1"""
+    x = _ckpt_mean_host(preds, K, B)
+    tag = np.asarray(tag, np.int64)
+    U = A * W
+    G = B // U
+    impact, mean, utag = np.zeros(G, np.float32), np.full((G, A), np.nan, np.float32), np.full(G, -1, np.int64)
+    for g in range(G):
+        real = [w for w in range(W) if tag[g * U + w] >= 0]
+        if real:
+            utag[g] = tag[g * U + real[-1]]
+            impact[g], mean[g] = _impact_of([[x[g * U + a * W + w] for w in real] for a in range(A)])
+    return impact, mean, utag
+
+
+def question_impact_host(A, targets, session, questions, scorer):
+    """``question_impact`` restated on the host, one ``scorer`` call: scorer(session, question, answer, target) ->
+    fp32 [m], the score of (the user of session[i], target[i]) with session[i]'s row plus the rating (question[i],
+    answer[i]) (label).  ``targets`` one list [W] or a row per session [S, W] (-1 = empty slot).  Returns
+    (impact [P], answer_mean [P, A]) fp32"""
+    t2 = _target_rows(targets)
+    trials, spans = [], []
+    for s, q in zip(np.asarray(session, np.int64), np.asarray(questions, np.int64)):
+        ts = [int(t) for t in t2[s if len(t2) > 1 else 0] if t >= 0]
+        spans.append(len(ts))
+        trials += [(int(s), int(q), a, t) for a in range(A) for t in ts]
+    x = np.asarray(scorer(*(np.array([tr[k] for tr in trials], np.int64) for k in range(4))), np.float32) \
+        if trials else np.zeros(0, np.float32)
+    impact, mean, o = np.zeros(len(spans), np.float32), np.zeros((len(spans), A), np.float32), 0
+    for p, n in enumerate(spans):
+        impact[p], mean[p] = _impact_of(x[o:o + A * n].reshape(A, n))
+        o += A * n
+    return impact, mean
+
+
+def elicit_host(row_ptr, col_idx, num_items, A, n, targets, scorer, questions=None):
+    """``elicit`` restated on the host: per session its questions (every item, one list [Q] or a row per session with
+    -1 padding; minus the items of its row ``col_idx[row_ptr[s]:row_ptr[s+1]]``), their impacts by
+    ``question_impact_host`` and the first n in ``recommend``'s order (impact descending, item ascending, NaN last).
+    Returns (items [S, n] int64, impact [S, n] fp32) padded with -1 / -inf"""
+    S = len(row_ptr) - 1
+    qs = None if questions is None else _target_rows(questions)
+    sess, qu = [], []
+    for s in range(S):
+        cand = np.arange(num_items) if qs is None else np.unique(qs[s if len(qs) > 1 else 0])
+        cand = cand[(cand >= 0) & ~np.isin(cand, np.asarray(col_idx[row_ptr[s]:row_ptr[s + 1]], np.int64))]
+        sess += [s] * len(cand)
+        qu += list(cand)
+    impact, _ = question_impact_host(A, targets, sess, qu, scorer)
+    sess, qu = np.asarray(sess, np.int64), np.asarray(qu, np.int64)
+    top_i, top_s = np.full((S, n), -1, np.int64), np.full((S, n), -np.inf, np.float32)
+    for s in range(S):
+        top_s[s], top_i[s] = rank_host(impact[sess == s], qu[sess == s], n)
+    return top_i, top_s
+
+
 class _TrialRows(object):
-    """one batch slot's trial rows of a counterfactual pass, and their igmc_sessions_t (``_c``): what
-    ``SubgraphExtractor.extract`` takes as ``sessions``"""
+    """one batch slot's trial rows of a counterfactual or question-impact pass, and their igmc_sessions_t (``_c``):
+    what ``SubgraphExtractor.extract`` takes as ``sessions``"""
 
     def __init__(self, users, row_ptr, col_idx, rating):
         self.users, self.row_ptr, self.col_idx, self.rating = users, row_ptr, col_idx, rating
@@ -1024,10 +1188,11 @@ class InferenceEngine(object):
                                                # or start_explain_nodes / start_attribute_nodes(users, items, m)
                                                # or start_draws(users, items, S): S dropout draws per pair
                                                # or start_counterfactual(users, items, rivals, max_removals)
+                                               # or start_elicit(sessions, n, targets) / start_question_impact(...)
         while eng.step():
             pass
         top_items, top_scores = eng.finish()   # (predict: scores; explain: an Explanation; attribute: an Attribution;
-                                               # counterfactual: a Counterfactual)
+                                               # counterfactual: a Counterfactual; question_impact: a QuestionImpact)
 
     An engine serves across updates of its ``RatingGraph`` (``graph.update``) between runs; an update during a run
     makes its next ``step`` raise RuntimeError.
@@ -1129,18 +1294,18 @@ class InferenceEngine(object):
                                   draws=d)
 
     def _plan_ranking(self, slots, k, m, cand, rows, exclude_rated, rated, retriever, args, sessions=None,
-                      by_item=False, draws=None):
+                      by_item=False, draws=None, **fields):
         """the plan of a ranking run over the query slots ``slots`` (int32, on the device) with ``_ranking_inputs``'
         (k, m, cand, rows): the candidate plan over every item or the list ``cand`` (``rated()``: the slots' summed row
         lengths, room for their rated positions in the list), or per-slot rows from ``rows`` or from the retriever entry
         ``retriever`` (leading arguments ``args``).  ``sessions``: the slots are these sessions.  ``by_item``: the
         slots are items and the candidates users - the plan runs on the graph's transposed view, whose rows are the
-        items' columns.  ``draws``: ``_draw_inputs``' dict of a run ranked by draws.  Returns the number of candidate
-        pairs."""
+        items' columns.  ``draws``: ``_draw_inputs``' dict of a run ranked by draws.  ``fields``: further run fields
+        (a question-ranking run's).  Returns the number of candidate pairs."""
         U, dev, g = int(slots.numel()), self.dev, self.graph
         run = dict(kind="recommend", U=U, k=k, version=g.version, sessions=sessions, users=slots, by_item=by_item,
                    top_s=torch.full((U, k), -float("inf"), dtype=torch.float32, device=dev),
-                   top_i=torch.full((U, k), -1, dtype=torch.int64, device=dev), **self._draw_run(draws))
+                   top_i=torch.full((U, k), -1, dtype=torch.int64, device=dev), **self._draw_run(draws), **fields)
         self.run = run
         if U == 0 or (cand is not None and len(cand) == 0) or (rows is not None and rows.shape[1] == 0):
             run["P"] = 0
@@ -1307,28 +1472,90 @@ class InferenceEngine(object):
         run["pu"], run["px"], run["py"] = (torch.from_numpy(a.astype(np.int32)).to(dev) for a in (users, items, rivals))
         run["Qd"] = _lib.Counterfactual(run["pu"].data_ptr(), run["px"].data_ptr(), run["py"].data_ptr(),
                                         run["out"].size.data_ptr(), run["removed"].data_ptr(), Q, M)
-        self._trial_rows()
+        self._trial_rows(self.B, g.max_row_deg)
         self._trial_pass()
         return Q
 
-    def _trial_rows(self):
-        """each slot's trial rows: B rows of up to the graph's longest row, as the session rows igmc_extract_sessions
-        reads (session g of slot g is its trial row)"""
-        L = max(self.graph.max_row_deg, 1)
-        if self.B * L > 2 ** 31 - 1:
-            raise NotImplementedError("batch_size * the longest rating row = %d trial-row entries, beyond int32"
-                                      % (self.B * L))
+    def _trial_rows(self, rows, row_deg):
+        """each slot's trial rows: room for ``rows`` rows of up to ``row_deg`` ratings, as the session rows
+        igmc_extract_sessions reads (sess[g] of slot g names its trial row)"""
+        n = rows * max(row_deg, 1)
+        if n > 2 ** 31 - 1:
+            raise NotImplementedError("%d trial rows of up to %d ratings = %d entries, beyond int32"
+                                      % (rows, row_deg, n))
         i32 = dict(dtype=torch.int32, device=self.dev)
         for s in self.slots:
             t = s.get("trial")
-            if t is None or t.cap < self.B * L:
+            if t is None or t.cap < n:
                 t = s["trial"] = _TrialRows(torch.zeros(self.B, **i32), torch.zeros(self.B + 1, **i32),
-                                            torch.zeros(self.B * L, **i32),
-                                            torch.zeros(self.B * L, dtype=torch.uint8, device=self.dev))
+                                            torch.zeros(n, **i32), torch.zeros(n, dtype=torch.uint8, device=self.dev))
             if "sess" not in s:
                 s["sess"] = torch.zeros(self.B, **i32)
-            t.max_row_deg = self.graph.max_row_deg
+            t.max_row_deg = row_deg
             t._c.max_row_deg = t.max_row_deg
+
+    # ---- question impact ----------------------------------------------------------------------------------------
+    def start_elicit(self, sessions, n, targets, questions=None):
+        """plan a question-ranking run (``elicit``): the units (session s, question q) are the candidate pairs of a
+        ranking run over the session rows (``questions`` as ``start_session_recommend``'s ``items``, rated items
+        always excluded); each batch holds G units of A answers x W targets, and each unit's impact is merged into its
+        session's top-n list.  One host sync (the unit total).  Returns the number of units."""
+        sessions = self._session_slots(sessions)
+        S = sessions.num_sessions
+        n, _, cand, rows = _ranking_inputs(n, self.B, questions, None, S, self.graph.num_items, "questions")
+        fields = self._elicit_run(sessions, targets, np.arange(S))
+        return self._plan_ranking(sessions._slots, n, None, cand, rows, True, lambda: sessions.nnz, None, None,
+                                  sessions, **fields)
+
+    def start_question_impact(self, sessions, session, questions, targets):
+        """plan a run over explicit units (session[i], questions[i]) (``question_impact``): per unit its impact and
+        answer means.  ValueError for a question the session already rated.  Returns the number of units."""
+        sessions = self._session_slots(sessions)
+        sess, q = _question_units(sessions, session, questions)
+        fields = self._elicit_run(sessions, targets, sess)
+        if len(sess):
+            rp, ci, _ = sessions.rows()
+            for s, item in zip(sess, q):
+                row = ci[rp[s]:rp[s + 1]]
+                p = int(np.searchsorted(row, item))
+                if p < len(row) and row[p] == item:
+                    raise ValueError("session %d already rated item %d: a rated item is not a question"
+                                     % (int(s), int(item)))
+        f32 = dict(dtype=torch.float32, device=self.dev)
+        return self._start_explicit("question_impact", sess, q, sessions=sessions,
+                                    impact=torch.empty(len(sess), **f32),
+                                    answer_mean=torch.empty(len(sess), fields["A"], **f32), **fields)
+
+    def _elicit_run(self, sessions, targets, queried):
+        """the run fields of a question-impact run (``_elicit_targets``' targets on the device, the answers A, target
+        width W, units per batch G and the trial rows' longest row), the slots' unit and trial-row buffers allocated"""
+        A, dev = self.model.num_relations, self.dev
+        t, per = _elicit_targets(targets, sessions.num_sessions, self.graph.num_items, A, self.B, queried)
+        W = t.shape[1]
+        L = sessions.max_row_deg + 1            # a trial row: the session row and the question
+        self._trial_rows(self.B // W, L)        # G * A <= B / W trial rows per batch
+        i32, i64 = dict(dtype=torch.int32, device=dev), dict(dtype=torch.int64, device=dev)
+        for s in self.slots:
+            if "gu" not in s:
+                s.update(gu=torch.zeros(self.B, **i32), gv=torch.zeros(self.B, **i32), gpid=torch.zeros(self.B, **i64),
+                         gtag=torch.zeros(self.B, **i64))
+        G = self.B // (A * W)
+        return dict(A=A, W=W, G=G, targets=torch.from_numpy(t).to(dev), per_session=per, row_deg=L,
+                    keys=torch.empty(G, dtype=torch.float32, device=dev))
+
+    def _elicit_stats(self, preds, s):
+        """a batch of units: per unit its impact merged into its session's top-n list (ranking), or its impact and
+        answer means scattered to its index"""
+        run, st = self.run, _stream_ptr()
+        rank = run["kind"] == "recommend"
+        outs = (run["keys"], None, None) if rank else (None, run["impact"], run["answer_mean"])
+        _lib.check(self.lib.igmc_elicit_stats(preds.data_ptr(), self.K, self.B, run["A"], run["W"],
+                                              s["tag"].data_ptr(), *(_lib.ptr(t) for t in outs), st),
+                   "igmc_elicit_stats")
+        if rank:
+            _lib.check(self.lib.igmc_topk_merge(run["keys"].data_ptr(), 1, run["G"], s["gtag"].data_ptr(),
+                                                s["gv"].data_ptr(), run["k"], run["top_s"].data_ptr(),
+                                                run["top_i"].data_ptr(), st), "igmc_topk_merge")
 
     def _trial_pass(self):
         """the next pass of a counterfactual run: the offsets of the queries' trial counts, their total T (the pass's
@@ -1577,10 +1804,11 @@ class InferenceEngine(object):
         ``total``: the positions of the pass (default: the run's pairs)."""
         run = self.run
         sessions = run.get("sessions")
-        # session rows served: a session run's, or the trial rows of a counterfactual run (never longer than the
-        # graph's rows)
-        self.extractor.serve_sessions(sessions.max_row_deg if sessions is not None else run.get("row_deg", 0))
-        per = run.get("G", self.B)      # pairs per batch: G on a run over draws
+        # session rows served: the trial rows of a counterfactual run (never longer than the graph's rows) or of a
+        # question-impact run (a session row and the question), else a session run's
+        row_deg = run["row_deg"] if "row_deg" in run else sessions.max_row_deg if sessions is not None else 0
+        self.extractor.serve_sessions(row_deg)
+        per = run.get("G", self.B)      # pairs per batch: G on a run over draws, G units on a question-impact run
         run["steps"] = ((run["P"] if total is None else total) + per - 1) // per
         if run.get("S"):
             self._draw_masks()
@@ -1615,6 +1843,22 @@ class InferenceEngine(object):
                                                      self.cursor.data_ptr(), self.B, s["u"].data_ptr(),
                                                      s["v"].data_ptr(), s["pid"].data_ptr(), s["tag"].data_ptr(),
                                                      s["j"].data_ptr(), err, _stream_ptr()), "igmc_occlusion_pairs")
+        elif run.get("A"):
+            # G units (session, question), then A x W positions each and per answer its trial row as session
+            # g * A + a, extracted in session mode
+            _lib.check(self.lib.igmc_candidate_pairs(C.byref(self._csr(run)), C.byref(run["Cd"]),
+                                                     self.cursor.data_ptr(), run["G"], s["gu"].data_ptr(),
+                                                     s["gv"].data_ptr(), s["gpid"].data_ptr(), s["gtag"].data_ptr(),
+                                                     err, _stream_ptr()), "igmc_candidate_pairs")
+            t = s["trial"]
+            _lib.check(self.lib.igmc_elicit_pairs(C.byref(sessions._c), self.graph.num_items, run["A"],
+                                                  run["targets"].data_ptr(), run["W"], run["per_session"],
+                                                  s["gu"].data_ptr(), s["gv"].data_ptr(), s["gtag"].data_ptr(), self.B,
+                                                  s["u"].data_ptr(), s["v"].data_ptr(), s["pid"].data_ptr(),
+                                                  s["tag"].data_ptr(), t.users.data_ptr(), t.row_ptr.data_ptr(),
+                                                  t.col_idx.data_ptr(), t.rating.data_ptr(), t.cap,
+                                                  s["sess"].data_ptr(), err, _stream_ptr()), "igmc_elicit_pairs")
+            sessions = t
         elif run.get("S"):
             # G pairs, then S consecutive draws of each over the B positions
             _lib.check(self.lib.igmc_candidate_pairs(C.byref(self._csr(run)), C.byref(run["Cd"]),
@@ -1635,7 +1879,7 @@ class InferenceEngine(object):
             _lib.check(self.lib.igmc_item_query_pairs(self.graph.num_items, self.B, s["u"].data_ptr(),
                                                       s["v"].data_ptr(), s["pid"].data_ptr(), err, _stream_ptr()),
                        "igmc_item_query_pairs")
-        if run.get("sessions") is not None:
+        if run.get("sessions") is not None and not run.get("A"):
             # links_u holds the session: to the session's user id, its pair id and the per-pair session index
             _lib.check(self.lib.igmc_session_pairs(C.byref(sessions._c), self.graph.num_items, self.B,
                                                    s["u"].data_ptr(), s["v"].data_ptr(), s["pid"].data_ptr(),
@@ -1694,6 +1938,8 @@ class InferenceEngine(object):
                 preds = self.preds
         if run.get("S"):
             return self._draw_stats(preds, s)
+        if run.get("A"):
+            return self._elicit_stats(preds, s)
         if run["kind"] == "recommend":
             ranked = s["u"] if run.get("by_item") else s["v"]      # the candidates: users on an item-side run
             _lib.check(self.lib.igmc_topk_merge(preds.data_ptr(), self.K, self.B, s["tag"].data_ptr(),
@@ -1812,6 +2058,8 @@ class InferenceEngine(object):
             return Draws(run["value"], run["mean"], run["std"])
         if run["kind"] == "counterfactual":
             return run["out"]
+        if run["kind"] == "question_impact":
+            return QuestionImpact(run["impact"], run["answer_mean"])
         return run["scores"]
 
     def _order(self, run):
@@ -1879,6 +2127,14 @@ class InferenceEngine(object):
 
     def counterfactual(self, users, items, rivals, max_removals=10):
         self.start_counterfactual(users, items, rivals, max_removals)
+        return self.finish()
+
+    def elicit(self, sessions, n, targets, questions=None):
+        self.start_elicit(sessions, n, targets, questions)
+        return self.finish()
+
+    def question_impact(self, sessions, session, questions, targets):
+        self.start_question_impact(sessions, session, questions, targets)
         return self.finish()
 
     def attribute_nodes(self, users, items, m=None):
@@ -2245,3 +2501,43 @@ def corated_items_sessions(sessions, m, exclude_rated=True):
                             sessions.num_sessions, m, exclude_rated, err, {})
     _lib.check_kernel_error(int(err.item()))
     return items, paths
+
+
+def elicit(model, sessions, n, targets, *, questions=None, h=1, sample_ratio=1.0, max_nodes_per_hop=None,
+           batch_size=256, checkpoints=None, sample_seed=0):
+    """per session the ``n`` items it should be asked to rate: (items [S, n] int64, impact [S, n] fp32) on the model's
+    device, row s for session s.  A question asks session s about an item q not in its row; its answers are the rating
+    labels a = 0..A-1 (A = model.num_relations).  x_a(t) is the eval score of (sessions.users[s], t) with the rating
+    (q, a) added to s's row: bit for bit ``predict_sessions`` of a session with s's edits plus the edit (q, a + 1)
+    (same pair id, sample_seed and checkpoint mean).  impact = the mean over s's real targets t, in slot order, of
+    max_a x_a(t) - min_a x_a(t), in fp64 and rounded once; a NaN score makes it NaN.  ``targets``: one list for every
+    session, or a 2-D array with a row per session (-1 = empty slot); duplicates count each time and rated items are
+    allowed (a target equal to q has range 0: a pair's own rating is never in its subgraph).  ``questions``: every
+    item (None), one list, or a 2-D array of per-session rows (-1 = empty slot); items of the session's row are never
+    questions.  Order: ``recommend``'s (impact descending, item ascending, NaN last); empty slots -1 / -inf.  The
+    results do not depend on batch_size, graph replay or the other sessions.  A question costs A x |targets| forwards;
+    A x the target width <= batch_size, 1 <= n <= IGMC_TOPK_MAX = 256.  The graph is not changed."""
+    sessions = _check_sessions(sessions)
+    S, ni = sessions.num_sessions, sessions.graph.num_items
+    _ranking_inputs(n, batch_size, questions, None, S, ni, "questions")
+    _elicit_targets(targets, S, ni, model.num_relations, batch_size, np.arange(S))
+    return _on_engine(model, sessions.graph, lambda eng: eng.elicit(sessions, n, targets, questions),
+                      h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
+
+
+def question_impact(model, sessions, session, questions, targets, *, h=1, sample_ratio=1.0, max_nodes_per_hop=None,
+                    batch_size=256, checkpoints=None, sample_seed=0):
+    """what asking session ``session[i]`` about item ``questions[i]`` would do: a ``QuestionImpact`` of impact [P]
+    (``elicit``'s key) and answer_mean [P, A] (per answer a the mean of x_a(t) over the session's real targets, in fp64
+    in slot order, rounded once; a NaN score makes that answer's mean NaN) fp32 on the model's device.  ``targets`` and
+    the keywords as ``elicit``'s.  ValueError for a question the session already rated."""
+    sessions = _check_sessions(sessions)
+    sess, q = _question_units(sessions, session, questions)
+    A = model.num_relations
+    _elicit_targets(targets, sessions.num_sessions, sessions.graph.num_items, A, batch_size, sess)
+    if len(sess) == 0:
+        dev = model.flat_params.device
+        return QuestionImpact(torch.zeros(0, dtype=torch.float32, device=dev),
+                              torch.zeros(0, A, dtype=torch.float32, device=dev))
+    return _on_engine(model, sessions.graph, lambda eng: eng.question_impact(sessions, sess, q, targets),
+                      h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)

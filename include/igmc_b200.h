@@ -886,6 +886,43 @@ int igmc_counterfactual_select(const igmc_csr_t* G, const igmc_counterfactual_t*
                                const float* trial_scores, int step, int32_t* count, uint8_t* found, int32_t* out_item,
                                int32_t* out_rating, float* score, float* rival_score, int* err, void* stream);
 
+/* ---- question impact for rating sessions (csrc/elicit.cu; igmc_b200/recommend.py: elicit, question_impact) ----
+ * A question asks session s (igmc_sessions_t) about an item q not in s's row; its answers are the labels a = 0..A-1.
+ * The trial row of (s, q, a) is s's row with (q, a) inserted at q's sorted position; x_a(t) is the eval score of
+ * (users[s], t) extracted in session mode (igmc_extract_sessions) with that trial row as the target row, pair id
+ * users[s] * num_items + t: bit for bit the score of a session with s's edits plus the edit (q, a + 1).  Targets
+ * t_w, w < W: one list for every session (per_session = 0: targets [W]) or a row per session (per_session = 1:
+ * targets [num_sessions, W]), -1 = an empty slot.  A unit (s, q) takes U = A * W consecutive batch positions, answer
+ * major: position i of the unit is answer i / W and target slot i % W.  A batch of B positions holds G = B / U units
+ * (U <= B); positions G*U..B-1 are padding, and so is the position of an empty target slot.  The unit stream
+ * (igmc_candidate_pairs over the session rows as a CSR view, exclude_rated = 1, or over explicit (session, question)
+ * pairs) runs with G slots per batch and writes unit_s (the session), unit_q (the question) and unit_tag. */
+
+/* Position i < G*U, unit g = i / U, answer a = (i % U) / W, target t = the slot i % W of session unit_s[g]:
+ * links_u = users[s], links_v = t, pair_id = links_u * num_items + links_v, tag = unit_tag[g] and sess = g * A + a
+ * (the W targets of one answer share one trial row).  An empty slot, and every position G*U..B-1 (as unit 0, answer
+ * 0), takes links_v = the unit's question and tag -1.  Trial row r = g * A + a, r < G * A: row_users[r] = users[s] and
+ * at [row_ptr[r], row_ptr[r+1]) s's row with (q, a) inserted, ascending, into row_col / row_rating: the session rows
+ * igmc_extract_sessions reads (row_ptr [G*A+1], row_cap entries; (B / W) * (the longest session row + 1) suffice).
+ * Two launches: one CTA for the positions and the block scan of the row lengths deg(s) + 1, one CTA per trial row.
+ * A session index, question or target outside its range (the unit then reads as session 0, question 0; the target
+ * as an empty slot), a question already in the session's row, or rows past row_cap (cut short at row_cap) set
+ * IGMC_ERR_CANDIDATES.  1 <= A <= 256, W >= 1, A * W <= B (else -1). */
+int igmc_elicit_pairs(const igmc_sessions_t* S, int num_items, int A, const int32_t* targets, int W, int per_session,
+                      const int32_t* unit_s, const int32_t* unit_q, const int64_t* unit_tag, int B, int32_t* links_u,
+                      int32_t* links_v, int64_t* pair_id, int64_t* tag, int32_t* row_users, int32_t* row_ptr,
+                      int32_t* row_col, uint8_t* row_rating, int row_cap, int32_t* sess, int* err, void* stream);
+
+/* Per unit g < G of the batch, over its n real target slots w (tag[g*U + w] >= 0) in slot order: x_a(w) = the fp32
+ * checkpoint mean of preds[.][g*U + a*W + w] (as igmc_topk_merge takes it), then in fp64 without fma contraction
+ *   impact = sum_w (max_a x_a(w) - min_a x_a(w)) / n,   answer_mean[a] = sum_w x_a(w) / n,
+ * each rounded once to fp32.  A NaN score of the unit makes its impact NaN, and the mean of its answer NaN.
+ * key != NULL: key [G] = impact for every unit (igmc_topk_merge with K = 1 and B = G then consumes it; a unit without
+ * real slots has key 0 and the merge skips its tag -1).  Otherwise, for the unit's tag t >= 0: impact[t] and
+ * answer_mean[t * A + a]. */
+int igmc_elicit_stats(const float* preds, int K, int B, int A, int W, const int64_t* tag, float* key, float* impact,
+                      float* answer_mean, void* stream);
+
 /* Version / build info: returns the compiled SM arch (90) so the host can refuse stale builds. */
 int igmc_build_info(void);
 
