@@ -251,6 +251,11 @@ _SIGS = {
     "igmc_elicit_pairs": [C.POINTER(Sessions), C.c_int, C.c_int, vp, C.c_int, C.c_int, vp, vp, vp, C.c_int, vp, vp, vp,
                           vp, vp, vp, vp, vp, C.c_int, vp, vp, vp],
     "igmc_elicit_stats": [vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp],
+    "igmc_rescore_plan_ws_bytes": [C.c_int, C.c_int, C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int)],
+    "igmc_rescore_plan": [C.POINTER(CSR), vp, C.c_int, vp, vp, C.c_int, vp, C.c_int, C.c_int, vp, C.c_int64, vp, vp,
+                          C.c_int64, vp, vp, vp, vp],
+    "igmc_cache_invalidate": [C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, vp],
+    "igmc_cache_settle": [C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp],
     "igmc_build_info": [],
     "igmc_model_plan": [C.POINTER(Model), C.c_int, C.c_int, C.c_int],
     "igmc_sortpool_plan": [C.POINTER(SortPool), C.c_int, C.c_int],

@@ -8,7 +8,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libigmc_b200.so")
 SOURCES = ["extract.cu", "batch.cu", "rgcn.cu", "rgcn_rs.cu", "rgcn_l2.cu", "optim.cu", "sortpool.cu",
            "recommend.cu", "retrieve.cu", "graph_update.cu", "explain.cu", "influence.cu", "session.cu",
-           "online.cu", "draws.cu", "counterfactual.cu", "elicit.cu"]
+           "online.cu", "draws.cu", "counterfactual.cu", "elicit.cu", "recommend_cache.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "-shared", "-DIGMC_SM_ARCH=90"]

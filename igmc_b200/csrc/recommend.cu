@@ -28,44 +28,6 @@ constexpr int PLAN_THREADS = 1024;
 constexpr int PAIR_THREADS = 512;
 constexpr int MERGE_THREADS = 256;
 
-__device__ __forceinline__ long long warp_incl_scan_ll(long long v, int lane) {
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    long long t = __shfl_up_sync(IGMC_FULL, v, o);
-    if (lane >= o) v += t;
-  }
-  return v;
-}
-
-// block-wide exclusive scan of one int64 per thread; `ws` >= 33 long longs of shared scratch; ends with a barrier
-__device__ __forceinline__ long long block_excl_scan_ll(long long v, long long* ws, long long* total) {
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
-  long long incl = warp_incl_scan_ll(v, lane);
-  if (lane == 31) ws[w] = incl;
-  __syncthreads();
-  if (w == 0) {
-    long long s = lane < nw ? ws[lane] : 0;
-    long long inc = warp_incl_scan_ll(s, lane);
-    ws[lane] = inc - s;
-    if (lane == 31) ws[32] = inc;
-  }
-  __syncthreads();
-  long long excl = ws[w] + incl - v;
-  *total = ws[32];
-  __syncthreads();
-  return excl;
-}
-
-// position of `item` in the ascending list a[0..n), or -1
-__device__ __forceinline__ int find_sorted(const int32_t* __restrict__ a, int n, int item) {
-  int lo = 0, hi = n;
-  while (lo < hi) {
-    const int mid = (lo + hi) >> 1;
-    if (a[mid] < item) lo = mid + 1; else hi = mid;
-  }
-  return (lo < n && a[lo] == item) ? lo : -1;
-}
-
 __global__ void __launch_bounds__(PLAN_THREADS) k_candidate_plan(igmc_csr_t G, igmc_candidates_t Cd, int* err) {
   __shared__ long long ws[33];
   const int U = Cd.num_query;

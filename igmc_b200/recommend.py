@@ -49,6 +49,9 @@ building a dataset of every candidate pair and looping over it in Python.  Here:
   the mean over ``targets`` of how far the answers move each target's score (csrc/elicit.cu);
   ``question_impact(model, sessions, session, questions, targets)`` -> that impact and the mean target score under
   each answer for explicit (session, question) units;
+* ``RecommendationCache(model, graph, users, k)`` -> ``recommend``'s lists kept exact across ``graph.update``: an update
+  rescores only the pairs whose h = 1 enclosing subgraph it can reach (csrc/recommend_cache.cu) and repairs the cached
+  lists with them;
 * ``InferenceEngine``: the pipelined, graph-replayed loop behind all of them.  Per step the side stream produces the next
   batch's candidate pairs (``igmc_candidate_pairs``, from a device cursor) and extracts it while the main stream runs
   the eval forward of the current batch (once per checkpoint) and merges its scores into the running per-user top-k
@@ -62,6 +65,7 @@ integer arithmetic for the CPU tests (tests/test_recommend_host.py).
 import collections
 import contextlib
 import ctypes as C
+import os
 
 import numpy as np
 import torch
@@ -74,7 +78,8 @@ __all__ = ["predict_pairs", "recommend", "corated_items", "explain_pairs", "Expl
            "Attribution", "pair_gradients", "influence", "self_influence", "Influence", "InferenceEngine",
            "RatingSessions", "predict_sessions", "recommend_sessions", "corated_items_sessions", "recommend_users",
            "corated_users", "explain_nodes", "NodeExplanation", "attribute_nodes", "NodeAttribution", "predict_draws",
-           "Draws", "counterfactual", "Counterfactual", "elicit", "question_impact", "QuestionImpact"]
+           "Draws", "counterfactual", "Counterfactual", "elicit", "question_impact", "QuestionImpact",
+           "RecommendationCache"]
 
 
 # ---- input validation (host) ----------------------------------------------------------------------------------------
@@ -492,6 +497,72 @@ def rank_host(scores, items, k):
     n = min(k, len(o))
     top_i[:n], top_s[:n] = items[o[:n]], scores[o[:n]]
     return top_s, top_i
+
+
+# ---- host twins of the cache repair kernels (csrc/recommend_cache.cu) ----------------------------------------------
+def rescore_plan_host(row_ptr, col_idx, num_items, users, edit_u, edit_v, cand=None, exclude_rated=True):
+    """twin of igmc_rescore_plan on the updated graph: (user_off [U+1] int64, items int32, full [U] uint8, candidate
+    total).  Slot j's items: its candidates (``cand`` or every item, minus the user's rated items when
+    ``exclude_rated``) that are b_i, or in row(a_i) when the user rated b_i; all of them when the user is some a_i"""
+    rp, ci = np.asarray(row_ptr, np.int64), np.asarray(col_idx, np.int64)
+    allowed = np.zeros(num_items, bool)
+    allowed[np.arange(num_items) if cand is None else np.asarray(cand, np.int64)] = True
+    out, full, total = [], [], 0
+    for u in np.asarray(users, np.int64).reshape(-1):
+        row = ci[rp[u]:rp[u + 1]]
+        mark = np.zeros(num_items, bool)
+        for a, b in zip(np.asarray(edit_u, np.int64).reshape(-1), np.asarray(edit_v, np.int64).reshape(-1)):
+            if a == u:
+                mark[:] = True
+                continue
+            mark[b] = True
+            if b in row:
+                mark[ci[rp[a]:rp[a + 1]]] = True
+        ok = allowed.copy()
+        if exclude_rated:
+            ok[row] = False
+        items = np.flatnonzero(mark & ok)
+        out.append(items)
+        full.append(len(items) == int(ok.sum()))
+        total += int(ok.sum())
+    user_off = np.concatenate([[0], np.cumsum([len(x) for x in out])]).astype(np.int64)
+    items = (np.concatenate(out) if out else np.zeros(0)).astype(np.int32)
+    return user_off, items, np.asarray(full, np.uint8), total
+
+
+def cache_invalidate_host(user_off, resc, full, complete, top_s, top_i):
+    """twin of igmc_cache_invalidate: (top_s, top_i, thr_s, thr_i) with the rescored items removed from every prefix
+    (all of a fully rescored slot's: its own user's edits may have changed its candidates) and the threshold key (item -1: none, -2: an empty prefix of a slot that is not complete)"""
+    top_s, top_i = np.array(top_s, np.float32), np.array(top_i, np.int64)
+    U, D = top_i.shape
+    thr_s, thr_i = np.full(U, -np.inf, np.float32), np.full(U, -1, np.int64)
+    for j in range(U):
+        n = int(np.argmin(np.r_[top_i[j] >= 0, False]))           # the leading entries with an item
+        if not (complete[j] or full[j]):
+            thr_i[j], thr_s[j] = (top_i[j, n - 1], top_s[j, n - 1]) if n else (-2, -np.inf)
+        keep = ~np.isin(top_i[j, :n], np.asarray(resc[user_off[j]:user_off[j + 1]], np.int64)) & (full[j] == 0)
+        s, i = top_s[j, :n][keep], top_i[j, :n][keep]
+        top_s[j], top_i[j] = -np.inf, -1
+        top_s[j, :len(s)], top_i[j, :len(i)] = s, i
+    return top_s, top_i, thr_s, thr_i
+
+
+def cache_settle_host(thr_s, thr_i, top_s, top_i, k):
+    """twin of igmc_cache_settle: (top_s, top_i, complete, redo) with every list cut to its exact depth"""
+    top_s, top_i = np.array(top_s, np.float32), np.array(top_i, np.int64)
+    U, D = top_i.shape
+    complete, redo = np.zeros(U, np.uint8), []
+    for j in range(U):
+        d = 0
+        if thr_i[j] != -2:
+            while d < D and top_i[j, d] >= 0 and (thr_i[j] == -1 or
+                                                   not _before(thr_s[j], thr_i[j], top_s[j, d], top_i[j, d])):
+                d += 1
+        top_s[j, d:], top_i[j, d:] = -np.inf, -1
+        complete[j] = thr_i[j] == -1 and d < D
+        if thr_i[j] != -1 and d < k:
+            redo.append(j)
+    return top_s, top_i, complete, np.asarray(redo, np.int32)
 
 
 # ---- host twins of the explanation kernels (csrc/explain.cu) --------------------------------------------------------
@@ -1357,6 +1428,21 @@ class InferenceEngine(object):
         """after the plan of a ranking run: its pair total (the run's one host sync), the first batch primed.  Returns
         the total."""
         run["Cd"].num_pairs = run["P"] = int(run["user_off"][run["U"]].item())
+        if run["P"] > 0:
+            self._prime()
+        return run["P"]
+
+    def _start_rescore(self, slots, user_off, cand, P, top_s, top_i):
+        """a ranking run over a plan made by the caller (``RecommendationCache``: igmc_rescore_plan): query slots
+        ``slots`` (int32 on the device), per slot its items in ``cand`` at ``user_off`` (P pairs in all, known on the
+        host), merged into the lists top_s / top_i [U, depth] as they stand instead of lists of -inf.  No host sync
+        beyond the model's plan of a new batch shape."""
+        run = self.run = dict(kind="recommend", U=int(slots.numel()), k=int(top_s.shape[1]), version=self.graph.version,
+                              sessions=None, users=slots, by_item=False, top_s=top_s, top_i=top_i, user_off=user_off,
+                              cand=cand, P=int(P))
+        Cd = run["Cd"] = _lib.Candidates()
+        Cd.users, Cd.user_off, Cd.num_query, Cd.cand = slots.data_ptr(), user_off.data_ptr(), run["U"], cand.data_ptr()
+        Cd.per_user, Cd.num_pairs = 1, run["P"]
         if run["P"] > 0:
             self._prime()
         return run["P"]
@@ -2388,6 +2474,174 @@ def recommend(model, graph, users, k, *, items=None, exclude_rated=True, retriev
     return _on_engine(model, graph, lambda eng: eng.recommend(users, k, items, exclude_rated, retrieve, draws, beta,
                                                               draw_seed),
                       h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
+
+
+class RecommendationCache(object):
+    """``recommend``'s lists for a fixed set of users, kept exact as ratings arrive (h = 1; DESIGN.md §19).
+
+        cache = RecommendationCache(model, graph, users, k=10, depth=50)
+        cache.update(u, v, values)             # graph.update, then only the pairs the edits can reach are rescored
+        top_items, top_scores = cache.lists()  # == recommend(model, graph, users, 10, ...) on the updated graph
+
+    An edit (a, b) changes the enclosing subgraph of (u, v) only when u = a, v = b, or u rated b and a rated v: every
+    other cached score stays what ``recommend`` computes, bit for bit.  Each slot keeps its ``depth`` best entries as an
+    exact prefix; a repair drops the rescored items from it, merges their new scores and keeps the entries that still
+    rank before every unlisted item.  A slot left with fewer than k exact entries is re-ranked in full.  Keywords as
+    ``recommend``'s (one shared ``items`` list or none); ``depth`` (k..IGMC_TOPK_MAX, default k): kept entries per
+    slot, a deeper list outlives more invalidations.
+
+    Host synchronisations of an ``update`` that needs no full rebuild or fallback: the parameter check, graph.update's,
+    the rescore total and the fallback count, four in all (three without rescored pairs; with ``checkpoints`` the
+    parameter check compares the files' stamps on the host).  Every list is rebuilt in full - ``update`` returns
+    full=True - when the item count grows (every pair id changes), the model's parameters or the checkpoint files
+    changed since the last build, the extractor's node capacity n_cap changes (it sets the kernel plan, and scores are
+    bit-identical on one batch shape), or the rescore plan reaches the pairs of a full run."""
+
+    def __init__(self, model, graph, users, k, *, depth=None, items=None, exclude_rated=True, h=1, sample_ratio=1.0,
+                 max_nodes_per_hop=None, batch_size=256, checkpoints=None, sample_seed=0, use_graph=True,
+                 retrieve=None, draws=None):
+        if draws is not None:
+            raise NotImplementedError("a cache keeps lists ranked by the eval score: a ranking by draws= is drawn anew "
+                                      "for every pair")
+        if int(h) != 1:
+            raise NotImplementedError("a cache repairs lists with h = 1 only: at h >= 2 an update reaches further by "
+                                      "a hop per hop")
+        users = _host_ids(users, "users", graph.shape[0])
+        k, m, cand, rows = _ranking_inputs(k, batch_size, items, retrieve, len(users), graph.shape[1])
+        if m is not None or rows is not None:
+            raise NotImplementedError("a cache takes one shared items list or none: per-user rows and retrieve= "
+                                      "candidates change with the graph")
+        depth = k if depth is None else _check_count(depth, "depth", _lib.TOPK_MAX)
+        if depth < k:
+            raise ValueError("depth must be at least k (%d), not %d" % (k, depth))
+        _check_merge_fits(depth, batch_size)
+        self.k, self.depth, self.exclude_rated = k, depth, bool(exclude_rated)
+        self._users, self._cand, self._checkpoints = users, cand, list(checkpoints or [])
+        self._args = [model, graph, h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed,
+                      use_graph]
+        self.eng = InferenceEngine(*self._args)
+        self.graph = self._args[1] = self.eng.graph
+        U, dev = len(users), self.eng.dev
+        i32, i64 = dict(dtype=torch.int32, device=dev), dict(dtype=torch.int64, device=dev)
+        self._slots = torch.from_numpy(users.astype(np.int32)).to(dev)
+        self._cand_dev = None if cand is None else torch.from_numpy(cand.astype(np.int32)).to(dev)
+        self._user_off, self._totals = torch.zeros(U + 1, **i64), torch.zeros(2, **i64)
+        self._full = torch.zeros(max(U, 1), dtype=torch.uint8, device=dev)
+        self._thr_s = torch.zeros(max(U, 1), dtype=torch.float32, device=dev)
+        self._thr_i, self._redo, self._redo_count = torch.zeros(max(U, 1), **i64), torch.zeros(max(U, 1), **i32), \
+            torch.zeros(1, **i32)
+        self._resc, self._ws = torch.zeros(1, **i32), torch.zeros(1, dtype=torch.uint8, device=dev)
+        self.refresh()
+
+    def _stamp(self):
+        return [(os.stat(p).st_mtime_ns, os.stat(p).st_size) for p in self._checkpoints]
+
+    def _stale_params(self):
+        """the scored parameters changed since the last build: the checkpoint files' stamps (host), or the model's
+        flat_params against the device copy taken then (one host sync)"""
+        if self._checkpoints:
+            return self._stamp() != self._built_from
+        return not torch.equal(self.eng.model.flat_params, self._built_from)
+
+    def _check_version(self):
+        if self.graph.version != self._version:
+            raise RuntimeError("the rating graph was updated outside this cache (graph.update): its lists belong to "
+                               "the old graph; call refresh()")
+
+    def refresh(self):
+        """rebuild every list with a full ranking run (also after an update made outside the cache).  Returns the
+        number of pairs scored."""
+        if self._checkpoints and self._stamp() != getattr(self, "_built_from", None):
+            self.eng.close()
+            self.eng = InferenceEngine(*self._args)     # reads the checkpoint files again
+        eng, g = self.eng, self.graph
+        self._built_from = self._stamp() if self._checkpoints else eng.model.flat_params.detach().clone()
+        P = eng.start_recommend(self._users, self.depth, self._cand, self.exclude_rated)
+        self._top_i, self._top_s = eng.finish()
+        self._complete = ((self._top_i >= 0).sum(1) < self.depth).to(torch.uint8)
+        eng.extractor._sync_graph()
+        self._version, self._num_items, self._cap = g.version, g.num_items, eng.extractor.cap
+        need = len(self._users) * (g.num_items if self._cand is None else len(self._cand))
+        if self._resc.numel() < need:
+            self._resc = torch.empty(need, dtype=torch.int32, device=eng.dev)
+        return P
+
+    def lists(self):
+        """(top_items [U, k] int64, top_scores [U, k] fp32) on the device: ``recommend``'s layout and order"""
+        self._check_version()
+        return self._top_i[:, :self.k].clone(), self._top_s[:, :self.k].clone()
+
+    def update(self, users, items, values, shape=None):
+        """``graph.update(users, items, values, shape)``, then the lists repaired.  Returns graph.update's counts and
+        rescored_pairs (pairs scored: the rescore plan's, or a full run's), rebuilt_users (slots re-ranked in full)
+        and full (every list rebuilt)."""
+        self._check_version()
+        g, eng, U = self.graph, self.eng, len(self._users)
+        stale = U > 0 and self._stale_params()
+        u, v, x, D = _update_inputs(users, items, values, g.capacity.users, g.capacity.items)
+        if any(torch.is_tensor(t) for t in (u, v, x)):
+            u, v, x = (_on_device_i32(t, eng.dev) for t in (u, v, x))
+        else:       # checked above: one pinned upload, no stream sync, and graph.update takes the edits as they are
+            up = torch.from_numpy(np.stack([u, v, x]).astype(np.int32)).pin_memory().to(eng.dev, non_blocking=True)
+            u, v, x = up[0], up[1], up[2]
+        out = dict(g.update(u, v, x, shape), rescored_pairs=0, rebuilt_users=0, full=False)
+        if U == 0 or (g.version == self._version and not stale):
+            self._version = g.version
+            return out
+        eng.extractor._sync_graph()
+        if stale or g.num_items != self._num_items or eng.extractor.cap != self._cap:
+            return dict(out, rescored_pairs=self.refresh(), full=True)
+        nbytes, chunk = C.c_int64(0), C.c_int(0)
+        lib, err = eng.lib, eng.extractor.err
+        _lib.check(lib.igmc_rescore_plan_ws_bytes(U, g.num_items, 0, C.byref(nbytes), C.byref(chunk)),
+                   "igmc_rescore_plan_ws_bytes")
+        if self._ws.numel() < nbytes.value:
+            self._ws = torch.empty(nbytes.value, dtype=torch.uint8, device=eng.dev)
+        _lib.check(lib.igmc_rescore_plan(C.byref(g._c), self._slots.data_ptr(), U, u.data_ptr(), v.data_ptr(), D,
+                                         _lib.ptr(self._cand_dev), 0 if self._cand is None else len(self._cand),
+                                         int(self.exclude_rated), self._ws.data_ptr(), self._ws.numel(),
+                                         self._user_off.data_ptr(), self._resc.data_ptr(), self._resc.numel(),
+                                         self._full.data_ptr(), self._totals.data_ptr(), err.data_ptr(),
+                                         _stream_ptr()), "igmc_rescore_plan")
+        P, total, code = (int(x) for x in torch.cat([self._totals, err.long()]).cpu())   # the rescore total
+        self._check_error(code)
+        if P > 0 and P >= total:
+            return dict(out, rescored_pairs=self.refresh(), full=True)
+        self._version = g.version
+        if P == 0:
+            return out
+        args = (U, self.depth)
+        _lib.check(lib.igmc_cache_invalidate(*args, self._user_off.data_ptr(), self._resc.data_ptr(),
+                                             self._full.data_ptr(), self._complete.data_ptr(), self._top_s.data_ptr(),
+                                             self._top_i.data_ptr(), self._thr_s.data_ptr(), self._thr_i.data_ptr(),
+                                             _stream_ptr()), "igmc_cache_invalidate")
+        eng._start_rescore(self._slots, self._user_off, self._resc, P, self._top_s, self._top_i)
+        while eng.step():
+            pass
+        eng.run = None
+        _lib.check(lib.igmc_cache_settle(*args, self.k, self._thr_s.data_ptr(), self._thr_i.data_ptr(),
+                                         self._top_s.data_ptr(), self._top_i.data_ptr(), self._complete.data_ptr(),
+                                         self._redo.data_ptr(), self._redo_count.data_ptr(), _stream_ptr()),
+                   "igmc_cache_settle")
+        F, code = (int(x) for x in torch.cat([self._redo_count, err]).cpu())          # the fallback count
+        self._check_error(code)
+        if F:
+            redo = self._redo[:F].long()
+            ti, ts = eng.recommend(self._users[redo.cpu().numpy()], self.depth, self._cand, self.exclude_rated)
+            self._top_i[redo], self._top_s[redo] = ti, ts
+            self._complete[redo] = ((ti >= 0).sum(1) < self.depth).to(torch.uint8)
+        return dict(out, rescored_pairs=P, rebuilt_users=F)
+
+    def _check_error(self, code):
+        if code:
+            self.eng.extractor.err.zero_()
+            self._version = None        # the lists are not known to be exact: refresh() rebuilds them
+            _lib.check_kernel_error(code)
+
+    def close(self):
+        """wait for the device and release the engine and the lists"""
+        self.eng.close()
+        self._top_i = self._top_s = self._resc = self._ws = None
 
 
 def corated_items(graph, users, m, exclude_rated=True):

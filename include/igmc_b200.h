@@ -923,6 +923,50 @@ int igmc_elicit_pairs(const igmc_sessions_t* S, int num_items, int A, const int3
 int igmc_elicit_stats(const float* preds, int K, int B, int A, int W, const int64_t* tag, float* key, float* impact,
                       float* answer_mean, void* stream);
 
+/* ---- cached top-k lists repaired after a rating-graph update (csrc/recommend_cache.cu; igmc_b200/recommend.py:
+ * RecommendationCache) ----
+ * With h = 1 the edits (a_i, b_i) of an update can change the enclosing subgraph, and so the score, only of the pairs
+ * in ({a_i} x every item) U (every user x {b_i}) U (col(b_i) x row(a_i)) (DESIGN.md §19).  A cache keeps per query slot
+ * j a list top_score / top_item [num_query, depth] whose leading entries (item >= 0) are an exact prefix of the slot's
+ * ranking (igmc_topk_merge's order) and whose rest is padding (item -1, score -inf); complete[j] = 1 when the prefix
+ * holds every candidate of the slot, else every unlisted candidate ranks after the last prefix entry. */
+
+/* Workspace of igmc_rescore_plan: the candidate bitmap (ceil(num_items / 32) words), then per slot of a chunk one
+ * bitmap row and two counts.  `bound` (<= 0: 256 MB) caps the bytes: past it the slots are processed in chunks of
+ * *chunk (written when chunk != NULL); a workspace of any size runs in chunks of what it holds. */
+int igmc_rescore_plan_ws_bytes(int num_query, int num_items, int64_t bound, int64_t* bytes, int* chunk);
+
+/* The rescore plan of an update, on the UPDATED graph G: per query slot j (user users[j]) the sorted, distinct
+ * candidate items of the affected set of the edits (edit_u[i], edit_v[i]) - every candidate when users[j] = some
+ * edit_u[i]; else edit_v[i], and row(edit_u[i]) when users[j] rated edit_v[i] - in igmc_candidate_pairs' per_user
+ * layout: user_off [num_query+1] int64 and out[user_off[j] ..) (out_cap entries; positions past it set
+ * IGMC_ERR_CANDIDATES).  Candidates: `cand` [num_cand] ascending (NULL: every item), minus the user's rated items when
+ * exclude_rated.  full[j] = 1 when every candidate of slot j is in its plan.  totals[0] = user_off[num_query],
+ * totals[1] = the candidates of every slot (the pairs of a full ranking run).  A user bitmap row per slot built with
+ * integer atomicOr, then a popcount scan: bit-identical across runs and chunk sizes.  Ids outside G set
+ * IGMC_ERR_CANDIDATES (an edit is skipped, a slot has no candidates).  -2 when `ws_bytes` holds no slot. */
+int igmc_rescore_plan(const igmc_csr_t* G, const int32_t* users, int num_query, const int32_t* edit_u,
+                      const int32_t* edit_v, int num_edits, const int32_t* cand, int num_cand, int exclude_rated,
+                      void* ws, int64_t ws_bytes, int64_t* user_off, int32_t* out, int64_t out_cap, uint8_t* full,
+                      int64_t* totals, int* err, void* stream);
+
+/* Before the merge of a repair, per slot j: the prefix without the items of out[user_off[j] .. user_off[j+1]) (binary
+ * search; nothing is kept when full[j], since an edit of the slot's own user can change its candidates), compacted in order and padded to depth; the threshold key thr_score / thr_item [j] = the last prefix entry
+ * before the removal, item -1 (none) when complete[j] or full[j], item -2 when the prefix is empty and the slot is
+ * not complete (nothing is known to be exact).  1 <= depth <= IGMC_TOPK_MAX. */
+int igmc_cache_invalidate(int num_query, int depth, const int64_t* user_off, const int32_t* resc, const uint8_t* full,
+                          const uint8_t* complete, float* top_score, int64_t* top_item, float* thr_score,
+                          int64_t* thr_item, void* stream);
+
+/* After the merge (igmc_topk_merge of the rescored pairs into the invalidated lists), per slot j: its exact depth d -
+ * every entry when the threshold is none, 0 for item -2, else the leading entries not ranked after the threshold key
+ * (igmc_topk_merge's order) - with padding past d; complete[j] = (no threshold and d < depth); and the slots with a
+ * threshold and d < k, ascending, in redo [*redo_count]: they are re-ranked over their whole catalogue.  One CTA.
+ * 1 <= k <= depth <= IGMC_TOPK_MAX. */
+int igmc_cache_settle(int num_query, int depth, int k, const float* thr_score, const int64_t* thr_item,
+                      float* top_score, int64_t* top_item, uint8_t* complete, int32_t* redo, int32_t* redo_count,
+                      void* stream);
+
 /* Version / build info: returns the compiled SM arch (90) so the host can refuse stale builds. */
 int igmc_build_info(void);
 
