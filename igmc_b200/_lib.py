@@ -35,6 +35,8 @@ ERR_NAMES = {
 TOPK_MAX = 256       # IGMC_TOPK_MAX
 DRAWS_MAX = 256      # IGMC_DRAWS_MAX
 COUNTERFACTUAL_MAX = 256   # IGMC_COUNTERFACTUAL_MAX
+GROUP_MAX = 64       # IGMC_GROUP_MAX
+GROUP_AGGREGATES = ("mean", "min", "max")   # IGMC_GROUP_AGG_MEAN, _MIN, _MAX
 
 # Kernel plan values (igmc_model_plan): 0 generic kernels, 1..4 relation-space cluster kernels (CTAs per subgraph),
 # PLAN_L2_BASE + c (c = 1, 2, 4, 8) the L2 plan with c CTAs per subgraph (IGMC_PLAN_L2 in include/igmc_b200.h).
@@ -251,7 +253,10 @@ _SIGS = {
     "igmc_elicit_pairs": [C.POINTER(Sessions), C.c_int, C.c_int, vp, C.c_int, C.c_int, vp, vp, vp, C.c_int, vp, vp, vp,
                           vp, vp, vp, vp, vp, C.c_int, vp, vp, vp],
     "igmc_elicit_stats": [vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp],
-    "igmc_rescore_plan_ws_bytes": [C.c_int, C.c_int, C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int)],
+    "igmc_group_rows": [C.POINTER(CSR), vp, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp, vp],
+    "igmc_group_pairs": [vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp],
+    "igmc_group_stats": [vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp],
+    "igmc_rescore_plan_ws_bytes":[C.c_int, C.c_int, C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int)],
     "igmc_rescore_plan": [C.POINTER(CSR), vp, C.c_int, vp, vp, C.c_int, vp, C.c_int, C.c_int, vp, C.c_int64, vp, vp,
                           C.c_int64, vp, vp, vp, vp],
     "igmc_cache_invalidate": [C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, vp],

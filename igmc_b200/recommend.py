@@ -49,6 +49,9 @@ building a dataset of every candidate pair and looping over it in Python.  Here:
   the mean over ``targets`` of how far the answers move each target's score (csrc/elicit.cu);
   ``question_impact(model, sessions, session, questions, targets)`` -> that impact and the mean target score under
   each answer for explicit (session, question) units;
+* ``recommend_groups(model, graph, groups, k)`` -> per group of users the ``k`` best items none of them rated, ranked
+  by the mean, minimum or maximum of the members' own scores (csrc/groups.cu); ``predict_groups(model, graph, groups,
+  group, items)`` -> that aggregate and every member's score for explicit (group, item) queries;
 * ``RecommendationCache(model, graph, users, k)`` -> ``recommend``'s lists kept exact across ``graph.update``: an update
   rescores only the pairs whose h = 1 enclosing subgraph it can reach (csrc/recommend_cache.cu) and repairs the cached
   lists with them;
@@ -79,7 +82,7 @@ __all__ = ["predict_pairs", "recommend", "corated_items", "explain_pairs", "Expl
            "RatingSessions", "predict_sessions", "recommend_sessions", "corated_items_sessions", "recommend_users",
            "corated_users", "explain_nodes", "NodeExplanation", "attribute_nodes", "NodeAttribution", "predict_draws",
            "Draws", "counterfactual", "Counterfactual", "elicit", "question_impact", "QuestionImpact",
-           "RecommendationCache"]
+           "RecommendationCache", "recommend_groups", "predict_groups", "GroupScores"]
 
 
 # ---- input validation (host) ----------------------------------------------------------------------------------------
@@ -1235,6 +1238,165 @@ def elicit_host(row_ptr, col_idx, num_items, A, n, targets, scorer, questions=No
     return top_i, top_s
 
 
+# ---- group recommendation (csrc/groups.cu) --------------------------------------------------------------------------
+# The result of predict_groups, per query (group, item): score [Q] fp32 (the aggregate) and members [Q, M] fp32 (each
+# member's own score, in member order, NaN past the group's size).
+GroupScores = collections.namedtuple("GroupScores", "score members")
+
+
+def _check_aggregate(aggregate):
+    """the IGMC_GROUP_AGG_* code of ``aggregate``: "mean", "min" (least misery) or "max" (most pleasure)"""
+    if not isinstance(aggregate, str) or aggregate not in _lib.GROUP_AGGREGATES:
+        raise ValueError("aggregate must be one of %s, not %r" % (", ".join(_lib.GROUP_AGGREGATES), aggregate))
+    return _lib.GROUP_AGGREGATES.index(aggregate)
+
+
+def _no_group_options(retrieve, draws):
+    if retrieve is not None:
+        raise NotImplementedError("group runs rank items= or every item: there is no group retriever (retrieve=)")
+    if draws is not None:
+        raise NotImplementedError("group runs rank by the eval score: draws= is not supported")
+
+
+def _group_members(groups, num_users, batch_size):
+    """the groups as a host int32 array [G, M] of their members in order, -1 past each group's size (M the largest
+    size).  ``groups``: a list of user-id sequences, or a 2-D integer array [G, width]; -1 entries are skipped.
+    IndexError for an id outside [0, num_users), ValueError for an empty group or a repeated member, and
+    ``_check_count``'s errors for M outside [1, min(batch_size, IGMC_GROUP_MAX)]: every member of a unit runs in one
+    batch"""
+    if torch.is_tensor(groups):
+        groups = groups.detach().cpu().numpy()
+    if isinstance(groups, np.ndarray) and groups.ndim != 2:
+        raise ValueError("groups as an array is 2-D [G, width], not %d-D" % groups.ndim)
+    rows = [np.asarray(r).reshape(-1) for r in groups]
+    rows = [r[r != -1] for r in rows]
+    for j, r in enumerate(rows):
+        if r.size == 0:
+            raise ValueError("group %d has no member" % j)
+        if not np.issubdtype(r.dtype, np.integer):
+            raise TypeError("groups must be integer user ids, not %s" % r.dtype)
+        if r.min() < 0 or r.max() >= num_users:
+            raise IndexError("groups: user id %d out of range [0, %d)" % (r.min() if r.min() < 0 else r.max(),
+                                                                         num_users))
+        if len(np.unique(r)) != len(r):
+            raise ValueError("group %d names a member twice" % j)
+    M = max([len(r) for r in rows], default=1)
+    _check_count(M, "the largest group size (at most batch_size and IGMC_GROUP_MAX = %d)" % _lib.GROUP_MAX,
+                 min(int(batch_size), _lib.GROUP_MAX))
+    out = np.full((len(rows), M), -1, np.int32)
+    for j, r in enumerate(rows):
+        out[j, :len(r)] = r
+    return out
+
+
+def group_rows_host(row_ptr, col_idx, members):
+    """twin of igmc_group_rows: (row_ptr [G+1] int32, col_idx int32), per group the sorted union of its members' rows
+    (-1 slots skipped)"""
+    members = np.asarray(members, np.int64)
+    out = []
+    for r in members.reshape(len(members), -1):
+        parts = [np.asarray(col_idx[row_ptr[u]:row_ptr[u + 1]], np.int64) for u in r[r >= 0]]
+        out.append(np.unique(np.concatenate(parts)) if parts else np.zeros(0, np.int64))
+    rp = np.concatenate([[0], np.cumsum([len(x) for x in out])]).astype(np.int32)
+    return rp, (np.concatenate(out) if out else np.zeros(0)).astype(np.int32)
+
+
+def group_pairs_host(members, num_items, unit_g, unit_v, unit_tag, B):
+    """twin of igmc_group_pairs: (links_u, links_v, pair_id, tag) [4, B] int64 of the Gu = B // M units (group
+    unit_g[u], item unit_v[u]) of members [G, M], position u * M + j member j; empty slots and the tail take the group's
+    first member and tag -1"""
+    members = np.asarray(members, np.int64)
+    M = members.shape[1]
+    Gu = B // M
+    out = np.zeros((4, B), np.int64)
+    for i in range(B):
+        real = i < Gu * M
+        u0, j = (i // M, i % M) if real else (0, 0)
+        g, v = int(unit_g[u0]), int(unit_v[u0])
+        m, lead = int(members[g, j]), int(members[g, 0])
+        u = m if m >= 0 else (lead if lead >= 0 else 0)
+        out[:, i] = (u, v, u * num_items + v, int(unit_tag[u0]) if real and m >= 0 else -1)
+    return out
+
+
+def _aggregate_of(x, aggregate):
+    """one unit's aggregate of its member scores x (fp32, member order) as igmc_group_stats computes it: "mean" a
+    sequential fp64 sum (Python floats: no fma, no pairwise order) / n, rounded once; "min" / "max" the first extreme
+    by strict compares; NaN when any x is"""
+    x = [np.float32(a) for a in x]
+    if any(np.isnan(a) for a in x):
+        return np.float32(np.nan)
+    if aggregate == "mean":
+        s = 0.0
+        for a in x:
+            s += float(a)
+        return np.float32(s / len(x))
+    best = x[0]
+    for a in x[1:]:
+        if (a < best) if aggregate == "min" else (a > best):
+            best = a
+    return np.float32(best)
+
+
+def group_stats_host(preds, K, B, M, aggregate, tag):
+    """twin of igmc_group_stats over one batch: (key [Gu], member scores [Gu, M] (NaN at padding), unit tag [Gu]) of
+    its Gu = B // M units; a unit without real positions has key 0 and tag -1"""
+    x = _ckpt_mean_host(preds, K, B)
+    tag = np.asarray(tag, np.int64)
+    Gu = B // M
+    key, xs, utag = np.zeros(Gu, np.float32), np.full((Gu, M), np.nan, np.float32), np.full(Gu, -1, np.int64)
+    for g in range(Gu):
+        real = np.array([j for j in range(M) if tag[g * M + j] >= 0], np.int64)
+        if len(real):
+            utag[g] = tag[g * M + real[-1]]
+            xs[g, real] = x[g * M + real]
+            key[g] = _aggregate_of(x[g * M + real], aggregate)
+    return key, xs, utag
+
+
+def predict_groups_host(members, group, items, aggregate, scorer):
+    """``predict_groups`` restated on the host, one ``scorer`` call: scorer(users, items) -> fp32 [n], the score of
+    each pair (``predict_pairs``).  Returns (score [Q], members [Q, M]) fp32"""
+    members = np.asarray(members, np.int64)
+    group, items = np.asarray(group, np.int64).reshape(-1), np.asarray(items, np.int64).reshape(-1)
+    who = [members[g][members[g] >= 0] for g in group]
+    u = np.concatenate(who).astype(np.int64) if who else np.zeros(0, np.int64)
+    v = np.repeat(items, [len(w) for w in who]).astype(np.int64)
+    x = np.asarray(scorer(u, v), np.float32) if len(u) else np.zeros(0, np.float32)
+    score, out, o = np.zeros(len(group), np.float32), np.full((len(group), members.shape[1]), np.nan, np.float32), 0
+    for q, w in enumerate(who):
+        out[q, :len(w)] = x[o:o + len(w)]
+        score[q] = _aggregate_of(x[o:o + len(w)], aggregate)
+        o += len(w)
+    return score, out
+
+
+def recommend_groups_host(row_ptr, col_idx, num_items, members, k, aggregate, scorer, items=None, exclude_rated=True):
+    """``recommend_groups`` restated on the host: per group its candidates (every item, one list [n] or a row per
+    group with -1 padding; minus the union of its members' rows when ``exclude_rated``), their aggregates by
+    ``predict_groups_host`` and the first k in ``recommend``'s order.  Returns (items [G, k] int64, scores [G, k] fp32)
+    padded with -1 / -inf"""
+    members = np.asarray(members, np.int64)
+    Gn = len(members)
+    urp, uci = group_rows_host(row_ptr, col_idx, members)
+    per = items is not None and np.ndim(items) == 2
+    grp, cand = [], []
+    for g in range(Gn):
+        c = np.arange(num_items) if items is None else np.unique(np.asarray(items[g] if per else items, np.int64))
+        c = c[c >= 0]
+        if exclude_rated:
+            c = c[~np.isin(c, uci[urp[g]:urp[g + 1]])]
+        grp.append(np.full(len(c), g, np.int64))
+        cand.append(c)
+    grp = np.concatenate(grp) if Gn else np.zeros(0, np.int64)
+    cand = np.concatenate(cand) if Gn else np.zeros(0, np.int64)
+    score, _ = predict_groups_host(members, grp, cand, aggregate, scorer)
+    top_i, top_s = np.full((Gn, k), -1, np.int64), np.full((Gn, k), -np.inf, np.float32)
+    for g in range(Gn):
+        top_s[g], top_i[g] = rank_host(score[grp == g], cand[grp == g], k)
+    return top_i, top_s
+
+
 class _TrialRows(object):
     """one batch slot's trial rows of a counterfactual or question-impact pass, and their igmc_sessions_t (``_c``):
     what ``SubgraphExtractor.extract`` takes as ``sessions``"""
@@ -1260,10 +1422,12 @@ class InferenceEngine(object):
                                                # or start_draws(users, items, S): S dropout draws per pair
                                                # or start_counterfactual(users, items, rivals, max_removals)
                                                # or start_elicit(sessions, n, targets) / start_question_impact(...)
+                                               # or start_recommend_groups(groups, k) / start_group_pairs(...)
         while eng.step():
             pass
         top_items, top_scores = eng.finish()   # (predict: scores; explain: an Explanation; attribute: an Attribution;
-                                               # counterfactual: a Counterfactual; question_impact: a QuestionImpact)
+                                               # counterfactual: a Counterfactual; question_impact: a QuestionImpact;
+                                               # group pairs: a GroupScores)
 
     An engine serves across updates of its ``RatingGraph`` (``graph.update``) between runs; an update during a run
     makes its next ``step`` raise RuntimeError.
@@ -1488,10 +1652,12 @@ class InferenceEngine(object):
 
     # ---- rating sessions ----------------------------------------------------------------------------------------
     def _csr(self, run):
-        """the rows the candidate kernels read: the graph's, its transposed view on an item-side run, or a session
-        run's rows as a CSR over its sessions"""
+        """the rows the candidate kernels read: the graph's, its transposed view on an item-side run, a session run's
+        rows as a CSR over its sessions, or a group run's member unions as a CSR over its groups"""
         if run.get("by_item"):
             return self.graph._ct
+        if run.get("group_view") is not None:
+            return run["group_view"]
         return run["sessions"]._view if run.get("sessions") is not None else self.graph._c
 
     def _session_slots(self, sessions):
@@ -1620,14 +1786,27 @@ class InferenceEngine(object):
         W = t.shape[1]
         L = sessions.max_row_deg + 1            # a trial row: the session row and the question
         self._trial_rows(self.B // W, L)        # G * A <= B / W trial rows per batch
-        i32, i64 = dict(dtype=torch.int32, device=dev), dict(dtype=torch.int64, device=dev)
+        self._unit_buffers()
+        G = self.B // (A * W)
+        return dict(A=A, W=W, G=G, targets=torch.from_numpy(t).to(dev), per_session=per, row_deg=L,
+                    keys=torch.empty(G, dtype=torch.float32, device=dev))
+
+    def _unit_buffers(self):
+        """each slot's unit stream: the G units of a batch (query slot, candidate, pair id, tag) before the kernel
+        that lays them out over the B positions"""
+        i32, i64 = dict(dtype=torch.int32, device=self.dev), dict(dtype=torch.int64, device=self.dev)
         for s in self.slots:
             if "gu" not in s:
                 s.update(gu=torch.zeros(self.B, **i32), gv=torch.zeros(self.B, **i32), gpid=torch.zeros(self.B, **i64),
                          gtag=torch.zeros(self.B, **i64))
-        G = self.B // (A * W)
-        return dict(A=A, W=W, G=G, targets=torch.from_numpy(t).to(dev), per_session=per, row_deg=L,
-                    keys=torch.empty(G, dtype=torch.float32, device=dev))
+
+    def _merge_unit_keys(self, s):
+        """a ranking run over units: the batch's G unit keys (run["keys"]) merged into the running top-k lists of
+        their query slots, ranked by the units' candidates (items, or users on an item-side run)"""
+        run = self.run
+        _lib.check(self.lib.igmc_topk_merge(run["keys"].data_ptr(), 1, run["G"], s["gtag"].data_ptr(),
+                                            s["gv"].data_ptr(), run["k"], run["top_s"].data_ptr(),
+                                            run["top_i"].data_ptr(), _stream_ptr()), "igmc_topk_merge")
 
     def _elicit_stats(self, preds, s):
         """a batch of units: per unit its impact merged into its session's top-n list (ranking), or its impact and
@@ -1639,9 +1818,73 @@ class InferenceEngine(object):
                                               s["tag"].data_ptr(), *(_lib.ptr(t) for t in outs), st),
                    "igmc_elicit_stats")
         if rank:
-            _lib.check(self.lib.igmc_topk_merge(run["keys"].data_ptr(), 1, run["G"], s["gtag"].data_ptr(),
-                                                s["gv"].data_ptr(), run["k"], run["top_s"].data_ptr(),
-                                                run["top_i"].data_ptr(), st), "igmc_topk_merge")
+            self._merge_unit_keys(s)
+
+    # ---- group recommendation -----------------------------------------------------------------------------------
+    def start_recommend_groups(self, groups, k, aggregate="mean", items=None, exclude_rated=True, retrieve=None,
+                               draws=None):
+        """plan a group ranking run (``recommend_groups``): query slot g is group g, and its rated items are the
+        union of its members' rows (igmc_group_rows, the CSR view ``_csr`` hands the candidate kernels).  Each batch
+        holds Gu = B / M units (group, item) of M member positions, and each unit's aggregate is merged into its
+        group's top-k list.  One host sync (the unit total).  Returns the number of units."""
+        _no_group_options(retrieve, draws)
+        g = self.graph
+        members = _group_members(groups, g.num_users, self.B)
+        k, _, cand, rows = _ranking_inputs(k, self.B, items, None, len(members), g.num_items)
+        fields = self._group_run(members, aggregate, union=True)
+        slots = torch.arange(len(members), dtype=torch.int32, device=self.dev)
+        return self._plan_ranking(slots, k, None, cand, rows, exclude_rated, lambda: fields["cap"], None, None,
+                                  **fields)
+
+    def start_group_pairs(self, groups, group, items, aggregate="mean"):
+        """plan a run over explicit queries (group[i], items[i]) (``predict_groups``): per query the aggregate and
+        each member's score.  Rated items are scored like any other.  Returns the number of queries."""
+        members = _group_members(groups, self.graph.num_users, self.B)
+        grp, items, _ = _host_pairs((len(members), self.graph.num_items), group, items, first="group")
+        fields = self._group_run(members, aggregate, union=False)
+        member_scores = torch.full((len(grp), members.shape[1]), float("nan"), dtype=torch.float32, device=self.dev)
+        return self._start_explicit("group_pairs", grp, items, member_scores=member_scores, **fields)
+
+    def _group_run(self, members, aggregate, union):
+        """the run fields of a group run over ``_group_members``' array: the members on the device, the width M, the
+        aggregate's code, Gu = B / M units per batch and the CSR view of the groups the candidate kernels read - with
+        ``union``, the union rows of igmc_group_rows (no host sync: their capacity, the summed member degrees, comes from
+        the host row pointers).  The slots' unit buffers are allocated."""
+        agg = _check_aggregate(aggregate)
+        Gn, M = members.shape
+        g, dev = self.graph, self.dev
+        self._unit_buffers()
+        f = dict(groups=torch.from_numpy(members).to(dev), width=M, agg=agg, G=self.B // M, cap=0,
+                 keys=torch.empty(self.B // M, dtype=torch.float32, device=dev),
+                 group_view=_lib.CSR(None, None, None, None, None, Gn, g.num_items))
+        if not union or Gn == 0:
+            return f
+        rp = g.host["row_ptr"]
+        m = members[members >= 0].astype(np.int64)
+        cap = f["cap"] = int((rp[m + 1] - rp[m]).sum())
+        if cap > 2 ** 31 - 1:
+            raise NotImplementedError("the groups' members hold %d ratings together, beyond int32" % cap)
+        i32 = dict(dtype=torch.int32, device=dev)
+        f["union"] = (torch.empty(Gn + 1, **i32), torch.empty(max(cap, 1), **i32))
+        ws = torch.empty(2 * Gn + 1 + cap, **i32)
+        _lib.check(self.lib.igmc_group_rows(C.byref(g._c), f["groups"].data_ptr(), Gn, M, f["union"][0].data_ptr(),
+                                            f["union"][1].data_ptr(), cap, ws.data_ptr(),
+                                            self.extractor.err.data_ptr(), _stream_ptr()), "igmc_group_rows")
+        f["group_view"] = _lib.CSR(f["union"][0].data_ptr(), f["union"][1].data_ptr(), None, None, None, Gn,
+                                   g.num_items)
+        return f
+
+    def _group_stats(self, preds, s):
+        """a batch of group units: per unit its aggregate merged into its group's top-k list (ranking), or its
+        aggregate and member scores scattered to its query index"""
+        run = self.run
+        rank = run["kind"] == "recommend"
+        outs = (run["keys"], None, None) if rank else (None, run["scores"], run["member_scores"])
+        _lib.check(self.lib.igmc_group_stats(preds.data_ptr(), self.K, self.B, run["width"], run["agg"],
+                                             s["tag"].data_ptr(), *(_lib.ptr(t) for t in outs), _stream_ptr()),
+                   "igmc_group_stats")
+        if rank:
+            self._merge_unit_keys(s)
 
     def _trial_pass(self):
         """the next pass of a counterfactual run: the offsets of the queries' trial counts, their total T (the pass's
@@ -1945,6 +2188,17 @@ class InferenceEngine(object):
                                                   t.col_idx.data_ptr(), t.rating.data_ptr(), t.cap,
                                                   s["sess"].data_ptr(), err, _stream_ptr()), "igmc_elicit_pairs")
             sessions = t
+        elif run.get("width"):
+            # Gu units (group, item), then one position per member
+            _lib.check(self.lib.igmc_candidate_pairs(C.byref(self._csr(run)), C.byref(run["Cd"]),
+                                                     self.cursor.data_ptr(), run["G"], s["gu"].data_ptr(),
+                                                     s["gv"].data_ptr(), s["gpid"].data_ptr(), s["gtag"].data_ptr(),
+                                                     err, _stream_ptr()), "igmc_candidate_pairs")
+            _lib.check(self.lib.igmc_group_pairs(run["groups"].data_ptr(), int(run["groups"].shape[0]), run["width"],
+                                                 self.graph.num_users, self.graph.num_items, s["gu"].data_ptr(),
+                                                 s["gv"].data_ptr(), s["gtag"].data_ptr(), self.B, s["u"].data_ptr(),
+                                                 s["v"].data_ptr(), s["pid"].data_ptr(), s["tag"].data_ptr(), err,
+                                                 _stream_ptr()), "igmc_group_pairs")
         elif run.get("S"):
             # G pairs, then S consecutive draws of each over the B positions
             _lib.check(self.lib.igmc_candidate_pairs(C.byref(self._csr(run)), C.byref(run["Cd"]),
@@ -2026,6 +2280,8 @@ class InferenceEngine(object):
             return self._draw_stats(preds, s)
         if run.get("A"):
             return self._elicit_stats(preds, s)
+        if run.get("width"):
+            return self._group_stats(preds, s)
         if run["kind"] == "recommend":
             ranked = s["u"] if run.get("by_item") else s["v"]      # the candidates: users on an item-side run
             _lib.check(self.lib.igmc_topk_merge(preds.data_ptr(), self.K, self.B, s["tag"].data_ptr(),
@@ -2045,10 +2301,7 @@ class InferenceEngine(object):
         _lib.check(self.lib.igmc_draws_stats(preds.data_ptr(), self.K, self.B, run["S"], s["tag"].data_ptr(),
                                              run["beta"], *(_lib.ptr(t) for t in outs), st), "igmc_draws_stats")
         if rank:
-            # the candidates before the mapping kernels: items, or users on an item-side run
-            _lib.check(self.lib.igmc_topk_merge(run["keys"].data_ptr(), 1, run["G"], s["gtag"].data_ptr(),
-                                                s["gv"].data_ptr(), run["k"], run["top_s"].data_ptr(),
-                                                run["top_i"].data_ptr(), st), "igmc_topk_merge")
+            self._merge_unit_keys(s)     # the candidates before the mapping kernels
 
     def _gradient(self, slot):
         """per parameter set: the eval forward of batch ``slot`` on the L2 plan, (DGCNN_RS) the SortPooling backward
@@ -2146,6 +2399,8 @@ class InferenceEngine(object):
             return run["out"]
         if run["kind"] == "question_impact":
             return QuestionImpact(run["impact"], run["answer_mean"])
+        if run["kind"] == "group_pairs":
+            return GroupScores(run["scores"], run["member_scores"])
         return run["scores"]
 
     def _order(self, run):
@@ -2221,6 +2476,15 @@ class InferenceEngine(object):
 
     def question_impact(self, sessions, session, questions, targets):
         self.start_question_impact(sessions, session, questions, targets)
+        return self.finish()
+
+    def recommend_groups(self, groups, k, aggregate="mean", items=None, exclude_rated=True, retrieve=None,
+                         draws=None):
+        self.start_recommend_groups(groups, k, aggregate, items, exclude_rated, retrieve, draws)
+        return self.finish()
+
+    def predict_groups(self, groups, group, items, aggregate="mean"):
+        self.start_group_pairs(groups, group, items, aggregate)
         return self.finish()
 
     def attribute_nodes(self, users, items, m=None):
@@ -2794,4 +3058,45 @@ def question_impact(model, sessions, session, questions, targets, *, h=1, sample
         return QuestionImpact(torch.zeros(0, dtype=torch.float32, device=dev),
                               torch.zeros(0, A, dtype=torch.float32, device=dev))
     return _on_engine(model, sessions.graph, lambda eng: eng.question_impact(sessions, sess, q, targets),
+                      h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
+
+
+# ---- group recommendation: public API -------------------------------------------------------------------------------
+def recommend_groups(model, graph, groups, k, *, aggregate="mean", items=None, exclude_rated=True, retrieve=None,
+                     draws=None, h=1, sample_ratio=1.0, max_nodes_per_hop=None, batch_size=256, checkpoints=None,
+                     sample_seed=0):
+    """per group of users the ``k`` best items for them together: (top_items [G, k] int64, top_scores [G, k] fp32) on
+    the model's device, row g for group g.  ``groups``: a list of user-id sequences or a 2-D integer array [G, width]
+    (-1 entries skipped); a group's members are distinct graph users, at most min(batch_size, IGMC_GROUP_MAX = 64) of
+    them.  x_j is member j's score of the item, bit for bit ``predict_pairs`` (same batch size and kernel plan); the
+    key ``aggregate``s them over the members: "mean" (summed in fp64 in member order, rounded once), "min" (least
+    misery) or "max" (most pleasure), the first in member order on ties; a NaN x_j makes the key NaN.  Candidates:
+    ``items`` as in ``recommend`` (every item, one list, or a row per group), minus every item any member rated when
+    ``exclude_rated``.  Order and padding: ``recommend``'s.  A group of one is ``recommend`` for its user.  Results do
+    not depend on the other groups of the run.  ``retrieve=`` and ``draws=`` are not supported (NotImplementedError)."""
+    _no_group_options(retrieve, draws)
+    _check_aggregate(aggregate)
+    members = _group_members(groups, graph.shape[0], batch_size)
+    k = _ranking_inputs(k, batch_size, items, None, len(members), graph.shape[1])[0]
+    if len(members) == 0:
+        dev = model.flat_params.device
+        return (torch.zeros(0, k, dtype=torch.int64, device=dev), torch.zeros(0, k, dtype=torch.float32, device=dev))
+    return _on_engine(model, graph, lambda eng: eng.recommend_groups(members, k, aggregate, items, exclude_rated),
+                      h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
+
+
+def predict_groups(model, graph, groups, group, items, *, aggregate="mean", h=1, sample_ratio=1.0,
+                   max_nodes_per_hop=None, batch_size=256, checkpoints=None, sample_seed=0):
+    """scores of explicit queries (groups[group[i]], items[i]): a ``GroupScores`` of score [Q] (``recommend_groups``'
+    key) and members [Q, M] (each member's own score in member order, NaN past the group's size; M the largest group
+    size), fp32 on the model's device - what a list shows beside each item for each member.  ``groups`` and the
+    keywords as ``recommend_groups``'.  Rated items are scored like any other, as in ``predict_pairs``."""
+    _check_aggregate(aggregate)
+    members = _group_members(groups, graph.shape[0], batch_size)
+    grp, items, _ = _host_pairs((len(members), graph.shape[1]), group, items, first="group")
+    if len(grp) == 0:
+        dev = model.flat_params.device
+        return GroupScores(torch.zeros(0, dtype=torch.float32, device=dev),
+                           torch.zeros(0, members.shape[1], dtype=torch.float32, device=dev))
+    return _on_engine(model, graph, lambda eng: eng.predict_groups(members, grp, items, aggregate),
                       h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)

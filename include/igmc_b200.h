@@ -923,6 +923,48 @@ int igmc_elicit_pairs(const igmc_sessions_t* S, int num_items, int A, const int3
 int igmc_elicit_stats(const float* preds, int K, int B, int A, int W, const int64_t* tag, float* key, float* impact,
                       float* answer_mean, void* stream);
 
+/* ---- group recommendation (csrc/groups.cu; igmc_b200/recommend.py: recommend_groups, predict_groups) ----
+ * A group is a row of `members` [num_groups, width] int32: its members are the row's user ids in order, -1 = an empty
+ * slot (the host puts them last).  The group's score of an item v aggregates x_j, member j's own eval score of
+ * (member, v) with pair id member * num_items + v: bit for bit predict_pairs' score of that pair.  The unit stream
+ * (igmc_candidate_pairs over the group rows as a CSR view of num_groups query slots, or over explicit (group, item)
+ * pairs) runs with Gu = B / width slots per batch and writes unit_g (the group), unit_v (the item) and unit_tag.  A unit
+ * takes `width` consecutive batch positions, position j its member j; positions Gu*width..B-1 are padding. */
+#define IGMC_GROUP_MAX 64
+#define IGMC_GROUP_AGG_MEAN 0   /* the members' mean, summed in fp64 in member order without fma, rounded once */
+#define IGMC_GROUP_AGG_MIN 1    /* least misery: the first smallest x_j */
+#define IGMC_GROUP_AGG_MAX 2    /* most pleasure: the first largest x_j */
+
+/* Per group the sorted, de-duplicated union of its members' rows of G: row_ptr [num_groups+1] and col_idx (cap
+ * entries; the summed member degrees always suffice).  With these, an igmc_csr_t {row_ptr, col_idx, NULL, NULL, NULL,
+ * num_groups, G.num_items} is what the candidate kernels read for a group run: query slot g is group g, its rated items
+ * the union.  ws: 2 * num_groups + 1 + cap int32.  Integer work only, one writer per output, so bit-identical across
+ * runs.  Four launches: the offsets of the concatenated member rows (one CTA), per group its first occurrences and their
+ * scan (one CTA per group), the union sizes' scan (one CTA), and each first occurrence written at its rank (one CTA per
+ * group).  A member id outside [-1, G.num_users) counts as an empty slot and sets IGMC_ERR_CANDIDATES, as do summed
+ * degrees beyond cap (the groups past it get empty rows).  1 <= width <= IGMC_GROUP_MAX, num_groups >= 1 (else -1). */
+int igmc_group_rows(const igmc_csr_t* G, const int32_t* members, int num_groups, int width, int32_t* row_ptr,
+                    int32_t* col_idx, int cap, int32_t* ws, int* err, void* stream);
+
+/* Position i < Gu*width, unit u = i / width, member slot j = i % width of group g = unit_g[u]: links_u = members[g][j],
+ * links_v = unit_v[u], pair_id = links_u * num_items + links_v (int64), tag = unit_tag[u].  An empty slot, and every
+ * position Gu*width..B-1 (as unit 0, slot 0), takes links_u = the group's first member (0 if it has none) and tag -1.
+ * A group outside [0, num_groups), an item outside [0, num_items) (the unit reads as group 0, item 0) or a member id
+ * outside [-1, num_users) (read as an empty slot) sets IGMC_ERR_CANDIDATES.  1 <= width <= min(B, IGMC_GROUP_MAX). */
+int igmc_group_pairs(const int32_t* members, int num_groups, int width, int num_users, int num_items,
+                     const int32_t* unit_g, const int32_t* unit_v, const int64_t* unit_tag, int B, int32_t* links_u,
+                     int32_t* links_v, int64_t* pair_id, int64_t* tag, int* err, void* stream);
+
+/* Per unit u < Gu of the batch, over its n real positions j (tag[u*width + j] >= 0) in member order: x_j = the fp32
+ * checkpoint mean of preds[.][u*width + j] (as igmc_topk_merge takes it) and the aggregate (IGMC_GROUP_AGG_*): mean =
+ * sum_j x_j in fp64 without fma contraction / n, rounded once to fp32; min / max = the smallest / largest x_j by strict
+ * compares, so an equal value (+0 and -0 too) resolves to the first in member order.  Any NaN x_j makes it NaN.
+ * key != NULL: key [Gu] = the aggregate of every unit (igmc_topk_merge with K = 1 and B = Gu then consumes it; a unit
+ * without real positions has key 0 and the merge skips its tag -1).  Otherwise, for the unit's tag t >= 0: score[t] and
+ * member_score[t * width + j] = x_j for the real positions, NaN for the others.  1 <= width <= min(B, IGMC_GROUP_MAX). */
+int igmc_group_stats(const float* preds, int K, int B, int width, int aggregate, const int64_t* tag, float* key,
+                     float* score, float* member_score, void* stream);
+
 /* ---- cached top-k lists repaired after a rating-graph update (csrc/recommend_cache.cu; igmc_b200/recommend.py:
  * RecommendationCache) ----
  * With h = 1 the edits (a_i, b_i) of an update can change the enclosing subgraph, and so the score, only of the pairs
