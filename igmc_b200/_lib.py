@@ -256,6 +256,12 @@ _SIGS = {
     "igmc_group_rows": [C.POINTER(CSR), vp, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp, vp],
     "igmc_group_pairs": [vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp],
     "igmc_group_stats": [vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp],
+    "igmc_diverse_ws_bytes": [C.c_int, C.c_int, C.c_int, C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int)],
+    "igmc_item_union": [vp, C.c_int64, C.c_int, vp, vp, vp, vp, vp, vp],
+    "igmc_cocount": [C.POINTER(CSR), vp, C.c_int, vp, C.c_int64, vp],
+    "igmc_diverse_select": [C.POINTER(CSR), vp, vp, C.c_int, C.c_int, C.c_int, C.c_float, vp, C.c_int, vp, vp, vp, vp,
+                            vp, vp],
+    "igmc_item_cosine": [C.POINTER(CSR), vp, C.c_int, vp, C.c_int, vp, vp, vp, vp],
     "igmc_rescore_plan_ws_bytes":[C.c_int, C.c_int, C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int)],
     "igmc_rescore_plan": [C.POINTER(CSR), vp, C.c_int, vp, vp, C.c_int, vp, C.c_int, C.c_int, vp, C.c_int64, vp, vp,
                           C.c_int64, vp, vp, vp, vp],

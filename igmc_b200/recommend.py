@@ -52,6 +52,9 @@ building a dataset of every candidate pair and looping over it in Python.  Here:
 * ``recommend_groups(model, graph, groups, k)`` -> per group of users the ``k`` best items none of them rated, ranked
   by the mean, minimum or maximum of the members' own scores (csrc/groups.cu); ``predict_groups(model, graph, groups,
   group, items)`` -> that aggregate and every member's score for explicit (group, item) queries;
+* ``recommend_diverse(model, graph, users, k, penalty)`` -> per user k items chosen greedily from its ``recommend``
+  pool, each by its score less ``penalty`` times its largest similarity to an item already chosen (csrc/diverse.cu);
+  ``item_similarity(graph, items)`` -> that similarity, the cosine of two items' binary rating columns, as a matrix;
 * ``RecommendationCache(model, graph, users, k)`` -> ``recommend``'s lists kept exact across ``graph.update``: an update
   rescores only the pairs whose h = 1 enclosing subgraph it can reach (csrc/recommend_cache.cu) and repairs the cached
   lists with them;
@@ -82,7 +85,8 @@ __all__ = ["predict_pairs", "recommend", "corated_items", "explain_pairs", "Expl
            "RatingSessions", "predict_sessions", "recommend_sessions", "corated_items_sessions", "recommend_users",
            "corated_users", "explain_nodes", "NodeExplanation", "attribute_nodes", "NodeAttribution", "predict_draws",
            "Draws", "counterfactual", "Counterfactual", "elicit", "question_impact", "QuestionImpact",
-           "RecommendationCache", "recommend_groups", "predict_groups", "GroupScores"]
+           "RecommendationCache", "recommend_groups", "predict_groups", "GroupScores", "recommend_diverse",
+           "item_similarity", "DiverseRecommendations"]
 
 
 # ---- input validation (host) ----------------------------------------------------------------------------------------
@@ -1397,6 +1401,140 @@ def recommend_groups_host(row_ptr, col_idx, num_items, members, k, aggregate, sc
     return top_i, top_s
 
 
+# ---- diversified lists and item similarity (csrc/diverse.cu) -------------------------------------------------------
+# The result of recommend_diverse, per query user: items [U, k] int64, scores [U, k] fp32 (each chosen item's model
+# score) and keys [U, k] fp32 (its penalised key when it was chosen); -1 / -inf / -inf past the pool's real entries.
+DiverseRecommendations = collections.namedtuple("DiverseRecommendations", "items scores keys")
+
+
+def _diverse_inputs(k, penalty, pool, batch_size):
+    """(k, pool, penalty) of a diverse run checked on the host: 1 <= k <= pool <= IGMC_TOPK_MAX, the pool fitting the
+    top-k merge at ``batch_size``, and penalty finite and >= 0 in fp32 (ValueError; -0 is taken as +0)"""
+    pool = _check_count(pool, "pool", _lib.TOPK_MAX)
+    k = _check_count(k, "k", _lib.TOPK_MAX)
+    if k > pool:
+        raise ValueError("k (%d) must not exceed pool (%d): the list is chosen from the pool" % (k, pool))
+    _check_merge_fits(pool, batch_size)
+    p = float(penalty)
+    with np.errstate(over="ignore"):
+        p = np.float32(p + 0.0) if p >= 0.0 else np.float32(np.nan)
+    if not np.isfinite(p):
+        raise ValueError("penalty must be finite and >= 0 in fp32, not %r" % (penalty,))
+    return k, pool, float(p)
+
+
+def item_union_host(items, num_items):
+    """twin of igmc_item_union: (map [num_items] int32, the union index of each item or -1; list [Nu] int32 ascending;
+    bad: an id outside [-1, num_items) was skipped)"""
+    items = np.asarray(items, np.int64).reshape(-1)
+    ok = (items >= 0) & (items < num_items)
+    bad = bool(((items < -1) | (items >= num_items)).any())
+    lst = np.unique(items[ok]).astype(np.int32)
+    mp = np.full(num_items, -1, np.int32)
+    mp[lst] = np.arange(len(lst), dtype=np.int32)
+    return mp, lst, bad
+
+
+def cocount_host(row_ptr, col_idx, num_users, num_items, union):
+    """twin of igmc_cocount: the upper triangle [Nu * (Nu - 1) / 2] uint32 of c = |col(a) & col(b)| over the union's
+    items (ascending, index i < j at i * (2 Nu - i - 1) / 2 + j - i - 1)"""
+    import scipy.sparse as ssp
+    union = np.asarray(union, np.int64)
+    nu = len(union)
+    rp = np.asarray(row_ptr, np.int64)
+    nnz = int(rp[num_users])
+    Bm = ssp.csr_matrix((np.ones(nnz, np.int64), np.asarray(col_idx[:nnz], np.int64), rp[:num_users + 1]),
+                        shape=(num_users, num_items))
+    Bu = Bm[:, union]
+    Cm = np.asarray((Bu.T @ Bu).toarray(), np.int64)
+    i, j = np.triu_indices(nu, 1)
+    return Cm[i, j].astype(np.uint32)
+
+
+def _tri_at(i, j, nu):
+    return i * (2 * nu - i - 1) // 2 + j - i - 1
+
+
+def item_cosine_host(c, da, db):
+    """twin of the kernels' cosine: c / sqrt(da * db) in Python floats (correctly rounded, as __ddiv_rn / __dsqrt_rn /
+    __dmul_rn), rounded once to fp32; 0 when da * db = 0"""
+    import math
+    da, db = int(da), int(db)
+    if da == 0 or db == 0:
+        return np.float32(0.0)
+    return np.float32(float(int(c)) / math.sqrt(float(da) * float(db)))
+
+
+def _cocount_at(table, nu, i, j, deg_i):
+    if i == j:
+        return int(deg_i)
+    a, b = min(i, j), max(i, j)
+    return int(table[_tri_at(a, b, nu)])
+
+
+def diverse_select_host(col_ptr, pool_item, pool_score, k, penalty, mp, table, nu):
+    """twin of igmc_diverse_select: (items [Q, k] int64, scores [Q, k] fp32, keys [Q, k] fp32, bad [Q] bool).  Per
+    query k greedy steps: key_j = score_j - penalty * m_j in fp32, the first unchosen real entry by ``_before`` with
+    the pool position as id, then m_j = max(m_j, sim(chosen, j)).  A query whose pool holds an id outside
+    [-1, num_items) or absent from ``mp`` is padding and flagged in bad"""
+    pool_item = np.asarray(pool_item, np.int64)
+    pool_score = np.asarray(pool_score, np.float32)
+    Q, P = pool_item.shape
+    ni = len(mp)
+    deg = np.diff(np.asarray(col_ptr, np.int64))
+    pen = np.float32(penalty)
+    out_i = np.full((Q, k), -1, np.int64)
+    out_s = np.full((Q, k), -np.inf, np.float32)
+    out_k = np.full((Q, k), -np.inf, np.float32)
+    bad = np.zeros(Q, bool)
+    for q in range(Q):
+        it, sc = pool_item[q], pool_score[q]
+        if ((it < -1) | (it >= ni)).any() or any(mp[v] < 0 or mp[v] >= nu for v in it[it >= 0]):
+            bad[q] = True
+            continue
+        live = it >= 0
+        idx = np.where(live, mp[np.clip(it, 0, ni - 1)], -1)
+        m = np.zeros(P, np.float32)
+        for s in range(k):
+            key = (sc - pen * m).astype(np.float32)            # fp32 product, then fp32 difference: no fma
+            best = -1
+            for j in np.flatnonzero(live):
+                if best < 0 or _before(key[j], j, key[best], best):
+                    best = int(j)
+            if best < 0:
+                break
+            out_i[q, s], out_s[q, s], out_k[q, s] = it[best], sc[best], key[best]
+            live[best] = False
+            c, dc = int(idx[best]), int(deg[it[best]])
+            for j in np.flatnonzero(live):
+                sim = item_cosine_host(_cocount_at(table, nu, int(idx[j]), c, deg[it[j]]), deg[it[j]], dc)
+                m[j] = max(m[j], sim)
+    return out_i, out_s, out_k, bad
+
+
+def item_similarity_host(row_ptr, col_idx, col_ptr, num_users, num_items, items):
+    """``item_similarity`` restated on the host: [Q, Q] fp32 of sim(items[a], items[b]) through the twins above"""
+    items = np.asarray(items, np.int64).reshape(-1)
+    mp, lst, _ = item_union_host(items, num_items)
+    table = cocount_host(row_ptr, col_idx, num_users, num_items, lst)
+    deg = np.diff(np.asarray(col_ptr, np.int64))
+    out = np.zeros((len(items), len(items)), np.float32)
+    for a, x in enumerate(items):
+        for b, y in enumerate(items):
+            out[a, b] = item_cosine_host(_cocount_at(table, len(lst), mp[x], mp[y], deg[x]), deg[x], deg[y])
+    return out
+
+
+def recommend_diverse_host(row_ptr, col_idx, col_ptr, num_users, num_items, users, k, penalty, pooler, pool=50):
+    """``recommend_diverse`` restated on the host: ``pooler(users, pool)`` -> (items [U, pool], scores [U, pool]), the
+    pools (``recommend``'s lists), then the union, the co-counts and the greedy selection by the twins.  Returns
+    (items, scores, keys) as ``DiverseRecommendations``' fields"""
+    pool_i, pool_s = (np.asarray(a) for a in pooler(users, pool))
+    mp, lst, _ = item_union_host(pool_i, num_items)
+    table = cocount_host(row_ptr, col_idx, num_users, num_items, lst)
+    return diverse_select_host(col_ptr, pool_i, pool_s, k, penalty, mp, table, len(lst))[:3]
+
+
 class _TrialRows(object):
     """one batch slot's trial rows of a counterfactual or question-impact pass, and their igmc_sessions_t (``_c``):
     what ``SubgraphExtractor.extract`` takes as ``sessions``"""
@@ -1423,11 +1561,12 @@ class InferenceEngine(object):
                                                # or start_counterfactual(users, items, rivals, max_removals)
                                                # or start_elicit(sessions, n, targets) / start_question_impact(...)
                                                # or start_recommend_groups(groups, k) / start_group_pairs(...)
+                                               # or start_recommend_diverse(users, k, penalty, pool)
         while eng.step():
             pass
         top_items, top_scores = eng.finish()   # (predict: scores; explain: an Explanation; attribute: an Attribution;
                                                # counterfactual: a Counterfactual; question_impact: a QuestionImpact;
-                                               # group pairs: a GroupScores)
+                                               # group pairs: a GroupScores; diverse: DiverseRecommendations)
 
     An engine serves across updates of its ``RatingGraph`` (``graph.update``) between runs; an update during a run
     makes its next ``step`` raise RuntimeError.
@@ -1476,6 +1615,7 @@ class InferenceEngine(object):
         self.run = None
         self._retrieve_ws = {}       # the retriever's workspace when its histograms do not fit in shared memory
         self._grad_plans = {}        # the model's plan cache while a gradient pass forces the L2 plan
+        self.diverse_ws_bytes = 0    # bound of a diverse run's co-count table (<= 0: 256 MB); past it users run in chunks
 
     # ---- one run: plan, prime, steps, finish --------------------------------------------------------------------
     def start_recommend(self, users, k, items=None, exclude_rated=True, retrieve=None, draws=None, beta=0.0,
@@ -1885,6 +2025,52 @@ class InferenceEngine(object):
                    "igmc_group_stats")
         if rank:
             self._merge_unit_keys(s)
+
+    # ---- diversified lists -----------------------------------------------------------------------------------------
+    def start_recommend_diverse(self, users, k, penalty, pool=50, items=None, exclude_rated=True, retrieve=None):
+        """plan a diversified ranking run (``recommend_diverse``): the ranking run of ``start_recommend(users, pool,
+        ...)``, whose lists are the pools; ``finish`` then chooses k items from each.  Returns the number of candidate
+        pairs."""
+        k, pool, penalty = _diverse_inputs(k, penalty, pool, self.B)
+        P = self.start_recommend(users, pool, items, exclude_rated, retrieve)
+        self.run["diverse"] = (k, penalty)
+        return P
+
+    def _diverse(self, pool_i, pool_s, k, penalty):
+        """the diverse stage over finished pools [U, pool]: per chunk of users (``diverse_ws_bytes`` bounds the
+        co-count table) the union of its pools, the co-counts over it and the greedy selection.  One host sync per
+        chunk (Nu with the error word).  Returns the ``DiverseRecommendations``."""
+        U, pool = pool_i.shape
+        g, dev, lib, err = self.graph, self.dev, self.lib, self.extractor.err
+        out = DiverseRecommendations(torch.full((U, k), -1, dtype=torch.int64, device=dev),
+                                     torch.full((U, k), -float("inf"), dtype=torch.float32, device=dev),
+                                     torch.full((U, k), -float("inf"), dtype=torch.float32, device=dev))
+        if U == 0:
+            return out
+        nbytes, chunk = C.c_int64(0), C.c_int(0)
+        _lib.check(lib.igmc_diverse_ws_bytes(U, pool, g.num_items, int(self.diverse_ws_bytes), C.byref(nbytes),
+                                             C.byref(chunk)), "igmc_diverse_ws_bytes")
+        i32 = dict(dtype=torch.int32, device=dev)
+        bitmap, mp = torch.empty((g.num_items + 31) // 32, **i32), torch.empty(g.num_items, **i32)
+        lst, nu = torch.empty(g.num_items, **i32), torch.empty(1, **i32)
+        table = torch.empty(max(nbytes.value // 4, 1), **i32)
+        for c0 in range(0, U, chunk.value):
+            n = min(chunk.value, U - c0)
+            _lib.check(lib.igmc_item_union(pool_i[c0].data_ptr(), n * pool, g.num_items, bitmap.data_ptr(),
+                                           mp.data_ptr(), lst.data_ptr(), nu.data_ptr(), err.data_ptr(),
+                                           _stream_ptr()), "igmc_item_union")
+            Nu, code = (int(x) for x in torch.cat([nu, err]).cpu())          # the chunk's host sync
+            if code:
+                err.zero_()
+            _lib.check_kernel_error(code)
+            _lib.check(lib.igmc_cocount(C.byref(g._c), mp.data_ptr(), Nu, table.data_ptr(), table.numel(),
+                                        _stream_ptr()), "igmc_cocount")
+            _lib.check(lib.igmc_diverse_select(C.byref(g._c), pool_i[c0].data_ptr(), pool_s[c0].data_ptr(), n, pool,
+                                               k, penalty, mp.data_ptr(), Nu, table.data_ptr(),
+                                               out.items[c0].data_ptr(), out.scores[c0].data_ptr(),
+                                               out.keys[c0].data_ptr(), err.data_ptr(), _stream_ptr()),
+                       "igmc_diverse_select")
+        return out
 
     def _trial_pass(self):
         """the next pass of a counterfactual run: the offsets of the queries' trial counts, their total T (the pass's
@@ -2383,6 +2569,8 @@ class InferenceEngine(object):
             self.extractor.err.zero_()
         _lib.check_kernel_error(code)
         self.run = None
+        if run.get("diverse"):
+            return self._diverse(run["top_i"], run["top_s"], *run["diverse"])
         if run["kind"] == "recommend":
             return run["top_i"], run["top_s"]
         if run["kind"] in _EXPLAIN_RESULTS:
@@ -2485,6 +2673,10 @@ class InferenceEngine(object):
 
     def predict_groups(self, groups, group, items, aggregate="mean"):
         self.start_group_pairs(groups, group, items, aggregate)
+        return self.finish()
+
+    def recommend_diverse(self, users, k, penalty, pool=50, items=None, exclude_rated=True, retrieve=None):
+        self.start_recommend_diverse(users, k, penalty, pool, items, exclude_rated, retrieve)
         return self.finish()
 
     def attribute_nodes(self, users, items, m=None):
@@ -3100,3 +3292,56 @@ def predict_groups(model, graph, groups, group, items, *, aggregate="mean", h=1,
                            torch.zeros(0, members.shape[1], dtype=torch.float32, device=dev))
     return _on_engine(model, graph, lambda eng: eng.predict_groups(members, grp, items, aggregate),
                       h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
+
+
+# ---- diversified lists and item similarity: public API ----------------------------------------------------------------
+def recommend_diverse(model, graph, users, k, penalty, *, pool=50, items=None, exclude_rated=True, retrieve=None, h=1,
+                      sample_ratio=1.0, max_nodes_per_hop=None, batch_size=256, checkpoints=None, sample_seed=0):
+    """per query user ``k`` items chosen from its pool so that the list is not spent on near-duplicates: a
+    ``DiverseRecommendations`` of items [U, k] int64, scores [U, k] fp32 (the model scores) and keys [U, k] fp32, on the
+    model's device.  The pool is exactly ``recommend(model, graph, users, pool, items=, exclude_rated=, retrieve=,
+    ...)``.  Step s chooses the unchosen pool entry of the largest key score - penalty * m, m its largest
+    ``item_similarity`` to an entry already chosen (0 at the first step), in fp32; equal keys by pool position, NaN
+    last; ``keys`` holds each item's key when it was chosen.  Slots past the pool's real entries hold -1 / -inf / -inf.
+    ``penalty``: rating units per unit of similarity, finite and >= 0 (ValueError); at 0 the result is ``recommend(...,
+    k)`` with keys == scores.  1 <= k <= pool <= IGMC_TOPK_MAX (k > pool: ValueError), and ``pool`` must fit the top-k
+    merge at ``batch_size``."""
+    k, pool, penalty = _diverse_inputs(k, penalty, pool, batch_size)
+    users = _host_ids(users, "users", graph.shape[0])
+    _ranking_inputs(pool, batch_size, items, retrieve, len(users), graph.shape[1])
+    if len(users) == 0:
+        dev = model.flat_params.device
+        return DiverseRecommendations(torch.zeros(0, k, dtype=torch.int64, device=dev),
+                                      torch.zeros(0, k, dtype=torch.float32, device=dev),
+                                      torch.zeros(0, k, dtype=torch.float32, device=dev))
+    return _on_engine(model, graph, lambda eng: eng.recommend_diverse(users, k, penalty, pool, items, exclude_rated,
+                                                                      retrieve),
+                      h, sample_ratio, max_nodes_per_hop, batch_size, checkpoints, sample_seed)
+
+
+def item_similarity(graph, items):
+    """[Q, Q] fp32 on the graph's device: sim(items[a], items[b]) = c / sqrt(d_a * d_b), c the number of users who rated
+    both (whatever the value) and d the items' rating counts, evaluated in fp64 with every operation correctly rounded
+    and rounded once; 0 when an item has no ratings, 1 on the diagonal otherwise.  The similarity ``recommend_diverse``
+    penalises, from the same kernels.  Repeated ids are allowed; IndexError for an id outside the graph."""
+    g = graph
+    if g.device is None:
+        raise RuntimeError("igmc_b200 item similarity runs on a CUDA device (there is no CPU path)")
+    ids = _host_ids(items, "items", g.num_items)
+    Q, dev, lib = len(ids), g.device, _lib.load()
+    out = torch.empty(Q, Q, dtype=torch.float32, device=dev)
+    if Q == 0:
+        return out
+    Nu = len(np.unique(ids))
+    i32 = dict(dtype=torch.int32, device=dev)
+    dids = torch.from_numpy(ids).to(dev)
+    bitmap, mp = torch.empty((g.num_items + 31) // 32, **i32), torch.empty(g.num_items, **i32)
+    lst, nu, err = torch.empty(g.num_items, **i32), torch.empty(1, **i32), torch.zeros(1, **i32)
+    table = torch.empty(max(Nu * (Nu - 1) // 2, 1), **i32)
+    _lib.check(lib.igmc_item_union(dids.data_ptr(), Q, g.num_items, bitmap.data_ptr(), mp.data_ptr(), lst.data_ptr(),
+                                   nu.data_ptr(), err.data_ptr(), _stream_ptr()), "igmc_item_union")
+    _lib.check(lib.igmc_cocount(C.byref(g._c), mp.data_ptr(), Nu, table.data_ptr(), table.numel(), _stream_ptr()),
+               "igmc_cocount")
+    _lib.check(lib.igmc_item_cosine(C.byref(g._c), dids.data_ptr(), Q, mp.data_ptr(), Nu, table.data_ptr(),
+                                    out.data_ptr(), err.data_ptr(), _stream_ptr()), "igmc_item_cosine")
+    return out

@@ -965,6 +965,47 @@ int igmc_group_pairs(const int32_t* members, int num_groups, int width, int num_
 int igmc_group_stats(const float* preds, int K, int B, int width, int aggregate, const int64_t* tag, float* key,
                      float* score, float* member_score, void* stream);
 
+/* ---- diversified lists and item-item similarity (csrc/diverse.cu; igmc_b200/recommend.py: recommend_diverse,
+ * item_similarity) ----
+ * sim(a, b) = c_ab / sqrt(d_a * d_b): c_ab = |col(a) & col(b)| (users who rated both, whatever the value), d_a the
+ * column degree (G.col_ptr), evaluated as (double)c / __dsqrt_rn(__dmul_rn((double)d_a, (double)d_b)) with every
+ * operation correctly rounded and rounded once to fp32; 0 when d_a * d_b = 0, so sim(a, a) = 1 for a rated item.  The
+ * counts are kept for a union of Nu items only, each with a dense index (its rank in item order): table[t(i, j)] = c of
+ * the items of union indices i < j, t(i, j) = i * (2 Nu - i - 1) / 2 + j - i - 1, Nu * (Nu - 1) / 2 uint32 entries. */
+
+/* The co-count table of a diverse run over num_query pools of `pool` items: *table_bytes for the largest union a chunk
+ * of *chunk queries can have, min(chunk * pool, num_items) items.  `bound` (<= 0: 256 MB) caps the table: past it the
+ * queries run in chunks of *chunk (written when chunk != NULL), never fewer than one. */
+int igmc_diverse_ws_bytes(int num_query, int pool, int num_items, int64_t bound, int64_t* table_bytes, int* chunk);
+
+/* The union of items [n] (int64; -1 = padding, skipped): bitmap [ceil(num_items / 32)] (zeroed here, then an integer
+ * atomicOr per item), then one CTA's popcount scan writes map [num_items] (the item's union index, -1 where absent),
+ * list [*nu] (the union, ascending) and *nu.  An id outside [-1, num_items) sets IGMC_ERR_CANDIDATES and is skipped. */
+int igmc_item_union(const int64_t* items, int64_t n, int num_items, uint32_t* bitmap, int32_t* map, int32_t* list,
+                    int32_t* nu, int* err, void* stream);
+
+/* table[t(i, j)] = the number of users of G whose row holds the items of union indices i < j (map from
+ * igmc_item_union, nu its size).  Zeroes the table, then one CTA per row adds 1 per pair of the row's union entries with
+ * an integer atomicAdd (rows are tiled, any length is exact): bit-identical across runs.  -2 when table_cap (entries)
+ * is below nu * (nu - 1) / 2. */
+int igmc_cocount(const igmc_csr_t* G, const int32_t* map, int nu, uint32_t* table, int64_t table_cap, void* stream);
+
+/* Greedy diversified selection, one CTA per query q over its pool pool_item / pool_score [num_query, pool] (a
+ * recommend list: item -1 = padding).  Before step s < k, each unchosen real entry j has m_j, its largest sim to an
+ * entry already chosen (0 at the first step), and key_j = __fsub_rn(score_j, __fmul_rn(penalty, m_j)); the step chooses
+ * the entry first under ranks_before (csrc/topk_merge.cuh) with the pool position as id.  out_item / out_score / out_key
+ * [num_query, k]: the chosen item, its pool score and its key when chosen; -1 / -inf / -inf past the real entries.  A
+ * pool item outside [-1, G.num_items) or absent from the map sets IGMC_ERR_CANDIDATES and the query's row becomes
+ * padding.  1 <= k <= pool <= IGMC_TOPK_MAX, penalty finite and >= 0 (else -1). */
+int igmc_diverse_select(const igmc_csr_t* G, const int64_t* pool_item, const float* pool_score, int num_query, int pool,
+                        int k, float penalty, const int32_t* map, int nu, const uint32_t* table, int64_t* out_item,
+                        float* out_score, float* out_key, int* err, void* stream);
+
+/* out [Q, Q] = sim(items[a], items[b]) (repeats allowed), with the map and table of a union holding every item.  An id
+ * outside the graph or the union sets IGMC_ERR_CANDIDATES and its entries are 0. */
+int igmc_item_cosine(const igmc_csr_t* G, const int64_t* items, int Q, const int32_t* map, int nu,
+                     const uint32_t* table, float* out, int* err, void* stream);
+
 /* ---- cached top-k lists repaired after a rating-graph update (csrc/recommend_cache.cu; igmc_b200/recommend.py:
  * RecommendationCache) ----
  * With h = 1 the edits (a_i, b_i) of an update can change the enclosing subgraph, and so the score, only of the pairs
