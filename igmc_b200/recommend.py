@@ -1762,21 +1762,31 @@ class InferenceEngine(object):
         d = _draw_inputs(draws, 0.0, draw_seed, self.B)
         users, items, _ = _host_pairs(self.graph.shape, users, items)
         P, S, f32 = len(users), d["S"], dict(dtype=torch.float32, device=self.dev)
-        return self._start_explicit("draws", users, items, value=torch.empty(P, S, **f32),
-                                    mean=torch.empty(P, **f32), std=torch.empty(P, **f32), **self._draw_run(d))
+        out = Draws(torch.empty(P, S, **f32), torch.empty(P, **f32), torch.empty(P, **f32))
+        return self._start_explicit("draws", users, items, **self._draw_run(d, out))
 
-    def _draw_run(self, d):
-        """the run fields of a run over draws (``_draw_inputs``' dict d, or None: none), the slots' draw buffers
-        allocated: per slot the G pairs of a batch before their expansion, the draw index and the hidden mask"""
+    def _draw_run(self, d, out=None):
+        """the run fields of a run over draws (``_draw_inputs``' dict d, or None: none): units of S draws of a pair
+        (``_unit_run``, ``out`` the Draws of an explicit run), the slots' draw index and hidden mask allocated"""
         if d is None:
             return {}
-        i32, i64 = dict(dtype=torch.int32, device=self.dev), dict(dtype=torch.int64, device=self.dev)
+        S, beta = d["S"], d["beta"]
+
+        def fan_out(s, err):
+            _lib.check(self.lib.igmc_draws_expand(S, self.B, s["gu"].data_ptr(), s["gv"].data_ptr(),
+                                                  s["gpid"].data_ptr(), s["gtag"].data_ptr(), s["u"].data_ptr(),
+                                                  s["v"].data_ptr(), s["pid"].data_ptr(), s["tag"].data_ptr(),
+                                                  s["draw"].data_ptr(), _stream_ptr()), "igmc_draws_expand")
+
+        def reduce(preds, s, key, value=None, mean=None, std=None):
+            _lib.check(self.lib.igmc_draws_stats(preds.data_ptr(), self.K, self.B, S, s["tag"].data_ptr(), beta,
+                                                 *(_lib.ptr(t) for t in (value, mean, std, key)), _stream_ptr()),
+                       "igmc_draws_stats")
         for s in self.slots:
             if "draw" not in s:
-                s.update(gu=torch.zeros(self.B, **i32), gv=torch.zeros(self.B, **i32), gpid=torch.zeros(self.B, **i64),
-                         gtag=torch.zeros(self.B, **i64), draw=torch.zeros(self.B, **i32),
+                s.update(draw=torch.zeros(self.B, dtype=torch.int32, device=self.dev),
                          hkeep=torch.ones(self.B * _lib.LIN1_OUT, dtype=torch.uint8, device=self.dev))
-        return dict(d, G=self.B // d["S"], keys=torch.empty(self.B, dtype=torch.float32, device=self.dev))
+        return dict(d, **self._unit_run(self.B // S, fan_out, reduce, out))
 
     def _draw_masks(self):
         """each slot's edge mask sized for the extractor's batch edge capacity, and its dropout descriptor: the
@@ -1904,7 +1914,9 @@ class InferenceEngine(object):
         answer means.  ValueError for a question the session already rated.  Returns the number of units."""
         sessions = self._session_slots(sessions)
         sess, q = _question_units(sessions, session, questions)
-        fields = self._elicit_run(sessions, targets, sess)
+        f32 = dict(dtype=torch.float32, device=self.dev)
+        out = QuestionImpact(torch.empty(len(sess), **f32), torch.empty(len(sess), self.model.num_relations, **f32))
+        fields = self._elicit_run(sessions, targets, sess, out)
         if len(sess):
             rp, ci, _ = sessions.rows()
             for s, item in zip(sess, q):
@@ -1913,52 +1925,48 @@ class InferenceEngine(object):
                 if p < len(row) and row[p] == item:
                     raise ValueError("session %d already rated item %d: a rated item is not a question"
                                      % (int(s), int(item)))
-        f32 = dict(dtype=torch.float32, device=self.dev)
-        return self._start_explicit("question_impact", sess, q, sessions=sessions,
-                                    impact=torch.empty(len(sess), **f32),
-                                    answer_mean=torch.empty(len(sess), fields["A"], **f32), **fields)
+        return self._start_explicit("question_impact", sess, q, sessions=sessions, **fields)
 
-    def _elicit_run(self, sessions, targets, queried):
-        """the run fields of a question-impact run (``_elicit_targets``' targets on the device, the answers A, target
-        width W, units per batch G and the trial rows' longest row), the slots' unit and trial-row buffers allocated"""
-        A, dev = self.model.num_relations, self.dev
+    def _elicit_run(self, sessions, targets, queried, out=None):
+        """the run fields of a question-impact run: units (session, question) of A answers x W targets
+        (``_unit_run``, ``out`` the QuestionImpact of an explicit run) over ``_elicit_targets``' targets, and the trial
+        rows' longest row; the slots' trial rows allocated"""
+        A = self.model.num_relations
         t, per = _elicit_targets(targets, sessions.num_sessions, self.graph.num_items, A, self.B, queried)
-        W = t.shape[1]
+        W, t = t.shape[1], torch.from_numpy(t).to(self.dev)
         L = sessions.max_row_deg + 1            # a trial row: the session row and the question
         self._trial_rows(self.B // W, L)        # G * A <= B / W trial rows per batch
-        self._unit_buffers()
-        G = self.B // (A * W)
-        return dict(A=A, W=W, G=G, targets=torch.from_numpy(t).to(dev), per_session=per, row_deg=L,
-                    keys=torch.empty(G, dtype=torch.float32, device=dev))
 
-    def _unit_buffers(self):
-        """each slot's unit stream: the G units of a batch (query slot, candidate, pair id, tag) before the kernel
-        that lays them out over the B positions"""
+        def fan_out(s, err):
+            # per answer its trial row as session g * A + a, extracted in session mode
+            tr = s["trial"]
+            _lib.check(self.lib.igmc_elicit_pairs(C.byref(sessions._c), self.graph.num_items, A, t.data_ptr(), W, per,
+                                                  s["gu"].data_ptr(), s["gv"].data_ptr(), s["gtag"].data_ptr(), self.B,
+                                                  s["u"].data_ptr(), s["v"].data_ptr(), s["pid"].data_ptr(),
+                                                  s["tag"].data_ptr(), tr.users.data_ptr(), tr.row_ptr.data_ptr(),
+                                                  tr.col_idx.data_ptr(), tr.rating.data_ptr(), tr.cap,
+                                                  s["sess"].data_ptr(), err, _stream_ptr()), "igmc_elicit_pairs")
+
+        def reduce(preds, s, key, impact=None, answer_mean=None):
+            _lib.check(self.lib.igmc_elicit_stats(preds.data_ptr(), self.K, self.B, A, W, s["tag"].data_ptr(),
+                                                  *(_lib.ptr(x) for x in (key, impact, answer_mean)), _stream_ptr()),
+                       "igmc_elicit_stats")
+        return dict(A=A, row_deg=L, **self._unit_run(self.B // (A * W), fan_out, reduce, out))
+
+    def _unit_run(self, G, fan_out, reduce, out=None):
+        """the run fields of a run over units, the slots' unit buffers allocated.  Each batch takes G units (query
+        slot, candidate, pair id, tag) of the candidate stream into the slot's gu / gv / gpid / gtag, and
+        ``fan_out(s, err)`` spreads unit g of slot ``s`` over the positions [g * B / G, (g + 1) * B / G) with the
+        tail positions tagged -1.  After the forward, ``reduce(preds, s, key, *out)`` turns each unit's positions into
+        one value: with ``out`` None (a ranking run) one key per unit into keys [G], merged into the top-k lists by
+        the unit's candidate; else the explicit run's outputs ``out``, scattered by the unit's tag."""
         i32, i64 = dict(dtype=torch.int32, device=self.dev), dict(dtype=torch.int64, device=self.dev)
         for s in self.slots:
             if "gu" not in s:
                 s.update(gu=torch.zeros(self.B, **i32), gv=torch.zeros(self.B, **i32), gpid=torch.zeros(self.B, **i64),
                          gtag=torch.zeros(self.B, **i64))
-
-    def _merge_unit_keys(self, s):
-        """a ranking run over units: the batch's G unit keys (run["keys"]) merged into the running top-k lists of
-        their query slots, ranked by the units' candidates (items, or users on an item-side run)"""
-        run = self.run
-        _lib.check(self.lib.igmc_topk_merge(run["keys"].data_ptr(), 1, run["G"], s["gtag"].data_ptr(),
-                                            s["gv"].data_ptr(), run["k"], run["top_s"].data_ptr(),
-                                            run["top_i"].data_ptr(), _stream_ptr()), "igmc_topk_merge")
-
-    def _elicit_stats(self, preds, s):
-        """a batch of units: per unit its impact merged into its session's top-n list (ranking), or its impact and
-        answer means scattered to its index"""
-        run, st = self.run, _stream_ptr()
-        rank = run["kind"] == "recommend"
-        outs = (run["keys"], None, None) if rank else (None, run["impact"], run["answer_mean"])
-        _lib.check(self.lib.igmc_elicit_stats(preds.data_ptr(), self.K, self.B, run["A"], run["W"],
-                                              s["tag"].data_ptr(), *(_lib.ptr(t) for t in outs), st),
-                   "igmc_elicit_stats")
-        if rank:
-            self._merge_unit_keys(s)
+        keys = torch.empty(G, dtype=torch.float32, device=self.dev) if out is None else None
+        return dict(G=G, fan_out=fan_out, reduce=reduce, keys=keys, out=out)
 
     # ---- group recommendation -----------------------------------------------------------------------------------
     def start_recommend_groups(self, groups, k, aggregate="mean", items=None, exclude_rated=True, retrieve=None,
@@ -1971,7 +1979,7 @@ class InferenceEngine(object):
         g = self.graph
         members = _group_members(groups, g.num_users, self.B)
         k, _, cand, rows = _ranking_inputs(k, self.B, items, None, len(members), g.num_items)
-        fields = self._group_run(members, aggregate, union=True)
+        fields = self._group_run(members, aggregate)
         slots = torch.arange(len(members), dtype=torch.int32, device=self.dev)
         return self._plan_ranking(slots, k, None, cand, rows, exclude_rated, lambda: fields["cap"], None, None,
                                   **fields)
@@ -1981,23 +1989,33 @@ class InferenceEngine(object):
         each member's score.  Rated items are scored like any other.  Returns the number of queries."""
         members = _group_members(groups, self.graph.num_users, self.B)
         grp, items, _ = _host_pairs((len(members), self.graph.num_items), group, items, first="group")
-        fields = self._group_run(members, aggregate, union=False)
-        member_scores = torch.full((len(grp), members.shape[1]), float("nan"), dtype=torch.float32, device=self.dev)
-        return self._start_explicit("group_pairs", grp, items, member_scores=member_scores, **fields)
+        f32 = dict(dtype=torch.float32, device=self.dev)
+        out = GroupScores(torch.empty(len(grp), **f32), torch.full((len(grp), members.shape[1]), float("nan"), **f32))
+        return self._start_explicit("group_pairs", grp, items, **self._group_run(members, aggregate, out))
 
-    def _group_run(self, members, aggregate, union):
-        """the run fields of a group run over ``_group_members``' array: the members on the device, the width M, the
-        aggregate's code, Gu = B / M units per batch and the CSR view of the groups the candidate kernels read - with
-        ``union``, the union rows of igmc_group_rows (no host sync: their capacity, the summed member degrees, comes from
-        the host row pointers).  The slots' unit buffers are allocated."""
+    def _group_run(self, members, aggregate, out=None):
+        """the run fields of a group run over ``_group_members``' array: units (group, item) of one position per
+        member (``_unit_run``, ``out`` the GroupScores of an explicit run), the members on the device, the width M,
+        and the CSR view of the groups the candidate kernels read - on a ranking run, the union rows of
+        igmc_group_rows (no host sync: their capacity, the summed member degrees, comes from the host row pointers)"""
         agg = _check_aggregate(aggregate)
         Gn, M = members.shape
         g, dev = self.graph, self.dev
-        self._unit_buffers()
-        f = dict(groups=torch.from_numpy(members).to(dev), width=M, agg=agg, G=self.B // M, cap=0,
-                 keys=torch.empty(self.B // M, dtype=torch.float32, device=dev),
-                 group_view=_lib.CSR(None, None, None, None, None, Gn, g.num_items))
-        if not union or Gn == 0:
+        groups = torch.from_numpy(members).to(dev)
+
+        def fan_out(s, err):
+            _lib.check(self.lib.igmc_group_pairs(groups.data_ptr(), Gn, M, g.num_users, g.num_items,
+                                                 s["gu"].data_ptr(), s["gv"].data_ptr(), s["gtag"].data_ptr(), self.B,
+                                                 s["u"].data_ptr(), s["v"].data_ptr(), s["pid"].data_ptr(),
+                                                 s["tag"].data_ptr(), err, _stream_ptr()), "igmc_group_pairs")
+
+        def reduce(preds, s, key, scores=None, member_scores=None):
+            _lib.check(self.lib.igmc_group_stats(preds.data_ptr(), self.K, self.B, M, agg, s["tag"].data_ptr(),
+                                                 *(_lib.ptr(t) for t in (key, scores, member_scores)), _stream_ptr()),
+                       "igmc_group_stats")
+        f = dict(groups=groups, cap=0, group_view=_lib.CSR(None, None, None, None, None, Gn, g.num_items),
+                 **self._unit_run(self.B // M, fan_out, reduce, out))
+        if out is not None or Gn == 0:
             return f
         rp = g.host["row_ptr"]
         m = members[members >= 0].astype(np.int64)
@@ -2007,24 +2025,12 @@ class InferenceEngine(object):
         i32 = dict(dtype=torch.int32, device=dev)
         f["union"] = (torch.empty(Gn + 1, **i32), torch.empty(max(cap, 1), **i32))
         ws = torch.empty(2 * Gn + 1 + cap, **i32)
-        _lib.check(self.lib.igmc_group_rows(C.byref(g._c), f["groups"].data_ptr(), Gn, M, f["union"][0].data_ptr(),
+        _lib.check(self.lib.igmc_group_rows(C.byref(g._c), groups.data_ptr(), Gn, M, f["union"][0].data_ptr(),
                                             f["union"][1].data_ptr(), cap, ws.data_ptr(),
                                             self.extractor.err.data_ptr(), _stream_ptr()), "igmc_group_rows")
         f["group_view"] = _lib.CSR(f["union"][0].data_ptr(), f["union"][1].data_ptr(), None, None, None, Gn,
                                    g.num_items)
         return f
-
-    def _group_stats(self, preds, s):
-        """a batch of group units: per unit its aggregate merged into its group's top-k list (ranking), or its
-        aggregate and member scores scattered to its query index"""
-        run = self.run
-        rank = run["kind"] == "recommend"
-        outs = (run["keys"], None, None) if rank else (None, run["scores"], run["member_scores"])
-        _lib.check(self.lib.igmc_group_stats(preds.data_ptr(), self.K, self.B, run["width"], run["agg"],
-                                             s["tag"].data_ptr(), *(_lib.ptr(t) for t in outs), _stream_ptr()),
-                   "igmc_group_stats")
-        if rank:
-            self._merge_unit_keys(s)
 
     # ---- diversified lists -----------------------------------------------------------------------------------------
     def start_recommend_diverse(self, users, k, penalty, pool=50, items=None, exclude_rated=True, retrieve=None):
@@ -2323,7 +2329,7 @@ class InferenceEngine(object):
         # question-impact run (a session row and the question), else a session run's
         row_deg = run["row_deg"] if "row_deg" in run else sessions.max_row_deg if sessions is not None else 0
         self.extractor.serve_sessions(row_deg)
-        per = run.get("G", self.B)      # pairs per batch: G on a run over draws, G units on a question-impact run
+        per = run["G"] if "fan_out" in run else self.B      # pairs per batch, or units on a run over units
         run["steps"] = ((run["P"] if total is None else total) + per - 1) // per
         if run.get("S"):
             self._draw_masks()
@@ -2358,43 +2364,15 @@ class InferenceEngine(object):
                                                      self.cursor.data_ptr(), self.B, s["u"].data_ptr(),
                                                      s["v"].data_ptr(), s["pid"].data_ptr(), s["tag"].data_ptr(),
                                                      s["j"].data_ptr(), err, _stream_ptr()), "igmc_occlusion_pairs")
-        elif run.get("A"):
-            # G units (session, question), then A x W positions each and per answer its trial row as session
-            # g * A + a, extracted in session mode
+        elif "fan_out" in run:
+            # G units, then the run's fan-out over the B positions (``_unit_run``)
             _lib.check(self.lib.igmc_candidate_pairs(C.byref(self._csr(run)), C.byref(run["Cd"]),
                                                      self.cursor.data_ptr(), run["G"], s["gu"].data_ptr(),
                                                      s["gv"].data_ptr(), s["gpid"].data_ptr(), s["gtag"].data_ptr(),
                                                      err, _stream_ptr()), "igmc_candidate_pairs")
-            t = s["trial"]
-            _lib.check(self.lib.igmc_elicit_pairs(C.byref(sessions._c), self.graph.num_items, run["A"],
-                                                  run["targets"].data_ptr(), run["W"], run["per_session"],
-                                                  s["gu"].data_ptr(), s["gv"].data_ptr(), s["gtag"].data_ptr(), self.B,
-                                                  s["u"].data_ptr(), s["v"].data_ptr(), s["pid"].data_ptr(),
-                                                  s["tag"].data_ptr(), t.users.data_ptr(), t.row_ptr.data_ptr(),
-                                                  t.col_idx.data_ptr(), t.rating.data_ptr(), t.cap,
-                                                  s["sess"].data_ptr(), err, _stream_ptr()), "igmc_elicit_pairs")
-            sessions = t
-        elif run.get("width"):
-            # Gu units (group, item), then one position per member
-            _lib.check(self.lib.igmc_candidate_pairs(C.byref(self._csr(run)), C.byref(run["Cd"]),
-                                                     self.cursor.data_ptr(), run["G"], s["gu"].data_ptr(),
-                                                     s["gv"].data_ptr(), s["gpid"].data_ptr(), s["gtag"].data_ptr(),
-                                                     err, _stream_ptr()), "igmc_candidate_pairs")
-            _lib.check(self.lib.igmc_group_pairs(run["groups"].data_ptr(), int(run["groups"].shape[0]), run["width"],
-                                                 self.graph.num_users, self.graph.num_items, s["gu"].data_ptr(),
-                                                 s["gv"].data_ptr(), s["gtag"].data_ptr(), self.B, s["u"].data_ptr(),
-                                                 s["v"].data_ptr(), s["pid"].data_ptr(), s["tag"].data_ptr(), err,
-                                                 _stream_ptr()), "igmc_group_pairs")
-        elif run.get("S"):
-            # G pairs, then S consecutive draws of each over the B positions
-            _lib.check(self.lib.igmc_candidate_pairs(C.byref(self._csr(run)), C.byref(run["Cd"]),
-                                                     self.cursor.data_ptr(), run["G"], s["gu"].data_ptr(),
-                                                     s["gv"].data_ptr(), s["gpid"].data_ptr(), s["gtag"].data_ptr(),
-                                                     err, _stream_ptr()), "igmc_candidate_pairs")
-            _lib.check(self.lib.igmc_draws_expand(run["S"], self.B, s["gu"].data_ptr(), s["gv"].data_ptr(),
-                                                  s["gpid"].data_ptr(), s["gtag"].data_ptr(), s["u"].data_ptr(),
-                                                  s["v"].data_ptr(), s["pid"].data_ptr(), s["tag"].data_ptr(),
-                                                  s["draw"].data_ptr(), _stream_ptr()), "igmc_draws_expand")
+            run["fan_out"](s, err)
+            if run.get("A"):
+                sessions = s["trial"]        # a question-impact unit's trial rows are its sessions
         else:
             _lib.check(self.lib.igmc_candidate_pairs(C.byref(self._csr(run)), C.byref(run["Cd"]),
                                                      self.cursor.data_ptr(), self.B, s["u"].data_ptr(),
@@ -2462,13 +2440,17 @@ class InferenceEngine(object):
             else:
                 self.preds[j].copy_(pred)
                 preds = self.preds
-        if run.get("S"):
-            return self._draw_stats(preds, s)
-        if run.get("A"):
-            return self._elicit_stats(preds, s)
-        if run.get("width"):
-            return self._group_stats(preds, s)
-        if run["kind"] == "recommend":
+        if "reduce" in run:
+            # one value per unit (``_unit_run``): scattered by tag, or a key merged by the unit's candidate (gv: before
+            # the mapping kernels)
+            if run["keys"] is None:
+                run["reduce"](preds, s, None, *run["out"])
+            else:
+                run["reduce"](preds, s, run["keys"])
+                _lib.check(self.lib.igmc_topk_merge(run["keys"].data_ptr(), 1, run["G"], s["gtag"].data_ptr(),
+                                                    s["gv"].data_ptr(), run["k"], run["top_s"].data_ptr(),
+                                                    run["top_i"].data_ptr(), _stream_ptr()), "igmc_topk_merge")
+        elif run["kind"] == "recommend":
             ranked = s["u"] if run.get("by_item") else s["v"]      # the candidates: users on an item-side run
             _lib.check(self.lib.igmc_topk_merge(preds.data_ptr(), self.K, self.B, s["tag"].data_ptr(),
                                                 ranked.data_ptr(), run["k"], run["top_s"].data_ptr(),
@@ -2477,17 +2459,6 @@ class InferenceEngine(object):
             out = run["occ"] if occlude else run["scores"]
             _lib.check(self.lib.igmc_score_scatter(preds.data_ptr(), self.K, self.B, s["tag"].data_ptr(),
                                                    out.data_ptr(), _stream_ptr()), "igmc_score_scatter")
-
-    def _draw_stats(self, preds, s):
-        """a batch of draws: per pair its statistics scattered to the run's outputs, or (ranking) its key
-        mean + beta * std merged into the running top-k lists over the batch's G pairs"""
-        run, st = self.run, _stream_ptr()
-        rank = run["kind"] == "recommend"
-        outs = (None, None, None, run["keys"]) if rank else (run["value"], run["mean"], run["std"], None)
-        _lib.check(self.lib.igmc_draws_stats(preds.data_ptr(), self.K, self.B, run["S"], s["tag"].data_ptr(),
-                                             run["beta"], *(_lib.ptr(t) for t in outs), st), "igmc_draws_stats")
-        if rank:
-            self._merge_unit_keys(s)     # the candidates before the mapping kernels
 
     def _gradient(self, slot):
         """per parameter set: the eval forward of batch ``slot`` on the L2 plan, (DGCNN_RS) the SortPooling backward
@@ -2581,14 +2552,8 @@ class InferenceEngine(object):
             return Influence(run["pro_i"], run["pro_v"], run["con_i"], run["con_v"])
         if run["kind"] == "self_influence":
             return run["self_out"]
-        if run["kind"] == "draws":
-            return Draws(run["value"], run["mean"], run["std"])
-        if run["kind"] == "counterfactual":
+        if run["kind"] in ("counterfactual", "draws", "question_impact", "group_pairs"):
             return run["out"]
-        if run["kind"] == "question_impact":
-            return QuestionImpact(run["impact"], run["answer_mean"])
-        if run["kind"] == "group_pairs":
-            return GroupScores(run["scores"], run["member_scores"])
         return run["scores"]
 
     def _order(self, run):
