@@ -3,7 +3,8 @@
 // A group is up to IGMC_GROUP_MAX users; its score of an item aggregates its members' own pair scores, each bit for bit
 // predict_pairs' score (pair id member * num_items + item).  So a group run is an ordinary candidate stream over group
 // slots whose units (group, item) expand to one batch position per member:
-//   k_gr_offsets  one CTA: per group the summed member degrees and their exclusive scan (the union's upper bound)
+//   k_gr_offsets  one CTA: per group the summed member degrees and their exclusive scan (the union's upper bound), in
+//                 64 bits and saturated at cap
 //   k_gr_flags    one CTA per group: every entry of the concatenated member rows flagged when no earlier member rated
 //                 the item, and the group's exclusive scan of the flags
 //   k_gr_scan     one CTA: row_ptr = the exclusive scan of the union sizes
@@ -32,9 +33,12 @@ __device__ __forceinline__ int member_at(const int32_t* __restrict__ members, in
   return m;
 }
 
-// the group's member rows in shared memory: start r0[j], length and the prefix cum[j] of the lengths (cum[M] = n)
+// the group's member rows in shared memory: start r0[j], length and the prefix cum[j] of the lengths (cum[M] = n).  Up
+// to IGMC_GROUP_MAX rows of up to 2^31 - 1 entries each: the prefix is kept in 64 bits, and group_entries only lets a
+// group whose n fits the int32 workspace through, so every position below n is an int.
 struct GroupRows {
-  int r0[IGMC_GROUP_MAX], cum[IGMC_GROUP_MAX + 1];
+  int r0[IGMC_GROUP_MAX];
+  long long cum[IGMC_GROUP_MAX + 1];
 };
 
 __device__ __forceinline__ void load_rows(const igmc_csr_t& G, const int32_t* __restrict__ members, int M, int g,
@@ -60,33 +64,37 @@ __device__ __forceinline__ int entry_at(const igmc_csr_t& G, const GroupRows& s,
     if (s.cum[mid] <= e) lo = mid; else hi = mid;
   }
   *j = lo;
-  return G.col_idx[s.r0[lo] + e - s.cum[lo]];
+  return G.col_idx[s.r0[lo] + (int)(e - s.cum[lo])];
 }
 
 // the group's entries when they fit the workspace (else none: k_gr_offsets set the error word)
 __device__ __forceinline__ int group_entries(const GroupRows& s, int M, const int32_t* __restrict__ off, int g,
                                              int cap) {
-  return (long long)off[g] + s.cum[M] <= cap ? s.cum[M] : 0;
+  return (long long)off[g] + s.cum[M] <= cap ? (int)s.cum[M] : 0;
 }
 
+// per group its summed member degrees and their exclusive scan, both in 64 bits (a group's sum reaches 64 * (2^31 - 1))
+// and the scan saturated at cap + 1: off[g] = min(prefix, cap), so a group whose entries end past cap reads none
 __global__ void __launch_bounds__(ROW_THREADS)
 k_gr_offsets(igmc_csr_t G, const int32_t* __restrict__ members, int num_groups, int M, int cap,
              int32_t* __restrict__ off, int* err) {
-  __shared__ int ws[33];
-  const int total = block_scan_chunks(
-      num_groups, ws,
-      [&](int g) {
-        int n = 0;
-        for (int j = 0; j < M; ++j) {
-          const int m = member_at(members, M, G.num_users, g, j, err);
-          if (m >= 0) n += G.row_ptr[m + 1] - G.row_ptr[m];
-        }
-        return n;
-      },
-      [&](int g, int prefix) { off[g] = prefix; });
+  __shared__ long long ws[33];
+  long long carry = 0;
+  for (int base = 0; base < num_groups; base += blockDim.x) {
+    const int g = base + threadIdx.x;
+    long long n = 0, tot;
+    if (g < num_groups)
+      for (int j = 0; j < M; ++j) {
+        const int m = member_at(members, M, G.num_users, g, j, err);
+        if (m >= 0) n += G.row_ptr[m + 1] - G.row_ptr[m];
+      }
+    const long long ex = block_excl_scan_ll(n, ws, &tot);
+    if (g < num_groups) off[g] = (int)min(carry + ex, (long long)cap);
+    carry = min(carry + tot, (long long)cap + 1);
+  }
   if (threadIdx.x == 0) {
-    off[num_groups] = total;
-    if (total > cap) igmc_set_err(err, IGMC_ERR_CANDIDATES);
+    off[num_groups] = (int)min(carry, (long long)cap);
+    if (carry > cap) igmc_set_err(err, IGMC_ERR_CANDIDATES);
   }
 }
 
@@ -104,7 +112,7 @@ k_gr_flags(igmc_csr_t G, const int32_t* __restrict__ members, int M, int cap, co
         int j;
         const int x = entry_at(G, s, M, e, &j);
         for (int q = 0; q < j; ++q)
-          if (find_sorted(G.col_idx + s.r0[q], s.cum[q + 1] - s.cum[q], x) >= 0) return 0;
+          if (find_sorted(G.col_idx + s.r0[q], (int)(s.cum[q + 1] - s.cum[q]), x) >= 0) return 0;
         return 1;
       },
       [&](int e, int prefix) { pre[o + e] = prefix; });
@@ -137,12 +145,13 @@ k_gr_write(igmc_csr_t G, const int32_t* __restrict__ members, int M, int cap, co
     int rank = 0;
     for (int q = 0; q < M; ++q) {
       const int32_t* r = G.col_idx + s.r0[q];
-      int lo = 0, hi = s.cum[q + 1] - s.cum[q];
+      const int c0 = (int)s.cum[q];
+      int lo = 0, hi = (int)(s.cum[q + 1] - s.cum[q]);
       while (lo < hi) {
         const int mid = (lo + hi) >> 1;
         if (r[mid] < x) lo = mid + 1; else hi = mid;
       }
-      rank += before(s.cum[q] + lo) - before(s.cum[q]);
+      rank += before(c0 + lo) - before(c0);
     }
     col_idx[base + rank] = x;
   }
