@@ -13,11 +13,11 @@ import numpy as np
 import pytest
 
 from igmc_b200 import recommend as rc
+from tests import support
 
 
 def _graph(rows, num_items):
-    rp = np.concatenate([[0], np.cumsum([len(r) for r in rows])]).astype(np.int32)
-    ci = np.concatenate([np.asarray(sorted(r), np.int64) for r in rows] or [np.zeros(0)]).astype(np.int32)
+    rp, ci = support.rows_csr([sorted(r) for r in rows])
     cols = [set() for _ in range(num_items)]
     for u, r in enumerate(rows):
         for v in r:
@@ -135,13 +135,6 @@ def _brute_select(cols, pool_i, pool_s, k, penalty):
     return out_i, out_s, out_k
 
 
-def _same(a, b):
-    a, b = np.asarray(a, np.float32), np.asarray(b, np.float32)
-    n = np.isnan(a)
-    return a.shape == b.shape and np.array_equal(n, np.isnan(b)) and np.array_equal(a[~n].view(np.uint32),
-                                                                                   b[~n].view(np.uint32))
-
-
 def _select(rows, ni, pool_i, pool_s, k, penalty):
     rp, ci, cp, cols = _graph(rows, ni)
     mp, lst, bad = rc.item_union_host(pool_i, ni)
@@ -168,7 +161,7 @@ def test_selection_matches_literal_loop(penalty):
     pool_i[0, 5], pool_i[0, 6] = 3, 17                              # items without raters: sim 0
     (gi, gs, gk, bad), (wi, ws, wk) = _select(rows, ni, pool_i, pool_s, k, penalty)
     assert not bad.any()
-    assert np.array_equal(gi, wi) and _same(gs, ws) and _same(gk, wk)
+    assert np.array_equal(gi, wi) and support.same(gs, ws) and support.same(gk, wk)
     assert (gi[3, 4:] == -1).all() and (gs[4, 1:] == -np.inf).all() and (gk[5] == -np.inf).all()
 
 
@@ -200,7 +193,7 @@ def test_penalty_zero_is_the_pool_prefix():
     pool_i[4, 12:], pool_s[4, 12:] = -1, -np.inf                    # a short pool
     for k in (1, 8, 20):
         (gi, gs, gk, _), _ = _select(rows, ni, pool_i, pool_s, k, 0.0)
-        assert np.array_equal(gi, pool_i[:, :k]) and _same(gs, pool_s[:, :k]) and _same(gk, gs)
+        assert np.array_equal(gi, pool_i[:, :k]) and support.same(gs, pool_s[:, :k]) and support.same(gk, gs)
 
 
 def test_recommend_diverse_host_composes_the_twins():
@@ -219,10 +212,10 @@ def test_recommend_diverse_host_composes_the_twins():
     gi, gs, gk = rc.recommend_diverse_host(rp, ci, cp, len(rows), ni, users, 5, 0.5, pooler, pool=15)
     pi, ps = pooler(users, 15)
     wi, ws, wk = _brute_select(cols, pi, ps, 5, 0.5)
-    assert np.array_equal(gi, wi) and _same(gs, ws) and _same(gk, wk)
+    assert np.array_equal(gi, wi) and support.same(gs, ws) and support.same(gk, wk)
     assert sorted(gi[1, :2].tolist()) == [3, 17] and (gi[1, 2:] == -1).all()   # user 5: only the unrated items
     hi, hs, _ = rc.recommend_diverse_host(rp, ci, cp, len(rows), ni, users, 5, 0.0, pooler, pool=15)
-    assert np.array_equal(hi, pi[:, :5]) and _same(hs, ps[:, :5])
+    assert np.array_equal(hi, pi[:, :5]) and support.same(hs, ps[:, :5])
 
 
 # ---- input checks -----------------------------------------------------------------------------------------------------

@@ -8,9 +8,6 @@ tests/online_cases.py, checked without a GPU.
 * the host twins of igmc_b200/recommend.py and igmc_b200/train_eval.py agree with the brute-force enumerations on the
   cases they run, so the twins other tests rely on are held to the contract at these regimes too: adj_dropout = 1
   keeps no edge, not even one whose hash has all 32 high bits set."""
-import os
-import re
-
 import numpy as np
 import pytest
 
@@ -20,26 +17,22 @@ from igmc_b200.models import _keep_threshold, edge_keep_reference, hidden_keep_r
 from tests import counterfactual_cases as cc
 from tests import draw_cases as dc
 from tests import online_cases as oc
+from tests import support
 from tests.ranking_cases import same_f32
 
 MODULES = (dc, cc, oc)
 CASES = [c for m in MODULES for c in m.all_cases()]
-CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "igmc_b200", "csrc")
 
 
 def _module(kernel):
     return next(m for m in MODULES if kernel in m.REQUIRED)
 
 
-def _id(c):
-    return "%s: %s" % (c["kernel"], c["name"])
-
-
 def _of(kernel):
     return [c for c in CASES if c["kernel"] == kernel]
 
 
-@pytest.mark.parametrize("case", CASES, ids=_id)
+@pytest.mark.parametrize("case", CASES, ids=support.pid)
 def test_case_reaches_its_regimes(case):
     got = _module(case["kernel"]).REGIMES[case["kernel"]](case)
     assert case["claims"] <= got, (case["claims"] - got)
@@ -56,19 +49,12 @@ def test_every_regime_is_reached(mod):
 
 @pytest.mark.parametrize("mod", MODULES, ids=lambda m: m.__name__)
 def test_claims_are_declared_not_derived(mod):
-    """every case states its claims as data: no builder computes them with the function they are checked against"""
-    with open(mod.__file__) as f:
-        src = f.read()
-    assert not re.search(r"claims\W*\]?\s*=\s*\w+_regimes\(", src)
-    assert all(c["claims"] for c in mod.all_cases())
+    support.claims_are_declared(mod)
 
 
 @pytest.mark.parametrize("mod", MODULES, ids=lambda m: m.__name__)
 def test_launch_constants_match_the_sources(mod):
-    for (src, name), value in mod.CONSTANTS.items():
-        with open(os.path.join(CSRC, src)) as f:
-            m = re.findall(r"constexpr\s+int\s+%s\s*=\s*(\d+)\s*;" % name, f.read())
-        assert m == [str(value)], (src, name, m, value)
+    support.launch_constants_match(mod.CONSTANTS)
 
 
 # ---- the brute force's own footing --------------------------------------------------------------------------------------
@@ -97,7 +83,7 @@ def test_dropout_at_one_keeps_nothing():
 
 
 # ---- the host twins against the brute force -----------------------------------------------------------------------------
-@pytest.mark.parametrize("case", _of("expand"), ids=_id)
+@pytest.mark.parametrize("case", _of("expand"), ids=support.pid)
 def test_draws_expand_twin(case):
     got = rc.draws_expand_host(case["S"], case["B"], case["pair_u"], case["pair_v"], case["pair_pid"],
                                case["pair_tag"])
@@ -105,7 +91,7 @@ def test_draws_expand_twin(case):
         assert np.array_equal(g, w)
 
 
-@pytest.mark.parametrize("case", _of("mask"), ids=_id)
+@pytest.mark.parametrize("case", _of("mask"), ids=support.pid)
 def test_draws_mask_twin(case):
     ek, hk = dc.mask_reference(case)
     gek, ghk = rc.draws_mask_host(case["edge_ptr"], case["pair_id"], case["tag"], case["draw"], case["p"],
@@ -114,7 +100,7 @@ def test_draws_mask_twin(case):
     assert np.array_equal(ghk, hk)
 
 
-@pytest.mark.parametrize("case", _of("stats"), ids=_id)
+@pytest.mark.parametrize("case", _of("stats"), ids=support.pid)
 def test_draws_stats_twin(case):
     x, mean, sd, key = dc.stats_reference(case)
     with np.errstate(all="ignore"):
@@ -122,8 +108,8 @@ def test_draws_stats_twin(case):
     assert same_f32(hx, x) and same_f32(hm, mean) and same_f32(hs, sd) and same_f32(hk, key)
 
 
-@pytest.mark.parametrize("case", [c for c in _of("cf_pairs") if c["name"] not in ("invalid ids",
-                                                                                  "candidate past the row")], ids=_id)
+@pytest.mark.parametrize("case", [c for c in _of("cf_pairs")
+                                  if c["name"] not in ("invalid ids", "candidate past the row")], ids=support.pid)
 def test_counterfactual_pairs_twin(case):
     rp, col, rat = cc.graph()
     for pos in case["cursors"]:
@@ -135,7 +121,7 @@ def test_counterfactual_pairs_twin(case):
             assert np.array_equal(g, w), pos
 
 
-@pytest.mark.parametrize("case", [c for c in _of("cf_select") if c["name"] != "not the plan's trials"], ids=_id)
+@pytest.mark.parametrize("case", [c for c in _of("cf_select") if c["name"] != "not the plan's trials"], ids=support.pid)
 def test_counterfactual_select_twin(case):
     rp, col, rat = cc.graph()
     want, err, _ = cc.select_reference(case)
@@ -155,7 +141,7 @@ def test_counterfactual_select_twin(case):
             assert np.array_equal(st[k], w), k
 
 
-@pytest.mark.parametrize("case", [c for c in _of("online_draw") if not c["empty"]], ids=_id)
+@pytest.mark.parametrize("case", [c for c in _of("online_draw") if not c["empty"]], ids=support.pid)
 def test_online_draw_twin(case):
     rp, col, rat, nu, ni = oc.graph()
     u, v, lab, pid, seeds, err, _ = oc.draw_reference(case)
@@ -166,7 +152,7 @@ def test_online_draw_twin(case):
         assert np.array_equal(g, w)
 
 
-@pytest.mark.parametrize("case", _of("append"), ids=_id)
+@pytest.mark.parametrize("case", _of("append"), ids=support.pid)
 def test_recent_append_twin(case):
     ring = (np.full(case["capacity"], oc.RING_SENT, np.int32), np.full(case["capacity"], oc.RING_SENT, np.int32),
             case["total"])

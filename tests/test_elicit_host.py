@@ -1,8 +1,6 @@
 """Question impact on the host: the numpy twins of igmc_elicit_pairs / igmc_elicit_stats against brute forces written
 from include/igmc_b200.h, elicit_host over a deterministic fake scorer against a hand-worked example, and the
 argument checks.  No GPU."""
-import os
-import re
 import types
 
 import numpy as np
@@ -10,22 +8,11 @@ import pytest
 
 from igmc_b200 import recommend as rc
 from tests import elicit_cases as ec
-
-CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "igmc_b200", "csrc")
-
-
-def _same(a, b):
-    a, b = np.asarray(a, np.float32), np.asarray(b, np.float32)
-    n = np.isnan(a)
-    return a.shape == b.shape and np.array_equal(n, np.isnan(b)) and np.array_equal(a[~n].view(np.uint32),
-                                                                                   b[~n].view(np.uint32))
+from tests import support
 
 
 def test_launch_constants_match_the_source():
-    for (src, name), value in ec.CONSTANTS.items():
-        with open(os.path.join(CSRC, src)) as f:
-            m = re.findall(r"constexpr\s+int\s+%s\s*=\s*(\d+)\s*;" % name, f.read())
-        assert m == [str(value)], (src, name, m, value)
+    support.launch_constants_match(ec.CONSTANTS)
 
 
 @pytest.mark.parametrize("case", ec.pair_cases(), ids=lambda c: c["name"])
@@ -72,7 +59,7 @@ def test_stats_twin_is_the_brute_force(case):
         if w is None:
             assert utag[g] == -1
             continue
-        assert _same(impact[g], w[0]) and _same(mean[g], w[1]) and utag[g] == w[2], g
+        assert support.same(impact[g], w[0]) and support.same(mean[g], w[1]) and utag[g] == w[2], g
 
 
 def test_stats_by_hand():

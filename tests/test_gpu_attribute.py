@@ -21,7 +21,8 @@ from igmc_b200.data import build_adj, synth_ratings
 from igmc_b200.util_functions import Batch, RatingGraph
 from tests import edge_weight_oracle as ewo
 from tests import pyg2_oracle
-from tests.test_gpu_explain import _ds, _model, _pairs, _r13, _subgraph, _with_cold_start
+from tests import support
+from tests.test_gpu_explain import _pairs, _subgraph, _with_cold_start
 from tests.test_gpu_graph_update import _apply_scipy
 
 pytestmark = pytest.mark.gpu
@@ -86,9 +87,9 @@ CASES = {
 @pytest.mark.parametrize("name", list(CASES))
 def test_grad_matches_fp64_autograd(name):
     dsn, R, h, mnph, kw, B = CASES[name]
-    A0 = {"r13": _r13, "r71": _r71}.get(dsn, lambda: _ds(dsn)["adj_train"])()
+    A0 = _r71() if dsn == "r71" else support.adj(dsn)
     A = _with_cold_start(A0)
-    m = _model(R, h, **kw)
+    m = support.model(R, h=h, **kw, pyg2_bias=True)
     u, v = _pairs(A)
     seed = 7
     ex = rc.attribute_pairs(m, A, u, v, h=h, max_nodes_per_hop=mnph, batch_size=B, sample_seed=seed)
@@ -130,8 +131,8 @@ def _run(eng, u, v, m=None):
 
 
 def test_score_ratings_order_topm_and_determinism():
-    A = _with_cold_start(_ds("ml_1m")["adj_train"])
-    m = _model(5)
+    A = _with_cold_start(support.adj("ml_1m"))
+    m = support.model(5)
     u, v = _pairs(A)
     base = rc.predict_pairs(m, A, u, v, max_nodes_per_hop=100, batch_size=50, sample_seed=2)
     exp = rc.explain_pairs(m, A, u, v, max_nodes_per_hop=100, batch_size=50, sample_seed=2)
@@ -174,8 +175,8 @@ def test_score_ratings_order_topm_and_determinism():
 
 
 def test_validation_and_empty_input():
-    A = _ds("ml_100k")["adj_train"]
-    m = _model(5)
+    A = support.adj("ml_100k")
+    m = support.model(5)
     with pytest.raises(IndexError):
         rc.attribute_pairs(m, A, [A.shape[0]], [0])
     with pytest.raises(ValueError):
@@ -189,14 +190,14 @@ def test_validation_and_empty_input():
 
 
 def test_three_checkpoints_are_the_fp32_mean():
-    A = _with_cold_start(_ds("ml_100k")["adj_train"])
-    m = _model(5)
+    A = _with_cold_start(support.adj("ml_100k"))
+    m = support.model(5)
     u, v = _pairs(A, small=True)
     with tempfile.TemporaryDirectory() as tmp:
         paths = []
         for c in range(3):
             paths.append(os.path.join(tmp, "model_checkpoint%d.pth" % c))
-            torch.save(_model(5, seed=c + 1).state_dict(), paths[-1])
+            torch.save(support.model(5, seed=c + 1).state_dict(), paths[-1])
         runs = []
         for ck in (paths, paths[:1], paths[1:2], paths[2:]):
             eng = rc.InferenceEngine(m, A, max_nodes_per_hop=200, batch_size=50, checkpoints=ck)
@@ -211,8 +212,8 @@ def test_three_checkpoints_are_the_fp32_mean():
 
 
 def test_engine_attributes_across_updates():
-    A = _ds("ml_1m")["adj_train"]
-    m = _model(5, rgcn="pyg-2")
+    A = support.adj("ml_1m")
+    m = support.model(5, rgcn="pyg-2", pyg2_bias=True)
     g = RatingGraph(A, reserve_nnz=2000)
     eng = rc.InferenceEngine(m, g, max_nodes_per_hop=100, batch_size=64, sample_seed=4)
     rng = np.random.default_rng(5)
@@ -238,8 +239,8 @@ def test_engine_attributes_across_updates():
 
 
 def test_steady_state_steps_do_not_sync():
-    A = _ds("ml_1m")["adj_train"]
-    m = _model(5, dgcnn=True)
+    A = support.adj("ml_1m")
+    m = support.model(5, dgcnn=True)
     eng = rc.InferenceEngine(m, A, max_nodes_per_hop=100, batch_size=2, sample_seed=1)
     u, v = np.arange(11, 23), np.arange(40, 52)
     outs = []

@@ -17,8 +17,9 @@ import torch
 
 from igmc_b200 import recommend as rc
 from tests import edge_weight_oracle as ewo
+from tests import support
 from tests.test_gpu_attribute import _kernel_perm, _ref
-from tests.test_gpu_explain import _ds, _model, _pairs, _r13, _subgraph, _with_cold_start
+from tests.test_gpu_explain import _pairs, _subgraph, _with_cold_start
 from tests.test_gpu_explain_nodes import _positions
 
 pytestmark = pytest.mark.gpu
@@ -62,9 +63,9 @@ CASES = {
 @pytest.mark.parametrize("name", list(CASES))
 def test_grad_matches_fp64_autograd(name):
     dsn, R, h, mnph, kw, B = CASES[name]
-    A0 = _r13() if dsn == "r13" else _ds(dsn)["adj_train"]
+    A0 = support.adj(dsn)
     A = _with_cold_start(A0)
-    m = _model(R, h, **kw)
+    m = support.model(R, h=h, **kw, pyg2_bias=True)
     u, v = _pairs(A)
     seed = 7
     eng = rc.InferenceEngine(m, A, h=h, max_nodes_per_hop=mnph, batch_size=B, sample_seed=seed)
@@ -98,8 +99,8 @@ def test_grad_matches_fp64_autograd(name):
 
 def test_grad_is_the_in_list_sum_of_the_raw_edge_grad():
     """the engine's node values against igmc_edge_grad of the same batch, summed in the documented order here"""
-    A = _with_cold_start(_ds("ml_1m")["adj_train"])
-    m = _model(5)
+    A = _with_cold_start(support.adj("ml_1m"))
+    m = support.model(5)
     u, v = _pairs(A)
     B = 4                                       # one gradient batch: all three pairs and a padded slot
     eng = rc.InferenceEngine(m, A, max_nodes_per_hop=100, batch_size=B, sample_seed=2)
@@ -134,8 +135,8 @@ def test_grad_is_the_in_list_sum_of_the_raw_edge_grad():
 
 
 def test_score_nodes_order_and_determinism():
-    A = _with_cold_start(_ds("ml_1m")["adj_train"])
-    m = _model(5)
+    A = _with_cold_start(support.adj("ml_1m"))
+    m = support.model(5)
     m.kernel_plan = 2                  # the base pass's plan at every batch size (the gradient pass forces L2)
     u, v = _pairs(A)
     base = rc.predict_pairs(m, A, u, v, max_nodes_per_hop=100, batch_size=50, sample_seed=2)
@@ -169,14 +170,14 @@ def test_score_nodes_order_and_determinism():
 
 
 def test_two_checkpoints_are_the_fp32_mean():
-    A = _with_cold_start(_ds("ml_100k")["adj_train"])
-    m = _model(5)
+    A = _with_cold_start(support.adj("ml_100k"))
+    m = support.model(5)
     u, v = _pairs(A, small=True)
     with tempfile.TemporaryDirectory() as tmp:
         paths = []
         for c in range(2):
             paths.append(os.path.join(tmp, "model_checkpoint%d.pth" % c))
-            torch.save(_model(5, seed=c + 1).state_dict(), paths[-1])
+            torch.save(support.model(5, seed=c + 1).state_dict(), paths[-1])
         runs = []
         for ck in (paths, paths[:1], paths[1:]):
             eng = rc.InferenceEngine(m, A, max_nodes_per_hop=200, batch_size=50, checkpoints=ck)

@@ -14,6 +14,7 @@ import torch
 from igmc_b200 import _lib
 from igmc_b200.util_functions import _stream_ptr
 from tests import foreign_batch_cases as fb
+from tests import support
 
 pytestmark = pytest.mark.gpu
 
@@ -24,14 +25,6 @@ R = 5
 SMEM_NCAP_MAX = 200 * 1024 // 8 - 1      # 2 (n_cap + 1) ints of shared memory within 200 KB
 
 
-def _dev(a, dtype):
-    return torch.from_numpy(np.ascontiguousarray(np.asarray(a).astype(dtype))).cuda()
-
-
-def _filled(n, dtype=torch.int32):
-    return torch.full((n + GUARD,), S32, dtype=dtype, device="cuda")
-
-
 def _take_err(err):
     code = int(err.item())
     err.zero_()
@@ -39,8 +32,8 @@ def _take_err(err):
 
 
 def _ptrs(batch, src, N, E, B, err):
-    batch_d, src_d = _dev(batch if N else [0], np.int64), _dev(src if E else [0], np.int64)
-    node_ptr, edge_ptr = _filled(B + 1), _filled(B + 1)
+    batch_d, src_d = support.dev_np(batch if N else [0], np.int64), support.dev_np(src if E else [0], np.int64)
+    node_ptr, edge_ptr = support.filled(B + 1, S32, torch.int32, GUARD), support.filled(B + 1, S32, torch.int32, GUARD)
     _lib.check(_lib.load().igmc_batch_ptrs(batch_d.data_ptr() if N else None, src_d.data_ptr(), N, E, B,
                                            node_ptr.data_ptr(), edge_ptr.data_ptr(), err.data_ptr(), _stream_ptr()),
                "igmc_batch_ptrs")
@@ -53,10 +46,10 @@ def _prepare(ei, et, node_ptr, edge_ptr, B, n_cap, symmetric, err, stride_pad=0)
     N, E = int(node_ptr[B]), ei.shape[1]
     buf = np.full((2, E + stride_pad), -5, np.int64)
     buf[:, :E] = ei
-    ei_d, et_d = _dev(buf.reshape(-1), np.int64), _dev(np.append(et, 0), np.int64)
-    np_d, ep_d = _dev(node_ptr[:B + 1], np.int32), _dev(edge_ptr[:B + 1], np.int32)
-    t = {k: _filled(N + 1 if k.endswith("ptr") else E) for k in ("in_ptr", "in_adj", "in_eid", "out_ptr", "out_adj",
-                                                                   "out_eid")}
+    ei_d, et_d = support.dev_np(buf.reshape(-1), np.int64), support.dev_np(np.append(et, 0), np.int64)
+    np_d, ep_d = support.dev_np(node_ptr[:B + 1], np.int32), support.dev_np(edge_ptr[:B + 1], np.int32)
+    t = {k: support.filled(N + 1 if k.endswith("ptr") else E, S32, torch.int32, GUARD)
+         for k in ("in_ptr", "in_adj", "in_eid", "out_ptr", "out_adj", "out_eid")}
     tmp = torch.zeros(E + 1, dtype=torch.int64, device="cuda")
     A = _lib.Adj(*(t[k].data_ptr() for k in ("in_ptr", "in_adj", "in_eid", "out_ptr", "out_adj", "out_eid")),
                  tmp.data_ptr(), int(symmetric))

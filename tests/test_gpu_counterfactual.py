@@ -4,8 +4,6 @@ The oracle is the contract: every trial score is ``predict_sessions`` of a sessi
 (bit for bit, at the same kernel plan and batch size), and the whole greedy path is ``counterfactual_host`` driven by
 ``predict_sessions``.  The kernels are checked byte for byte against their numpy twins."""
 import ctypes as C
-import functools
-import os
 import tempfile
 
 import numpy as np
@@ -14,40 +12,13 @@ import torch
 
 from igmc_b200 import _lib
 from igmc_b200 import recommend as rc
-from igmc_b200.data import build_adj, make_synthetic_dataset, synth_ratings
 from igmc_b200.util_functions import RatingGraph
+from tests import support
 
 pytestmark = pytest.mark.gpu
 
 SENT32, SENT8, SENTF = -77, 0xAB, -7.5
 GUARD = 16
-
-
-@functools.lru_cache(maxsize=None)
-def _ds(name):
-    if name == "r13":
-        u, v, lab = synth_ratings(400, 300, 9000, 13, seed=4)
-        return build_adj(u, v, lab, 400, 300)
-    return make_synthetic_dataset(name, seed=0)["adj_train"]
-
-
-def _model(R, h=1, rgcn="pyg-1.4", dgcnn=False, nb=4, seed=0):
-    from igmc_b200.models import DGCNN_RS, IGMC
-    torch.manual_seed(seed)
-    if dgcnn:
-        m = DGCNN_RS(2 * h + 2, latent_dim=[32, 32, 32, 1], k=30, num_relations=R, num_bases=nb, regression=True,
-                     rgcn=rgcn)
-    else:
-        m = IGMC(2 * h + 2, latent_dim=[32] * 4, num_relations=R, num_bases=nb, regression=True, rgcn=rgcn)
-    return m.cuda()
-
-
-def _same(a, b):
-    """fp32 arrays equal bit for bit, NaN matching any NaN"""
-    a, b = np.asarray(a, np.float32), np.asarray(b, np.float32)
-    n = np.isnan(a)
-    return a.shape == b.shape and np.array_equal(n, np.isnan(b)) and np.array_equal(a[~n].view(np.uint32),
-                                                                                   b[~n].view(np.uint32))
 
 
 def _host(cf):
@@ -58,7 +29,7 @@ def _equal(a, b):
     for f in rc.Counterfactual._fields:
         x, y = getattr(a, f), getattr(b, f)
         if f in ("score", "rival_score"):
-            assert _same(x, y), f
+            assert support.same(x, y), f
         else:
             assert np.array_equal(np.asarray(x), np.asarray(y)), f
 
@@ -84,10 +55,6 @@ def _session_scorer(m, g, **kw):
 
 
 # ---- 1. kernels against their twins ---------------------------------------------------------------------------------
-def _dev(a, dtype):
-    return torch.as_tensor(np.asarray(a)).to(dtype).cuda()
-
-
 def _kernel_state(g, users, M, step, rng):
     """a mid-run state: R of step - 1 random positions per query, counts of the next pass"""
     Q = len(users)
@@ -107,7 +74,7 @@ def _kernel_state(g, users, M, step, rng):
 
 @pytest.mark.parametrize("B,step", [(1, 0), (7, 0), (1, 2), (7, 1), (64, 3), (256, 2)])
 def test_kernels_match_twins(B, step):
-    A = _ds("ml_100k")
+    A = support.adj("ml_100k")
     g = RatingGraph(A)
     rng = np.random.default_rng(B + step)
     h = g.host
@@ -123,10 +90,10 @@ def test_kernels_match_twins(B, step):
     P2 = 2 * int(offsets[-1])
     L = max(g.max_row_deg, 1)
     lib = _lib.load()
-    du, dx, dy = _dev(users, torch.int32), _dev(items, torch.int32), _dev(rivals, torch.int32)
-    dsize, drem = _dev(size, torch.int32), _dev(removed, torch.int32)
+    du, dx, dy = support.dev(users, torch.int32), support.dev(items, torch.int32), support.dev(rivals, torch.int32)
+    dsize, drem = support.dev(size, torch.int32), support.dev(removed, torch.int32)
     Qd = _lib.Counterfactual(du.data_ptr(), dx.data_ptr(), dy.data_ptr(), dsize.data_ptr(), drem.data_ptr(), Q, M)
-    doff = _dev(offsets, torch.int64)
+    doff = support.dev(offsets, torch.int64)
     err = torch.zeros(1, dtype=torch.int32, device="cuda")
     cursor = torch.zeros(1, dtype=torch.int64, device="cuda")
     for pos in list(range(0, P2, B))[:6] + [P2 + 5]:                    # the last: an all-padding batch
@@ -157,9 +124,9 @@ def test_kernels_match_twins(B, step):
     st = dict(removed=removed.copy(), size=size.copy(), count=count.copy(), found=np.zeros(Q, bool),
               items=np.full((Q, M), SENT32, np.int32), ratings=np.full((Q, M), SENT32, np.int32),
               score=np.full((Q, M + 1), SENTF, np.float32), rival_score=np.full((Q, M + 1), SENTF, np.float32))
-    dev = {k: _dev(v, torch.uint8 if k == "found" else torch.from_numpy(v).dtype) for k, v in st.items()}
+    dev = {k: support.dev(v, torch.uint8 if k == "found" else torch.from_numpy(v).dtype) for k, v in st.items()}
     Qd.size, Qd.removed = dev["size"].data_ptr(), dev["removed"].data_ptr()
-    dscores = _dev(scores, torch.float32)
+    dscores = support.dev(scores, torch.float32)
     assert lib.igmc_counterfactual_select(C.byref(g._c), C.byref(Qd), doff.data_ptr(), dscores.data_ptr(), step,
                                           dev["count"].data_ptr(), dev["found"].data_ptr(), dev["items"].data_ptr(),
                                           dev["ratings"].data_ptr(), dev["score"].data_ptr(),
@@ -169,16 +136,16 @@ def test_kernels_match_twins(B, step):
     for k, v in st.items():
         got = dev[k].cpu().numpy()
         if k in ("score", "rival_score"):
-            assert _same(got, v), k
+            assert support.same(got, v), k
         else:
             assert np.array_equal(got.astype(v.dtype), v), k
 
 
 # ---- 2. every trial score is predict_sessions' ----------------------------------------------------------------------
 def test_trial_scores_equal_predict_sessions():
-    A = _ds("ml_1m")
+    A = support.adj("ml_1m")
     g = RatingGraph(A)
-    m = _model(5)
+    m = support.model(5)
     m.kernel_plan = 2
     B, kw = 64, dict(max_nodes_per_hop=100)
     try:
@@ -214,7 +181,7 @@ def test_trial_scores_equal_predict_sessions():
                     tu += [u, u]
                     dl += [d, d]
                     tt += [items[q], rivals[q]]
-            assert _same(scorer(tu, dl, tt), scores)
+            assert support.same(scorer(tu, dl, tt), scores)
     finally:
         m.kernel_plan = "auto"
 
@@ -236,31 +203,18 @@ CASES = {
 }
 
 
-def _checkpoints(m, K, d):
-    paths = []
-    own = {k: v.clone() for k, v in m.state_dict().items()}
-    for k in range(K):
-        torch.manual_seed(100 + k)
-        with torch.no_grad():
-            m.flat_params.add_(torch.randn_like(m.flat_params) * 0.05)
-        paths.append(os.path.join(d, "ck%d.pt" % k))
-        torch.save(m.state_dict(), paths[-1])
-    m.load_state_dict(own)
-    return paths
-
-
 @pytest.mark.parametrize("name", list(CASES))
 def test_path_equals_host_loop(name):
     dsn, h, mnph, kw, plan, K = CASES[name]
-    A = _ds(dsn)
+    A = support.adj(dsn)
     R = 13 if dsn == "r13" else 5
     g = RatingGraph(A)
-    m = _model(R, h=h, **kw)
+    m = support.model(R, h=h, **kw)
     m.kernel_plan = plan
     B = 50
     try:
         with tempfile.TemporaryDirectory() as d:
-            ck = _checkpoints(m, K, d) if K else None
+            ck = support.checkpoints(m, K, d) if K else None
             opts = dict(h=h, max_nodes_per_hop=mnph, batch_size=B, checkpoints=ck, sample_seed=3)
             users, items, rivals = _queries(m, g, 3, len(name), hi=25, **opts)
             M = 4
@@ -276,7 +230,7 @@ def test_path_equals_host_loop(name):
                 g2 = RatingGraph(A)
                 g2.update(np.full(t, users[q]), got.items[q, :t], np.zeros(t, np.int64))
                 s = rc.predict_pairs(m, g2, [users[q]] * 2, [items[q], rivals[q]], **opts).cpu().numpy()
-                assert _same(s, [got.score[q, t], got.rival_score[q, t]])
+                assert support.same(s, [got.score[q, t], got.rival_score[q, t]])
                 if got.found[q]:
                     assert rc._before(s[1], rivals[q], s[0], items[q])
     finally:
@@ -307,9 +261,9 @@ def _run(m, g, users, items, rivals, M, B, use_graph=True, sync_check=False):
 
 
 def test_independent_of_batch_replay_and_other_queries():
-    A = _ds("ml_1m")
+    A = support.adj("ml_1m")
     g = RatingGraph(A)
-    m = _model(5)
+    m = support.model(5)
     users, items, rivals = _queries(m, g, 101, 5, hi=200, max_nodes_per_hop=100)
     M = 3
     base = _run(m, g, users[:2], items[:2], rivals[:2], M, 50)
@@ -324,9 +278,9 @@ def test_independent_of_batch_replay_and_other_queries():
 
 
 def test_steps_inside_a_pass_do_not_sync():
-    A = _ds("ml_1m")
+    A = support.adj("ml_1m")
     g = RatingGraph(A)
-    m = _model(5)
+    m = support.model(5)
     users, items, rivals = _queries(m, g, 6, 9, lo=40, hi=120, max_nodes_per_hop=100)
     a = _run(m, g, users, items, rivals, 2, 16, sync_check=True)
     _equal(a, _run(m, g, users, items, rivals, 2, 16))
@@ -334,9 +288,9 @@ def test_steps_inside_a_pass_do_not_sync():
 
 # ---- 5. validation ------------------------------------------------------------------------------------------------------
 def test_validation_and_updates():
-    A = _ds("ml_100k")
+    A = support.adj("ml_100k")
     g = RatingGraph(A, reserve_nnz=10)
-    m = _model(5)
+    m = support.model(5)
     nu, ni = A.shape
     eng = rc.InferenceEngine(m, g, batch_size=32)
     try:

@@ -12,8 +12,6 @@ InferenceEngine.start_recommend_diverse; csrc/diverse.cu).
   depend on the other users; two runs are bit-identical; the diverse stage makes at most one host sync per chunk; a
   graph.update between runs is served and one during a run raises."""
 import ctypes as C
-import functools
-import os
 import tempfile
 import warnings
 
@@ -24,55 +22,13 @@ import torch
 
 from igmc_b200 import _lib
 from igmc_b200 import recommend as rc
-from igmc_b200.data import build_adj, make_synthetic_dataset, synth_ratings
 from igmc_b200.util_functions import RatingGraph, _stream_ptr
+from tests import support
 
 pytestmark = pytest.mark.gpu
 
 SENT32, SENTF = -77, -7.5
 GUARD = 16
-
-
-@functools.lru_cache(maxsize=None)
-def _ds(name):
-    if name == "r13":
-        u, v, lab = synth_ratings(400, 300, 9000, 13, seed=4)
-        return build_adj(u, v, lab, 400, 300)
-    return make_synthetic_dataset(name, seed=0)["adj_train"]
-
-
-def _model(R, rgcn="pyg-1.4", dgcnn=False, seed=0):
-    from igmc_b200.models import DGCNN_RS, IGMC
-    torch.manual_seed(seed)
-    if dgcnn:
-        m = DGCNN_RS(4, latent_dim=[32, 32, 32, 1], k=30, num_relations=R, num_bases=4, regression=True, rgcn=rgcn)
-    else:
-        m = IGMC(4, latent_dim=[32] * 4, num_relations=R, num_bases=4, regression=True, rgcn=rgcn)
-    return m.cuda()
-
-
-def _checkpoints(m, K, d):
-    paths = []
-    own = {k: v.clone() for k, v in m.state_dict().items()}
-    for k in range(K):
-        torch.manual_seed(100 + k)
-        with torch.no_grad():
-            m.flat_params.add_(torch.randn_like(m.flat_params) * 0.05)
-        paths.append(os.path.join(d, "ck%d.pt" % k))
-        torch.save(m.state_dict(), paths[-1])
-    m.load_state_dict(own)
-    return paths
-
-
-def _dev(a, dtype=torch.int32):
-    return torch.as_tensor(np.asarray(a)).to(dtype).cuda()
-
-
-def _same(a, b):
-    a, b = np.asarray(a, np.float32), np.asarray(b, np.float32)
-    n = np.isnan(a)
-    return a.shape == b.shape and np.array_equal(n, np.isnan(b)) and np.array_equal(a[~n].view(np.uint32),
-                                                                                   b[~n].view(np.uint32))
 
 
 def _users(g, n, seed):
@@ -96,7 +52,7 @@ def _toy_graph(long_row=2500, ni=3000, nu=300, seed=0):
 
 
 def _union(items, ni):
-    items = _dev(items, torch.int64)
+    items = support.dev(items, torch.int64)
     bitmap = torch.full(((ni + 31) // 32,), SENT32, dtype=torch.int32, device="cuda")
     mp = torch.full((ni + GUARD,), SENT32, dtype=torch.int32, device="cuda")
     lst = torch.full((ni + GUARD,), SENT32, dtype=torch.int32, device="cuda")
@@ -158,7 +114,7 @@ def _select(g, pool_i, pool_s, k, penalty, mp, Nu, table):
     os_ = torch.full((Q * k + GUARD,), SENTF, dtype=torch.float32, device="cuda")
     ok = torch.full((Q * k + GUARD,), SENTF, dtype=torch.float32, device="cuda")
     err = torch.zeros(1, dtype=torch.int32, device="cuda")
-    di, ds = _dev(pool_i, torch.int64), _dev(pool_s, torch.float32)
+    di, ds = support.dev(pool_i, torch.int64), support.dev(pool_s, torch.float32)
     code = _lib.load().igmc_diverse_select(C.byref(g._c), di.data_ptr(), ds.data_ptr(), Q, P, k, penalty,
                                            mp.data_ptr(), Nu, table.data_ptr(), oi.data_ptr(), os_.data_ptr(),
                                            ok.data_ptr(), err.data_ptr(), _stream_ptr())
@@ -186,13 +142,13 @@ def test_select_kernel_matches_twin(P, k, penalty):
     Nu = len(lst)
     table = rc.cocount_host(hp["row_ptr"], hp["col_idx"], g.num_users, ni, lst)
     want = rc.diverse_select_host(hp["col_ptr"], pool_i, pool_s, k, penalty, mp, table, Nu)
-    dt = _dev(table.view(np.int32)) if Nu > 1 else torch.zeros(1, dtype=torch.int32, device="cuda")
-    code, err, gi, gs, gk = _select(g, pool_i, pool_s, k, penalty, _dev(mp), Nu, dt)
+    dt = support.dev(table.view(np.int32)) if Nu > 1 else torch.zeros(1, dtype=torch.int32, device="cuda")
+    code, err, gi, gs, gk = _select(g, pool_i, pool_s, k, penalty, support.dev(mp), Nu, dt)
     assert code == 0 and err == 0
     n = Q * k
     assert np.array_equal(gi[:n], want[0].reshape(-1)) and (gi[n:] == SENT32).all()
-    assert _same(gs[:n], want[1].reshape(-1)) and (gs[n:] == SENTF).all()
-    assert _same(gk[:n], want[2].reshape(-1)) and (gk[n:] == SENTF).all()
+    assert support.same(gs[:n], want[1].reshape(-1)) and (gs[n:] == SENTF).all()
+    assert support.same(gk[:n], want[2].reshape(-1)) and (gk[n:] == SENTF).all()
 
 
 def test_select_kernel_flags_bad_pools():
@@ -205,11 +161,12 @@ def test_select_kernel_flags_bad_pools():
     table = rc.cocount_host(hp["row_ptr"], hp["col_idx"], g.num_users, ni, lst)
     want = rc.diverse_select_host(hp["col_ptr"], pool_i, pool_s, 2, 1.0, mp, table, len(lst))
     assert want[3].tolist() == [False, True, True, True]
-    code, err, gi, gs, gk = _select(g, pool_i, pool_s, 2, 1.0, _dev(mp), len(lst), _dev(table.view(np.int32)))
+    code, err, gi, gs, gk = _select(g, pool_i, pool_s, 2, 1.0, support.dev(mp), len(lst),
+                                    support.dev(table.view(np.int32)))
     assert code == 0 and err == 7
-    assert np.array_equal(gi[:8], want[0].reshape(-1)) and _same(gs[:8], want[1].reshape(-1))
-    assert _same(gk[:8], want[2].reshape(-1))
-    lib, p = _lib.load(), _dev(mp).data_ptr()
+    assert np.array_equal(gi[:8], want[0].reshape(-1)) and support.same(gs[:8], want[1].reshape(-1))
+    assert support.same(gk[:8], want[2].reshape(-1))
+    lib, p = _lib.load(), support.dev(mp).data_ptr()
     for P, k, pen in ((3, 4, 1.0), (257, 2, 1.0), (3, 2, -1.0), (3, 2, float("inf")), (3, 2, float("nan"))):
         assert lib.igmc_diverse_select(C.byref(g._c), p, p, 1, P, k, pen, p, 3, p, p, p, p, None, None) == -1
 
@@ -220,7 +177,7 @@ def test_item_similarity_kernel_and_public_matches_twin_toy():
     items = np.array([7, 7, 2999, 0, 15, 2, 7, 100, 2999], np.int64)
     got = rc.item_similarity(g, items).cpu().numpy()
     want = rc.item_similarity_host(hp["row_ptr"], hp["col_idx"], hp["col_ptr"], g.num_users, g.num_items, items)
-    assert _same(got, want)
+    assert support.same(got, want)
     with pytest.raises(IndexError):
         rc.item_similarity(g, [1, g.num_items])
     assert rc.item_similarity(g, []).shape == (0, 0)
@@ -228,14 +185,14 @@ def test_item_similarity_kernel_and_public_matches_twin_toy():
 
 @pytest.mark.parametrize("name", ["ml_1m", "flixster"])
 def test_item_similarity_matches_twin(name):
-    g = RatingGraph(_ds(name))
+    g = RatingGraph(support.adj(name))
     hp = g.host
     rng = np.random.default_rng(0)
     items = rng.choice(g.num_items, 400)                                         # repeats included
     items[:5] = np.argsort(-np.diff(hp["col_ptr"]))[:5]                          # the most rated items
     got = rc.item_similarity(g, items).cpu().numpy()
     want = rc.item_similarity_host(hp["row_ptr"], hp["col_idx"], hp["col_ptr"], g.num_users, g.num_items, items)
-    assert _same(got, want)
+    assert support.same(got, want)
     d = np.diff(hp["col_ptr"])[items]
     assert (np.diag(got)[d > 0] == 1).all() and (np.diag(got)[d == 0] == 0).all()
 
@@ -263,19 +220,19 @@ def _check_lists(eng, g, users, k, penalty, pool, **kw):
     want = rc.recommend_diverse_host(hp["row_ptr"], hp["col_idx"], hp["col_ptr"], g.num_users, g.num_items, users, k,
                                      penalty, pooler, pool)
     assert np.array_equal(got.items.cpu().numpy(), want[0]), (k, penalty, pool, kw.keys())
-    assert _same(got.scores.cpu().numpy(), want[1]) and _same(got.keys.cpu().numpy(), want[2])
+    assert support.same(got.scores.cpu().numpy(), want[1]) and support.same(got.keys.cpu().numpy(), want[2])
     return got
 
 
 @pytest.mark.parametrize("name", list(CASES))
 def test_lists_equal_host_composition(name):
     dsn, mnph, kw, plan, K = CASES[name]
-    g = RatingGraph(_ds(dsn))
-    m = _model(13 if dsn == "r13" else 5, **kw)
+    g = RatingGraph(support.adj(dsn))
+    m = support.model(13 if dsn == "r13" else 5, **kw)
     m.kernel_plan = plan
     try:
         with tempfile.TemporaryDirectory() as d:
-            ck = _checkpoints(m, K, d) if K else None
+            ck = support.checkpoints(m, K, d) if K else None
             eng = rc.InferenceEngine(m, g, max_nodes_per_hop=mnph, batch_size=64, checkpoints=ck, sample_seed=3)
             try:
                 ni = g.num_items
@@ -298,15 +255,15 @@ def test_lists_equal_host_composition(name):
 
 # ---- 3. penalty 0, chunks, independence, syncs and updates ---------------------------------------------------------------
 def test_penalty_zero_is_recommend_and_chunks_change_nothing():
-    g = RatingGraph(_ds("ml_1m"))
-    m = _model(5)
+    g = RatingGraph(support.adj("ml_1m"))
+    m = support.model(5)
     users = _users(g, 24, 5)
     eng = rc.InferenceEngine(m, g, max_nodes_per_hop=100, batch_size=256)
     try:
         ti, ts = eng.recommend(users, 10)
         got = eng.recommend_diverse(users, 10, 0.0, pool=60)
-        assert torch.equal(got.items, ti) and _same(got.scores.cpu().numpy(), ts.cpu().numpy())
-        assert _same(got.keys.cpu().numpy(), got.scores.cpu().numpy())
+        assert torch.equal(got.items, ti) and support.same(got.scores.cpu().numpy(), ts.cpu().numpy())
+        assert support.same(got.keys.cpu().numpy(), got.scores.cpu().numpy())
         pub = rc.recommend_diverse(m, g, users, 10, 0.0, pool=60, max_nodes_per_hop=100)
         assert torch.equal(pub.items, ti)
         base = eng.recommend_diverse(users, 10, 1.5, pool=60)
@@ -318,11 +275,11 @@ def test_penalty_zero_is_recommend_and_chunks_change_nothing():
         assert chunk.value == 2
         small = eng.recommend_diverse(users, 10, 1.5, pool=60)
         for a, b in zip(small, base):
-            assert _same(a.cpu().numpy(), b.cpu().numpy())
+            assert support.same(a.cpu().numpy(), b.cpu().numpy())
         eng.diverse_ws_bytes = 1                                                  # one user per chunk
         one = eng.recommend_diverse(users, 10, 1.5, pool=60)
         for a, b in zip(one, base):
-            assert _same(a.cpu().numpy(), b.cpu().numpy())
+            assert support.same(a.cpu().numpy(), b.cpu().numpy())
     finally:
         eng.close()
 
@@ -340,20 +297,20 @@ def _stage_syncs(eng, pi, ps):
 
 
 def test_independent_deterministic_sync_count():
-    g = RatingGraph(_ds("ml_1m"))
-    m = _model(5)
+    g = RatingGraph(support.adj("ml_1m"))
+    m = support.model(5)
     users = _users(g, 12, 9)
     eng = rc.InferenceEngine(m, g, max_nodes_per_hop=100, batch_size=128)
     try:
         a = eng.recommend_diverse(users, 10, 1.0)
         b = eng.recommend_diverse(users, 10, 1.0)
         for x, y in zip(a, b):
-            assert _same(x.cpu().numpy(), y.cpu().numpy())
+            assert support.same(x.cpu().numpy(), y.cpu().numpy())
         more = np.r_[_users(g, 5, 77), users]
         c = eng.recommend_diverse(more, 10, 1.0)
         pos = [int(np.flatnonzero(more == u)[0]) for u in users]
         for x, y in zip(c, a):
-            assert _same(x.cpu().numpy()[pos], y.cpu().numpy())
+            assert support.same(x.cpu().numpy()[pos], y.cpu().numpy())
         pi, ps = eng.recommend(users, 50)
         got, one = _stage_syncs(eng, pi, ps)
         assert one == 1                                                           # one chunk: one sync
@@ -361,14 +318,14 @@ def test_independent_deterministic_sync_count():
         again, per_user = _stage_syncs(eng, pi, ps)
         assert 1 <= per_user <= len(users)                                        # at most one per chunk
         for x, y in zip(got, again):
-            assert _same(x.cpu().numpy(), y.cpu().numpy())
+            assert support.same(x.cpu().numpy(), y.cpu().numpy())
     finally:
         eng.close()
 
 
 def test_served_across_updates():
-    g = RatingGraph(_ds("ml_100k"), reserve_nnz=50)
-    m = _model(5)
+    g = RatingGraph(support.adj("ml_100k"), reserve_nnz=50)
+    m = support.model(5)
     users = np.array([1, 2, 40, 41], np.int64)
     eng = rc.InferenceEngine(m, g, max_nodes_per_hop=100, batch_size=64)
     try:

@@ -17,25 +17,13 @@ from igmc_b200.util_functions import _stream_ptr
 from tests import counterfactual_cases as cc
 from tests import draw_cases as dc
 from tests import online_cases as oc
+from tests import support
 from tests.ranking_cases import same_f32
 
 pytestmark = pytest.mark.gpu
 
 GUARD = 64
 S32, S64, S8, SF = -777, -(2 ** 40) - 7, 0xAB, -7.5     # sentinels: no kernel writes any of them
-
-
-def _id(c):
-    return c["name"]
-
-
-def _dev(a, dtype):
-    a = np.asarray(a)
-    return torch.from_numpy(np.ascontiguousarray((a if a.size else np.zeros(1)).astype(dtype))).cuda()
-
-
-def _filled(n, value, dtype):
-    return torch.full((n + GUARD,), value, dtype=dtype, device="cuda")
 
 
 def _with_guard(a, value):
@@ -48,11 +36,6 @@ def _exact(t, want, value):
     got = t.cpu().numpy()
     w = _with_guard(np.asarray(want).astype(got.dtype), value)
     assert got.shape == w.shape and np.array_equal(got, w), np.flatnonzero(got != w)[:5]
-
-
-def _assert_claims(mod, case):
-    got = mod.REGIMES[case["kernel"]](case)
-    assert case["claims"] <= got, ("the case no longer reaches", case["claims"] - got)
 
 
 @pytest.fixture
@@ -68,41 +51,37 @@ def _take_err(e):
     return v
 
 
-def _csr(row_ptr, col, rating, nu, ni):
-    """igmc_csr_t of host arrays (rows only); (struct, keep-alive)"""
-    t = (_dev(row_ptr, np.int32), _dev(col, np.int32), _dev(rating, np.uint8))
-    return _lib.CSR(t[0].data_ptr(), t[1].data_ptr(), t[2].data_ptr(), None, None, nu, ni), t
-
-
 # ---- igmc_draws_expand ------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("case", [c for c in dc.all_cases() if c["kernel"] == "expand"], ids=_id)
+@pytest.mark.parametrize("case", [c for c in dc.all_cases() if c["kernel"] == "expand"], ids=support.name_id)
 def test_draws_expand(case):
-    _assert_claims(dc, case)
+    support.assert_claims(dc.REGIMES, case)
     lib = _lib.load()
     S, B = case["S"], case["B"]
-    ins = [_dev(case["pair_u"], np.int32), _dev(case["pair_v"], np.int32), _dev(case["pair_pid"], np.int64),
-           _dev(case["pair_tag"], np.int64)]
+    ins = [support.dev_np(support.nonempty(case[k]), dt) for k, dt in
+           (("pair_u", np.int32), ("pair_v", np.int32), ("pair_pid", np.int64), ("pair_tag", np.int64))]
     sent = (S32, S32, S64, S64, S32)
-    outs = [_filled(B, s, d) for s, d in zip(sent, (torch.int32, torch.int32, torch.int64, torch.int64, torch.int32))]
+    outs = [support.filled(B, s, d, GUARD)
+            for s, d in zip(sent, (torch.int32, torch.int32, torch.int64, torch.int64, torch.int32))]
     assert lib.igmc_draws_expand(S, B, *(t.data_ptr() for t in ins + outs), _stream_ptr()) == 0
     for o, w, s in zip(outs, dc.expand_reference(case), sent):
         _exact(o, w, s)
 
 
 # ---- igmc_draws_mask --------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("case", [c for c in dc.all_cases() if c["kernel"] == "mask"], ids=_id)
+@pytest.mark.parametrize("case", [c for c in dc.all_cases() if c["kernel"] == "mask"], ids=support.name_id)
 def test_draws_mask(case):
     """p = 1 keeps no edge, the one whose hash has all 32 high bits set included; a hash at the threshold is kept,
     one below it dropped"""
-    _assert_claims(dc, case)
+    support.assert_claims(dc.REGIMES, case)
     lib = _lib.load()
     ep = case["edge_ptr"]
     B, E = len(ep) - 1, int(ep[-1])
-    dep = _dev(ep, np.int32)
+    dep = support.dev_np(support.nonempty(ep), np.int32)
     O = _lib.BatchOut()
     O.edge_ptr = dep.data_ptr()
-    pid, tag, draw = _dev(case["pair_id"], np.int64), _dev(case["tag"], np.int64), _dev(case["draw"], np.int32)
-    ek, hk = _filled(E, S8, torch.uint8), _filled(B * dc.LIN1_OUT, S8, torch.uint8)
+    pid, tag, draw = (support.dev_np(support.nonempty(case[k]), dt)
+                      for k, dt in (("pair_id", np.int64), ("tag", np.int64), ("draw", np.int32)))
+    ek, hk = support.filled(E, S8, torch.uint8, GUARD), support.filled(B * dc.LIN1_OUT, S8, torch.uint8, GUARD)
     assert lib.igmc_draws_mask(C.byref(O), B, pid.data_ptr(), tag.data_ptr(), draw.data_ptr(), case["p"], case["seed"],
                                ek.data_ptr(), hk.data_ptr(), _stream_ptr()) == 0
     wek, whk = dc.mask_reference(case)
@@ -111,20 +90,21 @@ def test_draws_mask(case):
 
 
 # ---- igmc_draws_stats -------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("case", [c for c in dc.all_cases() if c["kernel"] == "stats"], ids=_id)
+@pytest.mark.parametrize("case", [c for c in dc.all_cases() if c["kernel"] == "stats"], ids=support.name_id)
 def test_draws_stats(case):
-    _assert_claims(dc, case)
+    support.assert_claims(dc.REGIMES, case)
     lib = _lib.load()
     K, B, S = case["K"], case["B"], case["S"]
-    dp, dt = _dev(case["preds"].reshape(-1), np.float32), _dev(case["tag"], np.int64)
+    dp = support.dev_np(support.nonempty(case["preds"].reshape(-1)), np.float32)
+    dt = support.dev_np(support.nonempty(case["tag"]), np.int64)
     want = dc.stats_outputs(case, SF)
     if case["mode"] == "key":
-        key = _filled(B // S, SF, torch.float32)
+        key = support.filled(B // S, SF, torch.float32, GUARD)
         assert lib.igmc_draws_stats(dp.data_ptr(), K, B, S, dt.data_ptr(), case["beta"], None, None, None,
                                     key.data_ptr(), _stream_ptr()) == 0
         assert same_f32(key.cpu().numpy(), _with_guard(want, SF))
         return
-    outs = [_filled(len(w), SF, torch.float32) for w in want]
+    outs = [support.filled(len(w), SF, torch.float32, GUARD) for w in want]
     assert lib.igmc_draws_stats(dp.data_ptr(), K, B, S, dt.data_ptr(), case["beta"], *(o.data_ptr() for o in outs),
                                 None, _stream_ptr()) == 0
     for o, w, name in zip(outs, want, ("value", "mean", "std")):
@@ -134,28 +114,29 @@ def test_draws_stats(case):
 # ---- igmc_counterfactual_pairs / _select -----------------------------------------------------------------------------
 def _cf_query(case, size=None, removed=None):
     """igmc_counterfactual_t of a case (size / removed: device tensors to use); (struct, keep-alive)"""
-    keep = [_dev(case["users"], np.int32), _dev(case["items"], np.int32), _dev(case["rivals"], np.int32),
-            size if size is not None else _dev(case["size"], np.int32),
-            removed if removed is not None else _dev(case["removed"].reshape(-1), np.int32)]
+    keep = [*(support.dev_np(support.nonempty(case[k]), np.int32) for k in ("users", "items", "rivals")),
+            size if size is not None else support.dev_np(support.nonempty(case["size"]), np.int32),
+            removed if removed is not None else support.dev_np(support.nonempty(case["removed"].reshape(-1)),
+                                                               np.int32)]
     return _lib.Counterfactual(*(t.data_ptr() for t in keep), len(case["users"]), case["M"]), keep
 
 
-@pytest.mark.parametrize("case", [c for c in cc.all_cases() if c["kernel"] == "cf_pairs"], ids=_id)
+@pytest.mark.parametrize("case", [c for c in cc.all_cases() if c["kernel"] == "cf_pairs"], ids=support.name_id)
 def test_counterfactual_pairs(case, err):
-    _assert_claims(cc, case)
+    support.assert_claims(cc.REGIMES, case)
     lib = _lib.load()
-    G, keep_g = _csr(*cc.graph(), cc.NU, cc.NI)
+    G, keep_g = support.csr_struct(*cc.graph(), cc.NU, cc.NI)
     Q, keep_q = _cf_query(case)
-    off = _dev(case["offsets"], np.int64)
+    off = support.dev_np(support.nonempty(case["offsets"]), np.int64)
     B = case["B"]
     for pos in case["cursors"]:
         row_cap = cc.row_cap_of(case, pos)
         u, v, pid, tag, ru, rptr, rcol, rrat, werr, rows = cc.pairs_reference(case, pos, row_cap)
         cursor = torch.tensor([pos], dtype=torch.int64, device="cuda")
-        lu, lv, dru, sess = (_filled(B, S32, torch.int32) for _ in range(4))
-        dpid, dtag = _filled(B, S64, torch.int64), _filled(B, S64, torch.int64)
-        drp = _filled(B + 1, S32, torch.int32)
-        dcol, drat = _filled(row_cap, S32, torch.int32), _filled(row_cap, S8, torch.uint8)
+        lu, lv, dru, sess = (support.filled(B, S32, torch.int32, GUARD) for _ in range(4))
+        dpid, dtag = support.filled(B, S64, torch.int64, GUARD), support.filled(B, S64, torch.int64, GUARD)
+        drp = support.filled(B + 1, S32, torch.int32, GUARD)
+        dcol, drat = support.filled(row_cap, S32, torch.int32, GUARD), support.filled(row_cap, S8, torch.uint8, GUARD)
         assert lib.igmc_counterfactual_pairs(C.byref(G), C.byref(Q), off.data_ptr(), case["step"], cursor.data_ptr(), B,
                                              lu.data_ptr(), lv.data_ptr(), dpid.data_ptr(), dtag.data_ptr(),
                                              dru.data_ptr(), drp.data_ptr(), dcol.data_ptr(), drat.data_ptr(), row_cap,
@@ -175,11 +156,11 @@ def test_counterfactual_pairs(case, err):
             assert np.array_equal(got_col[:n], rcol) and np.array_equal(got_rat[:n], rrat), pos
 
 
-@pytest.mark.parametrize("case", [c for c in cc.all_cases() if c["kernel"] == "cf_select"], ids=_id)
+@pytest.mark.parametrize("case", [c for c in cc.all_cases() if c["kernel"] == "cf_select"], ids=support.name_id)
 def test_counterfactual_select(case, err):
-    _assert_claims(cc, case)
+    support.assert_claims(cc.REGIMES, case)
     lib = _lib.load()
-    G, keep_g = _csr(*cc.graph(), cc.NU, cc.NI)
+    G, keep_g = support.csr_struct(*cc.graph(), cc.NU, cc.NI)
     want, werr, _ = cc.select_reference(case)
     Qn, M = len(case["users"]), case["M"]
     start = dict(removed=(case["removed"], S32, np.int32), size=(case["size"], S32, np.int32),
@@ -187,9 +168,10 @@ def test_counterfactual_select(case, err):
                  items=(np.full(Qn * M, cc.S32), S32, np.int32), ratings=(np.full(Qn * M, cc.S32), S32, np.int32),
                  score=(np.full(Qn * (M + 1), cc.SF), SF, np.float32),
                  rival_score=(np.full(Qn * (M + 1), cc.SF), SF, np.float32))
-    dev = {k: _dev(_with_guard(np.asarray(a).astype(d), s), d) for k, (a, s, d) in start.items()}
+    dev = {k: support.dev_np(_with_guard(np.asarray(a).astype(d), s), d) for k, (a, s, d) in start.items()}
     Q, keep_q = _cf_query(case, dev["size"], dev["removed"])
-    off, sc = _dev(case["offsets"], np.int64), _dev(case["scores"], np.float32)
+    off = support.dev_np(support.nonempty(case["offsets"]), np.int64)
+    sc = support.dev_np(support.nonempty(case["scores"]), np.float32)
     assert lib.igmc_counterfactual_select(C.byref(G), C.byref(Q), off.data_ptr(), sc.data_ptr(), case["step"],
                                           *(dev[k].data_ptr() for k in ("count", "found", "items", "ratings", "score",
                                                                         "rival_score")),
@@ -203,17 +185,17 @@ def test_counterfactual_select(case, err):
 
 
 # ---- igmc_online_draw / igmc_online_recent_append ---------------------------------------------------------------------
-@pytest.mark.parametrize("case", [c for c in oc.all_cases() if c["kernel"] == "online_draw"], ids=_id)
+@pytest.mark.parametrize("case", [c for c in oc.all_cases() if c["kernel"] == "online_draw"], ids=support.name_id)
 def test_online_draw(case, err):
-    _assert_claims(oc, case)
+    support.assert_claims(oc.REGIMES, case)
     lib = _lib.load()
-    G, keep_g = _csr(*oc.graph(case["empty"]))
-    ring_u, ring_v = _dev(case["ring"][0], np.int32), _dev(case["ring"][1], np.int32)
+    G, keep_g = support.csr_struct(*oc.graph(case["empty"]))
+    ring_u, ring_v = (support.dev_np(support.nonempty(r), np.int32) for r in case["ring"][:2])
     total = torch.tensor([case["total"]], dtype=torch.int64, device="cuda")
     step = torch.tensor([case["step_count"]], dtype=torch.int64, device="cuda")
     B = case["B"]
-    lu, lv, lab = (_filled(B, S32, torch.int32) for _ in range(3))
-    pid, seeds = _filled(B, S64, torch.int64), _filled(3, S64, torch.int64)
+    lu, lv, lab = (support.filled(B, S32, torch.int32, GUARD) for _ in range(3))
+    pid, seeds = support.filled(B, S64, torch.int64, GUARD), support.filled(3, S64, torch.int64, GUARD)
     assert lib.igmc_online_draw(C.byref(G), ring_u.data_ptr(), ring_v.data_ptr(), case["capacity"], total.data_ptr(),
                                 case["thresh"], step.data_ptr(), case["step_ahead"], case["sample_seed"],
                                 case["drop_seed"], B, lu.data_ptr(), lv.data_ptr(), lab.data_ptr(), pid.data_ptr(),
@@ -225,17 +207,17 @@ def test_online_draw(case, err):
     assert int(total.item()) == case["total"] and int(step.item()) == case["step_count"]
 
 
-@pytest.mark.parametrize("case", [c for c in oc.all_cases() if c["kernel"] == "append"], ids=_id)
+@pytest.mark.parametrize("case", [c for c in oc.all_cases() if c["kernel"] == "append"], ids=support.name_id)
 def test_recent_append(case, err):
     """call after call: the ring, its count and the error word"""
-    _assert_claims(oc, case)
+    support.assert_claims(oc.REGIMES, case)
     lib = _lib.load()
     cap = case["capacity"]
-    ring_u, ring_v = _filled(cap, oc.RING_SENT, torch.int32), _filled(cap, oc.RING_SENT, torch.int32)
+    ring_u, ring_v = (support.filled(cap, oc.RING_SENT, torch.int32, GUARD) for _ in range(2))
     total = torch.tensor([case["total"]], dtype=torch.int64, device="cuda")
     for (u, v, x), (wu, wv, wt, werr) in zip(case["calls"], oc.append_reference(case)):
         D = len(u)
-        ins = [_dev(a, np.int32) for a in (u, v, x)]
+        ins = [support.dev_np(support.nonempty(a), np.int32) for a in (u, v, x)]
         ptrs = [t.data_ptr() for t in ins] if D else [None] * 3     # D = 0: no launch, no inputs needed
         assert lib.igmc_online_recent_append(*ptrs, D, ring_u.data_ptr(), ring_v.data_ptr(), cap, total.data_ptr(),
                                              err.data_ptr(), _stream_ptr()) == 0
@@ -270,7 +252,7 @@ def test_argument_checks(err):
     for bad in (float("nan"), float("inf"), -float("inf")):
         assert lib.igmc_draws_stats(p, 1, 4, 2, p, bad, None, None, None, p, st) == -2, bad
     # igmc_counterfactual_pairs / _select: a query set with 1 <= max_removals <= 256, B > 0, step >= 0, buffers (-1)
-    G, keep_g = _csr(*cc.graph(), cc.NU, cc.NI)
+    G, keep_g = support.csr_struct(*cc.graph(), cc.NU, cc.NI)
     for nq, M in ((0, 4), (1, 0), (1, cc.CF_MAX + 1)):
         Q = _lib.Counterfactual(p, p, p, p, p, nq, M)
         assert lib.igmc_counterfactual_pairs(C.byref(G), C.byref(Q), p, 1, p, 4, *([p] * 8), 16, p, p, st) == -1
@@ -282,7 +264,7 @@ def test_argument_checks(err):
     assert lib.igmc_counterfactual_select(C.byref(G), C.byref(Q), p, p, -1, *([p] * 6), p, st) == -1
     assert lib.igmc_counterfactual_select(C.byref(G), C.byref(Q), p, p, 1, None, *([p] * 5), p, st) == -1
     # igmc_online_draw: the graph (-1), the ring (-2), recent_thresh in [0, 2^32] (-3), the step (-4), the outputs (-5)
-    Go, keep_o = _csr(*oc.graph())
+    Go, keep_o = support.csr_struct(*oc.graph())
     args = dict(G=C.byref(Go), ru=p, rv=p, cap=8, total=p, thresh=2 ** 31, step=p, ahead=0, B=4, err=err.data_ptr())
 
     def draw(**kw):

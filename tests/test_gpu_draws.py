@@ -8,7 +8,6 @@
   eval ranking;
 * an engine kept across graph.update matches a fresh one; steady-state steps make no host synchronisation."""
 import ctypes as C
-import functools
 import os
 import tempfile
 
@@ -19,40 +18,18 @@ import torch
 
 from igmc_b200 import _lib
 from igmc_b200 import recommend as rc
-from igmc_b200.data import build_adj, make_synthetic_dataset, synth_ratings
 from igmc_b200.util_functions import RatingGraph, SubgraphExtractor
 from oracle import pyg_restated
 from tests import pyg2_oracle
+from tests import support
 from tests.test_gpu_graph_update import _apply_scipy
 
 pytestmark = pytest.mark.gpu
 
 
-@functools.lru_cache(maxsize=None)
-def _ds(name):
-    return make_synthetic_dataset(name, seed=0)
-
-
-@functools.lru_cache(maxsize=None)
-def _r13():
-    u, v, lab = synth_ratings(400, 300, 9000, 13, seed=4)
-    return build_adj(u, v, lab, 400, 300)
-
-
 def _with_cold_start(A):
     """A with one more user and one more item, neither rated: the pair (new user, new item) has no ratings at all"""
     return ssp.csr_matrix(ssp.bmat([[A, None], [None, ssp.csr_matrix((1, 1), dtype=A.dtype)]]), dtype=A.dtype)
-
-
-def _model(R, h=1, rgcn="pyg-1.4", dgcnn=False, nb=4, seed=0):
-    from igmc_b200.models import DGCNN_RS, IGMC
-    torch.manual_seed(seed)
-    if dgcnn:
-        m = DGCNN_RS(2 * h + 2, latent_dim=[32, 32, 32, 1], k=30, num_relations=R, num_bases=nb, regression=True,
-                     rgcn=rgcn)
-    else:
-        m = IGMC(2 * h + 2, latent_dim=[32] * 4, num_relations=R, num_bases=nb, regression=True, rgcn=rgcn)
-    return m.cuda()
 
 
 def _random_pairs(A, n, seed):
@@ -65,32 +42,15 @@ SENT32, SENT8, SENTF = -77, 0xAB, -7.5
 GUARD = 16
 
 
-def _dev(a, dtype):
-    return torch.as_tensor(np.asarray(a)).to(dtype).cuda()
-
-
-def _same(a, b):
-    """fp32 arrays equal bit for bit, NaN matching any NaN (the device and numpy write different NaN payloads)"""
-    a, b = np.asarray(a, np.float32), np.asarray(b, np.float32)
-    n = np.isnan(a)
-    return a.shape == b.shape and np.array_equal(n, np.isnan(b)) and np.array_equal(a[~n].view(np.uint32),
-                                                                                   b[~n].view(np.uint32))
-
-
-def _filled(n, dtype, value):
-    return torch.full((n + GUARD,), value, dtype=dtype, device="cuda")
-
-
 def _expand_and_extract(A, R, S, B, u, v, ptag, h=1, mnph=100, seed=3):
     """the expand kernel on G = B // S pairs (checked against its twin with guards), then the extraction of its B
     positions; returns (expanded host arrays, batch, extractor)"""
     lib = _lib.load()
     G = B // S
     ni = A.shape[1]
-    pu, pv = _dev(u[:G], torch.int32), _dev(v[:G], torch.int32)
-    ppid, pt = _dev(u[:G].astype(np.int64) * ni + v[:G], torch.int64), _dev(ptag[:G], torch.int64)
-    out = [_filled(B, torch.int32, SENT32), _filled(B, torch.int32, SENT32), _filled(B, torch.int64, SENT32),
-           _filled(B, torch.int64, SENT32), _filled(B, torch.int32, SENT32)]
+    pu, pv = support.dev(u[:G], torch.int32), support.dev(v[:G], torch.int32)
+    ppid, pt = support.dev(u[:G].astype(np.int64) * ni + v[:G], torch.int64), support.dev(ptag[:G], torch.int64)
+    out = [support.filled(B, SENT32, d) for d in (torch.int32, torch.int32, torch.int64, torch.int64, torch.int32)]
     _lib.check(lib.igmc_draws_expand(S, B, pu.data_ptr(), pv.data_ptr(), ppid.data_ptr(), pt.data_ptr(),
                                      *(t.data_ptr() for t in out), None), "igmc_draws_expand")
     want = rc.draws_expand_host(S, B, u[:G], v[:G], u[:G].astype(np.int64) * ni + v[:G], ptag[:G])
@@ -107,10 +67,10 @@ def _expand_and_extract(A, R, S, B, u, v, ptag, h=1, mnph=100, seed=3):
                                   "h=2"])
 def test_kernels_match_twins(case):
     lib = _lib.load()
-    A = _with_cold_start(_ds("ml_1m")["adj_train"])
+    A = _with_cold_start(support.adj("ml_1m"))
     R, h = 5, 1
     nu, ni = A.shape[0] - 1, A.shape[1] - 1
-    u, v = _random_pairs(_ds("ml_1m")["adj_train"], 256, seed=len(case))
+    u, v = _random_pairs(support.adj("ml_1m"), 256, seed=len(case))
     ptag = np.arange(256, dtype=np.int64)
     S, B = dict(zip(["B=1", "B=50 S=8 tail", "B=256 S=8", "B=256 S=3 tail pairs", "cold start", "h=2"],
                     [(1, 1), (8, 50), (8, 256), (3, 256), (4, 32), (2, 20)]))[case]
@@ -126,9 +86,9 @@ def test_kernels_match_twins(case):
     E = int(edge_ptr[-1])
     if case == "cold start":
         assert edge_ptr[1] == edge_ptr[0]
-    dpid, dtag, ddraw = _dev(pid, torch.int64), _dev(tag, torch.int64), _dev(draw, torch.int32)
+    dpid, dtag, ddraw = support.dev(pid, torch.int64), support.dev(tag, torch.int64), support.dev(draw, torch.int32)
     for p, seed in ((0.2, 0), (0.0, 2 ** 64 - 1), (0.5, 12345)):
-        ek, hk = _filled(E, torch.uint8, SENT8), _filled(B * 128, torch.uint8, SENT8)
+        ek, hk = support.filled(E, SENT8, torch.uint8), support.filled(B * 128, SENT8, torch.uint8)
         _lib.check(lib.igmc_draws_mask(C.byref(O), B, dpid.data_ptr(), dtag.data_ptr(), ddraw.data_ptr(), p, seed,
                                        ek.data_ptr(), hk.data_ptr(), None), "igmc_draws_mask")
         wek, whk = rc.draws_mask_host(edge_ptr, pid, tag, draw, p, seed)
@@ -145,17 +105,17 @@ def test_kernels_match_twins(case):
         preds = rng.normal(3.0, 1.0, size=(K, B)).astype(np.float32)
         if B > 8:
             preds[0, 5], preds[K - 1, S + 1] = np.nan, np.inf
-        dp = _dev(preds.reshape(-1), torch.float32)
+        dp = support.dev(preds.reshape(-1), torch.float32)
         for beta in (0.0, 1.0, -2.5):
-            key = _filled(G, torch.float32, SENTF)
+            key = support.filled(G, SENTF, torch.float32)
             _lib.check(lib.igmc_draws_stats(dp.data_ptr(), K, B, S, dtag.data_ptr(), beta, None, None, None,
                                             key.data_ptr(), None), "igmc_draws_stats")
             x, mean, sd, wkey = rc.draws_stats_host(preds, K, B, S, beta)
             gk = key.cpu().numpy()
-            assert _same(gk[:G], wkey), (case, K, beta)
+            assert support.same(gk[:G], wkey), (case, K, beta)
             assert (gk[G:] == SENTF).all()
-        value, mo, so = _filled(P * S, torch.float32, SENTF), _filled(P, torch.float32, SENTF), \
-            _filled(P, torch.float32, SENTF)
+        value, mo, so = support.filled(P * S, SENTF, torch.float32), support.filled(P, SENTF, torch.float32), \
+            support.filled(P, SENTF, torch.float32)
         _lib.check(lib.igmc_draws_stats(dp.data_ptr(), K, B, S, dtag.data_ptr(), 0.0, value.data_ptr(), mo.data_ptr(),
                                         so.data_ptr(), None, None), "igmc_draws_stats")
         wv = np.full(P * S + GUARD, SENTF, np.float32)
@@ -165,7 +125,7 @@ def test_kernels_match_twins(case):
             if t >= 0:
                 wv[t * S:(t + 1) * S], wm[t], ws[t] = x[g], mean[g], sd[g]
         for got, want in ((value, wv), (mo, wm), (so, ws)):
-            assert _same(got.cpu().numpy(), want), (case, K)
+            assert support.same(got.cpu().numpy(), want), (case, K)
     # argument checks of the entry points
     assert lib.igmc_draws_expand(0, B, *([None] * 9), None) != 0
     assert lib.igmc_draws_expand(_lib.DRAWS_MAX + 1, 4096, *([None] * 9), None) != 0
@@ -230,9 +190,9 @@ def _alone(m, A, R, u, v, S, draw_seed, h, mnph, seed, plan):
 @pytest.mark.parametrize("name", list(CASES))
 def test_each_draw_is_the_model_alone(name):
     dsn, h, mnph, kw, force, plan = CASES[name]
-    A = _with_cold_start(_r13() if dsn == "r13" else _ds(dsn)["adj_train"])
+    A = _with_cold_start(support.adj(dsn))
     R = 13 if dsn == "r13" else 5
-    m = _model(R, h, **kw)
+    m = support.model(R, h=h, **kw)
     m.kernel_plan = force
     u, v = _case_pairs(A)
     S, B, seed, ds = 8, 64, 7, 0x5EED
@@ -252,9 +212,9 @@ def test_each_draw_is_the_model_alone(name):
 
 @pytest.mark.parametrize("rgcn", ["pyg-1.4", "pyg-2"])
 def test_draws_against_the_fp64_oracle(rgcn):
-    A = _with_cold_start(_ds("ml_1m")["adj_train"])
+    A = _with_cold_start(support.adj("ml_1m"))
     R, mnph, seed, S, ds = 5, 100, 7, 4, 11
-    m = _model(R, rgcn=rgcn)
+    m = support.model(R, rgcn=rgcn)
     ref = pyg2_oracle.igmc_ref(rgcn, 4, (32,) * 4, R, 4, m.adj_dropout)
     ref.load_state_dict({k: v.double().cpu() for k, v in m.state_dict().items()})
     ref = pyg_restated.set_formulation(ref.double(), "transform").cuda().train()
@@ -274,8 +234,8 @@ def test_draws_against_the_fp64_oracle(rgcn):
 
 # ---- 3. independence of the batch, the run and the other pairs -------------------------------------------------------------
 def test_draws_do_not_depend_on_batch_run_or_neighbours():
-    A = _ds("ml_1m")["adj_train"]
-    m = _model(5)
+    A = support.adj("ml_1m")
+    m = support.model(5)
     m.kernel_plan = 2
     u, v = _random_pairs(A, 40, seed=3)
     S, kw = 8, dict(max_nodes_per_hop=100, sample_seed=1)
@@ -301,8 +261,8 @@ def test_draws_do_not_depend_on_batch_run_or_neighbours():
 
 
 def test_checkpoints_average_each_draw():
-    A = _ds("ml_100k")["adj_train"]
-    m = _model(5)
+    A = support.adj("ml_100k")
+    m = support.model(5)
     m.kernel_plan = 2
     u, v = _random_pairs(A, 30, seed=5)
     kw = dict(max_nodes_per_hop=100, batch_size=64, draw_seed=3)
@@ -310,7 +270,7 @@ def test_checkpoints_average_each_draw():
         paths = []
         for c in range(3):
             paths.append(os.path.join(tmp, "c%d.pth" % c))
-            torch.save(_model(5, seed=c + 1).state_dict(), paths[-1])
+            torch.save(support.model(5, seed=c + 1).state_dict(), paths[-1])
         got = rc.predict_draws(m, A, u, v, 4, checkpoints=paths, **kw)
         each = [rc.predict_draws(m, A, u, v, 4, checkpoints=[p], **kw).value for p in paths]
     e = [x.cpu().numpy() for x in each]
@@ -330,7 +290,7 @@ def _check_ranking(top_i, top_s, rows, keys_of, k):
     for j, cands in enumerate(rows):
         ws, wi = _stable_rank(keys_of(j, cands), cands, k)
         assert np.array_equal(top_i[j], wi), (j, top_i[j][:5], wi[:5])
-        assert _same(top_s[j], ws), j
+        assert support.same(top_s[j], ws), j
 
 
 def _keys(m, A, users, items, S, beta, kw):
@@ -342,8 +302,8 @@ def _keys(m, A, users, items, S, beta, kw):
 
 @pytest.mark.parametrize("S", [1, 8])
 def test_recommend_ranks_by_the_keys_of_predict_draws(S):
-    A = _ds("ml_100k")["adj_train"]
-    m = _model(5)
+    A = support.adj("ml_100k")
+    m = support.model(5)
     m.kernel_plan = 2
     ni = A.shape[1]
     users = np.array([3, 17, 250])
@@ -377,8 +337,8 @@ def test_recommend_ranks_by_the_keys_of_predict_draws(S):
 
 
 def test_recommend_users_ranks_by_the_keys_of_predict_draws():
-    A = _ds("ml_100k")["adj_train"]
-    m = _model(5)
+    A = support.adj("ml_100k")
+    m = support.model(5)
     m.kernel_plan = 2
     items = np.array([5, 99])
     kw = dict(max_nodes_per_hop=100, batch_size=128, draw_seed=4)
@@ -399,8 +359,8 @@ def test_recommend_users_ranks_by_the_keys_of_predict_draws():
 
 def test_recommend_sessions_equal_recommend_on_the_edited_graph():
     from tests.test_gpu_sessions import _A_s, _edits, _rows
-    A = _ds("ml_100k")["adj_train"]
-    m = _model(5)
+    A = support.adj("ml_100k")
+    m = support.model(5)
     m.kernel_plan = 2
     rng = np.random.default_rng(6)
     nu = A.shape[0]
@@ -421,8 +381,8 @@ def test_recommend_sessions_equal_recommend_on_the_edited_graph():
 
 
 def test_draws_none_is_the_eval_ranking():
-    A = _ds("ml_100k")["adj_train"]
-    m = _model(5)
+    A = support.adj("ml_100k")
+    m = support.model(5)
     users = np.array([1, 2, 40])
     kw = dict(max_nodes_per_hop=100, batch_size=128)
     eng = rc.InferenceEngine(m, A, **kw)
@@ -443,8 +403,8 @@ def test_draws_none_is_the_eval_ranking():
 
 # ---- 5. lifecycle ------------------------------------------------------------------------------------------------------
 def test_engine_across_updates_and_sync_free_steps():
-    A = _ds("ml_100k")["adj_train"]
-    m = _model(5)
+    A = support.adj("ml_100k")
+    m = support.model(5)
     m.kernel_plan = 2
     g = RatingGraph(A, reserve_nnz=2000)
     kw = dict(max_nodes_per_hop=100, batch_size=64)

@@ -24,8 +24,9 @@ from igmc_b200 import recommend as rc
 from igmc_b200.models import l2_cluster
 from igmc_b200.util_functions import RatingGraph, SubgraphExtractor, _stream_ptr
 from tests import error_bounds as eb
+from tests import support
 from tests.test_gpu_error_bounds import _many_relations, _ml_100k_batch, _scaled, _small
-from tests.test_gpu_explain import _ds, _pairs, _with_cold_start
+from tests.test_gpu_explain import _pairs, _with_cold_start
 from tests.test_gpu_regimes import _extracted
 
 pytestmark = pytest.mark.gpu
@@ -46,7 +47,7 @@ def _dgcnn(NB, rgcn="pyg-1.4"):
 
 
 def _ml_1m(B=16, mnph=100):
-    ds = _ds("ml_1m")
+    ds = support.dataset("ml_1m")
     tu, tv, tl = ds["train"]
     idx = np.arange(B)
     return _extracted(ds["adj_train"], (tu[idx], tv[idx], tl[idx]), 5, 1, mnph)
@@ -60,7 +61,7 @@ def _ml_1m_uncapped():
 
 def _cold_start():
     """a rated pair, an unrated pair and the cold-start pair (a subgraph without edges) of ml_1m*"""
-    A = _with_cold_start(_ds("ml_1m")["adj_train"])
+    A = _with_cold_start(support.adj("ml_1m"))
     u, v = _pairs(A)
     return _extracted(A, (u, v, np.zeros(3, np.int64)), 5, 1, 100)
 
@@ -202,7 +203,7 @@ def test_attribute_pairs_is_the_bounded_raw_gradient(dgcnn):
     """attribute_pairs on NB = 2 models (the reference's default): every per-rating value is bit for bit the sum of
     the two directed-edge values of igmc_edge_grad on a batch of the same pairs, sampling seed and B, on the plan the
     engine chose, and that sum is within KAPPA["edge"] of ref_j + ref_{j+m} with M_j + M_{j+m}"""
-    A = _with_cold_start(_ds("ml_1m")["adj_train"])
+    A = _with_cold_start(support.adj("ml_1m"))
     m = _dgcnn(2) if dgcnn else _igmc(4, 5, 2)
     m.eval()
     u, v = _pairs(A)

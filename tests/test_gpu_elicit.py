@@ -3,8 +3,6 @@
 The oracle is the contract: every score x_a(t) is ``predict_sessions`` of a session with the session's edits plus the
 edit (q, a + 1) (bit for bit, at the same kernel plan and batch size), aggregated by ``question_impact_host``; the
 ranking is a stable sort of ``question_impact``'s keys in ``recommend``'s order."""
-import functools
-import os
 import tempfile
 
 import numpy as np
@@ -12,36 +10,10 @@ import pytest
 import torch
 
 from igmc_b200 import recommend as rc
-from igmc_b200.data import build_adj, make_synthetic_dataset, synth_ratings
 from igmc_b200.util_functions import RatingGraph
+from tests import support
 
 pytestmark = pytest.mark.gpu
-
-
-@functools.lru_cache(maxsize=None)
-def _ds(name):
-    if name == "r13":
-        u, v, lab = synth_ratings(400, 300, 9000, 13, seed=4)
-        return build_adj(u, v, lab, 400, 300)
-    return make_synthetic_dataset(name, seed=0)["adj_train"]
-
-
-def _model(R, h=1, rgcn="pyg-1.4", dgcnn=False, nb=4, seed=0):
-    from igmc_b200.models import DGCNN_RS, IGMC
-    torch.manual_seed(seed)
-    if dgcnn:
-        m = DGCNN_RS(2 * h + 2, latent_dim=[32, 32, 32, 1], k=30, num_relations=R, num_bases=nb, regression=True,
-                     rgcn=rgcn)
-    else:
-        m = IGMC(2 * h + 2, latent_dim=[32] * 4, num_relations=R, num_bases=nb, regression=True, rgcn=rgcn)
-    return m.cuda()
-
-
-def _same(a, b):
-    a, b = np.asarray(a, np.float32), np.asarray(b, np.float32)
-    n = np.isnan(a)
-    return a.shape == b.shape and np.array_equal(n, np.isnan(b)) and np.array_equal(a[~n].view(np.uint32),
-                                                                                   b[~n].view(np.uint32))
 
 
 def _specs(g, R, seed):
@@ -111,31 +83,18 @@ CASES = {
 }
 
 
-def _checkpoints(m, K, d):
-    paths = []
-    own = {k: v.clone() for k, v in m.state_dict().items()}
-    for k in range(K):
-        torch.manual_seed(100 + k)
-        with torch.no_grad():
-            m.flat_params.add_(torch.randn_like(m.flat_params) * 0.05)
-        paths.append(os.path.join(d, "ck%d.pt" % k))
-        torch.save(m.state_dict(), paths[-1])
-    m.load_state_dict(own)
-    return paths
-
-
 # ---- 1. every impact and answer mean is the host aggregation over predict_sessions ----------------------------------
 @pytest.mark.parametrize("name", list(CASES))
 def test_impacts_equal_host_aggregation(name):
     dsn, h, mnph, ratio, kw, plan, K = CASES[name]
-    A = _ds(dsn)
+    A = support.adj(dsn)
     R = 13 if dsn == "r13" else 5
     g = RatingGraph(A)
-    m = _model(R, h=h, **kw)
+    m = support.model(R, h=h, **kw)
     m.kernel_plan = plan
     try:
         with tempfile.TemporaryDirectory() as d:
-            ck = _checkpoints(m, K, d) if K else None
+            ck = support.checkpoints(m, K, d) if K else None
             B = max(64, 4 * R)
             opts = dict(h=h, max_nodes_per_hop=mnph, sample_ratio=ratio, batch_size=B, checkpoints=ck, sample_seed=3)
             specs = _specs(g, R, len(name))
@@ -150,7 +109,7 @@ def test_impacts_equal_host_aggregation(name):
             for targets in (shared, per):
                 got = rc.question_impact(m, S, us, uq, targets, **opts)
                 imp, mean = rc.question_impact_host(R, targets, us, uq, scorer)
-                assert _same(got.impact.cpu().numpy(), imp) and _same(got.answer_mean.cpu().numpy(), mean)
+                assert support.same(got.impact.cpu().numpy(), imp) and support.same(got.answer_mean.cpu().numpy(), mean)
                 assert np.isfinite(imp).all()
     finally:
         m.kernel_plan = "auto"
@@ -165,9 +124,9 @@ def _ranked(impact, us, uq, S, n):
 
 
 def test_ranking_equals_stable_sort_of_impacts():
-    A = _ds("ml_100k")
+    A = support.adj("ml_100k")
     g = RatingGraph(A)
-    m = _model(5)
+    m = support.model(5)
     ni = g.shape[1]
     specs = _specs(g, 5, 1)
     S = _sessions(g, specs)
@@ -193,7 +152,7 @@ def test_ranking_equals_stable_sort_of_impacts():
         uq = np.concatenate(cand).astype(np.int64)
         imp = rc.question_impact(m, S, us, uq, targets, **opts).impact.cpu().numpy()
         want_i, want_s = _ranked(imp, us, uq, 4, n)
-        assert np.array_equal(items.cpu().numpy(), want_i) and _same(top.cpu().numpy(), want_s)
+        assert np.array_equal(items.cpu().numpy(), want_i) and support.same(top.cpu().numpy(), want_s)
     assert (items.cpu().numpy()[1, 3:] == -1).all()
 
 
@@ -220,9 +179,9 @@ def _run(m, g, S, n, targets, questions, B, use_graph=True, sync_check=False):
 
 
 def test_independent_of_batch_replay_and_other_sessions():
-    A = _ds("ml_1m")
+    A = support.adj("ml_1m")
     g = RatingGraph(A)
-    m = _model(5)
+    m = support.model(5)
     specs = _specs(g, 5, 4)
     S = _sessions(g, specs)
     targets = [11, 12, 13]                                                 # W = 3, U = 15
@@ -230,21 +189,21 @@ def test_independent_of_batch_replay_and_other_sessions():
     base = _run(m, g, S, 10, targets, questions, 64)
     for B in (15, 16, 256):                                                # B = U exactly, and padded tails
         got = _run(m, g, S, 10, targets, questions, B)
-        assert np.array_equal(got[0], base[0]) and _same(got[1], base[1])
+        assert np.array_equal(got[0], base[0]) and support.same(got[1], base[1])
     for got in (_run(m, g, S, 10, targets, questions, 64, use_graph=False), _run(m, g, S, 10, targets, questions, 64)):
-        assert np.array_equal(got[0], base[0]) and _same(got[1], base[1])
+        assert np.array_equal(got[0], base[0]) and support.same(got[1], base[1])
     more = _sessions(g, specs + [(5, []), (g.shape[0] + 1, [(3, 2)])])    # added sessions
     got = _run(m, g, more, 10, targets, questions, 64)
-    assert np.array_equal(got[0][:4], base[0]) and _same(got[1][:4], base[1])
+    assert np.array_equal(got[0][:4], base[0]) and support.same(got[1][:4], base[1])
     sync = _run(m, g, S, 10, targets, questions, 32, sync_check=True)
-    assert np.array_equal(sync[0], base[0]) and _same(sync[1], base[1])
+    assert np.array_equal(sync[0], base[0]) and support.same(sync[1], base[1])
 
 
 # ---- 4. validation ------------------------------------------------------------------------------------------------------
 def test_validation_and_updates():
-    A = _ds("ml_100k")
+    A = support.adj("ml_100k")
     g = RatingGraph(A, reserve_nnz=10)
-    m = _model(5)
+    m = support.model(5)
     nu, ni = A.shape
     S = _sessions(g, [(0, []), (nu + 1, [(4, 2)])])
     rated = int(g.host["col_idx"][g.host["row_ptr"][0]])
@@ -290,6 +249,6 @@ def test_validation_and_updates():
         S2 = _sessions(g, [(0, []), (nu + 1, [(4, 2)])])
         got = eng.question_impact(S2, [0], [rated], [1, 2])                # now a question
         want = rc.question_impact(m, S2, [0], [rated], [1, 2], batch_size=32)
-        assert _same(got.impact.cpu().numpy(), want.impact.cpu().numpy())
+        assert support.same(got.impact.cpu().numpy(), want.impact.cpu().numpy())
     finally:
         eng.close()

@@ -10,27 +10,12 @@ import torch
 from igmc_b200 import _lib
 from igmc_b200 import recommend as rc
 from tests import elicit_cases as ec
+from tests import support
 
 pytestmark = pytest.mark.gpu
 
 SENT32, SENT8, SENTF = -77, 0xAB, -7.5
 GUARD = 16
-
-
-def _dev(a, dtype):
-    return torch.as_tensor(np.asarray(a)).to(dtype).cuda()
-
-
-def _same(a, b):
-    """fp32 arrays equal bit for bit, NaN matching any NaN (an inf - inf carries the device's NaN payload)"""
-    a, b = np.asarray(a, np.float32), np.asarray(b, np.float32)
-    n = np.isnan(a)
-    return a.shape == b.shape and np.array_equal(n, np.isnan(b)) and np.array_equal(a[~n].view(np.uint32),
-                                                                                   b[~n].view(np.uint32))
-
-
-def _full(n, value, dtype):
-    return torch.full((n + GUARD,), value, dtype=dtype, device="cuda")
 
 
 def _pairs(c, row_cap=None):
@@ -41,15 +26,17 @@ def _pairs(c, row_cap=None):
     W, A, B = t2.shape[1], c["A"], c["B"]
     L = max(len(r) for r in c["rows"]) + 1
     cap = (B // W) * L if row_cap is None else row_cap
-    keep = [_dev(c["users"], torch.int32), _dev(rp, torch.int32), _dev(np.r_[ci, 0], torch.int32),
-            _dev(np.r_[rt, 0], torch.uint8)]
+    keep = [support.dev(c["users"], torch.int32), support.dev(rp, torch.int32), support.dev(np.r_[ci, 0], torch.int32),
+            support.dev(np.r_[rt, 0], torch.uint8)]
     Sd = _lib.Sessions(*(t.data_ptr() for t in keep), S, L - 1)
-    targets = _dev(t2, torch.int32)
-    us, uq, ut = _dev(c["unit_s"], torch.int32), _dev(c["unit_q"], torch.int32), _dev(c["unit_tag"], torch.int64)
-    out = dict(u=_full(B, SENT32, torch.int32), v=_full(B, SENT32, torch.int32), pid=_full(B, SENT32, torch.int64),
-               tag=_full(B, SENT32, torch.int64), ru=_full(B, SENT32, torch.int32), rptr=_full(B + 1, SENT32, torch.int32),
-               rcol=_full(cap, SENT32, torch.int32), rrat=_full(cap, SENT8, torch.uint8),
-               sess=_full(B, SENT32, torch.int32))
+    targets = support.dev(t2, torch.int32)
+    us, uq = support.dev(c["unit_s"], torch.int32), support.dev(c["unit_q"], torch.int32)
+    ut = support.dev(c["unit_tag"], torch.int64)
+    out = dict(u=support.filled(B, SENT32, torch.int32), v=support.filled(B, SENT32, torch.int32),
+               pid=support.filled(B, SENT32, torch.int64), tag=support.filled(B, SENT32, torch.int64),
+               ru=support.filled(B, SENT32, torch.int32), rptr=support.filled(B + 1, SENT32, torch.int32),
+               rcol=support.filled(cap, SENT32, torch.int32), rrat=support.filled(cap, SENT8, torch.uint8),
+               sess=support.filled(B, SENT32, torch.int32))
     err = torch.zeros(1, dtype=torch.int32, device="cuda")
     rc_ = _lib.load().igmc_elicit_pairs(C.byref(Sd), c["num_items"], A, targets.data_ptr(), W, int(len(t2) > 1),
                                         us.data_ptr(), uq.data_ptr(), ut.data_ptr(), B, out["u"].data_ptr(),
@@ -126,24 +113,24 @@ def test_stats_kernel_matches_twin(case, form):
     c = case
     K, B, A, W = c["K"], c["B"], c["A"], c["W"]
     G = B // (A * W)
-    preds = _dev(np.asarray(c["preds"], np.float32).reshape(K, B), torch.float32)
-    tag = _dev(c["tag"], torch.int64)
+    preds = support.dev(np.asarray(c["preds"], np.float32).reshape(K, B), torch.float32)
+    tag = support.dev(c["tag"], torch.int64)
     impact, mean, utag = rc.elicit_stats_host(np.asarray(c["preds"], np.float32), K, B, A, W, c["tag"])
     T = int(max(c["tag"])) + 1
-    key = _full(G, SENTF, torch.float32)
-    imp = _full(T, SENTF, torch.float32)
-    am = _full(T * A, SENTF, torch.float32)
+    key = support.filled(G, SENTF, torch.float32)
+    imp = support.filled(T, SENTF, torch.float32)
+    am = support.filled(T * A, SENTF, torch.float32)
     args = (key.data_ptr(), None, None) if form == "key" else (None, imp.data_ptr(), am.data_ptr())
     assert _lib.load().igmc_elicit_stats(preds.data_ptr(), K, B, A, W, tag.data_ptr(), *args, None) == 0
     torch.cuda.synchronize()
     key, imp, am = key.cpu().numpy(), imp.cpu().numpy(), am.cpu().numpy()
     if form == "key":
         real = utag >= 0
-        assert _same(key[:G][real], impact[real]) and (key[:G][~real] == 0).all()
+        assert support.same(key[:G][real], impact[real]) and (key[:G][~real] == 0).all()
         assert (key[G:] == SENTF).all()
     else:
         want_i, want_m = np.full(T, SENTF, np.float32), np.full((T, A), SENTF, np.float32)
         for g in np.flatnonzero(utag >= 0):
             want_i[utag[g]], want_m[utag[g]] = impact[g], mean[g]
-        assert _same(imp[:T], want_i) and _same(am[:T * A], want_m.reshape(-1))
+        assert support.same(imp[:T], want_i) and support.same(am[:T * A], want_m.reshape(-1))
         assert (imp[T:] == SENTF).all() and (am[T * A:] == SENTF).all()

@@ -8,7 +8,6 @@
 * a masked forward that drops nothing is the eval forward bit for bit;
 * the order is the documented one, top-m is a prefix of it, and results do not depend on B or graph replay;
 * checkpoints, graph updates, and steady-state steps without a host synchronisation."""
-import functools
 import os
 import tempfile
 
@@ -19,45 +18,18 @@ import torch
 
 from igmc_b200 import _lib
 from igmc_b200 import recommend as rc
-from igmc_b200.data import build_adj, make_synthetic_dataset, synth_ratings
 from igmc_b200.util_functions import Batch, RatingGraph, SubgraphExtractor
 from oracle import extract_np, pyg_restated
 from tests import pyg2_oracle
+from tests import support
 from tests.test_gpu_graph_update import _apply_scipy
 
 pytestmark = pytest.mark.gpu
 
 
-@functools.lru_cache(maxsize=None)
-def _ds(name):
-    return make_synthetic_dataset(name, seed=0)
-
-
-@functools.lru_cache(maxsize=None)
-def _r13():
-    nu, ni = 400, 300
-    u, v, lab = synth_ratings(nu, ni, 9000, 13, seed=4)
-    return build_adj(u, v, lab, nu, ni)
-
-
 def _with_cold_start(A):
     """A with one more user and one more item, neither rated: the pair (new user, new item) has no ratings at all"""
     return ssp.csr_matrix(ssp.bmat([[A, None], [None, ssp.csr_matrix((1, 1), dtype=A.dtype)]]), dtype=A.dtype)
-
-
-def _model(R, h=1, rgcn="pyg-1.4", dgcnn=False, seed=0):
-    from igmc_b200.models import DGCNN_RS, IGMC
-    torch.manual_seed(seed)
-    if dgcnn:
-        m = DGCNN_RS(2 * h + 2, latent_dim=[32, 32, 32, 1], k=30, num_relations=R, num_bases=4, regression=True,
-                     rgcn=rgcn)
-    else:
-        m = IGMC(2 * h + 2, latent_dim=[32] * 4, num_relations=R, num_bases=4, regression=True, rgcn=rgcn)
-    if rgcn == "pyg-2":
-        with torch.no_grad():
-            for c in m.convs:
-                c.bias.uniform_(-0.3, 0.3)
-    return m.cuda()
 
 
 def _pairs(A, small=False):
@@ -151,10 +123,10 @@ INEXACT = {"plan 1 ml_1m"}      # the cases held to a bound instead of bit equal
 @pytest.mark.parametrize("name", list(CASES))
 def test_occluded_scores_equal_the_masked_forward(name):
     dsn, h, mnph, kw, force, plan, small = CASES[name]
-    A0 = _r13() if dsn == "r13" else _ds(dsn)["adj_train"]
+    A0 = support.adj(dsn)
     R = 13 if dsn == "r13" else 5
     A = _with_cold_start(A0)
-    m = _model(R, h, **kw)
+    m = support.model(R, h=h, **kw, pyg2_bias=True)
     m.kernel_plan = force
     u, v = _pairs(A, small)
     B, seed = 64, 7
@@ -205,8 +177,8 @@ def test_occluded_scores_equal_the_masked_forward(name):
 def test_all_ones_mask_is_the_eval_forward():
     for dsn, kw, force in (("ml_1m", {}, "auto"), ("ml_1m", dict(dgcnn=True), "auto"), ("ml_1m", {}, 0),
                            ("ml_1m", dict(rgcn="pyg-2"), 4)):
-        A = _ds(dsn)["adj_train"]
-        m = _model(5, **kw)
+        A = support.adj(dsn)
+        m = support.model(5, **kw, pyg2_bias=True)
         m.kernel_plan = force
         ex = SubgraphExtractor(RatingGraph(A), [0], [0], [0], np.arange(1, 6, dtype=np.float32), 1, 1.0, 100,
                                max_batch=50, seed=3)
@@ -224,10 +196,10 @@ def test_all_ones_mask_is_the_eval_forward():
 # ---- 2. against the fp64 restated forward --------------------------------------------------------------------------------
 @pytest.mark.parametrize("rgcn", ["pyg-1.4", "pyg-2"])
 def test_occluded_scores_against_oracle(rgcn):
-    A0 = _ds("ml_1m")["adj_train"]
+    A0 = support.adj("ml_1m")
     A = _with_cold_start(A0)
     R, mnph, seed = 5, 100, 7
-    m = _model(R, rgcn=rgcn)
+    m = support.model(R, rgcn=rgcn, pyg2_bias=True)
     ref = pyg2_oracle.igmc_ref(rgcn, 4, (32,) * 4, R, 4, 0.0)
     ref.load_state_dict({k: v.double().cpu() for k, v in m.state_dict().items()})
     ref = pyg_restated.set_formulation(ref.double(), "transform").cuda().eval()
@@ -271,8 +243,8 @@ def test_occluded_scores_against_oracle(rgcn):
 
 # ---- 3. order, top-m, determinism ----------------------------------------------------------------------------------------
 def test_order_topm_and_determinism():
-    A = _with_cold_start(_ds("ml_1m")["adj_train"])
-    m = _model(5)
+    A = _with_cold_start(support.adj("ml_1m"))
+    m = support.model(5)
     m.kernel_plan = 2                  # the same plan at both batch sizes
     u, v = _pairs(A)
     results = {}
@@ -306,8 +278,8 @@ def test_order_topm_and_determinism():
 
 
 def test_validation_and_empty_input():
-    A = _ds("ml_100k")["adj_train"]
-    m = _model(5)
+    A = support.adj("ml_100k")
+    m = support.model(5)
     with pytest.raises(IndexError):
         rc.explain_pairs(m, A, [A.shape[0]], [0])
     with pytest.raises(ValueError):
@@ -328,14 +300,14 @@ def test_validation_and_empty_input():
 
 # ---- 4. checkpoints --------------------------------------------------------------------------------------------------------
 def test_two_checkpoints_are_the_fp32_mean():
-    A = _with_cold_start(_ds("ml_100k")["adj_train"])
-    m = _model(5)
+    A = _with_cold_start(support.adj("ml_100k"))
+    m = support.model(5)
     u, v = _pairs(A, small=True)
     with tempfile.TemporaryDirectory() as tmp:
         paths = []
         for c in range(2):
             paths.append(os.path.join(tmp, "model_checkpoint%d.pth" % c))
-            torch.save(_model(5, seed=c + 1).state_dict(), paths[-1])
+            torch.save(support.model(5, seed=c + 1).state_dict(), paths[-1])
         runs = []
         for ck in (paths, paths[:1], paths[1:]):
             eng = rc.InferenceEngine(m, A, max_nodes_per_hop=200, batch_size=50, checkpoints=ck)
@@ -350,8 +322,8 @@ def test_two_checkpoints_are_the_fp32_mean():
 
 # ---- 5. graph updates --------------------------------------------------------------------------------------------------------
 def test_engine_explains_across_updates():
-    A = _ds("ml_1m")["adj_train"]
-    m = _model(5)
+    A = support.adj("ml_1m")
+    m = support.model(5)
     g = RatingGraph(A, reserve_nnz=2000)
     eng = rc.InferenceEngine(m, g, max_nodes_per_hop=100, batch_size=64, sample_seed=4)
     rng = np.random.default_rng(5)
@@ -378,8 +350,8 @@ def test_engine_explains_across_updates():
 
 # ---- 6. steady state ----------------------------------------------------------------------------------------------------------
 def test_steady_state_steps_do_not_sync():
-    A = _ds("ml_1m")["adj_train"]
-    m = _model(5)
+    A = support.adj("ml_1m")
+    m = support.model(5)
     eng = rc.InferenceEngine(m, A, max_nodes_per_hop=100, batch_size=50, sample_seed=1)
     u, v = np.array([11, 12]), np.array([40, 41])
     outs = []

@@ -22,7 +22,8 @@ from igmc_b200 import recommend as rc
 from igmc_b200.util_functions import Batch, RatingGraph
 from oracle import extract_np, pyg_restated
 from tests import pyg2_oracle
-from tests.test_gpu_explain import _ds, _expected_order, _model, _pairs, _r13, _subgraph, _with_cold_start
+from tests import support
+from tests.test_gpu_explain import _expected_order, _pairs, _subgraph, _with_cold_start
 from tests.test_gpu_graph_update import _apply_scipy
 
 pytestmark = pytest.mark.gpu
@@ -98,10 +99,10 @@ INEXACT = {"plan 1 ml_1m"}      # held to 8 ulps, as test_gpu_explain holds expl
 @pytest.mark.parametrize("name", list(CASES))
 def test_occluded_scores_equal_the_node_filtered_forward(name):
     dsn, h, mnph, kw, force, plan, small = CASES[name]
-    A0 = _r13() if dsn == "r13" else _ds(dsn)["adj_train"]
+    A0 = support.adj(dsn)
     R = 13 if dsn == "r13" else 5
     A = _with_cold_start(A0)
-    m = _model(R, h, **kw)
+    m = support.model(R, h=h, **kw, pyg2_bias=True)
     m.kernel_plan = force
     u, v = _pairs(A, small)
     B, seed = 64, 7
@@ -143,8 +144,8 @@ def test_occluded_scores_equal_the_node_filtered_forward(name):
 # ---- 2. a node with one rating is that rating's explain_pairs entry ------------------------------------------------------
 @pytest.mark.parametrize("kw", [{}, dict(dgcnn=True)], ids=["IGMC", "DGCNN_RS"])
 def test_single_rating_node_is_the_rating_delta(kw):
-    A = _ds("ml_100k")["adj_train"]
-    m = _model(5, **kw)
+    A = support.adj("ml_100k")
+    m = support.model(5, **kw, pyg2_bias=True)
     u, v = np.array([3, 40, 100]), np.array([7, 50, 2])
     args = dict(max_nodes_per_hop=50, batch_size=64, sample_seed=3)
     nd = rc.explain_nodes(m, A, u, v, **args)
@@ -169,9 +170,9 @@ def test_single_rating_node_is_the_rating_delta(kw):
 # ---- 3. against the fp64 restated forward ----------------------------------------------------------------------------------
 @pytest.mark.parametrize("rgcn", ["pyg-1.4", "pyg-2"])
 def test_occluded_scores_against_oracle(rgcn):
-    A = _with_cold_start(_ds("ml_1m")["adj_train"])
+    A = _with_cold_start(support.adj("ml_1m"))
     R, mnph, seed = 5, 100, 7
-    m = _model(R, rgcn=rgcn)
+    m = support.model(R, rgcn=rgcn, pyg2_bias=True)
     ref = pyg2_oracle.igmc_ref(rgcn, 4, (32,) * 4, R, 4, 0.0)
     ref.load_state_dict({k: v.double().cpu() for k, v in m.state_dict().items()})
     ref = pyg_restated.set_formulation(ref.double(), "transform").cuda().eval()
@@ -214,8 +215,8 @@ def test_occluded_scores_against_oracle(rgcn):
 
 # ---- 4. order, top-m, padding, determinism ---------------------------------------------------------------------------------
 def test_order_topm_and_determinism():
-    A = _with_cold_start(_ds("ml_1m")["adj_train"])
-    m = _model(5)
+    A = _with_cold_start(support.adj("ml_1m"))
+    m = support.model(5)
     m.kernel_plan = 2                  # the same plan at every batch size
     u, v = _pairs(A)
     results = {}
@@ -249,8 +250,8 @@ def test_order_topm_and_determinism():
 
 
 def test_validation_and_empty_input():
-    A = _ds("ml_100k")["adj_train"]
-    m = _model(5)
+    A = support.adj("ml_100k")
+    m = support.model(5)
     with pytest.raises(IndexError):
         rc.explain_nodes(m, A, [A.shape[0]], [0])
     with pytest.raises(NotImplementedError):
@@ -265,14 +266,14 @@ def test_validation_and_empty_input():
 
 # ---- 5. checkpoints, graph updates, steady state ---------------------------------------------------------------------------
 def test_two_checkpoints_are_the_fp32_mean():
-    A = _with_cold_start(_ds("ml_100k")["adj_train"])
-    m = _model(5)
+    A = _with_cold_start(support.adj("ml_100k"))
+    m = support.model(5)
     u, v = _pairs(A, small=True)
     with tempfile.TemporaryDirectory() as tmp:
         paths = []
         for c in range(2):
             paths.append(os.path.join(tmp, "model_checkpoint%d.pth" % c))
-            torch.save(_model(5, seed=c + 1).state_dict(), paths[-1])
+            torch.save(support.model(5, seed=c + 1).state_dict(), paths[-1])
         runs = []
         for ck in (paths, paths[:1], paths[1:]):
             eng = rc.InferenceEngine(m, A, max_nodes_per_hop=200, batch_size=50, checkpoints=ck)
@@ -286,8 +287,8 @@ def test_two_checkpoints_are_the_fp32_mean():
 
 
 def test_engine_explains_nodes_across_updates():
-    A = _ds("ml_1m")["adj_train"]
-    m = _model(5)
+    A = support.adj("ml_1m")
+    m = support.model(5)
     g = RatingGraph(A, reserve_nnz=2000)
     eng = rc.InferenceEngine(m, g, max_nodes_per_hop=100, batch_size=64, sample_seed=4)
     rng = np.random.default_rng(5)
@@ -313,8 +314,8 @@ def test_engine_explains_nodes_across_updates():
 
 
 def test_steady_state_steps_do_not_sync():
-    A = _ds("ml_1m")["adj_train"]
-    m = _model(5)
+    A = support.adj("ml_1m")
+    m = support.model(5)
     eng = rc.InferenceEngine(m, A, max_nodes_per_hop=100, batch_size=50, sample_seed=1)
     u, v = np.array([11, 12]), np.array([40, 41])
     outs = []

@@ -9,6 +9,7 @@ import pytest
 import torch
 
 from igmc_b200.data import build_adj, make_synthetic_dataset, synth_ratings
+from tests import support
 from tests.helpers import IMG_HDR, XCH, XR, own_cap_of
 
 pytestmark = pytest.mark.gpu
@@ -23,14 +24,6 @@ def _batch(A, pairs, R, mnph, B=None, seed=3):
                          seed=seed)
     idx = np.arange(len(pu)) if B is None else np.random.default_rng(0).choice(len(pu), B, replace=False)
     return d.extract_batch(idx)
-
-
-def _model(R, adj_dropout, plan="auto"):
-    from igmc_b200.models import IGMC
-    torch.manual_seed(0)
-    m = IGMC(4, latent_dim=[32] * 4, num_relations=R, num_bases=4, regression=True, adj_dropout=adj_dropout).cuda()
-    m.kernel_plan = plan
-    return m
 
 
 def _check_images(m, b, training):
@@ -105,7 +98,7 @@ def test_run_flags_ml_1m():
     ds = make_synthetic_dataset("ml_1m", seed=0)
     b = _batch(ds["adj_train"], ds["train"], 5, 100, B=50)
     for p in (0.0, 0.2):
-        staged = _check_images(_model(5, p), b, True)
+        staged = _check_images(support.model(5, adj_dropout=p), b, True)
         assert staged["fwd"].all() and staged["bwd"].all()
 
 
@@ -113,7 +106,7 @@ def test_run_flags_ml_100k_dropout():
     """ml_100k*, mnph 200, edge dropout 0.2: compacted kept lists"""
     ds = make_synthetic_dataset("ml_100k", seed=0)
     b = _batch(ds["adj_train"], ds["train"], 5, 200, B=50)
-    staged = _check_images(_model(5, 0.2), b, True)
+    staged = _check_images(support.model(5, adj_dropout=0.2), b, True)
     assert staged["fwd"].any()
 
 
@@ -122,7 +115,7 @@ def test_run_flags_twelve_relations():
     u, v, lab = synth_ratings(400, 300, 9000, num_classes=12, seed=5)
     A = build_adj(u, v, lab, 400, 300)
     b = _batch(A, (u, v, lab), 12, 60, B=40)
-    m = _model(12, 0.2)
+    m = support.model(12, adj_dropout=0.2)
     _check_images(m, b, True)
     _check_images(m, b, False)
 
@@ -141,5 +134,7 @@ def test_unstaged_lists_carry_no_masks():
     pick = np.array([blk[17], bg[0], blk[5000], bg[1]])
     b = _batch(A, (u[pick], v[pick], lab[pick]), 5, 100)
     assert b._priv["n_cap"] == 202
-    staged = _check_images(_model(5, 0.2, plan=2), b, True)
+    m = support.model(5, adj_dropout=0.2)
+    m.kernel_plan = 2
+    staged = _check_images(m, b, True)
     assert np.any((staged["fwd"] == 1) & (staged["bwd"] == 0)), "no CTA with staged forward and global backward lists"

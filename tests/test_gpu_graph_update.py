@@ -6,7 +6,6 @@
 * capacity overflow and invalid device input leave the graph unchanged; the five device pointers never change;
 * an extractor and an InferenceEngine kept across updates give the bits a fresh one on RatingGraph(A_updated) gives;
 * an update during an engine run, and a TrainEngine whose graph changed after its first step, raise."""
-import functools
 
 import numpy as np
 import pytest
@@ -14,17 +13,13 @@ import scipy.sparse as ssp
 import torch
 
 from igmc_b200 import recommend as rc
-from igmc_b200.data import build_adj, make_synthetic_dataset, synth_ratings
+from igmc_b200.data import make_synthetic_dataset
 from igmc_b200.util_functions import RatingGraph, SubgraphExtractor, graph_update_host
+from tests import support
 
 pytestmark = pytest.mark.gpu
 
 ARRAYS = ("row_ptr", "col_idx", "rating", "col_ptr", "row_idx")
-
-
-@functools.lru_cache(maxsize=None)
-def _ds(name):
-    return make_synthetic_dataset(name, seed=0)
 
 
 def _apply_scipy(A, u, v, x, shape):
@@ -76,7 +71,7 @@ def _assert_graph_equal(g, A_want):
 
 @pytest.mark.parametrize("name", ["ml_100k", "ml_1m", "flixster"])
 def test_update_matches_twin_and_rebuild(name):
-    ds = _ds(name)
+    ds = support.dataset(name)
     A, R = ds["adj_train"], ds["num_relations"]
     rng = np.random.default_rng(5)
     for n in (1, 1000, 100000):
@@ -96,7 +91,7 @@ def test_update_matches_twin_and_rebuild(name):
 
 
 def test_chain_of_updates_and_growth_to_capacity():
-    ds = _ds("ml_100k")
+    ds = support.dataset("ml_100k")
     A = ds["adj_train"]
     g = RatingGraph(A, reserve_nnz=20000, reserve_users=40, reserve_items=30)
     cu, ci, _ = g.capacity
@@ -117,7 +112,7 @@ def test_chain_of_updates_and_growth_to_capacity():
 
 
 def test_shape_only_and_noop_updates():
-    A = _ds("ml_100k")["adj_train"]
+    A = support.adj("ml_100k")
     g = RatingGraph(A, reserve_users=3, reserve_items=2)
     v0 = g.version
     coo = A.tocoo()
@@ -133,7 +128,7 @@ def test_shape_only_and_noop_updates():
 
 
 def test_overflow_and_invalid_device_input_leave_the_graph():
-    A = _ds("ml_100k")["adj_train"]
+    A = support.adj("ml_100k")
     g = RatingGraph(A, reserve_nnz=10, reserve_users=2)
     snap = {k: t.clone() for k, t in g.dev.items()}
     fields = (g.shape, g.nnz, g.max_row_deg, g.max_col_deg, g.version)
@@ -177,7 +172,7 @@ def _batch_arrays(b):
 @pytest.mark.parametrize("h,mnph,fast", [(1, None, True), (1, 100, True), (1, None, False), (1, 100, False),
                                          (2, 30, True), (2, None, True)])
 def test_extractor_follows_updates(h, mnph, fast):
-    A = _ds("ml_100k")["adj_train"]
+    A = support.adj("ml_100k")
     g = RatingGraph(A, reserve_nnz=10000)
     cv = np.arange(1, 6, dtype=np.float32)
     kept = SubgraphExtractor(g, [0], [0], [0], cv, h, 1.0, mnph, max_batch=64, seed=3, fast=fast)
@@ -202,26 +197,13 @@ def test_extractor_follows_updates(h, mnph, fast):
         assert caps[-1] > caps[0]            # the workspace was re-reserved for the grown degrees
 
 
-def _model(R, seed=0):
-    from igmc_b200.models import IGMC
-    torch.manual_seed(seed)
-    return IGMC(4, latent_dim=[32] * 4, num_relations=R, num_bases=4, regression=True).cuda()
-
-
-@functools.lru_cache(maxsize=None)
-def _r13():
-    nu, ni = 400, 300
-    u, v, lab = synth_ratings(nu, ni, 9000, 13, seed=4)
-    return build_adj(u, v, lab, nu, ni)
-
-
 @pytest.mark.parametrize("case", ["ml_1m plan 2", "r13 plan 0"])
 def test_engine_serves_across_updates(case):
     if case == "ml_1m plan 2":
-        A, R, mnph, plan = _ds("ml_1m")["adj_train"], 5, 100, 2
+        A, R, mnph, plan = support.adj("ml_1m"), 5, 100, 2
     else:
-        A, R, mnph, plan = _r13(), 13, 50, 0
-    m = _model(R)
+        A, R, mnph, plan = support.adj("r13"), 13, 50, 0
+    m = support.model(R)
     g = RatingGraph(A, reserve_nnz=5000, reserve_users=3, reserve_items=2)
     eng = rc.InferenceEngine(m, g, max_nodes_per_hop=mnph, batch_size=50, sample_seed=5)
     rng = np.random.default_rng(1)
@@ -258,8 +240,8 @@ def test_engine_serves_across_updates(case):
 
 
 def test_update_during_a_run_raises():
-    A = _ds("ml_100k")["adj_train"]
-    m = _model(5)
+    A = support.adj("ml_100k")
+    m = support.model(5)
     g = RatingGraph(A, reserve_nnz=10)
     eng = rc.InferenceEngine(m, g, max_nodes_per_hop=50, batch_size=50)
     eng.start_recommend([1, 2, 3], 5)

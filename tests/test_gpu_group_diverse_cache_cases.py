@@ -16,6 +16,7 @@ from igmc_b200 import recommend as rc
 from igmc_b200.data import build_adj, synth_ratings
 from igmc_b200.util_functions import RatingGraph
 from tests import group_diverse_cache_cases as gc
+from tests import support
 from tests.ranking_cases import same_f32
 
 pytestmark = pytest.mark.gpu
@@ -23,10 +24,6 @@ pytestmark = pytest.mark.gpu
 S32, SF, S8 = -77, -7.5, 0xAB
 GUARD = 16
 CASES = gc.all_cases()
-
-
-def _id(c):
-    return "%s: %s" % (c["kernel"], c["name"])
 
 
 def _of(kernel):
@@ -43,15 +40,11 @@ def _release_inputs():
     _ALIVE.clear()
 
 
-def _dev(a, dtype=torch.int32):
-    a = np.asarray(a)
-    t = torch.as_tensor(a if a.size else np.zeros(1, a.dtype)).to(dtype).cuda()
+def _alive(a, dtype=torch.int32):
+    """a host array on the device (an empty one as one zero), kept alive for the rest of the session"""
+    t = support.dev(support.nonempty(a), dtype)
     _ALIVE.append(t)
     return t
-
-
-def _full(n, value, dtype=torch.int32):
-    return torch.full((max(int(n), 0) + GUARD,), value, dtype=dtype, device="cuda")
 
 
 def _err():
@@ -61,11 +54,11 @@ def _err():
 class _Graph:
     """a device CSR (with columns when asked) kept alive with its tensors"""
     def __init__(self, rp, ci, num_users, num_items, cols=False):
-        self.keep = [_dev(rp), _dev(ci)]
+        self.keep = [_alive(rp), _alive(ci)]
         cp = None
         if cols:
             cp_h, ri = gc.columns(rp, ci, num_items)
-            self.keep += [_dev(cp_h), _dev(ri)]
+            self.keep += [_alive(cp_h), _alive(ri)]
             cp = self.keep[2].data_ptr()
         self.c = _lib.CSR(self.keep[0].data_ptr(), self.keep[1].data_ptr(), None, cp,
                           self.keep[3].data_ptr() if cols else None, num_users, num_items)
@@ -77,15 +70,15 @@ def _group_rows(case):
     g = _Graph(rp, ci, case["num_users"], int(ci.max()) + 1)
     members, cap = case["members"], case["cap"]
     G, M = members.shape
-    row_ptr, col = _full(G + 1, S32), _full(cap, S32)
-    ws, err, dm = torch.empty(2 * G + 1 + cap, dtype=torch.int32, device="cuda"), _err(), _dev(members)
+    row_ptr, col = support.filled(G + 1, S32), support.filled(cap, S32)
+    ws, err, dm = torch.empty(2 * G + 1 + cap, dtype=torch.int32, device="cuda"), _err(), _alive(members)
     code = _lib.load().igmc_group_rows(C.byref(g.c), dm.data_ptr(), G, M, row_ptr.data_ptr(), col.data_ptr(), cap,
                                        ws.data_ptr(), err.data_ptr(), None)
     torch.cuda.synchronize()
     return code, int(err.item()), row_ptr.cpu().numpy(), col.cpu().numpy(), (rp, ci)
 
 
-@pytest.mark.parametrize("case", _of("group_rows"), ids=_id)
+@pytest.mark.parametrize("case", _of("group_rows"), ids=support.pid)
 def test_group_rows(case):
     code, err, got_rp, got_ci, (rp, ci) = _group_rows(case)
     want_rp, want_ci, want_err = gc.group_rows_reference(case, rp, ci)
@@ -110,9 +103,9 @@ def test_group_rows_argument_checks():
 def _group_pairs(case):
     B = case["B"]
     members = case["members"]
-    out = {k: _full(B, S32, dt) for k, dt in (("u", torch.int32), ("v", torch.int32), ("pid", torch.int64),
+    out = {k: support.filled(B, S32, dt) for k, dt in (("u", torch.int32), ("v", torch.int32), ("pid", torch.int64),
                                                ("tag", torch.int64))}
-    keep = [_dev(members), _dev(case["unit_g"]), _dev(case["unit_v"]), _dev(case["unit_tag"], torch.int64)]
+    keep = [_alive(members), _alive(case["unit_g"]), _alive(case["unit_v"]), _alive(case["unit_tag"], torch.int64)]
     err = _err()
     code = _lib.load().igmc_group_pairs(keep[0].data_ptr(), len(members), members.shape[1], case["num_users"],
                                         case["num_items"], keep[1].data_ptr(), keep[2].data_ptr(), keep[3].data_ptr(),
@@ -122,7 +115,7 @@ def _group_pairs(case):
     return code, int(err.item()), [out[k].cpu().numpy() for k in ("u", "v", "pid", "tag")]
 
 
-@pytest.mark.parametrize("case", _of("group_pairs"), ids=_id)
+@pytest.mark.parametrize("case", _of("group_pairs"), ids=support.pid)
 def test_group_pairs(case):
     code, err, got = _group_pairs(case)
     want, want_err = gc.group_pairs_reference(case)
@@ -143,16 +136,16 @@ def test_group_pairs_argument_checks():
 
 @pytest.mark.parametrize("form", ["key", "scatter"])
 @pytest.mark.parametrize("agg", ["mean", "min", "max"])
-@pytest.mark.parametrize("case", _of("group_stats"), ids=_id)
+@pytest.mark.parametrize("case", _of("group_stats"), ids=support.pid)
 def test_group_stats(case, agg, form):
     K, B, M, tag = case["K"], case["B"], case["M"], case["tag"]
     Gu = B // M
     T = int(tag.max()) + 1
-    key, score, ms = _full(Gu, SF, torch.float32), _full(T, SF, torch.float32), _full(T * M, SF, torch.float32)
+    key, score, ms = (support.filled(n, SF, torch.float32) for n in (Gu, T, T * M))
     outs = (key.data_ptr(), None, None) if form == "key" else (None, score.data_ptr(), ms.data_ptr())
-    preds = _dev(np.asarray(case["preds"], np.float32).reshape(K, B), torch.float32)
+    preds = _alive(np.asarray(case["preds"], np.float32).reshape(K, B), torch.float32)
     assert _lib.load().igmc_group_stats(preds.data_ptr(), K, B, M, _lib.GROUP_AGGREGATES.index(agg),
-                                        _dev(tag, torch.int64).data_ptr(), *outs, None) == 0
+                                        _alive(tag, torch.int64).data_ptr(), *outs, None) == 0
     torch.cuda.synchronize()
     want = gc.group_stats_reference(case, agg)
     nan = float("nan")
@@ -181,16 +174,16 @@ def test_group_stats_argument_checks():
 
 # ---- diverse.cu -----------------------------------------------------------------------------------------------------------
 def _union(items, ni):
-    d = _dev(items, torch.int64)
-    bitmap = _full((ni + 31) // 32, S32)
-    mp, lst, nu, err = _full(ni, S32), _full(ni, S32), _full(1, S32), _err()
+    d = _alive(items, torch.int64)
+    bitmap = support.filled((ni + 31) // 32, S32)
+    mp, lst, nu, err = support.filled(ni, S32), support.filled(ni, S32), support.filled(1, S32), _err()
     code = _lib.load().igmc_item_union(d.data_ptr(), len(items), ni, bitmap.data_ptr(), mp.data_ptr(), lst.data_ptr(),
                                        nu.data_ptr(), err.data_ptr(), None)
     torch.cuda.synchronize()
     return code, int(err.item()), bitmap, mp, lst, nu
 
 
-@pytest.mark.parametrize("case", _of("item_union"), ids=_id)
+@pytest.mark.parametrize("case", _of("item_union"), ids=support.pid)
 def test_item_union(case):
     ni = case["num_items"]
     code, err, bitmap, mp, lst, nu = _union(case["items"], ni)
@@ -220,15 +213,15 @@ def count_graph():
     return _Graph(rp, ci, gc.COUNT_NU, gc.COUNT_NI)
 
 
-@pytest.mark.parametrize("case", _of("cocount"), ids=_id)
+@pytest.mark.parametrize("case", _of("cocount"), ids=support.pid)
 def test_cocount(case, count_graph):
     u = np.asarray(case["union"], np.int64)
     Nu = len(u)
     mp = np.full(gc.COUNT_NI, -1, np.int32)
     mp[u] = np.arange(Nu)
     need = Nu * (Nu - 1) // 2
-    table = _full(need, S32)
-    code = _lib.load().igmc_cocount(C.byref(count_graph.c), _dev(mp).data_ptr(), Nu, table.data_ptr(), case["cap"],
+    table = support.filled(need, S32)
+    code = _lib.load().igmc_cocount(C.byref(count_graph.c), _alive(mp).data_ptr(), Nu, table.data_ptr(), case["cap"],
                                     None)
     torch.cuda.synchronize()
     got = table.cpu().numpy()
@@ -260,7 +253,7 @@ def test_huge_table():
     ni = gc.HUGE_NU
     rp, ci = gc.csr([np.asarray(r) for r in gc.HUGE_ROWS])
     g = _Graph(rp, ci, len(gc.HUGE_ROWS), ni, cols=True)
-    mp = _dev(np.arange(ni))
+    mp = _alive(np.arange(ni))
     table = torch.full((need + GUARD,), S32, dtype=torch.int32, device="cuda")
     try:
         assert _lib.load().igmc_cocount(C.byref(g.c), mp.data_ptr(), ni, table.data_ptr(), need, None) == 0
@@ -269,9 +262,9 @@ def test_huge_table():
         assert table[idx].cpu().tolist() == [nz[i] for i in sorted(nz)]
         assert int(table[:need].sum(dtype=torch.int64)) == sum(nz.values())    # nothing else counted
         assert (table[need:].cpu().numpy() == S32).all()
-        items = _dev(gc.HUGE_ITEMS, torch.int64)
+        items = _alive(gc.HUGE_ITEMS, torch.int64)
         Q = len(gc.HUGE_ITEMS)
-        out, err = _full(Q * Q, SF, torch.float32), _err()
+        out, err = support.filled(Q * Q, SF, torch.float32), _err()
         assert _lib.load().igmc_item_cosine(C.byref(g.c), items.data_ptr(), Q, mp.data_ptr(), ni, table.data_ptr(),
                                             out.data_ptr(), err.data_ptr(), None) == 0
         torch.cuda.synchronize()
@@ -281,9 +274,10 @@ def test_huge_table():
         # the greedy selection reads the same entries: pool = the items, scores equal, penalty 1
         pool = np.array([gc.HUGE_ITEMS[:6]], np.int64)
         sc = np.ones((1, 6), np.float32)
-        oi, os_, ok = _full(6, S32, torch.int64), _full(6, SF, torch.float32), _full(6, SF, torch.float32)
-        assert _lib.load().igmc_diverse_select(C.byref(g.c), _dev(pool, torch.int64).data_ptr(),
-                                               _dev(sc, torch.float32).data_ptr(), 1, 6, 6, 1.0, mp.data_ptr(), ni,
+        oi, os_, ok = support.filled(6, S32, torch.int64), support.filled(6, SF, torch.float32), \
+            support.filled(6, SF, torch.float32)
+        assert _lib.load().igmc_diverse_select(C.byref(g.c), _alive(pool, torch.int64).data_ptr(),
+                                               _alive(sc, torch.float32).data_ptr(), 1, 6, 6, 1.0, mp.data_ptr(), ni,
                                                table.data_ptr(), oi.data_ptr(), os_.data_ptr(), ok.data_ptr(),
                                                err.data_ptr(), None) == 0
         torch.cuda.synchronize()
@@ -324,20 +318,21 @@ def _device_union(g, items, ni, nu_users):
     """map, list and table of the union of items built by the kernels under test (checked above)"""
     code, err, _, mp, lst, nu = _union(np.asarray(items, np.int64).reshape(-1), ni)
     Nu = int(nu[0])
-    table = _full(Nu * (Nu - 1) // 2, S32)
+    table = support.filled(Nu * (Nu - 1) // 2, S32)
     assert _lib.load().igmc_cocount(C.byref(g.c), mp.data_ptr(), Nu, table.data_ptr(), Nu * (Nu - 1) // 2, None) == 0
     return mp, Nu, table
 
 
-@pytest.mark.parametrize("case", _of("select"), ids=_id)
+@pytest.mark.parametrize("case", _of("select"), ids=support.pid)
 def test_diverse_select(case, select_graph):
     pi, ps, k = case["pool_item"], case["pool_score"], case["k"]
     Q, P = pi.shape
     mp, Nu, table = _device_union(select_graph, pi, gc.SEL_NI, gc.SEL_NU)
-    oi, os_, ok, err = _full(Q * k, S32, torch.int64), _full(Q * k, SF, torch.float32), _full(Q * k, SF,
-                                                                                              torch.float32), _err()
-    code = _lib.load().igmc_diverse_select(C.byref(select_graph.c), _dev(pi, torch.int64).data_ptr(),
-                                           _dev(ps, torch.float32).data_ptr(), Q, P, k, case["penalty"],
+    oi, os_, ok = support.filled(Q * k, S32, torch.int64), support.filled(Q * k, SF, torch.float32), \
+        support.filled(Q * k, SF, torch.float32)
+    err = _err()
+    code = _lib.load().igmc_diverse_select(C.byref(select_graph.c), _alive(pi, torch.int64).data_ptr(),
+                                           _alive(ps, torch.float32).data_ptr(), Q, P, k, case["penalty"],
                                            mp.data_ptr(), Nu, table.data_ptr(), oi.data_ptr(), os_.data_ptr(),
                                            ok.data_ptr(), err.data_ptr(), None)
     torch.cuda.synchronize()
@@ -362,14 +357,14 @@ def test_diverse_select_argument_checks(select_graph):
                                    None, None) == 0
 
 
-@pytest.mark.parametrize("case", _of("cosine"), ids=_id)
+@pytest.mark.parametrize("case", _of("cosine"), ids=support.pid)
 def test_item_cosine(case, select_graph):
     items = case["items"]
     Q = len(items)
     mp, Nu, table = _device_union(select_graph, items, gc.SEL_NI, gc.SEL_NU)
-    out, err = _full(Q * Q, SF, torch.float32), _err()
-    assert _lib.load().igmc_item_cosine(C.byref(select_graph.c), _dev(items, torch.int64).data_ptr(), Q, mp.data_ptr(),
-                                        Nu, table.data_ptr(), out.data_ptr(), err.data_ptr(), None) == 0
+    out, err = support.filled(Q * Q, SF, torch.float32), _err()
+    assert _lib.load().igmc_item_cosine(C.byref(select_graph.c), _alive(items, torch.int64).data_ptr(), Q,
+                                        mp.data_ptr(), Nu, table.data_ptr(), out.data_ptr(), err.data_ptr(), None) == 0
     torch.cuda.synchronize()
     got = out.cpu().numpy()
     assert int(err.item()) == 0
@@ -381,9 +376,9 @@ def test_item_cosine_flags_ids_outside_the_union(select_graph):
     a, b, c = np.unique(ci)[:3].tolist()
     mp, Nu, table = _device_union(select_graph, [a, c], gc.SEL_NI, gc.SEL_NU)
     items = np.array([a, b, gc.SEL_NI, -1, c], np.int64)                   # b: not in the union
-    out, err = _full(25, SF, torch.float32), _err()
+    out, err = support.filled(25, SF, torch.float32), _err()
     lib = _lib.load()
-    assert lib.igmc_item_cosine(C.byref(select_graph.c), _dev(items, torch.int64).data_ptr(), 5, mp.data_ptr(), Nu,
+    assert lib.igmc_item_cosine(C.byref(select_graph.c), _alive(items, torch.int64).data_ptr(), 5, mp.data_ptr(), Nu,
                                 table.data_ptr(), out.data_ptr(), err.data_ptr(), None) == 0
     torch.cuda.synchronize()
     got = out.cpu().numpy()[:25].reshape(5, 5)
@@ -394,7 +389,7 @@ def test_item_cosine_flags_ids_outside_the_union(select_graph):
     assert lib.igmc_item_cosine(C.byref(select_graph.c), p, 3, p, 3, None, p, p, None) == -1
 
 
-@pytest.mark.parametrize("case", _of("ws_bytes"), ids=_id)
+@pytest.mark.parametrize("case", _of("ws_bytes"), ids=support.pid)
 def test_diverse_ws_bytes(case):
     nbytes, chunk = C.c_int64(-1), C.c_int(-1)
     assert _lib.load().igmc_diverse_ws_bytes(*case["args"], C.byref(nbytes), C.byref(chunk)) == 0
@@ -409,13 +404,12 @@ def test_diverse_ws_bytes(case):
 def _rescore(case, g, chunk, out_cap):
     U, ni = len(case["users"]), case["num_items"]
     ws = torch.empty(gc.plan_ws_bytes(ni, chunk), dtype=torch.uint8, device="cuda")
-    user_off, out = _full(U + 1, S32, torch.int64), _full(max(out_cap, 0), S32)
-    full, totals, err = _full(U, S8, torch.uint8), torch.full((2 + GUARD,), S32, dtype=torch.int64, device="cuda"), \
-        _err()
+    user_off, out = support.filled(U + 1, S32, torch.int64), support.filled(max(out_cap, 0), S32)
+    full, totals, err = support.filled(U, S8, torch.uint8), support.filled(2, S32, torch.int64), _err()
     cand = case["cand"]
-    cd = None if cand is None else _dev(cand)
-    eu, ev = _dev(case["edit_u"]), _dev(case["edit_v"])
-    code = _lib.load().igmc_rescore_plan(C.byref(g.c), _dev(case["users"]).data_ptr(), U, eu.data_ptr(),
+    cd = None if cand is None else _alive(cand)
+    eu, ev = _alive(case["edit_u"]), _alive(case["edit_v"])
+    code = _lib.load().igmc_rescore_plan(C.byref(g.c), _alive(case["users"]).data_ptr(), U, eu.data_ptr(),
                                          ev.data_ptr(), len(case["edit_u"]), _lib.ptr(cd),
                                          0 if cand is None else len(cand), case["exclude"], ws.data_ptr(), ws.numel(),
                                          user_off.data_ptr(), out.data_ptr(), out_cap, full.data_ptr(),
@@ -424,7 +418,7 @@ def _rescore(case, g, chunk, out_cap):
     return code, int(err.item()), [t.cpu().numpy() for t in (user_off, out, full, totals)]
 
 
-@pytest.mark.parametrize("case", _of("rescore"), ids=_id)
+@pytest.mark.parametrize("case", _of("rescore"), ids=support.pid)
 def test_rescore_plan_every_chunk_size(case):
     rp, ci = gc.cache_graph(case["num_items"])
     g = _Graph(rp, ci, gc.CACHE_NU, case["num_items"])
@@ -462,15 +456,16 @@ def test_rescore_plan_argument_checks():
     torch.cuda.synchronize()
 
 
-@pytest.mark.parametrize("case", _of("invalidate"), ids=_id)
+@pytest.mark.parametrize("case", _of("invalidate"), ids=support.pid)
 def test_cache_invalidate(case):
     U, D = case["top_i"].shape
-    ts, ti = _dev(np.r_[case["top_s"].reshape(-1), [SF] * GUARD], torch.float32), \
-        _dev(np.r_[case["top_i"].reshape(-1), [S32] * GUARD], torch.int64)
-    thr_s, thr_i = _full(U, SF, torch.float32), _full(U, S32, torch.int64)
-    assert _lib.load().igmc_cache_invalidate(U, D, _dev(case["user_off"], torch.int64).data_ptr(),
-                                             _dev(case["resc"]).data_ptr(), _dev(case["full"], torch.uint8).data_ptr(),
-                                             _dev(case["complete"], torch.uint8).data_ptr(), ts.data_ptr(),
+    ts, ti = _alive(np.r_[case["top_s"].reshape(-1), [SF] * GUARD], torch.float32), \
+        _alive(np.r_[case["top_i"].reshape(-1), [S32] * GUARD], torch.int64)
+    thr_s, thr_i = support.filled(U, SF, torch.float32), support.filled(U, S32, torch.int64)
+    assert _lib.load().igmc_cache_invalidate(U, D, _alive(case["user_off"], torch.int64).data_ptr(),
+                                             _alive(case["resc"]).data_ptr(),
+                                             _alive(case["full"], torch.uint8).data_ptr(),
+                                             _alive(case["complete"], torch.uint8).data_ptr(), ts.data_ptr(),
                                              ti.data_ptr(), thr_s.data_ptr(), thr_i.data_ptr(), None) == 0
     torch.cuda.synchronize()
     ws, wi, wts, wti = gc.invalidate_reference(case)
@@ -481,14 +476,14 @@ def test_cache_invalidate(case):
         assert (got[n:] == sent).all()
 
 
-@pytest.mark.parametrize("case", _of("settle"), ids=_id)
+@pytest.mark.parametrize("case", _of("settle"), ids=support.pid)
 def test_cache_settle(case):
     U, D = case["top_i"].shape
-    ts, ti = _dev(np.r_[case["top_s"].reshape(-1), [SF] * GUARD], torch.float32), \
-        _dev(np.r_[case["top_i"].reshape(-1), [S32] * GUARD], torch.int64)
-    complete, redo, cnt = _full(U, S8, torch.uint8), _full(U, S32), _full(1, S32)
-    assert _lib.load().igmc_cache_settle(U, D, case["k"], _dev(case["thr_s"], torch.float32).data_ptr(),
-                                         _dev(case["thr_i"], torch.int64).data_ptr(), ts.data_ptr(), ti.data_ptr(),
+    ts, ti = _alive(np.r_[case["top_s"].reshape(-1), [SF] * GUARD], torch.float32), \
+        _alive(np.r_[case["top_i"].reshape(-1), [S32] * GUARD], torch.int64)
+    complete, redo, cnt = support.filled(U, S8, torch.uint8), support.filled(U, S32), support.filled(1, S32)
+    assert _lib.load().igmc_cache_settle(U, D, case["k"], _alive(case["thr_s"], torch.float32).data_ptr(),
+                                         _alive(case["thr_i"], torch.int64).data_ptr(), ts.data_ptr(), ti.data_ptr(),
                                          complete.data_ptr(), redo.data_ptr(), cnt.data_ptr(), None) == 0
     torch.cuda.synchronize()
     ws, wi, wc, wr = gc.settle_reference(case)

@@ -10,8 +10,6 @@ start_group_pairs; csrc/groups.cu).
 * results do not depend on the other groups or on graph replay, two runs are bit-identical, steps make no host sync,
   and a graph.update between runs is served while one during a run raises."""
 import ctypes as C
-import functools
-import os
 import tempfile
 
 import numpy as np
@@ -20,55 +18,13 @@ import torch
 
 from igmc_b200 import _lib
 from igmc_b200 import recommend as rc
-from igmc_b200.data import build_adj, make_synthetic_dataset, synth_ratings
 from igmc_b200.util_functions import RatingGraph, _stream_ptr
+from tests import support
 
 pytestmark = pytest.mark.gpu
 
 SENT32, SENTF = -77, -7.5
 GUARD = 16
-
-
-@functools.lru_cache(maxsize=None)
-def _ds(name):
-    if name == "r13":
-        u, v, lab = synth_ratings(400, 300, 9000, 13, seed=4)
-        return build_adj(u, v, lab, 400, 300)
-    return make_synthetic_dataset(name, seed=0)["adj_train"]
-
-
-def _model(R, rgcn="pyg-1.4", dgcnn=False, seed=0):
-    from igmc_b200.models import DGCNN_RS, IGMC
-    torch.manual_seed(seed)
-    if dgcnn:
-        m = DGCNN_RS(4, latent_dim=[32, 32, 32, 1], k=30, num_relations=R, num_bases=4, regression=True, rgcn=rgcn)
-    else:
-        m = IGMC(4, latent_dim=[32] * 4, num_relations=R, num_bases=4, regression=True, rgcn=rgcn)
-    return m.cuda()
-
-
-def _checkpoints(m, K, d):
-    paths = []
-    own = {k: v.clone() for k, v in m.state_dict().items()}
-    for k in range(K):
-        torch.manual_seed(100 + k)
-        with torch.no_grad():
-            m.flat_params.add_(torch.randn_like(m.flat_params) * 0.05)
-        paths.append(os.path.join(d, "ck%d.pt" % k))
-        torch.save(m.state_dict(), paths[-1])
-    m.load_state_dict(own)
-    return paths
-
-
-def _dev(a, dtype=torch.int32):
-    return torch.as_tensor(np.asarray(a)).to(dtype).cuda()
-
-
-def _same(a, b):
-    a, b = np.asarray(a, np.float32), np.asarray(b, np.float32)
-    n = np.isnan(a)
-    return a.shape == b.shape and np.array_equal(n, np.isnan(b)) and np.array_equal(a[~n].view(np.uint32),
-                                                                                   b[~n].view(np.uint32))
 
 
 def _groups(g, seed, sizes=(1, 2, 3, 5)):
@@ -87,7 +43,7 @@ def _toy_csr():
     rows = [[1, 4, 7], [], [0, 4, 9, 11], [2, 7], [4], [1, 3, 5, 7, 9, 11], list(range(0, 300, 2))]
     rp = np.concatenate([[0], np.cumsum([len(r) for r in rows])]).astype(np.int32)
     ci = np.concatenate([np.asarray(r, np.int64) for r in rows]).astype(np.int32)
-    keep = [_dev(rp), _dev(ci)]
+    keep = [support.dev(rp), support.dev(ci)]
     G = _lib.CSR(keep[0].data_ptr(), keep[1].data_ptr(), None, None, None, len(rows), 300)
     return G, keep, rp, ci
 
@@ -98,7 +54,7 @@ def _group_rows(G, members, cap):
     col = torch.full((max(cap, 1) + GUARD,), SENT32, dtype=torch.int32, device="cuda")
     ws = torch.empty(2 * Gn + 1 + cap, dtype=torch.int32, device="cuda")
     err = torch.zeros(1, dtype=torch.int32, device="cuda")
-    dm = _dev(members)
+    dm = support.dev(members)
     code = _lib.load().igmc_group_rows(C.byref(G), dm.data_ptr(), Gn, M, row_ptr.data_ptr(), col.data_ptr(), cap,
                                        ws.data_ptr(), err.data_ptr(), _stream_ptr())
     torch.cuda.synchronize()
@@ -154,7 +110,7 @@ def test_group_pairs_kernel_matches_twin(B):
            for k, dt in (("u", torch.int32), ("v", torch.int32), ("pid", torch.int64), ("tag", torch.int64))}
     err = torch.zeros(1, dtype=torch.int32, device="cuda")
     lib = _lib.load()
-    keep = [_dev(members), _dev(ug), _dev(uv), _dev(ut, torch.int64)]
+    keep = [support.dev(members), support.dev(ug), support.dev(uv), support.dev(ut, torch.int64)]
     assert lib.igmc_group_pairs(keep[0].data_ptr(), 3, 3, nu, ni, keep[1].data_ptr(), keep[2].data_ptr(),
                                 keep[3].data_ptr(), B, out["u"].data_ptr(), out["v"].data_ptr(),
                                 out["pid"].data_ptr(), out["tag"].data_ptr(), err.data_ptr(), None) == 0
@@ -168,7 +124,8 @@ def test_group_pairs_kernel_matches_twin(B):
                 dict(members=np.array([[5, 6, -1], [0, -1, -1], [3, 1, 4]] * 1, np.int32))):
         args = dict(members=members, ug=ug, uv=uv)
         args.update(bad)
-        keep = [_dev(args["members"]), _dev(args["ug"]), _dev(args["uv"]), _dev(ut, torch.int64)]
+        keep = [support.dev(args["members"]), support.dev(args["ug"]), support.dev(args["uv"]),
+                support.dev(ut, torch.int64)]
         err.zero_()
         assert lib.igmc_group_pairs(keep[0].data_ptr(), 3, 3, nu, ni, keep[1].data_ptr(), keep[2].data_ptr(),
                                     keep[3].data_ptr(), B, out["u"].data_ptr(), out["v"].data_ptr(),
@@ -203,19 +160,19 @@ def test_group_stats_kernel_matches_twin(agg, form):
     ds = torch.full((T + GUARD,), SENTF, device="cuda")
     dm = torch.full((T * M + GUARD,), SENTF, device="cuda")
     outs = (dk.data_ptr(), None, None) if form == "key" else (None, ds.data_ptr(), dm.data_ptr())
-    assert _lib.load().igmc_group_stats(_dev(preds, torch.float32).data_ptr(), K, B, M,
-                                        _lib.GROUP_AGGREGATES.index(agg), _dev(tag, torch.int64).data_ptr(), *outs,
-                                        None) == 0
+    assert _lib.load().igmc_group_stats(support.dev(preds, torch.float32).data_ptr(), K, B, M,
+                                        _lib.GROUP_AGGREGATES.index(agg), support.dev(tag, torch.int64).data_ptr(),
+                                        *outs, None) == 0
     torch.cuda.synchronize()
     if form == "key":
         got = dk.cpu().numpy()
-        assert _same(got[:Gu], key) and (got[Gu:] == SENTF).all()
+        assert support.same(got[:Gu], key) and (got[Gu:] == SENTF).all()
     else:
         want_s, want_m = np.full(T, SENTF, np.float32), np.full((T, M), SENTF, np.float32)
         for g in np.flatnonzero(utag >= 0):
             want_s[utag[g]], want_m[utag[g]] = key[g], xs[g]
         got_s, got_m = ds.cpu().numpy(), dm.cpu().numpy()
-        assert _same(got_s[:T], want_s) and _same(got_m[:T * M], want_m.reshape(-1))
+        assert support.same(got_s[:T], want_s) and support.same(got_m[:T * M], want_m.reshape(-1))
         assert (got_s[T:] == SENTF).all() and (got_m[T * M:] == SENTF).all()
     p = dk.data_ptr()
     lib = _lib.load()
@@ -225,8 +182,8 @@ def test_group_stats_kernel_matches_twin(agg, form):
 
 
 def test_engine_raises_on_bad_device_ids():
-    g = RatingGraph(_ds("ml_100k"))
-    m = _model(5)
+    g = RatingGraph(support.adj("ml_100k"))
+    m = support.model(5)
     eng = rc.InferenceEngine(m, g, max_nodes_per_hop=50, batch_size=64)
     try:
         eng.start_group_pairs([[1, 2], [3]], [0, 1, 1], [4, 5, 6])
@@ -264,13 +221,13 @@ def _table_scorer(eng, members, ni):
 @pytest.mark.parametrize("name", list(CASES))
 def test_lists_equal_host_composition(name):
     dsn, mnph, kw, plan, K = CASES[name]
-    A = _ds(dsn)
+    A = support.adj(dsn)
     g = RatingGraph(A)
-    m = _model(13 if dsn == "r13" else 5, **kw)
+    m = support.model(13 if dsn == "r13" else 5, **kw)
     m.kernel_plan = plan
     try:
         with tempfile.TemporaryDirectory() as d:
-            ck = _checkpoints(m, K, d) if K else None
+            ck = support.checkpoints(m, K, d) if K else None
             eng = rc.InferenceEngine(m, g, max_nodes_per_hop=mnph, batch_size=64, checkpoints=ck, sample_seed=3)
             try:
                 ni = g.num_items
@@ -290,14 +247,15 @@ def test_lists_equal_host_composition(name):
                     wi, ws = rc.recommend_groups_host(hp["row_ptr"], hp["col_idx"], ni, members, 10, agg, scorer,
                                                       items, excl)
                     assert np.array_equal(ti.cpu().numpy(), wi), (items is None, excl, agg)
-                    assert _same(ts.cpu().numpy(), ws)
+                    assert support.same(ts.cpu().numpy(), ws)
                     q = np.repeat(np.arange(len(groups)), 10)
                     top = ti.cpu().numpy().reshape(-1)
                     ok = top >= 0
                     got = eng.predict_groups(groups, q[ok], top[ok], agg)
                     want_s, want_m = rc.predict_groups_host(members, q[ok], top[ok], agg, scorer)
-                    assert _same(got.score.cpu().numpy(), want_s) and _same(got.members.cpu().numpy(), want_m)
-                    assert _same(got.score.cpu().numpy(), ts.cpu().numpy().reshape(-1)[ok])
+                    assert support.same(got.score.cpu().numpy(), want_s)
+                    assert support.same(got.members.cpu().numpy(), want_m)
+                    assert support.same(got.score.cpu().numpy(), ts.cpu().numpy().reshape(-1)[ok])
             finally:
                 eng.close()
     finally:
@@ -306,8 +264,8 @@ def test_lists_equal_host_composition(name):
 
 # ---- 3. edge cases ------------------------------------------------------------------------------------------------------
 def test_group_of_one_rated_everything_and_short_lists():
-    g = RatingGraph(_ds("ml_100k"))
-    m = _model(5)
+    g = RatingGraph(support.adj("ml_100k"))
+    m = support.model(5)
     opts = dict(max_nodes_per_hop=100, batch_size=64)
     users = [3, 17, 250]
     want_i, want_s = rc.recommend(m, g, users, 10, **opts)
@@ -353,23 +311,23 @@ def _run(m, g, groups, k, agg, B=64, use_graph=True, sync_check=False):
 
 
 def test_independent_of_other_groups_and_replay_and_sync_free():
-    g = RatingGraph(_ds("ml_1m"))
-    m = _model(5)
+    g = RatingGraph(support.adj("ml_1m"))
+    m = support.model(5)
     groups = _groups(g, 5)
     for agg in ("mean", "min"):
         base = _run(m, g, groups, 10, agg)
         for got in (_run(m, g, groups, 10, agg), _run(m, g, groups, 10, agg, use_graph=False),
                     _run(m, g, groups, 10, agg, sync_check=True)):
-            assert np.array_equal(got[0], base[0]) and _same(got[1], base[1])
+            assert np.array_equal(got[0], base[0]) and support.same(got[1], base[1])
         more = _groups(g, 9, sizes=(4, 2)) + groups + [[7]]                   # other groups around them, M = 5 still
         got = _run(m, g, more, 10, agg)
-        assert np.array_equal(got[0][2:-1], base[0]) and _same(got[1][2:-1], base[1])
+        assert np.array_equal(got[0][2:-1], base[0]) and support.same(got[1][2:-1], base[1])
 
 
 def test_served_across_updates():
-    A = _ds("ml_100k")
+    A = support.adj("ml_100k")
     g = RatingGraph(A, reserve_nnz=50)
-    m = _model(5)
+    m = support.model(5)
     groups = [[1, 2, 3], [40, 41]]
     eng = rc.InferenceEngine(m, g, max_nodes_per_hop=100, batch_size=64)
     try:
@@ -381,7 +339,7 @@ def test_served_across_updates():
         scorer = _table_scorer(eng, members, g.num_items)
         hp = g.host
         wi, ws = rc.recommend_groups_host(hp["row_ptr"], hp["col_idx"], g.num_items, members, 5, "min", scorer)
-        assert np.array_equal(ti.cpu().numpy(), wi) and _same(ts.cpu().numpy(), ws)
+        assert np.array_equal(ti.cpu().numpy(), wi) and support.same(ts.cpu().numpy(), ws)
         assert int(free[0]) not in ti.cpu().numpy()[0]                         # newly rated by a member: excluded
         eng.start_recommend_groups(groups, 5)
         g.update([2], [int(free[1])], [3])
@@ -390,6 +348,6 @@ def test_served_across_updates():
                 pass
         got = eng.predict_groups(groups, [0], [int(free[1])])
         want = rc.predict_groups(m, g, groups, [0], [int(free[1])], max_nodes_per_hop=100, batch_size=64)
-        assert _same(got.score.cpu().numpy(), want.score.cpu().numpy())
+        assert support.same(got.score.cpu().numpy(), want.score.cpu().numpy())
     finally:
         eng.close()

@@ -23,8 +23,9 @@ from igmc_b200.util_functions import RatingGraph, SubgraphExtractor
 from oracle import extract_np
 from tests import error_bounds as eb
 from tests import pyg2_oracle
+from tests import support
 from tests.helpers import batch_equal
-from tests.test_gpu_explain import _ds, _model, _pairs, _r13, _subgraph, _with_cold_start
+from tests.test_gpu_explain import _pairs, _subgraph, _with_cold_start
 
 pytestmark = pytest.mark.gpu
 
@@ -78,7 +79,7 @@ CASES = {
 @pytest.mark.parametrize("name", list(CASES))
 def test_pair_gradients_match_fp64_autograd(name):
     dsn, R, h, mnph, NB, rgcn, mb, plan, B = CASES[name]
-    A = _with_cold_start(_r13() if dsn == "r13" else _ds(dsn)["adj_train"])
+    A = _with_cold_start(support.adj(dsn))
     m = _mk(R, h, rgcn, NB, mb, plan)
     u, v = _pairs(A)
     y = np.array([3.0, 1.0, 5.0])
@@ -107,10 +108,10 @@ def _train_batch(A, R, u, v, lab, mnph, seed, B):
 
 @pytest.mark.parametrize("plan", [1, 2, 4, 0, _lib.plan_l2(2)])
 def test_pair_gradients_sum_to_the_train_step(plan):
-    A = _ds("ml_1m")["adj_train"]
+    A = support.adj("ml_1m")
     R = 13 if plan == 0 else 5
     if plan == 0:
-        A = _r13()
+        A = support.adj("r13")
     m = _mk(R, plan=plan)
     m.adj_dropout, m.hidden_dropout_p = 0.0, 0.0
     coo = A.tocoo()
@@ -143,7 +144,7 @@ def test_pair_gradients_sum_to_the_train_step(plan):
 
 
 def _setup(R=5, plan="auto", N=200, T=12, seed=0):
-    A = _ds("ml_1m")["adj_train"]
+    A = support.adj("ml_1m")
     m = _mk(R, plan=plan, seed=seed)
     coo = A.tocoo()
     rng = np.random.default_rng(3)
@@ -287,6 +288,6 @@ def test_steady_state_steps_do_not_sync_and_updates_raise():
             eng.step()
     finally:
         eng.close()
-    d = _model(5, dgcnn=True)
+    d = support.model(5, dgcnn=True)
     with pytest.raises(NotImplementedError):
         rc.pair_gradients(d, A, train[0][:2], train[1][:2])

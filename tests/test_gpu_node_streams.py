@@ -17,6 +17,7 @@ import torch
 from igmc_b200 import _lib
 from igmc_b200.util_functions import _stream_ptr
 from tests import node_stream_cases as ns
+from tests import support
 
 pytestmark = pytest.mark.gpu
 
@@ -24,14 +25,6 @@ GUARD = 64
 S32 = -777
 FSENT = 0x7f80dead
 ERR_CANDIDATES = 7     # IGMC_ERR_CANDIDATES (csrc/common.cuh)
-
-
-def _dev(a, dtype):
-    return torch.from_numpy(np.ascontiguousarray(np.asarray(a).astype(dtype))).cuda()
-
-
-def _filled(n, value, dtype):
-    return torch.full((n + GUARD,), value, dtype=dtype, device="cuda")
 
 
 def _take_err(err):
@@ -45,10 +38,10 @@ def _batch_out(bt):
     ecap = E + 16
     ei = np.zeros((2, ecap), np.int64)
     ei[0, :E], ei[1, :E] = bt["src"], bt["dst"]
-    t = dict(node_ptr=_dev(bt["node_ptr"], np.int32), edge_ptr=_dev(bt["edge_ptr"], np.int32),
-             edge_index=_dev(ei.reshape(-1), np.int64), node_label=_dev(bt["node_label"], np.uint8),
-             node_gid=_dev(bt["node_gid"], np.int32), adj_in_ptr=_dev(bt["in_ptr"], np.int32),
-             adj_eid=_dev(np.concatenate([bt["in_eid"], [0]]), np.int32))
+    t = dict(node_ptr=support.dev_np(bt["node_ptr"], np.int32), edge_ptr=support.dev_np(bt["edge_ptr"], np.int32),
+             edge_index=support.dev_np(ei.reshape(-1), np.int64), node_label=support.dev_np(bt["node_label"], np.uint8),
+             node_gid=support.dev_np(bt["node_gid"], np.int32), adj_in_ptr=support.dev_np(bt["in_ptr"], np.int32),
+             adj_eid=support.dev_np(np.concatenate([bt["in_eid"], [0]]), np.int32))
     O = _lib.BatchOut()
     O.edge_cap = ecap
     for k, v in t.items():
@@ -68,8 +61,8 @@ def test_node_count(name, err):
     B = len(shapes)
     tag = np.arange(B)[::-1] * 2            # pair 2 * (B - 1 - g); the odd pairs are untouched
     tag[0] = -1
-    out = _filled(2 * B, S32, torch.int32)
-    node_ptr, tag_d = _dev(bt["node_ptr"], np.int32), _dev(tag, np.int64)     # alive until the kernel has run
+    out = support.filled(2 * B, S32, torch.int32, GUARD)
+    node_ptr, tag_d = support.dev_np(bt["node_ptr"], np.int32), support.dev_np(tag, np.int64)  # alive until it has run
     _lib.check(_lib.load().igmc_explain_node_count(node_ptr.data_ptr(), tag_d.data_ptr(), B, out.data_ptr(),
                                                    _stream_ptr()),
                "igmc_explain_node_count")
@@ -96,9 +89,9 @@ def test_node_occlusion_mask(name, where, err):
     if B > 1:
         tag[1] = -1                            # a padding graph: nothing dropped, nothing recorded
     T = 3 * B + 1
-    keep = _filled(E, 7, torch.uint8)
-    rec = [_filled(T, S32, torch.int32) for _ in range(3)]
-    tag_d, j_d = _dev(tag, np.int64), _dev(j, np.int32)
+    keep = support.filled(E, 7, torch.uint8, GUARD)
+    rec = [support.filled(T, S32, torch.int32, GUARD) for _ in range(3)]
+    tag_d, j_d = support.dev_np(tag, np.int64), support.dev_np(j, np.int32)
     _lib.check(lib.igmc_node_occlusion_mask(C.byref(O), B, tag_d.data_ptr(), j_d.data_ptr(), keep.data_ptr(),
                                             rec[0].data_ptr(), rec[1].data_ptr(), rec[2].data_ptr(), err.data_ptr(),
                                             _stream_ptr()), "igmc_node_occlusion_mask")
@@ -147,14 +140,14 @@ def test_node_grad_scatter(name, K, err):
     grads = [rng.standard_normal(E + 1).astype(np.float32) for _ in range(K)]
     if E:
         grads[0][rng.integers(0, E, 3)] = [np.inf, -0.0, 1e30]
-    out = _filled(T, 0.0, torch.float32)
+    out = support.filled(T, 0.0, torch.float32, GUARD)
     out.view(torch.int32).fill_(FSENT)
-    rec = [_filled(T, S32, torch.int32) for _ in range(3)]
+    rec = [support.filled(T, S32, torch.int32, GUARD) for _ in range(3)]
     want = np.full(T, FSENT, np.int32).view(np.float32)
     want_rec = np.full((3, T), S32)
-    tag_d, off_d = _dev(tag, np.int64), _dev(off, np.int64)
+    tag_d, off_d = support.dev_np(tag, np.int64), support.dev_np(off, np.int64)
     for k in range(K):
-        g_dev = _dev(grads[k], np.float32)
+        g_dev = support.dev_np(grads[k], np.float32)
         _lib.check(lib.igmc_node_grad_scatter(C.byref(O), B, tag_d.data_ptr(), g_dev.data_ptr(), off_d.data_ptr(), k,
                                               K, out.data_ptr(), rec[0].data_ptr(), rec[1].data_ptr(),
                                               rec[2].data_ptr(), err.data_ptr(), _stream_ptr()),
@@ -190,11 +183,11 @@ def test_node_grad_scatter_rejects_a_foreign_count(err):
     npos[0] += 1                                   # the base pass counted another subgraph for pair 0
     off = np.concatenate([[0], np.cumsum(npos)]).astype(np.int64)
     T = int(off[-1])
-    out = _filled(T, 0.0, torch.float32)
+    out = support.filled(T, 0.0, torch.float32, GUARD)
     out.view(torch.int32).fill_(FSENT)
-    rec = [_filled(T, S32, torch.int32) for _ in range(3)]
-    g = _dev(np.ones(int(bt["edge_ptr"][-1]) + 1), np.float32)
-    tag_d, off_d = _dev(np.arange(B), np.int64), _dev(off, np.int64)
+    rec = [support.filled(T, S32, torch.int32, GUARD) for _ in range(3)]
+    g = support.dev_np(np.ones(int(bt["edge_ptr"][-1]) + 1), np.float32)
+    tag_d, off_d = support.dev_np(np.arange(B), np.int64), support.dev_np(off, np.int64)
     _lib.check(_lib.load().igmc_node_grad_scatter(C.byref(O), B, tag_d.data_ptr(), g.data_ptr(), off_d.data_ptr(), 0,
                                                   1, out.data_ptr(),
                                                   rec[0].data_ptr(), rec[1].data_ptr(), rec[2].data_ptr(),

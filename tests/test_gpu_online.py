@@ -19,17 +19,13 @@ import torch
 from igmc_b200 import _lib
 from igmc_b200 import recommend as rc
 from igmc_b200 import train_eval as te
-from igmc_b200.data import build_adj, make_synthetic_dataset, synth_ratings
-from igmc_b200.models import DGCNN_RS, IGMC, FusedAdam
+from igmc_b200.data import build_adj, synth_ratings
+from igmc_b200.models import IGMC, FusedAdam
 from igmc_b200.train_eval import OnlineTrainer, online_draw_host, recent_append_host, recent_threshold
 from igmc_b200.util_functions import RatingGraph, SubgraphExtractor, _stream_ptr
+from tests import support
 
 pytestmark = pytest.mark.gpu
-
-
-@functools.lru_cache(maxsize=None)
-def _ds(name):
-    return make_synthetic_dataset(name, seed=0)
 
 
 @functools.lru_cache(maxsize=None)
@@ -106,7 +102,7 @@ def _check_draw(g, ring, frac, count, ahead, B, err, ss=17, ds=0x1234ABCD):
 
 @pytest.mark.parametrize("name", ["ml_1m", "tiny"])
 def test_draw_matches_twin(name):
-    A = _ds(name)["adj_train"]
+    A = support.adj(name)
     g = RatingGraph(A, reserve_nnz=5000, reserve_users=4, reserve_items=3)
     err = torch.zeros(1, dtype=torch.int32, device="cuda")
     rng = np.random.default_rng(2)
@@ -139,15 +135,6 @@ def test_draw_matches_twin(name):
 
 
 # ---- 2. ten trainer steps against the per-step calls -----------------------------------------------------------------
-def _model(kind, R, rgcn="pyg-1.4", seed=0):
-    torch.manual_seed(seed)
-    if kind == "dgcnn":
-        return DGCNN_RS(4, latent_dim=[32, 32, 32, 1], k=30, num_relations=R, num_bases=4, regression=True,
-                        rgcn=rgcn).cuda()
-    return IGMC(4, latent_dim=[32] * 4, num_relations=R, num_bases=4, regression=True, adj_dropout=0.2,
-                rgcn=rgcn).cuda()
-
-
 def _manual_steps(m, opt, g, mnph, B, ARR, steps, ss, window, frac, cv):
     """the trainer's steps through the per-step calls: pairs from the twin at step counter + k"""
     ex = SubgraphExtractor(g, [0], [0], [0], cv, 1, 1.0, mnph, max_batch=B, seed=ss)
@@ -192,11 +179,11 @@ CASES = {"ml_1m rs": ("ml_1m", "igmc", 5, "pyg-1.4", 100, True),
 @pytest.mark.parametrize("case", list(CASES))
 def test_trainer_steps_match_per_step_calls(case):
     name, kind, R, rgcn, mnph, use_graph = CASES[case]
-    A = _ds("ml_1m")["adj_train"] if name == "ml_1m" else _small(13, 400, 300, 9000)
+    A = support.adj("ml_1m") if name == "ml_1m" else _small(13, 400, 300, 9000)
     B, ARR, steps, ss, frac = 50, 0.001, 10, 3, 0.5
     g = RatingGraph(A, reserve_nnz=100)
     cv = np.arange(1, R + 1, dtype=np.float32)
-    m, m2 = _model(kind, R, rgcn), _model(kind, R, rgcn)
+    m, m2 = (support.model(R, rgcn=rgcn, dgcnn=kind == "dgcnn", adj_dropout=0.2) for _ in range(2))
     opt, opt2 = FusedAdam(m, lr=1e-3), FusedAdam(m2, lr=1e-3)
     tr = OnlineTrainer(m, g, opt, batch_size=B, ARR=ARR, max_nodes_per_hop=mnph, recent_fraction=frac,
                        recent_capacity=256, sample_seed=ss, use_graph=use_graph)
@@ -219,7 +206,7 @@ def test_trainer_steps_match_per_step_calls(case):
 
 # ---- 3. following updates ---------------------------------------------------------------------------------------------
 def _copy(m, opt, kind="igmc", R=5):
-    m2 = _model(kind, R)
+    m2 = support.model(R, dgcnn=kind == "dgcnn", adj_dropout=0.2)
     m2.load_state_dict(m.state_dict())
     o2 = FusedAdam(m2, lr=opt.param_groups[0]["lr"])
     o2.load_state_dict(opt.state_dict())
@@ -238,7 +225,7 @@ def test_trainer_follows_a_chain_of_updates():
     A = _uniform()
     R, B, cap = 5, 50, 512
     g = RatingGraph(A, reserve_nnz=3000, reserve_users=10, reserve_items=10)
-    m = _model("igmc", R)
+    m = support.model(R, adj_dropout=0.2)
     opt = FusedAdam(m, lr=1e-3)
     kw = dict(batch_size=B, ARR=0.001, max_nodes_per_hop=None, recent_fraction=0.4, recent_capacity=cap, sample_seed=9)
     tr = OnlineTrainer(m, g, opt, **kw)
@@ -285,12 +272,12 @@ def test_train_calls_continue_the_pipeline():
     between (its staged images share the model's cache) leaves the next call training on its own batch."""
     from igmc_b200.train_eval import TrainEngine
     from igmc_b200.util_functions import MyDynamicDataset
-    ds = _ds("ml_1m")
+    ds = support.dataset("ml_1m")
     A = ds["adj_train"]
     tu, tv, tl = ds["train"]
     out = []
     for split in (True, False):
-        m = _model("igmc", 5)
+        m = support.model(5, adj_dropout=0.2)
         opt = FusedAdam(m, lr=1e-3)
         tr = OnlineTrainer(m, RatingGraph(A), opt, batch_size=50, max_nodes_per_hop=100)
         losses = [tr.train(3), tr.train(7)] if split else [tr.train(10)]
@@ -313,9 +300,9 @@ def test_train_calls_continue_the_pipeline():
 
 # ---- 4. serving --------------------------------------------------------------------------------------------------------
 def test_engine_built_before_fine_tuning_serves_the_new_weights():
-    A = _ds("ml_1m")["adj_train"]
+    A = support.adj("ml_1m")
     g = RatingGraph(A, reserve_nnz=1000)
-    m = _model("igmc", 5)
+    m = support.model(5, adj_dropout=0.2)
     opt = FusedAdam(m, lr=1e-3)
     eng = rc.InferenceEngine(m, g, max_nodes_per_hop=100, batch_size=50, sample_seed=2)
     users = np.array([0, 5, 77])
@@ -343,7 +330,7 @@ def _rmse(m, g, u, v, lab):
 
 def test_fine_tuning_on_new_ratings_lowers_their_error():
     from igmc_b200.util_functions import MyDynamicDataset
-    ds = _ds("ml_1m")
+    ds = support.dataset("ml_1m")
     A = ds["adj_train"].tocoo()
     rng = np.random.default_rng(0)
     users = rng.choice(ds["num_users"], 200, replace=False)
@@ -376,9 +363,9 @@ def test_fine_tuning_on_new_ratings_lowers_their_error():
 
 # ---- 6. argument checks ------------------------------------------------------------------------------------------------
 def test_argument_checks(monkeypatch):
-    A = _ds("tiny")["adj_train"]
+    A = support.adj("tiny")
     g = RatingGraph(A, reserve_nnz=10)
-    m = _model("igmc", 5)
+    m = support.model(5, adj_dropout=0.2)
     opt = FusedAdam(m)
     bad = [dict(recent_fraction=-0.1), dict(recent_fraction=1.5), dict(batch_size=0), dict(h=2),
            dict(recent_capacity=0)]

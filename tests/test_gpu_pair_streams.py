@@ -23,6 +23,7 @@ from igmc_b200.data import make_synthetic_dataset
 from igmc_b200.util_functions import _stream_ptr
 from oracle import extract_np
 from tests import pair_stream_cases as ps
+from tests import support
 from tests.ranking_cases import same_f32
 
 pytestmark = pytest.mark.gpu
@@ -32,25 +33,8 @@ GUARD = 64
 S32, S64 = -777, -(2 ** 40) - 7      # integer sentinels: no kernel writes either
 
 
-def _id(c):
-    return c["name"]
-
-
 def _of(kernel):
     return [c for c in CASES if c["kernel"] == kernel]
-
-
-def _dev(a, dtype):
-    return torch.from_numpy(np.ascontiguousarray(np.asarray(a).astype(dtype))).cuda()
-
-
-def _filled(n, value, dtype):
-    return torch.full((n + GUARD,), value, dtype=dtype, device="cuda")
-
-
-def _assert_claims(case):
-    got = ps.REGIMES[case["kernel"]](case)
-    assert case["claims"] <= got, ("the case no longer reaches", case["claims"] - got)
 
 
 @pytest.fixture
@@ -67,30 +51,23 @@ def _take_err(e):
     return v
 
 
-def _csr(A):
-    """igmc_csr_t of a scipy matrix: rows only (the pair-stream kernels read no columns); (struct, keep-alive)"""
-    t = (_dev(A.indptr, np.int32), _dev(A.indices if A.nnz else [0], np.int32),
-         _dev((A.data - 1) if A.nnz else [0], np.uint8))
-    return _lib.CSR(t[0].data_ptr(), t[1].data_ptr(), t[2].data_ptr(), None, None, A.shape[0], A.shape[1]), t
-
-
 def _guard_ok(t, n, value):
     return bool((t[n:].cpu() == value).all())
 
 
 # ---- igmc_candidate_plan ------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("case", _of("plan"), ids=_id)
+@pytest.mark.parametrize("case", _of("plan"), ids=support.name_id)
 def test_candidate_plan(case, err):
-    _assert_claims(case)
+    support.assert_claims(ps.REGIMES, case)
     lib, A = _lib.load(), ps.plan_graph()
-    G, keep = _csr(A)
+    G, keep = support.csr_struct(A.indptr, A.indices, A.data - 1, *A.shape)
     uo, ro, rp, _ = ps.plan_reference(case)
     users, U = case["users"], len(case["users"])
-    du = _dev(users, np.int32)
-    dc = None if case["cand"] is None else _dev(case["cand"], np.int32)
+    du = support.dev_np(users, np.int32)
+    dc = None if case["cand"] is None else support.dev_np(case["cand"], np.int32)
     nrated = int(sum(len(ps.row(A, int(u))) for u in users))
-    user_off, rated_off, rated_pos = _filled(U + 1, S64, torch.int64), _filled(U + 1, S64, torch.int64), \
-        _filled(nrated, S32, torch.int32)
+    user_off, rated_off = (support.filled(U + 1, S64, torch.int64, GUARD) for _ in range(2))
+    rated_pos = support.filled(nrated, S32, torch.int32, GUARD)
     Cd = _lib.Candidates()
     Cd.users, Cd.cand, Cd.user_off = du.data_ptr(), _lib.ptr(dc), user_off.data_ptr()
     Cd.rated_off, Cd.rated_pos = rated_off.data_ptr(), rated_pos.data_ptr()
@@ -107,16 +84,16 @@ def test_candidate_plan(case, err):
 
 
 # ---- igmc_candidate_lists -----------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("case", _of("lists"), ids=_id)
+@pytest.mark.parametrize("case", _of("lists"), ids=support.name_id)
 def test_candidate_lists(case, err):
-    _assert_claims(case)
+    support.assert_claims(ps.REGIMES, case)
     lib, A = _lib.load(), ps.plan_graph()
-    G, keep = _csr(A)
+    G, keep = support.csr_struct(A.indptr, A.indices, A.data - 1, *A.shape)
     uo, lists, want_err, _ = ps.lists_reference(case)
     rows = case["rows"]
     U, width = rows.shape
-    du, dr = _dev(case["users"], np.int32), _dev(rows, np.int32)
-    user_off, out = _filled(U + 1, S64, torch.int64), _filled(U * width, S32, torch.int32)
+    du, dr = support.dev_np(case["users"], np.int32), support.dev_np(rows, np.int32)
+    user_off, out = support.filled(U + 1, S64, torch.int64, GUARD), support.filled(U * width, S32, torch.int32, GUARD)
     nbytes = C.c_int64(0)
     _lib.check(lib.igmc_candidate_lists_ws_bytes(U, width, C.byref(nbytes)), "igmc_candidate_lists_ws_bytes")
     ws = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device="cuda")
@@ -137,7 +114,7 @@ def _pairs_candidates(case, A):
     Cd, keep = _lib.Candidates(), []
 
     def put(a, dtype):
-        t = _dev(a if len(a) else [0], dtype)
+        t = support.dev_np(a if len(a) else [0], dtype)
         keep.append(t)
         return t.data_ptr()
     if case["mode"] == "explicit":
@@ -160,8 +137,8 @@ def _pairs_candidates(case, A):
 
 
 def _pair_outs(n):
-    return (_filled(n, S32, torch.int32), _filled(n, S32, torch.int32), _filled(n, S64, torch.int64),
-            _filled(n, S64, torch.int64))
+    return tuple(support.filled(n, s, d, GUARD) for s, d in ((S32, torch.int32), (S32, torch.int32), (S64, torch.int64),
+                                                             (S64, torch.int64)))
 
 
 def _launch_pairs(lib, G, Cd, cursor, B, outs, at, err):
@@ -178,12 +155,12 @@ def _check_outs(outs, want, n):
         assert _guard_ok(o, n, s)
 
 
-@pytest.mark.parametrize("case", _of("pairs"), ids=_id)
+@pytest.mark.parametrize("case", _of("pairs"), ids=support.name_id)
 def test_candidate_pairs(case, err):
     """the cursor walked from 0 in steps of B through one all-padding batch past the end"""
-    _assert_claims(case)
+    support.assert_claims(ps.REGIMES, case)
     lib, A = _lib.load(), ps.plan_graph()
-    G, keep_g = _csr(A)
+    G, keep_g = support.csr_struct(A.indptr, A.indices, A.data - 1, *A.shape)
     Cd, keep, P, stream = _pairs_candidates(case, A)
     B = case["B"]
     nb = (P + B - 1) // B + 1
@@ -199,21 +176,21 @@ def test_candidate_pairs(case, err):
 
 
 # ---- the int64 regime ---------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("case", _of("int64"), ids=_id)
+@pytest.mark.parametrize("case", _of("int64"), ids=support.name_id)
 def test_int64_positions(case, err):
     """the plan of 1 120 query slots over 2^22 + 3 items passes 2^32 (a half-catalogue list 2^31): user_off exact;
     igmc_candidate_pairs with the cursor set to positions straddling 2^31 - 1, 2^31, 2^32 and P - B"""
-    _assert_claims(case)
+    support.assert_claims(ps.REGIMES, case)
     lib, A = _lib.load(), ps.big_graph()
-    G, keep_g = _csr(A)
+    G, keep_g = support.csr_struct(A.indptr, A.indices, A.data - 1, *A.shape)
     users, U = case["users"], len(case["users"])
     counts, rp = ps.big_counts(case)
     uo = ps.prefix(counts)
-    du = _dev(users, np.int32)
-    dc = None if case["cand"] is None else _dev(case["cand"], np.int32)
+    du = support.dev_np(users, np.int32)
+    dc = None if case["cand"] is None else support.dev_np(case["cand"], np.int32)
     nrated = int(sum(len(ps.row(A, int(u))) for u in users))
-    user_off, rated_off, rated_pos = _filled(U + 1, S64, torch.int64), _filled(U + 1, S64, torch.int64), \
-        _filled(nrated, S32, torch.int32)
+    user_off, rated_off = (support.filled(U + 1, S64, torch.int64, GUARD) for _ in range(2))
+    rated_pos = support.filled(nrated, S32, torch.int32, GUARD)
     Cd = _lib.Candidates()
     Cd.users, Cd.cand, Cd.user_off = du.data_ptr(), _lib.ptr(dc), user_off.data_ptr()
     Cd.rated_off, Cd.rated_pos = rated_off.data_ptr(), rated_pos.data_ptr()
@@ -240,18 +217,18 @@ def test_int64_positions(case, err):
 
 
 # ---- igmc_session_pairs -------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("case", _of("session"), ids=_id)
+@pytest.mark.parametrize("case", _of("session"), ids=support.name_id)
 def test_session_pairs(case, err):
-    _assert_claims(case)
+    support.assert_claims(ps.REGIMES, case)
     lib = _lib.load()
-    users = _dev(case["users"], np.int32)
+    users = support.dev_np(case["users"], np.int32)
     Sv = _lib.Sessions()
     Sv.users, Sv.num_sessions = users.data_ptr(), len(case["users"])
     B = len(case["links_u"])
-    lu = _filled(B, S32, torch.int32)
-    lu[:B] = _dev(case["links_u"], np.int32)
-    lv = _dev(case["links_v"], np.int32)
-    pid, sess = _filled(B, S64, torch.int64), _filled(B, S32, torch.int32)
+    lu = support.filled(B, S32, torch.int32, GUARD)
+    lu[:B] = support.dev_np(case["links_u"], np.int32)
+    lv = support.dev_np(case["links_v"], np.int32)
+    pid, sess = support.filled(B, S64, torch.int64, GUARD), support.filled(B, S32, torch.int32, GUARD)
     _lib.check(lib.igmc_session_pairs(C.byref(Sv), case["num_items"], B, lu.data_ptr(), lv.data_ptr(), pid.data_ptr(),
                                       sess.data_ptr(), err.data_ptr(), _stream_ptr()), "igmc_session_pairs")
     u, p, s, want_err = ps.session_reference(case)
@@ -262,42 +239,43 @@ def test_session_pairs(case, err):
 
 
 # ---- igmc_explain_count / igmc_explain_offsets --------------------------------------------------------------------------
-@pytest.mark.parametrize("case", _of("count"), ids=_id)
+@pytest.mark.parametrize("case", _of("count"), ids=support.name_id)
 def test_explain_count(case, err):
-    _assert_claims(case)
+    support.assert_claims(ps.REGIMES, case)
     lib = _lib.load()
-    ep, tag = _dev(case["edge_ptr"], np.int32), _dev(case["tag"], np.int64)
-    ne = _filled(case["P"], S32, torch.int32)
+    ep, tag = support.dev_np(case["edge_ptr"], np.int32), support.dev_np(case["tag"], np.int64)
+    ne = support.filled(case["P"], S32, torch.int32, GUARD)
     _lib.check(lib.igmc_explain_count(ep.data_ptr(), tag.data_ptr(), len(case["tag"]), ne.data_ptr(), _stream_ptr()),
                "igmc_explain_count")
     assert np.array_equal(ne[:case["P"]].cpu().numpy(), ps.count_reference(case, S32))
     assert _guard_ok(ne, case["P"], S32)
 
 
-@pytest.mark.parametrize("case", _of("offsets"), ids=_id)
+@pytest.mark.parametrize("case", _of("offsets"), ids=support.name_id)
 def test_explain_offsets(case, err):
-    _assert_claims(case)
+    support.assert_claims(ps.REGIMES, case)
     lib = _lib.load()
     P = len(case["num_edges"])
-    ne = _dev(case["num_edges"], np.int32)
-    off = _filled(P + 1, S64, torch.int64)
+    ne = support.dev_np(case["num_edges"], np.int32)
+    off = support.filled(P + 1, S64, torch.int64, GUARD)
     _lib.check(lib.igmc_explain_offsets(ne.data_ptr(), P, off.data_ptr(), _stream_ptr()), "igmc_explain_offsets")
     assert np.array_equal(off[:P + 1].cpu().numpy(), ps.offsets_reference(case)) and _guard_ok(off, P + 1, S64)
 
 
 # ---- igmc_occlusion_pairs -----------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("case", _of("occl"), ids=_id)
+@pytest.mark.parametrize("case", _of("occl"), ids=support.name_id)
 def test_occlusion_pairs(case, err):
-    _assert_claims(case)
+    support.assert_claims(ps.REGIMES, case)
     lib, A = _lib.load(), ps.plan_graph()
-    G, keep_g = _csr(A)
+    G, keep_g = support.csr_struct(A.indptr, A.indices, A.data - 1, *A.shape)
     off = ps.offsets_reference(case)
     P, B = len(case["num_edges"]), case["B"]
-    pu, pv, doff = _dev(case["pair_u"], np.int32), _dev(case["pair_v"], np.int32), _dev(off, np.int64)
+    pu, pv = support.dev_np(case["pair_u"], np.int32), support.dev_np(case["pair_v"], np.int32)
+    doff = support.dev_np(off, np.int64)
     curs = ps.occl_cursors(case)
     n = len(curs) * B
     lu, lv, pid, tag = _pair_outs(n)
-    j = _filled(n, S32, torch.int32)
+    j = support.filled(n, S32, torch.int32, GUARD)
     cursor = torch.zeros(1, dtype=torch.int64, device="cuda")
     walk = case["cursors"] is None
     for i, pos in enumerate(curs):
@@ -322,8 +300,9 @@ def test_occlusion_pairs(case, err):
 
 # ---- igmc_occlusion_mask / igmc_edge_grad_scatter -----------------------------------------------------------------------
 def _batch_out(bt):
-    t = dict(edge_ptr=_dev(bt["edge_ptr"], np.int32), edge_index=_dev(bt["edge_index"].reshape(-1), np.int64),
-             edge_type=_dev(bt["edge_type"], np.int64), node_gid=_dev(bt["node_gid"], np.int32))
+    t = dict(edge_ptr=support.dev_np(bt["edge_ptr"], np.int32),
+             edge_index=support.dev_np(bt["edge_index"].reshape(-1), np.int64),
+             edge_type=support.dev_np(bt["edge_type"], np.int64), node_gid=support.dev_np(bt["node_gid"], np.int32))
     O = _lib.BatchOut()
     O.edge_cap = bt["edge_cap"]
     for k, v in t.items():
@@ -332,17 +311,17 @@ def _batch_out(bt):
 
 
 def _records(T):
-    return [_filled(T, S32, torch.int32) for _ in range(3)]
+    return [support.filled(T, S32, torch.int32, GUARD) for _ in range(3)]
 
 
-@pytest.mark.parametrize("case", _of("mask"), ids=_id)
+@pytest.mark.parametrize("case", _of("mask"), ids=support.name_id)
 def test_occlusion_mask(case, err):
-    _assert_claims(case)
+    support.assert_claims(ps.REGIMES, case)
     lib = _lib.load()
     O, keep_t = _batch_out(case["batch"])
     B, T, E = len(case["ms"]), case["T"], int(case["batch"]["edge_ptr"][-1])
-    tag, j = _dev(case["tag"], np.int64), _dev(case["j"], np.int32)
-    keep = _filled(case["batch"]["edge_cap"], 7, torch.uint8)
+    tag, j = support.dev_np(case["tag"], np.int64), support.dev_np(case["j"], np.int32)
+    keep = support.filled(case["batch"]["edge_cap"], 7, torch.uint8, GUARD)
     rec = _records(T)
     _lib.check(lib.igmc_occlusion_mask(C.byref(O), B, tag.data_ptr(), j.data_ptr(), keep.data_ptr(), rec[0].data_ptr(),
                                        rec[1].data_ptr(), rec[2].data_ptr(), err.data_ptr(), _stream_ptr()),
@@ -354,24 +333,24 @@ def test_occlusion_mask(case, err):
         assert np.array_equal(r[:T].cpu().numpy(), w) and _guard_ok(r, T, S32)
 
 
-@pytest.mark.parametrize("case", _of("scatter"), ids=_id)
+@pytest.mark.parametrize("case", _of("scatter"), ids=support.name_id)
 def test_edge_grad_scatter(case, err):
     """K checkpoints in order; user / item / rating written at k = 0 only (reset to the sentinel before k = 1)"""
-    _assert_claims(case)
+    support.assert_claims(ps.REGIMES, case)
     lib = _lib.load()
     O, keep_t = _batch_out(case["batch"])
     B, K = len(case["ms"]), case["K"]
     T = int(case["offsets"][-1])
-    tag, off = _dev(case["tag"], np.int64), _dev(case["offsets"], np.int64)
+    tag, off = support.dev_np(case["tag"], np.int64), support.dev_np(case["offsets"], np.int64)
     grads = ps.scatter_grads(case)
     sentinel = np.asarray([0x7f80dead], np.int32).view(np.float32)[0]
-    out = _filled(T, 0.0, torch.float32)
+    out = support.filled(T, 0.0, torch.float32, GUARD)
     out.view(torch.int32).fill_(0x7f80dead)
     rec = _records(T)
     outs, wr, want_err = ps.scatter_reference(case, grads, sentinel, S32)
     written = wr[0] != S32
     for k in range(K):
-        g = _dev(grads[k], np.float32)
+        g = support.dev_np(grads[k], np.float32)
         _lib.check(lib.igmc_edge_grad_scatter(C.byref(O), B, tag.data_ptr(), g.data_ptr(), off.data_ptr(), k, K,
                                               out.data_ptr(), rec[0].data_ptr(), rec[1].data_ptr(), rec[2].data_ptr(),
                                               err.data_ptr(), _stream_ptr()), "igmc_edge_grad_scatter")

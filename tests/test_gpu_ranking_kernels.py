@@ -23,23 +23,11 @@ from igmc_b200 import recommend as rc
 from igmc_b200.data import make_synthetic_dataset
 from igmc_b200.util_functions import RatingGraph, _stream_ptr
 from tests import ranking_cases as rcs
+from tests import support
 
 pytestmark = pytest.mark.gpu
 
 CASES = rcs.all_cases()
-
-
-def _id(c):
-    return c["name"]
-
-
-def _dev(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
-def _assert_claims(case, extra=None):
-    got = rcs.REGIMES[case["kernel"]](case) if extra is None else extra
-    assert case["claims"] <= got, ("the case no longer reaches", case["claims"] - got)
 
 
 def _sync():
@@ -54,7 +42,7 @@ def _run_merge(lib, case, cuts):
     for pr, tag, it, (a, b) in rcs.merge_calls(case, cuts):
         B = len(tag)
         assert lib.igmc_topk_fits(k, B) == 1
-        p, t, i = _dev(pr), _dev(tag), _dev(it)
+        p, t, i = support.dev_np(pr), support.dev_np(tag), support.dev_np(it)
         _lib.check(lib.igmc_topk_merge(p.data_ptr(), K, B, t.data_ptr(), i.data_ptr(), k, ts.data_ptr(),
                                        ti.data_ptr(), _stream_ptr()), "igmc_topk_merge")
         ws, wi = rcs.merge_reference(case, b)
@@ -64,9 +52,9 @@ def _run_merge(lib, case, cuts):
     return ts, ti
 
 
-@pytest.mark.parametrize("case", [c for c in CASES if c["kernel"] == "merge"], ids=_id)
+@pytest.mark.parametrize("case", [c for c in CASES if c["kernel"] == "merge"], ids=support.name_id)
 def test_topk_merge(case):
-    _assert_claims(case)
+    support.assert_claims(rcs.REGIMES, case)
     lib = _lib.load()
     finals = [_run_merge(lib, case, cuts) for cuts in case["cuts"]]
     for ts, ti in finals[1:]:     # independent of where the batches were cut
@@ -98,15 +86,15 @@ def test_topk_merge_refuses_past_227_kb():
 
 
 # ---- igmc_score_scatter -------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("case", [c for c in CASES if c["kernel"] == "scatter"], ids=_id)
+@pytest.mark.parametrize("case", [c for c in CASES if c["kernel"] == "scatter"], ids=support.name_id)
 def test_score_scatter(case):
-    _assert_claims(case)
+    support.assert_claims(rcs.REGIMES, case)
     lib = _lib.load()
     preds, tag, n = rcs.scatter_data(case)
     sentinel = rcs.f32_bits([0x7f80dead])[0]
     out = torch.full((n,), float(sentinel), dtype=torch.float32, device="cuda")
     out.view(torch.int32).fill_(0x7f80dead)
-    p, t = _dev(preds), _dev(tag)
+    p, t = support.dev_np(preds), support.dev_np(tag)
     _lib.check(lib.igmc_score_scatter(p.data_ptr(), case["K"], len(tag), t.data_ptr(), out.data_ptr(), _stream_ptr()),
                "igmc_score_scatter")
     got = out.cpu().numpy()
@@ -120,9 +108,9 @@ def test_score_scatter(case):
 
 
 # ---- igmc_influence_topk ------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("case", [c for c in CASES if c["kernel"] == "influence"], ids=_id)
+@pytest.mark.parametrize("case", [c for c in CASES if c["kernel"] == "influence"], ids=support.name_id)
 def test_influence_topk(case):
-    _assert_claims(case)
+    support.assert_claims(rcs.REGIMES, case)
     lib = _lib.load()
     T, k = case["T"], case["k"]
     finals = []
@@ -135,7 +123,7 @@ def test_influence_topk(case):
         for c, (S, tag, (a, b)) in enumerate(calls):
             B = len(tag)
             assert lib.igmc_topk_fits(k, B) == 1
-            s, t = _dev(S), _dev(tag)
+            s, t = support.dev_np(S), support.dev_np(tag)
             _lib.check(lib.igmc_influence_topk(s.data_ptr(), B, T, t.data_ptr(), k, pv.data_ptr(), pi.data_ptr(),
                                                cv.data_ptr(), ci.data_ptr(), _stream_ptr()), "igmc_influence_topk")
             if c == len(calls) - 1 or T <= 3:
@@ -150,9 +138,9 @@ def test_influence_topk(case):
 
 
 # ---- igmc_occlusion_order -----------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("case", [c for c in CASES if c["kernel"] == "occlusion"], ids=_id)
+@pytest.mark.parametrize("case", [c for c in CASES if c["kernel"] == "occlusion"], ids=support.name_id)
 def test_occlusion_order(case):
-    _assert_claims(case)
+    support.assert_claims(rcs.REGIMES, case)
     lib = _lib.load()
     score, occluded, offsets, user, item, rating = rcs.occlusion_data(case)
     P, T, m = len(offsets) - 1, int(offsets[-1]), case["m"]
@@ -162,9 +150,9 @@ def test_occlusion_order(case):
     n = P * m if m else T
     outs = [torch.full((max(n, 1),), 12345, dtype=torch.int32, device="cuda") for _ in range(3)]
     od = torch.full((max(n, 1),), 12345.0, dtype=torch.float32, device="cuda")
-    d_score = None if score is None else _dev(score)
-    d_occ, d_off = _dev(occluded if T else np.zeros(1, np.float32)), _dev(offsets)
-    d_u, d_i, d_r = (_dev(x if T else np.zeros(1, np.int32)) for x in (user, item, rating))
+    d_score = None if score is None else support.dev_np(score)
+    d_occ, d_off = support.dev_np(occluded if T else np.zeros(1, np.float32)), support.dev_np(offsets)
+    d_u, d_i, d_r = (support.dev_np(x if T else np.zeros(1, np.int32)) for x in (user, item, rating))
     _lib.check(lib.igmc_occlusion_order(_lib.ptr(d_score), d_occ.data_ptr(), d_off.data_ptr(), P, T, d_u.data_ptr(),
                                         d_i.data_ptr(), d_r.data_ptr(), m, ws.data_ptr(), ws.numel(),
                                         outs[0].data_ptr(), outs[1].data_ptr(), outs[2].data_ptr(), od.data_ptr(),
@@ -201,17 +189,17 @@ def _corated_call(lib, g, users, m, exclude, slack=0):
     items = torch.full((U, m), 777, dtype=torch.int32, device="cuda")
     paths = torch.full((U, m), 777, dtype=torch.int32, device="cuda")
     err = torch.zeros(1, dtype=torch.int32, device="cuda")
-    du = _dev(np.asarray(users, np.int32))
+    du = support.dev_np(np.asarray(users, np.int32))
     _lib.check(lib.igmc_corated_items(C.byref(g._c), du.data_ptr(), U, m, int(exclude), ws.data_ptr(), nbytes.value,
                                       items.data_ptr(), paths.data_ptr(), err.data_ptr(), _stream_ptr()),
                "igmc_corated_items")
     return items.cpu().numpy(), paths.cpu().numpy(), int(err.item()), nbytes.value, ws[nbytes.value:].cpu().numpy()
 
 
-@pytest.mark.parametrize("case", [c for c in CASES if c["kernel"] == "corated"], ids=_id)
+@pytest.mark.parametrize("case", [c for c in CASES if c["kernel"] == "corated"], ids=support.name_id)
 def test_corated_items(case):
     A, g = _graph(case["graph"])
-    _assert_claims(case, rcs.corated_regimes(case, A))
+    support.assert_claims(rcs.REGIMES, case, rcs.corated_regimes(case, A))
     lib = _lib.load()
     nu, ni = A.shape
     items, paths, err, nbytes, tail = _corated_call(lib, g, case["users"], case["m"], case["exclude"], slack=1 << 16)
@@ -272,12 +260,6 @@ def test_corated_global_regime_many_users():
 
 
 # ---- end to end through InferenceEngine ---------------------------------------------------------------------------------
-def _model(R, seed=0):
-    from igmc_b200.models import IGMC
-    torch.manual_seed(seed)
-    return IGMC(4, latent_dim=[32] * 4, num_relations=R, num_bases=4, regression=True).cuda()
-
-
 def _cold_catalogue():
     A = make_synthetic_dataset("ml_100k", seed=0)["adj_train"]
     nu, ni = A.shape
@@ -288,7 +270,7 @@ def test_cold_catalogue_ties_fill_the_tail():
     A, warm = _cold_catalogue()
     nu, ni = A.shape
     cold = np.arange(warm, ni)
-    m = _model(5)
+    m = support.model(5)
     m.kernel_plan = 1                 # the same plan at every batch size
     mnph = 100
     users = np.array([3, 400, 942])
@@ -327,7 +309,7 @@ def test_nan_checkpoint():
     """an ensemble with a checkpoint whose lin2.bias is NaN: every score is NaN, so each top-k is the first k
     candidates by item and each explanation is in rating order, as a model whose every delta is 0 orders it"""
     A = make_synthetic_dataset("ml_100k", seed=0)["adj_train"]
-    m = _model(5)
+    m = support.model(5)
     users = np.array([5, 6])
     with tempfile.TemporaryDirectory() as tmp:
         good, bad, flat = (os.path.join(tmp, n) for n in ("good.pth", "nan.pth", "flat.pth"))
@@ -360,7 +342,7 @@ def test_engine_refuses_unrunnable_batch_before_launch():
     sessions, influence, the public functions); the engine then serves k = 255 and an explicit-pair run"""
     ds = make_synthetic_dataset("tiny", seed=0)
     A = ds["adj_train"]
-    m = _model(5)
+    m = support.model(5)
     eng = rc.InferenceEngine(m, A, batch_size=19114)
     with pytest.raises(ValueError, match="top-k merge"):
         eng.recommend([0, 1], 256)

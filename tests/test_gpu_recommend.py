@@ -7,7 +7,6 @@
   several batches and several users per batch; never a rated item with exclude_rated;
 * a three-checkpoint ensemble; steady-state steps without a host synchronisation."""
 import ctypes as C
-import functools
 import os
 import tempfile
 
@@ -17,40 +16,12 @@ import torch
 
 from igmc_b200 import _lib
 from igmc_b200 import recommend as rc
-from igmc_b200.data import build_adj, make_synthetic_dataset, synth_ratings
 from igmc_b200.util_functions import RatingGraph, SubgraphExtractor, _stream_ptr
 from oracle import extract_np, pyg_restated
 from tests import pyg2_oracle
+from tests import support
 
 pytestmark = pytest.mark.gpu
-
-
-@functools.lru_cache(maxsize=None)
-def _ds(name):
-    return make_synthetic_dataset(name, seed=0)
-
-
-@functools.lru_cache(maxsize=None)
-def _r13():
-    """a 13-level rating matrix: more relations than the relation-space plans take (plan 0)"""
-    nu, ni = 400, 300
-    u, v, lab = synth_ratings(nu, ni, 9000, 13, seed=4)
-    return dict(adj_train=build_adj(u, v, lab, nu, ni), num_relations=13, num_users=nu, num_items=ni)
-
-
-def _model(R, h=1, rgcn="pyg-1.4", dgcnn=False, seed=0):
-    from igmc_b200.models import DGCNN_RS, IGMC
-    torch.manual_seed(seed)
-    if dgcnn:
-        m = DGCNN_RS(2 * h + 2, latent_dim=[32, 32, 32, 1], k=30, num_relations=R, num_bases=4, regression=True,
-                     rgcn=rgcn)
-    else:
-        m = IGMC(2 * h + 2, latent_dim=[32] * 4, num_relations=R, num_bases=4, regression=True, rgcn=rgcn)
-    if rgcn == "pyg-2":
-        with torch.no_grad():
-            for c in m.convs:
-                c.bias.uniform_(-0.3, 0.3)
-    return m.cuda()
 
 
 def _mixed_pairs(A, n, seed):
@@ -96,7 +67,7 @@ def _loop_scores(m, A, u, v, B, h, mnph, seed):
 @pytest.mark.parametrize("exclude", [True, False])
 @pytest.mark.parametrize("which", ["all", "none", "some", "row"])
 def test_candidate_kernels_match_host_twin(which, exclude):
-    A = _ds("ml_100k")["adj_train"]
+    A = support.adj("ml_100k")
     g = RatingGraph(A)
     rp, ci, ni = g.host["row_ptr"].astype(np.int64), g.host["col_idx"].astype(np.int64), g.num_items
     deg = np.diff(rp)
@@ -107,7 +78,7 @@ def test_candidate_kernels_match_host_twin(which, exclude):
     cand = dict(all=None, none=unrated[:3] if len(unrated) else np.array([ni - 1]),
                 some=np.unique(rng.choice(ni, 300)), row=ci[rp[5]:rp[6]].copy())[which]
     plan = rc.candidate_plan_host(rp, ci, ni, users, cand, exclude)
-    eng = rc.InferenceEngine(_model(5), A, batch_size=64, max_nodes_per_hop=10)
+    eng = rc.InferenceEngine(support.model(5), A, batch_size=64, max_nodes_per_hop=10)
     P = eng.start_recommend(users, 5, items=cand, exclude_rated=exclude)
     assert P == int(plan[0][-1])
     run = eng.run
@@ -150,9 +121,9 @@ PLANS = {
 @pytest.mark.parametrize("name", list(PLANS))
 def test_predict_pairs_equals_eval_forward(name):
     dsn, h, mnph, B, kw, plan = PLANS[name]
-    ds = _r13() if dsn == "r13" else _ds(dsn)
+    ds = support.dataset(dsn)
     A = ds["adj_train"]
-    m = _model(ds["num_relations"], h, **kw)
+    m = support.model(ds["num_relations"], h=h, **kw, pyg2_bias=True)
     u, v = _mixed_pairs(A, 2 * B + 17, seed=1)
     got = rc.predict_pairs(m, A, u, v, h=h, max_nodes_per_hop=mnph, batch_size=B, sample_seed=7)
     want = _loop_scores(m, A, u, v, B, h, mnph, 7)
@@ -172,9 +143,9 @@ def test_predict_pairs_equals_eval_forward(name):
 # ---- 3. against the fp64 restated forward -----------------------------------------------------------------------------
 @pytest.mark.parametrize("rgcn", ["pyg-1.4", "pyg-2"])
 def test_predict_pairs_against_oracle(rgcn):
-    ds = _ds("ml_1m")
+    ds = support.dataset("ml_1m")
     A, R, mnph, seed = ds["adj_train"], 5, 100, 7
-    m = _model(R, rgcn=rgcn)
+    m = support.model(R, rgcn=rgcn, pyg2_bias=True)
     ref = pyg2_oracle.igmc_ref(rgcn, 4, (32,) * 4, R, 4, 0.0)
     ref.load_state_dict({k: v.double().cpu() for k, v in m.state_dict().items()})
     ref = pyg_restated.set_formulation(ref.double(), "transform").cuda().eval()
@@ -218,9 +189,9 @@ def _check_topk(A, users, cand, exclude, ks, scores_of, ti_ts):
 def test_recommend_matches_sorted_predictions():
     """ml_1m* full catalogue of 3 users (a user spans many batches) and a 40-item list for 12 users (several users per
     batch); k = 1, 10, 100; B = 50 and 256 on the same plan; CUDA graphs on and off"""
-    ds = _ds("ml_1m")
+    ds = support.dataset("ml_1m")
     A, mnph = ds["adj_train"], 100
-    m = _model(5)
+    m = support.model(5)
     m.kernel_plan = 1                      # the same plan at both batch sizes
     cases = [(np.array([3, 10, 4000]), None), (np.arange(100, 112), np.random.default_rng(0).choice(3706, 40))]
     for users, cand in cases:
@@ -257,9 +228,9 @@ def test_recommend_matches_sorted_predictions():
 def test_recommend_short_lists_pad():
     """a user with fewer candidates than k: item -1 / score -inf in the empty slots; a user who rated every candidate
     gets only empty slots"""
-    ds = _ds("ml_100k")
+    ds = support.dataset("ml_100k")
     A = ds["adj_train"]
-    m = _model(5)
+    m = support.model(5)
     u0 = 0
     row = A.indices[A.indptr[u0]:A.indptr[u0 + 1]]
     cand = np.concatenate([row[:3], np.setdiff1d(np.arange(A.shape[1]), row)[:4]])
@@ -273,14 +244,14 @@ def test_recommend_short_lists_pad():
 
 # ---- 5. ensemble --------------------------------------------------------------------------------------------------------
 def test_ensemble_of_three_checkpoints():
-    ds = _ds("ml_100k")
+    ds = support.dataset("ml_100k")
     A, mnph = ds["adj_train"], 200
-    m = _model(5)
+    m = support.model(5)
     u, v = _mixed_pairs(A, 130, seed=4)
     with tempfile.TemporaryDirectory() as tmp:
         paths = []
         for c in range(3):
-            mc = _model(5, seed=c + 1)
+            mc = support.model(5, seed=c + 1)
             paths.append(os.path.join(tmp, "model_checkpoint%d.pth" % c))
             torch.save(mc.state_dict(), paths[-1])
         own = m.flat_params.clone()
@@ -301,9 +272,9 @@ def test_ensemble_of_three_checkpoints():
 
 # ---- 6. steady state: no host synchronisation, repeatable, clean error word ---------------------------------------------
 def test_steady_state_steps_do_not_sync():
-    ds = _ds("ml_1m")
+    ds = support.dataset("ml_1m")
     A = ds["adj_train"]
-    m = _model(5)
+    m = support.model(5)
     eng = rc.InferenceEngine(m, A, max_nodes_per_hop=100, batch_size=50, sample_seed=1)
     outs = []
     try:

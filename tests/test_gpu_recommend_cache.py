@@ -22,14 +22,10 @@ import torch
 from igmc_b200 import _lib
 from igmc_b200 import recommend as rc
 from igmc_b200.util_functions import RatingGraph, _stream_ptr
-from tests import test_gpu_recommend as tr
+from tests import support
 from tests.test_recommend_cache_host import _slot_case
 
 pytestmark = pytest.mark.gpu
-
-
-def _dev(a, dt=torch.int32):
-    return torch.as_tensor(np.asarray(a)).to(dt).cuda()
 
 
 @pytest.mark.parametrize("bound", [0, 4000])
@@ -37,7 +33,7 @@ def _dev(a, dt=torch.int32):
 def test_rescore_plan_kernel_matches_twin(bound, shared, exclude):
     lib = _lib.load()
     rng = np.random.default_rng(3)
-    A = tr._r13()["adj_train"]
+    A = support.adj("r13")
     g = RatingGraph(A)
     h = g.host
     U, ni = 70, g.num_items
@@ -59,9 +55,10 @@ def test_rescore_plan_kernel_matches_twin(bound, shared, exclude):
         full = torch.full((U + 1,), 9, dtype=torch.uint8, device="cuda")
         totals, err = torch.zeros(2, dtype=torch.int64, device="cuda"), torch.zeros(1, dtype=torch.int32,
                                                                                      device="cuda")
-        cd = None if cand is None else _dev(cand)
-        assert lib.igmc_rescore_plan(C.byref(g._c), _dev(users).data_ptr(), U, _dev(eu if len(eu) else [0]).data_ptr(),
-                                     _dev(ev if len(ev) else [0]).data_ptr(), len(eu), _lib.ptr(cd),
+        cd = None if cand is None else support.dev(cand)
+        assert lib.igmc_rescore_plan(C.byref(g._c), support.dev(users).data_ptr(), U,
+                                     support.dev(eu if len(eu) else [0]).data_ptr(),
+                                     support.dev(ev if len(ev) else [0]).data_ptr(), len(eu), _lib.ptr(cd),
                                      0 if cand is None else len(cand), int(exclude), ws.data_ptr(), ws.numel(),
                                      user_off.data_ptr(), out.data_ptr(), cap, full.data_ptr(), totals.data_ptr(),
                                      err.data_ptr(), _stream_ptr()) == 0
@@ -85,11 +82,12 @@ def test_invalidate_and_settle_kernels_match_twins(D, k):
     user_off = np.concatenate([[0], np.cumsum([len(c[5]) for c in cases])]).astype(np.int64)
     resc = np.concatenate([c[5] for c in cases] + [np.zeros(1)]).astype(np.int32)
     ws_, wi, wts, wti = rc.cache_invalidate_host(user_off, resc, full, complete, top_s, top_i)
-    ds, di = _dev(np.r_[top_s.reshape(-1), 5.0], torch.float32), _dev(np.r_[top_i.reshape(-1), 77], torch.int64)
+    ds = support.dev(np.r_[top_s.reshape(-1), 5.0], torch.float32)
+    di = support.dev(np.r_[top_i.reshape(-1), 77], torch.int64)
     ts, ti = torch.full((U + 1,), 3.0, device="cuda"), torch.full((U + 1,), 77, dtype=torch.int64, device="cuda")
-    dcomp = _dev(np.r_[complete, 9], torch.uint8)
-    assert lib.igmc_cache_invalidate(U, D, _dev(user_off, torch.int64).data_ptr(), _dev(resc).data_ptr(),
-                                     _dev(full, torch.uint8).data_ptr(), dcomp.data_ptr(), ds.data_ptr(),
+    dcomp = support.dev(np.r_[complete, 9], torch.uint8)
+    assert lib.igmc_cache_invalidate(U, D, support.dev(user_off, torch.int64).data_ptr(), support.dev(resc).data_ptr(),
+                                     support.dev(full, torch.uint8).data_ptr(), dcomp.data_ptr(), ds.data_ptr(),
                                      di.data_ptr(), ts.data_ptr(), ti.data_ptr(), _stream_ptr()) == 0
     assert np.array_equal(ds[:-1].cpu().numpy().view(np.uint32), ws_.reshape(-1).view(np.uint32))
     assert np.array_equal(di[:-1].cpu().numpy(), wi.reshape(-1)) and float(ds[-1]) == 5.0 and int(di[-1]) == 77
@@ -99,12 +97,13 @@ def test_invalidate_and_settle_kernels_match_twins(D, k):
     for j, c in enumerate(cases):
         ws_[j], wi[j] = rc.topk_merge_host(ws_[j], wi[j], c[1][c[5]], c[5])
     gs, gi, gcomp, gredo = rc.cache_settle_host(wts, wti, ws_, wi, k)
-    ds, di = _dev(np.r_[ws_.reshape(-1), 5.0], torch.float32), _dev(np.r_[wi.reshape(-1), 77], torch.int64)
+    ds = support.dev(np.r_[ws_.reshape(-1), 5.0], torch.float32)
+    di = support.dev(np.r_[wi.reshape(-1), 77], torch.int64)
     redo, cnt = torch.full((U + 1,), -7, dtype=torch.int32, device="cuda"), torch.zeros(1, dtype=torch.int32,
                                                                                         device="cuda")
-    assert lib.igmc_cache_settle(U, D, k, _dev(wts, torch.float32).data_ptr(), _dev(wti, torch.int64).data_ptr(),
-                                 ds.data_ptr(), di.data_ptr(), dcomp.data_ptr(), redo.data_ptr(), cnt.data_ptr(),
-                                 _stream_ptr()) == 0
+    assert lib.igmc_cache_settle(U, D, k, support.dev(wts, torch.float32).data_ptr(),
+                                 support.dev(wti, torch.int64).data_ptr(), ds.data_ptr(), di.data_ptr(),
+                                 dcomp.data_ptr(), redo.data_ptr(), cnt.data_ptr(), _stream_ptr()) == 0
     assert np.array_equal(ds[:-1].cpu().numpy().view(np.uint32), gs.reshape(-1).view(np.uint32))
     assert np.array_equal(di[:-1].cpu().numpy(), gi.reshape(-1)) and int(di[-1]) == 77
     assert np.array_equal(dcomp[:U].cpu().numpy(), gcomp) and int(dcomp[U]) == 9
@@ -162,11 +161,11 @@ CONFIGS = {
 
 def _setup(cfg):
     if cfg.get("r13"):
-        A, R = tr._r13()["adj_train"], 13
+        A, R = support.adj("r13"), 13
     else:
-        d = tr._ds("ml_100k")
+        d = support.dataset("ml_100k")
         A, R = d["adj_train"], 5
-    m = tr._model(R, rgcn=cfg.get("rgcn", "pyg-1.4"), dgcnn=cfg.get("dgcnn", False))
+    m = support.model(R, rgcn=cfg.get("rgcn", "pyg-1.4"), dgcnn=cfg.get("dgcnn", False), pyg2_bias=True)
     if "plan" in cfg:
         m.kernel_plan = cfg["plan"]
     g = RatingGraph(A, reserve_nnz=20000, reserve_users=8, reserve_items=4)
@@ -185,7 +184,7 @@ def _run_chain(cfg, tmp):
         paths = []
         for c in range(cfg["ckpt"]):
             torch.manual_seed(100 + c)
-            m2 = tr._model(m.num_relations)
+            m2 = support.model(m.num_relations)
             paths.append(os.path.join(tmp, "ck%d.pth" % c))
             torch.save(m2.state_dict(), paths[-1])
     kw = dict(items=items, exclude_rated=cfg.get("items") != "all", max_nodes_per_hop=cfg["mnph"],

@@ -12,7 +12,6 @@ csrc/recommend.cu).
 * an item nobody rated, a new item added by graph.update, recommend and recommend_users interleaved on one engine;
   steady-state steps without a host synchronisation."""
 import ctypes as C
-import functools
 import os
 import tempfile
 
@@ -23,36 +22,11 @@ import torch
 
 from igmc_b200 import _lib
 from igmc_b200 import recommend as rc
-from igmc_b200.data import build_adj, load_flixster, make_synthetic_dataset, synth_ratings
+from igmc_b200.data import build_adj, synth_ratings
 from igmc_b200.util_functions import RatingGraph, _stream_ptr
+from tests import support
 
 pytestmark = pytest.mark.gpu
-
-
-@functools.lru_cache(maxsize=None)
-def _ds(name):
-    if name == "flixster":
-        return load_flixster()
-    if name == "r13":
-        nu, ni = 400, 300
-        u, v, lab = synth_ratings(nu, ni, 9000, 13, seed=4)
-        return dict(adj_train=build_adj(u, v, lab, nu, ni), num_relations=13)
-    return make_synthetic_dataset(name, seed=0)
-
-
-def _model(R, h=1, rgcn="pyg-1.4", dgcnn=False, seed=0):
-    from igmc_b200.models import DGCNN_RS, IGMC
-    torch.manual_seed(seed)
-    if dgcnn:
-        m = DGCNN_RS(2 * h + 2, latent_dim=[32, 32, 32, 1], k=30, num_relations=R, num_bases=4, regression=True,
-                     rgcn=rgcn)
-    else:
-        m = IGMC(2 * h + 2, latent_dim=[32] * 4, num_relations=R, num_bases=4, regression=True, rgcn=rgcn)
-    if rgcn == "pyg-2":
-        with torch.no_grad():
-            for c in m.convs:
-                c.bias.uniform_(-0.3, 0.3)
-    return m.cuda()
 
 
 def _twin(g, items, m, exclude):
@@ -85,7 +59,7 @@ def _raters(A, v):
 # ---- 1. the item-side retriever against its twin ----------------------------------------------------------------------
 @pytest.mark.parametrize("name", ["tiny", "ml_100k", "ml_1m", "flixster"])
 def test_corated_users_match_twin(name):
-    A = _ds(name)["adj_train"]
+    A = support.adj(name)
     g = RatingGraph(A)
     nu, ni = g.shape
     items = _query_items(A, 60, seed=1)
@@ -133,7 +107,7 @@ def test_corated_users_global_memory_regime(transpose):
 
 def test_corated_users_invalid_ids_set_the_error_word():
     """an item id outside G: IGMC_ERR_CANDIDATES and a padding row; the other rows are the twin's"""
-    A = _ds("ml_100k")["adj_train"]
+    A = support.adj("ml_100k")
     g = RatingGraph(A)
     nu, ni = g.shape
     lib = _lib.load()
@@ -182,7 +156,7 @@ def _apply_chain(g, cur, rng, steps, n):
 
 def test_corated_users_follow_graph_updates():
     """a chain of inserts, relabels, deletes and new users / items: the same bytes as a fresh graph of the result"""
-    A = ssp.csr_matrix(_ds("ml_100k")["adj_train"])
+    A = ssp.csr_matrix(support.adj("ml_100k"))
     g = RatingGraph(A, reserve_nnz=20000, reserve_users=50, reserve_items=40)
     old = g.shape
     cur = _apply_chain(g, A.copy(), np.random.default_rng(5), 4, 3000)
@@ -201,7 +175,7 @@ def test_corated_users_follow_graph_updates():
 @pytest.mark.parametrize("exclude", [True, False])
 def test_item_and_user_side_counts_agree(exclude):
     """m = num_users and m = num_items: the dense count matrices of corated_users and corated_items are transposes"""
-    A = _ds("ml_100k")["adj_train"]
+    A = support.adj("ml_100k")
     g = RatingGraph(A)
     nu, ni = g.shape
     iu, ip = (x.cpu().numpy() for x in rc.corated_items(g, np.arange(nu), ni, exclude_rated=exclude))
@@ -255,8 +229,8 @@ def test_item_query_pairs_direct():
 def test_item_side_batches_match_the_twins(which):
     """the candidate kernels on the transposed view then igmc_item_query_pairs, every batch of a run and one past its
     end (the tag -1 tail), against the host twins on the transposed arrays"""
-    A = _ds("ml_100k")["adj_train"]
-    m = _model(5)
+    A = support.adj("ml_100k")
+    m = support.model(5)
     nu, ni = A.shape
     items = np.array([0, 50, 50, ni - 1, 7], np.int64)
     users = None if which == "all" else np.unique(np.random.default_rng(1).choice(nu, 200))
@@ -346,10 +320,10 @@ def test_recommend_users_scores_equal_predict_pairs(name):
     """k = 256 keeps every candidate of a 120-user list: the lists show every score, each bit for bit predict_pairs'
     at the same B and plan; rated pairs (exclude_rated=False) are scored without their target edge, as there"""
     dsn, h, mnph, kw, plan = PLANS[name]
-    ds = _ds(dsn)
+    ds = support.dataset(dsn)
     A = ds["adj_train"]
     nu = A.shape[0]
-    m = _model(ds["num_relations"], h, **kw)
+    m = support.model(ds["num_relations"], h=h, **kw, pyg2_bias=True)
     items = _query_items(A, 2, seed=4)[[0, 2, 4, 5]]
     rng = np.random.default_rng(6)
     users = np.unique(np.concatenate([rng.choice(nu, 100, replace=False), _raters(A, items[2])[:20]]))
@@ -369,8 +343,8 @@ def test_recommend_users_scores_equal_predict_pairs(name):
 
 def test_recommend_users_three_checkpoints():
     """the ensemble score of every pair is the fp32 mean, in checkpoint order, of three single-checkpoint runs"""
-    A = _ds("ml_100k")["adj_train"]
-    m = _model(5)
+    A = support.adj("ml_100k")
+    m = support.model(5)
     items = np.array([0, 10, 200], np.int64)
     users = np.arange(0, 943, 9)
     opts = dict(max_nodes_per_hop=200, batch_size=50, sample_seed=3)
@@ -378,7 +352,7 @@ def test_recommend_users_three_checkpoints():
         paths = []
         for c in range(3):
             paths.append(os.path.join(tmp, "model_checkpoint%d.pth" % c))
-            torch.save(_model(5, seed=c + 1).state_dict(), paths[-1])
+            torch.save(support.model(5, seed=c + 1).state_dict(), paths[-1])
         ens = rc.recommend_users(m, A, items, 256, users=users, checkpoints=paths, **opts)
         single = [rc.recommend_users(m, A, items, 256, users=users, checkpoints=[p], **opts) for p in paths]
     lists = _item_lists(A, items, users, True)
@@ -401,9 +375,9 @@ def test_recommend_users_three_checkpoints():
 def test_recommend_users_lists_and_determinism():
     """ml_1m*: every user (an item spans many batches), a shared 300-user list and per-item rows (several items per
     batch), exclude_rated on and off, k = 1, 10 and 256; B = 50 and 256 on one plan, CUDA graphs on and off"""
-    A = _ds("ml_1m")["adj_train"]
+    A = support.adj("ml_1m")
     nu, ni = A.shape
-    m = _model(5)
+    m = support.model(5)
     m.kernel_plan = 1                       # the same plan at both batch sizes
     mnph = 100
     rng = np.random.default_rng(8)
@@ -451,8 +425,8 @@ def test_recommend_users_lists_and_determinism():
 
 def test_recommend_users_retrieve_equals_retrieved_rows():
     """retrieve=M ranks exactly the rows corated_users returns; a device tensor of rows gives the same lists"""
-    A = _ds("ml_1m")["adj_train"]
-    m = _model(5)
+    A = support.adj("ml_1m")
+    m = support.model(5)
     items = np.array([2, 40, 41, 1000], np.int64)
     opts = dict(max_nodes_per_hop=100, batch_size=128, sample_seed=2)
     for M in (60, 300):
@@ -474,10 +448,10 @@ def test_item_nobody_rated_and_a_new_item():
     """an item without ratings has no bridge (corated_users is all padding) and is still ranked against every user by
     the model; a new item added by graph.update with three ratings is ranked by an engine kept across the update as a
     fresh engine ranks it, and an update during a run makes the next step raise"""
-    A = ssp.csr_matrix(_ds("ml_100k")["adj_train"])
+    A = ssp.csr_matrix(support.adj("ml_100k"))
     nu, ni = A.shape
     g = RatingGraph(A, reserve_nnz=100, reserve_items=4)
-    m = _model(5)
+    m = support.model(5)
     opts = dict(max_nodes_per_hop=200, batch_size=64, sample_seed=1)
     g.update([], [], [], shape=(nu, ni + 1))          # item ni: nobody rated it
     users, paths = rc.corated_users(g, [ni], 10)
@@ -512,8 +486,8 @@ def test_item_nobody_rated_and_a_new_item():
 
 def test_recommend_and_recommend_users_interleaved():
     """one engine alternating user-side and item-side runs gives what separate engines give"""
-    A = _ds("ml_100k")["adj_train"]
-    m = _model(5)
+    A = support.adj("ml_100k")
+    m = support.model(5)
     opts = dict(max_nodes_per_hop=200, batch_size=64, sample_seed=2)
     users, items = np.array([1, 2, 300]), np.array([4, 5, 900])
     eng = rc.InferenceEngine(m, A, **opts)
@@ -531,8 +505,8 @@ def test_recommend_and_recommend_users_interleaved():
 
 
 def test_recommend_users_steady_state_steps_do_not_sync():
-    A = _ds("ml_1m")["adj_train"]
-    m = _model(5)
+    A = support.adj("ml_1m")
+    m = support.model(5)
     eng = rc.InferenceEngine(m, A, max_nodes_per_hop=100, batch_size=50, sample_seed=1)
     outs = []
     try:

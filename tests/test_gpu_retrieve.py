@@ -9,7 +9,6 @@
   catalogue restricted to the items with a bridge;
 * steady-state steps of a retrieve run do not synchronise."""
 import ctypes
-import functools
 
 import numpy as np
 import pytest
@@ -18,27 +17,11 @@ import torch
 
 from igmc_b200 import _lib
 from igmc_b200 import recommend as rc
-from igmc_b200.data import build_adj, load_flixster, make_synthetic_dataset, synth_ratings
+from igmc_b200.data import build_adj, synth_ratings
 from igmc_b200.util_functions import RatingGraph
+from tests import support
 
 pytestmark = pytest.mark.gpu
-
-
-@functools.lru_cache(maxsize=None)
-def _ds(name):
-    if name == "flixster":
-        return load_flixster()
-    if name == "r13":
-        nu, ni = 400, 300
-        u, v, lab = synth_ratings(nu, ni, 9000, 13, seed=4)
-        return dict(adj_train=build_adj(u, v, lab, nu, ni), num_relations=13)
-    return make_synthetic_dataset(name, seed=0)
-
-
-def _model(R, seed=0):
-    from igmc_b200.models import IGMC
-    torch.manual_seed(seed)
-    return IGMC(4, latent_dim=[32] * 4, num_relations=R, num_bases=4, regression=True).cuda()
 
 
 def _twin(g, users, m, exclude):
@@ -56,7 +39,7 @@ def _query_users(nu, A, n, seed):
 # ---- 1. the retriever against its twin ----------------------------------------------------------------------------------
 @pytest.mark.parametrize("name", ["ml_100k", "ml_1m", "flixster", "tiny"])
 def test_corated_items_match_twin(name):
-    A = _ds(name)["adj_train"]
+    A = support.adj(name)
     g = RatingGraph(A)
     nu, ni = g.shape
     users = _query_users(nu, A, min(60, nu - 4), seed=1)
@@ -91,7 +74,7 @@ def test_corated_items_global_memory_regime():
 
 def test_corated_items_follow_graph_updates():
     """a chain of inserts, relabels, deletes and new users / items: the same bytes as a fresh graph of the result"""
-    A = ssp.csr_matrix(_ds("ml_100k")["adj_train"])
+    A = ssp.csr_matrix(support.adj("ml_100k"))
     g = RatingGraph(A, reserve_nnz=20000, reserve_users=50, reserve_items=40)
     rng = np.random.default_rng(5)
     cur = A.copy()
@@ -170,9 +153,9 @@ PLANS = {
 @pytest.mark.parametrize("name", list(PLANS))
 def test_recommend_per_user_lists(name):
     dsn, mnph, plan = PLANS[name]
-    ds = _ds(dsn)
+    ds = support.dataset(dsn)
     A = ds["adj_train"]
-    m = _model(ds["num_relations"])
+    m = support.model(ds["num_relations"])
     users = np.array([3, 10, 10, 25, 7], np.int64)
     rows = _rows(A, users, 40, seed=4)
     first = None
@@ -200,9 +183,9 @@ def test_recommend_per_user_lists(name):
 
 
 def test_recommend_retrieve_equals_retrieved_lists():
-    ds = _ds("ml_1m")
+    ds = support.dataset("ml_1m")
     A, mnph = ds["adj_train"], 100
-    m = _model(5)
+    m = support.model(5)
     users = np.array([2, 40, 41, 1000], np.int64)
     items, _ = rc.corated_items(A, users, 60)
     a = rc.recommend(m, A, users, 20, retrieve=60, max_nodes_per_hop=mnph, batch_size=128, sample_seed=2)
@@ -213,9 +196,9 @@ def test_recommend_retrieve_equals_retrieved_lists():
 
 def test_retrieve_all_items_equals_bridged_full_catalogue():
     """retrieve=num_items ranks exactly the unrated items with at least one bridge"""
-    ds = _ds("ml_100k")
+    ds = support.dataset("ml_100k")
     A, mnph = ds["adj_train"], 200
-    m = _model(5)
+    m = support.model(5)
     g = RatingGraph(A)
     ni = g.num_items
     users = np.array([5, 300], np.int64)
@@ -234,9 +217,9 @@ def test_retrieve_all_items_equals_bridged_full_catalogue():
 
 
 def test_retrieve_steady_state_steps_do_not_sync():
-    ds = _ds("ml_1m")
+    ds = support.dataset("ml_1m")
     A = ds["adj_train"]
-    m = _model(5)
+    m = support.model(5)
     eng = rc.InferenceEngine(m, A, max_nodes_per_hop=100, batch_size=50, sample_seed=1)
     outs = []
     try:
@@ -261,9 +244,9 @@ def test_retrieve_steady_state_steps_do_not_sync():
 
 def test_invalid_device_rows_set_the_error_word():
     """device rows are checked by the kernel: an id outside [-1, num_items) is a kernel error, nothing is scored"""
-    ds = _ds("tiny")
+    ds = support.dataset("tiny")
     A = ds["adj_train"]
-    m = _model(5)
+    m = support.model(5)
     rows = torch.tensor([[0, 1, A.shape[1]]], device="cuda")
     with pytest.raises(RuntimeError, match="kernel error 7"):
         rc.recommend(m, A, [0], 3, items=rows, max_nodes_per_hop=10, batch_size=16)

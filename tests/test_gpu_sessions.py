@@ -3,7 +3,6 @@
 The oracle is the contract's equivalence: session s's subgraphs, scores, top-k lists and retrieved items are bit for
 bit those of the graph functions on RatingGraph(A_s), A_s = the graph with session s's edits applied to users[s]'s
 row, at the same kernel plan and batch size."""
-import functools
 import os
 import tempfile
 
@@ -13,36 +12,14 @@ import scipy.sparse as ssp
 import torch
 
 from igmc_b200 import recommend as rc
-from igmc_b200.data import build_adj, make_synthetic_dataset, synth_ratings
+from igmc_b200.data import make_synthetic_dataset
 from igmc_b200.util_functions import RatingGraph, SubgraphExtractor
 from oracle import extract_np
+from tests import support
 
 pytestmark = pytest.mark.gpu
 
 ARRAYS = ("row_ptr", "col_idx", "rating", "col_ptr", "row_idx")
-
-
-@functools.lru_cache(maxsize=None)
-def _ds(name):
-    return make_synthetic_dataset(name, seed=0)
-
-
-@functools.lru_cache(maxsize=None)
-def _r13():
-    nu, ni = 400, 300
-    u, v, lab = synth_ratings(nu, ni, 9000, 13, seed=4)
-    return build_adj(u, v, lab, nu, ni)
-
-
-def _model(R, rgcn="pyg-1.4", dgcnn=False, seed=0, h=1):
-    from igmc_b200.models import DGCNN_RS, IGMC
-    torch.manual_seed(seed)
-    if dgcnn:
-        m = DGCNN_RS(2 * h + 2, latent_dim=[32, 32, 32, 1], k=30, num_relations=R, num_bases=4, regression=True,
-                     rgcn=rgcn)
-    else:
-        m = IGMC(2 * h + 2, latent_dim=[32] * 4, num_relations=R, num_bases=4, regression=True, rgcn=rgcn)
-    return m.cuda()
 
 
 def _rows(A, users, session, items, values):
@@ -97,7 +74,7 @@ def _batch_arrays(b):
 
 # ---- 1. the session rows --------------------------------------------------------------------------------------------
 def test_session_rows_match_twin_and_invalid_input_raises():
-    A = _ds("ml_100k")["adj_train"]
+    A = support.adj("ml_100k")
     g = RatingGraph(A)
     rng = np.random.default_rng(0)
     nu = A.shape[0]
@@ -134,7 +111,7 @@ EXTRACT_CASES = [(1, None, 1.0, True), (1, None, 1.0, False), (1, 30, 1.0, True)
 
 @pytest.mark.parametrize("h,mnph,ratio,fast", EXTRACT_CASES)
 def test_extraction_equals_graph_with_edits(h, mnph, ratio, fast):
-    A = _ds("ml_100k")["adj_train"]
+    A = support.adj("ml_100k")
     nu, ni = A.shape
     g = RatingGraph(A)
     rng = np.random.default_rng(h * 10 + (mnph or 0))
@@ -211,35 +188,35 @@ def _scores_equal(A, m, plan, mnph, B, checkpoints=None, seed=5):
 def test_scores_equal_graph_with_edits(case):
     from igmc_b200 import _lib
     if case == "ml_1m plan 2":
-        A, m, plan, mnph = _ds("ml_1m")["adj_train"], _model(5), 2, 100
+        A, m, plan, mnph = support.adj("ml_1m"), support.model(5), 2, 100
     elif case == "ml_100k plan 4":
-        A, m, plan, mnph = _ds("ml_100k")["adj_train"], _model(5), 4, 200
+        A, m, plan, mnph = support.adj("ml_100k"), support.model(5), 4, 200
     elif case == "r13 plan 0":
-        A, m, plan, mnph = _r13(), _model(13), 0, 50
+        A, m, plan, mnph = support.adj("r13"), support.model(13), 0, 50
     elif case == "ml_100k L2":
-        A, m, plan, mnph = _ds("ml_100k")["adj_train"], _model(5), _lib.plan_l2(2), 100
+        A, m, plan, mnph = support.adj("ml_100k"), support.model(5), _lib.plan_l2(2), 100
     elif case == "pyg-2":
-        A, m, plan, mnph = _ds("ml_100k")["adj_train"], _model(5, rgcn="pyg-2"), 2, 100
+        A, m, plan, mnph = support.adj("ml_100k"), support.model(5, rgcn="pyg-2"), 2, 100
     else:
-        A, m, plan, mnph = _ds("ml_100k")["adj_train"], _model(5, dgcnn=True), "auto", 100
+        A, m, plan, mnph = support.adj("ml_100k"), support.model(5, dgcnn=True), "auto", 100
     _scores_equal(A, m, plan, mnph, 50)
 
 
 def test_three_checkpoints():
-    A = _ds("ml_100k")["adj_train"]
-    m = _model(5)
+    A = support.adj("ml_100k")
+    m = support.model(5)
     with tempfile.TemporaryDirectory() as tmp:
         paths = []
         for c in range(3):
             paths.append(os.path.join(tmp, "c%d.pth" % c))
-            torch.save(_model(5, seed=c + 1).state_dict(), paths[-1])
+            torch.save(support.model(5, seed=c + 1).state_dict(), paths[-1])
         _scores_equal(A, m, 2, 100, 50, checkpoints=paths)
 
 
 # ---- 4. ranking and retrieval ----------------------------------------------------------------------------------------
 def test_recommend_and_retrieval_equal_graph_with_edits():
-    A = _ds("ml_100k")["adj_train"]
-    m = _model(5)
+    A = support.adj("ml_100k")
+    m = support.model(5)
     m.kernel_plan = 2
     rng = np.random.default_rng(2)
     g = RatingGraph(A)
@@ -269,8 +246,8 @@ def test_recommend_and_retrieval_equal_graph_with_edits():
 
 
 def test_empty_edits_equal_plain_functions():
-    A = _ds("ml_100k")["adj_train"]
-    m = _model(5)
+    A = support.adj("ml_100k")
+    m = support.model(5)
     g = RatingGraph(A)
     users = np.array([4, 9, 4])
     sess = rc.RatingSessions(g, users)
@@ -289,9 +266,9 @@ def test_independence_and_graph_untouched():
     from igmc_b200.train_eval import FusedAdam, TrainEngine
     from igmc_b200.util_functions import MyDynamicDataset
     ds = make_synthetic_dataset("tiny", seed=0)
-    A = _ds("ml_100k")["adj_train"]
+    A = support.adj("ml_100k")
     g = RatingGraph(A)
-    m = _model(5)
+    m = support.model(5)
     m.kernel_plan = 2
     rng = np.random.default_rng(7)
     users, session, items, values = _session_case(A, rng, S=8, D=120)
@@ -330,9 +307,9 @@ def test_independence_and_graph_untouched():
 
 
 def test_stale_sessions_raise_and_steady_state_at_scale():
-    A = _ds("ml_1m")["adj_train"]
+    A = support.adj("ml_1m")
     g = RatingGraph(A, reserve_nnz=10)
-    m = _model(5)
+    m = support.model(5)
     rng = np.random.default_rng(3)
     nu = A.shape[0]
     S = 1100

@@ -7,29 +7,23 @@
 * the host twins of igmc_b200/recommend.py agree with the brute-force enumerations on every valid case the host can
   enumerate, so the twins the GPU tests compare with are held to the header's contracts at these regimes too."""
 import os
-import re
 
 import numpy as np
 import pytest
 
 from igmc_b200 import recommend as rc
 from tests import group_diverse_cache_cases as gc
+from tests import support
 from tests.ranking_cases import same_f32
 
 CASES = gc.all_cases()
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "igmc_b200", "csrc")
-
-
-def _id(c):
-    return "%s: %s" % (c["kernel"], c["name"])
 
 
 def _of(kernel, host=True):
     return [c for c in CASES if c["kernel"] == kernel and not (host and c.get("graph") == "big")]
 
 
-@pytest.mark.parametrize("case", CASES, ids=_id)
+@pytest.mark.parametrize("case", CASES, ids=support.pid)
 def test_case_reaches_its_regimes(case):
     got = gc.REGIMES[case["kernel"]](case)
     assert case["claims"] <= got, (case["claims"] - got)
@@ -44,24 +38,15 @@ def test_every_regime_is_reached():
 
 
 def test_claims_are_declared_not_derived():
-    """every case states its claims as data: no builder computes them with the function they are checked against"""
-    with open(gc.__file__) as f:
-        src = f.read()
-    assert not re.search(r"claims\W*\]?\s*=\s*\w*regimes", src) and not re.search(r"claims=\w*regimes", src)
-    assert all(isinstance(c["claims"], set) and c["claims"] for c in CASES)
+    support.claims_are_declared(gc, CASES)
 
 
 def test_launch_constants_match_the_sources():
-    with open(os.path.join(ROOT, "include", "igmc_b200.h")) as f:
-        defines = dict(re.findall(r"#define\s+(IGMC_\w+)\s+(\d+)", f.read()))
-    for (src, name), value in gc.CONSTANTS.items():
-        with open(os.path.join(CSRC, src)) as f:
-            m = re.findall(r"constexpr\s+int\s+%s\s*=\s*(\w+)\s*;" % name, f.read())
-        assert [defines.get(x, x) for x in m] == [str(value)], (src, name, m, value)
+    support.launch_constants_match(gc.CONSTANTS)
 
 
 def test_the_count_grid_is_what_the_cases_pass():
-    with open(os.path.join(CSRC, "diverse.cu")) as f:
+    with open(os.path.join(support.CSRC, "diverse.cu")) as f:
         assert "min(G->num_users, %d)" % gc.COUNT_GRID in f.read()
     assert gc.COUNT_NU > gc.COUNT_GRID and max(gc.LONG_ROWS) >= gc.COUNT_GRID
 
@@ -75,7 +60,7 @@ def test_the_degree_sum_case_wraps_an_int32():
 
 
 # ---- the host twins against the brute force -----------------------------------------------------------------------------
-@pytest.mark.parametrize("case", [c for c in _of("group_rows") if "bad_member" not in c["claims"]], ids=_id)
+@pytest.mark.parametrize("case", [c for c in _of("group_rows") if "bad_member" not in c["claims"]], ids=support.pid)
 def test_group_rows_twin(case):
     rp, ci = gc.graph_of(case)
     want_rp, want_ci, err = gc.group_rows_reference(case)
@@ -87,7 +72,7 @@ def test_group_rows_twin(case):
     assert np.array_equal(got_rp, want_rp) and np.array_equal(got_ci, want_ci)
 
 
-@pytest.mark.parametrize("case", [c for c in _of("group_pairs") if not c["invalid"]], ids=_id)
+@pytest.mark.parametrize("case", [c for c in _of("group_pairs") if not c["invalid"]], ids=support.pid)
 def test_group_pairs_twin(case):
     want, err = gc.group_pairs_reference(case)
     assert err == 0
@@ -98,7 +83,7 @@ def test_group_pairs_twin(case):
 
 
 @pytest.mark.parametrize("agg", ["mean", "min", "max"])
-@pytest.mark.parametrize("case", _of("group_stats"), ids=_id)
+@pytest.mark.parametrize("case", _of("group_stats"), ids=support.pid)
 def test_group_stats_twin(case, agg):
     want = gc.group_stats_reference(case, agg)
     with np.errstate(all="ignore"):
@@ -115,7 +100,7 @@ def test_group_mean_differs_from_an_fp32_sum():
     assert want[1][0] == gc.f32(1 / 3) and want[0][0] == gc.FLT_MAX and want[11][0] == 0.0
 
 
-@pytest.mark.parametrize("case", [c for c in _of("item_union") if "bad_id" not in c["claims"]], ids=_id)
+@pytest.mark.parametrize("case", [c for c in _of("item_union") if "bad_id" not in c["claims"]], ids=support.pid)
 def test_item_union_twin(case):
     mp, lst, err = gc.item_union_reference(case)
     got_mp, got_lst, bad = rc.item_union_host(case["items"], case["num_items"])
@@ -123,7 +108,7 @@ def test_item_union_twin(case):
     assert np.array_equal(got_mp, mp) and np.array_equal(got_lst, lst)
 
 
-@pytest.mark.parametrize("case", _of("cocount"), ids=_id)
+@pytest.mark.parametrize("case", _of("cocount"), ids=support.pid)
 def test_cocount_twin(case):
     want, code = gc.cocount_reference(case)
     if code:
@@ -141,7 +126,7 @@ def test_huge_reference_footing():
     assert i * (2 * gc.HUGE_NU - i - 1) > 2 ** 32
 
 
-@pytest.mark.parametrize("case", [c for c in _of("select") if "bad_id" not in c["claims"]], ids=_id)
+@pytest.mark.parametrize("case", [c for c in _of("select") if "bad_id" not in c["claims"]], ids=support.pid)
 def test_diverse_select_twin(case):
     rp, ci = gc.select_graph()
     cp, _ = gc.columns(rp, ci, gc.SEL_NI)
@@ -155,7 +140,7 @@ def test_diverse_select_twin(case):
     assert np.array_equal(got[0], want[0]) and same_f32(got[1], want[1]) and same_f32(got[2], want[2])
 
 
-@pytest.mark.parametrize("case", _of("cosine"), ids=_id)
+@pytest.mark.parametrize("case", _of("cosine"), ids=support.pid)
 def test_item_cosine_twin(case):
     rp, ci = gc.select_graph()
     cp, _ = gc.columns(rp, ci, gc.SEL_NI)
@@ -163,7 +148,7 @@ def test_item_cosine_twin(case):
     assert same_f32(got, gc.cosine_reference(case))
 
 
-@pytest.mark.parametrize("case", [c for c in _of("rescore") if "edit:bad" not in c["claims"]], ids=_id)
+@pytest.mark.parametrize("case", [c for c in _of("rescore") if "edit:bad" not in c["claims"]], ids=support.pid)
 def test_rescore_plan_twin(case):
     rp, ci = gc.cache_graph(case["num_items"])
     off, items, full, totals, err = gc.rescore_reference(case)
@@ -174,7 +159,7 @@ def test_rescore_plan_twin(case):
     assert (int(g_off[-1]), g_total) == totals
 
 
-@pytest.mark.parametrize("case", _of("invalidate"), ids=_id)
+@pytest.mark.parametrize("case", _of("invalidate"), ids=support.pid)
 def test_cache_invalidate_twin(case):
     want = gc.invalidate_reference(case)
     got = rc.cache_invalidate_host(case["user_off"], case["resc"], case["full"], case["complete"], case["top_s"],
@@ -183,7 +168,7 @@ def test_cache_invalidate_twin(case):
         assert same_f32(g, w) if g.dtype == np.float32 else np.array_equal(g, w)
 
 
-@pytest.mark.parametrize("case", _of("settle"), ids=_id)
+@pytest.mark.parametrize("case", _of("settle"), ids=support.pid)
 def test_cache_settle_twin(case):
     want = gc.settle_reference(case)
     got = rc.cache_settle_host(case["thr_s"], case["thr_i"], case["top_s"], case["top_i"], case["k"])
@@ -191,7 +176,7 @@ def test_cache_settle_twin(case):
         assert same_f32(g, w) if g.dtype == np.float32 else np.array_equal(g, w)
 
 
-@pytest.mark.parametrize("case", _of("ws_bytes"), ids=_id)
+@pytest.mark.parametrize("case", _of("ws_bytes"), ids=support.pid)
 def test_ws_bytes_reference_is_the_largest_fitting_chunk(case):
     q, pool, ni, bound = case["args"]
     nbytes, c = gc.ws_reference(case)

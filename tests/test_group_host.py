@@ -7,19 +7,14 @@ import torch
 
 from igmc_b200 import _lib
 from igmc_b200 import recommend as rc
-
-
-def _csr(rows):
-    rp = np.concatenate([[0], np.cumsum([len(r) for r in rows])]).astype(np.int32)
-    ci = np.concatenate([np.asarray(r, np.int64) for r in rows] + [np.zeros(0, np.int64)]).astype(np.int32)
-    return rp, ci
+from tests import support
 
 
 ROWS = [[1, 4, 7], [], [0, 4, 9, 11], [2, 7], [4], [1, 3, 5, 7, 9, 11]]
 
 
 def test_group_rows_twin_is_the_union():
-    rp, ci = _csr(ROWS)
+    rp, ci = support.rows_csr(ROWS)
     members = np.array([[0, 2, -1], [1, -1, -1], [3, 0, 5], [4, 1, 0]], np.int32)   # overlaps, an empty row, dups
     urp, uci = rc.group_rows_host(rp, ci, members)
     assert urp.dtype == np.int32 and uci.dtype == np.int32
@@ -114,7 +109,7 @@ def test_group_stats_twin(agg):
 
 
 def test_predict_and_recommend_host_compose_pair_scores():
-    rp, ci = _csr(ROWS)
+    rp, ci = support.rows_csr(ROWS)
     ni = 12
     members = np.array([[0, 2], [4, -1], [3, 1]], np.int32)
 

@@ -2,18 +2,17 @@
 that its shared memory does not grow with the subgraph, which entry points refuse it, and that ``select_plan`` picks
 it exactly where no shared-memory plan fits."""
 import ctypes
+import functools
 
 import pytest
 
 from igmc_b200 import _lib
 from igmc_b200.models import l2_cluster, select_plan
+from tests import support
+
+_cpu_model = functools.partial(support.model, seed=None, cuda=False)   # plan queries: unseeded, on the host
 
 SMS = 132   # H100 SXM
-
-
-def _model(R, in0=4, NB=4, L=4):
-    from igmc_b200.models import IGMC
-    return IGMC(in0, latent_dim=[32] * L, num_relations=R, num_bases=NB, regression=True)
 
 
 def _plan_bytes(m, n_cap, plan):
@@ -25,7 +24,7 @@ def _plan_bytes(m, n_cap, plan):
 @pytest.mark.parametrize("n_cap", [802, 1476, 8000])
 def test_l2_plan_accepts_large_subgraphs(R, n_cap):
     for NB in (2, 4):
-        m = _model(R, NB=NB)
+        m = _cpu_model(R, nb=NB)
         for c in (1, 2, 4, 8):
             f, b = _plan_bytes(m, n_cap, _lib.plan_l2(c))
             assert f > 0 and b > 0, (R, NB, n_cap, c, f, b)
@@ -37,19 +36,19 @@ def test_l2_plan_accepts_large_subgraphs(R, n_cap):
 
 
 def test_l2_plan_limits():
-    m = _model(5)
+    m = _cpu_model(5)
     assert min(_plan_bytes(m, _lib.L2_MAX_NODES + 1, _lib.plan_l2(2))) < 0       # 16-bit neighbour field
     for bad in (_lib.PLAN_L2_BASE, _lib.plan_l2(3), _lib.plan_l2(16)):            # cluster sizes other than 1/2/4/8
         assert min(_plan_bytes(m, 802, bad)) < 0, bad
-    assert min(_plan_bytes(_model(256, in0=8, L=8), 802, _lib.plan_l2(8))) > 0   # any R <= 256, up to 8 layers
-    assert min(_plan_bytes(_model(257), 802, _lib.plan_l2(2))) < 0
+    assert min(_plan_bytes(_cpu_model(256, in0=8, layers=8), 802, _lib.plan_l2(8))) > 0   # any R <= 256, up to 8 layers
+    assert min(_plan_bytes(_cpu_model(257), 802, _lib.plan_l2(2))) < 0
 
 
 def test_l2_plan_rejected_by_cluster_only_entry_points():
     """the one-launch train kernel and the list images exist for the relation-space plans only; the forward and
     backward refuse the plan's shape errors before they touch a device pointer"""
     lib = _lib.load()
-    m = _model(5)
+    m = _cpu_model(5)
     c = ctypes.byref(m._cmodel)
     img = _lib.Stage()
     S = _lib.Saved()
@@ -93,7 +92,7 @@ def test_select_plan_keeps_existing_plans(R):
     l2_seen = 0
     for NB in (2, 4):
         for in0 in (4, 6, 8):
-            m = _model(R, in0=in0, NB=NB)
+            m = _cpu_model(R, in0=in0, nb=NB)
             for B in (16, 50):
                 for n_cap in N_CAPS:
                     old = _old_rule(m, n_cap, B, SMS)
@@ -107,7 +106,7 @@ def test_select_plan_keeps_existing_plans(R):
 
 
 def test_select_plan_forced_and_refused():
-    m = _model(5)
+    m = _cpu_model(5)
     assert select_plan(m._cmodel, 402, 50, SMS, want=_lib.plan_l2(4)) == _lib.plan_l2(4)
     assert select_plan(m._cmodel, 402, 50, SMS, want=0) == 0
     with pytest.raises(RuntimeError, match="no kernel plan fits"):

@@ -6,28 +6,21 @@
   csrc/session.cu, so a changed block size flags the cases before they silently stop reaching a chunk boundary;
 * the host twins of igmc_b200/recommend.py agree with the brute-force enumerations on the cases they run at a sensible
   size, so the twins other tests rely on are held to the contract at these regimes too."""
-import os
-import re
-
 import numpy as np
 import pytest
 
 from igmc_b200 import recommend as rc
 from tests import pair_stream_cases as ps
+from tests import support
 
 CASES = ps.all_cases()
-CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "igmc_b200", "csrc")
-
-
-def _id(c):
-    return "%s: %s" % (c["kernel"], c["name"])
 
 
 def _of(kernel):
     return [c for c in CASES if c["kernel"] == kernel]
 
 
-@pytest.mark.parametrize("case", CASES, ids=_id)
+@pytest.mark.parametrize("case", CASES, ids=support.pid)
 def test_case_reaches_its_regimes(case):
     got = ps.REGIMES[case["kernel"]](case)
     assert case["claims"] <= got, (case["claims"] - got)
@@ -50,18 +43,11 @@ def test_every_pair_mode_reaches_every_batch_regime():
 
 
 def test_claims_are_declared_not_derived():
-    """every case states its claims as data: no builder computes them with the function they are checked against"""
-    with open(ps.__file__) as f:
-        src = f.read()
-    assert not re.search(r"claims\W*\]?\s*=\s*\w+_regimes\(", src)
-    assert all(c["claims"] for c in CASES if c["name"] != "B=1 P=3")
+    support.claims_are_declared(ps, [c for c in CASES if c["name"] != "B=1 P=3"])
 
 
 def test_launch_constants_match_the_sources():
-    for (src, name), value in ps.CONSTANTS.items():
-        with open(os.path.join(CSRC, src)) as f:
-            m = re.findall(r"constexpr\s+int\s+%s\s*=\s*(\d+)\s*;" % name, f.read())
-        assert m == [str(value)], (src, name, m, value)
+    support.launch_constants_match(ps.CONSTANTS)
 
 
 def test_the_big_graph_passes_int64():
@@ -76,7 +62,7 @@ def test_the_big_graph_passes_int64():
 
 
 # ---- the host twins against the brute force -----------------------------------------------------------------------------
-@pytest.mark.parametrize("case", _of("plan"), ids=_id)
+@pytest.mark.parametrize("case", _of("plan"), ids=support.pid)
 def test_plan_twin(case):
     A = ps.plan_graph()
     uo, ro, rp, _ = ps.plan_reference(case)
@@ -88,7 +74,7 @@ def test_plan_twin(case):
         assert np.array_equal(hro, ro) and np.array_equal(hrp, rp)
 
 
-@pytest.mark.parametrize("case", _of("lists"), ids=_id)
+@pytest.mark.parametrize("case", _of("lists"), ids=support.pid)
 def test_lists_twin(case):
     A = ps.plan_graph()
     uo, lists, _, _ = ps.lists_reference(case)
@@ -96,7 +82,7 @@ def test_lists_twin(case):
     assert np.array_equal(hu, uo) and np.array_equal(hl, lists)
 
 
-@pytest.mark.parametrize("case", [c for c in _of("pairs") if c["mode"] in ("no_list", "shared")], ids=_id)
+@pytest.mark.parametrize("case", [c for c in _of("pairs") if c["mode"] in ("no_list", "shared")], ids=support.pid)
 def test_pairs_twin(case):
     """the first batch, one across a user boundary and the last two"""
     A = ps.plan_graph()
@@ -112,12 +98,12 @@ def test_pairs_twin(case):
             assert np.array_equal(g, w), pos
 
 
-@pytest.mark.parametrize("case", _of("offsets"), ids=_id)
+@pytest.mark.parametrize("case", _of("offsets"), ids=support.pid)
 def test_offsets_twin(case):
     assert np.array_equal(rc.explain_offsets_host(case["num_edges"]), ps.offsets_reference(case))
 
 
-@pytest.mark.parametrize("case", [c for c in _of("occl") if "invalid" not in c["name"]], ids=_id)
+@pytest.mark.parametrize("case", [c for c in _of("occl") if "invalid" not in c["name"]], ids=support.pid)
 def test_occlusion_pairs_twin(case):
     off = ps.offsets_reference(case)
     for pos in ps.occl_cursors(case)[:40] + ps.occl_cursors(case)[-3:]:
@@ -127,7 +113,7 @@ def test_occlusion_pairs_twin(case):
             assert np.array_equal(g, w), pos
 
 
-@pytest.mark.parametrize("case", _of("mask"), ids=_id)
+@pytest.mark.parametrize("case", _of("mask"), ids=support.pid)
 def test_mask_twin(case):
     keep, _, _ = ps.mask_reference(case, -1)
     ms = np.asarray(case["ms"])
@@ -135,7 +121,7 @@ def test_mask_twin(case):
     assert np.array_equal(rc.occlusion_mask_host(case["batch"]["edge_ptr"], case["tag"], j), keep)
 
 
-@pytest.mark.parametrize("case", [c for c in _of("scatter") if "disagree" not in c["name"]], ids=_id)
+@pytest.mark.parametrize("case", [c for c in _of("scatter") if "disagree" not in c["name"]], ids=support.pid)
 def test_scatter_twin(case):
     grads = ps.scatter_grads(case)
     outs, _, err = ps.scatter_reference(case, grads, np.float32(0), -1)

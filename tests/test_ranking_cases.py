@@ -9,15 +9,12 @@ import pytest
 
 from igmc_b200 import recommend as rc
 from tests import ranking_cases as rcs
+from tests import support
 
 CASES = rcs.all_cases()
 
 
-def _id(c):
-    return "%s: %s" % (c["kernel"], c["name"])
-
-
-@pytest.mark.parametrize("case", CASES, ids=_id)
+@pytest.mark.parametrize("case", CASES, ids=support.pid)
 def test_case_reaches_its_regimes(case):
     got = rcs.REGIMES[case["kernel"]](case)
     assert case["claims"] <= got, (case["claims"] - got)
@@ -60,7 +57,7 @@ def test_topk_fits_boundary_restated():
 
 
 # ---- the host twins against the brute-force orders ---------------------------------------------------------------------
-@pytest.mark.parametrize("case", [c for c in CASES if c["kernel"] == "merge"], ids=_id)
+@pytest.mark.parametrize("case", [c for c in CASES if c["kernel"] == "merge"], ids=support.pid)
 def test_merge_twins_match_brute_force(case):
     slot, item, preds = rcs.merge_stream(case)
     s = rcs.ckpt_mean(preds)
@@ -82,7 +79,7 @@ def test_merge_twins_match_brute_force(case):
                 assert np.array_equal(top_i, wi) and rcs.same_f32(top_s, ws), (cuts, b)
 
 
-@pytest.mark.parametrize("case", [c for c in CASES if c["kernel"] == "influence"], ids=_id)
+@pytest.mark.parametrize("case", [c for c in CASES if c["kernel"] == "influence"], ids=support.pid)
 def test_influence_twin_matches_brute_force(case):
     idx, vals = rcs.influence_stream(case)
     want = rcs.influence_reference(case, len(idx))
@@ -97,7 +94,7 @@ def test_influence_twin_matches_brute_force(case):
 
 @pytest.mark.parametrize("case", [c for c in CASES if c["kernel"] == "occlusion" and
                                   (sum(c["lengths"]) < 10 ** 5 or c["name"] in ("big m=0 score=True", "big m=1 score=False"))],
-                         ids=_id)
+                         ids=support.pid)
 def test_occlusion_twin_matches_brute_force(case):
     score, occluded, offsets, _, _, _ = rcs.occlusion_data(case)
     order, delta = rcs.occlusion_reference(case)
@@ -106,7 +103,8 @@ def test_occlusion_twin_matches_brute_force(case):
     assert np.array_equal(o, order)
 
 
-@pytest.mark.parametrize("case", [c for c in CASES if c["kernel"] == "corated" and c["graph"] != "bytes"], ids=_id)
+@pytest.mark.parametrize("case", [c for c in CASES if c["kernel"] == "corated" and c["graph"] != "bytes"],
+                         ids=support.pid)
 def test_corated_twin_matches_brute_force(case):
     A = rcs.GRAPHS[case["graph"]]()
     nu, ni = A.shape

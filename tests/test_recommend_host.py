@@ -10,18 +10,7 @@ import scipy.sparse as ssp
 import torch
 
 from igmc_b200 import recommend as rc
-
-
-def _csr(nu, ni, density, seed, full_rows=(), empty_rows=()):
-    rng = np.random.default_rng(seed)
-    dense = rng.random((nu, ni)) < density
-    for u in full_rows:
-        dense[u] = True
-    for u in empty_rows:
-        dense[u] = False
-    A = ssp.csr_matrix(np.where(dense, rng.integers(1, 6, (nu, ni)), 0).astype(np.float32))
-    A.sort_indices()
-    return A
+from tests import support
 
 
 def _brute(A, users, cand, exclude):
@@ -49,7 +38,7 @@ CASES = [
 @pytest.mark.parametrize("case", range(len(CASES)))
 @pytest.mark.parametrize("B", [1, 7, 64])
 def test_candidate_plan_and_pairs_match_brute_force(case, exclude, B):
-    A = _csr(12, 30, 0.3, seed=case, full_rows=(0,), empty_rows=(1,))
+    A = support.random_csr(12, 30, 0.3, seed=case, full_rows=(0,), empty_rows=(1,))
     A = ssp.csr_matrix(A)
     A.data[A.indices == A.shape[1] - 1] = 0       # the last item has no rating: a list of it hits no row
     A.eliminate_zeros()
@@ -81,7 +70,7 @@ def test_candidate_plan_and_pairs_match_brute_force(case, exclude, B):
 
 
 def test_rated_everything_and_unrated_nothing():
-    A = _csr(4, 9, 0.0, 0, full_rows=(0, 3))
+    A = support.random_csr(4, 9, 0.0, 0, full_rows=(0, 3))
     rp, ci = A.indptr.astype(np.int64), A.indices.astype(np.int64)
     for users in ([0, 3], [0], [3, 0, 3]):
         plan = rc.candidate_plan_host(rp, ci, 9, np.array(users), None, True)
@@ -129,7 +118,7 @@ def test_streaming_topk_order(k, seed):
 
 def test_validation_errors():
     nu, ni = 5, 7
-    A = _csr(nu, ni, 0.4, 3)
+    A = support.random_csr(nu, ni, 0.4, 3)
     m = type("M", (), {})()
     m.flat_params = torch.zeros(1)
     with pytest.raises(ValueError):

@@ -10,16 +10,7 @@ import scipy.sparse as ssp
 import torch
 
 from igmc_b200 import recommend as rc
-
-
-def _csr(nu, ni, density, seed, empty_rows=(), empty_cols=()):
-    rng = np.random.default_rng(seed)
-    dense = rng.random((nu, ni)) < density
-    dense[list(empty_rows)] = False
-    dense[:, list(empty_cols)] = False
-    A = ssp.csr_matrix(np.where(dense, rng.integers(1, 6, (nu, ni)), 0).astype(np.float32))
-    A.sort_indices()
-    return A
+from tests import support
 
 
 def _brute_counts(A, v, exclude):
@@ -53,7 +44,7 @@ def _brute_top(c, m):
 def test_corated_users_twin_matches_brute_force(seed, m, exclude):
     """empty rows and columns (users and items without ratings), m = 1, m beyond the reachable users, m = num_users"""
     nu, ni = 16, 11
-    A = _csr(nu, ni, 0.25 + 0.1 * seed, seed, empty_rows=(2, 9), empty_cols=(4,))
+    A = support.random_csr(nu, ni, 0.25 + 0.1 * seed, seed, empty_rows=(2, 9), empty_cols=(4,))
     m = min(m, nu)
     items = np.array([0, 4, 3, 3, 10, 7], np.int64)
     rp, ci = A.indptr.astype(np.int64), A.indices.astype(np.int64)
@@ -107,7 +98,7 @@ def _dense_counts(ids, paths, n):
 def test_item_side_counts_are_the_user_side_counts(seed, exclude):
     """corated_users_host(items)[v][u] == corated_host(users)[u][v] for every pair: one count seen from either side"""
     nu, ni = 21, 17
-    A = _csr(nu, ni, 0.15 + 0.08 * seed, 10 + seed, empty_rows=(0,), empty_cols=(5,))
+    A = support.random_csr(nu, ni, 0.15 + 0.08 * seed, 10 + seed, empty_rows=(0,), empty_cols=(5,))
     rp, ci = A.indptr.astype(np.int64), A.indices.astype(np.int64)
     iu, ip = rc.corated_host(rp, ci, nu, ni, np.arange(nu), ni, exclude)
     uu, up = rc.corated_users_host(rp, ci, nu, ni, np.arange(ni), nu, exclude)
@@ -130,7 +121,7 @@ def test_item_query_pairs_twin_enumerates_the_item_side_pairs(which, exclude):
     order, its candidate users ascending as (user, item) pairs with pair id u * num_items + v; the tail repeats the
     last pair with tag -1"""
     nu, ni = 13, 9
-    A = _csr(nu, ni, 0.3, 5, empty_rows=(4,), empty_cols=(2,))
+    A = support.random_csr(nu, ni, 0.3, 5, empty_rows=(4,), empty_cols=(2,))
     trp, tci = _transposed_host(A)
     items = np.array([1, 2, 8, 1, 0], np.int64)
     cand = None if which == "all" else np.array([0, 3, 4, 7, 11, 12], np.int64)
@@ -172,7 +163,7 @@ def _fake_model():
 
 def test_validation_of_recommend_users():
     nu, ni = 6, 5
-    A = _csr(nu, ni, 0.4, 3)
+    A = support.random_csr(nu, ni, 0.4, 3)
     m = _fake_model()
     for k in (0, 257):
         with pytest.raises((ValueError, NotImplementedError)):
@@ -205,7 +196,7 @@ def test_validation_of_recommend_users():
 
 def test_validation_of_corated_users():
     nu, ni = 6, 5
-    A = _csr(nu, ni, 0.4, 3)
+    A = support.random_csr(nu, ni, 0.4, 3)
     for M in (0, nu + 1):                     # 1 <= m <= num_users
         with pytest.raises(ValueError):
             rc.corated_users(A, [0], M)

@@ -9,19 +9,7 @@ import scipy.sparse as ssp
 import torch
 
 from igmc_b200 import recommend as rc
-
-
-def _csr(nu, ni, density, seed, empty_rows=(), single_cols=()):
-    rng = np.random.default_rng(seed)
-    dense = rng.random((nu, ni)) < density
-    for u in empty_rows:
-        dense[u] = False
-    for v in single_cols:                     # items with exactly one rater
-        dense[:, v] = False
-        dense[int(rng.integers(nu)), v] = True
-    A = ssp.csr_matrix(np.where(dense, rng.integers(1, 6, (nu, ni)), 0).astype(np.float32))
-    A.sort_indices()
-    return A
+from tests import support
 
 
 def _brute_paths(A, u, exclude):
@@ -54,7 +42,7 @@ def _brute_top(p, m):
 def test_corated_twin_matches_brute_force(seed, m, exclude):
     """users without ratings, items with one rater, m beyond the reachable set, m = 1 and m >= num_items"""
     nu, ni = 14, 25
-    A = _csr(nu, ni, 0.2 + 0.1 * seed, seed, empty_rows=(3,), single_cols=(4, 9))
+    A = support.random_csr(nu, ni, 0.2 + 0.1 * seed, seed, empty_rows=(3,), single_cols=(4, 9))
     m = min(m, ni)
     users = np.array([0, 3, 5, 5, 13, 1], np.int64)
     rp, ci = A.indptr.astype(np.int64), A.indices.astype(np.int64)
@@ -85,7 +73,7 @@ def test_corated_twin_reachability_and_ties():
 @pytest.mark.parametrize("exclude", [True, False])
 def test_candidate_lists_twin(exclude):
     """dedupe, -1 slots, rated removal, a row of only empty slots, a user without ratings"""
-    A = _csr(6, 20, 0.3, 7, empty_rows=(2,))
+    A = support.random_csr(6, 20, 0.3, 7, empty_rows=(2,))
     rp, ci = A.indptr.astype(np.int64), A.indices.astype(np.int64)
     users = np.array([0, 2, 4, 0], np.int64)
     row0 = ci[rp[0]:rp[1]]
@@ -112,7 +100,7 @@ def _fake_model():
 
 def test_validation_of_rows_and_retrieve():
     nu, ni = 5, 7
-    A = _csr(nu, ni, 0.4, 3)
+    A = support.random_csr(nu, ni, 0.4, 3)
     m = _fake_model()
     with pytest.raises(ValueError):            # row count != len(users)
         rc.recommend(m, A, [0, 1], 3, items=np.zeros((3, 2), np.int64))
